@@ -93,6 +93,8 @@ def _lib():
   lib.edtb200_profile_passes.restype = ci
   lib.edtb200_pass_ms.argtypes = [ci, vp]
   lib.edtb200_pass_ms.restype = ci
+  lib.edtb200_last_later_launch.argtypes = [vp]
+  lib.edtb200_last_later_launch.restype = ci
   lib.edtb200_slab_stage_bytes.argtypes = [i64, i64, ci, ci]
   lib.edtb200_slab_stage_bytes.restype = i64
   lib.edtb200_slab_step.argtypes = [vp, ci, i64, i64, i64, f32, f32, f32, ci, ci, ci, ci, vp, ci, vp, vp, vp,
@@ -119,6 +121,20 @@ def _check(rc):
 
 def device_count():
   return int(_lib().edtb200_device_count())
+
+
+LATER_LAUNCH_FIELDS = ("kernel", "tx", "tma", "wide", "ctas", "int_hull", "epilogue", "all_double")
+
+
+def last_later_launch():
+  """Kernel variant of the last Y / Z pass this thread launched (edtb200_last_later_launch), as a
+  dict: kernel "tile" or "long", tile width tx, tma, wide, ctas (per SM), int_hull, epilogue,
+  all_double (every candidate formed in double)."""
+  info = (ctypes.c_int * len(LATER_LAUNCH_FIELDS))()
+  _check(_lib().edtb200_last_later_launch(info))
+  out = dict(zip(LATER_LAUNCH_FIELDS, (int(v) for v in info)))
+  out["kernel"] = "tile" if out["kernel"] == 0 else "long"
+  return out
 
 
 def nvl(val, default_val):

@@ -24,6 +24,7 @@ namespace edtb200 {
 namespace host {
 
 thread_local char g_error[512] = "";
+thread_local LaterLaunch g_last_later;
 
 int fail(int code, const char* fmt, ...) {
   va_list ap;
@@ -392,13 +393,14 @@ int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines
 
 // fmax: an upper bound of the finite samples in f when they are known to be integer-valued (the
 // product of earlier passes with integer weights^2), or -1: enables the integer hull tests.
+// exact: every candidate sum of the pass is exact in double (sums_exact).
 int dispatch_later(int label_bytes, const void* labels, float* f, const edtb200::LineGeom& g, float w,
-                   int lo, int hi, int flags, DeviceCache& dc, cudaStream_t s, bool pdl = false, double fmax = -1.0) {
+                   int lo, int hi, int flags, DeviceCache& dc, cudaStream_t s, bool pdl, double fmax, bool exact) {
   switch (label_bytes) {
-    case 1: return launch_later<1>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax);
-    case 2: return launch_later<2>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax);
-    case 4: return launch_later<4>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax);
-    default: return launch_later<8>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax);
+    case 1: return launch_later<1>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
+    case 2: return launch_later<2>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
+    case 4: return launch_later<4>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
+    default: return launch_later<8>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
   }
 }
 
@@ -415,6 +417,79 @@ double integer_bound(const float* w, const int64_t* n, int k) {
     bound += (double)w2 * (double)n[i] * (double)n[i];
   }
   return bound < 2147483000.0 ? bound : -1.0;
+}
+
+// Is every candidate w2 * d^2 + f (d < n) of a later-axis pass exact in double, when the finite
+// samples are at most fmax and every sample, like w2, is a whole multiple of `unit`?  w2 * d^2 is
+// exact in double (24 + 24 bits), so the sum is exact when it spans at most 53 bits from `unit`
+// up.  Then the tile kernel's one fused multiply-add rounds the very sum the reference rounds once
+// from double (src/edt.hpp:232), and the results agree bit for bit; otherwise they may differ by
+// one ulp at a double-rounding tie.
+bool sums_exact(double fmax, double unit, float w2, int64_t n) {
+  return fmax + (double)w2 * (double)n * (double)n < 0x1p53 * unit;
+}
+
+// Spacing of float32 values at v > 0 (0: the smallest subnormal): every float32 of magnitude v
+// or more is a whole multiple of it.
+double float_spacing(float v) { return (double)nextafterf(v, INFINITY) - (double)v; }
+
+// Lowest set bit of v > 0 (a power of two); 0 for v <= 0 or not finite.
+double lowest_bit(double v) {
+  if (!(v > 0.0) || !std::isfinite(v)) return 0.0;
+  int e = 0;
+  const double m = frexp(v, &e);                                   // v = m 2^e, m in [0.5, 1)
+  const unsigned long long mant = (unsigned long long)ldexp(m, 53);
+  return ldexp(1.0, e - 53 + __builtin_ctzll(mant));
+}
+
+// sums_exact for the later-axis pass along axis k of a transform (weight w[k], length n[k]),
+// whose samples are what the passes along axes 0..k-1 made, at most the sum of w2 * n^2 over those
+// axes (the factor 2 covers their float32 rounding).  The unit:
+//  - when the X pass is exact (every distance j * w[0] below 2^24 units of b0 = lowest_bit(w[0])),
+//    its squares are multiples of b0^2, every w2 = fl32(w * w) is a multiple of its lowest set bit,
+//    and float32 rounding keeps a multiple of a power of two P a multiple of P: so every sample and
+//    candidate is a multiple of the least of b0^2 and those bits (1 or more for integer weights,
+//    1/4 for weights of 0.5, ...);
+//  - otherwise every positive sample is at least the least squared weight (the X pass's smallest
+//    distance is one step), so half the float32 spacing there divides them all.
+bool transform_sums_exact(const float* w, const int64_t* n, int k) {
+  double top = 0.0;
+  float least = INFINITY;
+  const double b0 = lowest_bit((double)w[0]);
+  double unit = b0 * b0;
+  const bool x_exact = b0 > 0.0 && (double)w[0] * (double)n[0] < 16777216.0 * b0;
+  for (int i = 0; i <= k; ++i) {
+    const float w2 = w[i] * w[i];
+    if (i < k) top += (double)w2 * (double)n[i] * (double)n[i];
+    least = fminf(least, w2);
+    if (i > 0) unit = fmin(unit, lowest_bit((double)w2));
+  }
+  if (!x_exact || !(unit > 0.0)) unit = 0.5 * float_spacing(least);
+  return sums_exact(2.0 * top, unit, w[k] * w[k], n[k]);
+}
+
+// Largest finite |f| (as float bits: non-negative floats order like their bits) and the exponent
+// of the lowest set bit over all finite non-zero samples, for edtb200_pass_later, whose samples
+// the host knows nothing about.  range = {0, 1024} on entry.
+__global__ void __launch_bounds__(256) sample_range_kernel(const float* __restrict__ f, int64_t count,
+                                                          int* range) {
+  unsigned int hi = 0u;
+  int low = 1024;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned int b = __float_as_uint(f[i]) & 0x7fffffffu;
+    if (b >= 0x7f800000u || b == 0u) continue;           // +inf (and nan) are not sites; 0 has no bit
+    hi = max(hi, b);
+    const unsigned int e = b >> 23, m = (b & 0x7fffffu) | (e ? 0x800000u : 0u);
+    low = min(low, (int)(e ? e : 1u) - 150 + (__ffs(m) - 1));
+  }
+  for (int o = 16; o; o >>= 1) {
+    hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    low = min(low, __shfl_xor_sync(0xffffffffu, low, o));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(reinterpret_cast<unsigned int*>(range), hi);
+    atomicMin(range + 1, low);
+  }
 }
 
 edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz) {
@@ -510,17 +585,17 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   mark_pass(1, stream);
   if (!rc && ndim >= 2) {
     nvtx_push("edt.y");
-    const float ws[1] = {wx}; const int64_t ns[1] = {sx};
+    const float ws[2] = {wx, wy}; const int64_t ns[2] = {sx, sy};
     rc = dispatch_later(label_bytes, labels, f, gy, wy, border, border, ndim == 2 ? epilogue : 0, dc, stream,
-                        /*pdl=*/true, integer_bound(ws, ns, 1));
+                        /*pdl=*/true, integer_bound(ws, ns, 1), transform_sums_exact(ws, ns, 1));
     nvtx_pop();
     mark_pass(2, stream);
   }
   if (!rc && ndim >= 3) {
     nvtx_push("edt.z");
-    const float ws[2] = {wx, wy}; const int64_t ns[2] = {sx, sy};
+    const float ws[3] = {wx, wy, wz}; const int64_t ns[3] = {sx, sy, sz};
     rc = dispatch_later(label_bytes, labels, f, gz, wz, border, border, epilogue, dc, stream, /*pdl=*/true,
-                        integer_bound(ws, ns, 2));
+                        integer_bound(ws, ns, 2), transform_sums_exact(ws, ns, 2));
     nvtx_pop();
     mark_pass(3, stream);
   }
@@ -859,11 +934,48 @@ int edtb200_pass_later(const void* labels_dev, int label_bytes, int axis, int64_
   DeviceCache* dc = nullptr;
   rc = probe(device, &dc);
   if (rc) return rc;
-  return dispatch_later(label_bytes, labels_dev, f_dev, geom_for_axis(axis, sx, sy, sz), w,
-                        border_lo != 0, border_hi != 0,
+  // The samples come from the caller: one reduction over them (and a wait for it) tells whether
+  // the pass's candidate sums are exact in double, and whether the integer hull tests apply.
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int64_t count = sx * sy * sz;
+  int* range_dev = nullptr;
+  CUDA_TRY(scratch_alloc(*dc, reinterpret_cast<void**>(&range_dev), 2 * sizeof(int), s));
+  const int init[2] = {0, 1024};
+  int range[2] = {0, 1024};
+  cudaError_t err = cudaMemcpyAsync(range_dev, init, sizeof(init), cudaMemcpyHostToDevice, s);
+  if (err == cudaSuccess) {
+    int64_t blocks = (count + 255) / 256;
+    if (blocks > (int64_t)dc->sm_count * 8) blocks = (int64_t)dc->sm_count * 8;
+    sample_range_kernel<<<(unsigned)blocks, 256, 0, s>>>(f_dev, count, range_dev);
+    err = cudaGetLastError();
+  }
+  if (err == cudaSuccess) err = cudaMemcpyAsync(range, range_dev, sizeof(range), cudaMemcpyDeviceToHost, s);
+  const cudaError_t freed = cudaFreeAsync(range_dev, s);        // on every path once allocated
+  if (err == cudaSuccess) err = freed;
+  if (err == cudaSuccess) err = cudaStreamSynchronize(s);
+  CUDA_TRY(err);
+  float fmax;
+  memcpy(&fmax, &range[0], sizeof(float));
+  const float w2 = w * w;
+  // every sample and every w2 d^2 is a multiple of `unit`; integer samples and w2 allow the
+  // integer hull tests
+  double unit = lowest_bit((double)w2);
+  if (range[1] < 1024) unit = fmin(unit, ldexp(1.0, range[1]));
+  const bool integral = range[1] >= 0 && w2 == floorf(w2);
+  const edtb200::LineGeom g = geom_for_axis(axis, sx, sy, sz);
+  return dispatch_later(label_bytes, labels_dev, f_dev, g, w, border_lo != 0, border_hi != 0,
                         ((flags & EDTB200_SQRT) ? edtb200::kSqrt : 0) |
                             ((flags & EDTB200_SIGNED) ? edtb200::kNegate : 0),
-                        *dc, static_cast<cudaStream_t>(stream));
+                        *dc, s, /*pdl=*/false, integral ? (double)fmax : -1.0, sums_exact(fmax, unit, w2, g.n));
+}
+
+int edtb200_last_later_launch(int* info) {
+  if (!info) return fail(EDTB200_EINVAL, "null pointer");
+  const LaterLaunch& l = g_last_later;
+  if (l.kernel < 0) return fail(EDTB200_EINVAL, "no later-axis pass has been launched on this thread");
+  const int v[8] = {l.kernel, l.tx, l.tma, l.wide, l.ctas, l.int_hull, l.epilogue, l.all_double};
+  memcpy(info, v, sizeof(v));
+  return 0;
 }
 
 int edtb200_slab_face_runs(const void* labels_dev, int label_bytes, int64_t sx, int64_t sy, int64_t sz,
@@ -1074,7 +1186,8 @@ int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64
       const float ws[2] = {wx, wy};
       const int64_t ns[2] = {sx, sy};
       if (!wrc) wrc = dispatch_later(label_bytes, me.lz, me.fz, geom_for_axis(1, sx, sy, me.zc), wy, border, border, 0,
-                                     *dc, me.stream, /*pdl=*/true, integer_bound(ws, ns, 1));
+                                     *dc, me.stream, /*pdl=*/true, integer_bound(ws, ns, 1),
+                                     transform_sums_exact(ws, ns, 1));
       if (wrc) note(wrc);
       MULTI_TRY(cudaEventRecord(me.after_y, me.stream));
     }
@@ -1090,10 +1203,10 @@ int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64
                            row_l, me.yc, src.zc, me.stream));
       }
       if (!wrc) {
-        const float ws[2] = {wx, wy};
-        const int64_t ns[2] = {sx, sy};
+        const float ws[3] = {wx, wy, wz};
+        const int64_t ns[3] = {sx, sy, sz};
         wrc = dispatch_later(label_bytes, me.ly, me.fy, geom_for_axis(2, sx, me.yc, sz), wz, border, border, epilogue,
-                             *dc, me.stream, /*pdl=*/false, integer_bound(ws, ns, 2));
+                             *dc, me.stream, /*pdl=*/false, integer_bound(ws, ns, 2), transform_sums_exact(ws, ns, 2));
         if (wrc) note(wrc);
       }
       MULTI_TRY(cudaEventRecord(me.after_z, me.stream));
@@ -1183,10 +1296,10 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   stamp(1);
   mark_pass(1, stream);
   nvtx_push("edt.y");
-  const float ws[2] = {wx, wy};
-  const int64_t ns[2] = {sx, sy};
+  const float ws[3] = {wx, wy, wz};
+  const int64_t ns[3] = {sx, sy, sz};
   rc = dispatch_later(label_bytes, labels_dev, f_dev, gy, wy, border, border, 0, *dc, stream, /*pdl=*/!verbose,
-                      integer_bound(ws, ns, 1));
+                      integer_bound(ws, ns, 1), transform_sums_exact(ws, ns, 1));
   nvtx_pop();
   if (rc) return rc;
   stamp(2);
@@ -1224,7 +1337,8 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   // Z pass on the slab, interior faces open
   nvtx_push("edt.z");
   rc = dispatch_later(label_bytes, labels_dev, f_dev, gz, wz, border && !has_lo, border && !has_hi, epilogue, *dc,
-                      stream, /*pdl=*/!verbose && (has_lo || has_hi), integer_bound(ws, ns, 2));
+                      stream, /*pdl=*/!verbose && (has_lo || has_hi), integer_bound(ws, ns, 2),
+                      transform_sums_exact(ws, ns, 2));
   nvtx_pop();
   if (rc) return rc;
 

@@ -90,9 +90,19 @@ int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream);
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
                  DeviceCache& dc, cudaStream_t stream);
+// exact: every candidate w2 * d^2 + f of the pass is exact in double (see sums_exact); when it is
+// not, the pass runs the long-line kernel with every candidate formed in double.
 template <int Bytes>
 int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
-                 int flags, DeviceCache& dc, cudaStream_t stream, bool pdl, double fmax);
+                 int flags, DeviceCache& dc, cudaStream_t stream, bool pdl, double fmax, bool exact);
+
+// Kernel variant of the last later-axis launch of the calling thread (edtb200_last_later_launch):
+// written by launch_later after a successful launch, read by nothing else.
+struct LaterLaunch {
+  int kernel = -1;      // 0 = tile kernel, 1 = long-line kernel, -1 = no launch yet
+  int tx = 0, tma = 0, wide = 0, ctas = 0, int_hull = 0, epilogue = 0, all_double = 0;
+};
+extern thread_local LaterLaunch g_last_later;
 
 // Shared memory of one tile of `tx` lines (see later_axis_tile_kernel); tile_path_ok tells whether
 // launch_later takes the shared-memory tile kernel for this geometry.

@@ -693,6 +693,17 @@ __device__ __forceinline__ uint32_t build_hull_rows_int(const TileLine<TX> ln, i
   return hb;
 }
 
+// Is candidate (d1, f1) not above candidate (d0, f0) in exact arithmetic?  Asked when their float32
+// values tie: rounded, the candidates along the hull are only weakly unimodal, and a walk that
+// steps on a rounded tie can pass the exact minimiser (and, walking up row by row, never come
+// back).  w2 (d1^2 - d0^2) is exact in double and so is f1 - f0, because the host gives the tile
+// kernels only passes whose every candidate sum is exact in double (launch_later); the sign of
+// their double sum is therefore exact.  d0, d1 are integers below 4096, so d^2 is exact in float32.
+__device__ __forceinline__ bool tie_not_above(float w2, float d1, float f1, float d0, float f0) {
+  const float dd = __fsub_rn(__fmul_rn(d1, d1), __fmul_rn(d0, d0));
+  return __dadd_rn(__dsub_rn((double)f1, (double)f0), __dmul_rn((double)w2, (double)dd)) <= 0.0;
+}
+
 // Outputs of the rows in `todo` (bit = row - i0): rows of runs that lie INSIDE the chunk (first
 // row at a bit of `starts`, last row at a bit of `ends`).  One loop over the marked rows for every
 // lane; a run's state is set up at its first row.  A run whose rows are not marked in `noncst` is
@@ -744,6 +755,7 @@ __device__ __forceinline__ void read_out_rows_local(const TileLine<TX> ln, int i
       while (v1 >= 0) {
         const float cand = __fmaf_rn(w2f, __fmul_rn(dv1, dv1), fv1);
         if (!(cand <= best)) break;
+        if (cand == best && !tie_not_above(w2f, dv1, fv1, dv, fv)) break;
         best = cand; v = v1; fv = fv1; dv = dv1;
         if (left) { v1 = __ffs(left) - 1; left &= left - 1u; fv1 = ln.fval(i0 + v1); dv1 = (float)(r - v1); }
         else v1 = -1;
@@ -803,7 +815,10 @@ __device__ __forceinline__ void walk_begin(HullWalk& w, const TileLine<TX> ln, i
       const float fu = ln.fval(u);
       const float du = (float)(lo - u);
       const float cand = __fmaf_rn(w2f, __fmul_rn(du, du), fu);
-      if (!(cand < best)) break;
+      // rounded to float32 the candidates are only weakly unimodal: two adjacent vertices that
+      // round to the same value may hide a lower one farther down, so ties are settled exactly
+      if (!(cand <= best)) break;
+      if (cand == best && !tie_not_above(w2f, du, fu, dv, fv)) break;
       best = cand; v = u; fv = fu; dv = du;
     }
     w.v = v; w.fv = fv; w.dv = dv;
@@ -1301,6 +1316,7 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
             while (w.v1 >= 0) {
               const float cand = __fmaf_rn(w2, __fmul_rn(w.dv1, w.dv1), w.fv1);
               if (!(cand <= best)) break;
+              if (cand == best && !tie_not_above(w2, w.dv1, w.fv1, w.dv, w.fv)) break;
               best = cand; w.v = w.v1; w.fv = w.fv1; w.dv = w.dv1;
               walk_advance<TX>(w, ln, i);
             }
@@ -1318,12 +1334,15 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
 }
 
 // ---------------------------------------------------------------------------------------
-// Later-axis pass for lines too long for a shared-memory tile (more than 4096 voxels).  Same
-// arithmetic as the tile kernel; distances of 4096 voxels and more, whose squares are not exact
-// in float32, go through double (parabola_at).
+// Later-axis pass for lines too long for a shared-memory tile (more than 4096 voxels), and for
+// passes whose candidate sums w2 * d^2 + f are not all exact in double (decided by the host).
+// Same arithmetic as the tile kernel; distances from `dbl_from` on go through double: 4096, whose
+// square is not exact in float32, or 0 for the inexact passes.  The double sum rounded once to
+// float32 is the reference's evaluation (src/edt.hpp:232); the single fused multiply-add equals it
+// only when the double sum is exact.
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ float parabola_at(float w2, int d, float height) {
-  if (d < 4096) {
+__device__ __forceinline__ float parabola_at(float w2, int d, float height, int dbl_from = 4096) {
+  if (d < dbl_from) {
     const float e = (float)d;
     return __fmaf_rn(w2, __fmul_rn(e, e), height);
   }
@@ -1340,7 +1359,7 @@ template <int Bytes>
 __global__ void __launch_bounds__(128)
 later_axis_long_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
                        const float* __restrict__ fin, float* __restrict__ fout, int* __restrict__ hull,
-                       LineGeom g, float w2, int border_lo, int border_hi, int flags) {
+                       LineGeom g, float w2, int border_lo, int border_hi, int flags, int dbl_from) {
   using LT = typename LabelOf<Bytes>::type;
   const int64_t lines_per_outer = g.inner_count;
   const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1385,16 +1404,22 @@ later_axis_long_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
     float fv = inf, fv1 = inf;
     if (top >= 0) { v = hull[base + (int64_t)a * ls]; fv = fin[base + (int64_t)v * ls]; }
     if (top >= 1) { v1 = hull[base + (int64_t)(a + 1) * ls]; fv1 = fin[base + (int64_t)v1 * ls]; }
+    // The walk compares the candidates as double sums, not rounded to float32: rounded, they are
+    // only weakly unimodal along the hull, and a step taken on a rounded tie can pass the
+    // minimiser for good.  (Exact wherever w2 d^2 + f is, see launch_later.)
     for (int i = a; i < b; ++i) {
       float best = inf;
       if (top >= 0) {
-        best = parabola_at(w2, abs(i - v), fv);
+        const double dv = (double)abs(i - v);
+        double bestd = __dadd_rn(__dmul_rn(w2d, dv * dv), (double)fv);
         while (k < top) {
-          const float cand = parabola_at(w2, abs(i - v1), fv1);
-          if (!(cand <= best)) break;
-          best = cand; ++k; v = v1; fv = fv1;
+          const double d1 = (double)abs(i - v1);
+          const double cand = __dadd_rn(__dmul_rn(w2d, d1 * d1), (double)fv1);
+          if (!(cand <= bestd)) break;
+          bestd = cand; ++k; v = v1; fv = fv1;
           if (k < top) { v1 = hull[base + (int64_t)(a + k + 1) * ls]; fv1 = fin[base + (int64_t)v1 * ls]; }
         }
+        best = parabola_at(w2, abs(i - v), fv, dbl_from);
       }
       if (lo_border) best = fminf(best, parabola_at(w2, i - a + 1, 0.0f));
       if (hi_border) best = fminf(best, parabola_at(w2, b - i, 0.0f));

@@ -149,6 +149,7 @@ int launch_tile(const void* labels, float* f, LineGeom g, float w2, int border_l
     auto kern = later_axis_tile_kernel<Bytes, TX, EPI, TMA, WIDE, CTAS, IH>;                        \
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
     CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, lab, f, g, tb, w2, border_lo, border_hi, flags, w2i)); \
+    g_last_later = LaterLaunch{0, TX, TMA, WIDE, CTAS, IH, EPI, 0};                                 \
   } while (0)
 #define EDT_LAUNCH_TILE(EPI, TMA)                                                                   \
   do {                                                                                              \
@@ -170,14 +171,16 @@ int launch_tile(const void* labels, float* f, LineGeom g, float w2, int border_l
 
 template <int Bytes>
 int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
-                 int flags, DeviceCache& dc, cudaStream_t stream, bool pdl, double fmax) {
+                 int flags, DeviceCache& dc, cudaStream_t stream, bool pdl, double fmax, bool exact) {
   using LT = typename LabelOf<Bytes>::type;
   LineGeom g = g0;
   const float w2 = w * w;                       // float product, as src/edt.hpp:181
 
   // ---- shared-memory tile kernel: whole lines x TX adjacent lines per CTA ----
+  // Its candidates are single fused multiply-adds, the reference's double sum rounded once only
+  // when that sum is exact: passes where it may not be go the long way.
   const bool fits32 = (int64_t)g.n * g.line_stride + 64 < (1LL << 32);
-  if (fits32 && g.n <= 4096 && g.inner_count < (1LL << 31)) {
+  if (exact && fits32 && g.n <= 4096 && g.inner_count < (1LL << 31)) {
     const bool aligned = reinterpret_cast<uintptr_t>(f) % 16 == 0 && g.line_stride % 4 == 0 &&
                          (g.outer_count <= 1 || g.outer_stride % 4 == 0);
     // Tile width: 128-byte rows (TX = 32) keep DRAM bursts and L2 lines whole, which matters more
@@ -220,8 +223,9 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
     return fail(EDTB200_ELIMIT, "too many lines");
   }
   later_axis_long_kernel<Bytes><<<(unsigned)blocks, 128, 0, stream>>>(
-      static_cast<const LT*>(labels), f, tmp, hull, g, w2, border_lo, border_hi, flags);
+      static_cast<const LT*>(labels), f, tmp, hull, g, w2, border_lo, border_hi, flags, exact ? 4096 : 0);
   CUDA_TRY(cudaGetLastError());
+  g_last_later = LaterLaunch{1, 0, 0, 0, 0, 0, flags != 0, !exact};
   CUDA_TRY(cudaMemcpyAsync(f, tmp, bytes, cudaMemcpyDeviceToDevice, stream));
   CUDA_TRY(cudaFreeAsync(hull, stream));
   CUDA_TRY(cudaFreeAsync(tmp, stream));
@@ -236,4 +240,4 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
                                               edtb200::host::DeviceCache&, cudaStream_t);                \
   template int edtb200::host::launch_later<B>(const void*, float*, const edtb200::LineGeom&, float, int, \
                                               int, int, edtb200::host::DeviceCache&, cudaStream_t, bool, \
-                                              double);
+                                              double, bool);

@@ -31,8 +31,9 @@ extern "C" {
 
 /* 100: round 1 (transform, per-axis passes, slab face kernels).  200: additions only --
  * edtb200_transform_multi, edtb200_slab_step / _stage_bytes / _pack, edtb200_label_stats / _extract,
- * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning. */
-#define EDTB200_VERSION 200
+ * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
+ * 201: additions only -- edtb200_last_later_launch. */
+#define EDTB200_VERSION 201
 
 /* flags */
 #define EDTB200_SQRT             1  /* emit sqrt(edtsq): reference _edt3d (src/edt.hpp:591-604) /
@@ -147,7 +148,10 @@ int edtb200_transform_voxel_graph(const void *labels, int label_bytes, const uns
  *     border_lo / border_hi say independently whether the low / high end of the axis is a
  *     volume face with black_border (an interior slab face is neither).
  *     pass_later works IN PLACE on f_dev (input = the previous pass's output) and only writes
- *     the elements whose value it changes.
+ *     the elements whose value it changes.  f_dev may hold any samples: pass_later first reduces
+ *     them on `stream` and waits for that (one small kernel) to learn whether every candidate
+ *     w^2 d^2 + f is exact in double; when one may not be, the pass forms every candidate in
+ *     double and rounds it once, as the reference does.
  */
 int edtb200_pass_first(const void *labels_dev, int label_bytes,
                        int64_t sx, int64_t sy, int64_t sz, float wx,
@@ -265,6 +269,13 @@ void edtb200_host_free(void *p);
  * first, second and third axis pass in milliseconds (0 for passes that did not run). */
 int edtb200_profile_passes(int enable);
 int edtb200_pass_ms(int steps_back, float *ms3);
+
+/* Which kernel variant the last later-axis (Y or Z) pass launched by the calling thread used, so
+ * that tests can tell which code paths they reached.  Read-only: it changes no launch.  Fills
+ * info[0..8): kernel (0 = shared-memory tile, 1 = long-line), tile width TX, TMA staging, wide
+ * CTA, CTAs per SM the tile kernel is compiled for, integer hull tests, epilogue (sqrt / sign in
+ * the store), every candidate formed in double.  EDTB200_EINVAL before any such launch. */
+int edtb200_last_later_launch(int *info);
 
 /* Free every cached device buffer / stream this library holds on all devices. */
 int edtb200_release(void);

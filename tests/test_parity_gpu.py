@@ -2,9 +2,9 @@
 
 Bar (BASELINE.json north_star): edtsq bit-exact on the integer squared-distance path;
 edt / sdf within 1 ULP after sqrt (0 expected: IEEE sqrt on identical inputs).  For
-non-integer anisotropy the kernels evaluate each candidate with one fused multiply-add,
-which equals the reference's double-precision evaluation rounded once except in
-astronomically rare double-rounding ties, so the same exact comparison is applied there.
+non-integer anisotropy the kernels use one fused multiply-add per candidate only where the
+host has proven the double sum exact (and the double form elsewhere), so the same exact
+comparison is applied there; tests/test_envelope_gpu.py covers the rounding edges.
 """
 import os
 import zlib

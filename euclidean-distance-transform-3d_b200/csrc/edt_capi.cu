@@ -49,20 +49,68 @@ EncodeTiledFn tensor_map_encoder() {
   return encode;
 }
 
-size_t tile_smem_bytes(int n, int tx, int rows_alloc) {
-  const int nchunks = (n + 31) >> 5;
-  return (size_t)rows_alloc * tx * 4 + (size_t)nchunks * tx * 12 + (size_t)((n + 3) & ~1) * 4 + 16 +
-         (size_t)nchunks * tx +    // + one flag byte per (chunk, line)
-         (size_t)tx * 4 + 4;       // + one word per line: chunks holding a run start
+// ---- PassArith: the arithmetic of a later-axis pass, from a transform or from its samples ----
+
+// Lowest set bit of v > 0 (a power of two); 0 for v <= 0 or not finite.
+static double lowest_bit(double v) {
+  if (!(v > 0.0) || !std::isfinite(v)) return 0.0;
+  int e = 0;
+  const double m = frexp(v, &e);                                   // v = m 2^e, m in [0.5, 1)
+  const unsigned long long mant = (unsigned long long)ldexp(m, 53);
+  return ldexp(1.0, e - 53 + __builtin_ctzll(mant));
 }
 
-// Will launch_later() take the shared-memory tile kernel for this geometry?  (same conditions)
-bool tile_path_ok(const LineGeom& g, const DeviceCache& dc) {
-  if (!((int64_t)g.n * g.line_stride + 64 < (1LL << 32) && g.n <= 4096 && g.inner_count < (1LL << 31))) return false;
-  const int nb = (g.n + 255) / 256;
-  int br = (g.n + nb - 1) / nb;
-  if (nb > 1) br = (br + 3) & ~3;
-  return tile_smem_bytes(g.n, 8, br * nb) <= (size_t)dc.max_smem_optin;
+// The rule both producers end in, for a pass with squared weight w2 over lines of n finite
+// samples that are at most `top`, whole multiples of `unit` (as w2 is), and integers not above
+// int_bound (-1: not known to be integers).
+static PassArith pass_arith(double int_bound, double top, double unit, float w2, int64_t n) {
+  const double reach = (double)w2 * (double)n * (double)n;
+  PassArith a;
+  a.int_hull = int_bound >= 0.0 && w2 == floorf(w2) && w2 >= 1.0f && w2 < 1048576.0f &&
+               int_bound + reach < 2147483000.0;
+  // w2 d^2 is exact in double (24 + 24 bits), so a sum is exact when it spans at most 53 bits from
+  // `unit` up; then one fused multiply-add rounds what the reference rounds once (src/edt.hpp:232).
+  a.exact = top + reach < 0x1p53 * unit;
+  return a;
+}
+
+// The samples are what the passes along axes 0..k-1 made, at most the sum of w2 * n^2 over those
+// axes (the factor 2 covers their float32 rounding); integers when every squared weight is one
+// and the X pass's distances j * w[0] are integers below 2^24.  The unit:
+//  - when the X pass is exact (every distance j * w[0] below 2^24 units of b0 = lowest_bit(w[0])),
+//    its squares are multiples of b0^2, every w2 = fl32(w * w) is a multiple of its lowest set bit,
+//    and float32 rounding keeps a multiple of a power of two P a multiple of P: so every sample and
+//    candidate is a multiple of the least of b0^2 and those bits (1 or more for integer weights,
+//    1/4 for weights of 0.5, ...);
+//  - otherwise every positive sample is at least the least squared weight (the X pass's smallest
+//    distance is one step), so half the float32 spacing there divides them all.
+PassArith transform_arith(const float* w, const int64_t* n, int k) {
+  double top = 0.0;
+  float least = INFINITY;
+  const double b0 = lowest_bit((double)w[0]);
+  double unit = b0 * b0;
+  const bool x_exact = b0 > 0.0 && (double)w[0] * (double)n[0] < 16777216.0 * b0;
+  bool integral = (double)w[0] == floor((double)w[0]) && (double)w[0] * (double)n[0] < 16777216.0;
+  for (int i = 0; i <= k; ++i) {
+    const float w2 = w[i] * w[i];
+    if (i < k) {
+      top += (double)w2 * (double)n[i] * (double)n[i];
+      integral = integral && w2 == floorf(w2) && w2 >= 1.0f;
+    }
+    least = fminf(least, w2);
+    if (i > 0) unit = fmin(unit, lowest_bit((double)w2));
+  }
+  if (!x_exact || !(unit > 0.0)) unit = 0.5 * ((double)nextafterf(least, INFINITY) - (double)least);
+  return pass_arith(integral ? top : -1.0, 2.0 * top, unit, w[k] * w[k], n[k]);
+}
+
+// Every sample and every w2 d^2 is a multiple of the least of 2^low and w2's lowest set bit; the
+// samples are integers when low >= 0.
+PassArith sampled_arith(float fmax, int low, float w, int64_t n) {
+  const float w2 = w * w;
+  double unit = lowest_bit((double)w2);
+  if (low < 1024) unit = fmin(unit, ldexp(1.0, low));
+  return pass_arith(low >= 0 ? (double)fmax : -1.0, fmax, unit, w2, n);
 }
 
 cudaError_t scratch_alloc(DeviceCache& dc, void** p, size_t bytes, cudaStream_t stream) {
@@ -391,81 +439,42 @@ int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines
   }
 }
 
-// fmax: an upper bound of the finite samples in f when they are known to be integer-valued (the
-// product of earlier passes with integer weights^2), or -1: enables the integer hull tests.
-// exact: every candidate sum of the pass is exact in double (sums_exact).
 int dispatch_later(int label_bytes, const void* labels, float* f, const edtb200::LineGeom& g, float w,
-                   int lo, int hi, int flags, DeviceCache& dc, cudaStream_t s, bool pdl, double fmax, bool exact) {
+                   int lo, int hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t s, bool pdl) {
   switch (label_bytes) {
-    case 1: return launch_later<1>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
-    case 2: return launch_later<2>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
-    case 4: return launch_later<4>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
-    default: return launch_later<8>(labels, f, g, w, lo, hi, flags, dc, s, pdl, fmax, exact);
+    case 1: return launch_later<1>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
+    case 2: return launch_later<2>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
+    case 4: return launch_later<4>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
+    default: return launch_later<8>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
   }
 }
 
-// Largest finite value the passes along axes of lengths n[0..k) with weights w[0..k) can have
-// produced, if all their squared weights (the float products the kernels use) are integers and
-// the distances stay exact in float32; else -1.  (An X-pass value is fl32(a_k^2) with a_k = k*w
-// exact below 2^24; a later pass adds w2 * d^2 to an earlier value.)
-double integer_bound(const float* w, const int64_t* n, int k) {
-  double bound = 0.0;
-  for (int i = 0; i < k; ++i) {
-    const float w2 = w[i] * w[i];
-    if (!(w2 == floorf(w2)) || w2 < 1.0f) return -1.0;
-    if (i == 0 && !((double)w[0] == floor((double)w[0]) && (double)w[0] * (double)n[0] < 16777216.0)) return -1.0;
-    bound += (double)w2 * (double)n[i] * (double)n[i];
-  }
-  return bound < 2147483000.0 ? bound : -1.0;
+// Kernel flags of a pass from the ABI flags: sqrt and sign act in the store of the last pass;
+// background-as-label (sdf) changes the first pass only -- later passes treat every run alike.
+int kernel_flags(int flags, bool first, bool last) {
+  const int epilogue = ((flags & EDTB200_SQRT) ? edtb200::kSqrt : 0) | ((flags & EDTB200_SIGNED) ? edtb200::kNegate : 0);
+  return (last ? epilogue : 0) | (first && (flags & EDTB200_SIGNED) ? edtb200::kZeroLabel : 0);
 }
 
-// Is every candidate w2 * d^2 + f (d < n) of a later-axis pass exact in double, when the finite
-// samples are at most fmax and every sample, like w2, is a whole multiple of `unit`?  w2 * d^2 is
-// exact in double (24 + 24 bits), so the sum is exact when it spans at most 53 bits from `unit`
-// up.  Then the tile kernel's one fused multiply-add rounds the very sum the reference rounds once
-// from double (src/edt.hpp:232), and the results agree bit for bit; otherwise they may differ by
-// one ulp at a double-rounding tie.
-bool sums_exact(double fmax, double unit, float w2, int64_t n) {
-  return fmax + (double)w2 * (double)n * (double)n < 0x1p53 * unit;
+// One transform: each of its passes derives its kernel flags and arithmetic from these.  w and n
+// are the weights and extents of the whole volume, whatever part of it a pass covers.
+struct Transform {
+  int label_bytes, ndim, flags, border;
+  float w[3];
+  int64_t n[3];
+};
+
+// The X pass over nlines rows.
+int x_pass(const Transform& t, const void* labels, float* f, int64_t nlines, DeviceCache& dc, cudaStream_t s) {
+  return dispatch_first(t.label_bytes, labels, f, nlines, t.n[0], t.w[0], t.border,
+                        kernel_flags(t.flags, true, t.ndim == 1), dc, s);
 }
 
-// Spacing of float32 values at v > 0 (0: the smallest subnormal): every float32 of magnitude v
-// or more is a whole multiple of it.
-double float_spacing(float v) { return (double)nextafterf(v, INFINITY) - (double)v; }
-
-// Lowest set bit of v > 0 (a power of two); 0 for v <= 0 or not finite.
-double lowest_bit(double v) {
-  if (!(v > 0.0) || !std::isfinite(v)) return 0.0;
-  int e = 0;
-  const double m = frexp(v, &e);                                   // v = m 2^e, m in [0.5, 1)
-  const unsigned long long mant = (unsigned long long)ldexp(m, 53);
-  return ldexp(1.0, e - 53 + __builtin_ctzll(mant));
-}
-
-// sums_exact for the later-axis pass along axis k of a transform (weight w[k], length n[k]),
-// whose samples are what the passes along axes 0..k-1 made, at most the sum of w2 * n^2 over those
-// axes (the factor 2 covers their float32 rounding).  The unit:
-//  - when the X pass is exact (every distance j * w[0] below 2^24 units of b0 = lowest_bit(w[0])),
-//    its squares are multiples of b0^2, every w2 = fl32(w * w) is a multiple of its lowest set bit,
-//    and float32 rounding keeps a multiple of a power of two P a multiple of P: so every sample and
-//    candidate is a multiple of the least of b0^2 and those bits (1 or more for integer weights,
-//    1/4 for weights of 0.5, ...);
-//  - otherwise every positive sample is at least the least squared weight (the X pass's smallest
-//    distance is one step), so half the float32 spacing there divides them all.
-bool transform_sums_exact(const float* w, const int64_t* n, int k) {
-  double top = 0.0;
-  float least = INFINITY;
-  const double b0 = lowest_bit((double)w[0]);
-  double unit = b0 * b0;
-  const bool x_exact = b0 > 0.0 && (double)w[0] * (double)n[0] < 16777216.0 * b0;
-  for (int i = 0; i <= k; ++i) {
-    const float w2 = w[i] * w[i];
-    if (i < k) top += (double)w2 * (double)n[i] * (double)n[i];
-    least = fminf(least, w2);
-    if (i > 0) unit = fmin(unit, lowest_bit((double)w2));
-  }
-  if (!x_exact || !(unit > 0.0)) unit = 0.5 * float_spacing(least);
-  return sums_exact(2.0 * top, unit, w[k] * w[k], n[k]);
+// The later pass along axis k over geometry g, with the borders lo / hi at the ends of its lines.
+int later_pass(const Transform& t, int k, const void* labels, float* f, const edtb200::LineGeom& g, int lo, int hi,
+               DeviceCache& dc, cudaStream_t s, bool pdl) {
+  return dispatch_later(t.label_bytes, labels, f, g, t.w[k], lo, hi, kernel_flags(t.flags, false, k == t.ndim - 1),
+                        transform_arith(t.w, t.n, k), dc, s, pdl);
 }
 
 // Largest finite |f| (as float bits: non-negative floats order like their bits) and the exponent
@@ -558,11 +567,7 @@ void nvtx_pop() { if (g_nvtx_pop) g_nvtx_pop(); }
 int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                float wx, float wy, float wz, int border, int flags, float* f,
                DeviceCache& dc, cudaStream_t stream) {
-  using namespace edtb200;
-  // sqrt / sign are applied by whichever pass is the last one; background-as-label (sdf)
-  // changes the first pass only -- later passes treat every run alike.
-  const int epilogue = ((flags & EDTB200_SQRT) ? kSqrt : 0) | ((flags & EDTB200_SIGNED) ? kNegate : 0);
-  const int zero_label = (flags & EDTB200_SIGNED) ? kZeroLabel : 0;
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   // The later passes are launched with programmatic stream serialization: the kernel before them
   // in the stream is our own previous pass, which never writes the labels, so their label staging
   // (before griddepcontrol.wait) may overlap its tail.  The per-axis entry points do not do this:
@@ -571,7 +576,6 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   // re-read wide labels, was tried and dropped: it made the later passes cheaper, but the first
   // pass dearer by more.)
   int rc = 0;
-  const edtb200::LineGeom gy = geom_for_axis(1, sx, sy, sz), gz = geom_for_axis(2, sx, sy, sz);
   // EDT_B200_VERBOSE=1: per-pass device times of every transform on stderr (SURVEY.md section 5).
   // The dump needs the passes to have finished, so a verbose transform synchronises its stream.
   static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
@@ -579,23 +583,18 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   if (verbose) g_profile = true;
   mark_pass(0, stream);
   nvtx_push("edt.x");
-  rc = dispatch_first(label_bytes, labels, f, sy * sz, sx, wx, border, zero_label | (ndim == 1 ? epilogue : 0), dc,
-                      stream);
+  rc = x_pass(t, labels, f, sy * sz, dc, stream);
   nvtx_pop();
   mark_pass(1, stream);
   if (!rc && ndim >= 2) {
     nvtx_push("edt.y");
-    const float ws[2] = {wx, wy}; const int64_t ns[2] = {sx, sy};
-    rc = dispatch_later(label_bytes, labels, f, gy, wy, border, border, ndim == 2 ? epilogue : 0, dc, stream,
-                        /*pdl=*/true, integer_bound(ws, ns, 1), transform_sums_exact(ws, ns, 1));
+    rc = later_pass(t, 1, labels, f, geom_for_axis(1, sx, sy, sz), border, border, dc, stream, /*pdl=*/true);
     nvtx_pop();
     mark_pass(2, stream);
   }
   if (!rc && ndim >= 3) {
     nvtx_push("edt.z");
-    const float ws[3] = {wx, wy, wz}; const int64_t ns[3] = {sx, sy, sz};
-    rc = dispatch_later(label_bytes, labels, f, gz, wz, border, border, epilogue, dc, stream, /*pdl=*/true,
-                        integer_bound(ws, ns, 2), transform_sums_exact(ws, ns, 2));
+    rc = later_pass(t, 2, labels, f, geom_for_axis(2, sx, sy, sz), border, border, dc, stream, /*pdl=*/true);
     nvtx_pop();
     mark_pass(3, stream);
   }
@@ -916,8 +915,8 @@ int edtb200_pass_first(const void* labels_dev, int label_bytes, int64_t sx, int6
   DeviceCache* dc = nullptr;
   rc = probe(device, &dc);
   if (rc) return rc;
-  const int kflags = ((flags & EDTB200_SQRT) ? edtb200::kSqrt : 0) |
-                     ((flags & EDTB200_SIGNED) ? edtb200::kZeroLabel : 0);
+  // EDTB200_SIGNED only makes the background an ordinary label here: no sign is applied
+  const int kflags = kernel_flags(flags, /*first=*/true, /*last=*/true) & ~edtb200::kNegate;
   return dispatch_first(label_bytes, labels_dev, f_dev, sy * sz, sx, wx, black_border != 0, kflags, *dc,
                         static_cast<cudaStream_t>(stream));
 }
@@ -956,17 +955,10 @@ int edtb200_pass_later(const void* labels_dev, int label_bytes, int axis, int64_
   CUDA_TRY(err);
   float fmax;
   memcpy(&fmax, &range[0], sizeof(float));
-  const float w2 = w * w;
-  // every sample and every w2 d^2 is a multiple of `unit`; integer samples and w2 allow the
-  // integer hull tests
-  double unit = lowest_bit((double)w2);
-  if (range[1] < 1024) unit = fmin(unit, ldexp(1.0, range[1]));
-  const bool integral = range[1] >= 0 && w2 == floorf(w2);
   const edtb200::LineGeom g = geom_for_axis(axis, sx, sy, sz);
   return dispatch_later(label_bytes, labels_dev, f_dev, g, w, border_lo != 0, border_hi != 0,
-                        ((flags & EDTB200_SQRT) ? edtb200::kSqrt : 0) |
-                            ((flags & EDTB200_SIGNED) ? edtb200::kNegate : 0),
-                        *dc, s, /*pdl=*/false, integral ? (double)fmax : -1.0, sums_exact(fmax, unit, w2, g.n));
+                        kernel_flags(flags, /*first=*/false, /*last=*/true), sampled_arith(fmax, range[1], w, g.n),
+                        *dc, s, /*pdl=*/false);
 }
 
 int edtb200_last_later_launch(int* info) {
@@ -1054,7 +1046,8 @@ int edtb200_slab_face_fixup(const void* labels_dev, int label_bytes, int64_t sx,
   const int64_t plane = sx * sy;
   const unsigned blocks = (unsigned)((plane + 255) / 256);
   using namespace edtb200;
-  const int kflags = ((flags & EDTB200_SQRT) ? kSqrt : 0) | ((flags & EDTB200_SIGNED) ? (kNegate | kZeroLabel) : 0);
+  // the last pass's store, on a transform whose first pass may have treated background as a label
+  const int kflags = kernel_flags(flags, /*first=*/true, /*last=*/true);
   const float w2 = wz * wz;
   switch (label_bytes) {
     case 1: face_fixup_kernel<1><<<blocks, 256, 0, stream>>>(static_cast<const uint8_t*>(labels_dev), f_dev, plane, (int)sz, high_face, halo, w2, static_cast<const uint8_t*>(nb_label_dev), nb_m_dev, nb_f_dev, kflags, inexact_dev); break;
@@ -1119,7 +1112,6 @@ cudaError_t copy_box(void* dst, size_t dst_row_bytes, int64_t dst_rows_per_slice
 int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                             float wx, float wy, float wz, int black_border, int flags, float* out,
                             const int* devices, int ndevices) {
-  using namespace edtb200;
   if (!devices || ndevices < 1) return fail(EDTB200_EINVAL, "no devices given");
   if (flags & (EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
     return fail(EDTB200_EINVAL, "edtb200_transform_multi splits a HOST volume over the devices");
@@ -1139,8 +1131,7 @@ int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64
                              nullptr);
 
   const int border = black_border != 0;
-  const int zero_label = (flags & EDTB200_SIGNED) ? kZeroLabel : 0;
-  const int epilogue = ((flags & EDTB200_SQRT) ? kSqrt : 0) | ((flags & EDTB200_SIGNED) ? kNegate : 0);
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   std::vector<MultiPart> parts(G);
   for (int d = 0; d < G; ++d) {
     MultiPart& p = parts[d];
@@ -1182,12 +1173,9 @@ int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64
     if (!wrc) {
       const char* src = static_cast<const char*>(labels) + (size_t)me.z0 * sy * row_l;
       wrc = upload(me.lz, src, (size_t)sx * sy * me.zc * label_bytes, me.device, me.stream);
-      if (!wrc) wrc = dispatch_first(label_bytes, me.lz, me.fz, sy * me.zc, sx, wx, border, zero_label, *dc, me.stream);
-      const float ws[2] = {wx, wy};
-      const int64_t ns[2] = {sx, sy};
-      if (!wrc) wrc = dispatch_later(label_bytes, me.lz, me.fz, geom_for_axis(1, sx, sy, me.zc), wy, border, border, 0,
-                                     *dc, me.stream, /*pdl=*/true, integer_bound(ws, ns, 1),
-                                     transform_sums_exact(ws, ns, 1));
+      if (!wrc) wrc = x_pass(t, me.lz, me.fz, sy * me.zc, *dc, me.stream);
+      if (!wrc) wrc = later_pass(t, 1, me.lz, me.fz, geom_for_axis(1, sx, sy, me.zc), border, border, *dc, me.stream,
+                                 /*pdl=*/true);
       if (wrc) note(wrc);
       MULTI_TRY(cudaEventRecord(me.after_y, me.stream));
     }
@@ -1203,10 +1191,8 @@ int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64
                            row_l, me.yc, src.zc, me.stream));
       }
       if (!wrc) {
-        const float ws[3] = {wx, wy, wz};
-        const int64_t ns[3] = {sx, sy, sz};
-        wrc = dispatch_later(label_bytes, me.ly, me.fy, geom_for_axis(2, sx, me.yc, sz), wz, border, border, epilogue,
-                             *dc, me.stream, /*pdl=*/false, integer_bound(ws, ns, 2), transform_sums_exact(ws, ns, 2));
+        wrc = later_pass(t, 2, me.ly, me.fy, geom_for_axis(2, sx, me.yc, sz), border, border, *dc, me.stream,
+                         /*pdl=*/false);
         if (wrc) note(wrc);
       }
       MULTI_TRY(cudaEventRecord(me.after_z, me.stream));
@@ -1274,9 +1260,7 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   if (rc) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
   const int border = black_border != 0;
-  const int zero_label = (flags & EDTB200_SIGNED) ? kZeroLabel : 0;
-  const int epilogue = ((flags & EDTB200_SQRT) ? kSqrt : 0) | ((flags & EDTB200_SIGNED) ? kNegate : 0);
-  const edtb200::LineGeom gy = geom_for_axis(1, sx, sy, sz), gz = geom_for_axis(2, sx, sy, sz);
+  const Transform t{label_bytes, 3, flags, border, {wx, wy, wz}, {sx, sy, sz}};
 
   // EDT_B200_VERBOSE=1: device time of every phase of the step on stderr (synchronises the stream)
   static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
@@ -1290,16 +1274,14 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   mark_pass(0, stream);              // per-pass events for bench.py (edtb200_profile_passes), as in run_passes
   // X and Y passes: slab-local
   nvtx_push("edt.x");
-  rc = dispatch_first(label_bytes, labels_dev, f_dev, sy * sz, sx, wx, border, zero_label, *dc, stream);
+  rc = x_pass(t, labels_dev, f_dev, sy * sz, *dc, stream);
   nvtx_pop();
   if (rc) return rc;
   stamp(1);
   mark_pass(1, stream);
   nvtx_push("edt.y");
-  const float ws[3] = {wx, wy, wz};
-  const int64_t ns[3] = {sx, sy, sz};
-  rc = dispatch_later(label_bytes, labels_dev, f_dev, gy, wy, border, border, 0, *dc, stream, /*pdl=*/!verbose,
-                      integer_bound(ws, ns, 1), transform_sums_exact(ws, ns, 1));
+  rc = later_pass(t, 1, labels_dev, f_dev, geom_for_axis(1, sx, sy, sz), border, border, *dc, stream,
+                  /*pdl=*/!verbose);
   nvtx_pop();
   if (rc) return rc;
   stamp(2);
@@ -1336,9 +1318,8 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   mark_pass(2, stream);              // "second pass" = Y plus the face staging kernel
   // Z pass on the slab, interior faces open
   nvtx_push("edt.z");
-  rc = dispatch_later(label_bytes, labels_dev, f_dev, gz, wz, border && !has_lo, border && !has_hi, epilogue, *dc,
-                      stream, /*pdl=*/!verbose && (has_lo || has_hi), integer_bound(ws, ns, 2),
-                      transform_sums_exact(ws, ns, 2));
+  rc = later_pass(t, 2, labels_dev, f_dev, geom_for_axis(2, sx, sy, sz), border && !has_lo, border && !has_hi, *dc,
+                  stream, /*pdl=*/!verbose && (has_lo || has_hi));
   nvtx_pop();
   if (rc) return rc;
 
@@ -1346,7 +1327,7 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   mark_pass(3, stream);
   if (has_lo || has_hi) {
     nvtx_push("edt.halo.fixup");
-    const int kflags = epilogue | zero_label;
+    const int kflags = kernel_flags(flags, /*first=*/true, /*last=*/true);
     const float w2 = wz * wz;
     const unsigned char* set_lo = has_lo ? lo + (size_t)parity * L.set_bytes : nullptr;
     const unsigned char* set_hi = has_hi ? hi + (size_t)parity * L.set_bytes : nullptr;

@@ -86,28 +86,32 @@ int step_table(DeviceCache& dc, float w, int count, cudaStream_t stream, const f
 // retired later without a device-wide synchronisation).
 int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream);
 
+// Arithmetic of one later-axis pass.  int_hull: every sample is an integer and every
+// g = f + w2 v^2 an exact 32-bit integer (the integer hull tests apply).  exact: every candidate
+// w2 d^2 + f is exact in double, so the tile kernels' fused multiply-add rounds the reference's
+// sum; otherwise the long-line kernel forms every candidate in double.
+struct PassArith { bool int_hull = false, exact = false; };
+// The pass along axis k of a transform with weights w[0..k] over the volume's extents n[0..k].
+PassArith transform_arith(const float* w, const int64_t* n, int k);
+// A pass with weight w over lines of n samples whose largest finite magnitude is fmax and whose
+// lowest set bit over the finite non-zero samples is 2^low (1024: there is none).
+PassArith sampled_arith(float fmax, int low, float w, int64_t n);
+
 // Axis-pass launchers, one instantiation per label width (edt_passes.cuh).
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
                  DeviceCache& dc, cudaStream_t stream);
-// exact: every candidate w2 * d^2 + f of the pass is exact in double (see sums_exact); when it is
-// not, the pass runs the long-line kernel with every candidate formed in double.
 template <int Bytes>
 int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
-                 int flags, DeviceCache& dc, cudaStream_t stream, bool pdl, double fmax, bool exact);
+                 int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl);
 
-// Kernel variant of the last later-axis launch of the calling thread (edtb200_last_later_launch):
-// written by launch_later after a successful launch, read by nothing else.
+// What a later-axis launch runs (plan_later in edt_passes.cuh); the last one launched on the
+// calling thread is kept for edtb200_last_later_launch.
 struct LaterLaunch {
   int kernel = -1;      // 0 = tile kernel, 1 = long-line kernel, -1 = no launch yet
   int tx = 0, tma = 0, wide = 0, ctas = 0, int_hull = 0, epilogue = 0, all_double = 0;
 };
 extern thread_local LaterLaunch g_last_later;
-
-// Shared memory of one tile of `tx` lines (see later_axis_tile_kernel); tile_path_ok tells whether
-// launch_later takes the shared-memory tile kernel for this geometry.
-size_t tile_smem_bytes(int n, int tx, int rows_alloc);
-bool tile_path_ok(const LineGeom& g, const DeviceCache& dc);
 
 }  // namespace host
 }  // namespace edtb200

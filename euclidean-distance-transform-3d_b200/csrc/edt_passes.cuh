@@ -29,8 +29,7 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
       reinterpret_cast<uintptr_t>(f) % 16 == 0) {
     const size_t smem = sizeof(float) * (size_t)(sx + 2);
     int64_t blocks = (nlines + 7) / 8;
-    static const int xgrid = getenv("EDTB200_X_GRID") ? atoi(getenv("EDTB200_X_GRID")) : 0;     // A/B switch
-    const int64_t cap = (int64_t)dc.sm_count * (xgrid ? xgrid : (sx > 512 ? 12 : 15));   // whole waves at 5 (rows <= 512) / 3 CTAs per SM
+    const int64_t cap = (int64_t)dc.sm_count * (sx > 512 ? 12 : 15);   // whole waves at 5 (rows <= 512) / 3 CTAs per SM
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
     const LT* lab = static_cast<const LT*>(labels);
@@ -107,106 +106,118 @@ inline void tile_boxes(int n, TileBoxes* tb) {
   if (tb->nboxes > 1) tb->box_rows = (tb->box_rows + 3) & ~3;      // keeps every box 128-byte aligned
 }
 
-template <int Bytes, int TX>
-int launch_tile(const void* labels, float* f, LineGeom g, float w2, int border_lo, int border_hi, int flags,
-                bool use_tma, cudaStream_t stream, bool pdl, bool noise, bool int_hull) {
-  using LT = typename LabelOf<Bytes>::type;
-  const int nchunks = (g.n + 31) >> 5;
-  TileBoxes tb;
-  tile_boxes(g.n, &tb);
-  g.tiles_per_outer = (int)((g.inner_count + TX - 1) / TX);
-  const int64_t tiles = (int64_t)g.tiles_per_outer * g.outer_count;
-  if (tiles > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many line tiles");
-  CUtensorMap map;
-  memset(&map, 0, sizeof(map));
-  if (use_tma && !make_tile_map(&map, f, g, TX, tb.box_rows)) use_tma = false;
-  const int rows_alloc = use_tma ? tb.box_rows * tb.nboxes : g.n;
-  const size_t smem = tile_smem_bytes(g.n, TX, rows_alloc);
-  constexpr int SUBS = 32 / TX;
-  int warps = (nchunks + SUBS - 1) / SUBS;
-  const bool wide = warps > 16;                 // long lines: one tile per SM, so give it 32 warps
-  if (warps > 32) warps = 32;
-  const LT* lab = static_cast<const LT*>(labels);
-  // Programmatic dependent launch: this pass may begin (label staging) while the previous pass of
-  // the stream drains its last wave; the kernel itself waits before touching the distances.
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)tiles);
-  cfg.blockDim = dim3((unsigned)(warps * 32));
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute pdl_attr[1];
-  pdl_attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  pdl_attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = pdl_attr;
-  static const bool pdl_off = getenv("EDTB200_NO_PDL") != nullptr;    // A/B switch for measurements
-  cfg.numAttrs = (pdl && !pdl_off) ? 1 : 0;   // only when the previous kernel of the stream is our own pass
-  const int w2i = int_hull ? (int)w2 : 0;
-  static const bool int_off = getenv("EDTB200_NO_INT_HULL") != nullptr;     // A/B switch for measurements
-  // integer hull tests are instantiated for the hot shape only (128-byte rows, TMA staging)
-  const bool ih = int_hull && !int_off && TX == 32 && use_tma;
-#define EDT_LAUNCH_ONE(EPI, TMA, WIDE, CTAS, IH)                                                    \
-  do {                                                                                              \
-    auto kern = later_axis_tile_kernel<Bytes, TX, EPI, TMA, WIDE, CTAS, IH>;                        \
-    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));   \
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, lab, f, g, tb, w2, border_lo, border_hi, flags, w2i)); \
-    g_last_later = LaterLaunch{0, TX, TMA, WIDE, CTAS, IH, EPI, 0};                                 \
-  } while (0)
-#define EDT_LAUNCH_TILE(EPI, TMA)                                                                   \
-  do {                                                                                              \
-    if constexpr (TX == 32 && TMA) {                                                                \
-      if (wide) { if (ih) EDT_LAUNCH_ONE(EPI, TMA, true, 3, true); else EDT_LAUNCH_ONE(EPI, TMA, true, 3, false); } \
-      else if (noise) { if (ih) EDT_LAUNCH_ONE(EPI, TMA, false, 2, true); else EDT_LAUNCH_ONE(EPI, TMA, false, 2, false); } \
-      else { if (ih) EDT_LAUNCH_ONE(EPI, TMA, false, 3, true); else EDT_LAUNCH_ONE(EPI, TMA, false, 3, false); } \
-    } else {                                                                                        \
-      if (wide) EDT_LAUNCH_ONE(EPI, TMA, true, 3, false); else EDT_LAUNCH_ONE(EPI, TMA, false, 3, false); \
-    }                                                                                               \
-  } while (0)
-  if (flags) { if (use_tma) EDT_LAUNCH_TILE(true, true); else EDT_LAUNCH_TILE(true, false); }
-  else       { if (use_tma) EDT_LAUNCH_TILE(false, true); else EDT_LAUNCH_TILE(false, false); }
-#undef EDT_LAUNCH_TILE
-#undef EDT_LAUNCH_ONE
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+// Shared memory of one tile of `tx` lines (see later_axis_tile_kernel).
+inline size_t tile_smem_bytes(int n, int tx, int rows_alloc) {
+  const int nchunks = (n + 31) >> 5;
+  return (size_t)rows_alloc * tx * 4 + (size_t)nchunks * tx * 12 + (size_t)((n + 3) & ~1) * 4 + 16 +
+         (size_t)nchunks * tx +    // + one flag byte per (chunk, line)
+         (size_t)tx * 4 + 4;       // + one word per line: chunks holding a run start
+}
+
+// Warps of a tile of `tx` lines (32-row chunks, 32 / tx lines per warp) before the cap at 32;
+// more than 16 makes the wide variant.
+inline int tile_warps(int n, int tx) { return (((n + 31) >> 5) * tx + 31) / 32; }
+
+// The plan of one later-axis pass: what launch_later runs for it.  Pure host logic.
+//   tma_ok       the volume is 16-byte aligned and (when asked again) its tensor map encoded
+//   noise        noise_predicted: 2 CTAs per SM instead of 3
+//   int_hull_off EDTB200_NO_INT_HULL
+inline LaterLaunch plan_later(const LineGeom& g, bool epilogue, PassArith arith, int max_smem_optin, bool tma_ok,
+                              bool noise, bool int_hull_off) {
+  // ---- shared-memory tile kernel: whole lines x tx adjacent lines per CTA ----
+  // Its candidates are single fused multiply-adds, the reference's double sum rounded once only
+  // when that sum is exact: passes where it may not be go the long way.
+  const bool fits32 = (int64_t)g.n * g.line_stride + 64 < (1LL << 32);
+  if (arith.exact && fits32 && g.n <= 4096 && g.inner_count < (1LL << 31)) {
+    // Tile width: 128-byte rows (TX = 32) keep DRAM bursts and L2 lines whole, which matters more
+    // than occupancy even at one CTA per SM; narrower tiles only when a 32-wide tile cannot fit.
+    TileBoxes tb;
+    tile_boxes(g.n, &tb);
+    int tx = 0;
+    for (int cand = 32; cand >= 8 && !tx; cand >>= 1)
+      if (tile_smem_bytes(g.n, cand, tb.box_rows * tb.nboxes) <= (size_t)max_smem_optin) tx = cand;
+    const bool wide = tx && tile_warps(g.n, tx) > 16;   // long lines: one tile per SM, so give it 32 warps
+    // Narrow tiles are compiled wide only: they are chosen when a 32-wide tile does not fit, which
+    // with sm_90a's 227 KB happens from 1597 rows on, where a 16-wide tile has 25 warps (and an
+    // 8-wide one, needed from about 3100 rows, as many).  Otherwise the long-line kernel runs.
+    if (tx == 32 || wide) {
+      const bool tma = tma_ok && g.inner_count >= tx;
+      // 2 CTAs per SM and the integer hull tests are compiled for the hot shape only (128-byte
+      // rows, TMA staging)
+      return LaterLaunch{0, tx, tma, wide, tx == 32 && tma && !wide && noise ? 2 : 3,
+                         arith.int_hull && !int_hull_off && tx == 32 && tma, epilogue, 0};
+    }
+  }
+  // ---- lines too long for a shared-memory tile, or sums not exact in double ----
+  return LaterLaunch{1, 0, 0, 0, 0, 0, epilogue, !arith.exact};
+}
+
+// The tile-kernel instance of plan p (Epi, TMA = p.epilogue, p.tma): only the variants
+// plan_later can produce are compiled.
+template <int Bytes>
+using TileKernel = decltype(&later_axis_tile_kernel<Bytes, 32, false, false, false, 3, false>);
+template <int Bytes, bool Epi, bool TMA>
+TileKernel<Bytes> tile_kernel(const LaterLaunch& p) {
+  if (p.tx == 16) return later_axis_tile_kernel<Bytes, 16, Epi, TMA, true, 3, false>;
+  if (p.tx == 8) return later_axis_tile_kernel<Bytes, 8, Epi, TMA, true, 3, false>;
+  if constexpr (TMA) {
+    if (p.wide) return p.int_hull ? later_axis_tile_kernel<Bytes, 32, Epi, true, true, 3, true>
+                                  : later_axis_tile_kernel<Bytes, 32, Epi, true, true, 3, false>;
+    if (p.ctas == 2) return p.int_hull ? later_axis_tile_kernel<Bytes, 32, Epi, true, false, 2, true>
+                                       : later_axis_tile_kernel<Bytes, 32, Epi, true, false, 2, false>;
+    return p.int_hull ? later_axis_tile_kernel<Bytes, 32, Epi, true, false, 3, true>
+                      : later_axis_tile_kernel<Bytes, 32, Epi, true, false, 3, false>;
+  }
+  return p.wide ? later_axis_tile_kernel<Bytes, 32, Epi, false, true, 3, false>
+                : later_axis_tile_kernel<Bytes, 32, Epi, false, false, 3, false>;
 }
 
 template <int Bytes>
 int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
-                 int flags, DeviceCache& dc, cudaStream_t stream, bool pdl, double fmax, bool exact) {
+                 int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl) {
   using LT = typename LabelOf<Bytes>::type;
   LineGeom g = g0;
   const float w2 = w * w;                       // float product, as src/edt.hpp:181
+  static const bool int_hull_off = getenv("EDTB200_NO_INT_HULL") != nullptr;     // A/B switch for measurements
+  const bool aligned = reinterpret_cast<uintptr_t>(f) % 16 == 0 && g.line_stride % 4 == 0 &&
+                       (g.outer_count <= 1 || g.outer_stride % 4 == 0);
+  const bool noise = noise_predicted(dc);
+  LaterLaunch p = plan_later(g, flags != 0, arith, dc.max_smem_optin, aligned, noise, int_hull_off);
 
-  // ---- shared-memory tile kernel: whole lines x TX adjacent lines per CTA ----
-  // Its candidates are single fused multiply-adds, the reference's double sum rounded once only
-  // when that sum is exact: passes where it may not be go the long way.
-  const bool fits32 = (int64_t)g.n * g.line_stride + 64 < (1LL << 32);
-  if (exact && fits32 && g.n <= 4096 && g.inner_count < (1LL << 31)) {
-    const bool aligned = reinterpret_cast<uintptr_t>(f) % 16 == 0 && g.line_stride % 4 == 0 &&
-                         (g.outer_count <= 1 || g.outer_stride % 4 == 0);
-    // Tile width: 128-byte rows (TX = 32) keep DRAM bursts and L2 lines whole, which matters more
-    // than occupancy even at one CTA per SM; narrower tiles only when a 32-wide tile cannot fit.
-    int tx = 0;
-    for (int cand = 32; cand >= 8 && !tx; cand >>= 1) {
-      TileBoxes tb;
-      tile_boxes(g.n, &tb);
-      if (tile_smem_bytes(g.n, cand, tb.box_rows * tb.nboxes) <= (size_t)dc.max_smem_optin) tx = cand;
-    }
-    if (tx) {
-      const bool use_tma = aligned && g.inner_count >= tx;
-      const bool noise = noise_predicted(dc);
-      // Integer hull tests: the caller vouches (fmax >= 0) that every finite sample of f is an
-      // integer not above fmax; with an integer w2 and fmax + w2 * n^2 < 2^31 every g = f + w2 v^2
-      // is an exact 32-bit integer.  fmax < 0 = unknown -> double.
-      const bool int_hull = fmax >= 0.0 && w2 == floorf(w2) && w2 >= 1.0f && w2 < 1048576.0f &&
-                            fmax + (double)w2 * (double)g.n * (double)g.n < 2147483000.0;
-      switch (tx) {
-        case 32: return launch_tile<Bytes, 32>(labels, f, g, w2, border_lo, border_hi, flags, use_tma, stream, pdl, noise, int_hull);
-        case 16: return launch_tile<Bytes, 16>(labels, f, g, w2, border_lo, border_hi, flags, use_tma, stream, pdl, noise, int_hull);
-        default: return launch_tile<Bytes, 8>(labels, f, g, w2, border_lo, border_hi, flags, use_tma, stream, pdl, noise, int_hull);
-      }
-    }
+  if (p.kernel == 0) {
+    TileBoxes tb;
+    tile_boxes(g.n, &tb);
+    g.tiles_per_outer = (int)((g.inner_count + p.tx - 1) / p.tx);
+    const int64_t tiles = (int64_t)g.tiles_per_outer * g.outer_count;
+    if (tiles > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many line tiles");
+    CUtensorMap map;
+    memset(&map, 0, sizeof(map));
+    if (p.tma && !make_tile_map(&map, f, g, p.tx, tb.box_rows))
+      p = plan_later(g, flags != 0, arith, dc.max_smem_optin, false, noise, int_hull_off);
+    const int warps = tile_warps(g.n, p.tx);
+    // Programmatic dependent launch: this pass may begin (label staging) while the previous pass of
+    // the stream drains its last wave; the kernel itself waits before touching the distances.
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)tiles);
+    cfg.blockDim = dim3((unsigned)((warps > 32 ? 32 : warps) * 32));
+    cfg.dynamicSmemBytes = tile_smem_bytes(g.n, p.tx, p.tma ? tb.box_rows * tb.nboxes : g.n);
+    cfg.stream = stream;
+    cudaLaunchAttribute pdl_attr[1];
+    pdl_attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    pdl_attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = pdl_attr;
+    cfg.numAttrs = pdl ? 1 : 0;   // only when the previous kernel of the stream is our own pass
+    const TileKernel<Bytes> kern =
+        p.epilogue ? (p.tma ? tile_kernel<Bytes, true, true>(p) : tile_kernel<Bytes, true, false>(p))
+                   : (p.tma ? tile_kernel<Bytes, false, true>(p) : tile_kernel<Bytes, false, false>(p));
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, static_cast<const LT*>(labels), f, g, tb, w2, border_lo, border_hi,
+                                flags, p.int_hull ? (int)w2 : 0));
+    g_last_later = p;
+    CUDA_TRY(cudaGetLastError());
+    return 0;
   }
-  // ---- lines too long for a shared-memory tile: out of place through a temporary volume ----
+  // ---- long-line kernel: out of place through a temporary volume ----
   const int64_t lines = g.inner_count * g.outer_count;
   const size_t bytes = sizeof(float) * (size_t)lines * (size_t)g.n;
   float* tmp = nullptr;
@@ -223,9 +234,9 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
     return fail(EDTB200_ELIMIT, "too many lines");
   }
   later_axis_long_kernel<Bytes><<<(unsigned)blocks, 128, 0, stream>>>(
-      static_cast<const LT*>(labels), f, tmp, hull, g, w2, border_lo, border_hi, flags, exact ? 4096 : 0);
+      static_cast<const LT*>(labels), f, tmp, hull, g, w2, border_lo, border_hi, flags, p.all_double ? 0 : 4096);
   CUDA_TRY(cudaGetLastError());
-  g_last_later = LaterLaunch{1, 0, 0, 0, 0, 0, flags != 0, !exact};
+  g_last_later = p;
   CUDA_TRY(cudaMemcpyAsync(f, tmp, bytes, cudaMemcpyDeviceToDevice, stream));
   CUDA_TRY(cudaFreeAsync(hull, stream));
   CUDA_TRY(cudaFreeAsync(tmp, stream));
@@ -239,5 +250,5 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
   template int edtb200::host::launch_first<B>(const void*, float*, int64_t, int64_t, float, int, int,    \
                                               edtb200::host::DeviceCache&, cudaStream_t);                \
   template int edtb200::host::launch_later<B>(const void*, float*, const edtb200::LineGeom&, float, int, \
-                                              int, int, edtb200::host::DeviceCache&, cudaStream_t, bool, \
-                                              double, bool);
+                                              int, int, edtb200::host::PassArith,                        \
+                                              edtb200::host::DeviceCache&, cudaStream_t, bool);

@@ -56,7 +56,6 @@ def main():
     print(json.dumps({"workload": name, "size": args.size, "label_bytes": L, "ms": round(ms, 4),
                       "Mvox_s": round(nvox / ms / 1e3, 1),
                       "alg_GBps": round((3 * L + 20) * nvox / ms / 1e6, 1),
-                      "slab_mb": os.environ.get("EDTB200_XY_SLAB_MB", "default"),
                       "finite_max": float(out[torch.isfinite(out)].max().item()) if torch.isfinite(out).any() else None}),
           flush=True)
     del lab, out

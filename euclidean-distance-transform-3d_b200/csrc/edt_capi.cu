@@ -1334,7 +1334,8 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
     const unsigned long long* flag_from_lo = reinterpret_cast<const unsigned long long*>(self + L.flag_from_lo);
     const unsigned long long* flag_from_hi = reinterpret_cast<const unsigned long long*>(self + L.flag_from_hi);
     cudaLaunchConfig_t fcfg = {};
-    fcfg.gridDim = grid; fcfg.blockDim = dim3(256); fcfg.dynamicSmemBytes = 0; fcfg.stream = stream;
+    fcfg.gridDim = dim3(grid.x);             // both faces of a line in one thread, low face first
+    fcfg.blockDim = dim3(256); fcfg.dynamicSmemBytes = 0; fcfg.stream = stream;
     cudaLaunchAttribute fattr[1];
     fattr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     fattr[0].val.programmaticStreamSerializationAllowed = 1;

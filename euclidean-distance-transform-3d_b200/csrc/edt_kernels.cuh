@@ -1438,8 +1438,13 @@ later_axis_long_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
 //   * neighbour label equal  : the neighbour's part of the run (m <= H rows, it must end inside
 //     the neighbour's slab) contributes its rows as sites, plus the zero-height site behind it.
 // Every such site lies outside the slab, so against the slab-local envelope its parabola only
-// gets worse (by at least 2*w2 per row) as rows move away from the face: the walk along a
-// column stops at the first row where no outside site improves the value.
+// gets worse (by at least 2*w2 per row) as rows move away from the face.  Every candidate is the
+// double sum w2 * d^2 + f rounded once to float32, the reference's evaluation.  The walk along a
+// column stops at the first row where the best outside candidate is STRICTLY above the row's
+// value: rounding is monotone, so that row's exact outside minimum is above its exact inside one,
+// and the gap only widens further on.  A rounded tie proves nothing (the exact difference may
+// still be negative and round lower a row later), so the walk goes on over ties; it stores only
+// values strictly below the current one.
 // Values are compared after the pass's epilogue: sqrt is monotone and the sign of a run is
 // fixed, so min() commutes with both.
 // ---------------------------------------------------------------------------------------
@@ -1504,7 +1509,7 @@ face_fixup_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, floa
   {
     const float cur0 = fabsf(f[row0 * plane + q]);
     const float reach0 = (flags & kSqrt) ? cur0 * cur0 * 1.000001f : cur0;
-    while (held < min(m, kSiteCap) && parabola_at(w2, 1 + held, 0.0f) < reach0) {
+    while (held < min(m, kSiteCap) && parabola_at(w2, 1 + held, 0.0f, 0) <= reach0) {
       sites[held] = nb_f[(high_face ? (int64_t)held : (int64_t)(H - 1 - held)) * plane + q];
       ++held;
     }
@@ -1513,24 +1518,25 @@ face_fixup_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, floa
     const int64_t at = (row0 + step * j) * plane + q;
     if (j > 0 && labels[at] != lab0) break;                   // end of the run inside this slab
     const float cur = fabsf(f[at]);
-    // a site at distance d costs at least w2 * d^2: beyond the current value's reach nothing helps
+    // a site at distance d costs at least w2 * d^2: strictly beyond the current value's reach it
+    // is strictly above the row's exact value, and stays so on every later row
     const float reach = (flags & kSqrt) ? cur * cur * 1.000001f : cur;
     // best outside site for row j: neighbour rows r = 0..m-1 at distance j + 1 + r, then (if the
     // run ends there) the zero-height site behind them at distance j + 1 + m
-    float best = unseen ? CUDART_INF_F : parabola_at(w2, j + 1 + m, 0.0f);
+    float best = unseen ? CUDART_INF_F : parabola_at(w2, j + 1 + m, 0.0f, 0);
     for (int r = 0; r < m; ++r) {
-      if (parabola_at(w2, j + 1 + r, 0.0f) >= reach) break;
+      if (parabola_at(w2, j + 1 + r, 0.0f, 0) > reach) break;
       const float height = r < held ? sites[r] : nb_f[(high_face ? (int64_t)r : (int64_t)(H - 1 - r)) * plane + q];
-      best = fminf(best, parabola_at(w2, j + 1 + r, height));
+      best = fminf(best, parabola_at(w2, j + 1 + r, height, 0));
     }
     if (flags & kSqrt) best = __fsqrt_rn(best);
     if (unseen) {
-      float bound = parabola_at(w2, j + H, 0.0f);
+      float bound = parabola_at(w2, j + H, 0.0f, 0);
       if (flags & kSqrt) bound = __fsqrt_rn(bound);
       if (!(fminf(best, cur) <= bound) && inexact) *inexact = 1;
     }
-    if (!(best < cur)) break;                                 // no outside site helps from here on
-    f[at] = negative ? -best : best;
+    if (best > cur) break;                                    // no outside site helps from here on
+    if (best < cur) f[at] = negative ? -best : best;
   }
 }
 

@@ -104,42 +104,14 @@ slab_stage_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, cons
   }
 }
 
-// Both faces in one launch (blockIdx.y = face); waits for the neighbour's staging set of `step`
-// and then does what face_fixup_kernel does, reading the neighbour's set over NVLink.
-// *status: bit 0 = halo too shallow for this volume (see face_fixup_kernel), bit 1 = the
-// neighbour never published the step (time-out).
+// One face of line q, as face_fixup_kernel does it, reading the neighbour's set over NVLink.
 template <int Bytes>
-__global__ void __launch_bounds__(256)
-slab_fixup_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, float* __restrict__ f, int64_t plane,
-                  int nz, int halo, float w2, int has_lo, int has_hi, const unsigned char* __restrict__ set_lo_peer,
-                  const unsigned char* __restrict__ set_hi_peer, SlabStageLayout L, unsigned long long step,
-                  const unsigned long long* flag_from_lo, const unsigned long long* flag_from_hi, int flags,
-                  int* __restrict__ status) {
+__device__ __forceinline__ void
+slab_fold_face(const typename LabelOf<Bytes>::type* __restrict__ labels, float* __restrict__ f, int64_t plane,
+               int64_t q, int nz, int halo, float w2, int high_face, const unsigned char* __restrict__ nb,
+               SlabStageLayout L, int flags, int* __restrict__ status) {
   using LT = typename LabelOf<Bytes>::type;
-  const int high_face = blockIdx.y;
-  if (high_face == 0 ? !has_lo : !has_hi) return;
-  // launched with programmatic stream serialization right behind the Z pass: the CTAs become
-  // resident during its last wave, wait for the neighbour's flag, and only then for the Z pass
-  __shared__ int ready;
-  if (threadIdx.x == 0) {
-    const unsigned long long* flag = high_face ? flag_from_hi : flag_from_lo;
-    int ok = 0;
-    for (long long spin = 0; spin < (1ll << 25); ++spin) {        // a few seconds, then give up
-      if (ld_acquire_sys_u64(flag) >= step) { ok = 1; break; }
-      __nanosleep(64);
-    }
-    ready = ok;
-  }
-  __syncthreads();
-  pdl_wait_for_previous_grid();            // f holds the Z pass's results from here on
-  if (!ready) {
-    if (threadIdx.x == 0) atomicOr(status, 2);
-    return;
-  }
-  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= plane) return;
   // the neighbour's set: for my low face its HIGH-face data, for my high face its LOW-face data
-  const unsigned char* nb = high_face ? set_hi_peer : set_lo_peer;
   const LT* nb_label = reinterpret_cast<const LT*>(nb + (high_face ? L.lab_lo : L.lab_hi));
   const unsigned char* nb_m = nb + (high_face ? L.m_lo : L.m_hi);
   const float* nb_f = reinterpret_cast<const float*>(nb + (high_face ? L.f_lo : L.f_hi));
@@ -164,32 +136,76 @@ slab_fixup_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, floa
   {
     const float cur0 = fabsf(f[row0 * plane + q]);
     const float reach0 = (flags & kSqrt) ? cur0 * cur0 * 1.000001f : cur0;
-    while (held < min(m, kSiteCap) && parabola_at(w2, 1 + held, 0.0f) < reach0) {
+    while (held < min(m, kSiteCap) && parabola_at(w2, 1 + held, 0.0f, 0) <= reach0) {
       sites[held] = nb_f[(high_face ? (int64_t)held : (int64_t)(H - 1 - held)) * plane + q];
       ++held;
     }
   }
+  // candidates, stop rule and stores as in face_fixup_kernel (edt_kernels.cuh)
   for (int j = 0; j < nz; ++j) {
     const int64_t at = (row0 + dir * j) * plane + q;
     if (j > 0 && labels[at] != lab0) break;                   // end of the run inside this slab
     const float cur = fabsf(f[at]);
-    // a site at distance d costs at least w2 * d^2: beyond the current value's reach nothing helps
+    // a site at distance d costs at least w2 * d^2: strictly beyond the current value's reach it
+    // is strictly above the row's exact value, and stays so on every later row
     const float reach = (flags & kSqrt) ? cur * cur * 1.000001f : cur;
-    float best = unseen ? CUDART_INF_F : parabola_at(w2, j + 1 + m, 0.0f);
+    float best = unseen ? CUDART_INF_F : parabola_at(w2, j + 1 + m, 0.0f, 0);
     for (int r = 0; r < m; ++r) {
-      if (parabola_at(w2, j + 1 + r, 0.0f) >= reach) break;
+      if (parabola_at(w2, j + 1 + r, 0.0f, 0) > reach) break;
       const float height = r < held ? sites[r] : nb_f[(high_face ? (int64_t)r : (int64_t)(H - 1 - r)) * plane + q];
-      best = fminf(best, parabola_at(w2, j + 1 + r, height));
+      best = fminf(best, parabola_at(w2, j + 1 + r, height, 0));
     }
     if (flags & kSqrt) best = __fsqrt_rn(best);
     if (unseen) {
-      float bound = parabola_at(w2, j + H, 0.0f);
+      float bound = parabola_at(w2, j + H, 0.0f, 0);
       if (flags & kSqrt) bound = __fsqrt_rn(bound);
       if (!(fminf(best, cur) <= bound)) atomicOr(status, 1);
     }
-    if (!(best < cur)) break;                                 // no outside site helps from here on
-    f[at] = negative ? -best : best;
+    if (best > cur) break;                                    // no outside site helps from here on
+    if (best < cur) f[at] = negative ? -best : best;
   }
+}
+
+// Both faces in one launch; waits for the neighbours' staging sets of `step` and then folds them
+// in.  One thread per (x,y) line folds the low face and THEN the high face: a run that spans the
+// slab is walked from both ends over the same rows, and the second walk must see the first one's
+// stores (the NCCL path's two launches give the same order).
+// *status: bit 0 = halo too shallow for this volume (see face_fixup_kernel), bit 1 = a
+// neighbour never published the step (time-out).
+template <int Bytes>
+__global__ void __launch_bounds__(256)
+slab_fixup_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, float* __restrict__ f, int64_t plane,
+                  int nz, int halo, float w2, int has_lo, int has_hi, const unsigned char* __restrict__ set_lo_peer,
+                  const unsigned char* __restrict__ set_hi_peer, SlabStageLayout L, unsigned long long step,
+                  const unsigned long long* flag_from_lo, const unsigned long long* flag_from_hi, int flags,
+                  int* __restrict__ status) {
+  if (!has_lo && !has_hi) return;
+  // launched with programmatic stream serialization right behind the Z pass: the CTAs become
+  // resident during its last wave, wait for the neighbours' flags, and only then for the Z pass
+  __shared__ int ready;
+  if (threadIdx.x == 0) {
+    int ok = 1;
+    for (int face = 0; face < 2 && ok; ++face) {
+      if (face == 0 ? !has_lo : !has_hi) continue;
+      const unsigned long long* flag = face ? flag_from_hi : flag_from_lo;
+      ok = 0;
+      for (long long spin = 0; spin < (1ll << 25); ++spin) {      // a few seconds, then give up
+        if (ld_acquire_sys_u64(flag) >= step) { ok = 1; break; }
+        __nanosleep(64);
+      }
+    }
+    ready = ok;
+  }
+  __syncthreads();
+  pdl_wait_for_previous_grid();            // f holds the Z pass's results from here on
+  if (!ready) {
+    if (threadIdx.x == 0) atomicOr(status, 2);
+    return;
+  }
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= plane) return;
+  if (has_lo) slab_fold_face<Bytes>(labels, f, plane, q, nz, halo, w2, 0, set_lo_peer, L, flags, status);
+  if (has_hi) slab_fold_face<Bytes>(labels, f, plane, q, nz, halo, w2, 1, set_hi_peer, L, flags, status);
 }
 
 // ---- Z slabs <-> Y slabs (the transposition fallback of the slab split) ----

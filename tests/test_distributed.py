@@ -17,6 +17,8 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import slab_cases  # noqa: E402
 
 
 class OraclePasses:
@@ -73,57 +75,15 @@ class OraclePasses:
 
   # numpy restatement of the two slab-face kernels (edt_kernels.cuh: face_runs_kernel, face_fixup_kernel)
   def face_runs(self, labels, high_face, halo, signed, overflow, out=None):
-    lab = labels.numpy()
-    nz = lab.shape[0]
-    rows = range(nz - 1, -1, -1) if high_face else range(nz)
-    face = lab[nz - 1 if high_face else 0]
-    m = np.zeros(face.shape, dtype=np.int64)
-    alive = np.ones(face.shape, dtype=bool)
-    for k, r in enumerate(rows):
-      if k > halo:
-        break
-      alive &= lab[r] == face
-      m += alive
-    too_long = (m > halo) | (m >= nz)
-    m[too_long] = halo + 1
-    if np.any(too_long & ((face != 0) | bool(signed))):
+    m, too_long = slab_cases.face_runs(labels.numpy(), high_face, halo, signed)
+    if too_long:
       overflow[0] = 1
-    return torch.from_numpy(m.astype(np.uint8))
+    return torch.from_numpy(m)
 
   def face_fixup(self, labels, f, high_face, halo, wz, sqrt, signed, nb_label, nb_m, nb_f, inexact):
-    lab, arr = labels.numpy(), f.numpy()
-    nbl, nbm, nbf = nb_label.numpy(), nb_m.numpy(), nb_f.numpy()
-    nz, sy, sx = lab.shape
-    w2 = np.float32(np.float32(wz) * np.float32(wz))
-    for y in range(sy):
-      for x in range(sx):
-        row0, step = (nz - 1, -1) if high_face else (0, 1)
-        lab0 = lab[row0, y, x]
-        if lab0 == 0 and not signed:
-          continue
-        m_raw = int(nbm[y, x]) if nbl[y, x] == lab0 else 0
-        unseen = m_raw > halo           # the neighbour's part of the run goes on behind the halo
-        m = min(m_raw, halo)
-        for j in range(nz):
-          r = row0 + step * j
-          if j > 0 and lab[r, y, x] != lab0:
-            break
-          best = np.float32(np.inf) if unseen else np.float32(np.float64(w2) * (j + 1 + m) ** 2)
-          for k in range(m):
-            src = k if high_face else halo - 1 - k
-            best = min(best, np.float32(np.float64(w2) * (j + 1 + k) ** 2 + np.float64(nbf[src, y, x])))
-          if sqrt:
-            best = np.sqrt(np.float32(best))
-          cur = abs(arr[r, y, x])
-          if unseen:
-            bound = np.float32(np.float64(w2) * (j + halo) ** 2)
-            if sqrt:
-              bound = np.sqrt(bound)
-            if not (min(best, cur) <= bound):
-              inexact[0] = 1
-          if not (best < cur):
-            break
-          arr[r, y, x] = -best if (signed and lab0 == 0) else best
+    if slab_cases.face_fixup(labels.numpy(), f.numpy(), high_face, halo, wz, sqrt, signed, nb_label.numpy(),
+                             nb_m.numpy(), nb_f.numpy()):
+      inexact[0] = 1
 
 
 def _free_port():
@@ -142,6 +102,12 @@ def _volume(case):
     vol[tuple(s // 2 for s in shape)] = 0
   elif kind == "solid":
     vol = np.full(shape, 7, dtype=np.int64)
+  elif kind == "tie":
+    vol = slab_cases.tie_volume(case[6])[0]
+  elif kind == "trap":
+    vol = slab_cases.stop_trap(case[6])[0]
+  elif kind == "span":
+    vol = slab_cases.span_volume(shape)
   elif kind == "stripes":       # z-runs of length 2 starting at odd z (slab faces cut them), some background
     z, y, x = np.meshgrid(*[np.arange(s) for s in shape], indexing="ij")
     vol = 1 + ((z + 1) // 2 + x + 2 * y) % 3
@@ -210,10 +176,22 @@ CASES = [
   ((16, 5, 7), "solid", (1.0, 1.0, 1.0), True, False, False, None),
   # ... unless the slabs are deep enough for the next halo depth (2 -> 8 rows: world 2 has 10-row slabs)
   ((20, 5, 7), "solid", (1.0, 1.0, 1.0), True, False, False, None),
+  # the fix-up's traps (tests/slab_cases.py): a double-rounding tie three rows behind a face ...
+  ((9, 1, 2), "tie", slab_cases.TIE_W, False, False, False, (3, 6)),
+  ((12, 1, 2), "tie", slab_cases.TIE_W, False, False, False, (3, 6, 3)),
+  # ... a rounded tie more than 4096 rows behind a face with a strictly lower row after it ...
+  ((12000, 1, 2), "trap", slab_cases.TRAP_W, False, False, False, (6000, 6000)),
+  ((12100, 1, 2), "trap", slab_cases.TRAP_W, False, False, False, (100, 6000, 6000)),
+  # ... and a run spanning the middle slab of three, walked from both faces
+  ((14, 3, 4), "span", (1.0, 1.0, 1.0), False, False, False, None),
+  ((14, 3, 4), "span", (2.0, 1.0, 1.0), False, True, True, None),
 ]
 # method taken when starting with halo=2, per world size
 EXPECT_HALO2 = {10: {2: "halo", 3: "halo"}, 11: {2: "halo", 3: "halo"}, 12: {2: "transpose", 3: "transpose"},
-                13: {2: "halo", 3: "transpose"}}
+                13: {2: "halo", 3: "transpose"}, 14: {2: "halo"}, 15: {3: "halo"}, 16: {2: "halo"}, 17: {3: "halo"},
+                18: {2: "transpose", 3: "halo"}, 19: {2: "transpose", 3: "halo"}}
+# with halo=64 only slabs deeper than 64 rows can take the halo method
+EXPECT_HALO64 = {16: {2: "halo"}, 17: {3: "halo"}}
 
 
 @pytest.mark.parametrize("world", [2, 3])
@@ -252,7 +230,7 @@ def test_slab_split_matches_single_volume(world):
           methods.add(method)
       assert len(methods) == 1, (world, idx, halo, methods)       # every rank took the same path
       if halo == 64:
-        assert methods == {"transpose"}
+        assert methods == {EXPECT_HALO64.get(idx, {}).get(world, "transpose")}, (world, idx, methods)
       elif idx in EXPECT_HALO2:
         assert methods == {EXPECT_HALO2[idx][world]}, (world, idx, methods)
       used.add((idx, methods.pop()))

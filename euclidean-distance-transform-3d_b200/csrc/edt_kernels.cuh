@@ -1429,115 +1429,4 @@ later_axis_long_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
   }
 }
 
-
-// ---------------------------------------------------------------------------------------
-// Z-slab decomposition across GPUs (see distributed.py): the third-axis pass of a slab is run
-// with its interior faces OPEN (no border term), and the voxels of the neighbouring slab are
-// folded in afterwards as extra candidates for the runs that touch the face:
-//   * neighbour label differs: the face is a run border -> one zero-height site at distance 1;
-//   * neighbour label equal  : the neighbour's part of the run (m <= H rows, it must end inside
-//     the neighbour's slab) contributes its rows as sites, plus the zero-height site behind it.
-// Every such site lies outside the slab, so against the slab-local envelope its parabola only
-// gets worse (by at least 2*w2 per row) as rows move away from the face.  Every candidate is the
-// double sum w2 * d^2 + f rounded once to float32, the reference's evaluation.  The walk along a
-// column stops at the first row where the best outside candidate is STRICTLY above the row's
-// value: rounding is monotone, so that row's exact outside minimum is above its exact inside one,
-// and the gap only widens further on.  A rounded tie proves nothing (the exact difference may
-// still be negative and round lower a row later), so the walk goes on over ties; it stores only
-// values strictly below the current one.
-// Values are compared after the pass's epilogue: sqrt is monotone and the sign of a run is
-// fixed, so min() commutes with both.
-// ---------------------------------------------------------------------------------------
-
-// m[q] = length of the run of equal labels that touches the face (capped at H + 1 = "too long"),
-// for every line q of the sx*sy plane; *overflow is raised if any foreground run is too long.
-template <int Bytes>
-__global__ void __launch_bounds__(256)
-face_runs_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, int64_t plane, int nz, int high_face,
-                 int H, int zero_is_label, uint8_t* __restrict__ m_out, int* __restrict__ overflow) {
-  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= plane) return;
-  const int64_t row0 = high_face ? (int64_t)(nz - 1) : 0;
-  const int64_t step = high_face ? -1 : 1;
-  const auto lab0 = labels[row0 * plane + q];
-  int m = 1;
-  const int limit = min(nz, H + 1);
-  while (m < limit && labels[(row0 + step * m) * plane + q] == lab0) ++m;
-  if (m > H || m >= nz) {                 // runs that are too long, or that span the whole slab
-    m = H + 1;
-    if (lab0 != 0 || zero_is_label) *overflow = 1;
-  }
-  m_out[q] = (uint8_t)m;
-}
-
-// Fold the neighbour's sites into the rows of this slab that belong to face-touching runs.
-//   nb_label : the neighbour's face plane of labels        nb_m : its face_runs_kernel output
-//   nb_f     : H planes of the neighbour's distances AFTER its second-axis pass, in the
-//              neighbour's own z order (for the low face these are its LAST H planes)
-// When the neighbour's part of the run is longer than the halo (nb_m = H + 1) its first H rows
-// are still folded in, and the sites behind them -- unseen, at distance >= j + 1 + H from row j,
-// so never cheaper than w2 * (j + 1 + H)^2 -- are ruled out by VALUE: if the combined result of a
-// row does not exceed that bound nothing unseen can beat it.  sqrt of the result is 1-Lipschitz
-// along the run (in units of w), so the bound holding at the face row implies it for every deeper
-// row; it is tested (with one row of slack against rounding) on every row the walk visits, and
-// *inexact is raised when it fails -- the caller then needs a deeper halo or the exact fallback.
-template <int Bytes>
-__global__ void __launch_bounds__(256)
-face_fixup_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, float* __restrict__ f,
-                  int64_t plane, int nz, int high_face, int H, float w2,
-                  const typename LabelOf<Bytes>::type* __restrict__ nb_label,
-                  const uint8_t* __restrict__ nb_m, const float* __restrict__ nb_f, int flags,
-                  int* __restrict__ inexact) {
-  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (q >= plane) return;
-  const int64_t row0 = high_face ? (int64_t)(nz - 1) : 0;
-  const int64_t step = high_face ? -1 : 1;
-  const auto lab0 = labels[row0 * plane + q];
-  const bool background = lab0 == 0;
-  if (background && !(flags & kZeroLabel)) return;            // plain EDT: background stays 0
-  const bool same = nb_label[q] == lab0;
-  const int m_raw = same ? (int)nb_m[q] : 0;
-  const bool unseen = m_raw > H;                              // the run goes on behind the halo
-  const int m = min(m_raw, H);                                // neighbour rows of this run that we hold
-  const bool negative = (flags & kNegate) && background;
-  // the neighbour's rows of this run, read ONCE (they may live in a peer GPU's memory): every row
-  // of the walk below needs them again.  Only those within reach of the face row's value are
-  // fetched: deeper rows of this slab reach no further into the neighbour (Lipschitz again).
-  constexpr int kSiteCap = 128;
-  float sites[kSiteCap];
-  int held = 0;
-  {
-    const float cur0 = fabsf(f[row0 * plane + q]);
-    const float reach0 = (flags & kSqrt) ? cur0 * cur0 * 1.000001f : cur0;
-    while (held < min(m, kSiteCap) && parabola_at(w2, 1 + held, 0.0f, 0) <= reach0) {
-      sites[held] = nb_f[(high_face ? (int64_t)held : (int64_t)(H - 1 - held)) * plane + q];
-      ++held;
-    }
-  }
-  for (int j = 0; j < nz; ++j) {
-    const int64_t at = (row0 + step * j) * plane + q;
-    if (j > 0 && labels[at] != lab0) break;                   // end of the run inside this slab
-    const float cur = fabsf(f[at]);
-    // a site at distance d costs at least w2 * d^2: strictly beyond the current value's reach it
-    // is strictly above the row's exact value, and stays so on every later row
-    const float reach = (flags & kSqrt) ? cur * cur * 1.000001f : cur;
-    // best outside site for row j: neighbour rows r = 0..m-1 at distance j + 1 + r, then (if the
-    // run ends there) the zero-height site behind them at distance j + 1 + m
-    float best = unseen ? CUDART_INF_F : parabola_at(w2, j + 1 + m, 0.0f, 0);
-    for (int r = 0; r < m; ++r) {
-      if (parabola_at(w2, j + 1 + r, 0.0f, 0) > reach) break;
-      const float height = r < held ? sites[r] : nb_f[(high_face ? (int64_t)r : (int64_t)(H - 1 - r)) * plane + q];
-      best = fminf(best, parabola_at(w2, j + 1 + r, height, 0));
-    }
-    if (flags & kSqrt) best = __fsqrt_rn(best);
-    if (unseen) {
-      float bound = parabola_at(w2, j + H, 0.0f, 0);
-      if (flags & kSqrt) bound = __fsqrt_rn(bound);
-      if (!(fminf(best, cur) <= bound) && inexact) *inexact = 1;
-    }
-    if (best > cur) break;                                    // no outside site helps from here on
-    if (best < cur) f[at] = negative ? -best : best;
-  }
-}
-
 }  // namespace edtb200

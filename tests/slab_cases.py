@@ -3,8 +3,7 @@ gloo test in tests/test_distributed.py).
 
 The Z-slab split runs the third-axis pass of every slab with its inner faces open and then folds
 the neighbour's rows of every run that crosses a face into the slab (face_runs_kernel and
-face_fixup_kernel in csrc/edt_kernels.cuh, slab_stage_kernel and slab_fixup_kernel in
-csrc/edt_slab.cuh).  This module restates those two steps in numpy on C-ordered (z, y, x) arrays,
+face_fixup_kernel, slab_stage_kernel and slab_fixup_kernel, all in csrc/edt_slab.cuh).  This module restates those two steps in numpy on C-ordered (z, y, x) arrays,
 restates the byte layout of the fused step's staging buffer, and builds seeded volumes, among them
 three that are traps for a fix-up that is subtly wrong:
 

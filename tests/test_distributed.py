@@ -73,7 +73,7 @@ class OraclePasses:
       else:
         block.copy_(src[:, s:s + c, :])
 
-  # numpy restatement of the two slab-face kernels (edt_kernels.cuh: face_runs_kernel, face_fixup_kernel)
+  # numpy restatement of the two slab-face kernels (edt_slab.cuh: face_runs_kernel, face_fixup_kernel)
   def face_runs(self, labels, high_face, halo, signed, overflow, out=None):
     m, too_long = slab_cases.face_runs(labels.numpy(), high_face, halo, signed)
     if too_long:

@@ -1,5 +1,6 @@
 """Inputs and plain restatements for the tests of the Z-slab split (tests/test_slab_*.py and the
-gloo test in tests/test_distributed.py).
+gloo tests in tests/test_distributed.py), and `OraclePasses`, the stand-in for
+distributed.CudaPasses that those gloo tests hand to slab_transform.
 
 The Z-slab split runs the third-axis pass of every slab with its inner faces open and then folds
 the neighbour's rows of every run that crosses a face into the slab (face_runs_kernel and
@@ -19,6 +20,7 @@ three that are traps for a fix-up that is subtly wrong:
 from fractions import Fraction
 
 import numpy as np
+import torch
 
 TIE_W = (float(np.float32(1.333549976348877)), 1.0, 2.0 ** -26)        # (w_z, w_y, w_x)
 # stop_trap: with w_z^2 = 1.5390757 and an in-plane height of w_x^2 = 16064.0 at the face row, the
@@ -184,6 +186,71 @@ def split_restated(oracle, vol, depths, w, black_border, sqrt, signed, halo, ari
       inexact |= face_fixup(lab, z, high_face, halo, w[0], sqrt, signed, nb_label, nb_m, nb_f, arith, stop)
     out.append(z)
   return np.concatenate(out, axis=0), inexact
+
+
+class OraclePasses:
+  """Stand-in for CudaPasses: same interface, numpy arithmetic from oracle/ (tests only)."""
+
+  def __init__(self, packed=True):
+    from oracle import oracle
+    self.oracle = oracle
+    self.signed = False
+    if not packed:                  # hide `repartition`: the transposition then slices and concatenates
+      self.repartition = None
+
+  def __getattribute__(self, name):
+    value = object.__getattribute__(self, name)
+    if name == "repartition" and value is None:
+      raise AttributeError(name)
+    return value
+
+  def empty_f32(self, shape):
+    return torch.zeros(shape, dtype=torch.float32)
+
+  def pass_first(self, labels, f, wx, black_border, signed):
+    lab = labels.numpy()
+    self.signed = bool(signed)
+    if signed:                      # background as an ordinary label == shift every label by one
+      lab = lab.astype(np.int64) + 1
+    f.copy_(torch.from_numpy(self.oracle.pass_first(lab, wx, black_border)))
+
+  def pass_later(self, labels, f, axis, w, border_lo, border_hi, sqrt=False, negate=False):
+    lab = labels.numpy().astype(np.int64)
+    zero = lab == 0
+    arr = f.numpy()
+    self.oracle.pass_later(lab + 1, arr, axis, w, border_lo, border_hi)   # +1: every run is foreground...
+    if not self.signed:
+      # ...except that plain EDT keeps background at 0 (its rows hold 0 already and stay 0)
+      arr[zero] = 0.0
+    if sqrt:
+      np.sqrt(arr, out=arr)
+    if negate:
+      arr[zero] *= -1.0
+
+
+  # torch restatement of slab_pack_kernel (edt_slab.cuh): slab (zc, sy, row) <-> per-rank blocks
+  def repartition(self, src, dst, ysplit, unpack=False):
+    slab = dst if unpack else src
+    zc, sy, row = slab.shape
+    flat = (src if unpack else dst).reshape(-1)
+    for s, c in ysplit:
+      block = flat[zc * s * row:zc * (s + c) * row].view(zc, c, row)
+      if unpack:
+        dst[:, s:s + c, :] = block
+      else:
+        block.copy_(src[:, s:s + c, :])
+
+  # the two slab-face kernels (edt_slab.cuh: face_runs_kernel, face_fixup_kernel), restated above
+  def face_runs(self, labels, high_face, halo, signed, overflow, out=None):
+    m, too_long = face_runs(labels.numpy(), high_face, halo, signed)
+    if too_long:
+      overflow[0] = 1
+    return torch.from_numpy(m)
+
+  def face_fixup(self, labels, f, high_face, halo, wz, sqrt, signed, nb_label, nb_m, nb_f, inexact):
+    if face_fixup(labels.numpy(), f.numpy(), high_face, halo, wz, sqrt, signed, nb_label.numpy(),
+                  nb_m.numpy(), nb_f.numpy()):
+      inexact[0] = 1
 
 
 # ---------------------------------------------------------------------------------------------

@@ -19,71 +19,7 @@ import torch.multiprocessing as mp
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import slab_cases  # noqa: E402
-
-
-class OraclePasses:
-  """Stand-in for CudaPasses: same interface, numpy arithmetic from oracle/ (tests only)."""
-
-  def __init__(self, packed=True):
-    from oracle import oracle
-    self.oracle = oracle
-    self.signed = False
-    if not packed:                  # hide `repartition`: the transposition then slices and concatenates
-      self.repartition = None
-
-  def __getattribute__(self, name):
-    value = object.__getattribute__(self, name)
-    if name == "repartition" and value is None:
-      raise AttributeError(name)
-    return value
-
-  def empty_f32(self, shape):
-    return torch.zeros(shape, dtype=torch.float32)
-
-  def pass_first(self, labels, f, wx, black_border, signed):
-    lab = labels.numpy()
-    self.signed = bool(signed)
-    if signed:                      # background as an ordinary label == shift every label by one
-      lab = lab.astype(np.int64) + 1
-    f.copy_(torch.from_numpy(self.oracle.pass_first(lab, wx, black_border)))
-
-  def pass_later(self, labels, f, axis, w, border_lo, border_hi, sqrt=False, negate=False):
-    lab = labels.numpy().astype(np.int64)
-    zero = lab == 0
-    arr = f.numpy()
-    self.oracle.pass_later(lab + 1, arr, axis, w, border_lo, border_hi)   # +1: every run is foreground...
-    if not self.signed:
-      # ...except that plain EDT keeps background at 0 (its rows hold 0 already and stay 0)
-      arr[zero] = 0.0
-    if sqrt:
-      np.sqrt(arr, out=arr)
-    if negate:
-      arr[zero] *= -1.0
-
-
-  # torch restatement of slab_pack_kernel (edt_slab.cuh): slab (zc, sy, row) <-> per-rank blocks
-  def repartition(self, src, dst, ysplit, unpack=False):
-    slab = dst if unpack else src
-    zc, sy, row = slab.shape
-    flat = (src if unpack else dst).reshape(-1)
-    for s, c in ysplit:
-      block = flat[zc * s * row:zc * (s + c) * row].view(zc, c, row)
-      if unpack:
-        dst[:, s:s + c, :] = block
-      else:
-        block.copy_(src[:, s:s + c, :])
-
-  # numpy restatement of the two slab-face kernels (edt_slab.cuh: face_runs_kernel, face_fixup_kernel)
-  def face_runs(self, labels, high_face, halo, signed, overflow, out=None):
-    m, too_long = slab_cases.face_runs(labels.numpy(), high_face, halo, signed)
-    if too_long:
-      overflow[0] = 1
-    return torch.from_numpy(m)
-
-  def face_fixup(self, labels, f, high_face, halo, wz, sqrt, signed, nb_label, nb_m, nb_f, inexact):
-    if slab_cases.face_fixup(labels.numpy(), f.numpy(), high_face, halo, wz, sqrt, signed, nb_label.numpy(),
-                             nb_m.numpy(), nb_f.numpy()):
-      inexact[0] = 1
+from slab_cases import OraclePasses  # noqa: E402
 
 
 def _free_port():
@@ -340,6 +276,25 @@ def test_split_extent():
   assert sum(c for _, c in ed.split_extent(4096, 8)) == 4096
 
 
+def test_halo_ladder():
+  """The halos a slab_transform call tries before the transposition (tests/test_slab_ladder.py runs them)."""
+  sys.path.insert(0, ROOT)
+  import edt_b200.distributed as ed
+  ladder = ed._halo_ladder
+  assert ladder("auto", 2, 10, 2) == [2, 8]                   # 32 does not fit into 10-row slabs
+  assert ladder("auto", 2, 5, 3) == [2]
+  assert ladder("auto", 8, 1000, 2) == [8, 32, 128]
+  assert ladder("auto", 8, 40, 2) == [8, 32]
+  assert ladder("auto", 100, 1000, 2) == [100, 128]
+  assert ladder("auto", 128, 1000, 2) == [128]
+  assert ladder("auto", 254, 255, 2) == [254]                 # 128 is not deeper than 254
+  assert ladder("auto", 64, 64, 2) == []                      # slabs must be deeper than the halo
+  assert ladder("halo", 8, 1000, 2) == [8]                    # one attempt, no retry
+  assert ladder("halo", 8, 8, 2) == []
+  assert ladder("transpose", 8, 1000, 2) == []
+  assert ladder("auto", 8, 1000, 1) == ladder("halo", 8, 1000, 1) == []
+
+
 # ---------------------------------------------------------------------------------------
 # the real thing: NCCL over 2 GPUs (skipped unless the box has at least two)
 # ---------------------------------------------------------------------------------------
@@ -376,8 +331,6 @@ def _nccl_worker(rank, world, port, queue):
         local = torch.from_numpy(vol[z0:z0 + zc].copy()).cuda()
         whole = edt_b200.edt_cuda(torch.from_numpy(vol).cuda(), an, bb, sqrt=sqrt, signed=signed)
         for method, peer in (("auto", None), ("transpose", None), ("auto", peer_halo), ("auto", "auto")):
-          if method == "auto" and peer is None and peer_halo is not None and False:
-            continue
           info = {}
           out = ed.slab_transform(local, an, bb, sqrt=sqrt, signed=signed, method=method, info=info,
                                   peer_halo=peer)

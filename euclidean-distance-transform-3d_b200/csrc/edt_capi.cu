@@ -431,22 +431,27 @@ int check_dims(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz)
 
 int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines, int64_t sx, float w,
                    int border, int flags, DeviceCache& dc, cudaStream_t s) {
-  switch (label_bytes) {
-    case 1: return launch_first<1>(labels, f, nlines, sx, w, border, flags, dc, s);
-    case 2: return launch_first<2>(labels, f, nlines, sx, w, border, flags, dc, s);
-    case 4: return launch_first<4>(labels, f, nlines, sx, w, border, flags, dc, s);
-    default: return launch_first<8>(labels, f, nlines, sx, w, border, flags, dc, s);
-  }
+  return with_label_width(label_bytes, [&](auto b) {
+    return launch_first<b>(labels, f, nlines, sx, w, border, flags, dc, s);
+  });
 }
 
 int dispatch_later(int label_bytes, const void* labels, float* f, const edtb200::LineGeom& g, float w,
                    int lo, int hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t s, bool pdl) {
-  switch (label_bytes) {
-    case 1: return launch_later<1>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
-    case 2: return launch_later<2>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
-    case 4: return launch_later<4>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
-    default: return launch_later<8>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
-  }
+  return with_label_width(label_bytes, [&](auto b) {
+    return launch_later<b>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
+  });
+}
+
+// Grows a cached device buffer to at least `need` bytes; what it held is not kept.
+template <class T>
+cudaError_t grow(T*& p, size_t& have, size_t need) {
+  if (have >= need) return cudaSuccess;
+  if (p) cudaFree(p);
+  p = nullptr; have = 0;
+  const cudaError_t e = cudaMalloc(&p, need);
+  if (e == cudaSuccess) have = need;
+  return e;
 }
 
 // Kernel flags of a pass from the ABI flags: sqrt and sign act in the store of the last pass;
@@ -667,23 +672,13 @@ int edtb200_transform(const void* labels, int label_bytes, int ndim, int64_t sx,
   const void* d_labels = labels;
   float* d_out = out;
   if (!lab_dev) {
-    if (dc->labels_bytes < lab_bytes) {
-      if (dc->labels) cudaFree(dc->labels);
-      dc->labels = nullptr; dc->labels_bytes = 0;
-      CUDA_TRY(cudaMalloc(&dc->labels, lab_bytes));
-      dc->labels_bytes = lab_bytes;
-    }
+    CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
     rc = upload(dc->labels, labels, lab_bytes, device, stream);
     if (rc) return rc;
     d_labels = dc->labels;
   }
   if (!out_dev) {
-    if (dc->dist_bytes < out_bytes) {
-      if (dc->dist) cudaFree(dc->dist);
-      dc->dist = nullptr; dc->dist_bytes = 0;
-      CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&dc->dist), out_bytes));
-      dc->dist_bytes = out_bytes;
-    }
+    CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
     d_out = dc->dist;
   }
   rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, d_out, *dc, stream);
@@ -718,19 +713,11 @@ int edtb200_transform_batch(const void* const* labels, float* const* outs, int c
   DeviceCache& dc = *dcp;
   std::lock_guard<std::mutex> host_call(dc.host_call);
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
-  auto grow = [](void** p, size_t* have, size_t need) -> cudaError_t {
-    if (*have >= need) return cudaSuccess;
-    if (*p) cudaFree(*p);
-    *p = nullptr; *have = 0;
-    cudaError_t e = cudaMalloc(p, need);
-    if (e == cudaSuccess) *have = need;
-    return e;
-  };
-  CUDA_TRY(grow(&dc.labels, &dc.labels_bytes, lab_bytes));
-  CUDA_TRY(grow(reinterpret_cast<void**>(&dc.dist), &dc.dist_bytes, out_bytes));
+  CUDA_TRY(grow(dc.labels, dc.labels_bytes, lab_bytes));
+  CUDA_TRY(grow(dc.dist, dc.dist_bytes, out_bytes));
   if (count > 1) {
-    CUDA_TRY(grow(&dc.labels2, &dc.labels2_bytes, lab_bytes));
-    CUDA_TRY(grow(reinterpret_cast<void**>(&dc.dist2), &dc.dist2_bytes, out_bytes));
+    CUDA_TRY(grow(dc.labels2, dc.labels2_bytes, lab_bytes));
+    CUDA_TRY(grow(dc.dist2, dc.dist2_bytes, out_bytes));
   }
   if (!dc.stream) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream, cudaStreamNonBlocking));
   if (!dc.stream_up) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_up, cudaStreamNonBlocking));
@@ -848,60 +835,52 @@ int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const uns
     stream = dc->stream;
   }
 
-  // stream-ordered scratch: the inputs when they come from the host, the doubled byte mask, the
-  // doubled distance volume, and the result when it goes back to the host
-  void *d_labels = nullptr, *d_graph = nullptr, *d_cells = nullptr, *d_doubled = nullptr, *d_result = nullptr;
-  auto release = [&]() {
-    void* all[] = {d_labels, d_graph, d_cells, d_doubled, d_result};
-    for (void* p : all) if (p) cudaFreeAsync(p, stream);
-  };
-  #define VG_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { release(); \
-      return fail(e_ == cudaErrorMemoryAllocation ? EDTB200_ENOMEM : EDTB200_ECUDA, "%s: %s", #expr, \
-                  cudaGetErrorString(e_)); } } while (0)
-  const void* lab = labels;
-  const uint8_t* gr = graph;
-  if (!in_dev) {
-    VG_TRY(scratch_alloc(*dc, &d_labels, (size_t)total * label_bytes, stream));
-    VG_TRY(scratch_alloc(*dc, &d_graph, (size_t)total, stream));
-    rc = upload(d_labels, labels, (size_t)total * label_bytes, device, stream);
-    if (!rc) rc = upload(d_graph, graph, (size_t)total, device, stream);
-    if (rc) { release(); return rc; }
-    lab = d_labels;
-    gr = static_cast<const uint8_t*>(d_graph);
-  }
-  VG_TRY(scratch_alloc(*dc, &d_cells, (size_t)total2, stream));
-  VG_TRY(scratch_alloc(*dc, &d_doubled, (size_t)total2 * sizeof(float), stream));
-  float* result = out;
-  if (!out_dev) {
-    VG_TRY(scratch_alloc(*dc, &d_result, (size_t)total * sizeof(float), stream));
-    result = static_cast<float*>(d_result);
-  }
+  {
+    // stream-ordered scratch: the inputs when they come from the host, the doubled byte mask, the
+    // doubled distance volume, and the result when it goes back to the host
+    Scratch d_labels, d_graph, d_cells, d_doubled, d_result;
+    const void* lab = labels;
+    const uint8_t* gr = graph;
+    if (!in_dev) {
+      CUDA_TRY(d_labels.alloc(*dc, (size_t)total * label_bytes, stream));
+      CUDA_TRY(d_graph.alloc(*dc, (size_t)total, stream));
+      rc = upload(d_labels.get(), labels, (size_t)total * label_bytes, device, stream);
+      if (!rc) rc = upload(d_graph.get(), graph, (size_t)total, device, stream);
+      if (rc) return rc;
+      lab = d_labels.get();
+      gr = d_graph.get<const uint8_t>();
+    }
+    CUDA_TRY(d_cells.alloc(*dc, (size_t)total2, stream));
+    CUDA_TRY(d_doubled.alloc(*dc, (size_t)total2 * sizeof(float), stream));
+    float* result = out;
+    if (!out_dev) {
+      CUDA_TRY(d_result.alloc(*dc, (size_t)total * sizeof(float), stream));
+      result = d_result.get<float>();
+    }
 
-  const int threads = 256;
-  const int blocks = (int)std::min<int64_t>((total + threads - 1) / threads, (int64_t)dc->sm_count * 32);
-  const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
-  uint8_t* cells = static_cast<uint8_t*>(d_cells);
-  switch (label_bytes) {
-    case 1: voxel_graph_expand_kernel<1><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float); break;
-    case 2: voxel_graph_expand_kernel<2><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float); break;
-    case 4: voxel_graph_expand_kernel<4><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float); break;
-    default: voxel_graph_expand_kernel<8><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float); break;
-  }
-  VG_TRY(cudaGetLastError());
-  // half the anisotropy (vg:102-107, 199-204); the sqrt is taken by the gather instead
-  rc = run_passes(cells, 1, ndim, sx2, sy2, sz2, wx / 2, wy / 2, wz / 2, border, 0,
-                  static_cast<float*>(d_doubled), *dc, stream);
-  if (rc) { release(); return rc; }
-  voxel_graph_gather_kernel<<<blocks, threads, 0, stream>>>(static_cast<const float*>(d_doubled), result, sx, sy, sz,
-                                                            (flags & EDTB200_SQRT) ? 1 : 0);
-  VG_TRY(cudaGetLastError());
-  if (!out_dev) {
-    rc = download(out, result, (size_t)total * sizeof(float), device, stream);
-    if (rc) { release(); return rc; }
-  }
-  release();
-  if (!(in_dev && out_dev)) VG_TRY(cudaStreamSynchronize(stream));
-  #undef VG_TRY
+    const int threads = 256;
+    const int blocks = (int)std::min<int64_t>((total + threads - 1) / threads, (int64_t)dc->sm_count * 32);
+    const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
+    uint8_t* cells = d_cells.get<uint8_t>();
+    rc = with_label_width(label_bytes, [&](auto b) {
+      voxel_graph_expand_kernel<b><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float);
+      CUDA_TRY(cudaGetLastError());
+      return 0;
+    });
+    if (rc) return rc;
+    // half the anisotropy (vg:102-107, 199-204); the sqrt is taken by the gather instead
+    rc = run_passes(cells, 1, ndim, sx2, sy2, sz2, wx / 2, wy / 2, wz / 2, border, 0, d_doubled.get<float>(), *dc,
+                    stream);
+    if (rc) return rc;
+    voxel_graph_gather_kernel<<<blocks, threads, 0, stream>>>(d_doubled.get<const float>(), result, sx, sy, sz,
+                                                              (flags & EDTB200_SQRT) ? 1 : 0);
+    CUDA_TRY(cudaGetLastError());
+    if (!out_dev) {
+      rc = download(out, result, (size_t)total * sizeof(float), device, stream);
+      if (rc) return rc;
+    }
+  }                                                  // the scratch frees are queued before the wait
+  if (!(in_dev && out_dev)) CUDA_TRY(cudaStreamSynchronize(stream));
   return 0;
 }
 
@@ -937,22 +916,19 @@ int edtb200_pass_later(const void* labels_dev, int label_bytes, int axis, int64_
   // the pass's candidate sums are exact in double, and whether the integer hull tests apply.
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int64_t count = sx * sy * sz;
-  int* range_dev = nullptr;
-  CUDA_TRY(scratch_alloc(*dc, reinterpret_cast<void**>(&range_dev), 2 * sizeof(int), s));
   const int init[2] = {0, 1024};
   int range[2] = {0, 1024};
-  cudaError_t err = cudaMemcpyAsync(range_dev, init, sizeof(init), cudaMemcpyHostToDevice, s);
-  if (err == cudaSuccess) {
+  {
+    Scratch range_dev;                                           // freed before the wait below
+    CUDA_TRY(range_dev.alloc(*dc, 2 * sizeof(int), s));
+    CUDA_TRY(cudaMemcpyAsync(range_dev.get(), init, sizeof(init), cudaMemcpyHostToDevice, s));
     int64_t blocks = (count + 255) / 256;
     if (blocks > (int64_t)dc->sm_count * 8) blocks = (int64_t)dc->sm_count * 8;
-    sample_range_kernel<<<(unsigned)blocks, 256, 0, s>>>(f_dev, count, range_dev);
-    err = cudaGetLastError();
+    sample_range_kernel<<<(unsigned)blocks, 256, 0, s>>>(f_dev, count, range_dev.get<int>());
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(range, range_dev.get(), sizeof(range), cudaMemcpyDeviceToHost, s));
   }
-  if (err == cudaSuccess) err = cudaMemcpyAsync(range, range_dev, sizeof(range), cudaMemcpyDeviceToHost, s);
-  const cudaError_t freed = cudaFreeAsync(range_dev, s);        // on every path once allocated
-  if (err == cudaSuccess) err = freed;
-  if (err == cudaSuccess) err = cudaStreamSynchronize(s);
-  CUDA_TRY(err);
+  CUDA_TRY(cudaStreamSynchronize(s));
   float fmax;
   memcpy(&fmax, &range[0], sizeof(float));
   const edtb200::LineGeom g = geom_for_axis(axis, sx, sy, sz);
@@ -987,14 +963,13 @@ int edtb200_slab_face_runs(const void* labels_dev, int label_bytes, int64_t sx, 
   const unsigned blocks = (unsigned)((plane + 255) / 256);
   const int zl = (flags & EDTB200_SIGNED) ? 1 : 0;
   using namespace edtb200;
-  switch (label_bytes) {
-    case 1: face_runs_kernel<1><<<blocks, 256, 0, stream>>>(static_cast<const uint8_t*>(labels_dev), plane, (int)sz, high_face, halo, zl, m_dev, overflow_dev); break;
-    case 2: face_runs_kernel<2><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(labels_dev), plane, (int)sz, high_face, halo, zl, m_dev, overflow_dev); break;
-    case 4: face_runs_kernel<4><<<blocks, 256, 0, stream>>>(static_cast<const uint32_t*>(labels_dev), plane, (int)sz, high_face, halo, zl, m_dev, overflow_dev); break;
-    default: face_runs_kernel<8><<<blocks, 256, 0, stream>>>(static_cast<const uint64_t*>(labels_dev), plane, (int)sz, high_face, halo, zl, m_dev, overflow_dev); break;
-  }
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+  return with_label_width(label_bytes, [&](auto b) {
+    using LT = typename LabelOf<b>::type;
+    face_runs_kernel<b><<<blocks, 256, 0, stream>>>(static_cast<const LT*>(labels_dev), plane, (int)sz, high_face,
+                                                    halo, zl, m_dev, overflow_dev);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  });
 }
 
 int edtb200_slab_pack(const void* src_dev, void* dst_dev, int64_t zc, int64_t sy, int64_t row_bytes, int parts,
@@ -1049,14 +1024,14 @@ int edtb200_slab_face_fixup(const void* labels_dev, int label_bytes, int64_t sx,
   // the last pass's store, on a transform whose first pass may have treated background as a label
   const int kflags = kernel_flags(flags, /*first=*/true, /*last=*/true);
   const float w2 = wz * wz;
-  switch (label_bytes) {
-    case 1: face_fixup_kernel<1><<<blocks, 256, 0, stream>>>(static_cast<const uint8_t*>(labels_dev), f_dev, plane, (int)sz, high_face, halo, w2, static_cast<const uint8_t*>(nb_label_dev), nb_m_dev, nb_f_dev, kflags, inexact_dev); break;
-    case 2: face_fixup_kernel<2><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(labels_dev), f_dev, plane, (int)sz, high_face, halo, w2, static_cast<const uint16_t*>(nb_label_dev), nb_m_dev, nb_f_dev, kflags, inexact_dev); break;
-    case 4: face_fixup_kernel<4><<<blocks, 256, 0, stream>>>(static_cast<const uint32_t*>(labels_dev), f_dev, plane, (int)sz, high_face, halo, w2, static_cast<const uint32_t*>(nb_label_dev), nb_m_dev, nb_f_dev, kflags, inexact_dev); break;
-    default: face_fixup_kernel<8><<<blocks, 256, 0, stream>>>(static_cast<const uint64_t*>(labels_dev), f_dev, plane, (int)sz, high_face, halo, w2, static_cast<const uint64_t*>(nb_label_dev), nb_m_dev, nb_f_dev, kflags, inexact_dev); break;
-  }
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+  return with_label_width(label_bytes, [&](auto b) {
+    using LT = typename LabelOf<b>::type;
+    face_fixup_kernel<b><<<blocks, 256, 0, stream>>>(static_cast<const LT*>(labels_dev), f_dev, plane, (int)sz,
+                                                     high_face, halo, w2, static_cast<const LT*>(nb_label_dev),
+                                                     nb_m_dev, nb_f_dev, kflags, inexact_dev);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  });
 }
 
 // ---- one host volume on several GPUs of this process ---------------------------------------
@@ -1300,17 +1275,15 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
     unsigned long long* flag_in_lo_peer = has_lo ? reinterpret_cast<unsigned long long*>(lo + L.flag_from_hi) : nullptr;
     unsigned long long* flag_in_hi_peer = has_hi ? reinterpret_cast<unsigned long long*>(hi + L.flag_from_lo) : nullptr;
     unsigned int* counter = reinterpret_cast<unsigned int*>(self + L.counter);
-#define EDT_STAGE(B, T)                                                                                          \
-    slab_stage_kernel<B><<<grid, 256, 0, stream>>>(static_cast<const T*>(labels_dev), f_dev, plane, (int)sz, halo, \
-                                                   has_lo, has_hi, set, L, step, flag_in_lo_peer, flag_in_hi_peer, counter)
-    switch (label_bytes) {
-      case 1: EDT_STAGE(1, uint8_t); break;
-      case 2: EDT_STAGE(2, uint16_t); break;
-      case 4: EDT_STAGE(4, uint32_t); break;
-      default: EDT_STAGE(8, uint64_t); break;
-    }
-#undef EDT_STAGE
-    CUDA_TRY(cudaGetLastError());
+    rc = with_label_width(label_bytes, [&](auto b) {
+      using LT = typename LabelOf<b>::type;
+      slab_stage_kernel<b><<<grid, 256, 0, stream>>>(static_cast<const LT*>(labels_dev), f_dev, plane, (int)sz, halo,
+                                                     has_lo, has_hi, set, L, step, flag_in_lo_peer, flag_in_hi_peer,
+                                                     counter);
+      CUDA_TRY(cudaGetLastError());
+      return 0;
+    });
+    if (rc) return rc;
     nvtx_pop();
   }
 
@@ -1341,18 +1314,15 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
     fattr[0].val.programmaticStreamSerializationAllowed = 1;
     fcfg.attrs = fattr;
     fcfg.numAttrs = verbose ? 0 : 1;         // behind our own Z pass, which triggers its dependents early
-#define EDT_FIXUP(B, T)                                                                                          \
-    CUDA_TRY(cudaLaunchKernelEx(&fcfg, slab_fixup_kernel<B>, static_cast<const T*>(labels_dev), f_dev, plane, (int)sz, \
-                                halo, w2, has_lo, has_hi, set_lo, set_hi, L, step, flag_from_lo, flag_from_hi, kflags, \
-                                status_dev))
-    switch (label_bytes) {
-      case 1: EDT_FIXUP(1, uint8_t); break;
-      case 2: EDT_FIXUP(2, uint16_t); break;
-      case 4: EDT_FIXUP(4, uint32_t); break;
-      default: EDT_FIXUP(8, uint64_t); break;
-    }
-#undef EDT_FIXUP
-    CUDA_TRY(cudaGetLastError());
+    rc = with_label_width(label_bytes, [&](auto b) {
+      using LT = typename LabelOf<b>::type;
+      CUDA_TRY(cudaLaunchKernelEx(&fcfg, slab_fixup_kernel<b>, static_cast<const LT*>(labels_dev), f_dev, plane,
+                                  (int)sz, halo, w2, has_lo, has_hi, set_lo, set_hi, L, step, flag_from_lo,
+                                  flag_from_hi, kflags, status_dev));
+      CUDA_TRY(cudaGetLastError());
+      return 0;
+    });
+    if (rc) return rc;
     nvtx_pop();
   }
   stamp(5);
@@ -1392,20 +1362,14 @@ int edtb200_label_stats(const void* labels_dev, int label_bytes, const float* dt
   const int64_t total = sx * sy * sz;
   if (total > 0) {
     const unsigned blocks = (unsigned)std::min<int64_t>((total + 255) / 256, (int64_t)dc->sm_count * 16);
-    switch (label_bytes) {
-#define EDT_STATS(B, T)                                                                                       \
-      case B:                                                                                                 \
-        label_stats_kernel<B><<<blocks, 256, 0, stream>>>(static_cast<const T*>(labels_dev), dt_dev, total,   \
-                                                          (int)sx, (int)sy, t);                               \
-        label_argmax_kernel<B><<<blocks, 256, 0, stream>>>(static_cast<const T*>(labels_dev), dt_dev, total, t); \
-        break;
-      EDT_STATS(1, uint8_t) EDT_STATS(2, uint16_t) EDT_STATS(4, uint32_t)
-      default:
-        label_stats_kernel<8><<<blocks, 256, 0, stream>>>(static_cast<const uint64_t*>(labels_dev), dt_dev, total,
-                                                          (int)sx, (int)sy, t);
-        label_argmax_kernel<8><<<blocks, 256, 0, stream>>>(static_cast<const uint64_t*>(labels_dev), dt_dev, total, t);
-#undef EDT_STATS
-    }
+    rc = with_label_width(label_bytes, [&](auto b) {
+      using LT = typename LabelOf<b>::type;
+      label_stats_kernel<b><<<blocks, 256, 0, stream>>>(static_cast<const LT*>(labels_dev), dt_dev, total, (int)sx,
+                                                        (int)sy, t);
+      label_argmax_kernel<b><<<blocks, 256, 0, stream>>>(static_cast<const LT*>(labels_dev), dt_dev, total, t);
+      return 0;
+    });
+    if (rc) return rc;
   }
   label_table_finish_kernel<<<(capacity + 255) / 256, 256, 0, stream>>>(t);
   CUDA_TRY(cudaGetLastError());
@@ -1433,14 +1397,13 @@ int edtb200_label_extract(const void* labels_dev, int label_bytes, const float* 
   const int bx = b[3] - b[0] + 1, by = b[4] - b[1] + 1, bz = b[5] - b[2] + 1;
   const int64_t rows = (int64_t)by * bz;
   const unsigned blocks = (unsigned)std::min<int64_t>((rows + 7) / 8, (int64_t)dc->sm_count * 16);
-  switch (label_bytes) {
-    case 1: label_extract_kernel<1><<<blocks, 256, 0, stream>>>(static_cast<const uint8_t*>(labels_dev), dt_dev, out_dev, (int)sx, (int)sy, b[0], b[1], b[2], bx, by, bz, key, erase); break;
-    case 2: label_extract_kernel<2><<<blocks, 256, 0, stream>>>(static_cast<const uint16_t*>(labels_dev), dt_dev, out_dev, (int)sx, (int)sy, b[0], b[1], b[2], bx, by, bz, key, erase); break;
-    case 4: label_extract_kernel<4><<<blocks, 256, 0, stream>>>(static_cast<const uint32_t*>(labels_dev), dt_dev, out_dev, (int)sx, (int)sy, b[0], b[1], b[2], bx, by, bz, key, erase); break;
-    default: label_extract_kernel<8><<<blocks, 256, 0, stream>>>(static_cast<const uint64_t*>(labels_dev), dt_dev, out_dev, (int)sx, (int)sy, b[0], b[1], b[2], bx, by, bz, key, erase); break;
-  }
-  CUDA_TRY(cudaGetLastError());
-  return 0;
+  return with_label_width(label_bytes, [&](auto w) {
+    using LT = typename LabelOf<w>::type;
+    label_extract_kernel<w><<<blocks, 256, 0, stream>>>(static_cast<const LT*>(labels_dev), dt_dev, out_dev, (int)sx,
+                                                        (int)sy, b[0], b[1], b[2], bx, by, bz, key, erase);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  });
 }
 
 void* edtb200_host_alloc(size_t bytes) {

@@ -2,13 +2,15 @@
 //
 // The library is compiled as five translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches) and edt_passes_b{1,2,4,8}.cu (the axis-pass
-// launchers of edt_passes.cuh instantiated for one label width each).
+// launchers of edt_passes.cuh instantiated for one label width each).  The run-time label width
+// becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
 #include "edt_kernels.cuh"
 
 #include <cstdint>
 #include <mutex>
+#include <type_traits>
 
 namespace edtb200 {
 namespace host {
@@ -23,6 +25,19 @@ int fail(int code, const char* fmt, ...);
       return ::edtb200::host::fail(e__ == cudaErrorMemoryAllocation ? EDTB200_ENOMEM : EDTB200_ECUDA, \
                                    "%s failed: %s", #expr, cudaGetErrorString(e__));            \
   } while (0)
+
+// Returns f(std::integral_constant<int, B>{}) for the label width B = label_bytes, so that f can
+// name the width-templated kernel or launcher for B and its label type LabelOf<B>::type.
+template <class F>
+int with_label_width(int label_bytes, F&& f) {
+  switch (label_bytes) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+  }
+  return fail(EDTB200_EINVAL, "label_bytes must be 1, 2, 4 or 8 (got %d)", label_bytes);
+}
 
 // cuTensorMapEncodeTiled, fetched through the runtime so that libcuda is not a link-time
 // dependency (the library must load on machines without a driver, e.g. for the build check).
@@ -79,6 +94,28 @@ struct DeviceCache {
 
 // Stream-ordered scratch from the device's private pool (never the process-wide default pool).
 cudaError_t scratch_alloc(DeviceCache& dc, void** p, size_t bytes, cudaStream_t stream);
+
+// One scratch_alloc allocation, freed on the stream it was taken on when its owner goes out of
+// scope -- on every exit of the call that took it.
+class Scratch {
+ public:
+  Scratch() = default;
+  Scratch(Scratch&& o) noexcept : p_(o.p_), stream_(o.stream_) { o.p_ = nullptr; }
+  Scratch& operator=(Scratch&&) = delete;
+  ~Scratch() { if (p_) cudaFreeAsync(p_, stream_); }
+  cudaError_t alloc(DeviceCache& dc, size_t bytes, cudaStream_t stream) {
+    stream_ = stream;
+    const cudaError_t e = scratch_alloc(dc, &p_, bytes, stream);
+    if (e != cudaSuccess) p_ = nullptr;
+    return e;
+  }
+  template <class T = void>
+  T* get() const { return static_cast<T*>(p_); }
+
+ private:
+  void* p_ = nullptr;
+  cudaStream_t stream_ = nullptr;
+};
 
 // Device table T[0..count) for weight w, cached per device.
 int step_table(DeviceCache& dc, float w, int count, cudaStream_t stream, const float** out);

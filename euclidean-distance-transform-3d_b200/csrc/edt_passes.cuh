@@ -2,6 +2,7 @@
 //
 // Included by edt_passes_b{1,2,4,8}.cu, each of which instantiates launch_first / launch_later
 // for ONE label width (the kernel templates are large; four translation units build in parallel).
+// edt_capi.cu reaches the instance for a run-time width through with_label_width (edt_host.h).
 // These launchers play the role of the per-axis loops of the reference's volume driver
 // (pyedt::_edt3dsq, src/edt.hpp:428-475): which kernel variant, which tile shape, which grid.
 #pragma once
@@ -220,26 +221,20 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
   // ---- long-line kernel: out of place through a temporary volume ----
   const int64_t lines = g.inner_count * g.outer_count;
   const size_t bytes = sizeof(float) * (size_t)lines * (size_t)g.n;
-  float* tmp = nullptr;
-  int* hull = nullptr;
-  CUDA_TRY(scratch_alloc(dc, reinterpret_cast<void**>(&tmp), bytes, stream));
-  if (scratch_alloc(dc, reinterpret_cast<void**>(&hull), bytes, stream) != cudaSuccess) {
+  Scratch tmp, hull;                            // freed on every exit, hull first
+  CUDA_TRY(tmp.alloc(dc, bytes, stream));
+  if (hull.alloc(dc, bytes, stream) != cudaSuccess) {
     cudaGetLastError();
-    cudaFreeAsync(tmp, stream);
     return fail(EDTB200_ENOMEM, "no device memory for the long-line scratch volumes");
   }
   const int64_t blocks = (lines + 127) / 128;
-  if (blocks > 0x7fffffffLL) {
-    cudaFreeAsync(tmp, stream); cudaFreeAsync(hull, stream);
-    return fail(EDTB200_ELIMIT, "too many lines");
-  }
+  if (blocks > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many lines");
   later_axis_long_kernel<Bytes><<<(unsigned)blocks, 128, 0, stream>>>(
-      static_cast<const LT*>(labels), f, tmp, hull, g, w2, border_lo, border_hi, flags, p.all_double ? 0 : 4096);
+      static_cast<const LT*>(labels), f, tmp.get<float>(), hull.get<int>(), g, w2, border_lo, border_hi, flags,
+      p.all_double ? 0 : 4096);
   CUDA_TRY(cudaGetLastError());
   g_last_later = p;
-  CUDA_TRY(cudaMemcpyAsync(f, tmp, bytes, cudaMemcpyDeviceToDevice, stream));
-  CUDA_TRY(cudaFreeAsync(hull, stream));
-  CUDA_TRY(cudaFreeAsync(tmp, stream));
+  CUDA_TRY(cudaMemcpyAsync(f, tmp.get(), bytes, cudaMemcpyDeviceToDevice, stream));
   return 0;
 }
 

@@ -103,7 +103,7 @@ def test_face_fixup_profiles_vs_restatement(passes, kind):
   for halo in (1, 2, 33, 130, 254):
     nz = 40 if halo > 100 else 70
     shape = (nz, 3, 11)
-    for nbytes in (1, 8):
+    for nbytes in (1, 2, 4, 8):
       k += 1
       lab = wide_labels(rng, shape, nbytes, 6)
       z = np.abs(ec.profile(rng, kind, shape))

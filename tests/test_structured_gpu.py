@@ -113,12 +113,12 @@ def test_wide_lines_and_rows_that_are_not_stored(edt, oracle, reference):
 
 # ---- per-label views ------------------------------------------------------------------
 
-def many_labels(shape, nlabels, seed, dtype=np.uint32):
+def many_labels(shape, nlabels, seed, dtype=np.uint32, high=10 ** 6):
   lab = voronoi_labels(shape, nlabels, seed, dtype)
   rng = np.random.default_rng(seed + 1)
   lab[rng.uniform(size=shape) < 0.1] = 0                      # some background
-  # spread the label values out (the table hashes them)
-  lut = np.concatenate([[0], rng.choice(np.arange(1, 10 ** 6), nlabels, replace=False)]).astype(dtype)
+  # spread the label values out over 1..high-1 (the table hashes them)
+  lut = np.concatenate([[0], rng.choice(np.arange(1, high), nlabels, replace=False)]).astype(dtype)
   return np.asfortranarray(lut[lab])
 
 
@@ -156,25 +156,40 @@ def test_each_against_reference_each(edt, reference, order):
 
 
 def test_label_stats_and_each_cuda(edt):
+  check_label_stats_and_each_cuda(edt, np.int64, 310, 10 ** 6)
+
+
+@pytest.mark.parametrize("dtype, nlabels, high", [(np.uint8, 200, 1 << 8), (np.int16, 310, 1 << 15),
+                                                  (np.int32, 310, 10 ** 6)], ids=["uint8", "int16", "int32"])
+def test_label_stats_and_each_cuda_narrow_labels(edt, dtype, nlabels, high):
+  """edtb200_label_stats and edtb200_label_extract at the label widths below 8 bytes."""
+  check_label_stats_and_each_cuda(edt, dtype, nlabels, high)
+
+
+def check_label_stats_and_each_cuda(edt, dtype, nlabels, high):
+  """label_stats_cuda and each_cuda on `nlabels` labels of `dtype` drawn from 1..high-1, one of
+  them negative where the dtype is signed, against numpy."""
   import torch
-  lab_np = np.ascontiguousarray(many_labels((40, 72, 65), 310, 13, np.int64))
-  lab_np[lab_np == lab_np.max()] = -5                           # a negative label: compared as raw bits
+  lab_np = np.ascontiguousarray(many_labels((40, 72, 65), nlabels, 13, dtype, high))
+  if np.issubdtype(dtype, np.signedinteger):
+    lab_np[lab_np == lab_np.max()] = -5                         # a negative label: compared as raw bits
   lab = torch.from_numpy(lab_np).cuda()
   dt = edt.edt_cuda(lab, (2.0, 1.0, 1.0), False, sqrt=True)
   dt_np = dt.cpu().numpy()
   stats = edt.label_stats_cuda(lab, dt)
-  keys = stats["labels"].cpu().numpy()
-  uniq = np.unique(lab_np)
+  keys = stats["labels"].cpu().numpy().view(np.uint64)        # the labels' raw bits, zero-extended
+  bits = lab_np.view("u%d" % lab_np.itemsize)
+  uniq = np.unique(bits)
   uniq = uniq[uniq != 0]
   assert sorted(keys.tolist()) == sorted(uniq.tolist())
-  flat_lab, flat_dt = lab_np.ravel(), dt_np.ravel()
+  flat_lab, flat_dt = bits.ravel(), dt_np.ravel()
   for k, cnt, mx, am, box in zip(keys.tolist(), stats["count"].tolist(), stats["max"].tolist(),
                                  stats["argmax"].tolist(), stats["box"].tolist()):
     where = np.flatnonzero(flat_lab == k)
     assert cnt == where.size
     assert np.float32(mx) == flat_dt[where].max()
     assert am == where[np.argmax(flat_dt[where])]               # first index of the maximum
-    idx = np.argwhere(lab_np == k)
+    idx = np.argwhere(bits == k)
     assert box[:3] == idx.min(0).tolist() and box[3:] == idx.max(0).tolist()
   n = 0
   for key, img in edt.each_cuda(lab, dt):

@@ -33,6 +33,7 @@ __all__ = [
   "edt", "edtsq", "sdf", "sdfsq",
   "edt1d", "edt1dsq", "edt2d", "edt2dsq", "edt3d", "edt3dsq",
   "edt_cuda", "transform_batch", "each", "each_cuda", "label_stats_cuda", "device_count", "library_path", "EDTError",
+  "feature_transform", "expand_labels",
 ]
 
 FLAG_SQRT = 1
@@ -73,6 +74,8 @@ def _lib():
   lib.edtb200_device_count.restype = ci
   lib.edtb200_transform.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp]
   lib.edtb200_transform.restype = ci
+  lib.edtb200_feature_transform.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
+  lib.edtb200_feature_transform.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
   lib.edtb200_transform_multi.restype = ci
   lib.edtb200_transform_batch.argtypes = [vp, vp, ci, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, ci]
@@ -631,6 +634,161 @@ def transform_batch(volumes, anisotropy=None, black_border=False, *, sqrt=False,
   _check(_lib().edtb200_transform_batch(lab_ptrs, out_ptrs, n, views[0].dtype.itemsize, nd, sx, sy, sz,
                                         wx, wy, wz, int(bool(black_border)), flags, int(device)))
   return outs
+
+
+# ---------------------------------------------------------------------------------------
+# feature transform: WHERE the nearest boundary is (scipy's return_indices), and expand_labels
+# ---------------------------------------------------------------------------------------
+
+def _feature_anisotropy(dims, anisotropy):
+  """Default and 1-D anisotropy handling of _front_door."""
+  if dims == 1:
+    anisotropy = nvl(anisotropy, 1.0)
+    if np.ndim(anisotropy) != 0:
+      anisotropy = np.asarray(anisotropy).reshape(-1)[0]
+    return (float(anisotropy),)
+  if dims in (2, 3):
+    anisotropy = tuple(float(a) for a in nvl(anisotropy, (1.0,) * dims))
+    if len(anisotropy) != dims:
+      raise ValueError("anisotropy must have one entry per dimension")
+    return anisotropy
+  raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
+
+
+def _feature_host(data, anisotropy, black_border, flags, want_dist, device):
+  """(distances or None, indices) of a numpy array through host buffers (edtb200_feature_transform)."""
+  if isinstance(data, list):
+    data = np.array(data)
+  data = np.asarray(data)
+  nd = data.ndim
+  anisotropy = _feature_anisotropy(nd, anisotropy)
+  if not data.flags.c_contiguous and not data.flags.f_contiguous:
+    data = np.ascontiguousarray(data)
+  order = "F" if data.flags.f_contiguous else "C"
+  labels = _label_view(data)
+  if labels is None:
+    raise TypeError("feature_transform: unsupported label dtype %s" % data.dtype)
+  # one plane per array axis, each in the input's memory order: for F order the planes are
+  # allocated with the axes reversed and viewed back
+  planes = np.empty((nd,) + (data.shape if order == "C" else data.shape[::-1]), dtype=np.int32)
+  dist = np.zeros(data.size, dtype=np.float32) if want_dist else None
+  if data.size:
+    (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
+    # x-fastest axis j is array axis j in F order, array axis nd - 1 - j in C order
+    ptrs = (ctypes.c_void_p * nd)(*[planes[j if order == "F" else nd - 1 - j].ctypes.data for j in range(nd)])
+    _check(_lib().edtb200_feature_transform(
+      labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), int(flags),
+      dist.ctypes.data if want_dist else None, ptrs, int(device), None))
+  indices = planes if order == "C" else planes.transpose((0,) + tuple(range(nd, 0, -1)))
+  return (dist.reshape(data.shape, order=order) if want_dist else None), indices
+
+
+def _feature_device(t, anisotropy, black_border, flags, want_dist):
+  """(distances or None, indices) of a torch CUDA tensor as torch CUDA tensors on its current
+  stream, without host copies.  A Fortran-ordered tensor goes through its transposed view, as in
+  _front_door_device, and its results are returned in its order."""
+  import torch
+  dims = t.dim()
+  anisotropy = _feature_anisotropy(dims, anisotropy)
+  if t.dtype in (torch.float32, torch.float64):
+    t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)     # -0.0 == +0.0
+  nbytes = _torch_label_bytes(torch).get(t.dtype)
+  if nbytes is None:
+    raise TypeError("feature_transform: unsupported label dtype %s" % t.dtype)
+  fortran = dims > 1 and not t.is_contiguous() and t.permute(*reversed(range(dims))).is_contiguous()
+  if fortran:
+    t = t.permute(*reversed(range(dims)))
+    anisotropy = tuple(reversed(anisotropy))
+  t = t.contiguous()
+  planes = torch.empty((dims,) + tuple(t.shape), dtype=torch.int32, device=t.device)
+  dist = torch.zeros(t.shape, dtype=torch.float32, device=t.device) if want_dist else None
+  if t.numel():
+    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape, anisotropy, False)
+    # x-fastest axis j is the caller's array axis j when it was F-ordered, else axis dims - 1 - j
+    ptrs = (ctypes.c_void_p * dims)(*[planes[j if fortran else dims - 1 - j].data_ptr() for j in range(dims)])
+    stream = torch.cuda.current_stream(t.device).cuda_stream
+    _check(_lib().edtb200_feature_transform(
+      t.data_ptr(), nbytes, dims, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
+      int(flags) | FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, dist.data_ptr() if want_dist else None, ptrs,
+      t.device.index, ctypes.c_void_p(stream)))
+  if fortran:
+    planes = planes.permute(0, *range(dims, 0, -1))
+    dist = dist.permute(*reversed(range(dims))) if want_dist else None
+  return dist, planes
+
+
+def feature_transform(data, anisotropy=None, black_border=False, *, signed=False, return_distances=False, device=0):
+  """The nearest site of every voxel: scipy.ndimage.distance_transform_edt(return_indices=True)
+  for multi-label volumes, on the GPU.
+
+  A site of voxel p is a voxel of another label, or with `black_border` a position just outside
+  the volume (one coordinate -1 or n).  Foreground voxels get a nearest site; background voxels
+  (label 0) get themselves, or with `signed=True` -- background as an ordinary label, as in sdf --
+  their nearest voxel of a non-zero label.  Where there is no site at all (only possible without
+  `black_border`) every coordinate is -1.  Among equally near sites, any one is returned, the same
+  one on every run.
+
+  Returns `indices`, int32 of shape (data.ndim,) + data.shape in scipy's layout (indices[k] is the
+  coordinate along array axis k, each plane in the input's memory order), or with
+  `return_distances=True` the pair (distances, indices), the distances equal to edt(data) (or
+  sdf(data) with `signed=True`) bit for bit.  Arguments are handled as by edt(); device-resident
+  input (a torch CUDA tensor or `__cuda_array_interface__`) returns torch CUDA tensors, computed on
+  the current stream."""
+  flags = FLAG_SQRT | (FLAG_SIGNED if signed else 0)
+  on_device = _device_array(data)
+  if on_device is not None:
+    dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances)
+  else:
+    dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device)
+  return (dist, idx) if return_distances else idx
+
+
+def _same_size_signed(torch, t):
+  """t viewed as a signed integer type of its width when torch's indexing may not take its own
+  (the unsigned types beyond uint8)."""
+  for name, signed in (("uint16", torch.int16), ("uint32", torch.int32), ("uint64", torch.int64)):
+    if t.dtype == getattr(torch, name, None):
+      return t.view(signed)
+  return t
+
+
+def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0):
+  """skimage.segmentation.expand_labels on the GPU: every background voxel (label 0) whose nearest
+  labelled voxel lies within `distance` takes that voxel's label; labelled voxels keep theirs.
+  "Within" compares the squared distance (as sdfsq computes it, in float64) with distance**2.
+  The result has the dtype, shape and memory order of `labels`; a torch CUDA tensor in gives one
+  out.  Built on feature_transform(signed=True): the labels are gathered on the device."""
+  import torch
+  on_device = _device_array(labels)
+  if on_device is None:
+    arr = np.asarray(labels)
+    if not arr.flags.c_contiguous and not arr.flags.f_contiguous:
+      arr = np.ascontiguousarray(arr)
+    if _label_view(arr) is None:
+      raise TypeError("expand_labels: unsupported label dtype %s" % arr.dtype)
+    raw = arr.view(np.uint8 if arr.dtype.itemsize == 1 else np.dtype("i%d" % arr.dtype.itemsize))
+    if arr.dtype.kind == "f":
+      raw = arr                              # folded by _feature_device and compared by value below
+    out = expand_labels(torch.from_numpy(raw).to(torch.device("cuda", int(device))), distance, anisotropy)
+    return out.cpu().numpy().view(arr.dtype)
+  t = on_device
+  if not t.is_contiguous() and not t.permute(*reversed(range(t.dim()))).is_contiguous():
+    t = t.contiguous()
+  dist, idx = _feature_device(t, anisotropy, False, FLAG_SIGNED, True)
+  if t.numel() == 0:
+    return t.clone()
+  # the site as a C-order linear index; -1 (no site) is masked out below
+  lin = torch.zeros(t.shape, dtype=torch.int64, device=t.device)
+  step = 1
+  for k in reversed(range(t.dim())):
+    lin += idx[k].to(torch.int64) * step
+    step *= int(t.shape[k])
+  take = _same_size_signed(torch, t)
+  grow = (take == 0) & (idx[0] >= 0) & (dist.abs().to(torch.float64) <= float(distance) ** 2)
+  grown = torch.where(grow, take.reshape(-1)[lin.clamp(min=0)], take)
+  out = torch.empty_like(t)                  # t's memory order
+  _same_size_signed(torch, out).copy_(grown)
+  return out
 
 
 # ---------------------------------------------------------------------------------------

@@ -619,6 +619,44 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   return rc;
 }
 
+// All passes of one feature transform on device-resident buffers: the site-tracking passes, out of
+// place and alternating between `dist` and one scratch volume so that the last lands in `dist`, then
+// the resolver.  dist may be null (the distances then stay in scratch).
+int run_feature_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                       float wx, float wy, float wz, int border, int flags, float* dist, int32_t* const idx[3],
+                       DeviceCache& dc, cudaStream_t s) {
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
+  const size_t total = (size_t)(sx * sy * sz);
+  Scratch own_dist, other, codes;
+  auto take = [&](Scratch& sc, size_t bytes) {
+    if (sc.alloc(dc, bytes, s) == cudaSuccess) return 0;
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the feature transform's scratch (%zu bytes)", bytes);
+  };
+  int rc = dist ? 0 : take(own_dist, total * sizeof(float));
+  if (!rc && ndim >= 2) rc = take(other, total * sizeof(float));
+  if (!rc) rc = take(codes, (size_t)ndim * total * sizeof(int));
+  if (rc) return rc;
+  float* buf[2] = {dist ? dist : own_dist.get<float>(), other.get<float>()};
+  int* code_planes[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < ndim; ++k) code_planes[k] = codes.get<int>() + (size_t)k * total;
+  // pass k writes buf[(ndim - 1 - k) % 2]: the last one (k = ndim - 1) writes buf[0]
+  rc = with_label_width(label_bytes, [&](auto b) {
+    return launch_first_sites<b>(labels, buf[(ndim - 1) % 2], code_planes[0], sy * sz, sx, wx, border,
+                                 kernel_flags(flags, true, ndim == 1), dc, s);
+  });
+  for (int k = 1; !rc && k < ndim; ++k) {
+    rc = with_label_width(label_bytes, [&](auto b) {
+      return launch_later_sites<b>(labels, buf[(ndim - k) % 2], buf[(ndim - 1 - k) % 2], code_planes[k],
+                                   geom_for_axis(k, sx, sy, sz), t.w[k], border, border,
+                                   kernel_flags(flags, false, k == ndim - 1), transform_arith(t.w, t.n, k), dc, s);
+    });
+  }
+  if (rc) return rc;
+  return with_label_width(label_bytes, [&](auto b) {
+    return launch_resolve_sites<b>(labels, code_planes, ndim, sx, sy, sz, !(flags & EDTB200_SIGNED), idx, dc, s);
+  });
+}
 
 }  // namespace
 
@@ -685,6 +723,76 @@ int edtb200_transform(const void* labels, int label_bytes, int ndim, int64_t sx,
   if (rc) return rc;
   if (!out_dev) {
     rc = download(out, d_out, out_bytes, device, stream);
+    if (rc) return rc;
+  }
+  CUDA_TRY(cudaStreamSynchronize(stream));
+  return 0;
+}
+
+int edtb200_feature_transform(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                              float wx, float wy, float wz, int black_border, int flags, float* dist_out,
+                              int32_t* const* idx_out, int device, void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  const int64_t total = sx * sy * sz;
+  if (total == 0) return 0;
+  if (!labels || !idx_out) return fail(EDTB200_EINVAL, "null pointer");
+  for (int k = 0; k < ndim; ++k)
+    if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  rc = probe(device, &dc);
+  if (rc) return rc;
+
+  const bool lab_dev = flags & EDTB200_LABELS_ON_DEVICE;
+  const bool out_dev = flags & EDTB200_OUT_ON_DEVICE;
+  const int border = black_border != 0;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  int32_t* idx[3] = {idx_out[0], ndim > 1 ? idx_out[1] : nullptr, ndim > 2 ? idx_out[2] : nullptr};
+
+  if (lab_dev && out_dev)
+    return run_feature_passes(labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, dist_out, idx, *dc,
+                              stream);
+
+  // host memory involved: staged as in edtb200_transform, synchronous on return
+  std::lock_guard<std::mutex> host_call(dc->host_call);
+  if (!stream && !lab_dev && !out_dev) {
+    if (!dc->stream) CUDA_TRY(cudaStreamCreateWithFlags(&dc->stream, cudaStreamNonBlocking));
+    stream = dc->stream;
+  }
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
+  const size_t idx_bytes = (size_t)total * sizeof(int32_t);
+  const void* d_labels = labels;
+  if (!lab_dev) {
+    CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+    rc = upload(dc->labels, labels, lab_bytes, device, stream);
+    if (rc) return rc;
+    d_labels = dc->labels;
+  }
+  float* d_dist = dist_out;
+  int32_t* d_idx[3] = {idx[0], idx[1], idx[2]};
+  Scratch planes;
+  if (!out_dev) {
+    if (dist_out) {
+      CUDA_TRY(grow(dc->dist, dc->dist_bytes, (size_t)total * sizeof(float)));
+      d_dist = dc->dist;
+    }
+    if (planes.alloc(*dc, (size_t)ndim * idx_bytes, stream) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(EDTB200_ENOMEM, "no device memory for the index planes");
+    }
+    for (int k = 0; k < ndim; ++k) d_idx[k] = planes.get<int32_t>() + (size_t)k * (size_t)total;
+  }
+  rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, d_dist, d_idx, *dc,
+                          stream);
+  if (rc) return rc;
+  if (!out_dev) {
+    if (dist_out) {
+      rc = download(dist_out, d_dist, (size_t)total * sizeof(float), device, stream);
+      if (rc) return rc;
+    }
+    for (int k = 0; k < ndim && !rc; ++k) rc = download(idx[k], d_idx[k], idx_bytes, device, stream);
     if (rc) return rc;
   }
   CUDA_TRY(cudaStreamSynchronize(stream));

@@ -141,6 +141,19 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
 template <int Bytes>
 int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
                  int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl);
+// The site-tracking passes of the feature transform and the kernel that resolves their codes
+// into coordinate planes (edt_passes.cuh, edt_feature.cuh).
+template <int Bytes>
+int launch_first_sites(const void* labels, float* f, int* codes, int64_t nlines, int64_t sx, float w, int border,
+                       int flags, DeviceCache& dc, cudaStream_t stream);
+template <int Bytes>
+int launch_later_sites(const void* labels, const float* fin, float* fout, int* codes, const LineGeom& g, float w,
+                       int border_lo, int border_hi, int flags, PassArith arith, DeviceCache& dc,
+                       cudaStream_t stream);
+template <int Bytes>
+int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim, int64_t sx, int64_t sy,
+                         int64_t sz, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
+                         cudaStream_t stream);
 
 // What a later-axis launch runs (plan_later in edt_passes.cuh); the last one launched on the
 // calling thread is kept for edtb200_last_later_launch.

@@ -32,6 +32,16 @@ enum : int { kSqrt = 1, kNegate = 2, kZeroLabel = 4 };
 
 constexpr int kNoBoundary = 0x3fffffff;
 
+// Site codes of the site-tracking passes (Sites = true), one int per voxel and pass:
+//   X pass      the site's x coordinate, -1 or sx for a volume face;
+//   Y / Z pass  the row of the hull vertex that won (>= 0), or a DIRECT site: the row a - 1 or b
+//               just outside the run, whose border term won (the site itself, not a sample of it),
+//               stored as site_direct(row) <= -1;
+//   any pass    kSiteNone where the distance is +inf.
+constexpr int kSiteNone = INT32_MIN;
+__host__ __device__ __forceinline__ int site_direct(int row) { return -2 - row; }
+__host__ __device__ __forceinline__ int site_direct_row(int code) { return -2 - code; }
+
 template <int Bytes> struct LabelOf;
 template <> struct LabelOf<1> { using type = uint8_t;  using wide = uint32_t; };
 template <> struct LabelOf<2> { using type = uint16_t; using wide = uint32_t; };
@@ -103,12 +113,14 @@ static __global__ void step_table_kernel(float w, int count, float* __restrict__
 //   sweep 3: per voxel, nearest boundary on each side with clz/ffs on its own word, then
 //            the table lookup and a coalesced float store.
 // B[j] (1 <= j < sx) says labels j-1 and j differ; B[0] and B[sx] are the volume faces.
+// Sites: also write each voxel's site code (see kSiteNone) to `codes`, laid out like `out`.
 // ---------------------------------------------------------------------------------------
-template <int Bytes>
+template <int Bytes, bool Sites = false>
 __global__ void __launch_bounds__(256)
 first_axis_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
                   float* __restrict__ out, int64_t nlines, int sx,
-                  const float* __restrict__ table, int border, int flags, RunStat stat) {
+                  const float* __restrict__ table, int border, int flags, RunStat stat,
+                  int* __restrict__ codes) {
   using LT = typename LabelOf<Bytes>::type;
   using WT = typename LabelOf<Bytes>::wide;
   extern __shared__ uint32_t smem_u32[];
@@ -214,6 +226,9 @@ first_axis_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
         float val = (k >= kNoBoundary) ? __int_as_float(0x7f800000) : __ldg(table + k);
         if (background && !(flags & kZeroLabel)) val = 0.0f;
         dst[p] = finish_value(val, background, flags);
+        // the site at jl - 1 (boundary bit jl is the step from it into this run) or jr; the lower
+        // one on a tie
+        if constexpr (Sites) codes[line * sx + p] = (k >= kNoBoundary) ? kSiteNone : (kl <= kr ? jl - 1 : jr);
       }
     }
     __syncwarp();
@@ -1355,11 +1370,13 @@ __device__ __forceinline__ float parabola_at(float w2, int d, float height, int 
 // O(n) per line, with the vertex stack in a global scratch volume `hull` laid out like f (entry
 // k of the run that starts at row a lives at row a + k of the same line) and everything read
 // through L1/L2.  Out of place (fin -> fout), so no synchronisation is needed.
-template <int Bytes>
+// Sites: also write each voxel's site code (see kSiteNone) to `codes`, laid out like fout.
+template <int Bytes, bool Sites = false>
 __global__ void __launch_bounds__(128)
 later_axis_long_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
                        const float* __restrict__ fin, float* __restrict__ fout, int* __restrict__ hull,
-                       LineGeom g, float w2, int border_lo, int border_hi, int flags, int dbl_from) {
+                       LineGeom g, float w2, int border_lo, int border_hi, int flags, int dbl_from,
+                       int* __restrict__ codes) {
   using LT = typename LabelOf<Bytes>::type;
   const int64_t lines_per_outer = g.inner_count;
   const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1421,8 +1438,22 @@ later_axis_long_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
         }
         best = parabola_at(w2, abs(i - v), fv, dbl_from);
       }
-      if (lo_border) best = fminf(best, parabola_at(w2, i - a + 1, 0.0f));
-      if (hi_border) best = fminf(best, parabola_at(w2, b - i, 0.0f));
+      if constexpr (Sites) {
+        // a border term is the distance to the voxel (or face) just outside the run, on this line
+        int site = top >= 0 ? v : kSiteNone;
+        if (lo_border) {
+          const float c = parabola_at(w2, i - a + 1, 0.0f);
+          if (c < best) { best = c; site = site_direct(a - 1); }
+        }
+        if (hi_border) {
+          const float c = parabola_at(w2, b - i, 0.0f);
+          if (c < best) { best = c; site = site_direct(b); }
+        }
+        codes[base + (int64_t)i * ls] = best < inf ? site : kSiteNone;
+      } else {
+        if (lo_border) best = fminf(best, parabola_at(w2, i - a + 1, 0.0f));
+        if (hi_border) best = fminf(best, parabola_at(w2, b - i, 0.0f));
+      }
       fout[base + (int64_t)i * ls] = finish_value(best, mine == 0, flags);
     }
     a = b;

@@ -7,12 +7,39 @@
 // (pyedt::_edt3dsq, src/edt.hpp:428-475): which kernel variant, which tile shape, which grid.
 #pragma once
 #include "edt_host.h"
+#include "edt_feature.cuh"
 
 #include <cstdlib>
 #include <cstring>
 
 namespace edtb200 {
 namespace host {
+
+// The generic first-axis kernel (any row length and alignment), one warp per row.
+template <int Bytes, bool Sites>
+int launch_first_generic(const void* labels, float* f, int* codes, int64_t nlines, int64_t sx, const float* table,
+                         int border, int flags, RunStat stat, DeviceCache& dc, cudaStream_t stream) {
+  using LT = typename LabelOf<Bytes>::type;
+  const int nwords = (int)(sx >> 5) + 1;
+  const size_t per_warp = sizeof(uint32_t) * 4 * (size_t)nwords;
+  int warps = 8;
+  while (warps > 1 && per_warp * warps > (size_t)dc.max_smem_optin) warps >>= 1;
+  if (per_warp * warps > (size_t)dc.max_smem_optin) {
+    return fail(EDTB200_ELIMIT, "first axis of %lld voxels exceeds the shared-memory line buffer",
+                (long long)sx);
+  }
+  const size_t smem = per_warp * warps;
+  auto kern = first_axis_kernel<Bytes, Sites>;
+  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int64_t blocks = (nlines + warps - 1) / warps;
+  const int64_t cap = (int64_t)dc.sm_count * 16;
+  if (blocks > cap) blocks = cap;
+  if (blocks < 1) blocks = 1;
+  kern<<<(unsigned)blocks, warps * 32, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table,
+                                                       border, flags, stat, codes);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
 
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
@@ -51,25 +78,24 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
     CUDA_TRY(cudaGetLastError());
     return step_table_used(dc, table, stream);
   }
-  const int nwords = (int)(sx >> 5) + 1;
-  const size_t per_warp = sizeof(uint32_t) * 4 * (size_t)nwords;
-  int warps = 8;
-  while (warps > 1 && per_warp * warps > (size_t)dc.max_smem_optin) warps >>= 1;
-  if (per_warp * warps > (size_t)dc.max_smem_optin) {
-    return fail(EDTB200_ELIMIT, "first axis of %lld voxels exceeds the shared-memory line buffer",
-                (long long)sx);
-  }
-  const size_t smem = per_warp * warps;
-  auto kern = first_axis_kernel<Bytes>;
-  CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int64_t blocks = (nlines + warps - 1) / warps;
-  const int64_t cap = (int64_t)dc.sm_count * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  kern<<<(unsigned)blocks, warps * 32, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table,
-                                                       border, flags, stat);
-  CUDA_TRY(cudaGetLastError());
-  return step_table_used(dc, table, stream);
+  const int rc = launch_first_generic<Bytes, false>(labels, f, nullptr, nlines, sx, table, border, flags, stat, dc,
+                                                    stream);
+  return rc ? rc : step_table_used(dc, table, stream);
+}
+
+// The site-tracking X pass (feature transform): the generic kernel, which also writes the site
+// codes.  It publishes no run statistic, so it does not steer the next transform's launches.
+template <int Bytes>
+int launch_first_sites(const void* labels, float* f, int* codes, int64_t nlines, int64_t sx, float w, int border,
+                       int flags, DeviceCache& dc, cudaStream_t stream) {
+  const float* table = nullptr;
+  int trc = step_table(dc, w, (int)sx + 1, stream, &table);
+  if (trc) return trc;
+  RunStat none;
+  memset(&none, 0, sizeof(none));
+  const int rc = launch_first_generic<Bytes, true>(labels, f, codes, nlines, sx, table, border, flags, none, dc,
+                                                   stream);
+  return rc ? rc : step_table_used(dc, table, stream);
 }
 
 // Did the first-axis pass of the PREVIOUS transform on this device see label noise (at least nine
@@ -231,10 +257,50 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
   if (blocks > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many lines");
   later_axis_long_kernel<Bytes><<<(unsigned)blocks, 128, 0, stream>>>(
       static_cast<const LT*>(labels), f, tmp.get<float>(), hull.get<int>(), g, w2, border_lo, border_hi, flags,
-      p.all_double ? 0 : 4096);
+      p.all_double ? 0 : 4096, nullptr);
   CUDA_TRY(cudaGetLastError());
   g_last_later = p;
   CUDA_TRY(cudaMemcpyAsync(f, tmp.get(), bytes, cudaMemcpyDeviceToDevice, stream));
+  return 0;
+}
+
+// The site-tracking later pass (feature transform): the long-line kernel on any line length, out
+// of place (fin -> fout), also writing the site codes.  Its arithmetic is the one launch_later
+// gives the long-line kernel, so its distances equal launch_later's for any plan.
+template <int Bytes>
+int launch_later_sites(const void* labels, const float* fin, float* fout, int* codes, const LineGeom& g, float w,
+                       int border_lo, int border_hi, int flags, PassArith arith, DeviceCache& dc,
+                       cudaStream_t stream) {
+  using LT = typename LabelOf<Bytes>::type;
+  const int64_t lines = g.inner_count * g.outer_count;
+  const int64_t blocks = (lines + 127) / 128;
+  if (blocks > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many lines");
+  Scratch hull;
+  if (hull.alloc(dc, sizeof(int) * (size_t)lines * (size_t)g.n, stream) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the long-line hull scratch");
+  }
+  later_axis_long_kernel<Bytes, true><<<(unsigned)blocks, 128, 0, stream>>>(
+      static_cast<const LT*>(labels), fin, fout, hull.get<int>(), g, w * w, border_lo, border_hi, flags,
+      arith.exact ? 4096 : 0, codes);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// Site codes of every pass -> one coordinate plane per axis (edt_feature.cuh).
+template <int Bytes>
+int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim, int64_t sx, int64_t sy,
+                         int64_t sz, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
+                         cudaStream_t stream) {
+  const int64_t total = sx * sy * sz;
+  int64_t blocks = (total + 255) / 256;
+  const int64_t cap = (int64_t)dc.sm_count * 8;
+  if (blocks > cap) blocks = cap;
+  SiteCodes c{{codes[0], codes[1], codes[2]}, ndim, sx, sy, sz};
+  SitePlanes out{{idx[0], idx[1], idx[2]}};
+  resolve_sites_kernel<Bytes><<<(unsigned)blocks, 256, 0, stream>>>(
+      static_cast<const typename LabelOf<Bytes>::type*>(labels), c, zero_is_background ? 1 : 0, out);
+  CUDA_TRY(cudaGetLastError());
   return 0;
 }
 
@@ -246,4 +312,13 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
                                               edtb200::host::DeviceCache&, cudaStream_t);                \
   template int edtb200::host::launch_later<B>(const void*, float*, const edtb200::LineGeom&, float, int, \
                                               int, int, edtb200::host::PassArith,                        \
-                                              edtb200::host::DeviceCache&, cudaStream_t, bool);
+                                              edtb200::host::DeviceCache&, cudaStream_t, bool);          \
+  template int edtb200::host::launch_first_sites<B>(const void*, float*, int*, int64_t, int64_t, float, int, \
+                                                    int, edtb200::host::DeviceCache&, cudaStream_t);     \
+  template int edtb200::host::launch_later_sites<B>(const void*, const float*, float*, int*,              \
+                                                    const edtb200::LineGeom&, float, int, int, int,      \
+                                                    edtb200::host::PassArith,                            \
+                                                    edtb200::host::DeviceCache&, cudaStream_t);          \
+  template int edtb200::host::launch_resolve_sites<B>(const void*, const int* const*, int, int64_t,      \
+                                                      int64_t, int64_t, bool, int32_t* const*,           \
+                                                      edtb200::host::DeviceCache&, cudaStream_t);

@@ -32,8 +32,8 @@ extern "C" {
 /* 100: round 1 (transform, per-axis passes, slab face kernels).  200: additions only --
  * edtb200_transform_multi, edtb200_slab_step / _stage_bytes / _pack, edtb200_label_stats / _extract,
  * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
- * 201: additions only -- edtb200_last_later_launch. */
-#define EDTB200_VERSION 201
+ * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform. */
+#define EDTB200_VERSION 202
 
 /* flags */
 #define EDTB200_SQRT             1  /* emit sqrt(edtsq): reference _edt3d (src/edt.hpp:591-604) /
@@ -84,6 +84,43 @@ int edtb200_transform(const void *labels, int label_bytes, int ndim,
                       float wx, float wy, float wz,
                       int black_border, int flags,
                       float *out, int device, void *stream);
+
+/* Feature transform: for every voxel p the coordinates of its nearest SITE, and optionally the
+ * distance to it -- what scipy.ndimage.distance_transform_edt(return_indices=True) returns, for
+ * multi-label volumes.
+ *
+ * A site of p is a voxel q whose label differs from p's, or with black_border a face position
+ * (one coordinate -1 or n on its axis, the others inside the volume).
+ *   foreground p                   a nearest site;
+ *   background p, no EDTB200_SIGNED p itself (distance 0, as edtb200_transform gives it);
+ *   background p, EDTB200_SIGNED   background is an ordinary label (as for sdf): the nearest voxel
+ *                                  of any non-zero label, or a face position;
+ *   no site at all                 every coordinate -1, distance +inf (-inf for signed
+ *                                  background).  Only possible without black_border.
+ * "Nearest" is in the transform's own float32 arithmetic: the distance from p to its site,
+ * evaluated as the passes evaluate it (the X step table, then each later axis's term added in
+ * double and rounded once to float32), is bit for bit what edtb200_transform returns for p.  Among
+ * equally near sites any one may be returned, the same one on every run.
+ *
+ *   idx_out   ndim int32 planes laid out like the labels: idx_out[0] the x coordinate of the site,
+ *             idx_out[1] y, idx_out[2] z.  One pointer per plane, so a caller may hand over the
+ *             planes of an array in any order.
+ *   dist_out  NULL, or sx*sy*sz float32 distances: EDTB200_SQRT / EDTB200_SIGNED as for
+ *             edtb200_transform, equal to its result bit for bit
+ *   flags     EDTB200_SIGNED, EDTB200_SQRT, EDTB200_LABELS_ON_DEVICE, and EDTB200_OUT_ON_DEVICE,
+ *             which covers dist_out and every index plane
+ * Device-resident calls are asynchronous on `stream`; calls touching host memory return after
+ * the results have landed.  Every pass runs the one-thread-per-line kernels (no tile kernel).
+ * Device memory of one call, for V voxels: the labels (V * label_bytes, when uploaded), the
+ * distances (4V), one scratch volume for the passes' ping-pong (4V, ndim >= 2), the long-line
+ * kernel's hull (4V, ndim >= 2), ndim code planes (4V each) and ndim index planes (4V each, when
+ * downloaded): 36 bytes per voxel beyond the labels in 3-D, so 512^3 with uint32 labels needs
+ * 40 * 2^27 bytes, about 5.4 GB.  An allocation that fails returns EDTB200_ENOMEM. */
+int edtb200_feature_transform(const void *labels, int label_bytes, int ndim,
+                              int64_t sx, int64_t sy, int64_t sz,
+                              float wx, float wy, float wz,
+                              int black_border, int flags, float *dist_out,
+                              int32_t *const *idx_out, int device, void *stream);
 
 /* The same transform of ONE host volume spread over several GPUs of this process
  * (`devices[0..ndevices)`, distinct ordinals): SURVEY.md section 8b's `devices[] / ndevices`.

@@ -355,6 +355,63 @@ int download(void* dst_host, const void* src_dev, size_t bytes, int device, cuda
   return 0;
 }
 
+// The device's private non-blocking stream, created on first use by the holder of host_call.
+cudaError_t private_stream(DeviceCache& dc) {
+  return dc.stream ? cudaSuccess : cudaStreamCreateWithFlags(&dc.stream, cudaStreamNonBlocking);
+}
+
+// The residency contract of include/edt_b200.h for one call whose inputs and outputs may lie in
+// host memory: open() takes the device's host_call lock unless every buffer is on the device and
+// picks the stream; in() / out() give the device address of each buffer, uploading a host input
+// into the caller's staging buffer or noting a download from it; finish() runs the downloads in
+// order and, when host memory is involved, waits for them.
+struct HostIO {
+  bool in_dev = false, out_dev = false;
+  cudaStream_t stream = nullptr;
+
+  int open(DeviceCache& dc, int device, int flags, void* stream_v) {
+    in_dev = flags & EDTB200_LABELS_ON_DEVICE;
+    out_dev = flags & EDTB200_OUT_ON_DEVICE;
+    device_ = device;
+    stream = static_cast<cudaStream_t>(stream_v);
+    if (in_dev && out_dev) return 0;         // asynchronous on the caller's stream, no lock
+    lock_ = std::unique_lock<std::mutex>(dc.host_call);
+    // Both sides on the host and no stream given: the private stream.  With one side on the device
+    // the legacy default stream (NULL) is kept: it is ordered after the work the caller queued on
+    // the default / blocking streams that produced that buffer.
+    if (!stream && !in_dev && !out_dev) {
+      CUDA_TRY(private_stream(dc));
+      stream = dc.stream;
+    }
+    return 0;
+  }
+  template <class T>
+  int in(const T* src, size_t bytes, void* staging, const T** dev) {
+    *dev = in_dev ? src : static_cast<const T*>(staging);
+    return in_dev ? 0 : upload(staging, src, bytes, device_, stream);
+  }
+  template <class T>
+  T* out(T* dst, size_t bytes, T* staging) {
+    if (out_dev) return dst;
+    downloads_[count_++] = {dst, staging, bytes};
+    return staging;
+  }
+  int finish() {
+    for (int i = 0; i < count_; ++i) {
+      const int rc = download(downloads_[i].dst, downloads_[i].src, downloads_[i].bytes, device_, stream);
+      if (rc) return rc;
+    }
+    if (!(in_dev && out_dev)) CUDA_TRY(cudaStreamSynchronize(stream));
+    return 0;
+  }
+
+ private:
+  struct Download { void* dst; const void* src; size_t bytes; };
+  Download downloads_[4];                    // at most the distances and three index planes
+  int count_ = 0, device_ = 0;
+  std::unique_lock<std::mutex> lock_;
+};
+
 // Restores the calling thread's current CUDA device when an entry point returns (callers such as
 // PyTorch rely on "their" current device staying put).
 struct DeviceGuard {
@@ -683,50 +740,18 @@ int edtb200_transform(const void* labels, int label_bytes, int ndim, int64_t sx,
 
   DeviceGuard restore_device;
   DeviceCache* dc = nullptr;
-  rc = probe(device, &dc);
-  if (rc) return rc;
-
-  const bool lab_dev = flags & EDTB200_LABELS_ON_DEVICE;
-  const bool out_dev = flags & EDTB200_OUT_ON_DEVICE;
-  const int border = black_border != 0;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-
-  // device-resident: asynchronous on the caller's stream, no library-wide or per-device lock held
-  if (lab_dev && out_dev)
-    return run_passes(labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, out, *dc, stream);
-
-  // host memory involved: stage through this device's cached buffers, synchronous on return.
-  // Calls on other devices proceed concurrently (per-device lock).
-  std::lock_guard<std::mutex> host_call(dc->host_call);
-  if (!stream && !lab_dev && !out_dev) {
-    // pure host call: a private non-blocking stream.  With one side on the device and no stream
-    // given, the legacy default stream (NULL) is kept: it is ordered after the work the caller
-    // queued on the default / blocking streams that produced that buffer.
-    if (!dc->stream) CUDA_TRY(cudaStreamCreateWithFlags(&dc->stream, cudaStreamNonBlocking));
-    stream = dc->stream;
-  }
-  const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
-  const size_t out_bytes = (size_t)total * sizeof(float);
-  const void* d_labels = labels;
-  float* d_out = out;
-  if (!lab_dev) {
-    CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
-    rc = upload(dc->labels, labels, lab_bytes, device, stream);
-    if (rc) return rc;
-    d_labels = dc->labels;
-  }
-  if (!out_dev) {
-    CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
-    d_out = dc->dist;
-  }
-  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, d_out, *dc, stream);
-  if (rc) return rc;
-  if (!out_dev) {
-    rc = download(out, d_out, out_bytes, device, stream);
-    if (rc) return rc;
-  }
-  CUDA_TRY(cudaStreamSynchronize(stream));
-  return 0;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  // host buffers are staged through this device's cached buffers
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
+  float* d_out = io.out(out, out_bytes, dc->dist);
+  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_out, *dc,
+                  io.stream);
+  return rc ? rc : io.finish();
 }
 
 int edtb200_feature_transform(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
@@ -742,61 +767,29 @@ int edtb200_feature_transform(const void* labels, int label_bytes, int ndim, int
 
   DeviceGuard restore_device;
   DeviceCache* dc = nullptr;
-  rc = probe(device, &dc);
-  if (rc) return rc;
-
-  const bool lab_dev = flags & EDTB200_LABELS_ON_DEVICE;
-  const bool out_dev = flags & EDTB200_OUT_ON_DEVICE;
-  const int border = black_border != 0;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  int32_t* idx[3] = {idx_out[0], ndim > 1 ? idx_out[1] : nullptr, ndim > 2 ? idx_out[2] : nullptr};
-
-  if (lab_dev && out_dev)
-    return run_feature_passes(labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, dist_out, idx, *dc,
-                              stream);
-
-  // host memory involved: staged as in edtb200_transform, synchronous on return
-  std::lock_guard<std::mutex> host_call(dc->host_call);
-  if (!stream && !lab_dev && !out_dev) {
-    if (!dc->stream) CUDA_TRY(cudaStreamCreateWithFlags(&dc->stream, cudaStreamNonBlocking));
-    stream = dc->stream;
-  }
-  const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
-  const size_t idx_bytes = (size_t)total * sizeof(int32_t);
-  const void* d_labels = labels;
-  if (!lab_dev) {
-    CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
-    rc = upload(dc->labels, labels, lab_bytes, device, stream);
-    if (rc) return rc;
-    d_labels = dc->labels;
-  }
-  float* d_dist = dist_out;
-  int32_t* d_idx[3] = {idx[0], idx[1], idx[2]};
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  // host buffers are staged through the cached labels and distances and one scratch for the planes;
+  // a distance volume and an index plane are 4 bytes per voxel
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, vol_bytes = (size_t)total * sizeof(float);
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
   Scratch planes;
-  if (!out_dev) {
-    if (dist_out) {
-      CUDA_TRY(grow(dc->dist, dc->dist_bytes, (size_t)total * sizeof(float)));
-      d_dist = dc->dist;
-    }
-    if (planes.alloc(*dc, (size_t)ndim * idx_bytes, stream) != cudaSuccess) {
+  if (!io.out_dev) {
+    if (dist_out) CUDA_TRY(grow(dc->dist, dc->dist_bytes, vol_bytes));
+    if (planes.alloc(*dc, (size_t)ndim * vol_bytes, io.stream) != cudaSuccess) {
       cudaGetLastError();
       return fail(EDTB200_ENOMEM, "no device memory for the index planes");
     }
-    for (int k = 0; k < ndim; ++k) d_idx[k] = planes.get<int32_t>() + (size_t)k * (size_t)total;
   }
-  rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, d_dist, d_idx, *dc,
-                          stream);
-  if (rc) return rc;
-  if (!out_dev) {
-    if (dist_out) {
-      rc = download(dist_out, d_dist, (size_t)total * sizeof(float), device, stream);
-      if (rc) return rc;
-    }
-    for (int k = 0; k < ndim && !rc; ++k) rc = download(idx[k], d_idx[k], idx_bytes, device, stream);
-    if (rc) return rc;
-  }
-  CUDA_TRY(cudaStreamSynchronize(stream));
-  return 0;
+  float* d_dist = dist_out ? io.out(dist_out, vol_bytes, dc->dist) : nullptr;
+  int32_t* d_idx[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < ndim; ++k)
+    d_idx[k] = io.out(idx_out[k], vol_bytes, io.out_dev ? nullptr : planes.get<int32_t>() + (size_t)k * total);
+  rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_dist,
+                          d_idx, *dc, io.stream);
+  return rc ? rc : io.finish();
 }
 
 int edtb200_transform_batch(const void* const* labels, float* const* outs, int count, int label_bytes, int ndim,
@@ -827,7 +820,7 @@ int edtb200_transform_batch(const void* const* labels, float* const* outs, int c
     CUDA_TRY(grow(dc.labels2, dc.labels2_bytes, lab_bytes));
     CUDA_TRY(grow(dc.dist2, dc.dist2_bytes, out_bytes));
   }
-  if (!dc.stream) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream, cudaStreamNonBlocking));
+  CUDA_TRY(private_stream(dc));
   if (!dc.stream_up) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_up, cudaStreamNonBlocking));
   if (!dc.stream_down) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_down, cudaStreamNonBlocking));
   for (int i = 0; i < 2; ++i) {
@@ -931,65 +924,45 @@ int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const uns
 
   DeviceGuard restore_device;
   DeviceCache* dc = nullptr;
-  rc = probe(device, &dc);
-  if (rc) return rc;
-  const bool in_dev = flags & EDTB200_LABELS_ON_DEVICE;
-  const bool out_dev = flags & EDTB200_OUT_ON_DEVICE;
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
-  std::unique_lock<std::mutex> host_call(dc->host_call, std::defer_lock);
-  if (!(in_dev && out_dev)) host_call.lock();          // staging buffers and the private stream
-  if (!stream && !in_dev && !out_dev) {
-    if (!dc->stream) CUDA_TRY(cudaStreamCreateWithFlags(&dc->stream, cudaStreamNonBlocking));
-    stream = dc->stream;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  const cudaStream_t stream = io.stream;
+  // stream-ordered scratch: the inputs when they come from the host, the doubled byte mask, the
+  // doubled distance volume, and the result when it goes back to the host.  It is freed when the
+  // call returns, after io.finish() has queued the download of the result.
+  Scratch d_labels, d_graph, d_cells, d_doubled, d_result;
+  if (!io.in_dev) {
+    CUDA_TRY(d_labels.alloc(*dc, (size_t)total * label_bytes, stream));
+    CUDA_TRY(d_graph.alloc(*dc, (size_t)total, stream));
   }
+  const void* lab = nullptr;
+  const uint8_t* gr = nullptr;
+  if ((rc = io.in(labels, (size_t)total * label_bytes, d_labels.get(), &lab)) ||
+      (rc = io.in(graph, (size_t)total, d_graph.get(), &gr)))
+    return rc;
+  CUDA_TRY(d_cells.alloc(*dc, (size_t)total2, stream));
+  CUDA_TRY(d_doubled.alloc(*dc, (size_t)total2 * sizeof(float), stream));
+  if (!io.out_dev) CUDA_TRY(d_result.alloc(*dc, (size_t)total * sizeof(float), stream));
+  float* result = io.out(out, (size_t)total * sizeof(float), d_result.get<float>());
 
-  {
-    // stream-ordered scratch: the inputs when they come from the host, the doubled byte mask, the
-    // doubled distance volume, and the result when it goes back to the host
-    Scratch d_labels, d_graph, d_cells, d_doubled, d_result;
-    const void* lab = labels;
-    const uint8_t* gr = graph;
-    if (!in_dev) {
-      CUDA_TRY(d_labels.alloc(*dc, (size_t)total * label_bytes, stream));
-      CUDA_TRY(d_graph.alloc(*dc, (size_t)total, stream));
-      rc = upload(d_labels.get(), labels, (size_t)total * label_bytes, device, stream);
-      if (!rc) rc = upload(d_graph.get(), graph, (size_t)total, device, stream);
-      if (rc) return rc;
-      lab = d_labels.get();
-      gr = d_graph.get<const uint8_t>();
-    }
-    CUDA_TRY(d_cells.alloc(*dc, (size_t)total2, stream));
-    CUDA_TRY(d_doubled.alloc(*dc, (size_t)total2 * sizeof(float), stream));
-    float* result = out;
-    if (!out_dev) {
-      CUDA_TRY(d_result.alloc(*dc, (size_t)total * sizeof(float), stream));
-      result = d_result.get<float>();
-    }
-
-    const int threads = 256;
-    const int blocks = (int)std::min<int64_t>((total + threads - 1) / threads, (int64_t)dc->sm_count * 32);
-    const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
-    uint8_t* cells = d_cells.get<uint8_t>();
-    rc = with_label_width(label_bytes, [&](auto b) {
-      voxel_graph_expand_kernel<b><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float);
-      CUDA_TRY(cudaGetLastError());
-      return 0;
-    });
-    if (rc) return rc;
-    // half the anisotropy (vg:102-107, 199-204); the sqrt is taken by the gather instead
-    rc = run_passes(cells, 1, ndim, sx2, sy2, sz2, wx / 2, wy / 2, wz / 2, border, 0, d_doubled.get<float>(), *dc,
-                    stream);
-    if (rc) return rc;
-    voxel_graph_gather_kernel<<<blocks, threads, 0, stream>>>(d_doubled.get<const float>(), result, sx, sy, sz,
-                                                              (flags & EDTB200_SQRT) ? 1 : 0);
+  const int threads = 256;
+  const int blocks = (int)std::min<int64_t>((total + threads - 1) / threads, (int64_t)dc->sm_count * 32);
+  const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
+  uint8_t* cells = d_cells.get<uint8_t>();
+  rc = with_label_width(label_bytes, [&](auto b) {
+    voxel_graph_expand_kernel<b><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float);
     CUDA_TRY(cudaGetLastError());
-    if (!out_dev) {
-      rc = download(out, result, (size_t)total * sizeof(float), device, stream);
-      if (rc) return rc;
-    }
-  }                                                  // the scratch frees are queued before the wait
-  if (!(in_dev && out_dev)) CUDA_TRY(cudaStreamSynchronize(stream));
-  return 0;
+    return 0;
+  });
+  if (rc) return rc;
+  // half the anisotropy (vg:102-107, 199-204); the sqrt is taken by the gather instead
+  rc = run_passes(cells, 1, ndim, sx2, sy2, sz2, wx / 2, wy / 2, wz / 2, border, 0, d_doubled.get<float>(), *dc,
+                  stream);
+  if (rc) return rc;
+  voxel_graph_gather_kernel<<<blocks, threads, 0, stream>>>(d_doubled.get<const float>(), result, sx, sy, sz,
+                                                            (flags & EDTB200_SQRT) ? 1 : 0);
+  CUDA_TRY(cudaGetLastError());
+  return io.finish();
 }
 
 int edtb200_pass_first(const void* labels_dev, int label_bytes, int64_t sx, int64_t sy, int64_t sz,
@@ -1240,7 +1213,7 @@ int edtb200_transform_multi(const void* labels, int label_bytes, int ndim, int64
       host_call = std::unique_lock<std::mutex>(dc->host_call);
       for (int o = 0; o < G; ++o)                                 // direct NVLink copies where possible
         if (o != d) { cudaDeviceEnablePeerAccess(parts[o].device, 0); cudaGetLastError(); }
-      if (!dc->stream) MULTI_TRY(cudaStreamCreateWithFlags(&dc->stream, cudaStreamNonBlocking));
+      MULTI_TRY(private_stream(*dc));
       me.stream = dc->stream;
       MULTI_TRY(cudaEventCreateWithFlags(&me.after_y, cudaEventDisableTiming));
       MULTI_TRY(cudaEventCreateWithFlags(&me.after_z, cudaEventDisableTiming));

@@ -48,6 +48,12 @@ extern "C" {
                                        IEEE floats and foreground means value > 0, as the reference's
                                        float instantiations test it (src/edt_voxel_graph.hpp:76, 151) */
 
+/* Residency, shared by edtb200_transform, edtb200_feature_transform and
+ * edtb200_transform_voxel_graph: without EDTB200_LABELS_ON_DEVICE / EDTB200_OUT_ON_DEVICE the
+ * inputs / outputs are host memory (pageable or pinned).  `stream` is a cudaStream_t (as void*) or
+ * NULL.  A call with both flags is asynchronous on `stream`; a call that touches host memory
+ * returns after its results have landed. */
+
 /* error codes */
 #define EDTB200_EINVAL  (-1)   /* bad argument */
 #define EDTB200_ECUDA   (-2)   /* CUDA runtime / driver error, or no device */
@@ -75,9 +81,7 @@ int edtb200_device_count(void);
  *   black_border non-zero: the volume faces count as background
  *   out          sx*sy*sz float32
  *   device       CUDA device ordinal
- *   stream       cudaStream_t (as void*) or NULL.  Device-resident calls (both *_ON_DEVICE
- *                flags) are asynchronous on `stream`; calls touching host memory return
- *                after the result has landed in `out`.
+ *   stream       see Residency above
  */
 int edtb200_transform(const void *labels, int label_bytes, int ndim,
                       int64_t sx, int64_t sy, int64_t sz,
@@ -108,9 +112,8 @@ int edtb200_transform(const void *labels, int label_bytes, int ndim,
  *   dist_out  NULL, or sx*sy*sz float32 distances: EDTB200_SQRT / EDTB200_SIGNED as for
  *             edtb200_transform, equal to its result bit for bit
  *   flags     EDTB200_SIGNED, EDTB200_SQRT, EDTB200_LABELS_ON_DEVICE, and EDTB200_OUT_ON_DEVICE,
- *             which covers dist_out and every index plane
- * Device-resident calls are asynchronous on `stream`; calls touching host memory return after
- * the results have landed.  Every pass runs the one-thread-per-line kernels (no tile kernel).
+ *             which covers dist_out and every index plane (Residency above)
+ * Every pass runs the one-thread-per-line kernels (no tile kernel).
  * Device memory of one call, for V voxels: the labels (V * label_bytes, when uploaded), the
  * distances (4V), one scratch volume for the passes' ping-pong (4V, ndim >= 2), the long-line
  * kernel's hull (4V, ndim >= 2), ndim code planes (4V each) and ndim index planes (4V each, when
@@ -162,7 +165,8 @@ int edtb200_transform_batch(const void *const *labels, float *const *outs, int c
  * Labels only say foreground (non-zero; > 0 with EDTB200_LABELS_FLOAT) or background here, as in
  * the reference.  The foreground is drawn on a doubled grid in which a forbidden edge is a
  * background cell, transformed with half the anisotropy, and sampled back; all of it on the device
- * (scratch: 1 + 4 bytes per doubled cell).  EDTB200_LABELS_ON_DEVICE covers `labels` AND `graph`.
+ * (scratch: 1 + 4 bytes per doubled cell).  Residency as above; EDTB200_LABELS_ON_DEVICE covers
+ * `labels` AND `graph`.
  * EDTB200_SIGNED is rejected: the reference's sdf with a graph is the difference of two such
  * transforms (src/edt.pyx:147-158), which the caller forms.
  */

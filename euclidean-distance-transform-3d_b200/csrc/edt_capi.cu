@@ -122,16 +122,23 @@ cudaError_t scratch_alloc(DeviceCache& dc, void** p, size_t bytes, cudaStream_t 
 // streams wait on the build event, so no host synchronisation and no per-call allocation.
 // When all slots are taken the least recently used table is retired: the retiring stream waits
 // for the last kernel of every stream that used the table (one event per user stream) and the
-// buffer is freed in stream order -- no device-wide synchronisation.
+// buffer is freed in stream order -- no device-wide synchronisation.  The table returned stays
+// pinned until step_table_used: another thread's launch that needs a new table must not retire it
+// while the kernel that reads it is not queued yet (its use is not recorded), so pinned tables are
+// never victims -- when every slot is pinned, the caller waits for one to be released.
 int step_table(DeviceCache& dc, float w, int count, cudaStream_t stream, const float** out) {
-  std::lock_guard<std::mutex> guard(dc.lock);
+  std::unique_lock<std::mutex> guard(dc.lock);
   uint32_t wbits;
   memcpy(&wbits, &w, sizeof(wbits));
   DeviceCache::Table* hit = nullptr;
-  DeviceCache::Table* victim = &dc.tables[0];
-  for (auto& t : dc.tables) {
-    if (t.data && t.wbits == wbits && t.count >= count) { hit = &t; break; }
-    if (t.stamp < victim->stamp) victim = &t;
+  DeviceCache::Table* victim = nullptr;
+  for (;;) {
+    for (auto& t : dc.tables) {
+      if (t.data && t.wbits == wbits && t.count >= count) { hit = &t; break; }
+      if (!t.pinned && (!victim || t.stamp < victim->stamp)) victim = &t;
+    }
+    if (hit || victim) break;
+    dc.table_unpinned.wait(guard);
   }
   if (!hit) {
     DeviceCache::Table& t = *victim;
@@ -157,15 +164,19 @@ int step_table(DeviceCache& dc, float w, int count, cudaStream_t stream, const f
     CUDA_TRY(cudaStreamWaitEvent(stream, hit->ready, 0));
   }
   hit->stamp = ++dc.table_clock;
+  ++hit->pinned;
   *out = hit->data;
   return 0;
 }
 
-// Called after the kernel that reads table `data` has been queued on `stream`.
-int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream) {
+// Called once the kernel that reads table `data` has been queued on `stream` (queued), or when its
+// launch failed (nothing to record).  A pinned table is never retired, so `data` still names it.
+int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream, bool queued) {
   std::lock_guard<std::mutex> guard(dc.lock);
   for (auto& t : dc.tables) {
     if (t.data != data) continue;
+    if (--t.pinned == 0) dc.table_unpinned.notify_all();
+    if (!queued) return 0;
     int slot = -1;
     for (int u = 0; u < DeviceCache::Table::kUsers; ++u)
       if (t.user_set[u] && t.user[u] == stream) { slot = u; break; }
@@ -179,6 +190,25 @@ int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream) {
     return 0;
   }
   return 0;
+}
+
+// The last CTA of an X launch is the one that draws ticket gridDim.x - 1, and it resets the counter
+// and the ticket: two launches that shared them at the same time (device-resident calls on two
+// streams take no lock) would leave the ticket off by the other grid's CTAs for good, and grids
+// smaller than that offset would never publish again.  So every launch takes the next pair of a
+// ring; a pair comes round again only after kStatSlots more launches, and its previous launch has
+// left it at zero by then unless that many X passes run at once.
+RunStat run_stat(DeviceCache& dc, unsigned long long voxels) {
+  RunStat st;
+  memset(&st, 0, sizeof(st));
+  std::lock_guard<std::mutex> guard(dc.lock);
+  if (!dc.stat_slots) return st;
+  char* slot = static_cast<char*>(dc.stat_slots) + 16 * (size_t)(dc.stat_next++ % DeviceCache::kStatSlots);
+  st.counter = reinterpret_cast<unsigned long long*>(slot);
+  st.ticket = reinterpret_cast<unsigned int*>(slot + 8);
+  st.publish = dc.stat_publish_dev;
+  st.voxels = voxels;
+  return st;
 }
 
 }  // namespace host
@@ -453,16 +483,17 @@ int probe(int device, DeviceCache** out) {
       dc.pool = nullptr;                 // fall back to the default pool, settings untouched
     }
     cudaGetLastError();
-    // run statistic of the first-axis pass: two device counters and two mapped host words
+    // run statistic of the first-axis pass: a ring of device counter / ticket pairs and two mapped
+    // host words
     void* stat = nullptr;
     void* host = nullptr;
-    if (cudaMalloc(&stat, 64) == cudaSuccess && cudaMemset(stat, 0, 64) == cudaSuccess &&
+    const size_t stat_bytes = 16 * (size_t)DeviceCache::kStatSlots;
+    if (cudaMalloc(&stat, stat_bytes) == cudaSuccess && cudaMemset(stat, 0, stat_bytes) == cudaSuccess &&
         cudaHostAlloc(&host, 64, cudaHostAllocMapped | cudaHostAllocPortable) == cudaSuccess) {
       memset(host, 0, 64);
       void* host_dev = nullptr;
       if (cudaHostGetDevicePointer(&host_dev, host, 0) == cudaSuccess) {
-        dc.stat_counter = static_cast<unsigned long long*>(stat);
-        dc.stat_ticket = reinterpret_cast<unsigned int*>(static_cast<char*>(stat) + 16);
+        dc.stat_slots = stat;
         dc.stat_publish_host = static_cast<volatile unsigned long long*>(host);
         dc.stat_publish_dev = static_cast<unsigned long long*>(host_dev);
       }

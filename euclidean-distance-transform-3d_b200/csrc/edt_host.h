@@ -8,6 +8,7 @@
 #include "../../include/edt_b200.h"
 #include "edt_kernels.cuh"
 
+#include <condition_variable>
 #include <cstdint>
 #include <mutex>
 #include <type_traits>
@@ -68,7 +69,9 @@ struct DeviceCache {
   cudaEvent_t ev_up[2] = {nullptr, nullptr}, ev_comp[2] = {nullptr, nullptr}, ev_down[2] = {nullptr, nullptr};
   // step tables T[k] of the first-axis pass, keyed by the weight's bits (see step_table_kernel).
   // A table remembers the streams that used it (one event each) so that it can be retired
-  // without a device-wide synchronisation when the cache is full.
+  // without a device-wide synchronisation when the cache is full.  `pinned` counts the launches
+  // that hold the table between step_table and step_table_used -- their use is not recorded yet,
+  // so the table must not be retired then.
   struct Table {
     float* data = nullptr; int count = 0; uint32_t wbits = 0; uint64_t stamp = 0;
     cudaEvent_t ready = nullptr; cudaStream_t built_on = nullptr;
@@ -77,14 +80,19 @@ struct DeviceCache {
     cudaEvent_t used[kUsers] = {nullptr, nullptr, nullptr, nullptr};
     bool user_set[kUsers] = {false, false, false, false};
     bool many_users = false;
+    int pinned = 0;
   };
   static constexpr int kTables = 16;
   Table tables[kTables];
   uint64_t table_clock = 0;
+  std::condition_variable table_unpinned;   // with `lock`: a pinned table was released
   cudaMemPool_t pool = nullptr;        // private pool of the stream-ordered scratch allocations
-  // run statistic of the first-axis pass (see RunStat): device counters + a mapped host word pair
-  unsigned long long* stat_counter = nullptr;
-  unsigned int* stat_ticket = nullptr;
+  // run statistic of the first-axis pass (see RunStat): a ring of device counter / ticket pairs,
+  // one per X launch (run_stat), so that X passes running at the same time on different streams
+  // count and publish apart; and a mapped host word pair that every launch publishes to
+  static constexpr int kStatSlots = 64;
+  void* stat_slots = nullptr;          // kStatSlots x 16 bytes: counter (8), ticket (4), padding
+  unsigned stat_next = 0;
   volatile unsigned long long* stat_publish_host = nullptr;
   unsigned long long* stat_publish_dev = nullptr;
   int sm_count = 0;
@@ -117,11 +125,37 @@ class Scratch {
   cudaStream_t stream_ = nullptr;
 };
 
-// Device table T[0..count) for weight w, cached per device.
+// Device table T[0..count) for weight w, cached per device; pinned until step_table_used.
 int step_table(DeviceCache& dc, float w, int count, cudaStream_t stream, const float** out);
-// To be called once the kernel reading table `data` is queued on `stream` (lets the table be
-// retired later without a device-wide synchronisation).
-int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream);
+// Unpins table `data`.  queued: the kernel reading it is queued on `stream` (recorded, so that the
+// table can be retired later without a device-wide synchronisation); false: the launch failed.
+int step_table_used(DeviceCache& dc, const float* data, cudaStream_t stream, bool queued);
+
+// The step table of one launch: pinned from get() until queued() says the kernel reading it is on
+// the stream, or until it goes out of scope on an early return.
+class StepTable {
+ public:
+  StepTable(DeviceCache& dc, cudaStream_t stream) : dc_(dc), stream_(stream) {}
+  StepTable(const StepTable&) = delete;
+  StepTable& operator=(const StepTable&) = delete;
+  ~StepTable() { if (data_) step_table_used(dc_, data_, stream_, false); }
+  int get(float w, int count) { return step_table(dc_, w, count, stream_, &data_); }
+  const float* data() const { return data_; }
+  int queued() {
+    const float* d = data_;
+    data_ = nullptr;
+    return step_table_used(dc_, d, stream_, true);
+  }
+
+ private:
+  DeviceCache& dc_;
+  cudaStream_t stream_;
+  const float* data_ = nullptr;
+};
+
+// The run statistic of one first-axis launch over `voxels` voxels: the next counter / ticket pair
+// of the device's ring (no counters: the launch publishes nothing).
+RunStat run_stat(DeviceCache& dc, unsigned long long voxels);
 
 // Arithmetic of one later-axis pass.  int_hull: every sample is an integer and every
 // g = f + w2 v^2 an exact 32-bit integer (the integer hull tests apply).  exact: every candidate

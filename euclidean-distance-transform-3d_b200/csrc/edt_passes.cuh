@@ -44,12 +44,11 @@ int launch_first_generic(const void* labels, float* f, int* codes, int64_t nline
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
                  DeviceCache& dc, cudaStream_t stream) {
-  const float* table = nullptr;
-  int trc = step_table(dc, w, (int)sx + 1, stream, &table);
+  StepTable step(dc, stream);
+  int trc = step.get(w, (int)sx + 1);
   if (trc) return trc;
-  RunStat stat;
-  stat.counter = dc.stat_counter; stat.ticket = dc.stat_ticket; stat.publish = dc.stat_publish_dev;
-  stat.voxels = (unsigned long long)nlines * (unsigned long long)sx;
+  const float* table = step.data();
+  const RunStat stat = run_stat(dc, (unsigned long long)nlines * (unsigned long long)sx);
 
   using LT = typename LabelOf<Bytes>::type;
   // register-resident vector kernel when rows are short and 16-byte aligned
@@ -76,11 +75,11 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
     else                EDT_LAUNCH_VEC(8);
 #undef EDT_LAUNCH_VEC
     CUDA_TRY(cudaGetLastError());
-    return step_table_used(dc, table, stream);
+    return step.queued();
   }
   const int rc = launch_first_generic<Bytes, false>(labels, f, nullptr, nlines, sx, table, border, flags, stat, dc,
                                                     stream);
-  return rc ? rc : step_table_used(dc, table, stream);
+  return rc ? rc : step.queued();
 }
 
 // The site-tracking X pass (feature transform): the generic kernel, which also writes the site
@@ -88,14 +87,14 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
 template <int Bytes>
 int launch_first_sites(const void* labels, float* f, int* codes, int64_t nlines, int64_t sx, float w, int border,
                        int flags, DeviceCache& dc, cudaStream_t stream) {
-  const float* table = nullptr;
-  int trc = step_table(dc, w, (int)sx + 1, stream, &table);
+  StepTable step(dc, stream);
+  int trc = step.get(w, (int)sx + 1);
   if (trc) return trc;
   RunStat none;
   memset(&none, 0, sizeof(none));
-  const int rc = launch_first_generic<Bytes, true>(labels, f, codes, nlines, sx, table, border, flags, none, dc,
-                                                   stream);
-  return rc ? rc : step_table_used(dc, table, stream);
+  const int rc = launch_first_generic<Bytes, true>(labels, f, codes, nlines, sx, step.data(), border, flags, none,
+                                                   dc, stream);
+  return rc ? rc : step.queued();
 }
 
 // Did the first-axis pass of the PREVIOUS transform on this device see label noise (at least nine

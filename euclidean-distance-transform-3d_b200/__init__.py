@@ -46,8 +46,16 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
 
+ENOMEM = -3               # EDTB200_ENOMEM
+
+
 class EDTError(RuntimeError):
-  """A C-ABI call failed (CUDA error, no device, unsupported size...)."""
+  """A C-ABI call failed (CUDA error, no device, unsupported size...).  `code` is the call's
+  EDTB200_E* return code (None where the error did not come from one)."""
+
+  def __init__(self, message, code=None):
+    super().__init__(message)
+    self.code = code
 
 
 def library_path():
@@ -74,6 +82,9 @@ def _lib():
   lib.edtb200_device_count.restype = ci
   lib.edtb200_transform.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp]
   lib.edtb200_transform.restype = ci
+  lib.edtb200_transform_chunked.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci,
+                                            ctypes.c_size_t, vp]
+  lib.edtb200_transform_chunked.restype = ci
   lib.edtb200_feature_transform.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
   lib.edtb200_feature_transform.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
@@ -119,7 +130,7 @@ def _lib():
 def _check(rc):
   if rc != 0:
     msg = _lib().edtb200_last_error()
-    raise EDTError("edt_b200 error %d: %s" % (rc, msg.decode("utf-8", "replace") if msg else "?"))
+    raise EDTError("edt_b200 error %d: %s" % (rc, msg.decode("utf-8", "replace") if msg else "?"), rc)
 
 
 def device_count():
@@ -257,7 +268,10 @@ def _result_buffer(count):
   return np.frombuffer(block, dtype=np.float32, count=count)
 
 
-def _transform_host(data, anisotropy, black_border, flags, device):
+def _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes=None):
+  """`max_device_bytes` (an int) streams the volume through one GPU in chunks within that budget
+  (edtb200_transform_chunked).  With None, a 2-D / 3-D volume whose one-shot transform runs out of
+  device memory is retried once that way, with the budget the device has free."""
   nd = data.ndim
   order = "F" if data.flags.f_contiguous else "C"
   if not data.flags.c_contiguous and not data.flags.f_contiguous:
@@ -277,9 +291,17 @@ def _transform_host(data, anisotropy, black_border, flags, device):
       labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz,
       int(bool(black_border)), int(flags), out.ctypes.data, arr, len(devs)))
     return out.reshape(data.shape, order=order)
-  _check(lib.edtb200_transform(
-    labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz,
-    int(bool(black_border)), int(flags), out.ctypes.data, int(device), None))
+  args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), int(flags),
+          out.ctypes.data, int(device))
+  if max_device_bytes is None:
+    try:
+      _check(lib.edtb200_transform(*args, None))
+      return out.reshape(data.shape, order=order)
+    except EDTError as e:
+      if e.code != ENOMEM or nd not in (2, 3):
+        raise
+    max_device_bytes = 0                    # too large for the device: stream it through in chunks
+  _check(lib.edtb200_transform_chunked(*args, int(max_device_bytes), None))
   return out.reshape(data.shape, order=order)
 
 
@@ -398,10 +420,26 @@ def _front_door_device(t, anisotropy, black_border, voxel_graph, flags, fixed_di
   return out.permute(*reversed(range(dims))) if fortran else out
 
 
-def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None):
+def _chunk_budget(max_device_bytes, on_device, voxel_graph, dims):
+  """max_device_bytes as an int, after rejecting what the chunked transform does not cover."""
+  if on_device:
+    raise ValueError("max_device_bytes streams a host array through the GPU; a device-resident array already fits")
+  if voxel_graph is not None:
+    raise ValueError("max_device_bytes cannot be combined with voxel_graph")
+  if dims not in (2, 3):
+    raise ValueError("max_device_bytes needs a 2-D or 3-D array, got %d-D" % dims)
+  budget = int(max_device_bytes)
+  if budget < 0:
+    raise ValueError("max_device_bytes must be non-negative (0: what the device has free)")
+  return budget
+
+
+def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None, max_device_bytes=None):
   """Argument handling of edtsq(), src/edt.pyx:276-310."""
   on_device = _device_array(data)
   if on_device is not None:
+    if max_device_bytes is not None:
+      _chunk_budget(max_device_bytes, True, voxel_graph, on_device.dim())
     return _front_door_device(on_device, anisotropy, black_border, voxel_graph, flags, fixed_dims)
   if isinstance(data, list):
     data = np.array(data)
@@ -409,6 +447,8 @@ def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixe
   dims = data.ndim
   if fixed_dims is not None and dims != fixed_dims:
     raise ValueError("expected a %d-D array, got %d-D" % (fixed_dims, dims))
+  if max_device_bytes is not None:
+    max_device_bytes = _chunk_budget(max_device_bytes, False, voxel_graph, dims)
   if data.size == 0:
     return np.zeros(shape=data.shape, dtype=np.float32)
   if voxel_graph is not None:
@@ -433,46 +473,58 @@ def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixe
     anisotropy = nvl(anisotropy, (1.0, 1.0, 1.0))
   else:
     raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
-  return _transform_host(data, anisotropy, black_border, flags, device)
+  return _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes)
 
 
 # ---------------------------------------------------------------------------------------
 # public API (signatures follow src/edt.pyx; `device` is keyword-only and additive)
 # ---------------------------------------------------------------------------------------
 
-def _pick(device, devices):
+def _pick(device, devices, max_device_bytes=None):
   """`devices` (a sequence of GPU ordinals: one host volume spread over them) wins over `device`."""
   if devices is None:
     return device
+  if max_device_bytes is not None:
+    raise ValueError("max_device_bytes streams through one GPU; it cannot be combined with devices=[...]")
   devs = [int(d) for d in devices]
   if not devs:
     raise ValueError("devices must name at least one GPU")
   return devs if len(devs) > 1 else devs[0]
 
 
+# `max_device_bytes=N` (every function below but the 1-D ones) streams a 2-D / 3-D host array
+# through one GPU in chunks that fit N bytes of device memory (0: what the GPU has free), with the
+# result of the one-shot transform bit for bit; with None a one-shot transform that runs out of
+# device memory falls back to that once (see _transform_host).
+
 def edtsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-          *, device=0, devices=None):
+          *, device=0, devices=None, max_device_bytes=None):
   """Squared anisotropic multi-label EDT of a 1-D, 2-D or 3-D array (src/edt.pyx:245-310).
   `devices=[0, 1, ...]` spreads one host volume over several GPUs (see _transform_host)."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, 0, _pick(device, devices))
+  return _front_door(data, anisotropy, black_border, voxel_graph, 0, _pick(device, devices, max_device_bytes),
+                     max_device_bytes=max_device_bytes)
 
 
 def edt(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-        *, device=0, devices=None):
+        *, device=0, devices=None, max_device_bytes=None):
   """Anisotropic multi-label EDT (src/edt.pyx:205-242); the sqrt is fused into the last pass."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, _pick(device, devices))
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, _pick(device, devices, max_device_bytes),
+                     max_device_bytes=max_device_bytes)
 
 
 def sdf(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-        *, device=0, devices=None):
+        *, device=0, devices=None, max_device_bytes=None):
   """Signed distance function, edt(data) - edt(data == 0) (src/edt.pyx:121-158), computed as
   one transform with background as a label and the sign applied in the last store."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT | FLAG_SIGNED, _pick(device, devices))
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT | FLAG_SIGNED,
+                     _pick(device, devices, max_device_bytes), max_device_bytes=max_device_bytes)
 
 
-def sdfsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, *, device=0, devices=None):
+def sdfsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, *, device=0, devices=None,
+          max_device_bytes=None):
   """Squared signed distance function (src/edt.pyx:161-202)."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SIGNED, _pick(device, devices))
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SIGNED, _pick(device, devices, max_device_bytes),
+                     max_device_bytes=max_device_bytes)
 
 
 def edt1dsq(data, anisotropy=1.0, black_border=False, *, device=0):
@@ -484,23 +536,27 @@ def edt1d(data, anisotropy=1.0, black_border=False, *, device=0):
 
 
 def edt2dsq(data, anisotropy=(1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-            *, device=0):
-  return _front_door(data, anisotropy, black_border, voxel_graph, 0, device, fixed_dims=2)
+            *, device=0, max_device_bytes=None):
+  return _front_door(data, anisotropy, black_border, voxel_graph, 0, device, fixed_dims=2,
+                     max_device_bytes=max_device_bytes)
 
 
 def edt2d(data, anisotropy=(1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-          *, device=0):
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, device, fixed_dims=2)
+          *, device=0, max_device_bytes=None):
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, device, fixed_dims=2,
+                     max_device_bytes=max_device_bytes)
 
 
 def edt3dsq(data, anisotropy=(1.0, 1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-            *, device=0):
-  return _front_door(data, anisotropy, black_border, voxel_graph, 0, device, fixed_dims=3)
+            *, device=0, max_device_bytes=None):
+  return _front_door(data, anisotropy, black_border, voxel_graph, 0, device, fixed_dims=3,
+                     max_device_bytes=max_device_bytes)
 
 
 def edt3d(data, anisotropy=(1.0, 1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-          *, device=0):
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, device, fixed_dims=3)
+          *, device=0, max_device_bytes=None):
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, device, fixed_dims=3,
+                     max_device_bytes=max_device_bytes)
 
 
 # ---------------------------------------------------------------------------------------

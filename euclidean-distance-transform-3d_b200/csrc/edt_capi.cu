@@ -14,6 +14,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <dlfcn.h>
+#include <algorithm>
+#include <chrono>
 #include <condition_variable>
 #include <functional>
 #include <mutex>
@@ -282,7 +284,31 @@ class CopyPool {
 std::mutex g_init;
 CopyPool* g_pools[2][kMaxDevices] = {};
 
-void parallel_memcpy(void* dst, const void* src, size_t bytes, int dir, int device) {
+// A box of host rows: `rows` rows of `width` bytes, row r at host + r * pitch.  Its device copy is
+// packed (row r at r * width), so byte i of the box is device byte i.  A contiguous buffer is the
+// box of one row.
+struct HostBox {
+  char* host;
+  size_t width, pitch, rows;
+  size_t bytes() const { return width * rows; }
+  bool packed() const { return rows == 1 || pitch == width; }
+};
+
+// Copies box bytes [off, off + n) between the box's host rows and `packed`, which holds box byte off
+// at its start; to_host: packed -> host rows.
+void copy_box_bytes(char* packed, const HostBox& b, size_t off, size_t n, bool to_host) {
+  while (n) {
+    const size_t r = off / b.width, c = off % b.width, len = b.width - c < n ? b.width - c : n;
+    char* h = b.host + r * b.pitch + c;
+    if (to_host) memcpy(h, packed, len);
+    else memcpy(packed, h, len);
+    packed += len; off += len; n -= len;
+  }
+}
+
+// Box bytes [off, off + bytes) between the host rows and the staging buffer `stage`, split over
+// the device's copy pool for direction dir (0: towards the device, gathering; 1: back, scattering).
+void parallel_copy(char* stage, const HostBox& b, size_t off, size_t bytes, int dir, int device) {
   CopyPool*& g_pool = g_pools[dir][device];
   if (!g_pool) {
     std::lock_guard<std::mutex> guard(g_init);
@@ -297,9 +323,8 @@ void parallel_memcpy(void* dst, const void* src, size_t bytes, int dir, int devi
   const int n = g_pool->size();
   const size_t slice = ((bytes + n - 1) / n + 4095) & ~size_t(4095);
   g_pool->run([&](int i) {
-    const size_t off = slice * (size_t)i;
-    if (off < bytes) memcpy(static_cast<char*>(dst) + off, static_cast<const char*>(src) + off,
-                            bytes - off < slice ? bytes - off : slice);
+    const size_t s = slice * (size_t)i;
+    if (s < bytes) copy_box_bytes(stage + s, b, off + s, bytes - s < slice ? bytes - s : slice, dir == 1);
   });
 }
 
@@ -331,12 +356,37 @@ int ensure_stage(int device, int dir) {
   return 0;
 }
 
-// host (pageable or pinned) -> device, stream-ordered; returns after the last chunk is queued
-int upload(void* dst_dev, const void* src_host, size_t bytes, int device, cudaStream_t stream) {
-  if (bytes < (size_t(4) << 20) || host_pointer_is_pinned(src_host)) {
-    CUDA_TRY(cudaMemcpyAsync(dst_dev, src_host, bytes, cudaMemcpyHostToDevice, stream));
+// The box copied directly by the DMA engine: one copy when it is packed, else one 2-D copy, or one
+// copy per row where a row pitch exceeds what cudaMemcpy2DAsync takes.
+int copy_box_direct(char* dev, const HostBox& b, int device, cudaStream_t stream, bool to_host) {
+  const cudaMemcpyKind kind = to_host ? cudaMemcpyDeviceToHost : cudaMemcpyHostToDevice;
+  if (b.packed()) {
+    CUDA_TRY(to_host ? cudaMemcpyAsync(b.host, dev, b.bytes(), kind, stream)
+                     : cudaMemcpyAsync(dev, b.host, b.bytes(), kind, stream));
     return 0;
   }
+  int max_pitch = 0;
+  CUDA_TRY(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, device));
+  if (b.pitch <= (size_t)max_pitch) {
+    CUDA_TRY(to_host ? cudaMemcpy2DAsync(b.host, b.pitch, dev, b.width, b.width, b.rows, kind, stream)
+                     : cudaMemcpy2DAsync(dev, b.width, b.host, b.pitch, b.width, b.rows, kind, stream));
+    return 0;
+  }
+  for (size_t r = 0; r < b.rows; ++r) {
+    char* h = b.host + r * b.pitch;
+    char* d = dev + r * b.width;
+    CUDA_TRY(to_host ? cudaMemcpyAsync(h, d, b.width, kind, stream) : cudaMemcpyAsync(d, h, b.width, kind, stream));
+  }
+  return 0;
+}
+
+// host box (pageable or pinned) -> packed device buffer, stream-ordered; returns after the last
+// chunk is queued.  Pageable rows are gathered into the staging buffers, a row longer than one
+// buffer in several pieces.
+int upload_box(void* dst_dev, const HostBox& box, int device, cudaStream_t stream) {
+  const size_t bytes = box.bytes();
+  char* dst = static_cast<char*>(dst_dev);
+  if (bytes < (size_t(4) << 20) || host_pointer_is_pinned(box.host)) return copy_box_direct(dst, box, device, stream, false);
   int rc = ensure_stage(device, 0);
   if (rc) return rc;
   StageBuffers& sb = g_stage[0][device];
@@ -347,20 +397,20 @@ int upload(void* dst_dev, const void* src_host, size_t bytes, int device, cudaSt
     // the DMA out of this buffer must have finished -- also the one queued by an EARLIER upload:
     // inside a batch the previous volume's copies may still be waiting in the stream
     CUDA_TRY(cudaEventSynchronize(sb.ev[b]));
-    parallel_memcpy(sb.buf[b], static_cast<const char*>(src_host) + off, n, 0, device);
-    CUDA_TRY(cudaMemcpyAsync(static_cast<char*>(dst_dev) + off, sb.buf[b], n, cudaMemcpyHostToDevice, stream));
+    parallel_copy(static_cast<char*>(sb.buf[b]), box, off, n, 0, device);
+    CUDA_TRY(cudaMemcpyAsync(dst + off, sb.buf[b], n, cudaMemcpyHostToDevice, stream));
     CUDA_TRY(cudaEventRecord(sb.ev[b], stream));
     off += n;
   }
   return 0;
 }
 
-// device -> host (pageable or pinned); complete on return for the pageable case
-int download(void* dst_host, const void* src_dev, size_t bytes, int device, cudaStream_t stream) {
-  if (bytes < (size_t(4) << 20) || host_pointer_is_pinned(dst_host)) {
-    CUDA_TRY(cudaMemcpyAsync(dst_host, src_dev, bytes, cudaMemcpyDeviceToHost, stream));
-    return 0;
-  }
+// packed device buffer -> host box (pageable or pinned); complete on return for the pageable case
+int download_box(const HostBox& box, const void* src_dev, int device, cudaStream_t stream) {
+  const size_t bytes = box.bytes();
+  const char* src = static_cast<const char*>(src_dev);
+  if (bytes < (size_t(4) << 20) || host_pointer_is_pinned(box.host))
+    return copy_box_direct(const_cast<char*>(src), box, device, stream, true);
   int rc = ensure_stage(device, 1);
   if (rc) return rc;
   StageBuffers& sb = g_stage[1][device];
@@ -372,17 +422,26 @@ int download(void* dst_host, const void* src_dev, size_t bytes, int device, cuda
     if (off < bytes) {
       b = k % kStages;
       n = bytes - off < kStageBytes ? bytes - off : kStageBytes;
-      CUDA_TRY(cudaMemcpyAsync(sb.buf[b], static_cast<const char*>(src_dev) + off, n, cudaMemcpyDeviceToHost, stream));
+      CUDA_TRY(cudaMemcpyAsync(sb.buf[b], src + off, n, cudaMemcpyDeviceToHost, stream));
       CUDA_TRY(cudaEventRecord(sb.ev[b], stream));
     }
     if (prev_b >= 0) {                                             // drain the chunk queued one step earlier
       CUDA_TRY(cudaEventSynchronize(sb.ev[prev_b]));
-      parallel_memcpy(static_cast<char*>(dst_host) + prev_off, sb.buf[prev_b], prev_n, 1, device);
+      parallel_copy(static_cast<char*>(sb.buf[prev_b]), box, prev_off, prev_n, 1, device);
     }
     prev_b = b; prev_off = off; prev_n = n;
     off += n;
   }
   return 0;
+}
+
+// contiguous host buffers: the box of one row
+int upload(void* dst_dev, const void* src_host, size_t bytes, int device, cudaStream_t stream) {
+  return upload_box(dst_dev, HostBox{static_cast<char*>(const_cast<void*>(src_host)), bytes, bytes, 1}, device, stream);
+}
+
+int download(void* dst_host, const void* src_dev, size_t bytes, int device, cudaStream_t stream) {
+  return download_box(HostBox{static_cast<char*>(dst_host), bytes, bytes, 1}, src_dev, device, stream);
 }
 
 // The device's private non-blocking stream, created on first use by the holder of host_call.
@@ -746,6 +805,111 @@ int run_feature_passes(const void* labels, int label_bytes, int ndim, int64_t sx
   });
 }
 
+// The steps of a two-slot pipeline over `count` items: each gets the item, its slot (k % 2) and the
+// stream to queue on.  `item` names an item in error messages ("volume", "chunk").  upload_writes_results:
+// the upload also fills the buffer the download reads (the passes work in place on uploaded data).
+struct PipelineSteps {
+  const char* item = "item";
+  bool upload_writes_results = false;
+  std::function<int(int k, int slot, cudaStream_t)> upload, passes, download;
+};
+
+// The device's three pipeline streams (uploads, passes = the private stream, downloads) and the
+// events that order the two slots; created on first use by the holder of host_call.
+int pipeline_streams(DeviceCache& dc) {
+  CUDA_TRY(private_stream(dc));
+  if (!dc.stream_up) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_up, cudaStreamNonBlocking));
+  if (!dc.stream_down) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_down, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; ++i) {
+    if (!dc.ev_up[i]) CUDA_TRY(cudaEventCreateWithFlags(&dc.ev_up[i], cudaEventDisableTiming));
+    if (!dc.ev_comp[i]) CUDA_TRY(cudaEventCreateWithFlags(&dc.ev_comp[i], cudaEventDisableTiming));
+    if (!dc.ev_down[i]) CUDA_TRY(cudaEventCreateWithFlags(&dc.ev_down[i], cudaEventDisableTiming));
+  }
+  return 0;
+}
+
+// Runs the steps of items 0..count-1 through two device slots, the caller holding host_call.  Item k
+// uses slot k % 2.  Three streams: uploads (fed by a helper thread, so that pageable buffers can be
+// staged in both directions at once), the passes, downloads (this thread).
+//   upload k    waits for the passes of k-2 (they read the slot's inputs), and with
+//               upload_writes_results for download k-2 as well (it reads what the upload overwrites)
+//   passes k    wait for upload k and for download k-2 (it reads the slot's results)
+//   download k  waits for the passes of k
+// Host-side counters make sure an event has been RECORDED before someone waits on it.  Returns when
+// every download has landed; after a failure, once the helper thread has ended and every stream is
+// idle.
+int run_pipeline(DeviceCache& dc, int device, int count, const PipelineSteps& steps) {
+  int rc = pipeline_streams(dc);
+  if (rc) return rc;
+  std::mutex m;
+  std::condition_variable cv;
+  int uploads_queued = 0, passes_queued = 0, downloads_queued = 0, failed = 0;
+  char upload_error[sizeof(g_error)] = "";
+  std::thread uploader([&] {
+    cudaSetDevice(device);
+    for (int k = 0; k < count; ++k) {
+      const int slot = k & 1;
+      int urc = 0;
+      if (k >= 2) {
+        std::unique_lock<std::mutex> l(m);
+        cv.wait(l, [&] {
+          return (passes_queued >= k - 1 && (!steps.upload_writes_results || downloads_queued >= k - 1)) || failed;
+        });
+        if (failed) return;
+        if (cudaStreamWaitEvent(dc.stream_up, dc.ev_comp[slot], 0) != cudaSuccess) urc = EDTB200_ECUDA;
+        if (!urc && steps.upload_writes_results && cudaStreamWaitEvent(dc.stream_up, dc.ev_down[slot], 0) != cudaSuccess)
+          urc = EDTB200_ECUDA;
+      }
+      if (!urc) urc = steps.upload(k, slot, dc.stream_up);
+      if (!urc && cudaEventRecord(dc.ev_up[slot], dc.stream_up) != cudaSuccess) urc = EDTB200_ECUDA;
+      std::lock_guard<std::mutex> l(m);
+      if (urc) {
+        failed = urc;
+        snprintf(upload_error, sizeof(upload_error), "upload of %s %d failed: %.400s", steps.item, k,
+                 urc == EDTB200_ECUDA ? cudaGetErrorString(cudaGetLastError()) : g_error);
+      } else {
+        uploads_queued = k + 1;
+      }
+      cv.notify_all();
+      if (urc) return;
+    }
+  });
+  auto bail = [&](int code) {
+    { std::lock_guard<std::mutex> l(m); if (!failed) failed = code; }
+    cv.notify_all();
+    uploader.join();
+    cudaStreamSynchronize(dc.stream_up); cudaStreamSynchronize(dc.stream); cudaStreamSynchronize(dc.stream_down);
+    return code;
+  };
+  #define PIPE_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { \
+      fail(EDTB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); return bail(EDTB200_ECUDA); } } while (0)
+  for (int k = 0; k < count; ++k) {
+    const int slot = k & 1;
+    {
+      std::unique_lock<std::mutex> l(m);
+      cv.wait(l, [&] { return uploads_queued >= k + 1 || failed; });
+      if (failed) { l.unlock(); uploader.join(); cudaDeviceSynchronize(); return fail(failed, "%s", upload_error); }
+    }
+    PIPE_TRY(cudaStreamWaitEvent(dc.stream, dc.ev_up[slot], 0));
+    if (k >= 2) PIPE_TRY(cudaStreamWaitEvent(dc.stream, dc.ev_down[slot], 0));
+    rc = steps.passes(k, slot, dc.stream);
+    if (rc) return bail(rc);
+    PIPE_TRY(cudaEventRecord(dc.ev_comp[slot], dc.stream));
+    { std::lock_guard<std::mutex> l(m); passes_queued = k + 1; }
+    cv.notify_all();
+    PIPE_TRY(cudaStreamWaitEvent(dc.stream_down, dc.ev_comp[slot], 0));
+    rc = steps.download(k, slot, dc.stream_down);
+    if (rc) return bail(rc);
+    PIPE_TRY(cudaEventRecord(dc.ev_down[slot], dc.stream_down));
+    { std::lock_guard<std::mutex> l(m); downloads_queued = k + 1; }
+    cv.notify_all();
+  }
+  #undef PIPE_TRY
+  uploader.join();
+  CUDA_TRY(cudaStreamSynchronize(dc.stream_down));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -851,85 +1015,204 @@ int edtb200_transform_batch(const void* const* labels, float* const* outs, int c
     CUDA_TRY(grow(dc.labels2, dc.labels2_bytes, lab_bytes));
     CUDA_TRY(grow(dc.dist2, dc.dist2_bytes, out_bytes));
   }
-  CUDA_TRY(private_stream(dc));
-  if (!dc.stream_up) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_up, cudaStreamNonBlocking));
-  if (!dc.stream_down) CUDA_TRY(cudaStreamCreateWithFlags(&dc.stream_down, cudaStreamNonBlocking));
-  for (int i = 0; i < 2; ++i) {
-    if (!dc.ev_up[i]) CUDA_TRY(cudaEventCreateWithFlags(&dc.ev_up[i], cudaEventDisableTiming));
-    if (!dc.ev_comp[i]) CUDA_TRY(cudaEventCreateWithFlags(&dc.ev_comp[i], cudaEventDisableTiming));
-    if (!dc.ev_down[i]) CUDA_TRY(cudaEventCreateWithFlags(&dc.ev_down[i], cudaEventDisableTiming));
-  }
   void* d_labels[2] = {dc.labels, dc.labels2};
   float* d_dist[2] = {dc.dist, dc.dist2};
   const int border = black_border != 0;
-
-  // Volume k uses slot k % 2.  Three streams: uploads (fed by a helper thread, so that pageable
-  // buffers can be staged in both directions at once), the passes, downloads (this thread).
-  //   upload k    waits for the passes of k-2 (they read the slot's labels)
-  //   passes k    wait for upload k and for download k-2 (it reads the slot's distances)
-  //   download k  waits for the passes of k
-  // Host-side counters make sure an event has been RECORDED before someone waits on it.
-  std::mutex m;
-  std::condition_variable cv;
-  int uploads_queued = 0, passes_queued = 0, failed = 0;
-  char upload_error[sizeof(g_error)] = "";
-  std::thread uploader([&] {
-    cudaSetDevice(device);
-    for (int k = 0; k < count; ++k) {
-      const int slot = k & 1;
-      int urc = 0;
-      if (k >= 2) {
-        std::unique_lock<std::mutex> l(m);
-        cv.wait(l, [&] { return passes_queued >= k - 1 || failed; });
-        if (failed) return;
-        if (cudaStreamWaitEvent(dc.stream_up, dc.ev_comp[slot], 0) != cudaSuccess) urc = EDTB200_ECUDA;
-      }
-      if (!urc) urc = upload(d_labels[slot], labels[k], lab_bytes, device, dc.stream_up);
-      if (!urc && cudaEventRecord(dc.ev_up[slot], dc.stream_up) != cudaSuccess) urc = EDTB200_ECUDA;
-      std::lock_guard<std::mutex> l(m);
-      if (urc) {
-        failed = urc;
-        snprintf(upload_error, sizeof(upload_error), "upload of volume %d failed: %.400s", k,
-                 urc == EDTB200_ECUDA ? cudaGetErrorString(cudaGetLastError()) : g_error);
-      } else {
-        uploads_queued = k + 1;
-      }
-      cv.notify_all();
-      if (urc) return;
-    }
-  });
-  auto bail = [&](int code) {
-    { std::lock_guard<std::mutex> l(m); if (!failed) failed = code; }
-    cv.notify_all();
-    uploader.join();
-    cudaStreamSynchronize(dc.stream_up); cudaStreamSynchronize(dc.stream); cudaStreamSynchronize(dc.stream_down);
-    return code;
+  PipelineSteps steps;
+  steps.item = "volume";
+  steps.upload = [&](int k, int slot, cudaStream_t s) { return upload(d_labels[slot], labels[k], lab_bytes, device, s); };
+  steps.passes = [&](int, int slot, cudaStream_t s) {
+    return run_passes(d_labels[slot], label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, d_dist[slot], dc, s);
   };
-  #define BATCH_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { \
-      fail(EDTB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); return bail(EDTB200_ECUDA); } } while (0)
-  for (int k = 0; k < count; ++k) {
-    const int slot = k & 1;
-    {
-      std::unique_lock<std::mutex> l(m);
-      cv.wait(l, [&] { return uploads_queued >= k + 1 || failed; });
-      if (failed) { l.unlock(); uploader.join(); cudaDeviceSynchronize(); return fail(failed, "%s", upload_error); }
-    }
-    BATCH_TRY(cudaStreamWaitEvent(dc.stream, dc.ev_up[slot], 0));
-    if (k >= 2) BATCH_TRY(cudaStreamWaitEvent(dc.stream, dc.ev_down[slot], 0));
-    rc = run_passes(d_labels[slot], label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, d_dist[slot], dc,
-                    dc.stream);
-    if (rc) return bail(rc);
-    BATCH_TRY(cudaEventRecord(dc.ev_comp[slot], dc.stream));
-    { std::lock_guard<std::mutex> l(m); passes_queued = k + 1; }
-    cv.notify_all();
-    BATCH_TRY(cudaStreamWaitEvent(dc.stream_down, dc.ev_comp[slot], 0));
-    rc = download(outs[k], d_dist[slot], out_bytes, device, dc.stream_down);
-    if (rc) return bail(rc);
-    BATCH_TRY(cudaEventRecord(dc.ev_down[slot], dc.stream_down));
+  steps.download = [&](int k, int slot, cudaStream_t s) { return download(outs[k], d_dist[slot], out_bytes, device, s); };
+  return run_pipeline(dc, device, count, steps);
+}
+
+}  // extern "C"
+
+// ---- one host volume larger than the device, streamed through it in chunks -------------------
+namespace {
+
+// One phase of edtb200_transform_chunked (the plan of include/edt_b200.h): `extent` slices of
+// `slice_bytes` device bytes each, in `count` chunks of at most `most` slices (count 0: the budget
+// is below `need`, the least that works).
+struct PhasePlan {
+  int64_t extent = 0, count = 0, most = 0;
+  size_t slice_bytes = 0, need = 0;
+  int64_t start(int64_t k) const { return extent * k / count; }        // chunk sizes differ by one at most
+  int64_t size(int64_t k) const { return start(k + 1) - start(k); }
+};
+
+// extent slices of slice_vox voxels; a chunk holds at most `cap` slices; `long_line`: the phase's
+// later pass takes the long-line kernel (8 more bytes per voxel of scratch).
+PhasePlan plan_phase(int64_t extent, int64_t slice_vox, int label_bytes, int64_t cap, bool long_line, size_t budget) {
+  PhasePlan p;
+  p.extent = extent;
+  p.slice_bytes = (size_t)slice_vox * (size_t)(label_bytes + 4 + (long_line ? 8 : 0));
+  p.need = (size_t)(extent < 2 ? extent : 2) * p.slice_bytes;
+  if (extent <= cap && (size_t)extent <= budget / p.slice_bytes) {
+    p.count = 1;
+  } else {
+    const int64_t c = std::min<int64_t>(cap, (int64_t)(budget / (2 * p.slice_bytes)));
+    if (c == 0) return p;
+    p.count = (extent + c - 1) / c;
   }
-  #undef BATCH_TRY
-  uploader.join();
-  CUDA_TRY(cudaStreamSynchronize(dc.stream_down));
+  p.most = (extent + p.count - 1) / p.count;
+  return p;
+}
+
+// Frees this device's cached whole-volume buffers and trims its private pool (the caller holds
+// host_call), so that a chunked call after a one-shot call that ran out of memory finds it free.
+void drop_volume_buffers(DeviceCache& dc) {
+  void* bufs[] = {dc.labels, dc.dist, dc.labels2, dc.dist2};
+  for (void* b : bufs) if (b) cudaFree(b);
+  dc.labels = dc.labels2 = nullptr; dc.dist = dc.dist2 = nullptr;
+  dc.labels_bytes = dc.labels2_bytes = dc.dist_bytes = dc.dist2_bytes = 0;
+  if (dc.pool) cudaMemPoolTrimTo(dc.pool, 0);
+  cudaGetLastError();
+}
+
+// The slots of one phase: labels, then distances, in one scratch allocation each.
+struct ChunkSlots {
+  Scratch buf[2];
+  void* labels[2] = {nullptr, nullptr};
+  float* dist[2] = {nullptr, nullptr};
+  int take(DeviceCache& dc, const PhasePlan& p, int64_t slice_vox, int label_bytes) {
+    const size_t vox = (size_t)p.most * (size_t)slice_vox;
+    const size_t lab = (vox * (size_t)label_bytes + 255) & ~size_t(255);
+    for (int i = 0; i < (p.count > 1 ? 2 : 1); ++i) {
+      if (buf[i].alloc(dc, lab + vox * sizeof(float), dc.stream) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(EDTB200_ENOMEM, "no device memory for a chunk slot of %zu bytes: give a smaller device_bytes",
+                    lab + vox * sizeof(float));
+      }
+      labels[i] = buf[i].get();
+      dist[i] = reinterpret_cast<float*>(buf[i].get<char>() + lab);
+    }
+    CUDA_TRY(cudaStreamSynchronize(dc.stream));   // allocated on the passes' stream, used on all three
+    return 0;
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                              float wx, float wy, float wz, int black_border, int flags, float* out,
+                              int device, size_t device_bytes, int64_t* chunks) {
+  if (chunks) chunks[0] = chunks[1] = 0;
+  if (flags & (EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_transform_chunked streams HOST buffers through the device; a volume on "
+                                "the device fits it: use edtb200_transform");
+  if (ndim != 2 && ndim != 3)
+    return fail(EDTB200_EINVAL, "edtb200_transform_chunked needs a 2-D or 3-D volume (got ndim %d)", ndim);
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  const int64_t total = sx * sy * sz;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
+  const char* lab_host = static_cast<const char*>(labels);
+  char* out_host = reinterpret_cast<char*>(out);
+  if (lab_host < out_host + out_bytes && out_host < lab_host + lab_bytes)
+    return fail(EDTB200_EINVAL, "labels and out overlap");
+
+  DeviceGuard restore_device;
+  DeviceCache* dcp = nullptr;
+  if ((rc = probe(device, &dcp))) return rc;
+  DeviceCache& dc = *dcp;
+  std::lock_guard<std::mutex> host_call(dc.host_call);
+  drop_volume_buffers(dc);
+  size_t budget = device_bytes;
+  if (budget == 0) {
+    size_t free_bytes = 0, total_bytes = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
+    budget = free_bytes > EDTB200_CHUNK_RESERVE ? free_bytes - EDTB200_CHUNK_RESERVE : 0;
+  }
+
+  // Phase 1 cuts the last axis (z slabs in 3-D, row ranges in 2-D): X pass, and in 3-D the Y pass.
+  // Phase 2 cuts the axis before it into boxes of whole lines along the last axis: the last pass.
+  const int border = black_border != 0;
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
+  const int last = ndim - 1;
+  const int64_t n_last = t.n[last], n_cut = t.n[last - 1];
+  const int64_t plane = total / n_last;                    // voxels of one phase-1 slice
+  const int64_t unit = ndim == 3 ? sx : 1;                 // voxels of one phase-2 slice per row
+  const int64_t line_vox = unit * n_last;                  // voxels of one phase-2 slice
+  const int64_t cap2 = std::max<int64_t>(1, (int64_t)((((int64_t)1 << 32) - 65) / line_vox));
+  const bool long1 = ndim == 3 && later_pass_is_long(geom_for_axis(1, sx, sy, sz), transform_arith(t.w, t.n, 1),
+                                                     dc.max_smem_optin);
+  const int64_t c2 = std::min(n_cut, cap2);
+  const edtb200::LineGeom g2 = ndim == 3 ? geom_for_axis(2, sx, c2, sz) : geom_for_axis(1, c2, sy, 1);
+  const bool long2 = later_pass_is_long(g2, transform_arith(t.w, t.n, last), dc.max_smem_optin);
+  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes, n_last, long1, budget);
+  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes, cap2, long2, budget);
+  if (p1.count == 0 || p2.count == 0)
+    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked transform needs at "
+                                "least %zu bytes", budget, std::max(p1.need, p2.need));
+  if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
+  if ((rc = pipeline_streams(dc))) return rc;
+
+  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
+  const auto t0 = std::chrono::steady_clock::now();
+  {
+    ChunkSlots slots;
+    if ((rc = slots.take(dc, p1, plane, label_bytes))) return rc;
+    PipelineSteps steps;
+    steps.item = "phase-1 chunk";
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      return upload(slots.labels[slot], lab_host + (size_t)(p1.start(k) * plane) * label_bytes,
+                    (size_t)(p1.size(k) * plane) * label_bytes, device, s);
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      int r = x_pass(t, slots.labels[slot], slots.dist[slot], plane / sx * p1.size(k), dc, s);
+      if (!r && ndim == 3)                                  // behind our own X pass
+        r = later_pass(t, 1, slots.labels[slot], slots.dist[slot], geom_for_axis(1, sx, sy, p1.size(k)), border,
+                       border, dc, s, /*pdl=*/true);
+      return r;
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      return download(out + p1.start(k) * plane, slots.dist[slot], (size_t)(p1.size(k) * plane) * sizeof(float),
+                      device, s);
+    };
+    if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
+  }
+  const auto t1 = std::chrono::steady_clock::now();
+  {
+    ChunkSlots slots;
+    if ((rc = slots.take(dc, p2, line_vox, label_bytes))) return rc;
+    // chunk k: n_last rows of size(k) * unit voxels, one row per index along the last axis
+    auto box = [&](const char* base, int64_t k, int bytes) {
+      return HostBox{const_cast<char*>(base) + (size_t)(p2.start(k) * unit) * bytes,
+                     (size_t)(p2.size(k) * unit) * bytes, (size_t)plane * bytes, (size_t)n_last};
+    };
+    PipelineSteps steps;
+    steps.item = "phase-2 chunk";
+    steps.upload_writes_results = true;            // the intermediate distances go up into the slot
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
+      return r ? r : upload_box(slots.dist[slot], box(out_host, k, sizeof(float)), device, s);
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      const int64_t c = p2.size(k);
+      const edtb200::LineGeom g = ndim == 3 ? geom_for_axis(2, sx, c, sz) : geom_for_axis(1, c, sy, 1);
+      return later_pass(t, last, slots.labels[slot], slots.dist[slot], g, border, border, dc, s, /*pdl=*/false);
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      return download_box(box(out_host, k, sizeof(float)), slots.dist[slot], device, s);
+    };
+    if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
+  }
+  if (verbose) {
+    const auto t2 = std::chrono::steady_clock::now();
+    const double ms1 = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    const double ms2 = std::chrono::duration<double, std::milli>(t2 - t1).count();
+    fprintf(stderr, "[edt_b200] chunked %lldx%lldx%lld L=%d  budget %zu  chunks %lld + %lld  up %.3f GB  down %.3f GB  "
+                    "phase 1 %.1f ms  phase 2 %.1f ms\n",
+            (long long)sx, (long long)sy, (long long)sz, label_bytes, budget, (long long)p1.count, (long long)p2.count,
+            (2.0 * label_bytes + 4.0) * (double)total / 1e9, 8.0 * (double)total / 1e9, ms1, ms2);
+  }
   return 0;
 }
 

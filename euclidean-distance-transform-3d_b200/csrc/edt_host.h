@@ -1,8 +1,9 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as five translation units so that the kernel templates build in
-// parallel: edt_capi.cu (C ABI, staging, caches) and edt_passes_b{1,2,4,8}.cu (the axis-pass
-// launchers of edt_passes.cuh instantiated for one label width each).  The run-time label width
+// The library is compiled as six translation units so that the kernel templates build in
+// parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
+// launchers of edt_passes.cuh instantiated for one label width each) and edt_plan.cu (the
+// later-axis plan for host code that launches nothing).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -188,6 +189,10 @@ template <int Bytes>
 int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim, int64_t sx, int64_t sy,
                          int64_t sz, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
                          cudaStream_t stream);
+
+// Whether plan_later (edt_passes.cuh) sends a later-axis pass over geometry g with arithmetic
+// `arith` to the long-line kernel (edt_plan.cu).
+bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin);
 
 // What a later-axis launch runs (plan_later in edt_passes.cuh); the last one launched on the
 // calling thread is kept for edtb200_last_later_launch.

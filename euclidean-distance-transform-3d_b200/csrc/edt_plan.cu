@@ -1,0 +1,15 @@
+// edt_plan.cu -- the later-axis plan (plan_later, edt_passes.cuh) for host code that only needs to
+// know which kernel a pass would take, not launch it.  It instantiates no launcher: those live in
+// edt_passes_b{1,2,4,8}.cu.
+#include "edt_passes.cuh"
+
+namespace edtb200 {
+namespace host {
+
+bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin) {
+  // tile or long-line does not depend on TMA, the CTA count or the integer hull switch
+  return plan_later(g, false, arith, max_smem_optin, true, false, false).kernel == 1;
+}
+
+}  // namespace host
+}  // namespace edtb200

@@ -40,8 +40,11 @@ inline float* run(T* labels, int ndim, int64_t sx, int64_t sy, int64_t sz, float
     for (int64_t i = 0; i < voxels; ++i) folded[i] = labels[i] + T(0);
     src = folded;
   }
-  const int rc = edtb200_transform(src, (int)sizeof(T), ndim, sx, sy, sz, wx, wy, wz, black_border ? 1 : 0,
-                                   flags, out, /*device=*/0, /*stream=*/nullptr);
+  int rc = edtb200_transform(src, (int)sizeof(T), ndim, sx, sy, sz, wx, wy, wz, black_border ? 1 : 0,
+                             flags, out, /*device=*/0, /*stream=*/nullptr);
+  if (rc == EDTB200_ENOMEM && ndim >= 2)         // larger than the device: stream it through in chunks
+    rc = edtb200_transform_chunked(src, (int)sizeof(T), ndim, sx, sy, sz, wx, wy, wz, black_border ? 1 : 0, flags,
+                                   out, /*device=*/0, /*device_bytes=*/0, /*chunks=*/nullptr);
   if (rc != 0) {
     if (!output) delete[] out;
     throw std::runtime_error(std::string("edt_b200: ") + edtb200_last_error());

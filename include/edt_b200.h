@@ -23,6 +23,7 @@
 #ifndef EDT_B200_H
 #define EDT_B200_H
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -32,7 +33,9 @@ extern "C" {
 /* 100: round 1 (transform, per-axis passes, slab face kernels).  200: additions only --
  * edtb200_transform_multi, edtb200_slab_step / _stage_bytes / _pack, edtb200_label_stats / _extract,
  * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
- * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform. */
+ * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
+ * Entry points added since (edtb200_transform_chunked) keep the number: every 202-level entry point
+ * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up. */
 #define EDTB200_VERSION 202
 
 /* flags */
@@ -152,6 +155,52 @@ int edtb200_transform_multi(const void *labels, int label_bytes, int ndim,
 int edtb200_transform_batch(const void *const *labels, float *const *outs, int count,
                             int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                             float wx, float wy, float wz, int black_border, int flags, int device);
+
+/* The same transform as edtb200_transform for a 2-D or 3-D HOST volume larger than the device's
+ * memory, streamed through one device in chunks; the result is edtb200_transform's bit for bit.
+ *
+ * Two phases, exact for any input, no halo.  The passes along the first axes couple only the
+ * voxels of one slice across the last axis, the last pass only the voxels of one line along it:
+ *   phase 1  chunks of whole slices across the last axis (z slabs in 3-D, row ranges in 2-D): the
+ *            labels go up, the X pass (and in 3-D the Y pass) runs, the distances come down into
+ *            `out`, which holds the intermediate result;
+ *   phase 2  chunks of whole lines along the last axis (y ranges in 3-D, x ranges in 2-D): the
+ *            labels and the intermediate distances go up, the last pass runs with the sqrt / sign
+ *            epilogue, the result comes down into `out`.
+ * Every pass sees whole lines and runs with the whole volume's weights and extents, so it makes the
+ * one-shot transform's arithmetic choices; the only borders are the volume's faces.  Each phase
+ * pipelines its chunks through two device slots as edtb200_transform_batch does.  PCIe traffic is
+ * (2 label_bytes + 4) bytes per voxel up and 8 down, against label_bytes and 4 for edtb200_transform:
+ * this is for volumes that do not fit.
+ *
+ * The plan, per phase, from the budget B:
+ *   slice   one slice (phase 1) or one line-set of the cut axis (phase 2: sx * sz voxels in 3-D, sy
+ *           in 2-D) costs slice = voxels * (label_bytes + 4 + s) bytes, with s = 8 when the phase's
+ *           later pass, over a chunk of the largest size allowed below, takes the long-line kernel
+ *           (its two scratch volumes) and 0 otherwise (2-D phase 1 has no later pass);
+ *   cap     phase-2 chunks hold fewer than 2^32 - 64 voxels, so that the last pass can take the
+ *           tile kernel where the one-shot transform could not;
+ *   chunks  one chunk when the whole extent fits B (and the cap); otherwise two slots with
+ *           c = min(cap, floor(B / (2 slice))) slices per chunk, EDTB200_ENOMEM when c == 0 in
+ *           either phase (the message names the smallest budget that works: the larger of the
+ *           two phases' min(extent, 2) * slice);
+ *   count   ceil(extent / c) chunks whose sizes differ by one at most.
+ *
+ *   labels, out   HOST buffers, pageable or pinned, that must not overlap; the *_ON_DEVICE flags
+ *                 are rejected.  flags: EDTB200_SQRT / EDTB200_SIGNED.  ndim is 2 or 3.
+ *   device_bytes  the device-memory budget B of the call; 0: the memory free on the device, less
+ *                 EDTB200_CHUNK_RESERVE.  Either way the device's cached whole-volume buffers (those
+ *                 edtb200_transform / _batch keep between calls) are freed first and its scratch
+ *                 pool trimmed, so a call that follows a one-shot EDTB200_ENOMEM finds that memory.
+ *   chunks        NULL, or int64_t[2] that receives {phase-1 chunks, phase-2 chunks}.
+ * Returns when the result has landed; after an error the contents of `out` are unspecified.  Nothing
+ * the call allocates on the device outlives it.  Calls on one device are serialised. */
+#define EDTB200_CHUNK_RESERVE 536870912   /* 512 MiB left free under a budget of 0 */
+int edtb200_transform_chunked(const void *labels, int label_bytes, int ndim,
+                              int64_t sx, int64_t sy, int64_t sz,
+                              float wx, float wy, float wz,
+                              int black_border, int flags, float *out,
+                              int device, size_t device_bytes, int64_t *chunks);
 
 /* Transform under a voxel connectivity graph (2-D or 3-D only).
  *

@@ -577,16 +577,17 @@ int check_dims(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz)
 }
 
 int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines, int64_t sx, float w,
-                   int border, int flags, DeviceCache& dc, cudaStream_t s) {
+                   int border, int flags, DeviceCache& dc, cudaStream_t s, const edtb200::XPlanes* planes = nullptr) {
   return with_label_width(label_bytes, [&](auto b) {
-    return launch_first<b>(labels, f, nlines, sx, w, border, flags, dc, s);
+    return launch_first<b>(labels, f, nlines, sx, w, border, flags, planes, dc, s);
   });
 }
 
 int dispatch_later(int label_bytes, const void* labels, float* f, const edtb200::LineGeom& g, float w,
-                   int lo, int hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t s, bool pdl) {
+                   int lo, int hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t s, bool pdl,
+                   const edtb200::RunBits* bits = nullptr) {
   return with_label_width(label_bytes, [&](auto b) {
-    return launch_later<b>(labels, f, g, w, lo, hi, flags, arith, dc, s, pdl);
+    return launch_later<b>(labels, bits, f, g, w, lo, hi, flags, arith, dc, s, pdl);
   });
 }
 
@@ -616,17 +617,64 @@ struct Transform {
   int64_t n[3];
 };
 
-// The X pass over nlines rows.
-int x_pass(const Transform& t, const void* labels, float* f, int64_t nlines, DeviceCache& dc, cudaStream_t s) {
-  return dispatch_first(t.label_bytes, labels, f, nlines, t.n[0], t.w[0], t.border,
-                        kernel_flags(t.flags, true, t.ndim == 1), dc, s);
+edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz);
+
+// The run-start planes that the X pass of one transform writes for its later passes (XPlanes): one
+// bit per voxel and later axis, stream-ordered scratch freed on the stream when the owner goes out
+// of scope.  They pay where the later passes only stream -- label noise (predicted from the previous
+// transform's run statistic, as the later passes' CTA count is) with labels of 4 or 8 bytes: there a
+// later pass moves 4 + 1/8 bytes per voxel instead of 8 or 12, for 1/4 byte more written and two
+// rows re-read from L1 / L2 by the X pass.  On narrower labels and on structured volumes the dearer
+// X pass costs more than the later passes gain (DESIGN.md section 4.1), so none are taken there;
+// nor for signed transforms, whose last pass needs the labels' background bits as well.
+struct RunPlanes {
+  Scratch mem;
+  edtb200::XPlanes x{};             // x.y null: none
+  edtb200::RunBits bits[3] = {};    // the later pass along axis k reads bits[k] (start null: none)
+  const edtb200::XPlanes* for_x() const { return x.y ? &x : nullptr; }
+  const edtb200::RunBits* for_axis(int k) const { return bits[k].start ? &bits[k] : nullptr; }
+};
+
+// Takes the planes for transform t over the volume (t.n[0], sy, sz) at labels / f where they pay;
+// taking none costs nothing (the later passes then read the labels).
+int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const float* f, int64_t sy, int64_t sz,
+                    DeviceCache& dc, cudaStream_t s) {
+  const int64_t sx = t.n[0];
+  if (t.ndim < 2 || t.label_bytes < 4 || (t.flags & EDTB200_SIGNED) || sx > 512 ||
+      !first_is_vec(labels, t.label_bytes, f, sx) || !label_noise_predicted(dc))
+    return 0;
+  bool tile = false;
+  for (int k = 1; k < t.ndim; ++k)
+    tile = tile || !later_pass_is_long(geom_for_axis(k, sx, sy, sz), transform_arith(t.w, t.n, k), dc.max_smem_optin);
+  if (!tile) return 0;
+  const int64_t wpr = (sx + 31) >> 5, words = sy * sz * wpr;
+  if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)words * (size_t)(t.ndim - 1), s) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;                        // no room: the later passes read the labels
+  }
+  uint32_t* p = rp.mem.get<uint32_t>();
+  rp.x.sy = sy;
+  rp.x.y = p;
+  rp.x.z = t.ndim == 3 ? p + words : nullptr;
+  // Y pass: outer = z, inner = x; Z pass: inner = y * sx + x, rows sy * wpr words apart
+  rp.bits[1] = edtb200::RunBits{rp.x.y, wpr, sy * wpr, sx, wpr};
+  if (t.ndim == 3) rp.bits[2] = edtb200::RunBits{rp.x.z, sy * wpr, 0, sx, wpr};
+  return 0;
 }
 
-// The later pass along axis k over geometry g, with the borders lo / hi at the ends of its lines.
+// The X pass over nlines rows; planes: the run-start planes it writes (null: none).
+int x_pass(const Transform& t, const void* labels, float* f, int64_t nlines, DeviceCache& dc, cudaStream_t s,
+           const RunPlanes* planes = nullptr) {
+  return dispatch_first(t.label_bytes, labels, f, nlines, t.n[0], t.w[0], t.border,
+                        kernel_flags(t.flags, true, t.ndim == 1), dc, s, planes ? planes->for_x() : nullptr);
+}
+
+// The later pass along axis k over geometry g, with the borders lo / hi at the ends of its lines;
+// planes: those its X pass wrote over the same volume (null: none).
 int later_pass(const Transform& t, int k, const void* labels, float* f, const edtb200::LineGeom& g, int lo, int hi,
-               DeviceCache& dc, cudaStream_t s, bool pdl) {
+               DeviceCache& dc, cudaStream_t s, bool pdl, const RunPlanes* planes = nullptr) {
   return dispatch_later(t.label_bytes, labels, f, g, t.w[k], lo, hi, kernel_flags(t.flags, false, k == t.ndim - 1),
-                        transform_arith(t.w, t.n, k), dc, s, pdl);
+                        transform_arith(t.w, t.n, k), dc, s, pdl, planes ? planes->for_axis(k) : nullptr);
 }
 
 // Largest finite |f| (as float bits: non-negative floats order like their bits) and the exponent
@@ -724,10 +772,12 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   // in the stream is our own previous pass, which never writes the labels, so their label staging
   // (before griddepcontrol.wait) may overlap its tail.  The per-axis entry points do not do this:
   // there the previous kernel is the caller's and may be the one producing the labels.
-  // (A one-byte neighbour-code plane written by the first pass, so that the later passes need not
-  // re-read wide labels, was tried and dropped: it made the later passes cheaper, but the first
-  // pass dearer by more.)
-  int rc = 0;
+  // On predicted label noise with wide labels the X pass also writes run-start bit planes, and the
+  // later passes read those instead of the labels (RunPlanes); a later pass reads its plane only
+  // after griddepcontrol.wait.
+  RunPlanes planes;
+  int rc = take_run_planes(planes, t, labels, f, sy, sz, dc, stream);
+  if (rc) return rc;
   // EDT_B200_VERBOSE=1: per-pass device times of every transform on stderr (SURVEY.md section 5).
   // The dump needs the passes to have finished, so a verbose transform synchronises its stream.
   static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
@@ -735,18 +785,20 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   if (verbose) g_profile = true;
   mark_pass(0, stream);
   nvtx_push("edt.x");
-  rc = x_pass(t, labels, f, sy * sz, dc, stream);
+  rc = x_pass(t, labels, f, sy * sz, dc, stream, &planes);
   nvtx_pop();
   mark_pass(1, stream);
   if (!rc && ndim >= 2) {
     nvtx_push("edt.y");
-    rc = later_pass(t, 1, labels, f, geom_for_axis(1, sx, sy, sz), border, border, dc, stream, /*pdl=*/true);
+    rc = later_pass(t, 1, labels, f, geom_for_axis(1, sx, sy, sz), border, border, dc, stream, /*pdl=*/true,
+                    &planes);
     nvtx_pop();
     mark_pass(2, stream);
   }
   if (!rc && ndim >= 3) {
     nvtx_push("edt.z");
-    rc = later_pass(t, 2, labels, f, geom_for_axis(2, sx, sy, sz), border, border, dc, stream, /*pdl=*/true);
+    rc = later_pass(t, 2, labels, f, geom_for_axis(2, sx, sy, sz), border, border, dc, stream, /*pdl=*/true,
+                    &planes);
     nvtx_pop();
     mark_pass(3, stream);
   }

@@ -169,13 +169,26 @@ PassArith transform_arith(const float* w, const int64_t* n, int k);
 // lowest set bit over the finite non-zero samples is 2^low (1024: there is none).
 PassArith sampled_arith(float fmax, int low, float w, int64_t n);
 
-// Axis-pass launchers, one instantiation per label width (edt_passes.cuh).
+// Whether launch_first runs the register-resident X kernel (rows of at most 1024 voxels, a multiple
+// of 4, labels and distances aligned for vector access) -- the only one that writes XPlanes.
+inline bool first_is_vec(const void* labels, int label_bytes, const float* f, int64_t sx) {
+  return sx % 4 == 0 && sx <= 1024 && reinterpret_cast<uintptr_t>(labels) % (4 * label_bytes) == 0 &&
+         reinterpret_cast<uintptr_t>(f) % 16 == 0;
+}
+
+// Axis-pass launchers, one instantiation per label width (edt_passes.cuh).  planes: the run-start
+// planes the X pass writes (null: none; only for labels of 4 or 8 bytes and rows of at most 512
+// voxels where first_is_vec holds).
+// bits: the later pass's run-start plane from such an X pass (null: none); it is read only where the
+// pass takes the label-noise tile kernel, otherwise the labels are.
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
-                 DeviceCache& dc, cudaStream_t stream);
+                 const XPlanes* planes, DeviceCache& dc, cudaStream_t stream);
 template <int Bytes>
-int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
-                 int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl);
+int launch_later(const void* labels, const RunBits* bits, float* f, const LineGeom& g0, float w, int border_lo,
+                 int border_hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl);
+// noise_predicted (edt_passes.cuh) for host code that launches nothing (edt_plan.cu).
+bool label_noise_predicted(const DeviceCache& dc);
 // The site-tracking passes of the feature transform and the kernel that resolves their codes
 // into coordinate planes (edt_passes.cuh, edt_feature.cuh).
 template <int Bytes>

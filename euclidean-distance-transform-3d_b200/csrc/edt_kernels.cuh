@@ -272,16 +272,39 @@ template <> struct Vec4Labels<8> {
   }
 };
 
+// Run-start bit planes that the X pass writes for the later passes, so that these read one bit
+// per voxel instead of a label (used on label noise, see run_passes).  One bit per voxel, x fastest,
+// every row (y, z) padded to wpr = ceil(sx / 32) whole words, row (y, z) at word (z * sy + y) * wpr:
+//   y   bit = y == 0 || L(x, y, z) != L(x, y - 1, z)     (the Y pass's run starts)
+//   z   bit = z == 0 || L(x, y, z) != L(x, y, z - 1)     (the Z pass's run starts; 3-D only, else null)
+struct XPlanes {
+  uint32_t* y;
+  uint32_t* z;
+  int64_t sy;              // rows per z
+};
+
+// A lane's 4-bit nibble of a 128-voxel block (voxels 4 lane .. 4 lane + 3) -> the block's 32-bit
+// word that holds it, in natural x order: word w of the block ends up in lanes 8w .. 8w + 7.
+__device__ __forceinline__ uint32_t nibbles_to_word(uint32_t nib, int lane) {
+  uint32_t v = nib << (4 * (lane & 7));
+  v |= __shfl_xor_sync(0xffffffffu, v, 1);
+  v |= __shfl_xor_sync(0xffffffffu, v, 2);
+  v |= __shfl_xor_sync(0xffffffffu, v, 4);
+  return v;
+}
+
 // Plain = true: squared EDT, background forced to 0, no sqrt / sign (the hot configuration);
 // Plain = false: behaviour selected by `flags` at run time.
-template <int Bytes, int K, bool Plain>
+// Planes: the run-start planes written (XPlanes): 0 none, 1 the y plane, 2 the y and z planes.
+template <int Bytes, int K, bool Plain, int Planes = 0>
 // Registers capped for occupancy: uncapped the kernel takes 64 (rows <= 512: 4 CTAs per SM) / 99 registers
 // (1024-voxel rows: 2 CTAs); at 48 / 80 it still has no spills and runs 5 / 3 CTAs per SM, which
-// hides more of the label-load latency (6 CTAs would need 40 registers, and there it spills).
-__global__ void __launch_bounds__(256, K >= 8 ? 3 : 5)
+// hides more of the label-load latency (6 CTAs would need 40 registers, and there it spills).  Writing
+// planes, rows <= 512 take 64 registers (4 CTAs per SM): at 48 they spill, which measured slower.
+__global__ void __launch_bounds__(256, K >= 8 ? 3 : (Planes ? 4 : 5))
 first_axis_vec_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
                       float* __restrict__ out, int64_t nlines, int sx,
-                      const float* __restrict__ table, int border, int flags, RunStat stat) {
+                      const float* __restrict__ table, int border, int flags, RunStat stat, XPlanes planes) {
   using LT = typename LabelOf<Bytes>::type;
   using WT = typename LabelOf<Bytes>::wide;
   extern __shared__ float table_s[];                 // T[0..sx], then +inf at sx + 1
@@ -299,8 +322,16 @@ first_axis_vec_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
   const bool keep_background = Plain ? false : (flags & kZeroLabel) != 0;
   unsigned int nstarts = 0;                          // label changes along x seen by this lane
 
-  for (int64_t line = (int64_t)blockIdx.x * warps + warp; line < nlines;
-       line += (int64_t)gridDim.x * warps) {
+  // Rows: grid-stride, or (Planes) one contiguous range per CTA with its warps side by side, so that
+  // row (y, z - 1), sy rows back, is read a few CTAs back in the same wave and comes from L2
+  int64_t line = (int64_t)blockIdx.x * warps + warp, line_end = nlines, step = (int64_t)gridDim.x * warps;
+  if (Planes > 0) {
+    const int64_t per = ((nlines + gridDim.x - 1) / gridDim.x + warps - 1) / warps * warps;
+    line = (int64_t)blockIdx.x * per + warp;
+    line_end = min(nlines, ((int64_t)blockIdx.x + 1) * per);
+    step = warps;
+  }
+  for (; line < line_end; line += step) {
     const LT* __restrict__ src = labels + line * sx;
     float* __restrict__ dst = out + line * sx;
 
@@ -401,6 +432,41 @@ first_axis_vec_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
       }
       *reinterpret_cast<float4*>(dst + q0) = make_float4(r[0], r[1], r[2], r[3]);
     }
+
+    // ---- run-start planes: compare with rows (y - 1, z) and (y, z - 1), pack nibbles into words ----
+    // The row's own labels are read again (from L1: this warp has just loaded them) rather than kept
+    // in registers through the boundary search, and a block's loads are issued only once the previous
+    // block's words exist (`dep`, a zero the compiler cannot see through): either way the kernel
+    // would spill at its register cap.
+    if constexpr (Planes > 0) {
+      const int64_t z = line / planes.sy, y = line - z * planes.sy;
+      const int64_t wrow = line * ((sx + 31) >> 5);
+      uint32_t dep = 0u;
+#pragma unroll
+      for (int b = 0; b < K; ++b) {
+        const int q0 = (b << 7) + (lane << 2) + (int)dep;
+        const bool in_row = q0 < sx;
+        const bool store = (lane & 7) == 0 && in_row;           // the word's first voxel is in the row
+        const int64_t wi = wrow + (q0 >> 5);
+        WT here[4], u[Planes][4];
+        if (in_row) {
+          Vec4Labels<Bytes>::load(src + q0, here);
+#pragma unroll
+          for (int a = 0; a < Planes; ++a)
+            if ((a == 0 ? y : z) > 0) Vec4Labels<Bytes>::load(src - (a == 0 ? (int64_t)sx : sx * planes.sy) + q0, u[a]);
+        }
+#pragma unroll
+        for (int a = 0; a < Planes; ++a) {
+          uint32_t nib = in_row ? 15u : 0u;                     // first row along the axis: all start
+          if (in_row && (a == 0 ? y : z) > 0)
+            nib = (u[a][0] != here[0] ? 1u : 0u) | (u[a][1] != here[1] ? 2u : 0u) |
+                  (u[a][2] != here[2] ? 4u : 0u) | (u[a][3] != here[3] ? 8u : 0u);
+          const uint32_t word = nibbles_to_word(nib, lane);
+          if (store) (a == 0 ? planes.y : planes.z)[wi] = word;
+          asm volatile("and.b32 %0, %1, 0;" : "=r"(dep) : "r"(word));
+        }
+      }
+    }
   }
   if (stat.counter) {
 #pragma unroll
@@ -445,6 +511,17 @@ struct LineGeom {
 struct TileBoxes {
   int box_rows;   // rows per TMA box (<= 256)
   int nboxes;     // boxes per tile; box_rows * nboxes >= n
+};
+
+// The run-start plane of one later-axis pass written by the X pass (XPlanes): for the line (outer o,
+// inner j) and row i the bit (j % sx) & 31 of word  o * outer_words + (j / sx) * wpr + (j % sx) / 32
+// + i * row_words.  Y pass: outer = z, inner = x; Z pass: inner = y * sx + x.
+struct RunBits {
+  const uint32_t* start;   // a run of equal labels starts at this row (always at row 0)
+  int64_t row_words;
+  int64_t outer_words;
+  int64_t sx;
+  int64_t wpr;
 };
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
@@ -852,12 +929,18 @@ __device__ __forceinline__ void walk_begin(HullWalk& w, const TileLine<TX> ln, i
 // only the streaming path runs.  The host picks per launch (edt_passes.cuh).
 // IntHull: hull tests in exact integer arithmetic (the host guarantees integer-valued samples with
 // f + w2 * n^2 < 2^31 and passes w2 as an integer in `w2i`); otherwise in double.
-template <int Bytes, int TX, bool Epilogue, bool UseTMA, bool Wide, int MinCtas, bool IntHull>
+// Bits: stage 0 reads the pass's run-start plane (RunBits, written by the X pass) instead of the
+// labels: 4 + 1/8 bytes per voxel instead of 4 + Bytes on label noise, where nothing is stored.  The
+// plane is read only after griddepcontrol.wait: the Z pass may start while the X pass is still
+// running (the Y pass lets its dependents start before it waits itself).  Compiled for the
+// label-noise shape only (2 CTAs per SM, TMA, 32-wide tiles, no background bits: unsigned transforms).
+template <int Bytes, int TX, bool Epilogue, bool UseTMA, bool Wide, int MinCtas, bool IntHull, bool Bits = false>
 __global__ void __launch_bounds__(Wide ? 1024 : 512, Wide ? 1 : MinCtas)
 later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
-                       const typename LabelOf<Bytes>::type* __restrict__ labels,
+                       const typename LabelOf<Bytes>::type* __restrict__ labels, const RunBits rb,
                        float* __restrict__ f, LineGeom g, TileBoxes tb, float w2,
                        int border_lo, int border_hi, int flags, int w2i) {
+  static_assert(!Bits || (UseTMA && !Wide), "the run-start plane is read by the TMA, non-wide variants only");
   using LT = typename LabelOf<Bytes>::type;
   extern __shared__ __align__(128) unsigned char smem_tile[];
   constexpr int SUBS = 32 / TX;                       // chunks handled side by side by one warp
@@ -933,8 +1016,39 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
     }
   }
 
+  // ============ stage 0 (Bits): run-start bits -> one word per (chunk, line) ============
+  if constexpr (Bits) {
+    pdl_wait_for_previous_grid();      // the plane is complete (written by the X pass)
+    if (live) {
+      const int64_t j = inner0 + x, q = j / rb.sx, rj = j - q * rb.sx;
+      const uint32_t* bstart = rb.start + (outer * rb.outer_words + q * rb.wpr + (rj >> 5));
+      const int bit = (int)(rj & 31);
+      const size_t rw = (size_t)rb.row_words;
+      for (int c = chunk0; c < nchunks; c += chunk_step) {
+        const int i0 = c << 5;
+        const uint32_t* sp = bstart + (size_t)i0 * rw;
+        uint32_t wstart = 0;
+        if (i0 + 32 <= n) {
+#pragma unroll
+          for (int r = 0; r < 32; ++r) wstart |= ((__ldg(sp + r * rw) >> bit) & 1u) << r;
+        } else {
+          for (int r = 0; r < n - i0; ++r) wstart |= ((__ldg(sp + r * rw) >> bit) & 1u) << r;
+          wstart |= 1u << (n - i0);        // pretend a run starts at row n (line end)
+        }
+        if (i0 == 0) wstart |= 1u;         // a run starts at row 0 by definition
+        sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wstart);
+        if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);   // no sign: not read
+      }
+    } else {
+      for (int c = chunk0; c < nchunks; c += chunk_step) {
+        sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);
+        if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);
+      }
+    }
+  }
+
   // ============ stage 0: labels -> run-start / background words ============
-  for (int c = chunk0; c < nchunks; c += chunk_step) {
+  for (int c = chunk0; !Bits && c < nchunks; c += chunk_step) {
     const int i0 = c << 5;
     uint32_t wstart = 0, wzero = 0, ext = 1u;      // ext: a run starts at row i0 + 32 (or the line ends there)
     if (live) {

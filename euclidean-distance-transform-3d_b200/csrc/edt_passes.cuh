@@ -41,33 +41,51 @@ int launch_first_generic(const void* labels, float* f, int* codes, int64_t nline
   return 0;
 }
 
+// The register-resident X kernel for K 128-voxel blocks per row, with the run-start planes `planes`
+// asks for (only compiled for labels of 4 and 8 bytes and rows of at most 512 voxels, where
+// run_passes writes them: on 1024-voxel rows the kernel would spill at its register cap).
+template <int Bytes, int K, bool Plain>
+void launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, const float* table, int border,
+                      int flags, RunStat stat, const XPlanes& planes, unsigned blocks, size_t smem,
+                      cudaStream_t stream) {
+  using LT = typename LabelOf<Bytes>::type;
+  auto kern = first_axis_vec_kernel<Bytes, K, Plain, 0>;
+  if constexpr (Bytes >= 4 && K <= 4) {
+    if (planes.y) kern = planes.z ? first_axis_vec_kernel<Bytes, K, Plain, 2> : first_axis_vec_kernel<Bytes, K, Plain, 1>;
+  }
+  kern<<<blocks, 256, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table, border, flags, stat,
+                                      planes);
+}
+
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
-                 DeviceCache& dc, cudaStream_t stream) {
+                 const XPlanes* planes, DeviceCache& dc, cudaStream_t stream) {
+  if (planes && (Bytes < 4 || sx > 512 || !first_is_vec(labels, Bytes, f, sx)))
+    return fail(EDTB200_EINVAL, "run-start planes asked of an X launch that cannot write them");
   StepTable step(dc, stream);
   int trc = step.get(w, (int)sx + 1);
   if (trc) return trc;
   const float* table = step.data();
   const RunStat stat = run_stat(dc, (unsigned long long)nlines * (unsigned long long)sx);
 
-  using LT = typename LabelOf<Bytes>::type;
   // register-resident vector kernel when rows are short and 16-byte aligned
-  if (sx % 4 == 0 && sx <= 1024 && reinterpret_cast<uintptr_t>(labels) % (4 * Bytes) == 0 &&
-      reinterpret_cast<uintptr_t>(f) % 16 == 0) {
+  if (first_is_vec(labels, Bytes, f, sx)) {
     const size_t smem = sizeof(float) * (size_t)(sx + 2);
     int64_t blocks = (nlines + 7) / 8;
     const int64_t cap = (int64_t)dc.sm_count * (sx > 512 ? 12 : 15);   // whole waves at 5 (rows <= 512) / 3 CTAs per SM
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    const LT* lab = static_cast<const LT*>(labels);
-#define EDT_LAUNCH_VEC(KK)                                                                              \
-  do {                                                                                                  \
-    if (flags == 0)                                                                                     \
-      first_axis_vec_kernel<Bytes, KK, true><<<(unsigned)blocks, 256, smem, stream>>>(                  \
-          lab, f, nlines, (int)sx, table, border, flags, stat);                                         \
-    else                                                                                                \
-      first_axis_vec_kernel<Bytes, KK, false><<<(unsigned)blocks, 256, smem, stream>>>(                 \
-          lab, f, nlines, (int)sx, table, border, flags, stat);                                         \
+    XPlanes none;
+    memset(&none, 0, sizeof(none));
+    const XPlanes& pl = planes ? *planes : none;
+#define EDT_LAUNCH_VEC(KK)                                                                                        \
+  do {                                                                                                            \
+    if (flags == 0)                                                                                               \
+      launch_first_vec<Bytes, KK, true>(labels, f, nlines, sx, table, border, flags, stat, pl, (unsigned)blocks,   \
+                                        smem, stream);                                                            \
+    else                                                                                                          \
+      launch_first_vec<Bytes, KK, false>(labels, f, nlines, sx, table, border, flags, stat, pl, (unsigned)blocks,  \
+                                         smem, stream);                                                           \
   } while (0)
     if (sx <= 128)      EDT_LAUNCH_VEC(1);
     else if (sx <= 256) EDT_LAUNCH_VEC(2);
@@ -198,9 +216,22 @@ TileKernel<Bytes> tile_kernel(const LaterLaunch& p) {
                 : later_axis_tile_kernel<Bytes, 32, Epi, false, false, 3, false>;
 }
 
+// The variant of the 2-CTA tile kernel that reads the X pass's run-start plane (labels of 4 and 8
+// bytes only; no background bits, so never for a signed pass).
 template <int Bytes>
-int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int border_lo, int border_hi,
-                 int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl) {
+TileKernel<Bytes> tile_kernel_bits(const LaterLaunch& p) {
+  if constexpr (Bytes >= 4) {
+    if (p.epilogue) return p.int_hull ? later_axis_tile_kernel<Bytes, 32, true, true, false, 2, true, true>
+                                      : later_axis_tile_kernel<Bytes, 32, true, true, false, 2, false, true>;
+    return p.int_hull ? later_axis_tile_kernel<Bytes, 32, false, true, false, 2, true, true>
+                      : later_axis_tile_kernel<Bytes, 32, false, true, false, 2, false, true>;
+  }
+  return nullptr;
+}
+
+template <int Bytes>
+int launch_later(const void* labels, const RunBits* bits, float* f, const LineGeom& g0, float w, int border_lo,
+                 int border_hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl) {
   using LT = typename LabelOf<Bytes>::type;
   LineGeom g = g0;
   const float w2 = w * w;                       // float product, as src/edt.hpp:181
@@ -233,12 +264,19 @@ int launch_later(const void* labels, float* f, const LineGeom& g0, float w, int 
     pdl_attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = pdl_attr;
     cfg.numAttrs = pdl ? 1 : 0;   // only when the previous kernel of the stream is our own pass
+    // the X pass's run-start plane is read where the plan is the label-noise variant (the prediction
+    // the plane was written for); any other plan reads the labels, and the plane goes unused
+    const bool use_bits = bits && Bytes >= 4 && p.tx == 32 && p.tma && !p.wide && p.ctas == 2 && !(flags & kNegate);
+    RunBits rb;
+    memset(&rb, 0, sizeof(rb));
+    if (use_bits) rb = *bits;
     const TileKernel<Bytes> kern =
-        p.epilogue ? (p.tma ? tile_kernel<Bytes, true, true>(p) : tile_kernel<Bytes, true, false>(p))
-                   : (p.tma ? tile_kernel<Bytes, false, true>(p) : tile_kernel<Bytes, false, false>(p));
+        use_bits ? tile_kernel_bits<Bytes>(p)
+        : p.epilogue ? (p.tma ? tile_kernel<Bytes, true, true>(p) : tile_kernel<Bytes, true, false>(p))
+                     : (p.tma ? tile_kernel<Bytes, false, true>(p) : tile_kernel<Bytes, false, false>(p));
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, static_cast<const LT*>(labels), f, g, tb, w2, border_lo, border_hi,
-                                flags, p.int_hull ? (int)w2 : 0));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, static_cast<const LT*>(labels), rb, f, g, tb, w2, border_lo,
+                                border_hi, flags, p.int_hull ? (int)w2 : 0));
     g_last_later = p;
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -308,10 +346,12 @@ int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim
 
 #define EDT_INSTANTIATE_PASSES(B)                                                                        \
   template int edtb200::host::launch_first<B>(const void*, float*, int64_t, int64_t, float, int, int,    \
-                                              edtb200::host::DeviceCache&, cudaStream_t);                \
-  template int edtb200::host::launch_later<B>(const void*, float*, const edtb200::LineGeom&, float, int, \
-                                              int, int, edtb200::host::PassArith,                        \
-                                              edtb200::host::DeviceCache&, cudaStream_t, bool);          \
+                                              const edtb200::XPlanes*, edtb200::host::DeviceCache&,      \
+                                              cudaStream_t);                                             \
+  template int edtb200::host::launch_later<B>(const void*, const edtb200::RunBits*, float*,              \
+                                              const edtb200::LineGeom&, float, int, int, int,            \
+                                              edtb200::host::PassArith, edtb200::host::DeviceCache&,     \
+                                              cudaStream_t, bool);                                       \
   template int edtb200::host::launch_first_sites<B>(const void*, float*, int*, int64_t, int64_t, float, int, \
                                                     int, edtb200::host::DeviceCache&, cudaStream_t);     \
   template int edtb200::host::launch_later_sites<B>(const void*, const float*, float*, int*,              \

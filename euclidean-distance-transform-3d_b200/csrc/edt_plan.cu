@@ -11,5 +11,7 @@ bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin) 
   return plan_later(g, false, arith, max_smem_optin, true, false, false).kernel == 1;
 }
 
+bool label_noise_predicted(const DeviceCache& dc) { return noise_predicted(dc); }
+
 }  // namespace host
 }  // namespace edtb200

@@ -623,8 +623,9 @@ edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz);
 // bit per voxel and later axis, stream-ordered scratch freed on the stream when the owner goes out
 // of scope.  They pay where the later passes only stream -- label noise (predicted from the previous
 // transform's run statistic, as the later passes' CTA count is) with labels of 4 or 8 bytes: there a
-// later pass moves 4 + 1/8 bytes per voxel instead of 8 or 12, for 1/4 byte more written and two
-// rows re-read from L1 / L2 by the X pass.  On narrower labels and on structured volumes the dearer
+// later pass moves 4 + 1/8 bytes per voxel instead of 8 or 12, for 1/4 byte more written by the X pass
+// (which stages its label rows in shared memory to compare neighbouring rows).  On narrower labels
+// and on structured volumes the dearer
 // X pass costs more than the later passes gain (DESIGN.md section 4.1), so none are taken there;
 // nor for signed transforms, whose last pass needs the labels' background bits as well.
 struct RunPlanes {

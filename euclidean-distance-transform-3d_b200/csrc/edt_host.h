@@ -169,8 +169,8 @@ PassArith transform_arith(const float* w, const int64_t* n, int k);
 // lowest set bit over the finite non-zero samples is 2^low (1024: there is none).
 PassArith sampled_arith(float fmax, int low, float w, int64_t n);
 
-// Whether launch_first runs the register-resident X kernel (rows of at most 1024 voxels, a multiple
-// of 4, labels and distances aligned for vector access) -- the only one that writes XPlanes.
+// Whether launch_first runs the register-resident X kernels (rows of at most 1024 voxels, a multiple
+// of 4, labels and distances aligned for vector access) -- the only ones that write XPlanes.
 inline bool first_is_vec(const void* labels, int label_bytes, const float* f, int64_t sx) {
   return sx % 4 == 0 && sx <= 1024 && reinterpret_cast<uintptr_t>(labels) % (4 * label_bytes) == 0 &&
          reinterpret_cast<uintptr_t>(f) % 16 == 0;

@@ -293,18 +293,126 @@ __device__ __forceinline__ uint32_t nibbles_to_word(uint32_t nib, int lane) {
   return v;
 }
 
+// One row of the register-resident X kernels, from its labels to its distances at dst: the lane's
+// labels v (voxels 128 b + 4 lane .. + 3 of block b; load(q0, v[b]) fetches the four at q0, zeros
+// past sx), run-start / background masks, nearest boundaries, table lookups from table_s (T[0..sx],
+// +inf at sx + 1) and float4 stores.  Adds the row's label changes along x to the lane's nstarts.
 // Plain = true: squared EDT, background forced to 0, no sqrt / sign (the hot configuration);
 // Plain = false: behaviour selected by `flags` at run time.
-// Planes: the run-start planes written (XPlanes): 0 none, 1 the y plane, 2 the y and z planes.
-template <int Bytes, int K, bool Plain, int Planes = 0>
+template <int Bytes, int K, bool Plain, class Load>
+__device__ __forceinline__ void first_axis_vec_row(Load load, float* __restrict__ dst, int sx, const float* table_s,
+                                                   int border, int flags, bool keep_background, int lane,
+                                                   unsigned lt_mask, unsigned gt_mask, unsigned int& nstarts) {
+  using WT = typename LabelOf<Bytes>::wide;
+  const unsigned full = 0xffffffffu;
+
+  // ---- labels -> per-block 4-bit "label changes here" / "is background" masks ----
+  WT v[K][4];
+#pragma unroll
+  for (int b = 0; b < K; ++b) {
+    const int q0 = (b << 7) + (lane << 2);
+    if (q0 < sx) load(q0, v[b]);
+    else { v[b][0] = v[b][1] = v[b][2] = v[b][3] = 0; }
+  }
+  uint32_t edges = 0, zeros = 0;                   // 4 bits per block
+  uint32_t occ[K];                                 // lanes owning at least one boundary
+#pragma unroll
+  for (int b = 0; b < K; ++b) {
+    const int q0 = (b << 7) + (lane << 2);
+    WT up = __shfl_up_sync(full, v[b][3], 1);
+    if (b > 0) {                                   // compile-time: warp-uniform
+      const WT tail = __shfl_sync(full, v[b > 0 ? b - 1 : 0][3], 31);
+      if (lane == 0) up = tail;
+    }
+    uint32_t m = 0, z = 0;
+    if (q0 < sx) {
+      if ((q0 == 0) ? (border != 0) : (v[b][0] != up)) m |= 1u;
+      if (v[b][1] != v[b][0]) m |= 2u;
+      if (v[b][2] != v[b][1]) m |= 4u;
+      if (v[b][3] != v[b][2]) m |= 8u;
+      if (v[b][0] == 0) z |= 1u;
+      if (v[b][1] == 0) z |= 2u;
+      if (v[b][2] == 0) z |= 4u;
+      if (v[b][3] == 0) z |= 8u;
+    }
+    occ[b] = __ballot_sync(full, m != 0);
+    edges |= m << (4 * b);
+    zeros |= z << (4 * b);
+  }
+  nstarts += __popc(edges);
+
+  // ---- nearest boundary strictly below / above the lane's 4 voxels, per block ----
+  // The ballots give the boundary-owning lanes; one shuffle fetches that lane's masks.
+  int kl_in[K], kr_in[K];          // kL of the voxel just below q0, kR seed for q0 + 3
+  {
+    uint32_t prev_occ = 0; int prev_b = 0;
+#pragma unroll
+    for (int b = 0; b < K; ++b) {
+      const int q0 = (b << 7) + (lane << 2);
+      const uint32_t mine = occ[b] & lt_mask;
+      const uint32_t pick = mine ? mine : prev_occ;
+      const int pb = mine ? b : prev_b;
+      const int sl = 31 - __clz(pick | 1u);
+      const uint32_t nib = (__shfl_sync(full, edges, sl) >> (4 * pb)) & 15u;
+      const int pos = (pb << 7) + (sl << 2) + 31 - __clz(nib | 1u);
+      kl_in[b] = pick ? (q0 - pos) : kNoBoundary;          // = kL(q0 - 1) + ... see below
+      if (occ[b]) { prev_occ = occ[b]; prev_b = b; }
+    }
+    uint32_t next_occ = 0; int next_b = 0;
+#pragma unroll
+    for (int b = K - 1; b >= 0; --b) {
+      const int q0 = (b << 7) + (lane << 2);
+      const uint32_t mine = occ[b] & gt_mask;
+      const uint32_t pick = mine ? mine : next_occ;
+      const int pb = mine ? b : next_b;
+      const int sl = __ffs(pick | 0x80000000u) - 1;
+      const uint32_t nib = (__shfl_sync(full, edges, sl) >> (4 * pb)) & 15u;
+      const int pos = (pb << 7) + (sl << 2) + __ffs(nib | 8u) - 1;
+      const int far = border ? (sx - (q0 + 3)) : kNoBoundary;
+      kr_in[b] = pick ? (pos - (q0 + 3)) : far;
+      if (occ[b]) { next_occ = occ[b]; next_b = b; }
+    }
+  }
+
+  // ---- distances (chains over the 4 voxels), table lookup, vector store ----
+#pragma unroll
+  for (int b = 0; b < K; ++b) {
+    const int q0 = (b << 7) + (lane << 2);
+    if (q0 >= sx) continue;
+    const uint32_t m = (edges >> (4 * b)) & 15u;
+    const uint32_t z = (zeros >> (4 * b)) & 15u;
+    // kL(q) = q - (nearest boundary position <= q) + 1:  1 at a boundary, else previous + 1
+    int kl[4], kr[4];
+    int run = kl_in[b];                    // q0 - pos: kL the voxel q0 would have without its own bit
+#pragma unroll
+    for (int e = 0; e < 4; ++e) { run = ((m >> e) & 1u) ? 1 : run + 1; kl[e] = run; }
+    // kR(q) = (nearest boundary position > q) - q:  1 if q + 1 is a boundary, else next + 1
+    run = kr_in[b];
+    kr[3] = run;
+#pragma unroll
+    for (int e = 2; e >= 0; --e) { run = ((m >> (e + 1)) & 1u) ? 1 : run + 1; kr[e] = run; }
+    float r[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      int k = min(min(kl[e], kr[e]), sx + 1);          // sx + 1 -> +inf (no boundary at all)
+      const bool background = (z >> e) & 1u;
+      if (background && !keep_background) k = 0;        // T[0] = 0
+      float val = table_s[k];
+      if (!Plain) val = finish_value(val, background, flags);
+      r[e] = val;
+    }
+    *reinterpret_cast<float4*>(dst + q0) = make_float4(r[0], r[1], r[2], r[3]);
+  }
+}
+
+template <int Bytes, int K, bool Plain>
 // Registers capped for occupancy: uncapped the kernel takes 64 (rows <= 512: 4 CTAs per SM) / 99 registers
 // (1024-voxel rows: 2 CTAs); at 48 / 80 it still has no spills and runs 5 / 3 CTAs per SM, which
-// hides more of the label-load latency (6 CTAs would need 40 registers, and there it spills).  Writing
-// planes, rows <= 512 take 64 registers (4 CTAs per SM): at 48 they spill, which measured slower.
-__global__ void __launch_bounds__(256, K >= 8 ? 3 : (Planes ? 4 : 5))
+// hides more of the label-load latency (6 CTAs would need 40 registers, and there it spills).
+__global__ void __launch_bounds__(256, K >= 8 ? 3 : 5)
 first_axis_vec_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
                       float* __restrict__ out, int64_t nlines, int sx,
-                      const float* __restrict__ table, int border, int flags, RunStat stat, XPlanes planes) {
+                      const float* __restrict__ table, int border, int flags, RunStat stat) {
   using LT = typename LabelOf<Bytes>::type;
   using WT = typename LabelOf<Bytes>::wide;
   extern __shared__ float table_s[];                 // T[0..sx], then +inf at sx + 1
@@ -322,151 +430,12 @@ first_axis_vec_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
   const bool keep_background = Plain ? false : (flags & kZeroLabel) != 0;
   unsigned int nstarts = 0;                          // label changes along x seen by this lane
 
-  // Rows: grid-stride, or (Planes) one contiguous range per CTA with its warps side by side, so that
-  // row (y, z - 1), sy rows back, is read a few CTAs back in the same wave and comes from L2
-  int64_t line = (int64_t)blockIdx.x * warps + warp, line_end = nlines, step = (int64_t)gridDim.x * warps;
-  if (Planes > 0) {
-    const int64_t per = ((nlines + gridDim.x - 1) / gridDim.x + warps - 1) / warps * warps;
-    line = (int64_t)blockIdx.x * per + warp;
-    line_end = min(nlines, ((int64_t)blockIdx.x + 1) * per);
-    step = warps;
-  }
-  for (; line < line_end; line += step) {
+  const int64_t step = (int64_t)gridDim.x * warps;
+  for (int64_t line = (int64_t)blockIdx.x * warps + warp; line < nlines; line += step) {
     const LT* __restrict__ src = labels + line * sx;
     float* __restrict__ dst = out + line * sx;
-
-    // ---- labels -> per-block 4-bit "label changes here" / "is background" masks ----
-    WT v[K][4];
-#pragma unroll
-    for (int b = 0; b < K; ++b) {
-      const int q0 = (b << 7) + (lane << 2);
-      if (q0 < sx) Vec4Labels<Bytes>::load(src + q0, v[b]);
-      else { v[b][0] = v[b][1] = v[b][2] = v[b][3] = 0; }
-    }
-    uint32_t edges = 0, zeros = 0;                   // 4 bits per block
-    uint32_t occ[K];                                 // lanes owning at least one boundary
-#pragma unroll
-    for (int b = 0; b < K; ++b) {
-      const int q0 = (b << 7) + (lane << 2);
-      WT up = __shfl_up_sync(full, v[b][3], 1);
-      if (b > 0) {                                   // compile-time: warp-uniform
-        const WT tail = __shfl_sync(full, v[b > 0 ? b - 1 : 0][3], 31);
-        if (lane == 0) up = tail;
-      }
-      uint32_t m = 0, z = 0;
-      if (q0 < sx) {
-        if ((q0 == 0) ? (border != 0) : (v[b][0] != up)) m |= 1u;
-        if (v[b][1] != v[b][0]) m |= 2u;
-        if (v[b][2] != v[b][1]) m |= 4u;
-        if (v[b][3] != v[b][2]) m |= 8u;
-        if (v[b][0] == 0) z |= 1u;
-        if (v[b][1] == 0) z |= 2u;
-        if (v[b][2] == 0) z |= 4u;
-        if (v[b][3] == 0) z |= 8u;
-      }
-      occ[b] = __ballot_sync(full, m != 0);
-      edges |= m << (4 * b);
-      zeros |= z << (4 * b);
-    }
-    nstarts += __popc(edges);
-
-    // ---- nearest boundary strictly below / above the lane's 4 voxels, per block ----
-    // The ballots give the boundary-owning lanes; one shuffle fetches that lane's masks.
-    int kl_in[K], kr_in[K];          // kL of the voxel just below q0, kR seed for q0 + 3
-    {
-      uint32_t prev_occ = 0; int prev_b = 0;
-#pragma unroll
-      for (int b = 0; b < K; ++b) {
-        const int q0 = (b << 7) + (lane << 2);
-        const uint32_t mine = occ[b] & lt_mask;
-        const uint32_t pick = mine ? mine : prev_occ;
-        const int pb = mine ? b : prev_b;
-        const int sl = 31 - __clz(pick | 1u);
-        const uint32_t nib = (__shfl_sync(full, edges, sl) >> (4 * pb)) & 15u;
-        const int pos = (pb << 7) + (sl << 2) + 31 - __clz(nib | 1u);
-        kl_in[b] = pick ? (q0 - pos) : kNoBoundary;          // = kL(q0 - 1) + ... see below
-        if (occ[b]) { prev_occ = occ[b]; prev_b = b; }
-      }
-      uint32_t next_occ = 0; int next_b = 0;
-#pragma unroll
-      for (int b = K - 1; b >= 0; --b) {
-        const int q0 = (b << 7) + (lane << 2);
-        const uint32_t mine = occ[b] & gt_mask;
-        const uint32_t pick = mine ? mine : next_occ;
-        const int pb = mine ? b : next_b;
-        const int sl = __ffs(pick | 0x80000000u) - 1;
-        const uint32_t nib = (__shfl_sync(full, edges, sl) >> (4 * pb)) & 15u;
-        const int pos = (pb << 7) + (sl << 2) + __ffs(nib | 8u) - 1;
-        const int far = border ? (sx - (q0 + 3)) : kNoBoundary;
-        kr_in[b] = pick ? (pos - (q0 + 3)) : far;
-        if (occ[b]) { next_occ = occ[b]; next_b = b; }
-      }
-    }
-
-    // ---- distances (chains over the 4 voxels), table lookup, vector store ----
-#pragma unroll
-    for (int b = 0; b < K; ++b) {
-      const int q0 = (b << 7) + (lane << 2);
-      if (q0 >= sx) continue;
-      const uint32_t m = (edges >> (4 * b)) & 15u;
-      const uint32_t z = (zeros >> (4 * b)) & 15u;
-      // kL(q) = q - (nearest boundary position <= q) + 1:  1 at a boundary, else previous + 1
-      int kl[4], kr[4];
-      int run = kl_in[b];                    // q0 - pos: kL the voxel q0 would have without its own bit
-#pragma unroll
-      for (int e = 0; e < 4; ++e) { run = ((m >> e) & 1u) ? 1 : run + 1; kl[e] = run; }
-      // kR(q) = (nearest boundary position > q) - q:  1 if q + 1 is a boundary, else next + 1
-      run = kr_in[b];
-      kr[3] = run;
-#pragma unroll
-      for (int e = 2; e >= 0; --e) { run = ((m >> (e + 1)) & 1u) ? 1 : run + 1; kr[e] = run; }
-      float r[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        int k = min(min(kl[e], kr[e]), sx + 1);          // sx + 1 -> +inf (no boundary at all)
-        const bool background = (z >> e) & 1u;
-        if (background && !keep_background) k = 0;        // T[0] = 0
-        float val = table_s[k];
-        if (!Plain) val = finish_value(val, background, flags);
-        r[e] = val;
-      }
-      *reinterpret_cast<float4*>(dst + q0) = make_float4(r[0], r[1], r[2], r[3]);
-    }
-
-    // ---- run-start planes: compare with rows (y - 1, z) and (y, z - 1), pack nibbles into words ----
-    // The row's own labels are read again (from L1: this warp has just loaded them) rather than kept
-    // in registers through the boundary search, and a block's loads are issued only once the previous
-    // block's words exist (`dep`, a zero the compiler cannot see through): either way the kernel
-    // would spill at its register cap.
-    if constexpr (Planes > 0) {
-      const int64_t z = line / planes.sy, y = line - z * planes.sy;
-      const int64_t wrow = line * ((sx + 31) >> 5);
-      uint32_t dep = 0u;
-#pragma unroll
-      for (int b = 0; b < K; ++b) {
-        const int q0 = (b << 7) + (lane << 2) + (int)dep;
-        const bool in_row = q0 < sx;
-        const bool store = (lane & 7) == 0 && in_row;           // the word's first voxel is in the row
-        const int64_t wi = wrow + (q0 >> 5);
-        WT here[4], u[Planes][4];
-        if (in_row) {
-          Vec4Labels<Bytes>::load(src + q0, here);
-#pragma unroll
-          for (int a = 0; a < Planes; ++a)
-            if ((a == 0 ? y : z) > 0) Vec4Labels<Bytes>::load(src - (a == 0 ? (int64_t)sx : sx * planes.sy) + q0, u[a]);
-        }
-#pragma unroll
-        for (int a = 0; a < Planes; ++a) {
-          uint32_t nib = in_row ? 15u : 0u;                     // first row along the axis: all start
-          if (in_row && (a == 0 ? y : z) > 0)
-            nib = (u[a][0] != here[0] ? 1u : 0u) | (u[a][1] != here[1] ? 2u : 0u) |
-                  (u[a][2] != here[2] ? 4u : 0u) | (u[a][3] != here[3] ? 8u : 0u);
-          const uint32_t word = nibbles_to_word(nib, lane);
-          if (store) (a == 0 ? planes.y : planes.z)[wi] = word;
-          asm volatile("and.b32 %0, %1, 0;" : "=r"(dep) : "r"(word));
-        }
-      }
-    }
+    first_axis_vec_row<Bytes, K, Plain>([&](int q0, WT* v) { Vec4Labels<Bytes>::load(src + q0, v); }, dst, sx,
+                                        table_s, border, flags, keep_background, lane, lt_mask, gt_mask, nstarts);
   }
   if (stat.counter) {
 #pragma unroll
@@ -605,6 +574,162 @@ __device__ __forceinline__ uint32_t lds_u8_volatile(uint32_t addr) {
 }
 __device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+}
+
+// ---------------------------------------------------------------------------------------
+// First-axis pass that also writes the run-start planes (XPlanes), for rows of sx <= 128*K
+// voxels on which first_axis_vec_kernel runs, labels of 4 or 8 bytes.
+//
+// A CTA of W warps owns bands of W consecutive rows y0 .. y0+W-1 (warp w: row y0 + w).  A *stage*
+// is one band at one z together with its halo row y0 - 1 (none when y0 = 0): (W+1) rows that are
+// contiguous in memory, so one thread stages them with one 1-D bulk copy completed on an mbarrier.
+// The CTA walks a contiguous range of (band, z) items, z fastest, through a ring of S stages issued
+// S - 1 ahead, so that every label is read from HBM once: the y plane compares a row with its
+// stage's previous row, the z plane with the same row one stage back (the range's first item, if
+// z > 0, is preceded by one extra stage that is only compared against).  In 2-D every item is a
+// band of its own and the halo row is the previous band's last.  Items are split evenly over one
+// persistent wave of CTAs.
+//
+// Shared memory: S mbarriers (64 bytes), the ring of S stages of (W+1)*sx labels, the step table.
+// ---------------------------------------------------------------------------------------
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, unsigned bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar))
+               : "memory");
+}
+
+// Four labels of 4 or 8 bytes from shared memory: one or two 16-byte reads.
+template <int Bytes>
+__device__ __forceinline__ void load4_shared(const typename LabelOf<Bytes>::type* p,
+                                             typename LabelOf<Bytes>::wide v[4]) {
+  if constexpr (Bytes == 4) {
+    const uint4 w = *reinterpret_cast<const uint4*>(p);
+    v[0] = w.x; v[1] = w.y; v[2] = w.z; v[3] = w.w;
+  } else {
+    const ulonglong2 a = reinterpret_cast<const ulonglong2*>(p)[0];
+    const ulonglong2 b = reinterpret_cast<const ulonglong2*>(p)[1];
+    v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
+  }
+}
+
+constexpr int kPlaneBarBytes = 64;     // room for the ring's mbarriers (S <= 8)
+
+// Planes: 1 the y plane, 2 the y and z planes.  The ring's depth S is `stages`; W is blockDim.x / 32.
+// Registers capped at the CTAs per SM that the ring leaves room for with 8 warps, 3 stages and 512-voxel
+// rows: 3 for 4-byte labels (57 KB), 2 for 8-byte ones (110 KB).
+template <int Bytes, int K, bool Plain, int Planes>
+__global__ void __launch_bounds__(256, Bytes == 8 ? 2 : 3)
+first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
+                         float* __restrict__ out, int64_t nlines, int sx,
+                         const float* __restrict__ table, int border, int flags, RunStat stat, XPlanes planes,
+                         int stages) {
+  static_assert(Bytes >= 4 && Planes >= 1 && Planes <= 2, "the bulk copies need 16-byte label rows");
+  using LT = typename LabelOf<Bytes>::type;
+  using WT = typename LabelOf<Bytes>::wide;
+  extern __shared__ __align__(16) unsigned char planes_smem[];
+  pdl_launch_dependents();                           // the second-axis pass may start staging labels
+
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5;
+  const int warps = blockDim.x >> 5;
+  const int64_t sy = planes.sy, nz = nlines / sy;
+  const int64_t nbands = (sy + warps - 1) / warps;
+  const size_t row_bytes = (size_t)sx * Bytes;
+  const size_t stage_bytes = (size_t)(warps + 1) * row_bytes;
+  uint64_t* bar = reinterpret_cast<uint64_t*>(planes_smem);
+  LT* ring = reinterpret_cast<LT*>(planes_smem + kPlaneBarBytes);
+  float* table_s = reinterpret_cast<float*>(planes_smem + kPlaneBarBytes + stages * stage_bytes);
+
+  // this CTA's items [j0, j1); stage i holds item first + i, and stage 0 only serves as the z
+  // neighbour of stage 1 when it is the extra one (pro = 1)
+  const int64_t items = nbands * nz;
+  const int64_t j0 = items * blockIdx.x / gridDim.x, j1 = items * (blockIdx.x + 1) / gridDim.x;
+  const int pro = (Planes == 2 && j0 < j1 && j0 % nz != 0) ? 1 : 0;
+  const int64_t first = j0 - pro, count = j1 - first;
+  int band = (int)(first / nz), z = (int)(first - band * nz);     // item of stage i, advanced per stage
+  // thread 0: the next stage to issue, its item and its slot
+  int64_t issued = 0;
+  int issue_band = band, issue_z = z, issue_slot = 0;
+  auto issue_next = [&]() {
+    const int64_t y0 = (int64_t)issue_band * warps;
+    const int halo = y0 > 0 ? 1 : 0;
+    const unsigned bytes = (unsigned)((halo + min((int64_t)warps, sy - y0)) * row_bytes);
+    uint64_t* b = bar + issue_slot;
+    mbar_expect_tx(b, bytes);
+    bulk_load(reinterpret_cast<unsigned char*>(ring) + issue_slot * stage_bytes + (1 - halo) * row_bytes,
+              labels + ((int64_t)issue_z * sy + y0 - halo) * sx, bytes, b);
+    if (++issue_z == nz) { issue_z = 0; ++issue_band; }
+    if (++issue_slot == stages) issue_slot = 0;
+    ++issued;
+  };
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < stages; ++s) mbar_init(bar + s, 1);
+    while (issued < stages - 1 && issued < count) issue_next();
+  }
+  for (int i = threadIdx.x; i <= sx; i += blockDim.x) table_s[i] = __ldg(table + i);
+  if (threadIdx.x == 0) table_s[sx + 1] = __int_as_float(0x7f800000);
+  __syncthreads();
+
+  const unsigned lt_mask = (1u << lane) - 1u;
+  const unsigned gt_mask = (lane == 31) ? 0u : (0xfffffffeu << lane);
+  const bool keep_background = Plain ? false : (flags & kZeroLabel) != 0;
+  const int64_t wpr = (sx + 31) >> 5;
+  unsigned int nstarts = 0;                          // label changes along x seen by this lane
+
+  int slot = 0, prev_slot = stages - 1;
+  unsigned phase = 0;
+  for (int64_t i = 0; i < count; ++i) {
+    mbar_wait(bar + slot, phase);
+    const int64_t y = (int64_t)band * warps + warp;
+    if (i >= pro && y < sy) {
+      const int64_t line = z * sy + y;
+      // this row is row warp + 1 of its stage (row 0: the halo row y - 1)
+      const LT* cur = ring + (size_t)slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
+      const LT* back = ring + (size_t)prev_slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
+      first_axis_vec_row<Bytes, K, Plain>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); }, out + line * sx,
+                                          sx, table_s, border, flags, keep_background, lane, lt_mask, gt_mask,
+                                          nstarts);
+      // ---- run-start planes: compare with rows (y - 1, z) and (y, z - 1); one nibble per lane and
+      // block -> the row's wpr words, word c in lane c, stored by one instruction per plane ----
+      uint32_t word[Planes] = {};
+#pragma unroll
+      for (int b = 0; b < K; ++b) {
+        const int q0 = (b << 7) + (lane << 2);
+        const bool in_row = q0 < sx;
+        WT here[4], u[Planes][4];
+        if (in_row) {
+          load4_shared<Bytes>(cur + q0, here);
+          load4_shared<Bytes>(cur - sx + q0, u[0]);
+          if (Planes == 2) load4_shared<Bytes>(back + q0, u[Planes - 1]);
+        }
+#pragma unroll
+        for (int a = 0; a < Planes; ++a) {
+          uint32_t nib = in_row ? 15u : 0u;                       // first row along the axis: all start
+          if (in_row && (a == 0 ? y : z) > 0)
+            nib = (u[a][0] != here[0] ? 1u : 0u) | (u[a][1] != here[1] ? 2u : 0u) |
+                  (u[a][2] != here[2] ? 4u : 0u) | (u[a][3] != here[3] ? 8u : 0u);
+          // word w of block b sits in lanes 8w .. 8w + 7; lane c takes word c = 4 b + w
+          const uint32_t got = __shfl_sync(full, nibbles_to_word(nib, lane), (lane & 3) << 3);
+          if ((lane >> 2) == b) word[a] = got;
+        }
+      }
+      if (lane < wpr) {
+        planes.y[line * wpr + lane] = word[0];
+        if (Planes == 2) planes.z[line * wpr + lane] = word[Planes - 1];
+      }
+    }
+    __syncthreads();                                 // stage i - 1 is read by no one any more
+    if (threadIdx.x == 0 && issued < count) issue_next();   // stage i + S - 1, into the slot of i - 1
+    prev_slot = slot;
+    if (++slot == stages) { slot = 0; phase ^= 1u; }
+    if (++z == nz) { z = 0; ++band; }
+  }
+  if (stat.counter) {
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) nstarts += __shfl_xor_sync(full, nstarts, s);
+  }
+  publish_run_stat(stat, nstarts, lane);
 }
 
 // ---- lower-envelope machinery shared by the three stages of later_axis_tile_kernel ----

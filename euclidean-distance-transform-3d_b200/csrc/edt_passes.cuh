@@ -41,20 +41,56 @@ int launch_first_generic(const void* labels, float* f, int* codes, int64_t nline
   return 0;
 }
 
-// The register-resident X kernel for K 128-voxel blocks per row, with the run-start planes `planes`
-// asks for (only compiled for labels of 4 and 8 bytes and rows of at most 512 voxels, where
-// run_passes writes them: on 1024-voxel rows the kernel would spill at its register cap).
+// Shared memory of first_axis_planes_kernel with `warps` rows per band and a ring of `stages`.
+inline size_t planes_smem_bytes(int64_t sx, int label_bytes, int warps, int stages) {
+  return kPlaneBarBytes + (size_t)stages * (size_t)(warps + 1) * (size_t)sx * label_bytes +
+         sizeof(float) * (size_t)(sx + 2);
+}
+
+// The register-resident X kernel for K 128-voxel blocks per row; with `planes` (planes->y non-null)
+// the kernel that also writes them, compiled for labels of 4 and 8 bytes and rows of at most 512
+// voxels only, where run_passes takes them.
 template <int Bytes, int K, bool Plain>
-void launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, const float* table, int border,
-                      int flags, RunStat stat, const XPlanes& planes, unsigned blocks, size_t smem,
-                      cudaStream_t stream) {
+int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, const float* table, int border,
+                     int flags, RunStat stat, const XPlanes* planes, DeviceCache& dc, cudaStream_t stream) {
   using LT = typename LabelOf<Bytes>::type;
-  auto kern = first_axis_vec_kernel<Bytes, K, Plain, 0>;
-  if constexpr (Bytes >= 4 && K <= 4) {
-    if (planes.y) kern = planes.z ? first_axis_vec_kernel<Bytes, K, Plain, 2> : first_axis_vec_kernel<Bytes, K, Plain, 1>;
+  if (!planes) {
+    const size_t smem = sizeof(float) * (size_t)(sx + 2);
+    int64_t blocks = (nlines + 7) / 8;
+    const int64_t cap = (int64_t)dc.sm_count * (sx > 512 ? 12 : 15);   // whole waves at 5 (rows <= 512) / 3 CTAs per SM
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    first_axis_vec_kernel<Bytes, K, Plain><<<(unsigned)blocks, 256, smem, stream>>>(
+        static_cast<const LT*>(labels), f, nlines, (int)sx, table, border, flags, stat);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
   }
-  kern<<<blocks, 256, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table, border, flags, stat,
-                                      planes);
+  if constexpr (Bytes >= 4 && K <= 4) {
+    // Bands of 8 rows through a ring of 3 stages: 57 KB for 512-voxel rows of 4-byte labels, so
+    // three CTAs per SM, each with one to two stages (18 KB) of labels in flight.  Measured on the
+    // 512^3 label-noise transform, 6 or 4 rows per band and rings of 4 or 6 stages were slower.
+    // Fewer rows per band where the ring does not fit (it always does for rows of at most 512 voxels).
+    int warps = 8;
+    const int stages = 3;
+    while (warps > 1 && planes_smem_bytes(sx, Bytes, warps, stages) > (size_t)dc.max_smem_optin) warps >>= 1;
+    const size_t smem = planes_smem_bytes(sx, Bytes, warps, stages);
+    if (smem > (size_t)dc.max_smem_optin)
+      return fail(EDTB200_ELIMIT, "run-start planes of %lld-voxel rows exceed the shared memory", (long long)sx);
+    auto kern = planes->z ? first_axis_planes_kernel<Bytes, K, Plain, 2> : first_axis_planes_kernel<Bytes, K, Plain, 1>;
+    CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, warps * 32, smem));
+    // one persistent wave, the (band, z) items split evenly over it
+    const int64_t items = (planes->sy + warps - 1) / warps * (nlines / planes->sy);
+    int64_t blocks = (int64_t)dc.sm_count * (per_sm > 0 ? per_sm : 1);
+    if (blocks > items) blocks = items;
+    if (blocks < 1) blocks = 1;
+    kern<<<(unsigned)blocks, warps * 32, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table,
+                                                         border, flags, stat, *planes, stages);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+  }
+  return fail(EDTB200_EINVAL, "run-start planes asked of an X launch that cannot write them");
 }
 
 template <int Bytes>
@@ -70,30 +106,13 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
 
   // register-resident vector kernel when rows are short and 16-byte aligned
   if (first_is_vec(labels, Bytes, f, sx)) {
-    const size_t smem = sizeof(float) * (size_t)(sx + 2);
-    int64_t blocks = (nlines + 7) / 8;
-    const int64_t cap = (int64_t)dc.sm_count * (sx > 512 ? 12 : 15);   // whole waves at 5 (rows <= 512) / 3 CTAs per SM
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    XPlanes none;
-    memset(&none, 0, sizeof(none));
-    const XPlanes& pl = planes ? *planes : none;
 #define EDT_LAUNCH_VEC(KK)                                                                                        \
-  do {                                                                                                            \
-    if (flags == 0)                                                                                               \
-      launch_first_vec<Bytes, KK, true>(labels, f, nlines, sx, table, border, flags, stat, pl, (unsigned)blocks,   \
-                                        smem, stream);                                                            \
-    else                                                                                                          \
-      launch_first_vec<Bytes, KK, false>(labels, f, nlines, sx, table, border, flags, stat, pl, (unsigned)blocks,  \
-                                         smem, stream);                                                           \
-  } while (0)
-    if (sx <= 128)      EDT_LAUNCH_VEC(1);
-    else if (sx <= 256) EDT_LAUNCH_VEC(2);
-    else if (sx <= 512) EDT_LAUNCH_VEC(4);
-    else                EDT_LAUNCH_VEC(8);
+  (flags == 0 ? launch_first_vec<Bytes, KK, true>(labels, f, nlines, sx, table, border, flags, stat, planes, dc, stream) \
+              : launch_first_vec<Bytes, KK, false>(labels, f, nlines, sx, table, border, flags, stat, planes, dc, stream))
+    const int rc = sx <= 128 ? EDT_LAUNCH_VEC(1) : sx <= 256 ? EDT_LAUNCH_VEC(2) : sx <= 512 ? EDT_LAUNCH_VEC(4)
+                                                                                            : EDT_LAUNCH_VEC(8);
 #undef EDT_LAUNCH_VEC
-    CUDA_TRY(cudaGetLastError());
-    return step.queued();
+    return rc ? rc : step.queued();
   }
   const int rc = launch_first_generic<Bytes, false>(labels, f, nullptr, nlines, sx, table, border, flags, stat, dc,
                                                     stream);

@@ -87,6 +87,9 @@ def _lib():
   lib.edtb200_transform_chunked.restype = ci
   lib.edtb200_feature_transform.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
   lib.edtb200_feature_transform.restype = ci
+  lib.edtb200_feature_transform_chunked.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci,
+                                                    ctypes.c_size_t, vp]
+  lib.edtb200_feature_transform_chunked.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
   lib.edtb200_transform_multi.restype = ci
   lib.edtb200_transform_batch.argtypes = [vp, vp, ci, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, ci]
@@ -711,8 +714,11 @@ def _feature_anisotropy(dims, anisotropy):
   raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
 
 
-def _feature_host(data, anisotropy, black_border, flags, want_dist, device):
-  """(distances or None, indices) of a numpy array through host buffers (edtb200_feature_transform)."""
+def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_device_bytes=None):
+  """(distances or None, indices) of a numpy array through host buffers (edtb200_feature_transform).
+  `max_device_bytes` (an int) streams a 2-D / 3-D array through one GPU in chunks within that budget
+  (edtb200_feature_transform_chunked); with None a one-shot call that runs out of device memory is
+  retried once that way, as _transform_host does."""
   if isinstance(data, list):
     data = np.array(data)
   data = np.asarray(data)
@@ -732,9 +738,18 @@ def _feature_host(data, anisotropy, black_border, flags, want_dist, device):
     (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
     # x-fastest axis j is array axis j in F order, array axis nd - 1 - j in C order
     ptrs = (ctypes.c_void_p * nd)(*[planes[j if order == "F" else nd - 1 - j].ctypes.data for j in range(nd)])
-    _check(_lib().edtb200_feature_transform(
-      labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), int(flags),
-      dist.ctypes.data if want_dist else None, ptrs, int(device), None))
+    lib = _lib()
+    args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
+            int(flags), dist.ctypes.data if want_dist else None, ptrs, int(device))
+    if max_device_bytes is None:
+      try:
+        _check(lib.edtb200_feature_transform(*args, None))
+      except EDTError as e:
+        if e.code != ENOMEM or nd not in (2, 3):
+          raise
+        max_device_bytes = 0                  # too large for the device: stream it through in chunks
+    if max_device_bytes is not None:
+      _check(lib.edtb200_feature_transform_chunked(*args, int(max_device_bytes), None))
   indices = planes if order == "C" else planes.transpose((0,) + tuple(range(nd, 0, -1)))
   return (dist.reshape(data.shape, order=order) if want_dist else None), indices
 
@@ -773,7 +788,8 @@ def _feature_device(t, anisotropy, black_border, flags, want_dist):
   return dist, planes
 
 
-def feature_transform(data, anisotropy=None, black_border=False, *, signed=False, return_distances=False, device=0):
+def feature_transform(data, anisotropy=None, black_border=False, *, signed=False, return_distances=False, device=0,
+                      max_device_bytes=None):
   """The nearest site of every voxel: scipy.ndimage.distance_transform_edt(return_indices=True)
   for multi-label volumes, on the GPU.
 
@@ -789,13 +805,20 @@ def feature_transform(data, anisotropy=None, black_border=False, *, signed=False
   `return_distances=True` the pair (distances, indices), the distances equal to edt(data) (or
   sdf(data) with `signed=True`) bit for bit.  Arguments are handled as by edt(); device-resident
   input (a torch CUDA tensor or `__cuda_array_interface__`) returns torch CUDA tensors, computed on
-  the current stream."""
+  the current stream.
+
+  `max_device_bytes=N` streams a 2-D / 3-D host array through one GPU in chunks that fit N bytes of
+  device memory (0: what the GPU has free), with the one-shot result bit for bit; with None a one-shot
+  call that runs out of device memory falls back to that once."""
   flags = FLAG_SQRT | (FLAG_SIGNED if signed else 0)
   on_device = _device_array(data)
+  if max_device_bytes is not None:
+    dims = on_device.dim() if on_device is not None else np.ndim(data)
+    max_device_bytes = _chunk_budget(max_device_bytes, on_device is not None, None, dims)
   if on_device is not None:
     dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances)
   else:
-    dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device)
+    dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device, max_device_bytes)
   return (dist, idx) if return_distances else idx
 
 
@@ -808,25 +831,63 @@ def _same_size_signed(torch, t):
   return t
 
 
-def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0):
+def _expand_host(arr, distance, anisotropy, device, max_device_bytes):
+  """expand_labels of a contiguous numpy array through the chunked feature transform: the labels are
+  gathered on the host, a bounded range of voxels at a time, at the background voxels that grow."""
+  dist, idx = _feature_host(arr, anisotropy, False, FLAG_SIGNED, True, device, max_device_bytes)
+  order = "F" if arr.flags.f_contiguous and not arr.flags.c_contiguous else "C"
+  out = arr.copy(order=order)
+  # every array here is contiguous in `order`, so these flat views follow memory
+  lab, sq, flat_out = arr.ravel(order=order), dist.ravel(order=order), out.ravel(order=order)
+  planes = [idx[k].ravel(order=order) for k in range(arr.ndim)]
+  limit = float(distance) ** 2
+  step = 1 << 22
+  for s in range(0, lab.size, step):
+    e = min(lab.size, s + step)
+    grow = np.flatnonzero((lab[s:e] == 0) & (planes[0][s:e] >= 0) & (np.abs(sq[s:e]).astype(np.float64) <= limit))
+    if grow.size:
+      site = np.ravel_multi_index(tuple(p[s:e][grow] for p in planes), arr.shape, order=order)
+      flat_out[s + grow] = lab[site]
+  return out
+
+
+def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device_bytes=None):
   """skimage.segmentation.expand_labels on the GPU: every background voxel (label 0) whose nearest
   labelled voxel lies within `distance` takes that voxel's label; labelled voxels keep theirs.
   "Within" compares the squared distance (as sdfsq computes it, in float64) with distance**2.
   The result has the dtype, shape and memory order of `labels`; a torch CUDA tensor in gives one
-  out.  Built on feature_transform(signed=True): the labels are gathered on the device."""
+  out.  Built on feature_transform(signed=True): the labels are gathered on the device.
+
+  `max_device_bytes=N` (2-D / 3-D host arrays) runs the feature transform in chunks that fit N bytes
+  of device memory (0: what the GPU has free) and gathers the labels on the host; with None a host
+  array too large for the device falls back to that once."""
   import torch
   on_device = _device_array(labels)
   if on_device is None:
     arr = np.asarray(labels)
     if not arr.flags.c_contiguous and not arr.flags.f_contiguous:
       arr = np.ascontiguousarray(arr)
+    if max_device_bytes is not None:
+      max_device_bytes = _chunk_budget(max_device_bytes, False, None, arr.ndim)
     if _label_view(arr) is None:
       raise TypeError("expand_labels: unsupported label dtype %s" % arr.dtype)
-    raw = arr.view(np.uint8 if arr.dtype.itemsize == 1 else np.dtype("i%d" % arr.dtype.itemsize))
-    if arr.dtype.kind == "f":
-      raw = arr                              # folded by _feature_device and compared by value below
-    out = expand_labels(torch.from_numpy(raw).to(torch.device("cuda", int(device))), distance, anisotropy)
-    return out.cpu().numpy().view(arr.dtype)
+    if max_device_bytes is None:
+      raw = arr.view(np.uint8 if arr.dtype.itemsize == 1 else np.dtype("i%d" % arr.dtype.itemsize))
+      if arr.dtype.kind == "f":
+        raw = arr                            # folded by _feature_device and compared by value below
+      try:
+        out = expand_labels(torch.from_numpy(raw).to(torch.device("cuda", int(device))), distance, anisotropy)
+        return out.cpu().numpy().view(arr.dtype)
+      except (EDTError, torch.cuda.OutOfMemoryError) as e:
+        if getattr(e, "code", ENOMEM) != ENOMEM or arr.ndim not in (2, 3):
+          raise
+      torch.cuda.empty_cache()               # what the one-shot attempt left cached goes back to the device
+      max_device_bytes = 0                   # too large for the device: the chunked path
+    if arr.size == 0:
+      return arr.copy()
+    return _expand_host(arr, distance, anisotropy, device, max_device_bytes)
+  if max_device_bytes is not None:
+    _chunk_budget(max_device_bytes, True, None, on_device.dim())
   t = on_device
   if not t.is_contiguous() and not t.permute(*reversed(range(t.dim()))).is_contiguous():
     t = t.contiguous()

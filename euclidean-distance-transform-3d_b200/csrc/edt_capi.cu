@@ -1086,9 +1086,9 @@ int edtb200_transform_batch(const void* const* labels, float* const* outs, int c
 // ---- one host volume larger than the device, streamed through it in chunks -------------------
 namespace {
 
-// One phase of edtb200_transform_chunked (the plan of include/edt_b200.h): `extent` slices of
-// `slice_bytes` device bytes each, in `count` chunks of at most `most` slices (count 0: the budget
-// is below `need`, the least that works).
+// One phase of edtb200_transform_chunked / edtb200_feature_transform_chunked (the plans of
+// include/edt_b200.h): `extent` slices of `slice_bytes` device bytes each, in `count` chunks of at
+// most `most` slices (count 0: the budget is below `need`, the least that works).
 struct PhasePlan {
   int64_t extent = 0, count = 0, most = 0;
   size_t slice_bytes = 0, need = 0;
@@ -1096,12 +1096,12 @@ struct PhasePlan {
   int64_t size(int64_t k) const { return start(k + 1) - start(k); }
 };
 
-// extent slices of slice_vox voxels; a chunk holds at most `cap` slices; `long_line`: the phase's
-// later pass takes the long-line kernel (8 more bytes per voxel of scratch).
-PhasePlan plan_phase(int64_t extent, int64_t slice_vox, int label_bytes, int64_t cap, bool long_line, size_t budget) {
+// extent slices of slice_vox voxels that cost voxel_bytes device bytes per voxel each (a slot's
+// buffers and the phase's per-launch scratch); a chunk holds at most `cap` slices.
+PhasePlan plan_phase(int64_t extent, int64_t slice_vox, size_t voxel_bytes, int64_t cap, size_t budget) {
   PhasePlan p;
   p.extent = extent;
-  p.slice_bytes = (size_t)slice_vox * (size_t)(label_bytes + 4 + (long_line ? 8 : 0));
+  p.slice_bytes = (size_t)slice_vox * voxel_bytes;
   p.need = (size_t)(extent < 2 ? extent : 2) * p.slice_bytes;
   if (extent <= cap && (size_t)extent <= budget / p.slice_bytes) {
     p.count = 1;
@@ -1125,27 +1125,59 @@ void drop_volume_buffers(DeviceCache& dc) {
   cudaGetLastError();
 }
 
-// The slots of one phase: labels, then distances, in one scratch allocation each.
+// The slots of one phase: labels, then `planes` volumes of 4 bytes per voxel (distances, site codes,
+// coordinates), in one scratch allocation each.
 struct ChunkSlots {
   Scratch buf[2];
   void* labels[2] = {nullptr, nullptr};
-  float* dist[2] = {nullptr, nullptr};
-  int take(DeviceCache& dc, const PhasePlan& p, int64_t slice_vox, int label_bytes) {
-    const size_t vox = (size_t)p.most * (size_t)slice_vox;
-    const size_t lab = (vox * (size_t)label_bytes + 255) & ~size_t(255);
+  size_t lab = 0, vox = 0;
+  int take(DeviceCache& dc, const PhasePlan& p, int64_t slice_vox, int label_bytes, int planes) {
+    vox = (size_t)p.most * (size_t)slice_vox;
+    lab = (vox * (size_t)label_bytes + 255) & ~size_t(255);
+    const size_t bytes = lab + (size_t)planes * vox * 4;
     for (int i = 0; i < (p.count > 1 ? 2 : 1); ++i) {
-      if (buf[i].alloc(dc, lab + vox * sizeof(float), dc.stream) != cudaSuccess) {
+      if (buf[i].alloc(dc, bytes, dc.stream) != cudaSuccess) {
         cudaGetLastError();
         return fail(EDTB200_ENOMEM, "no device memory for a chunk slot of %zu bytes: give a smaller device_bytes",
-                    lab + vox * sizeof(float));
+                    bytes);
       }
       labels[i] = buf[i].get();
-      dist[i] = reinterpret_cast<float*>(buf[i].get<char>() + lab);
     }
     CUDA_TRY(cudaStreamSynchronize(dc.stream));   // allocated on the passes' stream, used on all three
     return 0;
   }
+  // volume j of slot `slot`
+  template <class T = float>
+  T* plane(int slot, int j) const { return reinterpret_cast<T*>(buf[slot].get<char>() + lab + (size_t)j * vox * 4); }
 };
+
+// The budget of a chunked call on a device whose host_call the caller holds: `device_bytes`, or with
+// 0 the memory free once the device's cached whole-volume buffers are dropped, less
+// EDTB200_CHUNK_RESERVE.  The buffers are dropped either way.
+int chunk_budget(DeviceCache& dc, size_t device_bytes, size_t* budget) {
+  drop_volume_buffers(dc);
+  *budget = device_bytes;
+  if (device_bytes == 0) {
+    size_t free_bytes = 0, total_bytes = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
+    *budget = free_bytes > EDTB200_CHUNK_RESERVE ? free_bytes - EDTB200_CHUNK_RESERVE : 0;
+  }
+  return 0;
+}
+
+// Phase-2 chunk k of plan p2 in a host volume of `bytes` per voxel: n_last rows of size(k) * unit
+// voxels, one row per index along the last axis, `plane` voxels apart.
+HostBox line_box(const void* base, const PhasePlan& p2, int64_t k, int64_t unit, int64_t plane, int64_t n_last,
+                 size_t bytes) {
+  return HostBox{static_cast<char*>(const_cast<void*>(base)) + (size_t)(p2.start(k) * unit) * bytes,
+                 (size_t)(p2.size(k) * unit) * bytes, (size_t)plane * bytes, (size_t)n_last};
+}
+
+// Whether host ranges [a, a + an) and [b, b + bn) share a byte.
+bool overlap(const void* a, size_t an, const void* b, size_t bn) {
+  const char *pa = static_cast<const char*>(a), *pb = static_cast<const char*>(b);
+  return pa < pb + bn && pb < pa + an;
+}
 
 }  // namespace
 
@@ -1168,21 +1200,15 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
   const char* lab_host = static_cast<const char*>(labels);
   char* out_host = reinterpret_cast<char*>(out);
-  if (lab_host < out_host + out_bytes && out_host < lab_host + lab_bytes)
-    return fail(EDTB200_EINVAL, "labels and out overlap");
+  if (overlap(lab_host, lab_bytes, out_host, out_bytes)) return fail(EDTB200_EINVAL, "labels and out overlap");
 
   DeviceGuard restore_device;
   DeviceCache* dcp = nullptr;
   if ((rc = probe(device, &dcp))) return rc;
   DeviceCache& dc = *dcp;
   std::lock_guard<std::mutex> host_call(dc.host_call);
-  drop_volume_buffers(dc);
-  size_t budget = device_bytes;
-  if (budget == 0) {
-    size_t free_bytes = 0, total_bytes = 0;
-    CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
-    budget = free_bytes > EDTB200_CHUNK_RESERVE ? free_bytes - EDTB200_CHUNK_RESERVE : 0;
-  }
+  size_t budget = 0;
+  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
 
   // Phase 1 cuts the last axis (z slabs in 3-D, row ranges in 2-D): X pass, and in 3-D the Y pass.
   // Phase 2 cuts the axis before it into boxes of whole lines along the last axis: the last pass.
@@ -1199,8 +1225,9 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
   const int64_t c2 = std::min(n_cut, cap2);
   const edtb200::LineGeom g2 = ndim == 3 ? geom_for_axis(2, sx, c2, sz) : geom_for_axis(1, c2, sy, 1);
   const bool long2 = later_pass_is_long(g2, transform_arith(t.w, t.n, last), dc.max_smem_optin);
-  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes, n_last, long1, budget);
-  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes, cap2, long2, budget);
+  // per voxel: the labels and the distances, and the long-line kernel's two scratch volumes
+  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes + 4 + (long1 ? 8 : 0), n_last, budget);
+  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes + 4 + (long2 ? 8 : 0), cap2, budget);
   if (p1.count == 0 || p2.count == 0)
     return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked transform needs at "
                                 "least %zu bytes", budget, std::max(p1.need, p2.need));
@@ -1211,7 +1238,7 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
   const auto t0 = std::chrono::steady_clock::now();
   {
     ChunkSlots slots;
-    if ((rc = slots.take(dc, p1, plane, label_bytes))) return rc;
+    if ((rc = slots.take(dc, p1, plane, label_bytes, 1))) return rc;
     PipelineSteps steps;
     steps.item = "phase-1 chunk";
     steps.upload = [&](int k, int slot, cudaStream_t s) {
@@ -1219,14 +1246,14 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
                     (size_t)(p1.size(k) * plane) * label_bytes, device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      int r = x_pass(t, slots.labels[slot], slots.dist[slot], plane / sx * p1.size(k), dc, s);
+      int r = x_pass(t, slots.labels[slot], slots.plane(slot, 0), plane / sx * p1.size(k), dc, s);
       if (!r && ndim == 3)                                  // behind our own X pass
-        r = later_pass(t, 1, slots.labels[slot], slots.dist[slot], geom_for_axis(1, sx, sy, p1.size(k)), border,
+        r = later_pass(t, 1, slots.labels[slot], slots.plane(slot, 0), geom_for_axis(1, sx, sy, p1.size(k)), border,
                        border, dc, s, /*pdl=*/true);
       return r;
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      return download(out + p1.start(k) * plane, slots.dist[slot], (size_t)(p1.size(k) * plane) * sizeof(float),
+      return download(out + p1.start(k) * plane, slots.plane(slot, 0), (size_t)(p1.size(k) * plane) * sizeof(float),
                       device, s);
     };
     if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
@@ -1234,26 +1261,22 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
   const auto t1 = std::chrono::steady_clock::now();
   {
     ChunkSlots slots;
-    if ((rc = slots.take(dc, p2, line_vox, label_bytes))) return rc;
-    // chunk k: n_last rows of size(k) * unit voxels, one row per index along the last axis
-    auto box = [&](const char* base, int64_t k, int bytes) {
-      return HostBox{const_cast<char*>(base) + (size_t)(p2.start(k) * unit) * bytes,
-                     (size_t)(p2.size(k) * unit) * bytes, (size_t)plane * bytes, (size_t)n_last};
-    };
+    if ((rc = slots.take(dc, p2, line_vox, label_bytes, 1))) return rc;
+    auto box = [&](const void* base, int64_t k, size_t bytes) { return line_box(base, p2, k, unit, plane, n_last, bytes); };
     PipelineSteps steps;
     steps.item = "phase-2 chunk";
     steps.upload_writes_results = true;            // the intermediate distances go up into the slot
     steps.upload = [&](int k, int slot, cudaStream_t s) {
       int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
-      return r ? r : upload_box(slots.dist[slot], box(out_host, k, sizeof(float)), device, s);
+      return r ? r : upload_box(slots.plane(slot, 0), box(out_host, k, sizeof(float)), device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
       const int64_t c = p2.size(k);
       const edtb200::LineGeom g = ndim == 3 ? geom_for_axis(2, sx, c, sz) : geom_for_axis(1, c, sy, 1);
-      return later_pass(t, last, slots.labels[slot], slots.dist[slot], g, border, border, dc, s, /*pdl=*/false);
+      return later_pass(t, last, slots.labels[slot], slots.plane(slot, 0), g, border, border, dc, s, /*pdl=*/false);
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      return download_box(box(out_host, k, sizeof(float)), slots.dist[slot], device, s);
+      return download_box(box(out_host, k, sizeof(float)), slots.plane(slot, 0), device, s);
     };
     if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
   }
@@ -1265,6 +1288,145 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
                     "phase 1 %.1f ms  phase 2 %.1f ms\n",
             (long long)sx, (long long)sy, (long long)sz, label_bytes, budget, (long long)p1.count, (long long)p2.count,
             (2.0 * label_bytes + 4.0) * (double)total / 1e9, 8.0 * (double)total / 1e9, ms1, ms2);
+  }
+  return 0;
+}
+
+int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy,
+                                      int64_t sz, float wx, float wy, float wz, int black_border, int flags,
+                                      float* dist_out, int32_t* const* idx_out, int device, size_t device_bytes,
+                                      int64_t* chunks) {
+  if (chunks) chunks[0] = chunks[1] = 0;
+  if (flags & (EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_feature_transform_chunked streams HOST buffers through the device; a volume "
+                                "on the device fits it: use edtb200_feature_transform");
+  if (ndim != 2 && ndim != 3)
+    return fail(EDTB200_EINVAL, "edtb200_feature_transform_chunked needs a 2-D or 3-D volume (got ndim %d)", ndim);
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  const int64_t total = sx * sy * sz;
+  if (total == 0) return 0;
+  if (!labels || !idx_out) return fail(EDTB200_EINVAL, "null pointer");
+  for (int k = 0; k < ndim; ++k)
+    if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, vol_bytes = (size_t)total * sizeof(float);
+  {
+    struct { const void* p; size_t n; const char* name; } host[5] = {
+        {labels, lab_bytes, "labels"}, {dist_out, vol_bytes, "dist_out"}, {idx_out[0], vol_bytes, "index plane 0"},
+        {idx_out[1], vol_bytes, "index plane 1"}, {ndim == 3 ? idx_out[2] : nullptr, vol_bytes, "index plane 2"}};
+    for (int i = 0; i < 5; ++i)
+      for (int j = i + 1; j < 5; ++j)
+        if (host[i].p && host[j].p && overlap(host[i].p, host[i].n, host[j].p, host[j].n))
+          return fail(EDTB200_EINVAL, "%s and %s overlap", host[i].name, host[j].name);
+  }
+
+  DeviceGuard restore_device;
+  DeviceCache* dcp = nullptr;
+  if ((rc = probe(device, &dcp))) return rc;
+  DeviceCache& dc = *dcp;
+  std::lock_guard<std::mutex> host_call(dc.host_call);
+  size_t budget = 0;
+  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+
+  // The phases of edtb200_transform_chunked, on the site-tracking passes.  Phase 1 resolves every
+  // voxel's site within its slice (3-D: (qx, qy); 2-D: the X code, qx), phase 2 follows the last
+  // axis's code to the partial site on the voxel's own line, which lies in the same chunk.
+  const int border = black_border != 0;
+  const bool zero_bg = !(flags & EDTB200_SIGNED);
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
+  const int last = ndim - 1;
+  const int64_t n_last = t.n[last], n_cut = t.n[last - 1];
+  const int64_t plane = total / n_last;                    // voxels of one phase-1 slice
+  const int64_t unit = ndim == 3 ? sx : 1;                 // voxels of one phase-2 slice per row
+  const int64_t line_vox = unit * n_last;                  // voxels of one phase-2 slice
+  // Slot volumes (4 bytes per voxel each) beside the labels:
+  //   phase 1, 3-D  0 X distances, then qx; 1 Y distances; 2 X codes; 3 Y codes, then qy
+  //   phase 1, 2-D  0 X distances; 1 X codes (= qx)
+  //   phase 2       0 intermediate distances, then x; 1 distances; 2 qx; 3 qy (3-D); `codes` the last
+  //                 axis's codes, then its coordinate; 5 y (3-D)
+  // and per launch of a later pass the long-line kernel's hull, 4 bytes per voxel of the chunk.
+  const int planes1 = ndim == 3 ? 4 : 2, planes2 = ndim == 3 ? 6 : 4, codes = ndim == 3 ? 4 : 3;
+  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes + 4 * planes1 + (ndim == 3 ? 4 : 0), n_last, budget);
+  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes + 4 * planes2 + 4, n_cut, budget);
+  if (p1.count == 0 || p2.count == 0)
+    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked feature transform "
+                                "needs at least %zu bytes", budget, std::max(p1.need, p2.need));
+  if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
+  if ((rc = pipeline_streams(dc))) return rc;
+
+  const char* lab_host = static_cast<const char*>(labels);
+  // the intermediate distances: dist_out, or bit-cast in the last axis's index plane, which phase 2
+  // reads them from before it writes that plane
+  float* mid = dist_out ? dist_out : reinterpret_cast<float*>(idx_out[last]);
+  {
+    ChunkSlots slots;
+    if ((rc = slots.take(dc, p1, plane, label_bytes, planes1))) return rc;
+    PipelineSteps steps;
+    steps.item = "phase-1 chunk";
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      return upload(slots.labels[slot], lab_host + (size_t)(p1.start(k) * plane) * label_bytes,
+                    (size_t)(p1.size(k) * plane) * label_bytes, device, s);
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      const int64_t c = p1.size(k);
+      const void* lab = slots.labels[slot];
+      return with_label_width(label_bytes, [&](auto b) {
+        int r = launch_first_sites<b>(lab, slots.plane(slot, 0), slots.plane<int>(slot, ndim == 3 ? 2 : 1),
+                                      plane / sx * c, sx, wx, border, kernel_flags(flags, true, false), dc, s);
+        if (r || ndim == 2) return r;
+        r = launch_later_sites<b>(lab, slots.plane(slot, 0), slots.plane(slot, 1), slots.plane<int>(slot, 3),
+                                  geom_for_axis(1, sx, sy, c), wy, border, border, kernel_flags(flags, false, false),
+                                  transform_arith(t.w, t.n, 1), dc, s);
+        return r ? r : launch_slice_sites<b>(lab, slots.plane<int>(slot, 2), slots.plane<int>(slot, 3), sx, sy, c,
+                                             zero_bg, slots.plane<int32_t>(slot, 0), dc, s);
+      });
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      const int64_t off = p1.start(k) * plane;
+      const size_t bytes = (size_t)(p1.size(k) * plane) * sizeof(float);
+      int r = download(mid + off, slots.plane(slot, ndim == 3 ? 1 : 0), bytes, device, s);
+      if (!r) r = download(idx_out[0] + off, slots.plane(slot, ndim == 3 ? 0 : 1), bytes, device, s);
+      if (!r && ndim == 3) r = download(idx_out[1] + off, slots.plane(slot, 3), bytes, device, s);
+      return r;
+    };
+    if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
+  }
+  {
+    ChunkSlots slots;
+    if ((rc = slots.take(dc, p2, line_vox, label_bytes, planes2))) return rc;
+    auto box = [&](const void* base, int64_t k, size_t bytes) { return line_box(base, p2, k, unit, plane, n_last, bytes); };
+    PipelineSteps steps;
+    steps.item = "phase-2 chunk";
+    steps.upload_writes_results = true;            // volume 0 goes up and comes back down as x
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
+      if (!r) r = upload_box(slots.plane(slot, 0), box(mid, k, sizeof(float)), device, s);
+      for (int a = 0; !r && a < ndim - 1; ++a) r = upload_box(slots.plane(slot, 2 + a), box(idx_out[a], k, 4), device, s);
+      return r;
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      const int64_t c = p2.size(k);
+      const edtb200::LineGeom g = ndim == 3 ? geom_for_axis(2, sx, c, sz) : geom_for_axis(1, c, sy, 1);
+      const edtb200::SiteBox sb{ndim, ndim == 3 ? sx : c, unit * c, n_last, p2.start(k)};
+      const void* lab = slots.labels[slot];
+      return with_label_width(label_bytes, [&](auto b) {
+        const int r = launch_later_sites<b>(lab, slots.plane(slot, 0), slots.plane(slot, 1),
+                                            slots.plane<int>(slot, codes), g, t.w[last], border, border,
+                                            kernel_flags(flags, false, true), transform_arith(t.w, t.n, last), dc, s);
+        return r ? r : launch_compose_sites<b>(lab, slots.plane<int>(slot, codes), slots.plane<int32_t>(slot, 2),
+                                               ndim == 3 ? slots.plane<int32_t>(slot, 3) : nullptr, sb, zero_bg,
+                                               slots.plane<int32_t>(slot, 0),
+                                               ndim == 3 ? slots.plane<int32_t>(slot, 5) : nullptr, dc, s);
+      });
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      int r = dist_out ? download_box(box(dist_out, k, sizeof(float)), slots.plane(slot, 1), device, s) : 0;
+      if (!r) r = download_box(box(idx_out[0], k, 4), slots.plane(slot, 0), device, s);
+      if (!r && ndim == 3) r = download_box(box(idx_out[1], k, 4), slots.plane(slot, 5), device, s);
+      if (!r) r = download_box(box(idx_out[last], k, 4), slots.plane(slot, codes), device, s);
+      return r;
+    };
+    if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
   }
   return 0;
 }

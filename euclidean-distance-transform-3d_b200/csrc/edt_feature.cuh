@@ -10,6 +10,10 @@
 // codes belong to another label and must not be followed.  The voxels the chain visits all carry
 // p's label, so the chain never meets a code of another run.  The code planes are read at other
 // voxels than the one written, so they are scratch, separate from the output planes.
+//
+// The chunked feature transform follows the same chain in two halves: slice_sites_kernel resolves
+// the X and Y codes of whole slices into each voxel's site within its slice, and compose_sites_kernel
+// follows the last axis's code to one of those partial sites on the voxel's own line.
 #pragma once
 #include "edt_kernels.cuh"
 
@@ -25,6 +29,19 @@ struct SitePlanes {
   int32_t* axis[3];       // x, y, z coordinate planes (the first ndim are written)
 };
 
+// What one later pass's site code says about a voxel's site along that axis.
+//   kStepSelf    the voxel is unsigned background, its own site (its code is not followed)
+//   kStepNone    no site at all (the distance is +inf)
+//   kStepDirect  the site is at `row` on this line: the voxel just outside the run (or a face)
+//   kStepVertex  the site is the site of the voxel at `row` on this line, found by the earlier axes
+enum : int { kStepSelf, kStepNone, kStepDirect, kStepVertex };
+__device__ __forceinline__ int site_step(bool self, int code, int* row) {
+  if (self) return kStepSelf;
+  if (code == kSiteNone) return kStepNone;
+  *row = code < 0 ? site_direct_row(code) : code;
+  return code < 0 ? kStepDirect : kStepVertex;
+}
+
 // zero_is_background: label 0 is background, whose site is the voxel itself (edt, unsigned);
 // otherwise (sdf) background is an ordinary label and is resolved like any other.
 template <int Bytes>
@@ -39,28 +56,100 @@ resolve_sites_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, S
     const int64_t py = rem / c.sx;
     const int64_t px = rem - py * c.sx;
     int64_t q[3] = {px, py, pz};
-    if (!(zero_is_background && labels[i] == 0)) {
-      bool direct = false, none = false;
-      if (c.ndim == 3) {
-        const int code = __ldg(c.axis[2] + i);
-        if (code == kSiteNone) none = true;
-        else if (code < 0) { q[2] = site_direct_row(code); direct = true; }
-        else q[2] = code;
-      }
-      if (c.ndim >= 2 && !direct && !none) {
-        const int code = __ldg(c.axis[1] + px + c.sx * (py + c.sy * q[2]));
-        if (code == kSiteNone) none = true;
-        else if (code < 0) { q[1] = site_direct_row(code); direct = true; }
-        else q[1] = code;
-      }
-      if (!direct && !none) {
-        const int code = __ldg(c.axis[0] + px + c.sx * (q[1] + c.sy * q[2]));
-        if (code == kSiteNone) none = true;
-        else q[0] = code;
-      }
-      if (none) q[0] = q[1] = q[2] = -1;
+    const bool self = zero_is_background && labels[i] == 0;
+    int step = self ? kStepSelf : kStepVertex;
+#pragma unroll
+    for (int k = 2; k >= 1; --k) {
+      if (k >= c.ndim || step != kStepVertex) continue;
+      int row = 0;
+      step = site_step(false, __ldg(c.axis[k] + px + c.sx * (q[1] + c.sy * q[2])), &row);
+      if (step != kStepNone) q[k] = row;
     }
-    for (int k = 0; k < c.ndim; ++k) out.axis[k][i] = (int32_t)q[k];
+    if (step == kStepVertex) {
+      const int code = __ldg(c.axis[0] + px + c.sx * (q[1] + c.sy * q[2]));
+      if (code == kSiteNone) step = kStepNone;
+      else q[0] = code;
+    }
+    if (step == kStepNone) q[0] = q[1] = q[2] = -1;
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      if (k < c.ndim) out.axis[k][i] = (int32_t)q[k];
+  }
+}
+
+// Chunked feature transform, phase 1 (3-D): the X and Y codes of a slab of whole slices
+// (sx, sy, sz) -> every voxel's site (qx, qy) within its own slice, kSiteNone in both where it has
+// none.  qy is written over the Y codes (each is read at its own voxel only); the X codes are read at
+// other rows, so qx goes to a separate plane.
+template <int Bytes>
+__global__ void __launch_bounds__(256)
+slice_sites_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, const int* __restrict__ xcodes,
+                   int* ycodes_qy, int64_t sx, int64_t sy, int64_t sz, int zero_is_background,
+                   int32_t* __restrict__ qx) {
+  const int64_t total = sx * sy * sz;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t line = i / sx;                 // y + sy * z
+    const int64_t px = i - line * sx;
+    const int64_t py = line % sy;
+    int row = 0;
+    const int step = site_step(zero_is_background && labels[i] == 0, ycodes_qy[i], &row);
+    int x = (int)px, y = (int)py;
+    if (step == kStepNone) {
+      x = y = kSiteNone;
+    } else if (step != kStepSelf) {
+      y = row;
+      if (step == kStepVertex) {
+        x = __ldg(xcodes + i + sx * ((int64_t)row - py));
+        if (x == kSiteNone) y = kSiteNone;
+      }
+    }
+    qx[i] = x;
+    ycodes_qy[i] = y;
+  }
+}
+
+// The box of whole lines along the last axis that one phase-2 chunk covers: `plane` voxels per
+// position along those lines (3-D: width * the box's y extent; 2-D: its x extent), lines of n voxels.
+// `origin` is the box's first index along the cut axis (3-D: y; 2-D: x) in the volume.
+struct SiteBox {
+  int ndim;
+  int64_t width, plane, n, origin;
+};
+
+// Chunked feature transform, phase 2: the last axis's codes -> every voxel's site in the volume.  A
+// vertex code names a row of the voxel's own line, whose partial site (px, py) came from phase 1
+// (part_x, part_y; kSiteNone: none); a direct code names the row on the voxel's own line.  The last
+// axis's coordinate is written over its codes (each read at its own voxel only); the partial planes
+// are read at other rows, so x (and y in 3-D) go to separate planes.
+template <int Bytes>
+__global__ void __launch_bounds__(256)
+compose_sites_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, int* codes_last,
+                     const int32_t* __restrict__ part_x, const int32_t* __restrict__ part_y, SiteBox b,
+                     int zero_is_background, int32_t* __restrict__ out_x, int32_t* __restrict__ out_y) {
+  const int64_t total = b.plane * b.n;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t pos = i / b.plane;             // along the last axis
+    const int64_t base = i - pos * b.plane;
+    const int64_t a = base % b.width;
+    // the voxel's own coordinates in the volume; in 2-D base is the x index in the box
+    int x = b.ndim == 3 ? (int)a : (int)(a + b.origin), y = (int)(base / b.width + b.origin);
+    int row = 0;
+    const int step = site_step(zero_is_background && labels[i] == 0, codes_last[i], &row);
+    int last = (int)pos;
+    if (step == kStepNone) {
+      x = y = last = -1;
+    } else if (step != kStepSelf) {
+      last = row;
+      if (step == kStepVertex) {
+        const int64_t j = base + (int64_t)row * b.plane;
+        x = __ldg(part_x + j);
+        if (b.ndim == 3) y = __ldg(part_y + j);
+        if (x == kSiteNone) x = y = last = -1;
+      }
+    }
+    out_x[i] = x;
+    if (b.ndim == 3) out_y[i] = y;
+    codes_last[i] = last;
   }
 }
 

@@ -8,6 +8,7 @@
 #pragma once
 #include "../../include/edt_b200.h"
 #include "edt_kernels.cuh"
+#include "edt_feature.cuh"       // SiteBox
 
 #include <condition_variable>
 #include <cstdint>
@@ -201,6 +202,16 @@ int launch_later_sites(const void* labels, const float* fin, float* fout, int* c
 template <int Bytes>
 int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim, int64_t sx, int64_t sy,
                          int64_t sz, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
+                         cudaStream_t stream);
+// The two halves of that resolution for the chunked feature transform (edt_feature.cuh): phase 1
+// resolves the X and Y codes of a slab into sites within each slice, phase 2 follows the last axis's
+// codes of a box of whole lines to those partial sites.
+template <int Bytes>
+int launch_slice_sites(const void* labels, const int* xcodes, int* ycodes_qy, int64_t sx, int64_t sy, int64_t sz,
+                       bool zero_is_background, int32_t* qx, DeviceCache& dc, cudaStream_t stream);
+template <int Bytes>
+int launch_compose_sites(const void* labels, int* codes_last, const int32_t* part_x, const int32_t* part_y,
+                         const SiteBox& box, bool zero_is_background, int32_t* out_x, int32_t* out_y, DeviceCache& dc,
                          cudaStream_t stream);
 
 // Whether plan_later (edt_passes.cuh) sends a later-axis pass over geometry g with arithmetic

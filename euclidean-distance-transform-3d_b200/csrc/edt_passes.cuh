@@ -360,6 +360,38 @@ int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim
   return 0;
 }
 
+// Grid of the chunked feature transform's site kernels: one thread per voxel, at most 8 CTAs per SM
+// (grid-stride loops beyond), as launch_resolve_sites.
+inline unsigned site_blocks(int64_t total, const DeviceCache& dc) {
+  const int64_t blocks = (total + 255) / 256, cap = (int64_t)dc.sm_count * 8;
+  return (unsigned)(blocks < 1 ? 1 : blocks > cap ? cap : blocks);
+}
+
+// Chunked feature transform, phase 1 in 3-D: the X and Y codes of a slab -> each voxel's site within
+// its slice (edt_feature.cuh); qy over the Y codes, qx into its own plane.
+template <int Bytes>
+int launch_slice_sites(const void* labels, const int* xcodes, int* ycodes_qy, int64_t sx, int64_t sy, int64_t sz,
+                       bool zero_is_background, int32_t* qx, DeviceCache& dc, cudaStream_t stream) {
+  slice_sites_kernel<Bytes><<<site_blocks(sx * sy * sz, dc), 256, 0, stream>>>(
+      static_cast<const typename LabelOf<Bytes>::type*>(labels), xcodes, ycodes_qy, sx, sy, sz,
+      zero_is_background ? 1 : 0, qx);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
+// Chunked feature transform, phase 2: the last axis's codes of a box of whole lines and the partial
+// sites of phase 1 -> each voxel's site (edt_feature.cuh); the last coordinate over the codes.
+template <int Bytes>
+int launch_compose_sites(const void* labels, int* codes_last, const int32_t* part_x, const int32_t* part_y,
+                         const SiteBox& box, bool zero_is_background, int32_t* out_x, int32_t* out_y, DeviceCache& dc,
+                         cudaStream_t stream) {
+  compose_sites_kernel<Bytes><<<site_blocks(box.plane * box.n, dc), 256, 0, stream>>>(
+      static_cast<const typename LabelOf<Bytes>::type*>(labels), codes_last, part_x, part_y, box,
+      zero_is_background ? 1 : 0, out_x, out_y);
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace host
 }  // namespace edtb200
 
@@ -379,4 +411,9 @@ int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim
                                                     edtb200::host::DeviceCache&, cudaStream_t);          \
   template int edtb200::host::launch_resolve_sites<B>(const void*, const int* const*, int, int64_t,      \
                                                       int64_t, int64_t, bool, int32_t* const*,           \
+                                                      edtb200::host::DeviceCache&, cudaStream_t);        \
+  template int edtb200::host::launch_slice_sites<B>(const void*, const int*, int*, int64_t, int64_t, int64_t, \
+                                                    bool, int32_t*, edtb200::host::DeviceCache&, cudaStream_t); \
+  template int edtb200::host::launch_compose_sites<B>(const void*, int*, const int32_t*, const int32_t*,  \
+                                                      const edtb200::SiteBox&, bool, int32_t*, int32_t*, \
                                                       edtb200::host::DeviceCache&, cudaStream_t);

@@ -34,7 +34,8 @@ extern "C" {
  * edtb200_transform_multi, edtb200_slab_step / _stage_bytes / _pack, edtb200_label_stats / _extract,
  * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
- * Entry points added since (edtb200_transform_chunked) keep the number: every 202-level entry point
+ * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked) keep the
+ * number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up. */
 #define EDTB200_VERSION 202
 
@@ -201,6 +202,50 @@ int edtb200_transform_chunked(const void *labels, int label_bytes, int ndim,
                               float wx, float wy, float wz,
                               int black_border, int flags, float *out,
                               int device, size_t device_bytes, int64_t *chunks);
+
+/* The same feature transform as edtb200_feature_transform for a 2-D or 3-D HOST volume larger than
+ * the device's memory, streamed through one device in the two phases of edtb200_transform_chunked;
+ * the distances and every index plane are edtb200_feature_transform's bit for bit.
+ *
+ * The site chain splits along the same phases: the last axis's code at p names a row of p's own line
+ * (or no site), and the codes of the first axes at that row only touch its slice.
+ *   phase 1  z slabs (3-D) / row ranges (2-D): the labels go up, the site-tracking X pass (and in 3-D
+ *            the Y pass) runs, and every voxel's site within its slice is resolved -- (qx, qy) in 3-D,
+ *            qx in 2-D -- and comes down with the intermediate distances: qx into idx_out[0], qy into
+ *            idx_out[1], the distances into dist_out (when NULL: bit-cast into idx_out[ndim - 1], which
+ *            phase 2 reads them from before it writes it).  "No site" stays apart from a face
+ *            coordinate -1 in those planes until phase 2 turns it into -1;
+ *   phase 2  y ranges of whole z lines (3-D) / x ranges of whole y lines (2-D): the labels, the
+ *            intermediate distances and the partial sites go up, the last pass runs with the sqrt /
+ *            sign epilogue, and each voxel's code along the last axis is followed to the partial site
+ *            on its own line; the index planes (and the distances when dist_out is given) come down.
+ * Every pass sees whole lines with the whole volume's weights and extents, so the site codes are the
+ * one-shot codes.  Both phases pipeline their chunks through two device slots.  PCIe traffic per
+ * voxel, in 3-D with distances: (2 label_bytes + 12) bytes up and 28 down, against label_bytes and 16
+ * for edtb200_feature_transform (2-D: 2 label_bytes + 8 up, 20 down): this is for volumes that do not
+ * fit.
+ *
+ * The plan is edtb200_transform_chunked's (slice, chunks, count; the ENOMEM message names the least
+ * budget that works) with these bytes per voxel, each slot's buffers plus the later pass's hull
+ * scratch of 4 bytes (every feature pass runs on the long-line kernel, so there is no phase-2 cap):
+ *   phase 1  3-D: label_bytes + 20 (two distance volumes, two code planes, hull); 2-D: label_bytes + 8
+ *            (distances, X codes; no later pass);
+ *   phase 2  3-D: label_bytes + 28 (intermediate and final distances, two partial site planes, the Z
+ *            codes, one more index plane, hull); 2-D: label_bytes + 20 (the same without qy and the
+ *            extra plane).
+ *
+ *   labels, dist_out, idx_out[0..ndim)  HOST buffers, pageable or pinned, no two of which overlap;
+ *                 dist_out may be NULL, no index plane may.  flags: EDTB200_SQRT / EDTB200_SIGNED;
+ *                 the *_ON_DEVICE flags are rejected.  ndim is 2 or 3.
+ *   device_bytes, chunks  as for edtb200_transform_chunked.
+ * Returns when the result has landed; after an error the contents of the outputs are unspecified.
+ * Calls on one device are serialised. */
+int edtb200_feature_transform_chunked(const void *labels, int label_bytes, int ndim,
+                                      int64_t sx, int64_t sy, int64_t sz,
+                                      float wx, float wy, float wz,
+                                      int black_border, int flags, float *dist_out,
+                                      int32_t *const *idx_out, int device,
+                                      size_t device_bytes, int64_t *chunks);
 
 /* Transform under a voxel connectivity graph (2-D or 3-D only).
  *

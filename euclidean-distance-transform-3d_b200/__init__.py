@@ -96,6 +96,9 @@ def _lib():
   lib.edtb200_transform_batch.restype = ci
   lib.edtb200_transform_voxel_graph.argtypes = [vp, ci, vp, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp]
   lib.edtb200_transform_voxel_graph.restype = ci
+  lib.edtb200_transform_voxel_graph_chunked.argtypes = [vp, ci, vp, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci,
+                                                        ctypes.c_size_t, vp]
+  lib.edtb200_transform_voxel_graph_chunked.restype = ci
   lib.edtb200_pass_first.argtypes = [vp, ci, i64, i64, i64, f32, ci, ci, vp, ci, vp]
   lib.edtb200_pass_first.restype = ci
   lib.edtb200_pass_later.argtypes = [vp, ci, ci, i64, i64, i64, f32, ci, ci, ci, vp, ci, vp]
@@ -316,7 +319,9 @@ def _graph_bytes(voxel_graph, order):
 
 
 def _transform_voxel_graph_host(data, voxel_graph, anisotropy, black_border, flags, device):
-  """__edt2dsq_voxel_graph / __edt3dsq_voxel_graph, src/edt.pyx:514-620, 736-844."""
+  """__edt2dsq_voxel_graph / __edt3dsq_voxel_graph, src/edt.pyx:514-620, 736-844.  A one-shot call
+  that runs out of device memory is retried once through edtb200_transform_voxel_graph_chunked, with
+  the budget the device has free."""
   order = "F" if data.flags.f_contiguous else "C"
   if not data.flags.c_contiguous and not data.flags.f_contiguous:
     data = np.ascontiguousarray(data)
@@ -336,9 +341,16 @@ def _transform_voxel_graph_host(data, voxel_graph, anisotropy, black_border, fla
   out = np.empty(data.size, dtype=np.float32)
   if isinstance(device, (list, tuple)):
     device = device[0]                      # the graph transform runs on one GPU
-  _check(_lib().edtb200_transform_voxel_graph(
-    labels.ctypes.data, labels.dtype.itemsize, graph.ctypes.data, data.ndim, sx, sy, sz, wx, wy, wz,
-    int(bool(black_border)), int(flags), out.ctypes.data, int(device), None))
+  lib = _lib()
+  args = (labels.ctypes.data, labels.dtype.itemsize, graph.ctypes.data, data.ndim, sx, sy, sz, wx, wy, wz,
+          int(bool(black_border)), int(flags), out.ctypes.data, int(device))
+  try:
+    _check(lib.edtb200_transform_voxel_graph(*args, None))
+  except EDTError as e:
+    if e.code != ENOMEM:
+      raise
+    # the doubled grid does not fit the device: stream it through in chunks
+    _check(lib.edtb200_transform_voxel_graph_chunked(*args, 0, None))
   return out.reshape(data.shape, order=order)
 
 

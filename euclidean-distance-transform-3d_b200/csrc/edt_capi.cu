@@ -18,6 +18,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <functional>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <vector>
@@ -1479,7 +1480,8 @@ int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const uns
   const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
   uint8_t* cells = d_cells.get<uint8_t>();
   rc = with_label_width(label_bytes, [&](auto b) {
-    voxel_graph_expand_kernel<b><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float);
+    voxel_graph_expand_kernel<b><<<blocks, threads, 0, stream>>>(lab, gr, cells, sx, sy, sz, ndim, border, as_float,
+                                                                 sy - 1, sz - 1);
     CUDA_TRY(cudaGetLastError());
     return 0;
   });
@@ -1488,10 +1490,175 @@ int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const uns
   rc = run_passes(cells, 1, ndim, sx2, sy2, sz2, wx / 2, wy / 2, wz / 2, border, 0, d_doubled.get<float>(), *dc,
                   stream);
   if (rc) return rc;
-  voxel_graph_gather_kernel<<<blocks, threads, 0, stream>>>(d_doubled.get<const float>(), result, sx, sy, sz,
-                                                            (flags & EDTB200_SQRT) ? 1 : 0);
+  voxel_graph_gather_kernel<<<blocks, threads, 0, stream>>>(d_doubled.get<const float>(), result, sx, sy, sz, 2,
+                                                            4 * sx, 8 * sx * sy, (flags & EDTB200_SQRT) ? 1 : 0);
   CUDA_TRY(cudaGetLastError());
   return io.finish();
+}
+
+int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, const unsigned char* graph, int ndim,
+                                          int64_t sx, int64_t sy, int64_t sz, float wx, float wy, float wz,
+                                          int black_border, int flags, float* out, int device, size_t device_bytes,
+                                          int64_t* chunks) {
+  using namespace edtb200;
+  if (chunks) chunks[0] = chunks[1] = 0;
+  if (flags & (EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_transform_voxel_graph_chunked streams HOST buffers through the device; a "
+                                "volume on the device fits it: use edtb200_transform_voxel_graph");
+  if (ndim != 2 && ndim != 3)
+    return fail(EDTB200_EINVAL, "a voxel graph needs a 2-D or 3-D volume (got ndim %d)", ndim);
+  if (flags & EDTB200_SIGNED)
+    return fail(EDTB200_EINVAL, "EDTB200_SIGNED is not defined with a voxel graph: subtract two transforms");
+  if ((flags & EDTB200_LABELS_FLOAT) && label_bytes != 4 && label_bytes != 8)
+    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  const int64_t total = sx * sy * sz;
+  if (total == 0) return 0;
+  if (!labels || !graph || !out) return fail(EDTB200_EINVAL, "null pointer");
+  int64_t sx2 = 2 * sx, sy2 = 2 * sy, sz2 = ndim == 3 ? 2 * sz : 1;
+  if ((rc = check_dims(1, ndim, sx2, sy2, sz2))) return rc;
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
+  if (overlap(labels, lab_bytes, out, out_bytes)) return fail(EDTB200_EINVAL, "labels and out overlap");
+  if (overlap(graph, (size_t)total, out, out_bytes)) return fail(EDTB200_EINVAL, "graph and out overlap");
+
+  DeviceGuard restore_device;
+  DeviceCache* dcp = nullptr;
+  if ((rc = probe(device, &dcp))) return rc;
+  DeviceCache& dc = *dcp;
+  std::lock_guard<std::mutex> host_call(dc.host_call);
+  size_t budget = 0;
+  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+
+  // The doubled grid's passes couple the cells of one line and the result samples even cells only,
+  // so after the passes along the first axes each voxel carries two cells into the last pass: those
+  // of its doubled line along the last axis at 2l and 2l + 1.
+  //   phase 1  slabs across the last axis: the slab's doubled mask, the X pass (and in 3-D the Y
+  //            pass over every doubled column), and the two cells per voxel come down: cell 2l into
+  //            `out`, cell 2l + 1 into a host scratch;
+  //   phase 2  boxes of whole lines along the last axis: both cells go up, are interleaved into the
+  //            box's doubled lines beside their mask, the last pass runs, the even cells come down.
+  // Every pass runs with the one-shot call's transform of the whole doubled grid.
+  const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
+  const Transform t{1, ndim, 0, border, {wx / 2, wy / 2, wz / 2}, {sx2, sy2, sz2}};
+  const int last = ndim - 1;
+  const int64_t n_last = ndim == 3 ? sz : sy, n_cut = ndim == 3 ? sy : sx;
+  const int64_t plane = total / n_last;                    // voxels of one phase-1 slice
+  const int64_t unit = ndim == 3 ? sx : 1;                 // voxels of one phase-2 slice per row
+  const int64_t line_vox = unit * n_last;                  // voxels of one phase-2 slice
+  const int cells = ndim == 3 ? 8 : 4;                     // doubled cells per voxel in phase 1
+  const int64_t cap2 = std::max<int64_t>(1, (int64_t)((((int64_t)1 << 32) - 65) / (2 * line_vox)));
+  const bool long1 = ndim == 3 && later_pass_is_long(geom_for_axis(1, sx2, sy2, sz2), transform_arith(t.w, t.n, 1),
+                                                     dc.max_smem_optin);
+  const int64_t c2 = std::min(n_cut, cap2);
+  const LineGeom g2 = ndim == 3 ? geom_for_axis(2, sx, c2, sz2) : geom_for_axis(1, c2, sy2, 1);
+  const bool long2 = later_pass_is_long(g2, transform_arith(t.w, t.n, last), dc.max_smem_optin);
+  // Slot volumes (4 bytes per voxel each) beside the labels and the graph:
+  //   phase 1  0 .. cells-1 the doubled distances; cells, cells+1 the two cells; then the doubled
+  //            mask (cells / 4 volumes)
+  //   phase 2  0, 1 the doubled lines; 2 cell 2l, then the result; 3 cell 2l + 1; 4 the lines' mask
+  // and per launch of a later pass the long-line kernel's two scratch volumes of the doubled cells.
+  const int planes1 = cells + 2 + cells / 4, planes2 = 5;
+  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes + 1 + 4 * planes1 + (long1 ? 8 * cells : 0), n_last,
+                                  budget);
+  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes + 1 + 4 * planes2 + (long2 ? 16 : 0), cap2, budget);
+  if (p1.count == 0 || p2.count == 0)
+    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked voxel-graph "
+                                "transform needs at least %zu bytes", budget, std::max(p1.need, p2.need));
+  if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
+  std::unique_ptr<float, decltype(&free)> odd_cells(static_cast<float*>(malloc(out_bytes)), &free);
+  if (!odd_cells)
+    return fail(EDTB200_ENOMEM, "no host memory for the %zu-byte scratch of the odd cells between the phases",
+                out_bytes);
+  if ((rc = pipeline_streams(dc))) return rc;
+
+  const char* lab_host = static_cast<const char*>(labels);
+  const int threads = 256;
+  auto blocks = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + threads - 1) / threads,
+                                                                                      (int64_t)dc.sm_count * 32)); };
+  {
+    ChunkSlots slots;
+    if ((rc = slots.take(dc, p1, plane, label_bytes + 1, planes1))) return rc;
+    PipelineSteps steps;
+    steps.item = "phase-1 chunk";
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      const size_t off = (size_t)(p1.start(k) * plane), n = (size_t)(p1.size(k) * plane);
+      const int r = upload(slots.labels[slot], lab_host + off * label_bytes, n * label_bytes, device, s);
+      return r ? r : upload(static_cast<char*>(slots.labels[slot]) + slots.vox * label_bytes, graph + off, n, device, s);
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      const int64_t c = p1.size(k), z0 = p1.start(k);
+      const int64_t cy = ndim == 3 ? sy : c, cz = ndim == 3 ? c : 1;              // the slab's extents
+      const uint8_t* gr = reinterpret_cast<const uint8_t*>(slots.labels[slot]) + slots.vox * label_bytes;
+      float* f = slots.plane(slot, 0);
+      uint8_t* mask = slots.plane<uint8_t>(slot, cells + 2);
+      int r = with_label_width(label_bytes, [&](auto b) {
+        voxel_graph_expand_kernel<b><<<blocks(c * plane), threads, 0, s>>>(
+            slots.labels[slot], gr, mask, sx, cy, cz, ndim, border, as_float,
+            ndim == 3 ? sy - 1 : sy - 1 - z0, ndim == 3 ? sz - 1 - z0 : 0);
+        CUDA_TRY(cudaGetLastError());
+        return 0;
+      });
+      if (!r) r = x_pass(t, mask, f, 2 * cy * (ndim == 3 ? 2 * cz : 1), dc, s);
+      if (!r && ndim == 3)                                  // behind our own X pass
+        r = later_pass(t, 1, mask, f, geom_for_axis(1, sx2, sy2, 2 * c), border, border, dc, s, /*pdl=*/true);
+      if (r) return r;
+      // cells 2l and 2l + 1 along the last axis: one doubled slice (3-D) or row (2-D) apart
+      const int64_t step = ndim == 3 ? 4 * sx * sy : 2 * sx;
+      for (int h = 0; h < 2; ++h) {
+        voxel_graph_gather_kernel<<<blocks(c * plane), threads, 0, s>>>(f + h * step, slots.plane(slot, cells + h), sx,
+                                                                          cy, cz, 2, 4 * sx, 8 * sx * sy, 0);
+        CUDA_TRY(cudaGetLastError());
+      }
+      return 0;
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      const int64_t off = p1.start(k) * plane;
+      const size_t bytes = (size_t)(p1.size(k) * plane) * sizeof(float);
+      const int r = download(out + off, slots.plane(slot, cells), bytes, device, s);
+      return r ? r : download(odd_cells.get() + off, slots.plane(slot, cells + 1), bytes, device, s);
+    };
+    if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
+  }
+  {
+    ChunkSlots slots;
+    if ((rc = slots.take(dc, p2, line_vox, label_bytes + 1, planes2))) return rc;
+    auto box = [&](const void* base, int64_t k, size_t bytes) { return line_box(base, p2, k, unit, plane, n_last, bytes); };
+    PipelineSteps steps;
+    steps.item = "phase-2 chunk";
+    steps.upload_writes_results = true;            // cell 2l goes up into the volume the result comes down from
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
+      if (!r) r = upload_box(static_cast<char*>(slots.labels[slot]) + slots.vox * label_bytes, box(graph, k, 1), device, s);
+      if (!r) r = upload_box(slots.plane(slot, 2), box(out, k, sizeof(float)), device, s);
+      return r ? r : upload_box(slots.plane(slot, 3), box(odd_cells.get(), k, sizeof(float)), device, s);
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      const int64_t c = p2.size(k), bp = unit * c;          // bp: the box's voxels per index of the last axis
+      const uint8_t* gr = reinterpret_cast<const uint8_t*>(slots.labels[slot]) + slots.vox * label_bytes;
+      float* f = slots.plane(slot, 0);
+      uint8_t* mask = slots.plane<uint8_t>(slot, 4);
+      int r = with_label_width(label_bytes, [&](auto b) {
+        voxel_graph_lines_kernel<b><<<blocks(bp * n_last), threads, 0, s>>>(
+            slots.labels[slot], gr, slots.plane(slot, 2), slots.plane(slot, 3), bp, n_last, ndim == 3 ? 0x10 : 0x04,
+            border, as_float, f, mask);
+        CUDA_TRY(cudaGetLastError());
+        return 0;
+      });
+      const LineGeom g = ndim == 3 ? geom_for_axis(2, sx, c, sz2) : geom_for_axis(1, c, sy2, 1);
+      if (!r) r = later_pass(t, last, mask, f, g, border, border, dc, s, /*pdl=*/false);
+      if (r) return r;
+      voxel_graph_gather_kernel<<<blocks(bp * n_last), threads, 0, s>>>(f, slots.plane(slot, 2), bp, n_last, 1, 1,
+                                                                         2 * bp, 0, (flags & EDTB200_SQRT) ? 1 : 0);
+      CUDA_TRY(cudaGetLastError());
+      return 0;
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      return download_box(box(out, k, sizeof(float)), slots.plane(slot, 2), device, s);
+    };
+    if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
+  }
+  return 0;
 }
 
 int edtb200_pass_first(const void* labels_dev, int label_bytes, int64_t sx, int64_t sy, int64_t sz,

@@ -13,6 +13,11 @@
 // per 2-byte store, rows of a warp contiguous), the ordinary three passes run on it as a one-byte
 // volume, and one kernel gathers the even cells (optionally through sqrt).  Everything stays on
 // the device; nothing of this is on the north-star path, so the kernels are plain streaming code.
+//
+// The chunked call (edtb200_transform_voxel_graph_chunked) draws the mask of one slab at a time
+// (the expand kernel's end_y / end_z place the volume's last slice), gathers two cells per voxel
+// with the strided gather, and rebuilds each voxel's doubled line along the last axis from those
+// two cells and its own graph byte (voxel_graph_lines_kernel).
 #pragma once
 
 #include <cstdint>
@@ -35,12 +40,14 @@ __device__ __forceinline__ bool voxel_is_foreground(const void* labels, int64_t 
   return false;
 }
 
-// One thread per source voxel; writes its 2 x 2 (x 2) cells.
+// One thread per source voxel; writes its 2 x 2 (x 2) cells.  end_y / end_z: the index, in this
+// volume, of the whole volume's last slice along y / z (sy - 1, sz - 1 unless the volume is a slab
+// of a larger one; beyond the slab when the slab does not hold it).
 template <int Bytes>
 __global__ void __launch_bounds__(256)
 voxel_graph_expand_kernel(const void* __restrict__ labels, const uint8_t* __restrict__ graph,
                           uint8_t* __restrict__ cells, int64_t sx, int64_t sy, int64_t sz, int ndim,
-                          int border, int as_float) {
+                          int border, int as_float, int64_t end_y, int64_t end_z) {
   const int64_t total = sx * sy * sz;
   const int64_t row2 = 2 * sx;                       // doubled row length
   const int64_t slice2 = row2 * 2 * sy;              // doubled slice size
@@ -49,8 +56,8 @@ voxel_graph_expand_kernel(const void* __restrict__ labels, const uint8_t* __rest
     const int64_t x = idx % sx, y = (idx / sx) % sy, z = idx / (sx * sy);
     const bool fg = voxel_is_foreground<Bytes>(labels, idx, as_float != 0);
     const uint8_t g = graph[idx];
-    const bool last_x = border && x == sx - 1, last_y = border && y == sy - 1,
-               last_z = border && z == sz - 1;
+    const bool last_x = border && x == sx - 1, last_y = border && y == end_y,
+               last_z = border && z == end_z;
     const int layers = ndim == 3 ? 2 : 1;
     for (int c = 0; c < layers; c++) {
       for (int b = 0; b < 2; b++) {
@@ -68,17 +75,42 @@ voxel_graph_expand_kernel(const void* __restrict__ labels, const uint8_t* __rest
   }
 }
 
-// out[x, y, z] = doubled[2x, 2y, 2z], through sqrt when asked.
+// out[x, y, z] = doubled[x * xs + y * ys + z * zs], through sqrt when asked: the even cells
+// (2x, 2y, 2z) of a doubled volume with xs = 2, ys = 4 sx, zs = 8 sx sy.
 __global__ void __launch_bounds__(256)
 voxel_graph_gather_kernel(const float* __restrict__ doubled, float* __restrict__ out, int64_t sx, int64_t sy,
-                          int64_t sz, int take_sqrt) {
+                          int64_t sz, int64_t xs, int64_t ys, int64_t zs, int take_sqrt) {
   const int64_t total = sx * sy * sz;
-  const int64_t row2 = 2 * sx, slice2 = row2 * 2 * sy;
   for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
     const int64_t x = idx % sx, y = (idx / sx) % sy, z = idx / (sx * sy);
-    float v = doubled[2 * z * slice2 + 2 * y * row2 + 2 * x];
+    float v = doubled[z * zs + y * ys + x * xs];
     out[idx] = take_sqrt ? sqrtf(v) : v;
+  }
+}
+
+// A box of whole lines along the last axis: n indices along it, `plane` voxels per index.  even /
+// odd hold cells 2l and 2l + 1 of each voxel's doubled line after the passes along the first axes;
+// they are interleaved into f, the box with its last axis doubled, and the line's mask is drawn as
+// the expand kernel draws it: cell 2l is the voxel's foreground, cell 2l + 1 the edge to the next
+// voxel along the last axis (graph bit `bit`: 0x10 in 3-D, 0x04 in 2-D), background on the volume's
+// last slice under a black border.  The box holds whole lines, so l == n - 1 is that slice.
+template <int Bytes>
+__global__ void __launch_bounds__(256)
+voxel_graph_lines_kernel(const void* __restrict__ labels, const uint8_t* __restrict__ graph,
+                         const float* __restrict__ even, const float* __restrict__ odd, int64_t plane, int64_t n,
+                         int bit, int border, int as_float, float* __restrict__ f, uint8_t* __restrict__ cells) {
+  const int64_t total = plane * n;
+  for (int64_t idx = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; idx < total;
+       idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = idx % plane, l = idx / plane;
+    const bool fg = voxel_is_foreground<Bytes>(labels, idx, as_float != 0);
+    const bool edge = fg && (graph[idx] & bit) && !(border && l == n - 1);
+    const int64_t at = 2 * l * plane + p;
+    f[at] = even[idx];
+    f[at + plane] = odd[idx];
+    cells[at] = fg ? 1 : 0;
+    cells[at + plane] = edge ? 1 : 0;
   }
 }
 

@@ -34,7 +34,8 @@ extern "C" {
  * edtb200_transform_multi, edtb200_slab_step / _stage_bytes / _pack, edtb200_label_stats / _extract,
  * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
- * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked) keep the
+ * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
+ * edtb200_transform_voxel_graph_chunked) keep the
  * number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up. */
 #define EDTB200_VERSION 202
@@ -269,6 +270,56 @@ int edtb200_transform_voxel_graph(const void *labels, int label_bytes, const uns
                                   float wx, float wy, float wz,
                                   int black_border, int flags,
                                   float *out, int device, void *stream);
+
+/* The same transform as edtb200_transform_voxel_graph for a 2-D or 3-D HOST volume whose doubled
+ * grid does not fit the device, streamed through one device in the two phases of
+ * edtb200_transform_chunked; the result is edtb200_transform_voxel_graph's bit for bit.
+ *
+ * Every pass of the doubled grid couples only the cells of one line, and the result samples the even
+ * cells only; so only the Y pass's columns at even x and the last pass's lines at even (x, y) matter,
+ * and each voxel carries two cells from the first phase into the second: those of its doubled line
+ * along the last axis, (2x, 2y, 2z) and (2x, 2y, 2z + 1) in 3-D, (2x, 2y) and (2x, 2y + 1) in 2-D.
+ * Both cells of that line's mask come from the voxel alone: cell 2l is foreground iff the voxel is,
+ * cell 2l + 1 iff the voxel is, its +z (3-D, bit 4) / +y (2-D, bit 2) edge is allowed, and it does not
+ * lie on the volume's last slice under a black border.
+ *   phase 1  z slabs (3-D) / row ranges (2-D): the labels and the graph go up, the slab's doubled
+ *            mask is drawn (the black border on the volume's last slice, not the slab's), the X pass
+ *            runs over every doubled row and in 3-D the Y pass over every doubled column (the odd-x
+ *            columns are not compacted away: that would cost a copy of the X distances for a pass
+ *            that is not the bottleneck), and the two cells come down: cell 2l into `out`, cell
+ *            2l + 1 into a host scratch of 4 bytes per voxel that the call allocates and frees
+ *            (EDTB200_ENOMEM when the host refuses it);
+ *   phase 2  y ranges of whole z lines (3-D) / x ranges of whole y lines (2-D): the labels, the graph
+ *            and both cells go up, are interleaved into the box's doubled lines beside their mask, the
+ *            last pass runs, and the even cells (through sqrt under EDTB200_SQRT) come down into `out`.
+ * Every pass runs with the one-shot call's transform of the whole doubled grid (half the weights,
+ * doubled extents), so it makes the one-shot arithmetic choices.  PCIe traffic per voxel:
+ * (2 label_bytes + 10) bytes up and 12 down, against label_bytes + 1 and 4 for
+ * edtb200_transform_voxel_graph: this is for volumes that do not fit.
+ *
+ * The plan is edtb200_transform_chunked's (slice, cap, chunks, count; the ENOMEM message names the
+ * least budget that works: the larger of the two phases' min(extent, 2) * slice) with these bytes per
+ * voxel, the slot's buffers plus the long-line kernel's two scratch volumes of doubled cells where the
+ * phase's later pass takes it (s1 = 64 in 3-D, s2 = 16):
+ *   phase 1  3-D: label_bytes + 49 (+ s1): labels, graph, 8 doubled distances, the two cells, the
+ *            doubled mask; 2-D: label_bytes + 29: the same with 4 doubled cells, and no later pass;
+ *   phase 2  label_bytes + 21 (+ s2): labels, graph, 2 doubled distances, the two cells, the mask of
+ *            the doubled lines (2 bytes held in 4);
+ *   cap      phase-2 chunks hold fewer than 2^32 - 64 doubled cells (sx * 2 sz per y in 3-D, 2 sy per
+ *            x in 2-D), so that the last pass can take the tile kernel where the one-shot call's could
+ *            not.
+ *
+ *   labels, graph, out  HOST buffers, pageable or pinned; out must not overlap labels or graph (the
+ *                 two inputs may overlap each other).  flags: EDTB200_SQRT, EDTB200_LABELS_FLOAT;
+ *                 EDTB200_SIGNED and the *_ON_DEVICE flags are rejected.  ndim is 2 or 3.
+ *   device_bytes, chunks  as for edtb200_transform_chunked.
+ * Returns when the result has landed; after an error the contents of `out` are unspecified.  Calls on
+ * one device are serialised. */
+int edtb200_transform_voxel_graph_chunked(const void *labels, int label_bytes, const unsigned char *graph,
+                                          int ndim, int64_t sx, int64_t sy, int64_t sz,
+                                          float wx, float wy, float wz,
+                                          int black_border, int flags, float *out,
+                                          int device, size_t device_bytes, int64_t *chunks);
 
 /* Single axis passes on DEVICE-resident data, for callers that split a volume into Z slabs
  * across GPUs (SURVEY.md section 8e): every rank runs the first- and second-axis passes on

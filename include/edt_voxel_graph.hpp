@@ -1,7 +1,8 @@
 // include/edt_voxel_graph.hpp -- C++ drop-in for the reference's voxel-connectivity-graph drivers
 // (reference src/edt_voxel_graph.hpp:54-236, namespace pyedt; the reference offers no `edt::`
 // facade for them): same names, template parameters, argument order and ownership, but the work
-// is done by edtb200_transform_voxel_graph on the GPU.
+// is done by edtb200_transform_voxel_graph on the GPU, or, for a volume whose doubled grid does not
+// fit the device, by edtb200_transform_voxel_graph_chunked.
 //
 //   float* dt = pyedt::_edt3dsq_voxel_graph<uint32_t, uint8_t>(labels, graph, sx, sy, sz,
 //                                                              wx, wy, wz, black_border);
@@ -36,9 +37,13 @@ inline float* voxel_graph_run(T* labels, GRAPH_TYPE* graph, int ndim, int64_t sx
   const int64_t voxels = sx * sy * (ndim > 2 ? sz : 1);
   float* out = workspace ? workspace : new float[voxels > 0 ? voxels : 1]();
   if (std::is_floating_point<T>::value) flags |= EDTB200_LABELS_FLOAT;
-  const int rc = edtb200_transform_voxel_graph(labels, (int)sizeof(T), reinterpret_cast<const unsigned char*>(graph),
-                                               ndim, sx, sy, sz, wx, wy, wz, black_border ? 1 : 0, flags, out,
-                                               /*device=*/0, /*stream=*/nullptr);
+  const unsigned char* g = reinterpret_cast<const unsigned char*>(graph);
+  int rc = edtb200_transform_voxel_graph(labels, (int)sizeof(T), g, ndim, sx, sy, sz, wx, wy, wz, black_border ? 1 : 0,
+                                         flags, out, /*device=*/0, /*stream=*/nullptr);
+  if (rc == EDTB200_ENOMEM)                      // larger than the device: stream it through in chunks
+    rc = edtb200_transform_voxel_graph_chunked(labels, (int)sizeof(T), g, ndim, sx, sy, sz, wx, wy, wz,
+                                               black_border ? 1 : 0, flags, out, /*device=*/0, /*device_bytes=*/0,
+                                               /*chunks=*/nullptr);
   if (rc != 0) {
     if (!workspace) delete[] out;
     throw std::runtime_error(std::string("edt_b200: ") + edtb200_last_error());

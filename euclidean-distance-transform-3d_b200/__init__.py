@@ -90,6 +90,12 @@ def _lib():
   lib.edtb200_feature_transform_chunked.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci,
                                                     ctypes.c_size_t, vp]
   lib.edtb200_feature_transform_chunked.restype = ci
+  lib.edtb200_transform_stack.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci,
+                                          ctypes.c_size_t, vp, vp]
+  lib.edtb200_transform_stack.restype = ci
+  lib.edtb200_feature_transform_stack.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci,
+                                                  vp]
+  lib.edtb200_feature_transform_stack.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
   lib.edtb200_transform_multi.restype = ci
   lib.edtb200_transform_batch.argtypes = [vp, vp, ci, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, ci]
@@ -449,8 +455,11 @@ def _chunk_budget(max_device_bytes, on_device, voxel_graph, dims):
   return budget
 
 
-def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None, max_device_bytes=None):
+def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None, max_device_bytes=None,
+                stacked=False):
   """Argument handling of edtsq(), src/edt.pyx:276-310."""
+  if stacked:
+    return _stack_front_door(data, anisotropy, black_border, voxel_graph, flags, device, max_device_bytes)
   on_device = _device_array(data)
   if on_device is not None:
     if max_device_bytes is not None:
@@ -492,13 +501,102 @@ def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixe
 
 
 # ---------------------------------------------------------------------------------------
+# stacks: same-shaped volumes along the slowest axis in memory, each transformed on its own with
+# one launch per pass for all of them (edtb200_transform_stack, edtb200_feature_transform_stack)
+# ---------------------------------------------------------------------------------------
+
+def _stack_dims(dims, voxel_graph=None):
+  """The volume ndim of a stacked array of `dims` dimensions, after rejecting what stacks do not cover."""
+  if voxel_graph is not None:
+    raise ValueError("stacked=True cannot be combined with voxel_graph")
+  if dims < 2 or dims > 4:
+    raise ValueError("stacked=True needs a 2-D to 4-D array: volumes of 1 to 3 dimensions along its slowest axis, "
+                     "got %d-D" % dims)
+  return dims - 1
+
+
+def _stack_anisotropy(vnd, anisotropy):
+  """One weight per volume axis (a scalar for 1-D volumes); default 1."""
+  if anisotropy is None:
+    return (1.0,) * vnd
+  if np.ndim(anisotropy) == 0 and vnd == 1:
+    return (float(anisotropy),)
+  weights = tuple(float(a) for a in np.asarray(anisotropy).reshape(-1))
+  if len(weights) != vnd:
+    raise ValueError("stacked=True: anisotropy must have one entry per volume axis (%d), got %d" % (vnd, len(weights)))
+  return weights
+
+
+def _stack_layout(shape, c_order, anisotropy):
+  """count, (sx, sy, sz), (wx, wy, wz) of a stack of `shape`: the slowest axis in memory (axis 0 in C
+  order, the last axis in F order) indexes the volumes, the others are one volume."""
+  count = int(shape[0] if c_order else shape[-1])
+  dims, weights = _x_fastest(shape[1:] if c_order else shape[:-1], anisotropy, not c_order)
+  return count, dims, weights
+
+
+def _stack_order(data):
+  """Memory order of a stacked numpy array ("C" wins where both apply), made contiguous if it is neither."""
+  if not data.flags.c_contiguous and not data.flags.f_contiguous:
+    data = np.ascontiguousarray(data)
+  return data, ("C" if data.flags.c_contiguous else "F")
+
+
+def _stack_front_door(data, anisotropy, black_border, voxel_graph, flags, device, max_device_bytes):
+  """edtsq(..., stacked=True) and friends: host arrays go through the GPU in groups of whole volumes
+  within `max_device_bytes` (None or 0: what the GPU has free); device arrays in one call."""
+  on_device = _device_array(data)
+  if on_device is None:
+    data = np.asarray(np.array(data) if isinstance(data, list) else data)
+  vnd = _stack_dims(on_device.dim() if on_device is not None else data.ndim, voxel_graph)
+  anisotropy = _stack_anisotropy(vnd, anisotropy)
+  if on_device is not None:
+    if max_device_bytes is not None:
+      raise ValueError("max_device_bytes streams a host array through the GPU; a device-resident array already fits")
+    return _stack_device(on_device, anisotropy, black_border, flags)
+  budget = 0 if max_device_bytes is None else int(max_device_bytes)
+  if budget < 0:
+    raise ValueError("max_device_bytes must be non-negative (0: what the device has free)")
+  data, order = _stack_order(data)
+  labels = _label_view(data) if data.size else None
+  if labels is None:
+    return np.zeros(data.shape, dtype=np.float32, order=order)
+  count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(data.shape, order == "C", anisotropy)
+  out = _result_buffer(data.size)
+  _check(_lib().edtb200_transform_stack(
+    labels.ctypes.data, labels.dtype.itemsize, vnd, sx, sy, sz, count, wx, wy, wz, int(bool(black_border)),
+    int(flags), out.ctypes.data, int(device), budget, None, None))
+  return out.reshape(data.shape, order=order)
+
+
+def _stack_device(t, anisotropy, black_border, flags):
+  """A device-resident stack: an F-ordered one goes through its transposed (C-ordered) view, whose axis 0
+  is then the volume index, with the volume's anisotropy reversed."""
+  import torch
+  dims = t.dim()
+  if t.numel() == 0:
+    return torch.zeros(t.shape, dtype=torch.float32, device=t.device)
+  if t.dtype in (torch.float32, torch.float64):
+    t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)     # -0.0 == +0.0
+  fortran = not t.is_contiguous() and t.permute(*reversed(range(dims))).is_contiguous()
+  if fortran:
+    t = t.permute(*reversed(range(dims)))
+    anisotropy = tuple(reversed(anisotropy))
+  out = edt_cuda(t, anisotropy, black_border, sqrt=bool(flags & FLAG_SQRT), signed=bool(flags & FLAG_SIGNED),
+                 stacked=True)
+  return out.permute(*reversed(range(dims))) if fortran else out
+
+
+# ---------------------------------------------------------------------------------------
 # public API (signatures follow src/edt.pyx; `device` is keyword-only and additive)
 # ---------------------------------------------------------------------------------------
 
-def _pick(device, devices, max_device_bytes=None):
+def _pick(device, devices, max_device_bytes=None, stacked=False):
   """`devices` (a sequence of GPU ordinals: one host volume spread over them) wins over `device`."""
   if devices is None:
     return device
+  if stacked:
+    raise ValueError("stacked=True runs on one GPU; it cannot be combined with devices=[...]")
   if max_device_bytes is not None:
     raise ValueError("max_device_bytes streams through one GPU; it cannot be combined with devices=[...]")
   devs = [int(d) for d in devices]
@@ -511,35 +609,46 @@ def _pick(device, devices, max_device_bytes=None):
 # through one GPU in chunks that fit N bytes of device memory (0: what the GPU has free), with the
 # result of the one-shot transform bit for bit; with None a one-shot transform that runs out of
 # device memory falls back to that once (see _transform_host).
+#
+# `stacked=True` (edt, edtsq, sdf, sdfsq, edt_cuda, feature_transform) takes a 2-D to 4-D array whose
+# slowest axis in memory (axis 0 of a C-ordered array, the last of an F-ordered one) indexes
+# independent volumes of 1 to 3 dimensions: each is transformed on its own, with one launch per pass
+# for the whole stack.  `anisotropy` has one entry per volume axis, black_border applies to every
+# volume's own faces, and the result has the input's shape and memory order, equal to np.stack of
+# the per-volume calls.  For host arrays max_device_bytes is the budget of the groups of whole volumes
+# that go through the GPU at once.
 
 def edtsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-          *, device=0, devices=None, max_device_bytes=None):
+          *, device=0, devices=None, max_device_bytes=None, stacked=False):
   """Squared anisotropic multi-label EDT of a 1-D, 2-D or 3-D array (src/edt.pyx:245-310).
   `devices=[0, 1, ...]` spreads one host volume over several GPUs (see _transform_host)."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, 0, _pick(device, devices, max_device_bytes),
-                     max_device_bytes=max_device_bytes)
+  return _front_door(data, anisotropy, black_border, voxel_graph, 0, _pick(device, devices, max_device_bytes, stacked),
+                     max_device_bytes=max_device_bytes, stacked=stacked)
 
 
 def edt(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-        *, device=0, devices=None, max_device_bytes=None):
+        *, device=0, devices=None, max_device_bytes=None, stacked=False):
   """Anisotropic multi-label EDT (src/edt.pyx:205-242); the sqrt is fused into the last pass."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, _pick(device, devices, max_device_bytes),
-                     max_device_bytes=max_device_bytes)
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT,
+                     _pick(device, devices, max_device_bytes, stacked), max_device_bytes=max_device_bytes,
+                     stacked=stacked)
 
 
 def sdf(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-        *, device=0, devices=None, max_device_bytes=None):
+        *, device=0, devices=None, max_device_bytes=None, stacked=False):
   """Signed distance function, edt(data) - edt(data == 0) (src/edt.pyx:121-158), computed as
   one transform with background as a label and the sign applied in the last store."""
   return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT | FLAG_SIGNED,
-                     _pick(device, devices, max_device_bytes), max_device_bytes=max_device_bytes)
+                     _pick(device, devices, max_device_bytes, stacked), max_device_bytes=max_device_bytes,
+                     stacked=stacked)
 
 
 def sdfsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, *, device=0, devices=None,
-          max_device_bytes=None):
+          max_device_bytes=None, stacked=False):
   """Squared signed distance function (src/edt.pyx:161-202)."""
-  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SIGNED, _pick(device, devices, max_device_bytes),
-                     max_device_bytes=max_device_bytes)
+  return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SIGNED,
+                     _pick(device, devices, max_device_bytes, stacked), max_device_bytes=max_device_bytes,
+                     stacked=stacked)
 
 
 def edt1dsq(data, anisotropy=1.0, black_border=False, *, device=0):
@@ -594,18 +703,24 @@ def _torch_label_bytes(torch):
 
 
 def edt_cuda(labels, anisotropy=None, black_border=False, *, sqrt=False, signed=False, out=None,
-             voxel_graph=None):
+             voxel_graph=None, stacked=False):
   """Transform a C-contiguous integer/bool torch CUDA tensor of 1-3 dims on its own device
   and current stream, asynchronously; returns a float32 CUDA tensor of the same shape
   (`out` may be passed to reuse a buffer).  Same semantics as edtsq/edt/sdfsq/sdf.
   `voxel_graph` (a uint8/int8 CUDA tensor of the same shape, 2-D / 3-D only, not with `signed`)
-  selects the connectivity-graph transform."""
+  selects the connectivity-graph transform.  `stacked=True` takes a (B, ...) tensor of 2-4 dims:
+  B volumes of 1-3 dims, each transformed on its own, one launch per pass for all of them
+  (`anisotropy`: one entry per volume axis)."""
   import torch
   if not (isinstance(labels, torch.Tensor) and labels.is_cuda):
     raise TypeError("edt_cuda expects a torch CUDA tensor")
   nd = labels.dim()
-  if nd < 1 or nd > 3:
+  if stacked:
+    vnd = _stack_dims(nd, voxel_graph)
+  elif nd < 1 or nd > 3:
     raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(nd))
+  else:
+    vnd = nd
   if not labels.is_contiguous():
     labels = labels.contiguous()
   nbytes = _torch_label_bytes(torch).get(labels.dtype)
@@ -619,16 +734,21 @@ def edt_cuda(labels, anisotropy=None, black_border=False, *, sqrt=False, signed=
   if labels.numel() == 0:
     return out
   if anisotropy is None:
-    anisotropy = (1.0,) * nd
-  elif nd == 1 and np.ndim(anisotropy) == 0:
+    anisotropy = (1.0,) * vnd
+  elif vnd == 1 and np.ndim(anisotropy) == 0:
     anisotropy = (float(anisotropy),)
-  (sx, sy, sz), (wx, wy, wz) = _x_fastest(labels.shape, anisotropy, False)
+  (sx, sy, sz), (wx, wy, wz) = _x_fastest(labels.shape[1:] if stacked else labels.shape, anisotropy, False)
   flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
   if sqrt:
     flags |= FLAG_SQRT
   if signed:
     flags |= FLAG_SIGNED
   stream = torch.cuda.current_stream(labels.device).cuda_stream
+  if stacked:
+    _check(_lib().edtb200_transform_stack(
+      labels.data_ptr(), nbytes, vnd, sx, sy, sz, int(labels.shape[0]), wx, wy, wz, int(bool(black_border)), flags,
+      out.data_ptr(), labels.device.index, 0, None, ctypes.c_void_p(stream)))
+    return out
   if voxel_graph is not None:
     if nd not in (2, 3):
       raise TypeError("Voxel connectivity graph is only supported for 2D and 3D. Got {}.".format(nd))
@@ -726,53 +846,71 @@ def _feature_anisotropy(dims, anisotropy):
   raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
 
 
-def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_device_bytes=None):
+def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_device_bytes=None, stacked=False):
   """(distances or None, indices) of a numpy array through host buffers (edtb200_feature_transform).
   `max_device_bytes` (an int) streams a 2-D / 3-D array through one GPU in chunks within that budget
   (edtb200_feature_transform_chunked); with None a one-shot call that runs out of device memory is
-  retried once that way, as _transform_host does."""
+  retried once that way, as _transform_host does.  stacked: a stack of volumes along the slowest axis
+  in memory (edtb200_feature_transform_stack), one index plane per volume axis."""
   if isinstance(data, list):
     data = np.array(data)
   data = np.asarray(data)
   nd = data.ndim
-  anisotropy = _feature_anisotropy(nd, anisotropy)
-  if not data.flags.c_contiguous and not data.flags.f_contiguous:
-    data = np.ascontiguousarray(data)
-  order = "F" if data.flags.f_contiguous else "C"
+  vnd = nd - 1 if stacked else nd           # index planes: one per (volume) axis
+  if stacked:
+    anisotropy = _stack_anisotropy(vnd, anisotropy)
+    data, order = _stack_order(data)
+  else:
+    anisotropy = _feature_anisotropy(nd, anisotropy)
+    if not data.flags.c_contiguous and not data.flags.f_contiguous:
+      data = np.ascontiguousarray(data)
+    order = "F" if data.flags.f_contiguous else "C"
   labels = _label_view(data)
   if labels is None:
     raise TypeError("feature_transform: unsupported label dtype %s" % data.dtype)
   # one plane per array axis, each in the input's memory order: for F order the planes are
   # allocated with the axes reversed and viewed back
-  planes = np.empty((nd,) + (data.shape if order == "C" else data.shape[::-1]), dtype=np.int32)
+  planes = np.empty((vnd,) + (data.shape if order == "C" else data.shape[::-1]), dtype=np.int32)
   dist = np.zeros(data.size, dtype=np.float32) if want_dist else None
   if data.size:
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
-    # x-fastest axis j is array axis j in F order, array axis nd - 1 - j in C order
-    ptrs = (ctypes.c_void_p * nd)(*[planes[j if order == "F" else nd - 1 - j].ctypes.data for j in range(nd)])
+    if stacked:
+      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(data.shape, order == "C", anisotropy)
+    else:
+      (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
+    # x-fastest axis j is array axis j in F order, array axis nd - 1 - j in C order (of a stack: its
+    # plane vnd - 1 - j, the volume index being array axis 0)
+    ptrs = (ctypes.c_void_p * vnd)(*[planes[j if order == "F" else vnd - 1 - j].ctypes.data for j in range(vnd)])
     lib = _lib()
-    args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
-            int(flags), dist.ctypes.data if want_dist else None, ptrs, int(device))
-    if max_device_bytes is None:
-      try:
-        _check(lib.edtb200_feature_transform(*args, None))
-      except EDTError as e:
-        if e.code != ENOMEM or nd not in (2, 3):
-          raise
-        max_device_bytes = 0                  # too large for the device: stream it through in chunks
-    if max_device_bytes is not None:
-      _check(lib.edtb200_feature_transform_chunked(*args, int(max_device_bytes), None))
+    dist_ptr = dist.ctypes.data if want_dist else None
+    if stacked:
+      _check(lib.edtb200_feature_transform_stack(
+        labels.ctypes.data, labels.dtype.itemsize, vnd, sx, sy, sz, count, wx, wy, wz, int(bool(black_border)),
+        int(flags), dist_ptr, ptrs, int(device), None))
+    else:
+      args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
+              int(flags), dist_ptr, ptrs, int(device))
+      if max_device_bytes is None:
+        try:
+          _check(lib.edtb200_feature_transform(*args, None))
+        except EDTError as e:
+          if e.code != ENOMEM or nd not in (2, 3):
+            raise
+          max_device_bytes = 0                # too large for the device: stream it through in chunks
+      if max_device_bytes is not None:
+        _check(lib.edtb200_feature_transform_chunked(*args, int(max_device_bytes), None))
   indices = planes if order == "C" else planes.transpose((0,) + tuple(range(nd, 0, -1)))
   return (dist.reshape(data.shape, order=order) if want_dist else None), indices
 
 
-def _feature_device(t, anisotropy, black_border, flags, want_dist):
+def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False):
   """(distances or None, indices) of a torch CUDA tensor as torch CUDA tensors on its current
   stream, without host copies.  A Fortran-ordered tensor goes through its transposed view, as in
-  _front_door_device, and its results are returned in its order."""
+  _front_door_device, and its results are returned in its order.  stacked: a stack of volumes
+  along the slowest axis in memory, one index plane per volume axis."""
   import torch
   dims = t.dim()
-  anisotropy = _feature_anisotropy(dims, anisotropy)
+  vnd = dims - 1 if stacked else dims       # index planes: one per (volume) axis
+  anisotropy = _stack_anisotropy(vnd, anisotropy) if stacked else _feature_anisotropy(dims, anisotropy)
   if t.dtype in (torch.float32, torch.float64):
     t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)     # -0.0 == +0.0
   nbytes = _torch_label_bytes(torch).get(t.dtype)
@@ -783,17 +921,25 @@ def _feature_device(t, anisotropy, black_border, flags, want_dist):
     t = t.permute(*reversed(range(dims)))
     anisotropy = tuple(reversed(anisotropy))
   t = t.contiguous()
-  planes = torch.empty((dims,) + tuple(t.shape), dtype=torch.int32, device=t.device)
+  planes = torch.empty((vnd,) + tuple(t.shape), dtype=torch.int32, device=t.device)
   dist = torch.zeros(t.shape, dtype=torch.float32, device=t.device) if want_dist else None
   if t.numel():
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape, anisotropy, False)
-    # x-fastest axis j is the caller's array axis j when it was F-ordered, else axis dims - 1 - j
-    ptrs = (ctypes.c_void_p * dims)(*[planes[j if fortran else dims - 1 - j].data_ptr() for j in range(dims)])
+    # x-fastest axis j is the caller's array axis j when it was F-ordered, else axis dims - 1 - j (of
+    # a stack: its plane vnd - 1 - j, the volume index being axis 0)
+    ptrs = (ctypes.c_void_p * vnd)(*[planes[j if fortran else vnd - 1 - j].data_ptr() for j in range(vnd)])
     stream = torch.cuda.current_stream(t.device).cuda_stream
-    _check(_lib().edtb200_feature_transform(
-      t.data_ptr(), nbytes, dims, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
-      int(flags) | FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, dist.data_ptr() if want_dist else None, ptrs,
-      t.device.index, ctypes.c_void_p(stream)))
+    dist_ptr = dist.data_ptr() if want_dist else None
+    flags = int(flags) | FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
+    if stacked:
+      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(t.shape, True, anisotropy)
+      _check(_lib().edtb200_feature_transform_stack(
+        t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, int(bool(black_border)), flags, dist_ptr, ptrs,
+        t.device.index, ctypes.c_void_p(stream)))
+    else:
+      (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape, anisotropy, False)
+      _check(_lib().edtb200_feature_transform(
+        t.data_ptr(), nbytes, dims, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags, dist_ptr, ptrs,
+        t.device.index, ctypes.c_void_p(stream)))
   if fortran:
     planes = planes.permute(0, *range(dims, 0, -1))
     dist = dist.permute(*reversed(range(dims))) if want_dist else None
@@ -801,7 +947,7 @@ def _feature_device(t, anisotropy, black_border, flags, want_dist):
 
 
 def feature_transform(data, anisotropy=None, black_border=False, *, signed=False, return_distances=False, device=0,
-                      max_device_bytes=None):
+                      max_device_bytes=None, stacked=False):
   """The nearest site of every voxel: scipy.ndimage.distance_transform_edt(return_indices=True)
   for multi-label volumes, on the GPU.
 
@@ -821,9 +967,24 @@ def feature_transform(data, anisotropy=None, black_border=False, *, signed=False
 
   `max_device_bytes=N` streams a 2-D / 3-D host array through one GPU in chunks that fit N bytes of
   device memory (0: what the GPU has free), with the one-shot result bit for bit; with None a one-shot
-  call that runs out of device memory falls back to that once."""
+  call that runs out of device memory falls back to that once.
+
+  `stacked=True` takes a 2-D to 4-D array whose slowest axis in memory indexes independent volumes,
+  as edt(stacked=True) does: `indices` then has shape (data.ndim - 1,) + data.shape and holds the
+  coordinates within each voxel's own volume.  The whole stack is staged on the GPU at once, so it
+  cannot be combined with max_device_bytes."""
   flags = FLAG_SQRT | (FLAG_SIGNED if signed else 0)
   on_device = _device_array(data)
+  if stacked:
+    _stack_dims(on_device.dim() if on_device is not None else np.ndim(data))
+    if max_device_bytes is not None:
+      raise ValueError("stacked=True stages the whole stack on the GPU at once; it cannot be combined with "
+                       "max_device_bytes")
+    if on_device is not None:
+      dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances, stacked=True)
+    else:
+      dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device, stacked=True)
+    return (dist, idx) if return_distances else idx
   if max_device_bytes is not None:
     dims = on_device.dim() if on_device is not None else np.ndim(data)
     max_device_bytes = _chunk_budget(max_device_bytes, on_device is not None, None, dims)

@@ -618,7 +618,9 @@ struct Transform {
   int64_t n[3];
 };
 
-edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz);
+// The lines of the later pass along `axis` over `count` volumes of (sx, sy, sz) laid end to end: the
+// outer dimension walks the volumes, so that no line crosses from one volume into the next.
+edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz, int64_t count = 1);
 
 // The run-start planes that the X pass of one transform writes for its later passes (XPlanes): one
 // bit per voxel and later axis, stream-ordered scratch freed on the stream when the owner goes out
@@ -637,30 +639,33 @@ struct RunPlanes {
   const edtb200::RunBits* for_axis(int k) const { return bits[k].start ? &bits[k] : nullptr; }
 };
 
-// Takes the planes for transform t over the volume (t.n[0], sy, sz) at labels / f where they pay;
-// taking none costs nothing (the later passes then read the labels).
+// Takes the planes for transform t over `count` volumes (t.n[0], sy, sz) laid end to end at labels / f
+// where they pay; taking none costs nothing (the later passes then read the labels).
 int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const float* f, int64_t sy, int64_t sz,
-                    DeviceCache& dc, cudaStream_t s) {
+                    int64_t count, DeviceCache& dc, cudaStream_t s) {
   const int64_t sx = t.n[0];
   if (t.ndim < 2 || t.label_bytes < 4 || (t.flags & EDTB200_SIGNED) || sx > 512 ||
-      !first_is_vec(labels, t.label_bytes, f, sx) || !label_noise_predicted(dc))
+      !first_is_vec(labels, t.label_bytes, f, sx) || !label_noise_predicted(dc) || sz * count > 0x7fffffffLL)
     return 0;
   bool tile = false;
   for (int k = 1; k < t.ndim; ++k)
-    tile = tile || !later_pass_is_long(geom_for_axis(k, sx, sy, sz), transform_arith(t.w, t.n, k), dc.max_smem_optin);
+    tile = tile ||
+           !later_pass_is_long(geom_for_axis(k, sx, sy, sz, count), transform_arith(t.w, t.n, k), dc.max_smem_optin);
   if (!tile) return 0;
-  const int64_t wpr = (sx + 31) >> 5, words = sy * sz * wpr;
+  const int64_t wpr = (sx + 31) >> 5, words = sy * sz * count * wpr;
   if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)words * (size_t)(t.ndim - 1), s) != cudaSuccess) {
     cudaGetLastError();
     return 0;                        // no room: the later passes read the labels
   }
   uint32_t* p = rp.mem.get<uint32_t>();
   rp.x.sy = sy;
+  rp.x.depth = sz;
   rp.x.y = p;
   rp.x.z = t.ndim == 3 ? p + words : nullptr;
-  // Y pass: outer = z, inner = x; Z pass: inner = y * sx + x, rows sy * wpr words apart
+  // Y pass: outer = z (of every volume), inner = x; Z pass: outer = volume, inner = y * sx + x, rows
+  // sy * wpr words apart
   rp.bits[1] = edtb200::RunBits{rp.x.y, wpr, sy * wpr, sx, wpr};
-  if (t.ndim == 3) rp.bits[2] = edtb200::RunBits{rp.x.z, sy * wpr, 0, sx, wpr};
+  if (t.ndim == 3) rp.bits[2] = edtb200::RunBits{rp.x.z, sy * wpr, sz * sy * wpr, sx, wpr};
   return 0;
 }
 
@@ -703,12 +708,13 @@ __global__ void __launch_bounds__(256) sample_range_kernel(const float* __restri
   }
 }
 
-edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz) {
+edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz, int64_t count) {
   edtb200::LineGeom g;
   if (axis == 1) {
-    g.outer_count = sz; g.outer_stride = sx * sy; g.inner_count = sx; g.line_stride = sx; g.n = (int)sy;
+    g.outer_count = sz * count; g.outer_stride = sx * sy; g.inner_count = sx; g.line_stride = sx; g.n = (int)sy;
   } else {
-    g.outer_count = 1; g.outer_stride = 0; g.inner_count = sx * sy; g.line_stride = sx * sy; g.n = (int)sz;
+    g.outer_count = count; g.outer_stride = count > 1 ? sx * sy * sz : 0; g.inner_count = sx * sy;
+    g.line_stride = sx * sy; g.n = (int)sz;
   }
   g.tiles_per_outer = 0;
   return g;
@@ -765,10 +771,13 @@ void nvtx_init() {
 void nvtx_push(const char* name) { nvtx_init(); if (g_nvtx_push) g_nvtx_push(name); }
 void nvtx_pop() { if (g_nvtx_pop) g_nvtx_pop(); }
 
-// All passes of one transform on device-resident buffers.
+// All passes of one transform on device-resident buffers: of `count` volumes of (sx, sy, sz) laid end
+// to end, each transformed on its own with one launch per pass for all of them.  Every pass keeps one
+// volume's extents for its arithmetic (transform_arith over t.n), so each volume gets the plan it
+// would get alone.
 int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                float wx, float wy, float wz, int border, int flags, float* f,
-               DeviceCache& dc, cudaStream_t stream) {
+               DeviceCache& dc, cudaStream_t stream, int64_t count = 1) {
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   // The later passes are launched with programmatic stream serialization: the kernel before them
   // in the stream is our own previous pass, which never writes the labels, so their label staging
@@ -778,7 +787,7 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   // later passes read those instead of the labels (RunPlanes); a later pass reads its plane only
   // after griddepcontrol.wait.
   RunPlanes planes;
-  int rc = take_run_planes(planes, t, labels, f, sy, sz, dc, stream);
+  int rc = take_run_planes(planes, t, labels, f, sy, sz, count, dc, stream);
   if (rc) return rc;
   // EDT_B200_VERBOSE=1: per-pass device times of every transform on stderr (SURVEY.md section 5).
   // The dump needs the passes to have finished, so a verbose transform synchronises its stream.
@@ -787,19 +796,19 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   if (verbose) g_profile = true;
   mark_pass(0, stream);
   nvtx_push("edt.x");
-  rc = x_pass(t, labels, f, sy * sz, dc, stream, &planes);
+  rc = x_pass(t, labels, f, sy * sz * count, dc, stream, &planes);
   nvtx_pop();
   mark_pass(1, stream);
   if (!rc && ndim >= 2) {
     nvtx_push("edt.y");
-    rc = later_pass(t, 1, labels, f, geom_for_axis(1, sx, sy, sz), border, border, dc, stream, /*pdl=*/true,
+    rc = later_pass(t, 1, labels, f, geom_for_axis(1, sx, sy, sz, count), border, border, dc, stream, /*pdl=*/true,
                     &planes);
     nvtx_pop();
     mark_pass(2, stream);
   }
   if (!rc && ndim >= 3) {
     nvtx_push("edt.z");
-    rc = later_pass(t, 2, labels, f, geom_for_axis(2, sx, sy, sz), border, border, dc, stream, /*pdl=*/true,
+    rc = later_pass(t, 2, labels, f, geom_for_axis(2, sx, sy, sz, count), border, border, dc, stream, /*pdl=*/true,
                     &planes);
     nvtx_pop();
     mark_pass(3, stream);
@@ -808,7 +817,7 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
     g_profile = profile_was;
     float ms[3] = {0.0f, 0.0f, 0.0f};
     if (!rc && edtb200_pass_ms(0, ms) == 0) {
-      const double nvox = (double)sx * (double)sy * (double)sz;
+      const double nvox = (double)sx * (double)sy * (double)sz * (double)count;
       const double total = ms[0] + ms[1] + ms[2];
       fprintf(stderr, "[edt_b200] %lldx%lldx%lld L=%d  x %.3f ms  y %.3f ms  z %.3f ms  total %.3f ms  "
                       "%.0f Mvox/s  %.0f GB/s algorithmic\n",
@@ -822,12 +831,14 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
 
 // All passes of one feature transform on device-resident buffers: the site-tracking passes, out of
 // place and alternating between `dist` and one scratch volume so that the last lands in `dist`, then
-// the resolver.  dist may be null (the distances then stay in scratch).
+// the resolver.  dist may be null (the distances then stay in scratch).  `count` volumes of
+// (sx, sy, sz) laid end to end are transformed each on its own, as run_passes does; the index planes
+// hold coordinates within each voxel's own volume.
 int run_feature_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                        float wx, float wy, float wz, int border, int flags, float* dist, int32_t* const idx[3],
-                       DeviceCache& dc, cudaStream_t s) {
+                       DeviceCache& dc, cudaStream_t s, int64_t count = 1) {
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
-  const size_t total = (size_t)(sx * sy * sz);
+  const size_t total = (size_t)(sx * sy * sz * count);
   Scratch own_dist, other, codes;
   auto take = [&](Scratch& sc, size_t bytes) {
     if (sc.alloc(dc, bytes, s) == cudaSuccess) return 0;
@@ -843,19 +854,20 @@ int run_feature_passes(const void* labels, int label_bytes, int ndim, int64_t sx
   for (int k = 0; k < ndim; ++k) code_planes[k] = codes.get<int>() + (size_t)k * total;
   // pass k writes buf[(ndim - 1 - k) % 2]: the last one (k = ndim - 1) writes buf[0]
   rc = with_label_width(label_bytes, [&](auto b) {
-    return launch_first_sites<b>(labels, buf[(ndim - 1) % 2], code_planes[0], sy * sz, sx, wx, border,
+    return launch_first_sites<b>(labels, buf[(ndim - 1) % 2], code_planes[0], sy * sz * count, sx, wx, border,
                                  kernel_flags(flags, true, ndim == 1), dc, s);
   });
   for (int k = 1; !rc && k < ndim; ++k) {
     rc = with_label_width(label_bytes, [&](auto b) {
       return launch_later_sites<b>(labels, buf[(ndim - k) % 2], buf[(ndim - 1 - k) % 2], code_planes[k],
-                                   geom_for_axis(k, sx, sy, sz), t.w[k], border, border,
+                                   geom_for_axis(k, sx, sy, sz, count), t.w[k], border, border,
                                    kernel_flags(flags, false, k == ndim - 1), transform_arith(t.w, t.n, k), dc, s);
     });
   }
   if (rc) return rc;
   return with_label_width(label_bytes, [&](auto b) {
-    return launch_resolve_sites<b>(labels, code_planes, ndim, sx, sy, sz, !(flags & EDTB200_SIGNED), idx, dc, s);
+    return launch_resolve_sites<b>(labels, code_planes, ndim, sx, sy, sz, count, !(flags & EDTB200_SIGNED), idx, dc,
+                                   s);
   });
 }
 
@@ -1006,39 +1018,8 @@ int edtb200_transform(const void* labels, int label_bytes, int ndim, int64_t sx,
 int edtb200_feature_transform(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                               float wx, float wy, float wz, int black_border, int flags, float* dist_out,
                               int32_t* const* idx_out, int device, void* stream_v) {
-  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
-  if (rc) return rc;
-  const int64_t total = sx * sy * sz;
-  if (total == 0) return 0;
-  if (!labels || !idx_out) return fail(EDTB200_EINVAL, "null pointer");
-  for (int k = 0; k < ndim; ++k)
-    if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
-
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
-  HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
-  // host buffers are staged through the cached labels and distances and one scratch for the planes;
-  // a distance volume and an index plane are 4 bytes per voxel
-  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, vol_bytes = (size_t)total * sizeof(float);
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
-  const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  Scratch planes;
-  if (!io.out_dev) {
-    if (dist_out) CUDA_TRY(grow(dc->dist, dc->dist_bytes, vol_bytes));
-    if (planes.alloc(*dc, (size_t)ndim * vol_bytes, io.stream) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the index planes");
-    }
-  }
-  float* d_dist = dist_out ? io.out(dist_out, vol_bytes, dc->dist) : nullptr;
-  int32_t* d_idx[3] = {nullptr, nullptr, nullptr};
-  for (int k = 0; k < ndim; ++k)
-    d_idx[k] = io.out(idx_out[k], vol_bytes, io.out_dev ? nullptr : planes.get<int32_t>() + (size_t)k * total);
-  rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_dist,
-                          d_idx, *dc, io.stream);
-  return rc ? rc : io.finish();
+  return edtb200_feature_transform_stack(labels, label_bytes, ndim, sx, sy, sz, 1, wx, wy, wz, black_border, flags,
+                                         dist_out, idx_out, device, stream_v);
 }
 
 int edtb200_transform_batch(const void* const* labels, float* const* outs, int count, int label_bytes, int ndim,
@@ -1430,6 +1411,118 @@ int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int n
     if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
   }
   return 0;
+}
+
+// Slot bytes of one group of edtb200_transform_stack on host buffers (include/edt_b200.h).
+constexpr size_t kStackGroupBytes = size_t(512) << 20;
+
+int edtb200_transform_stack(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                            int64_t count, float wx, float wy, float wz, int black_border, int flags, float* out,
+                            int device, size_t device_bytes, int64_t* groups, void* stream_v) {
+  if (groups) *groups = 0;
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  const int64_t vol = sx * sy * sz;
+  if (vol == 0 || count == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const bool in_dev = flags & EDTB200_LABELS_ON_DEVICE, out_dev = flags & EDTB200_OUT_ON_DEVICE;
+  if (in_dev != out_dev)
+    return fail(EDTB200_EINVAL, "edtb200_transform_stack takes labels and out both on the device or both on the host");
+  const size_t vol_lab = (size_t)vol * (size_t)label_bytes, vol_out = (size_t)vol * sizeof(float);
+  const char* lab_host = static_cast<const char*>(labels);
+  if (!in_dev && overlap(lab_host, vol_lab * (size_t)count, out, vol_out * (size_t)count))
+    return fail(EDTB200_EINVAL, "labels and out overlap");
+
+  DeviceGuard restore_device;
+  DeviceCache* dcp = nullptr;
+  if ((rc = probe(device, &dcp))) return rc;
+  DeviceCache& dc = *dcp;
+  const int border = black_border != 0;
+  if (in_dev) {                                  // asynchronous on the caller's stream, no lock
+    rc = run_passes(labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, out, dc,
+                    static_cast<cudaStream_t>(stream_v), count);
+    if (!rc && groups) *groups = 1;
+    return rc;
+  }
+
+  // Host buffers: groups of whole volumes through two device slots, planned as a phase of
+  // edtb200_transform_chunked whose slices are volumes.
+  std::lock_guard<std::mutex> host_call(dc.host_call);
+  size_t budget = 0;
+  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
+  bool long_any = false;                         // a later pass takes the long-line kernel: its scratch
+  for (int k = 1; k < ndim; ++k)
+    long_any = long_any || later_pass_is_long(geom_for_axis(k, sx, sy, sz), transform_arith(t.w, t.n, k),
+                                              dc.max_smem_optin);
+  // A group holds at most kStackGroupBytes of slot, so that a large stack runs as several groups whose
+  // uploads and downloads overlap each other's passes, as edtb200_transform_batch's volumes do.
+  const size_t voxel_bytes = label_bytes + 4 + (long_any ? 8 : 0);
+  const int64_t most = std::max<int64_t>(1, (int64_t)(kStackGroupBytes / ((size_t)vol * voxel_bytes)));
+  const PhasePlan p = plan_phase(count, vol, voxel_bytes, most, budget);
+  if (p.count == 0)
+    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one group of volumes: the stack needs at "
+                                "least %zu bytes", budget, p.need);
+  if (p.count > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many groups of volumes");
+  if ((rc = pipeline_streams(dc))) return rc;
+  ChunkSlots slots;
+  if ((rc = slots.take(dc, p, vol, label_bytes, 1))) return rc;
+  PipelineSteps steps;
+  steps.item = "group";
+  steps.upload = [&](int k, int slot, cudaStream_t s) {
+    return upload(slots.labels[slot], lab_host + (size_t)p.start(k) * vol_lab, (size_t)p.size(k) * vol_lab, device, s);
+  };
+  steps.passes = [&](int k, int slot, cudaStream_t s) {
+    return run_passes(slots.labels[slot], label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags,
+                      slots.plane(slot, 0), dc, s, p.size(k));
+  };
+  steps.download = [&](int k, int slot, cudaStream_t s) {
+    return download(out + p.start(k) * vol, slots.plane(slot, 0), (size_t)p.size(k) * vol_out, device, s);
+  };
+  if ((rc = run_pipeline(dc, device, (int)p.count, steps))) return rc;   // every download has landed
+  if (groups) *groups = p.count;
+  return 0;
+}
+
+int edtb200_feature_transform_stack(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy,
+                                    int64_t sz, int64_t count, float wx, float wy, float wz, int black_border,
+                                    int flags, float* dist_out, int32_t* const* idx_out, int device, void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  const int64_t vol = sx * sy * sz;
+  if (vol == 0 || count == 0) return 0;
+  if (!labels || !idx_out) return fail(EDTB200_EINVAL, "null pointer");
+  for (int k = 0; k < ndim; ++k)
+    if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
+  const int64_t total = vol * count;
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  // host buffers are staged through the cached labels and distances and one scratch for the planes;
+  // a distance volume and an index plane are 4 bytes per voxel
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, vol_bytes = (size_t)total * sizeof(float);
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  Scratch planes;
+  if (!io.out_dev) {
+    if (dist_out) CUDA_TRY(grow(dc->dist, dc->dist_bytes, vol_bytes));
+    if (planes.alloc(*dc, (size_t)ndim * vol_bytes, io.stream) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(EDTB200_ENOMEM, "no device memory for the index planes");
+    }
+  }
+  float* d_dist = dist_out ? io.out(dist_out, vol_bytes, dc->dist) : nullptr;
+  int32_t* d_idx[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < ndim; ++k)
+    d_idx[k] = io.out(idx_out[k], vol_bytes, io.out_dev ? nullptr : planes.get<int32_t>() + (size_t)k * total);
+  rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_dist,
+                          d_idx, *dc, io.stream, count);
+  return rc ? rc : io.finish();
 }
 
 int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const unsigned char* graph, int ndim,

@@ -19,10 +19,13 @@
 
 namespace edtb200 {
 
+// A stack of volumes laid end to end along z is sz / depth volumes of depth slices each: a Z code is
+// a row within its voxel's own volume, and so is the z coordinate written.
 struct SiteCodes {
   const int* axis[3];     // x, y, z code planes (the first ndim are read)
   int ndim;
   int64_t sx, sy, sz;
+  int64_t depth;          // slices per volume (sz: one volume)
 };
 
 struct SitePlanes {
@@ -55,18 +58,19 @@ resolve_sites_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, S
     const int64_t rem = i - pz * plane;
     const int64_t py = rem / c.sx;
     const int64_t px = rem - py * c.sx;
-    int64_t q[3] = {px, py, pz};
+    const int64_t z0 = c.depth == c.sz ? 0 : pz / c.depth * c.depth;     // the volume's first slice
+    int64_t q[3] = {px, py, pz - z0};
     const bool self = zero_is_background && labels[i] == 0;
     int step = self ? kStepSelf : kStepVertex;
 #pragma unroll
     for (int k = 2; k >= 1; --k) {
       if (k >= c.ndim || step != kStepVertex) continue;
       int row = 0;
-      step = site_step(false, __ldg(c.axis[k] + px + c.sx * (q[1] + c.sy * q[2])), &row);
+      step = site_step(false, __ldg(c.axis[k] + px + c.sx * (q[1] + c.sy * (z0 + q[2]))), &row);
       if (step != kStepNone) q[k] = row;
     }
     if (step == kStepVertex) {
-      const int code = __ldg(c.axis[0] + px + c.sx * (q[1] + c.sy * q[2]));
+      const int code = __ldg(c.axis[0] + px + c.sx * (q[1] + c.sy * (z0 + q[2])));
       if (code == kSiteNone) step = kStepNone;
       else q[0] = code;
     }

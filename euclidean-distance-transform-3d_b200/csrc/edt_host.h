@@ -201,7 +201,7 @@ int launch_later_sites(const void* labels, const float* fin, float* fout, int* c
                        cudaStream_t stream);
 template <int Bytes>
 int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim, int64_t sx, int64_t sy,
-                         int64_t sz, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
+                         int64_t sz, int64_t count, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
                          cudaStream_t stream);
 // The two halves of that resolution for the chunked feature transform (edt_feature.cuh): phase 1
 // resolves the X and Y codes of a slab into sites within each slice, phase 2 follows the last axis's

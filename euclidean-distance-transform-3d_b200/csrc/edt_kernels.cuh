@@ -277,10 +277,13 @@ template <> struct Vec4Labels<8> {
 // every row (y, z) padded to wpr = ceil(sx / 32) whole words, row (y, z) at word (z * sy + y) * wpr:
 //   y   bit = y == 0 || L(x, y, z) != L(x, y - 1, z)     (the Y pass's run starts)
 //   z   bit = z == 0 || L(x, y, z) != L(x, y, z - 1)     (the Z pass's run starts; 3-D only, else null)
+// In a stack of volumes laid end to end along z, z counts within the voxel's own volume: every
+// depth-th slice starts a volume, and its z bits are all set.
 struct XPlanes {
   uint32_t* y;
   uint32_t* z;
   int64_t sy;              // rows per z
+  int64_t depth;           // slices per volume (z planes only)
 };
 
 // A lane's 4-bit nibble of a 128-voxel block (voxels 4 lane .. 4 lane + 3) -> the block's 32-bit
@@ -648,6 +651,7 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
   const int pro = (Planes == 2 && j0 < j1 && j0 % nz != 0) ? 1 : 0;
   const int64_t first = j0 - pro, count = j1 - first;
   int band = (int)(first / nz), z = (int)(first - band * nz);     // item of stage i, advanced per stage
+  int vz = (int)(z % planes.depth);                  // z within its volume, advanced with z
   // thread 0: the next stage to issue, its item and its slot
   int64_t issued = 0;
   int issue_band = band, issue_z = z, issue_slot = 0;
@@ -706,7 +710,7 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
 #pragma unroll
         for (int a = 0; a < Planes; ++a) {
           uint32_t nib = in_row ? 15u : 0u;                       // first row along the axis: all start
-          if (in_row && (a == 0 ? y : z) > 0)
+          if (in_row && (a == 0 ? y > 0 : vz != 0))
             nib = (u[a][0] != here[0] ? 1u : 0u) | (u[a][1] != here[1] ? 2u : 0u) |
                   (u[a][2] != here[2] ? 4u : 0u) | (u[a][3] != here[3] ? 8u : 0u);
           // word w of block b sits in lanes 8w .. 8w + 7; lane c takes word c = 4 b + w
@@ -723,6 +727,7 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
     if (threadIdx.x == 0 && issued < count) issue_next();   // stage i + S - 1, into the slot of i - 1
     prev_slot = slot;
     if (++slot == stages) { slot = 0; phase ^= 1u; }
+    if (++vz == planes.depth) vz = 0;                // nz is a whole number of volumes: wraps with z
     if (++z == nz) { z = 0; ++band; }
   }
   if (stat.counter) {

@@ -343,16 +343,17 @@ int launch_later_sites(const void* labels, const float* fin, float* fout, int* c
   return 0;
 }
 
-// Site codes of every pass -> one coordinate plane per axis (edt_feature.cuh).
+// Site codes of every pass -> one coordinate plane per axis (edt_feature.cuh), over `count` volumes
+// of (sx, sy, sz) laid end to end.
 template <int Bytes>
 int launch_resolve_sites(const void* labels, const int* const codes[3], int ndim, int64_t sx, int64_t sy,
-                         int64_t sz, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
+                         int64_t sz, int64_t count, bool zero_is_background, int32_t* const idx[3], DeviceCache& dc,
                          cudaStream_t stream) {
-  const int64_t total = sx * sy * sz;
+  const int64_t total = sx * sy * sz * count;
   int64_t blocks = (total + 255) / 256;
   const int64_t cap = (int64_t)dc.sm_count * 8;
   if (blocks > cap) blocks = cap;
-  SiteCodes c{{codes[0], codes[1], codes[2]}, ndim, sx, sy, sz};
+  SiteCodes c{{codes[0], codes[1], codes[2]}, ndim, sx, sy, sz * count, sz};
   SitePlanes out{{idx[0], idx[1], idx[2]}};
   resolve_sites_kernel<Bytes><<<(unsigned)blocks, 256, 0, stream>>>(
       static_cast<const typename LabelOf<Bytes>::type*>(labels), c, zero_is_background ? 1 : 0, out);
@@ -410,7 +411,7 @@ int launch_compose_sites(const void* labels, int* codes_last, const int32_t* par
                                                     edtb200::host::PassArith,                            \
                                                     edtb200::host::DeviceCache&, cudaStream_t);          \
   template int edtb200::host::launch_resolve_sites<B>(const void*, const int* const*, int, int64_t,      \
-                                                      int64_t, int64_t, bool, int32_t* const*,           \
+                                                      int64_t, int64_t, int64_t, bool, int32_t* const*,  \
                                                       edtb200::host::DeviceCache&, cudaStream_t);        \
   template int edtb200::host::launch_slice_sites<B>(const void*, const int*, int*, int64_t, int64_t, int64_t, \
                                                     bool, int32_t*, edtb200::host::DeviceCache&, cudaStream_t); \

@@ -35,8 +35,8 @@ extern "C" {
  * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
- * edtb200_transform_voxel_graph_chunked) keep the
- * number: every 202-level entry point
+ * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack)
+ * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up. */
 #define EDTB200_VERSION 202
 
@@ -129,6 +129,53 @@ int edtb200_feature_transform(const void *labels, int label_bytes, int ndim,
                               float wx, float wy, float wz,
                               int black_border, int flags, float *dist_out,
                               int32_t *const *idx_out, int device, void *stream);
+
+/* A stack of `count` volumes of one geometry (sx, sy, sz), laid back to back (volume b starts at
+ * voxel b * sx * sy * sz), each transformed on its own as edtb200_transform would: its result is
+ * that call's bit for bit.  No line crosses from one volume into the next, black_border applies to
+ * every volume's own faces, and every pass keeps one volume's extents for its arithmetic.  Each pass
+ * is ONE launch over the whole stack (the X pass over count * sy * sz rows; the Y pass walks
+ * count * sz slices; the Z pass walks the volumes), so many small volumes cost what one volume of
+ * their total size costs -- for example the 2-D transform of every z slice of an anisotropic stack
+ * (ndim 2, count = depth), or a batch of masks of a training step.
+ *
+ *   labels, out   count * sx*sy*sz labels / float32; BOTH on the device (EDTB200_LABELS_ON_DEVICE |
+ *                 EDTB200_OUT_ON_DEVICE) or both on the host: mixed residency is EDTB200_EINVAL
+ *   flags         EDTB200_SQRT / EDTB200_SIGNED and the residency flags
+ *   device_bytes  host buffers only (ignored on the device): the budget B of the call's device memory,
+ *                 0 = the memory free on the device less EDTB200_CHUNK_RESERVE
+ *   groups        NULL, or int64_t[1] that receives the number of groups the call ran (1 on the device;
+ *                 0 on an error or an empty stack)
+ * On the device the call is asynchronous on `stream` and takes no lock.  Host buffers go through the
+ * device in groups of whole volumes, pipelined through two device slots as edtb200_transform_batch
+ * pipelines its volumes, planned as one phase of edtb200_transform_chunked whose slices are volumes:
+ * a volume costs V (label_bytes + 4 + s) bytes, s = 8 when a later pass takes the long-line kernel
+ * (its two scratch volumes); a group holds at most 512 MiB of those bytes (at least one volume), so
+ * that the copies of one group overlap the passes of the next; one group when the whole stack fits B
+ * and that cap, else two slots of min(cap, floor(B / (2 * that))) volumes each; EDTB200_ENOMEM when
+ * not even one volume fits, and the message names the least budget that works.  On label noise the X pass may also take the run-start planes of
+ * at most 1/4 byte per voxel outside the budget (none when there is no room).  The device's cached
+ * whole-volume buffers are freed first, as edtb200_transform_chunked does, and the host call returns
+ * when every result has landed; labels and out must not overlap.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, emptiness (count 0 or
+ * an empty volume returns 0 touching nothing), pointers, residency, overlap, device. */
+int edtb200_transform_stack(const void *labels, int label_bytes, int ndim,
+                            int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                            float wx, float wy, float wz,
+                            int black_border, int flags, float *out,
+                            int device, size_t device_bytes, int64_t *groups, void *stream);
+
+/* edtb200_feature_transform of a stack of `count` volumes laid back to back, as for
+ * edtb200_transform_stack: each volume on its own, one launch per pass for the whole stack.  Every
+ * plane (idx_out[k], dist_out) covers the whole stack, and the coordinates are those within the
+ * voxel's own volume (a face site is -1 or n on its axis of that volume; no site is -1 everywhere).
+ * Residency and device memory as edtb200_feature_transform, for count * sx*sy*sz voxels: host buffers
+ * are staged in one shot, with no grouping and no chunking. */
+int edtb200_feature_transform_stack(const void *labels, int label_bytes, int ndim,
+                                    int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                                    float wx, float wy, float wz,
+                                    int black_border, int flags, float *dist_out,
+                                    int32_t *const *idx_out, int device, void *stream);
 
 /* The same transform of ONE host volume spread over several GPUs of this process
  * (`devices[0..ndevices)`, distinct ordinals): SURVEY.md section 8b's `devices[] / ndevices`.

@@ -76,6 +76,21 @@ solid = np.ones((48, 96, 40), dtype=np.uint16, order="F")
 solid[:, :, 20:] = 2
 check("solid edt", edt.edt(solid, anisotropy=(2, 1, 3), black_border=True),
       oracle.edt(solid, anisotropy=(2, 1, 3), black_border=True))
+# stacks (stacked=True): one launch per pass over many volumes -- the plane plan on label noise whose
+# next volume repeats the last slice, odd-sized volumes (Z pass without TMA), long-line weights, host
+# groups and the feature resolver across volumes
+noise = rng.integers(1, 1 << 20, (4, 9, 40, 64)).astype(np.uint32)
+noise[1:, 0] = noise[:-1, -1]
+for _ in range(2):
+  got = edt.edtsq(noise, stacked=True)
+check("stack noise", got, np.stack([oracle.edtsq(v) for v in noise]))
+odd = np.stack([cases.random_volume(rng, (5, 7, 9), "blocks", np.uint16) for _ in range(6)])
+check("stack odd", edt.sdf(odd, black_border=True, stacked=True), np.stack([oracle.sdf(v, black_border=True) for v in odd]))
+check("stack long", edt.edtsq(odd, anisotropy=(0.7, 1.3, 2.9), stacked=True, max_device_bytes=2 * 315 * 14),
+      np.stack([oracle.edtsq(v, anisotropy=(0.7, 1.3, 2.9)) for v in odd]))
+_, idx = edt.feature_transform(odd, stacked=True, return_distances=True)
+for b in range(len(odd)):
+  check("stack feature %d" % b, idx[:, b], edt.feature_transform(odd[b]))
 # per-label statistics and box-restricted extraction
 import torch  # noqa: E402
 lt = torch.from_numpy(np.ascontiguousarray(vor.astype(np.int32))).cuda()

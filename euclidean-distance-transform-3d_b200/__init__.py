@@ -46,6 +46,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
 
+ECUDA = -2                # EDTB200_ECUDA
 ENOMEM = -3               # EDTB200_ENOMEM
 
 
@@ -96,6 +97,8 @@ def _lib():
   lib.edtb200_feature_transform_stack.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci,
                                                   vp]
   lib.edtb200_feature_transform_stack.restype = ci
+  lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
+  lib.edtb200_expand_gather.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
   lib.edtb200_transform_multi.restype = ci
   lib.edtb200_transform_batch.argtypes = [vp, vp, ci, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, ci]
@@ -610,8 +613,8 @@ def _pick(device, devices, max_device_bytes=None, stacked=False):
 # result of the one-shot transform bit for bit; with None a one-shot transform that runs out of
 # device memory falls back to that once (see _transform_host).
 #
-# `stacked=True` (edt, edtsq, sdf, sdfsq, edt_cuda, feature_transform) takes a 2-D to 4-D array whose
-# slowest axis in memory (axis 0 of a C-ordered array, the last of an F-ordered one) indexes
+# `stacked=True` (edt, edtsq, sdf, sdfsq, edt_cuda, feature_transform, expand_labels) takes a 2-D to
+# 4-D array whose slowest axis in memory (axis 0 of a C-ordered array, the last of an F-ordered one) indexes
 # independent volumes of 1 to 3 dimensions: each is transformed on its own, with one launch per pass
 # for the whole stack.  `anisotropy` has one entry per volume axis, black_border applies to every
 # volume's own faces, and the result has the input's shape and memory order, equal to np.stack of
@@ -995,15 +998,6 @@ def feature_transform(data, anisotropy=None, black_border=False, *, signed=False
   return (dist, idx) if return_distances else idx
 
 
-def _same_size_signed(torch, t):
-  """t viewed as a signed integer type of its width when torch's indexing may not take its own
-  (the unsigned types beyond uint8)."""
-  for name, signed in (("uint16", torch.int16), ("uint32", torch.int32), ("uint64", torch.int64)):
-    if t.dtype == getattr(torch, name, None):
-      return t.view(signed)
-  return t
-
-
 def _expand_host(arr, distance, anisotropy, device, max_device_bytes):
   """expand_labels of a contiguous numpy array through the chunked feature transform: the labels are
   gathered on the host, a bounded range of voxels at a time, at the background voxels that grow."""
@@ -1024,18 +1018,86 @@ def _expand_host(arr, distance, anisotropy, device, max_device_bytes):
   return out
 
 
-def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device_bytes=None):
+def _expand_device(t, distance, anisotropy, stacked):
+  """expand_labels of a torch CUDA tensor (with `stacked`, a stack of volumes along its slowest axis in
+  memory) on its current stream: the signed feature transform, then one gather kernel
+  (edtb200_expand_gather) over the memory-order view and the x-fastest index planes the transform
+  used.  The result keeps t's strides."""
+  import torch
+  dims = t.dim()
+  if not t.is_contiguous() and not t.permute(*reversed(range(dims))).is_contiguous():
+    t = t.contiguous()
+  dist, idx = _feature_device(t, anisotropy, False, FLAG_SIGNED, True, stacked=stacked)
+  if t.numel() == 0:
+    return t.clone()
+  # _feature_device returns F-ordered planes where it ran on the transposed view
+  fortran = dims > 1 and not idx[0].is_contiguous()
+  lab = (t.permute(*reversed(range(dims))) if fortran else t).contiguous()
+  vnd = dims - 1 if stacked else dims
+  count = int(lab.shape[0]) if stacked else 1
+  (sx, sy, sz), _ = _x_fastest(lab.shape[1:] if stacked else lab.shape, (1.0,) * vnd, False)
+  # x-fastest axis j is the caller's axis j when F-ordered, else axis vnd - 1 - j (as in _feature_device)
+  ptrs = (ctypes.c_void_p * vnd)(*[idx[j if fortran else vnd - 1 - j].data_ptr() for j in range(vnd)])
+  flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE | (FLAG_LABELS_FLOAT if lab.is_floating_point() else 0)
+  out = torch.empty_like(lab)
+  stream = torch.cuda.current_stream(lab.device).cuda_stream
+  _check(_lib().edtb200_expand_gather(
+    lab.data_ptr(), lab.element_size(), vnd, sx, sy, sz, count, dist.data_ptr(), ptrs, float(distance) ** 2, flags,
+    out.data_ptr(), lab.device.index, ctypes.c_void_p(stream)))
+  return out.permute(*reversed(range(dims))) if fortran else out
+
+
+def _expand_stack(labels, on_device, distance, anisotropy, device, max_device_bytes):
+  """expand_labels(stacked=True).  A host stack is uploaded whole, grown on the device and copied back,
+  as a host volume is; one that does not fit raises EDTError with code ENOMEM."""
+  import torch
+  arr = None if on_device is not None else np.asarray(np.array(labels) if isinstance(labels, list) else labels)
+  vnd = _stack_dims(on_device.dim() if on_device is not None else arr.ndim)
+  if max_device_bytes is not None:
+    raise ValueError("stacked=True stages the whole stack on the GPU at once; it cannot be combined with "
+                     "max_device_bytes")
+  anisotropy = _stack_anisotropy(vnd, anisotropy)
+  if on_device is not None:
+    return _expand_device(on_device, distance, anisotropy, True)
+  arr, order = _stack_order(arr)
+  if _label_view(arr) is None:
+    raise TypeError("expand_labels: unsupported label dtype %s" % arr.dtype)
+  if arr.size == 0:
+    return arr.copy(order=order)
+  if device_count() == 0:
+    raise EDTError("edt_b200 error %d: no usable CUDA device; this library has no CPU fallback" % ECUDA, ECUDA)
+  raw = arr if arr.dtype.kind == "f" else arr.view(np.uint8 if arr.itemsize == 1 else np.dtype("i%d" % arr.itemsize))
+  try:
+    out = _expand_device(torch.from_numpy(raw).to(torch.device("cuda", int(device))), distance, anisotropy, True)
+  except torch.cuda.OutOfMemoryError as e:
+    raise EDTError("edt_b200 error %d: the stack of %d bytes does not fit on the GPU (%s)" % (ENOMEM, arr.nbytes, e),
+                   ENOMEM) from e
+  return out.cpu().numpy().view(arr.dtype)
+
+
+def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device_bytes=None, stacked=False):
   """skimage.segmentation.expand_labels on the GPU: every background voxel (label 0) whose nearest
   labelled voxel lies within `distance` takes that voxel's label; labelled voxels keep theirs.
-  "Within" compares the squared distance (as sdfsq computes it, in float64) with distance**2.
-  The result has the dtype, shape and memory order of `labels`; a torch CUDA tensor in gives one
-  out.  Built on feature_transform(signed=True): the labels are gathered on the device.
+  "Within" compares the squared distance (as sdfsq computes it, in float64) with distance**2, so a
+  negative distance acts as its magnitude, NaN grows nothing and inf grows every background voxel of
+  a volume that has a label.  For float labels background is the value 0 (-0.0 too), and every
+  label, -0.0 and NaN payloads included, is copied bit for bit.  The result has the dtype, shape and
+  memory order of `labels`; a torch CUDA tensor in gives one out, computed on the current stream.
+  Built on feature_transform(signed=True); one CUDA kernel then gathers the labels on the device.
 
   `max_device_bytes=N` (2-D / 3-D host arrays) runs the feature transform in chunks that fit N bytes
   of device memory (0: what the GPU has free) and gathers the labels on the host; with None a host
-  array too large for the device falls back to that once."""
+  array too large for the device falls back to that once.
+
+  `stacked=True` takes a 2-D to 4-D array whose slowest axis in memory indexes independent volumes,
+  as edt(stacked=True) does: every volume grows on its own, with one launch per pass for the whole
+  stack, and the result equals np.stack of the per-volume calls.  `anisotropy` has one entry per
+  volume axis.  The whole stack is staged on the GPU at once: it cannot be combined with
+  max_device_bytes, and a host stack that does not fit raises EDTError with code ENOMEM."""
   import torch
   on_device = _device_array(labels)
+  if stacked:
+    return _expand_stack(labels, on_device, distance, anisotropy, device, max_device_bytes)
   if on_device is None:
     arr = np.asarray(labels)
     if not arr.flags.c_contiguous and not arr.flags.f_contiguous:
@@ -1061,24 +1123,7 @@ def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device
     return _expand_host(arr, distance, anisotropy, device, max_device_bytes)
   if max_device_bytes is not None:
     _chunk_budget(max_device_bytes, True, None, on_device.dim())
-  t = on_device
-  if not t.is_contiguous() and not t.permute(*reversed(range(t.dim()))).is_contiguous():
-    t = t.contiguous()
-  dist, idx = _feature_device(t, anisotropy, False, FLAG_SIGNED, True)
-  if t.numel() == 0:
-    return t.clone()
-  # the site as a C-order linear index; -1 (no site) is masked out below
-  lin = torch.zeros(t.shape, dtype=torch.int64, device=t.device)
-  step = 1
-  for k in reversed(range(t.dim())):
-    lin += idx[k].to(torch.int64) * step
-    step *= int(t.shape[k])
-  take = _same_size_signed(torch, t)
-  grow = (take == 0) & (idx[0] >= 0) & (dist.abs().to(torch.float64) <= float(distance) ** 2)
-  grown = torch.where(grow, take.reshape(-1)[lin.clamp(min=0)], take)
-  out = torch.empty_like(t)                  # t's memory order
-  _same_size_signed(torch, out).copy_(grown)
-  return out
+  return _expand_device(on_device, distance, anisotropy, False)
 
 
 # ---------------------------------------------------------------------------------------

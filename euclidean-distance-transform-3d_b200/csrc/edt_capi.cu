@@ -1525,6 +1525,36 @@ int edtb200_feature_transform_stack(const void* labels, int label_bytes, int ndi
   return rc ? rc : io.finish();
 }
 
+int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                          int64_t count, const float* sqdist, const int32_t* const* idx, double limit_sq, int flags,
+                          void* out, int device, void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (sx * sy * sz == 0 || count == 0) return 0;
+  if (!labels || !sqdist || !idx) return fail(EDTB200_EINVAL, "null pointer");
+  for (int k = 0; k < ndim; ++k)
+    if (!idx[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
+  if (!out) return fail(EDTB200_EINVAL, "null pointer");
+  const int both = EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE;
+  if ((flags & both) != both || (flags & ~(both | EDTB200_LABELS_FLOAT)))
+    return fail(EDTB200_EINVAL, "edtb200_expand_gather works on device buffers only: flags must be "
+                                "EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE, optionally with EDTB200_LABELS_FLOAT "
+                                "(got %d)", flags);
+  const bool as_float = flags & EDTB200_LABELS_FLOAT;
+  if (as_float && label_bytes != 4 && label_bytes != 8)
+    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  if ((rc = probe(device, &dc))) return rc;
+  const int32_t* planes[3] = {idx[0], ndim >= 2 ? idx[1] : nullptr, ndim >= 3 ? idx[2] : nullptr};
+  return with_label_width(label_bytes, [&](auto b) {        // asynchronous on the caller's stream, no lock
+    return launch_expand_gather<b>(labels, sqdist, planes, ndim, sx, sy, sz, count, limit_sq, as_float, out, *dc,
+                                   static_cast<cudaStream_t>(stream_v));
+  });
+}
+
 int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const unsigned char* graph, int ndim,
                                   int64_t sx, int64_t sy, int64_t sz, float wx, float wy, float wz,
                                   int black_border, int flags, float* out, int device, void* stream_v) {

@@ -81,6 +81,50 @@ resolve_sites_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, S
   }
 }
 
+// What expand_gather_kernel reads besides the labels: a signed feature transform's squared distances
+// and x-fastest index planes (the first ndim are read) over the stack of count volumes of
+// (sx, sy, sz) laid back to back, `vol` voxels each.  Coordinates are within each voxel's own volume,
+// and idx[0] is -1 where there is no site.
+struct ExpandSites {
+  const float* sqdist;
+  const int32_t* axis[3];
+  int ndim;
+  int64_t sx, sy, sz, vol, total;
+};
+
+// expand_labels: every background voxel whose nearest site lies within the limit takes that site's
+// label; every other voxel keeps its own.  A voxel grows iff it is background, has a site (idx[0]
+// >= 0) inside its volume, and (double)|sqdist| <= limit_sq.  Background is a label whose bits are all
+// zero, or with as_float (4- or 8-byte IEEE labels) whose value is zero, so that -0.0 is background
+// too.  Labels are copied as raw bits, so -0.0 and NaN payloads survive.  A labelled voxel reads
+// nothing but its label; a background voxel reads its site's distance only when it has one, and the
+// other planes only when it grows.
+// `out` may be `labels` itself (no __restrict__ on either): only background voxels change, and a
+// background voxel reads only its own label and its site's, and a site -- the nearest voxel of
+// another label to a background voxel under the signed transform -- is always a labelled voxel,
+// which nobody writes.  A site outside the volume (a face position of a black_border transform) has
+// no label and grows nothing.
+template <int Bytes>
+__global__ void __launch_bounds__(256)
+expand_gather_kernel(const typename LabelOf<Bytes>::type* labels, ExpandSites s, double limit_sq, int as_float,
+                     typename LabelOf<Bytes>::type* out) {
+  using LT = typename LabelOf<Bytes>::type;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < s.total; i += (int64_t)gridDim.x * blockDim.x) {
+    LT v = labels[i];
+    const LT magnitude = as_float ? (LT)(v << 1) : v;      // the sign bit shifted out: -0.0 == 0
+    if (magnitude == 0) {
+      const int64_t qx = __ldg(s.axis[0] + i);
+      if (qx >= 0 && (double)fabsf(__ldg(s.sqdist + i)) <= limit_sq) {
+        const int64_t qy = s.ndim >= 2 ? __ldg(s.axis[1] + i) : 0;
+        const int64_t qz = s.ndim >= 3 ? __ldg(s.axis[2] + i) : 0;
+        if (qx < s.sx && (uint64_t)qy < (uint64_t)s.sy && (uint64_t)qz < (uint64_t)s.sz)
+          v = labels[i - i % s.vol + (qz * s.sy + qy) * s.sx + qx];
+      }
+    }
+    out[i] = v;
+  }
+}
+
 // Chunked feature transform, phase 1 (3-D): the X and Y codes of a slab of whole slices
 // (sx, sy, sz) -> every voxel's site (qx, qy) within its own slice, kSiteNone in both where it has
 // none.  qy is written over the Y codes (each is read at its own voxel only); the X codes are read at

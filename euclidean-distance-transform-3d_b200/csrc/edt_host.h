@@ -213,6 +213,12 @@ template <int Bytes>
 int launch_compose_sites(const void* labels, int* codes_last, const int32_t* part_x, const int32_t* part_y,
                          const SiteBox& box, bool zero_is_background, int32_t* out_x, int32_t* out_y, DeviceCache& dc,
                          cudaStream_t stream);
+// expand_labels' gather from a signed feature transform's distances and index planes over `count`
+// volumes (edt_feature.cuh); as_float: 4- / 8-byte IEEE labels, -0.0 is background.  out may be labels.
+template <int Bytes>
+int launch_expand_gather(const void* labels, const float* sqdist, const int32_t* const idx[3], int ndim, int64_t sx,
+                         int64_t sy, int64_t sz, int64_t count, double limit_sq, bool as_float, void* out,
+                         DeviceCache& dc, cudaStream_t stream);
 
 // Whether plan_later (edt_passes.cuh) sends a later-axis pass over geometry g with arithmetic
 // `arith` to the long-line kernel (edt_plan.cu).

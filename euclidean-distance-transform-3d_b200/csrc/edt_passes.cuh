@@ -393,6 +393,22 @@ int launch_compose_sites(const void* labels, int* codes_last, const int32_t* par
   return 0;
 }
 
+// expand_labels' gather over `count` volumes of (sx, sy, sz) laid end to end (edt_feature.cuh); out
+// may be labels.
+template <int Bytes>
+int launch_expand_gather(const void* labels, const float* sqdist, const int32_t* const idx[3], int ndim, int64_t sx,
+                         int64_t sy, int64_t sz, int64_t count, double limit_sq, bool as_float, void* out,
+                         DeviceCache& dc, cudaStream_t stream) {
+  using LT = typename LabelOf<Bytes>::type;
+  const int64_t vol = sx * sy * sz;
+  const ExpandSites s{sqdist, {idx[0], ndim >= 2 ? idx[1] : nullptr, ndim >= 3 ? idx[2] : nullptr}, ndim,
+                      sx, sy, sz, vol, vol * count};
+  expand_gather_kernel<Bytes><<<site_blocks(s.total, dc), 256, 0, stream>>>(
+      static_cast<const LT*>(labels), s, limit_sq, as_float ? 1 : 0, static_cast<LT*>(out));
+  CUDA_TRY(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace host
 }  // namespace edtb200
 
@@ -417,4 +433,7 @@ int launch_compose_sites(const void* labels, int* codes_last, const int32_t* par
                                                     bool, int32_t*, edtb200::host::DeviceCache&, cudaStream_t); \
   template int edtb200::host::launch_compose_sites<B>(const void*, int*, const int32_t*, const int32_t*,  \
                                                       const edtb200::SiteBox&, bool, int32_t*, int32_t*, \
+                                                      edtb200::host::DeviceCache&, cudaStream_t);        \
+  template int edtb200::host::launch_expand_gather<B>(const void*, const float*, const int32_t* const*, int, \
+                                                      int64_t, int64_t, int64_t, int64_t, double, bool, void*, \
                                                       edtb200::host::DeviceCache&, cudaStream_t);

@@ -35,7 +35,8 @@ extern "C" {
  * edtb200_host_alloc / _free; every 100-level entry point keeps its signature and meaning.
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
- * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack)
+ * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
+ * edtb200_expand_gather)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up. */
 #define EDTB200_VERSION 202
@@ -49,9 +50,10 @@ extern "C" {
                                        (src/edt.pyx:121-202) */
 #define EDTB200_LABELS_ON_DEVICE 4  /* `labels` is a device pointer on `device` */
 #define EDTB200_OUT_ON_DEVICE    8  /* `out` is a device pointer on `device` */
-#define EDTB200_LABELS_FLOAT    16  /* edtb200_transform_voxel_graph only: the 4- / 8-byte labels are
+#define EDTB200_LABELS_FLOAT    16  /* edtb200_transform_voxel_graph: the 4- / 8-byte labels are
                                        IEEE floats and foreground means value > 0, as the reference's
-                                       float instantiations test it (src/edt_voxel_graph.hpp:76, 151) */
+                                       float instantiations test it (src/edt_voxel_graph.hpp:76, 151);
+                                       edtb200_expand_gather: background means value == 0 */
 
 /* Residency, shared by edtb200_transform, edtb200_feature_transform and
  * edtb200_transform_voxel_graph: without EDTB200_LABELS_ON_DEVICE / EDTB200_OUT_ON_DEVICE the
@@ -176,6 +178,38 @@ int edtb200_feature_transform_stack(const void *labels, int label_bytes, int ndi
                                     float wx, float wy, float wz,
                                     int black_border, int flags, float *dist_out,
                                     int32_t *const *idx_out, int device, void *stream);
+
+/* expand_labels' gather (skimage.segmentation.expand_labels): every background voxel whose nearest
+ * labelled voxel lies within the limit takes that voxel's label, every other voxel keeps its own.
+ * The inputs are what edtb200_feature_transform_stack (or edtb200_feature_transform, count 1) returns
+ * with EDTB200_SIGNED, without EDTB200_SQRT and without black_border, for `count` volumes of
+ * (sx, sy, sz) laid back to back (volume b starts at voxel b * sx * sy * sz).
+ *   labels   count * sx*sy*sz labels of `label_bytes` (1, 2, 4 or 8) bytes, as given to that transform
+ *            but with float labels left as they are (not canonicalised)
+ *   sqdist   the transform's float32 squared distances (signed: negative on background)
+ *   idx      ndim int32 planes, idx[0] x, idx[1] y, idx[2] z: every voxel's site within its own
+ *            volume, idx[0] -1 where there is none
+ *   limit_sq the squared limit: a background voxel p grows iff idx[0][p] >= 0 and
+ *            (double)|sqdist[p]| <= limit_sq.  A caller with a distance d passes d * d, so a negative d
+ *            acts as |d|, NaN grows nothing and +inf grows every voxel that has a site.  A site
+ *            outside its volume (a face position of a black_border transform) grows nothing.
+ *   flags    EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE (every buffer is on `device`: host
+ *            buffers are not accepted), optionally with EDTB200_LABELS_FLOAT
+ *   out      count * sx*sy*sz labels; the grown volume.  It may be `labels` itself (in place).
+ * Background is a label whose bits are all zero; with EDTB200_LABELS_FLOAT (4- / 8-byte IEEE labels)
+ * a label whose value is zero, so -0.0 is background too.  Labels are copied as raw bits: -0.0 and
+ * NaN payloads survive exactly.  In place is exact because only background voxels change, and a
+ * background voxel reads only its own label and its site's, which is always a labelled voxel.
+ * One launch, asynchronous on `stream`, no lock, no allocation; it reads each input once: the
+ * labels, and for background voxels their first plane, and only where they have a site their
+ * distance, and only where they grow the other planes and the site's label.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, emptiness (count 0
+ * or an empty volume returns 0 touching nothing), pointers (labels, sqdist, idx, idx[k] for k < ndim,
+ * out: "null pointer" / "null index plane k"), residency and flags, EDTB200_LABELS_FLOAT width, device. */
+int edtb200_expand_gather(const void *labels, int label_bytes, int ndim,
+                          int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                          const float *sqdist, const int32_t *const *idx,
+                          double limit_sq, int flags, void *out, int device, void *stream);
 
 /* The same transform of ONE host volume spread over several GPUs of this process
  * (`devices[0..ndevices)`, distinct ordinals): SURVEY.md section 8b's `devices[] / ndevices`.

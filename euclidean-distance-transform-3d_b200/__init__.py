@@ -97,6 +97,14 @@ def _lib():
   lib.edtb200_feature_transform_stack.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci,
                                                   vp]
   lib.edtb200_feature_transform_stack.restype = ci
+  lib.edtb200_transform_bounded.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp,
+                                            ctypes.c_double]
+  lib.edtb200_transform_bounded.restype = ci
+  lib.edtb200_feature_transform_bounded.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp,
+                                                    ctypes.c_double]
+  lib.edtb200_feature_transform_bounded.restype = ci
+  lib.edtb200_bounded_plan.argtypes = [ci, i64, i64, i64, f32, f32, f32, ctypes.c_double, vp, vp]
+  lib.edtb200_bounded_plan.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
@@ -157,13 +165,29 @@ LATER_LAUNCH_FIELDS = ("kernel", "tx", "tma", "wide", "ctas", "int_hull", "epilo
 
 def last_later_launch():
   """Kernel variant of the last Y / Z pass this thread launched (edtb200_last_later_launch), as a
-  dict: kernel "tile" or "long", tile width tx, tma, wide, ctas (per SM), int_hull, epilogue,
-  all_double (every candidate formed in double)."""
+  dict: kernel "tile", "long" or "window" (a bounded transform's window kernel, whose radius is in
+  tx), tile width tx, tma, wide, ctas (per SM), int_hull, epilogue, all_double (every candidate
+  formed in double)."""
   info = (ctypes.c_int * len(LATER_LAUNCH_FIELDS))()
   _check(_lib().edtb200_last_later_launch(info))
   out = dict(zip(LATER_LAUNCH_FIELDS, (int(v) for v in info)))
-  out["kernel"] = "tile" if out["kernel"] == 0 else "long"
+  out["kernel"] = {0: "tile", 1: "long", 2: "window"}[out["kernel"]]
   return out
+
+
+def _bound(max_distance, voxel_graph=None, devices=None, stacked=False, max_device_bytes=None):
+  """max_distance as a float (None: unbounded), after rejecting a bad value and what the bounded
+  transforms do not cover."""
+  if max_distance is None:
+    return None
+  d = float(max_distance)
+  if not d >= 0.0:
+    raise ValueError("max_distance must be zero or more, got %r" % (max_distance,))
+  for given, name in ((voxel_graph is not None, "voxel_graph"), (devices is not None, "devices=[...]"),
+                      (stacked, "stacked=True"), (max_device_bytes is not None, "max_device_bytes")):
+    if given:
+      raise ValueError("max_distance cannot be combined with %s" % name)
+  return None if d == float("inf") else d
 
 
 def nvl(val, default_val):
@@ -283,10 +307,11 @@ def _result_buffer(count):
   return np.frombuffer(block, dtype=np.float32, count=count)
 
 
-def _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes=None):
+def _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes=None, bound=None):
   """`max_device_bytes` (an int) streams the volume through one GPU in chunks within that budget
   (edtb200_transform_chunked).  With None, a 2-D / 3-D volume whose one-shot transform runs out of
-  device memory is retried once that way, with the budget the device has free."""
+  device memory is retried once that way, with the budget the device has free.  `bound`: the
+  bounded transform's max_distance (edtb200_transform_bounded, one shot only)."""
   nd = data.ndim
   order = "F" if data.flags.f_contiguous else "C"
   if not data.flags.c_contiguous and not data.flags.f_contiguous:
@@ -308,6 +333,9 @@ def _transform_host(data, anisotropy, black_border, flags, device, max_device_by
     return out.reshape(data.shape, order=order)
   args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), int(flags),
           out.ctypes.data, int(device))
+  if bound is not None:
+    _check(lib.edtb200_transform_bounded(*args, None, bound))
+    return out.reshape(data.shape, order=order)
   if max_device_bytes is None:
     try:
       _check(lib.edtb200_transform(*args, None))
@@ -389,7 +417,7 @@ def _device_array(data):
   return None
 
 
-def _front_door_device(t, anisotropy, black_border, voxel_graph, flags, fixed_dims):
+def _front_door_device(t, anisotropy, black_border, voxel_graph, flags, fixed_dims, bound=None):
   """Device-resident input to the reference-named functions: same semantics, result returned as a
   torch CUDA tensor (which itself exports DLPack and `__cuda_array_interface__`).  A Fortran-ordered
   array is transformed through its transposed (C-ordered) view with the anisotropy reversed, which
@@ -440,7 +468,7 @@ def _front_door_device(t, anisotropy, black_border, voxel_graph, flags, fixed_di
     out = edt_cuda(t, anisotropy, black_border, sqrt=sqrt, voxel_graph=graph)
     out -= edt_cuda(t == 0, anisotropy, black_border, sqrt=sqrt, voxel_graph=graph)
   else:
-    out = edt_cuda(t, anisotropy, black_border, sqrt=sqrt, signed=signed, voxel_graph=graph)
+    out = edt_cuda(t, anisotropy, black_border, sqrt=sqrt, signed=signed, voxel_graph=graph, max_distance=bound)
   return out.permute(*reversed(range(dims))) if fortran else out
 
 
@@ -459,15 +487,15 @@ def _chunk_budget(max_device_bytes, on_device, voxel_graph, dims):
 
 
 def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None, max_device_bytes=None,
-                stacked=False):
-  """Argument handling of edtsq(), src/edt.pyx:276-310."""
+                stacked=False, bound=None):
+  """Argument handling of edtsq(), src/edt.pyx:276-310.  bound: max_distance after _bound."""
   if stacked:
     return _stack_front_door(data, anisotropy, black_border, voxel_graph, flags, device, max_device_bytes)
   on_device = _device_array(data)
   if on_device is not None:
     if max_device_bytes is not None:
       _chunk_budget(max_device_bytes, True, voxel_graph, on_device.dim())
-    return _front_door_device(on_device, anisotropy, black_border, voxel_graph, flags, fixed_dims)
+    return _front_door_device(on_device, anisotropy, black_border, voxel_graph, flags, fixed_dims, bound)
   if isinstance(data, list):
     data = np.array(data)
   data = np.asarray(data)
@@ -500,7 +528,7 @@ def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixe
     anisotropy = nvl(anisotropy, (1.0, 1.0, 1.0))
   else:
     raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
-  return _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes)
+  return _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes, bound)
 
 
 # ---------------------------------------------------------------------------------------
@@ -620,70 +648,87 @@ def _pick(device, devices, max_device_bytes=None, stacked=False):
 # volume's own faces, and the result has the input's shape and memory order, equal to np.stack of
 # the per-volume calls.  For host arrays max_device_bytes is the budget of the groups of whole volumes
 # that go through the GPU at once.
+#
+# `max_distance=d` (every function below, edt_cuda and feature_transform) computes only the distances
+# up to d: where the unbounded squared distance S (|S| for sdf / sdfsq) has (double)S <= d * d the
+# result is the unbounded one bit for bit, elsewhere +inf (-inf on signed background); unsigned
+# background stays 0.  Later passes then only look d / w rows either way (include/edt_b200.h,
+# DESIGN.md section 5).  None or +inf is the unbounded transform; d = 0 is allowed, a negative or NaN
+# d is a ValueError, and so is max_distance with voxel_graph, devices=[...], stacked=True or
+# max_device_bytes.
 
 def edtsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-          *, device=0, devices=None, max_device_bytes=None, stacked=False):
+          *, device=0, devices=None, max_device_bytes=None, stacked=False, max_distance=None):
   """Squared anisotropic multi-label EDT of a 1-D, 2-D or 3-D array (src/edt.pyx:245-310).
   `devices=[0, 1, ...]` spreads one host volume over several GPUs (see _transform_host)."""
+  bound = _bound(max_distance, voxel_graph, devices, stacked, max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, 0, _pick(device, devices, max_device_bytes, stacked),
-                     max_device_bytes=max_device_bytes, stacked=stacked)
+                     max_device_bytes=max_device_bytes, stacked=stacked, bound=bound)
 
 
 def edt(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-        *, device=0, devices=None, max_device_bytes=None, stacked=False):
+        *, device=0, devices=None, max_device_bytes=None, stacked=False, max_distance=None):
   """Anisotropic multi-label EDT (src/edt.pyx:205-242); the sqrt is fused into the last pass."""
+  bound = _bound(max_distance, voxel_graph, devices, stacked, max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT,
                      _pick(device, devices, max_device_bytes, stacked), max_device_bytes=max_device_bytes,
-                     stacked=stacked)
+                     stacked=stacked, bound=bound)
 
 
 def sdf(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
-        *, device=0, devices=None, max_device_bytes=None, stacked=False):
+        *, device=0, devices=None, max_device_bytes=None, stacked=False, max_distance=None):
   """Signed distance function, edt(data) - edt(data == 0) (src/edt.pyx:121-158), computed as
   one transform with background as a label and the sign applied in the last store."""
+  bound = _bound(max_distance, voxel_graph, devices, stacked, max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT | FLAG_SIGNED,
                      _pick(device, devices, max_device_bytes, stacked), max_device_bytes=max_device_bytes,
-                     stacked=stacked)
+                     stacked=stacked, bound=bound)
 
 
 def sdfsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, *, device=0, devices=None,
-          max_device_bytes=None, stacked=False):
+          max_device_bytes=None, stacked=False, max_distance=None):
   """Squared signed distance function (src/edt.pyx:161-202)."""
+  bound = _bound(max_distance, voxel_graph, devices, stacked, max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SIGNED,
                      _pick(device, devices, max_device_bytes, stacked), max_device_bytes=max_device_bytes,
-                     stacked=stacked)
+                     stacked=stacked, bound=bound)
 
 
-def edt1dsq(data, anisotropy=1.0, black_border=False, *, device=0):
-  return _front_door(data, anisotropy, black_border, None, 0, device, fixed_dims=1)
+def edt1dsq(data, anisotropy=1.0, black_border=False, *, device=0, max_distance=None):
+  return _front_door(data, anisotropy, black_border, None, 0, device, fixed_dims=1, bound=_bound(max_distance))
 
 
-def edt1d(data, anisotropy=1.0, black_border=False, *, device=0):
-  return _front_door(data, anisotropy, black_border, None, FLAG_SQRT, device, fixed_dims=1)
+def edt1d(data, anisotropy=1.0, black_border=False, *, device=0, max_distance=None):
+  return _front_door(data, anisotropy, black_border, None, FLAG_SQRT, device, fixed_dims=1,
+                     bound=_bound(max_distance))
 
 
 def edt2dsq(data, anisotropy=(1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-            *, device=0, max_device_bytes=None):
+            *, device=0, max_device_bytes=None, max_distance=None):
+  bound = _bound(max_distance, voxel_graph, max_device_bytes=max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, 0, device, fixed_dims=2,
-                     max_device_bytes=max_device_bytes)
+                     max_device_bytes=max_device_bytes, bound=bound)
 
 
 def edt2d(data, anisotropy=(1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-          *, device=0, max_device_bytes=None):
+          *, device=0, max_device_bytes=None, max_distance=None):
+  bound = _bound(max_distance, voxel_graph, max_device_bytes=max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, device, fixed_dims=2,
-                     max_device_bytes=max_device_bytes)
+                     max_device_bytes=max_device_bytes, bound=bound)
 
 
 def edt3dsq(data, anisotropy=(1.0, 1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-            *, device=0, max_device_bytes=None):
+            *, device=0, max_device_bytes=None, max_distance=None):
+  bound = _bound(max_distance, voxel_graph, max_device_bytes=max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, 0, device, fixed_dims=3,
-                     max_device_bytes=max_device_bytes)
+                     max_device_bytes=max_device_bytes, bound=bound)
 
 
 def edt3d(data, anisotropy=(1.0, 1.0, 1.0), black_border=False, parallel=1, voxel_graph=None,
-          *, device=0, max_device_bytes=None):
+          *, device=0, max_device_bytes=None, max_distance=None):
+  bound = _bound(max_distance, voxel_graph, max_device_bytes=max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, FLAG_SQRT, device, fixed_dims=3,
-                     max_device_bytes=max_device_bytes)
+                     max_device_bytes=max_device_bytes, bound=bound)
 
 
 # ---------------------------------------------------------------------------------------
@@ -706,17 +751,18 @@ def _torch_label_bytes(torch):
 
 
 def edt_cuda(labels, anisotropy=None, black_border=False, *, sqrt=False, signed=False, out=None,
-             voxel_graph=None, stacked=False):
+             voxel_graph=None, stacked=False, max_distance=None):
   """Transform a C-contiguous integer/bool torch CUDA tensor of 1-3 dims on its own device
   and current stream, asynchronously; returns a float32 CUDA tensor of the same shape
   (`out` may be passed to reuse a buffer).  Same semantics as edtsq/edt/sdfsq/sdf.
   `voxel_graph` (a uint8/int8 CUDA tensor of the same shape, 2-D / 3-D only, not with `signed`)
   selects the connectivity-graph transform.  `stacked=True` takes a (B, ...) tensor of 2-4 dims:
   B volumes of 1-3 dims, each transformed on its own, one launch per pass for all of them
-  (`anisotropy`: one entry per volume axis)."""
+  (`anisotropy`: one entry per volume axis).  `max_distance`: the bounded transform, as for edtsq."""
   import torch
   if not (isinstance(labels, torch.Tensor) and labels.is_cuda):
     raise TypeError("edt_cuda expects a torch CUDA tensor")
+  bound = _bound(max_distance, voxel_graph, stacked=stacked)
   nd = labels.dim()
   if stacked:
     vnd = _stack_dims(nd, voxel_graph)
@@ -765,9 +811,12 @@ def edt_cuda(labels, anisotropy=None, black_border=False, *, sqrt=False, signed=
       labels.data_ptr(), nbytes, voxel_graph.data_ptr(), nd, sx, sy, sz, wx, wy, wz,
       int(bool(black_border)), flags, out.data_ptr(), labels.device.index, ctypes.c_void_p(stream)))
     return out
-  _check(_lib().edtb200_transform(
-    labels.data_ptr(), nbytes, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags,
-    out.data_ptr(), labels.device.index, ctypes.c_void_p(stream)))
+  args = (labels.data_ptr(), nbytes, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags, out.data_ptr(),
+          labels.device.index, ctypes.c_void_p(stream))
+  if bound is not None:
+    _check(_lib().edtb200_transform_bounded(*args, bound))
+  else:
+    _check(_lib().edtb200_transform(*args))
   return out
 
 
@@ -849,12 +898,14 @@ def _feature_anisotropy(dims, anisotropy):
   raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
 
 
-def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_device_bytes=None, stacked=False):
+def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_device_bytes=None, stacked=False,
+                  bound=None):
   """(distances or None, indices) of a numpy array through host buffers (edtb200_feature_transform).
   `max_device_bytes` (an int) streams a 2-D / 3-D array through one GPU in chunks within that budget
   (edtb200_feature_transform_chunked); with None a one-shot call that runs out of device memory is
   retried once that way, as _transform_host does.  stacked: a stack of volumes along the slowest axis
-  in memory (edtb200_feature_transform_stack), one index plane per volume axis."""
+  in memory (edtb200_feature_transform_stack), one index plane per volume axis.  bound: the bounded
+  feature transform's max_distance (edtb200_feature_transform_bounded, one shot only)."""
   if isinstance(data, list):
     data = np.array(data)
   data = np.asarray(data)
@@ -892,7 +943,9 @@ def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_
     else:
       args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
               int(flags), dist_ptr, ptrs, int(device))
-      if max_device_bytes is None:
+      if bound is not None:
+        _check(lib.edtb200_feature_transform_bounded(*args, None, bound))
+      elif max_device_bytes is None:
         try:
           _check(lib.edtb200_feature_transform(*args, None))
         except EDTError as e:
@@ -905,7 +958,7 @@ def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_
   return (dist.reshape(data.shape, order=order) if want_dist else None), indices
 
 
-def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False):
+def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False, bound=None):
   """(distances or None, indices) of a torch CUDA tensor as torch CUDA tensors on its current
   stream, without host copies.  A Fortran-ordered tensor goes through its transposed view, as in
   _front_door_device, and its results are returned in its order.  stacked: a stack of volumes
@@ -940,9 +993,12 @@ def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False
         t.device.index, ctypes.c_void_p(stream)))
     else:
       (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape, anisotropy, False)
-      _check(_lib().edtb200_feature_transform(
-        t.data_ptr(), nbytes, dims, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags, dist_ptr, ptrs,
-        t.device.index, ctypes.c_void_p(stream)))
+      args = (t.data_ptr(), nbytes, dims, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags, dist_ptr, ptrs,
+              t.device.index, ctypes.c_void_p(stream))
+      if bound is not None:
+        _check(_lib().edtb200_feature_transform_bounded(*args, bound))
+      else:
+        _check(_lib().edtb200_feature_transform(*args))
   if fortran:
     planes = planes.permute(0, *range(dims, 0, -1))
     dist = dist.permute(*reversed(range(dims))) if want_dist else None
@@ -950,7 +1006,7 @@ def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False
 
 
 def feature_transform(data, anisotropy=None, black_border=False, *, signed=False, return_distances=False, device=0,
-                      max_device_bytes=None, stacked=False):
+                      max_device_bytes=None, stacked=False, max_distance=None):
   """The nearest site of every voxel: scipy.ndimage.distance_transform_edt(return_indices=True)
   for multi-label volumes, on the GPU.
 
@@ -975,7 +1031,13 @@ def feature_transform(data, anisotropy=None, black_border=False, *, signed=False
   `stacked=True` takes a 2-D to 4-D array whose slowest axis in memory indexes independent volumes,
   as edt(stacked=True) does: `indices` then has shape (data.ndim - 1,) + data.shape and holds the
   coordinates within each voxel's own volume.  The whole stack is staged on the GPU at once, so it
-  cannot be combined with max_device_bytes."""
+  cannot be combined with max_device_bytes.
+
+  `max_distance=d` finds only the sites within d: inside that band the distances follow edt's bounded
+  rule and the sites are as above; outside it every coordinate is -1 and the distance +inf (-inf on
+  signed background).  Unsigned background still maps to itself.  It cannot be combined with stacked
+  or max_device_bytes."""
+  bound = _bound(max_distance, stacked=stacked, max_device_bytes=max_device_bytes)
   flags = FLAG_SQRT | (FLAG_SIGNED if signed else 0)
   on_device = _device_array(data)
   if stacked:
@@ -992,9 +1054,10 @@ def feature_transform(data, anisotropy=None, black_border=False, *, signed=False
     dims = on_device.dim() if on_device is not None else np.ndim(data)
     max_device_bytes = _chunk_budget(max_device_bytes, on_device is not None, None, dims)
   if on_device is not None:
-    dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances)
+    dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances, bound=bound)
   else:
-    dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device, max_device_bytes)
+    dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device, max_device_bytes,
+                              bound=bound)
   return (dist, idx) if return_distances else idx
 
 

@@ -829,14 +829,56 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   return rc;
 }
 
+// All passes of one bounded transform (include/edt_b200.h) on device-resident buffers: the X pass,
+// then each later pass in the window kernel where bp says so (out of place) and in launch_later
+// otherwise (in place, without its sqrt / sign), then -- unless the last pass was a window pass,
+// which cuts in its store -- the cut.  The X pass writes f or one scratch volume, whichever makes the
+// last window pass land in f.
+int run_bounded_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                       float wx, float wy, float wz, int border, int flags, float* f, const BoundedPlan& bp,
+                       DeviceCache& dc, cudaStream_t s) {
+  const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
+  const int64_t total = sx * sy * sz;
+  int windows = 0;
+  for (int k = 1; k < ndim; ++k) windows += bp.windowed[k] ? 1 : 0;
+  Scratch other;
+  if (windows && other.alloc(dc, sizeof(float) * (size_t)total, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the bounded transform's scratch volume");
+  }
+  float* buf[2] = {f, other.get<float>()};
+  int cur = windows % 2;
+  int rc = dispatch_first(label_bytes, labels, buf[cur], sy * sz, sx, wx, border, kernel_flags(flags, true, false),
+                          dc, s);
+  for (int k = 1; !rc && k < ndim; ++k) {
+    const edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz);
+    const PassArith arith = transform_arith(t.w, t.n, k);
+    if (bp.windowed[k]) {
+      rc = with_label_width(label_bytes, [&](auto b) {
+        return launch_later_window<b>(labels, buf[cur], buf[cur ^ 1], nullptr, g, t.w[k], (int)bp.radius[k], border,
+                                      border, kernel_flags(flags, false, k == ndim - 1), arith, bp.bound, dc, s);
+      });
+      cur ^= 1;
+    } else {
+      rc = dispatch_later(label_bytes, labels, buf[cur], g, t.w[k], border, border, 0, arith, dc, s, /*pdl=*/false);
+    }
+  }
+  if (rc || (ndim >= 2 && bp.windowed[ndim - 1])) return rc;
+  return with_label_width(label_bytes, [&](auto b) {
+    return launch_bounded_cut<b>(labels, f, nullptr, total, bp.bound, kernel_flags(flags, false, true), dc, s);
+  });
+}
+
 // All passes of one feature transform on device-resident buffers: the site-tracking passes, out of
 // place and alternating between `dist` and one scratch volume so that the last lands in `dist`, then
 // the resolver.  dist may be null (the distances then stay in scratch).  `count` volumes of
 // (sx, sy, sz) laid end to end are transformed each on its own, as run_passes does; the index planes
-// hold coordinates within each voxel's own volume.
+// hold coordinates within each voxel's own volume.  bp: a bounded feature transform (count 1), whose
+// later passes take the window kernel where it says so; when the last pass does not, that pass runs
+// without its sqrt / sign and the cut follows it, on the distances and the last pass's codes.
 int run_feature_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                        float wx, float wy, float wz, int border, int flags, float* dist, int32_t* const idx[3],
-                       DeviceCache& dc, cudaStream_t s, int64_t count = 1) {
+                       DeviceCache& dc, cudaStream_t s, int64_t count = 1, const BoundedPlan* bp = nullptr) {
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   const size_t total = (size_t)(sx * sy * sz * count);
   Scratch own_dist, other, codes;
@@ -853,17 +895,28 @@ int run_feature_passes(const void* labels, int label_bytes, int ndim, int64_t sx
   int* code_planes[3] = {nullptr, nullptr, nullptr};
   for (int k = 0; k < ndim; ++k) code_planes[k] = codes.get<int>() + (size_t)k * total;
   // pass k writes buf[(ndim - 1 - k) % 2]: the last one (k = ndim - 1) writes buf[0]
+  const bool cut = bp && !(ndim >= 2 && bp->windowed[ndim - 1]);
   rc = with_label_width(label_bytes, [&](auto b) {
     return launch_first_sites<b>(labels, buf[(ndim - 1) % 2], code_planes[0], sy * sz * count, sx, wx, border,
-                                 kernel_flags(flags, true, ndim == 1), dc, s);
+                                 kernel_flags(flags, true, ndim == 1 && !cut), dc, s);
   });
   for (int k = 1; !rc && k < ndim; ++k) {
+    const int kflags = kernel_flags(flags, false, k == ndim - 1 && !cut);
     rc = with_label_width(label_bytes, [&](auto b) {
+      if (bp && bp->windowed[k])
+        return launch_later_window<b>(labels, buf[(ndim - k) % 2], buf[(ndim - 1 - k) % 2], code_planes[k],
+                                      geom_for_axis(k, sx, sy, sz, count), t.w[k], (int)bp->radius[k], border,
+                                      border, kflags, transform_arith(t.w, t.n, k), bp->bound, dc, s);
       return launch_later_sites<b>(labels, buf[(ndim - k) % 2], buf[(ndim - 1 - k) % 2], code_planes[k],
-                                   geom_for_axis(k, sx, sy, sz, count), t.w[k], border, border,
-                                   kernel_flags(flags, false, k == ndim - 1), transform_arith(t.w, t.n, k), dc, s);
+                                   geom_for_axis(k, sx, sy, sz, count), t.w[k], border, border, kflags,
+                                   transform_arith(t.w, t.n, k), dc, s);
     });
   }
+  if (!rc && cut)
+    rc = with_label_width(label_bytes, [&](auto b) {
+      return launch_bounded_cut<b>(labels, buf[0], code_planes[ndim - 1], (int64_t)total, bp->bound,
+                                   kernel_flags(flags, false, true), dc, s);
+    });
   if (rc) return rc;
   return with_label_width(label_bytes, [&](auto b) {
     return launch_resolve_sites<b>(labels, code_planes, ndim, sx, sy, sz, count, !(flags & EDTB200_SIGNED), idx, dc,
@@ -1485,9 +1538,15 @@ int edtb200_transform_stack(const void* labels, int label_bytes, int ndim, int64
   return 0;
 }
 
-int edtb200_feature_transform_stack(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy,
-                                    int64_t sz, int64_t count, float wx, float wy, float wz, int black_border,
-                                    int flags, float* dist_out, int32_t* const* idx_out, int device, void* stream_v) {
+}  // extern "C"
+
+namespace {
+
+// max_distance: null for the unbounded feature transform, else the bounded one's (count 1), checked
+// after the pointers.
+int feature_transform_any(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                          int64_t count, float wx, float wy, float wz, int black_border, int flags, float* dist_out,
+                          int32_t* const* idx_out, int device, void* stream_v, const double* max_distance) {
   int rc = check_dims(label_bytes, ndim, sx, sy, sz);
   if (rc) return rc;
   if (count < 0) return fail(EDTB200_EINVAL, "negative count");
@@ -1496,6 +1555,15 @@ int edtb200_feature_transform_stack(const void* labels, int label_bytes, int ndi
   if (!labels || !idx_out) return fail(EDTB200_EINVAL, "null pointer");
   for (int k = 0; k < ndim; ++k)
     if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
+  if (max_distance && !(*max_distance >= 0.0))
+    return fail(EDTB200_EINVAL, "max_distance must be zero or more (got %g)", *max_distance);
+  BoundedPlan plan;
+  const BoundedPlan* bp = nullptr;
+  if (max_distance && !std::isinf(*max_distance)) {
+    const float w[3] = {wx, wy, wz};
+    plan = bounded_plan(ndim, w, *max_distance, /*sites=*/true);
+    bp = &plan;
+  }
   const int64_t total = vol * count;
 
   DeviceGuard restore_device;
@@ -1521,8 +1589,73 @@ int edtb200_feature_transform_stack(const void* labels, int label_bytes, int ndi
   for (int k = 0; k < ndim; ++k)
     d_idx[k] = io.out(idx_out[k], vol_bytes, io.out_dev ? nullptr : planes.get<int32_t>() + (size_t)k * total);
   rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_dist,
-                          d_idx, *dc, io.stream, count);
+                          d_idx, *dc, io.stream, count, bp);
   return rc ? rc : io.finish();
+}
+
+}  // namespace
+
+extern "C" {
+
+int edtb200_feature_transform_stack(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy,
+                                    int64_t sz, int64_t count, float wx, float wy, float wz, int black_border,
+                                    int flags, float* dist_out, int32_t* const* idx_out, int device, void* stream_v) {
+  return feature_transform_any(labels, label_bytes, ndim, sx, sy, sz, count, wx, wy, wz, black_border, flags,
+                               dist_out, idx_out, device, stream_v, nullptr);
+}
+
+int edtb200_feature_transform_bounded(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy,
+                                      int64_t sz, float wx, float wy, float wz, int black_border, int flags,
+                                      float* dist_out, int32_t* const* idx_out, int device, void* stream_v,
+                                      double max_distance) {
+  return feature_transform_any(labels, label_bytes, ndim, sx, sy, sz, 1, wx, wy, wz, black_border, flags, dist_out,
+                               idx_out, device, stream_v, &max_distance);
+}
+
+int edtb200_transform_bounded(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                              float wx, float wy, float wz, int black_border, int flags, float* out, int device,
+                              void* stream_v, double max_distance) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  const int64_t total = sx * sy * sz;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  if (!(max_distance >= 0.0)) return fail(EDTB200_EINVAL, "max_distance must be zero or more (got %g)", max_distance);
+  if (std::isinf(max_distance))
+    return edtb200_transform(labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border, flags, out, device,
+                             stream_v);
+  const float w[3] = {wx, wy, wz};
+  const BoundedPlan bp = bounded_plan(ndim, w, max_distance, /*sites=*/false);
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  // host buffers are staged through this device's cached buffers, as edtb200_transform stages them
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
+  float* d_out = io.out(out, out_bytes, dc->dist);
+  rc = run_bounded_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_out, bp,
+                          *dc, io.stream);
+  return rc ? rc : io.finish();
+}
+
+int edtb200_bounded_plan(int ndim, int64_t sx, int64_t sy, int64_t sz, float wx, float wy, float wz,
+                         double max_distance, int64_t radius[3], int windowed[3]) {
+  int rc = check_dims(1, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (!(max_distance >= 0.0)) return fail(EDTB200_EINVAL, "max_distance must be zero or more (got %g)", max_distance);
+  if (!radius || !windowed) return fail(EDTB200_EINVAL, "null pointer");
+  const float w[3] = {wx, wy, wz};
+  const BoundedPlan bp = bounded_plan(ndim, w, max_distance, false), sp = bounded_plan(ndim, w, max_distance, true);
+  for (int k = 0; k < 3; ++k) {
+    radius[k] = k < ndim ? bp.radius[k] : 0;
+    windowed[k] = k < ndim ? (bp.windowed[k] ? 1 : 0) | (sp.windowed[k] ? 2 : 0) : 0;
+  }
+  return 0;
 }
 
 int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,

@@ -1,9 +1,10 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as six translation units so that the kernel templates build in
+// The library is compiled as seven translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
-// launchers of edt_passes.cuh instantiated for one label width each) and edt_plan.cu (the
-// later-axis plan for host code that launches nothing).  The run-time label width
+// launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
+// later-axis plan for host code that launches nothing) and edt_bounded.cu (the bounded
+// transforms' kernels).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -220,6 +221,35 @@ int launch_expand_gather(const void* labels, const float* sqdist, const int32_t*
                          int64_t sy, int64_t sz, int64_t count, double limit_sq, bool as_float, void* out,
                          DeviceCache& dc, cudaStream_t stream);
 
+// The plan of a bounded transform (plan_bounded, edt_passes.cuh): the cut B -- the largest float32
+// whose double is at most max_distance^2 -- and per axis the window radius R_k and whether the later
+// pass along it takes the window kernel (edt_bounded.cuh).
+struct BoundedPlan {
+  float bound = 0.0f;
+  int64_t radius[3] = {0, 0, 0};
+  bool windowed[3] = {false, false, false};
+};
+// The largest radius a window kernel is launched with (its tile then holds 64 + 256 rows).
+constexpr int kWindowRadiusLimit = 128;
+// plan_bounded with the windows of at most EDTB200_BOUNDED_WINDOW_MAX rows (sites: the feature
+// transform's EDTB200_BOUNDED_SITES_WINDOW_MAX), or EDTB200_BOUNDED_RMAX for both (an A/B switch for
+// measurements; -1: no pass is windowed) (edt_plan.cu).  max_distance >= 0.
+BoundedPlan bounded_plan(int ndim, const float w[3], double max_distance, bool sites);
+
+// The bounded transforms' kernels (edt_bounded.cuh, one instantiation per label width in
+// edt_bounded.cu).  launch_later_window: the later pass along g out of place (fin -> fout) over the
+// samples within `radius` rows, the rows above `bound` written as +inf; codes non-null: also the
+// site codes, as launch_later_sites writes them; flags: sqrt / sign in the store (last pass only).
+// launch_bounded_cut: in place over `total` voxels, +inf above `bound` (and kSiteNone in codes, when
+// given), then flags' sqrt / sign.
+template <int Bytes>
+int launch_later_window(const void* labels, const float* fin, float* fout, int* codes, const LineGeom& g, float w,
+                        int radius, int border_lo, int border_hi, int flags, PassArith arith, float bound,
+                        DeviceCache& dc, cudaStream_t stream);
+template <int Bytes>
+int launch_bounded_cut(const void* labels, float* f, int* codes, int64_t total, float bound, int flags,
+                       DeviceCache& dc, cudaStream_t stream);
+
 // Whether plan_later (edt_passes.cuh) sends a later-axis pass over geometry g with arithmetic
 // `arith` to the long-line kernel (edt_plan.cu).
 bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin);
@@ -227,7 +257,8 @@ bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin);
 // What a later-axis launch runs (plan_later in edt_passes.cuh); the last one launched on the
 // calling thread is kept for edtb200_last_later_launch.
 struct LaterLaunch {
-  int kernel = -1;      // 0 = tile kernel, 1 = long-line kernel, -1 = no launch yet
+  int kernel = -1;      // 0 = tile kernel, 1 = long-line kernel, 2 = window kernel, -1 = no launch yet
+  // tx: the tile width, or the window kernel's radius
   int tx = 0, tma = 0, wide = 0, ctas = 0, int_hull = 0, epilogue = 0, all_double = 0;
 };
 extern thread_local LaterLaunch g_last_later;

@@ -9,6 +9,8 @@
 #include "edt_host.h"
 #include "edt_feature.cuh"
 
+#include <cfloat>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 
@@ -213,6 +215,35 @@ inline LaterLaunch plan_later(const LineGeom& g, bool epilogue, PassArith arith,
   }
   // ---- lines too long for a shared-memory tile, or sums not exact in double ----
   return LaterLaunch{1, 0, 0, 0, 0, 0, epilogue, !arith.exact};
+}
+
+// The plan of a bounded transform with max_distance d >= 0 (include/edt_b200.h, DESIGN.md section 5).
+// Pure host logic.  B is the largest float32 with (double)B <= d^2; a later pass along axis k needs
+// only the samples v with (double)w2 (i - v)^2 < nextafterf(B, +inf), i.e. within R_k rows, and takes
+// the window kernel when R_k <= rmax.  R_k is found by bisection on that very test (monotone in r),
+// capped at 2^62, which also stands for "no bound" (B = FLT_MAX, or w2 = 0).
+inline BoundedPlan plan_bounded(int ndim, const float w[3], double d, int64_t rmax) {
+  BoundedPlan p;
+  const double L = d * d;
+  if (L >= (double)FLT_MAX) {
+    p.bound = FLT_MAX;
+  } else {
+    p.bound = (float)L;
+    if ((double)p.bound > L) p.bound = nextafterf(p.bound, -INFINITY);
+  }
+  const double above = (double)nextafterf(p.bound, INFINITY);
+  for (int k = 0; k < ndim; ++k) {
+    const double w2 = (double)(w[k] * w[k]);          // the float product the passes use
+    int64_t lo = 0, hi = (int64_t)1 << 62;            // w2 * lo^2 < above always holds (above > 0)
+    while (lo < hi) {
+      const int64_t mid = lo + (hi - lo + 1) / 2;
+      if (w2 * (double)mid * (double)mid < above) lo = mid;
+      else hi = mid - 1;
+    }
+    p.radius[k] = lo;
+    p.windowed[k] = k >= 1 && lo <= rmax;
+  }
+  return p;
 }
 
 // The tile-kernel instance of plan p (Epi, TMA = p.epilogue, p.tma): only the variants

@@ -13,5 +13,14 @@ bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin) 
 
 bool label_noise_predicted(const DeviceCache& dc) { return noise_predicted(dc); }
 
+BoundedPlan bounded_plan(int ndim, const float w[3], double max_distance, bool sites) {
+  int64_t rmax = sites ? EDTB200_BOUNDED_SITES_WINDOW_MAX : EDTB200_BOUNDED_WINDOW_MAX;
+  if (const char* env = getenv("EDTB200_BOUNDED_RMAX")) {      // A/B switch for measurements
+    rmax = atoll(env);
+    if (rmax > kWindowRadiusLimit) rmax = kWindowRadiusLimit;
+  }
+  return plan_bounded(ndim, w, max_distance, rmax);
+}
+
 }  // namespace host
 }  // namespace edtb200

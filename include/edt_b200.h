@@ -132,6 +132,63 @@ int edtb200_feature_transform(const void *labels, int label_bytes, int ndim,
                               int black_border, int flags, float *dist_out,
                               int32_t *const *idx_out, int device, void *stream);
 
+/* Bounded transforms: only the distances up to max_distance = d, for callers that clamp, grow or
+ * query within a radius.  Let L = (double)d * (double)d and S the squared value the unbounded call
+ * gives a voxel (its edtsq, or |sdfsq| with EDTB200_SIGNED).
+ *   transform          the bounded result is the unbounded one bit for bit where (double)S <= L, and
+ *                      +inf elsewhere (-inf on signed background); unsigned background stays 0.  The
+ *                      cut is made on the squared value, before sqrt and sign, as expand_labels'
+ *                      (double)|sqdist| <= limit_sq.  This holds for edtsq, edt, sdfsq and sdf.
+ *   feature transform  inside the band distances as above and sites as edtb200_feature_transform's
+ *                      (the distance to the site is the distance returned, bit for bit); outside it
+ *                      every coordinate -1 and the distance +inf (-inf on signed background), the "no
+ *                      site" encoding; unsigned background maps to itself.  Among equally near sites
+ *                      any one may be returned, the same one on every run.
+ *   d = +inf           the unbounded call, unchanged.  d = 0 is allowed; a negative or NaN d is
+ *                      EDTB200_EINVAL.
+ * How: with B the largest float32 with (double)B <= L, a later-axis pass along axis k only needs the
+ * samples within R_k rows of a voxel, R_k the largest r >= 0 with (double)w2_k * r * r <
+ * nextafterf(B, +inf), w2_k = fl32(w_k * w_k).  A pass with R_k up to a limit runs a window kernel
+ * (2 R_k + 1 rows, no hull, no scratch beyond one ping-pong volume); any other pass runs the unbounded
+ * kernel, and a streaming kernel applies the cut.  The limits were measured on an H100
+ * (records/h100/bounded_bench.txt): the window kernel beats the feature transform's long-line kernel
+ * at every radius measured (up to 32), but the distance transform's tile kernels only at radii of 2
+ * or less, and not on blocky labels.  edtb200_last_later_launch reports a window pass as kernel 2 with its radius in info[1]. */
+#define EDTB200_BOUNDED_WINDOW_MAX 2         /* edtb200_transform_bounded */
+#define EDTB200_BOUNDED_SITES_WINDOW_MAX 32  /* edtb200_feature_transform_bounded */
+
+/* edtb200_transform with max_distance (the bounded transform above).  Residency, staging and
+ * asynchrony as edtb200_transform; device memory: one more float32 volume of scratch when a later
+ * pass takes the window kernel.  An allocation that fails returns EDTB200_ENOMEM (there is no
+ * chunked retry).  Checks, in order: as edtb200_transform (label width, ndim, sizes, emptiness,
+ * pointers), then max_distance, then the device. */
+int edtb200_transform_bounded(const void *labels, int label_bytes, int ndim,
+                              int64_t sx, int64_t sy, int64_t sz,
+                              float wx, float wy, float wz,
+                              int black_border, int flags,
+                              float *out, int device, void *stream, double max_distance);
+
+/* edtb200_feature_transform with max_distance (the bounded feature transform above).  Residency and
+ * checks as there, then max_distance, then the device.  A window pass needs no long-line hull (4 bytes
+ * per voxel while a long-line pass runs), so in 3-D, when every later pass takes the window kernel,
+ * the device memory beyond the labels is 32 bytes per voxel instead of 36. */
+int edtb200_feature_transform_bounded(const void *labels, int label_bytes, int ndim,
+                                      int64_t sx, int64_t sy, int64_t sz,
+                                      float wx, float wy, float wz,
+                                      int black_border, int flags, float *dist_out,
+                                      int32_t *const *idx_out, int device, void *stream,
+                                      double max_distance);
+
+/* The plan of a bounded transform, pure host logic (no device needed): radius[k] = R_k for every axis
+ * k < ndim (capped at 2^62, which also stands for "no bound": d = +inf, or w2_k = 0), and in windowed[k]
+ * bit 0 where edtb200_transform_bounded's later pass along axis k (k >= 1) takes the window kernel
+ * (R_k <= EDTB200_BOUNDED_WINDOW_MAX), bit 1 where edtb200_feature_transform_bounded's does
+ * (R_k <= EDTB200_BOUNDED_SITES_WINDOW_MAX).  Entries k >= ndim are 0.
+ * Checks, in order: ndim, sizes (as edtb200_transform), max_distance, pointers. */
+int edtb200_bounded_plan(int ndim, int64_t sx, int64_t sy, int64_t sz,
+                         float wx, float wy, float wz, double max_distance,
+                         int64_t radius[3], int windowed[3]);
+
 /* A stack of `count` volumes of one geometry (sx, sy, sz), laid back to back (volume b starts at
  * voxel b * sx * sy * sz), each transformed on its own as edtb200_transform would: its result is
  * that call's bit for bit.  No line crosses from one volume into the next, black_border applies to
@@ -539,7 +596,8 @@ int edtb200_pass_ms(int steps_back, float *ms3);
 
 /* Which kernel variant the last later-axis (Y or Z) pass launched by the calling thread used, so
  * that tests can tell which code paths they reached.  Read-only: it changes no launch.  Fills
- * info[0..8): kernel (0 = shared-memory tile, 1 = long-line), tile width TX, TMA staging, wide
+ * info[0..8): kernel (0 = shared-memory tile, 1 = long-line, 2 = the bounded transforms' window
+ * kernel, with its radius in place of the tile width), tile width TX, TMA staging, wide
  * CTA, CTAs per SM the tile kernel is compiled for, integer hull tests, epilogue (sqrt / sign in
  * the store), every candidate formed in double.  EDTB200_EINVAL before any such launch. */
 int edtb200_last_later_launch(int *info);

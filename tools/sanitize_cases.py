@@ -91,6 +91,17 @@ check("stack long", edt.edtsq(odd, anisotropy=(0.7, 1.3, 2.9), stacked=True, max
 _, idx = edt.feature_transform(odd, stacked=True, return_distances=True)
 for b in range(len(odd)):
   check("stack feature %d" % b, idx[:, b], edt.feature_transform(odd[b]))
+# bounded transforms (max_distance): window passes with and without sites, a pass that falls back to
+# the unbounded kernel, and a zero-radius pass; each against the oracle's transform with the band applied
+def banded(unbounded, sq, d):
+  keep = np.abs(sq).astype(np.float64) <= d * d
+  return np.where(keep, unbounded, np.where(np.signbit(sq), -np.inf, np.inf)).astype(np.float32)
+blk = np.asfortranarray(cases.random_volume(rng, (40, 36, 30), "blocks", np.uint32))
+for d, an in ((2.5, (1, 1, 1)), (7.9, (0.7, 1.3, 2.9)), (40.0, (1, 4, 1)), (24.0, (6, 6, 30))):
+  sq = oracle.sdfsq(blk, anisotropy=an)
+  check("bounded sdf %g" % d, edt.sdf(blk, anisotropy=an, max_distance=d), banded(oracle.sdf(blk, anisotropy=an), sq, d))
+  dist, _ = edt.feature_transform(blk, an, signed=True, return_distances=True, max_distance=d)
+  check("bounded feature %g" % d, dist, banded(oracle.sdf(blk, anisotropy=an), sq, d))
 # per-label statistics and box-restricted extraction
 import torch  # noqa: E402
 lt = torch.from_numpy(np.ascontiguousarray(vor.astype(np.int32))).cuda()

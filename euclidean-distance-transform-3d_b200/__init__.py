@@ -167,10 +167,11 @@ def last_later_launch():
   """Kernel variant of the last Y / Z pass this thread launched (edtb200_last_later_launch), as a
   dict: kernel "tile", "long" or "window" (a bounded transform's window kernel, whose radius is in
   tx), tile width tx, tma, wide, ctas (per SM), int_hull, epilogue, all_double (every candidate
-  formed in double)."""
-  info = (ctypes.c_int * len(LATER_LAUNCH_FIELDS))()
+  formed in double), settled (tiles the X pass left settled were skipped)."""
+  # the plan fields (LATER_LAUNCH_FIELDS), then whether settled tiles were skipped
+  info = (ctypes.c_int * (len(LATER_LAUNCH_FIELDS) + 1))()
   _check(_lib().edtb200_last_later_launch(info))
-  out = dict(zip(LATER_LAUNCH_FIELDS, (int(v) for v in info)))
+  out = dict(zip(LATER_LAUNCH_FIELDS + ("settled",), (int(v) for v in info)))
   out["kernel"] = {0: "tile", 1: "long", 2: "window"}[out["kernel"]]
   return out
 

@@ -652,8 +652,9 @@ int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const
     tile = tile ||
            !later_pass_is_long(geom_for_axis(k, sx, sy, sz, count), transform_arith(t.w, t.n, k), dc.max_smem_optin);
   if (!tile) return 0;
-  const int64_t wpr = (sx + 31) >> 5, words = sy * sz * count * wpr;
-  if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)words * (size_t)(t.ndim - 1), s) != cudaSuccess) {
+  // per later axis: the run-start plane (wpr words per row), then the settled plane (one word per row)
+  const int64_t wpr = (sx + 31) >> 5, rows = sy * sz * count, words = rows * wpr;
+  if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)(words + rows) * (size_t)(t.ndim - 1), s) != cudaSuccess) {
     cudaGetLastError();
     return 0;                        // no room: the later passes read the labels
   }
@@ -661,11 +662,23 @@ int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const
   rp.x.sy = sy;
   rp.x.depth = sz;
   rp.x.y = p;
-  rp.x.z = t.ndim == 3 ? p + words : nullptr;
+  rp.x.settled_y = p + words;
+  rp.x.z = t.ndim == 3 ? p + words + rows : nullptr;
+  rp.x.settled_z = t.ndim == 3 ? p + 2 * words + rows : nullptr;
+  rp.x.ty = t.w[1] * t.w[1];         // the float products the later passes compare with (launch_later)
+  rp.x.tz = t.ndim == 3 ? t.w[2] * t.w[2] : 0.0f;
   // Y pass: outer = z (of every volume), inner = x; Z pass: outer = volume, inner = y * sx + x, rows
-  // sy * wpr words apart
-  rp.bits[1] = edtb200::RunBits{rp.x.y, wpr, sy * wpr, sx, wpr};
-  if (t.ndim == 3) rp.bits[2] = edtb200::RunBits{rp.x.z, sy * wpr, sz * sy * wpr, sx, wpr};
+  // sy * wpr words apart.  Settled words: Y pass at z * sy + y, Z pass at volume * sz * sy + z * sy + y.
+  rp.bits[1] = edtb200::RunBits{rp.x.y, wpr, sy * wpr, sx, wpr, rp.x.settled_y, 1, sy, nullptr, 0.0f};
+  if (t.ndim == 3) {
+    rp.bits[2] = edtb200::RunBits{rp.x.z, sy * wpr, sz * sy * wpr, sx, wpr, rp.x.settled_z, sy, sz * sy, nullptr, 0.0f};
+    // the Y pass refreshes the Z pass's settled plane only where the Z pass may skip tiles (no
+    // epilogue, integer hull: see launch_later)
+    if (kernel_flags(t.flags, false, true) == 0 && transform_arith(t.w, t.n, 2).int_hull) {
+      rp.bits[1].refresh = rp.x.settled_z;
+      rp.bits[1].refresh_t = rp.x.tz;
+    }
+  }
   return 0;
 }
 
@@ -1974,7 +1987,7 @@ int edtb200_last_later_launch(int* info) {
   if (!info) return fail(EDTB200_EINVAL, "null pointer");
   const LaterLaunch& l = g_last_later;
   if (l.kernel < 0) return fail(EDTB200_EINVAL, "no later-axis pass has been launched on this thread");
-  const int v[8] = {l.kernel, l.tx, l.tma, l.wide, l.ctas, l.int_hull, l.epilogue, l.all_double};
+  const int v[9] = {l.kernel, l.tx, l.tma, l.wide, l.ctas, l.int_hull, l.epilogue, l.all_double, l.settled};
   memcpy(info, v, sizeof(v));
   return 0;
 }

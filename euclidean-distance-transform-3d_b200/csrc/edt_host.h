@@ -260,6 +260,7 @@ struct LaterLaunch {
   int kernel = -1;      // 0 = tile kernel, 1 = long-line kernel, 2 = window kernel, -1 = no launch yet
   // tx: the tile width, or the window kernel's radius
   int tx = 0, tma = 0, wide = 0, ctas = 0, int_hull = 0, epilogue = 0, all_double = 0;
+  int settled = 0;      // tiles whose voxels the X pass left settled are skipped (launch_later)
 };
 extern thread_local LaterLaunch g_last_later;
 

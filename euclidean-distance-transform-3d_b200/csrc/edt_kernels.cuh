@@ -279,11 +279,19 @@ template <> struct Vec4Labels<8> {
 //   z   bit = z == 0 || L(x, y, z) != L(x, y, z - 1)     (the Z pass's run starts; 3-D only, else null)
 // In a stack of volumes laid end to end along z, z counts within the voxel's own volume: every
 // depth-th slice starts a volume, and its z bits are all set.
+// Beside them the settled planes, one word per row (y, z) at word z * sy + y: bit s set when every
+// voxel of the row's 32-voxel x-segment s ends the X pass at f <= t (padding voxels past sx count as
+// settled).  A later pass with w2 = t leaves such a voxel as it is (DESIGN.md section 4.1), so it may
+// skip a tile whose bits are all set.
+//   settled_y   t = ty, the Y pass's w2        settled_z   t = tz, the Z pass's (3-D only, else null)
 struct XPlanes {
   uint32_t* y;
   uint32_t* z;
   int64_t sy;              // rows per z
   int64_t depth;           // slices per volume (z planes only)
+  uint32_t* settled_y;
+  uint32_t* settled_z;
+  float ty, tz;
 };
 
 // A lane's 4-bit nibble of a 128-voxel block (voxels 4 lane .. 4 lane + 3) -> the block's 32-bit
@@ -302,10 +310,14 @@ __device__ __forceinline__ uint32_t nibbles_to_word(uint32_t nib, int lane) {
 // +inf at sx + 1) and float4 stores.  Adds the row's label changes along x to the lane's nstarts.
 // Plain = true: squared EDT, background forced to 0, no sqrt / sign (the hot configuration);
 // Plain = false: behaviour selected by `flags` at run time.
-template <int Bytes, int K, bool Plain, class Load>
+// Settled = true (first_axis_planes_kernel only): also clears bit b of set_y / set_z where a value
+// stored for the lane's four voxels of block b exceeds ty / tz (lanes past sx leave theirs set).
+template <int Bytes, int K, bool Plain, bool Settled = false, class Load>
 __device__ __forceinline__ void first_axis_vec_row(Load load, float* __restrict__ dst, int sx, const float* table_s,
                                                    int border, int flags, bool keep_background, int lane,
-                                                   unsigned lt_mask, unsigned gt_mask, unsigned int& nstarts) {
+                                                   unsigned lt_mask, unsigned gt_mask, unsigned int& nstarts,
+                                                   float ty = 0.0f, float tz = 0.0f, uint32_t* set_y = nullptr,
+                                                   uint32_t* set_z = nullptr) {
   using WT = typename LabelOf<Bytes>::wide;
   const unsigned full = 0xffffffffu;
 
@@ -404,6 +416,11 @@ __device__ __forceinline__ void first_axis_vec_row(Load load, float* __restrict_
       if (!Plain) val = finish_value(val, background, flags);
       r[e] = val;
     }
+    if constexpr (Settled) {                          // one compare per block and plane
+      const float most = fmaxf(fmaxf(r[0], r[1]), fmaxf(r[2], r[3]));
+      if (!(most <= ty)) *set_y &= ~(1u << b);
+      if (!(most <= tz)) *set_z &= ~(1u << b);
+    }
     *reinterpret_cast<float4*>(dst + q0) = make_float4(r[0], r[1], r[2], r[3]);
   }
 }
@@ -488,12 +505,21 @@ struct TileBoxes {
 // The run-start plane of one later-axis pass written by the X pass (XPlanes): for the line (outer o,
 // inner j) and row i the bit (j % sx) & 31 of word  o * outer_words + (j / sx) * wpr + (j % sx) / 32
 // + i * row_words.  Y pass: outer = z, inner = x; Z pass: inner = y * sx + x.
+// With `settled` (the pass's settled plane, XPlanes) a tile whose voxels all have f <= w2 ends before
+// it loads anything: for the line (o, j) and row i the bit (j % sx) / 32 of word o * settled_outer +
+// j / sx + i * settled_row.  With `refresh` (the Y pass: the Z pass's settled plane, same layout)
+// every tile that runs sets the bits of its rows that it leaves at f <= refresh_t.
 struct RunBits {
   const uint32_t* start;   // a run of equal labels starts at this row (always at row 0)
   int64_t row_words;
   int64_t outer_words;
   int64_t sx;
   int64_t wpr;
+  const uint32_t* settled;
+  int64_t settled_row;
+  int64_t settled_outer;
+  uint32_t* refresh;
+  float refresh_t;
 };
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
@@ -691,9 +717,27 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
       // this row is row warp + 1 of its stage (row 0: the halo row y - 1)
       const LT* cur = ring + (size_t)slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
       const LT* back = ring + (size_t)prev_slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
-      first_axis_vec_row<Bytes, K, Plain>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); }, out + line * sx,
-                                          sx, table_s, border, flags, keep_background, lane, lt_mask, gt_mask,
-                                          nstarts);
+      uint32_t set_y = 0xffffffffu, set_z = 0xffffffffu;
+      first_axis_vec_row<Bytes, K, Plain, true>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); },
+                                                out + line * sx, sx, table_s, border, flags, keep_background, lane,
+                                                lt_mask, gt_mask, nstarts, planes.ty, planes.tz, &set_y, &set_z);
+      // ---- settled planes: segment 4 b + w of the row is lanes 8 w .. 8 w + 7 of block b ----
+      uint32_t seg_y = 0u, seg_z = 0u;
+#pragma unroll
+      for (int b = 0; b < K; ++b) {
+        uint32_t v = __ballot_sync(full, (set_y >> b) & 1u);
+        v &= v >> 4; v &= v >> 2; v &= v >> 1;               // bit 8 w: all of lanes 8 w .. 8 w + 7
+        seg_y |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
+        if (Planes == 2) {
+          v = __ballot_sync(full, (set_z >> b) & 1u);
+          v &= v >> 4; v &= v >> 2; v &= v >> 1;
+          seg_z |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
+        }
+      }
+      if (lane == 0) {
+        planes.settled_y[line] = seg_y | (0xffffffffu << (4 * K));
+        if (Planes == 2) planes.settled_z[line] = seg_z | (0xffffffffu << (4 * K));
+      }
       // ---- run-start planes: compare with rows (y - 1, z) and (y, z - 1); one nibble per lane and
       // block -> the row's wpr words, word c in lane c, stored by one instruction per plane ----
       uint32_t word[Planes] = {};
@@ -1053,6 +1097,29 @@ __device__ __forceinline__ void walk_begin(HullWalk& w, const TileLine<TX> ln, i
   }
 }
 
+// The Y pass's refresh of the Z pass's settled plane (RunBits::refresh) by a tile that ran, after all
+// its stores: values only fall within a pass, so bits only go from clear to set.  Thread t takes row t
+// (blockDim.x >= n: no wide tiles).  When at most 32 of the tile's rows have the bit clear, one warp
+// per such row re-reads its values (L2-hot) and sets the bit if none exceeds refresh_t; with more,
+// the bits stay clear, which is still correct.  Other tiles of the same rows own the words' other
+// bits, hence the atomic.  Its first barrier orders the tile's stores before the re-reads.
+__device__ __forceinline__ void refresh_settled(const RunBits& rb, const float* f, const LineGeom& g, int64_t outer,
+                                                int64_t inner0, int n) {
+  const int t = threadIdx.x, lane = t & 31;
+  const uint32_t bit = 1u << (int)(inner0 >> 5);       // the tile is x-segment inner0 / 32 of its rows
+  uint32_t* const words = rb.refresh + outer * rb.settled_outer;
+  const bool clear = t < n && !(words[(int64_t)t * rb.settled_row] & bit);
+  const int nclear = __syncthreads_count(clear);
+  if (nclear == 0 || nclear > 32) return;
+  const bool live = inner0 + lane < g.inner_count;     // padding lines count as settled
+  const float* col = f + (outer * g.outer_stride + inner0 + lane);
+  for (uint32_t m = __ballot_sync(0xffffffffu, clear); m; m &= m - 1u) {
+    const int64_t i = (t & ~31) + __ffs(m) - 1;
+    const float v = live ? col[i * g.line_stride] : 0.0f;
+    if (__all_sync(0xffffffffu, v <= rb.refresh_t) && lane == 0) atomicOr(words + i * rb.settled_row, bit);
+  }
+}
+
 // MinCtas: CTAs of 512 threads per SM the kernel is compiled for.  3 (40 registers, a few spills)
 // is what the envelope stages want -- they are latency-bound and the third CTA's warps hide it;
 // 2 (60 registers, no spills) is faster when nearly every run is one row long (label noise), where
@@ -1064,6 +1131,8 @@ __device__ __forceinline__ void walk_begin(HullWalk& w, const TileLine<TX> ln, i
 // plane is read only after griddepcontrol.wait: the Z pass may start while the X pass is still
 // running (the Y pass lets its dependents start before it waits itself).  Compiled for the
 // label-noise shape only (2 CTAs per SM, TMA, 32-wide tiles, no background bits: unsigned transforms).
+// It also skips settled tiles and refreshes the Z pass's settled plane, where the host passes those
+// planes in rb (launch_later).
 template <int Bytes, int TX, bool Epilogue, bool UseTMA, bool Wide, int MinCtas, bool IntHull, bool Bits = false>
 __global__ void __launch_bounds__(Wide ? 1024 : 512, Wide ? 1 : MinCtas)
 later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
@@ -1118,6 +1187,26 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
 
   pdl_launch_dependents();             // the next pass may start staging its labels during our tail
   if (!UseTMA) pdl_wait_for_previous_grid();           // plain loads of f happen in the staging loop
+  // (Bits) A tile whose voxels all have f <= w2 keeps every value (DESIGN.md section 4.1): it ends
+  // here, before its mbarrier, tile load or border table.  Thread t checks row t, in every row q of
+  // the settled plane that the tile's lines [j0, j1) reach, the x-segments they cover.
+  if constexpr (Bits && !Epilogue) {
+    if (rb.settled) {
+      pdl_wait_for_previous_grid();    // the plane is complete (Z pass: and refreshed by the Y pass)
+      const int64_t j0 = inner0, j1 = min(inner0 + TX, g.inner_count);
+      const int64_t q0 = j0 / rb.sx, q1 = (j1 - 1) / rb.sx;
+      bool settled = true;
+      for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const uint32_t* sp = rb.settled + (outer * rb.settled_outer + (int64_t)i * rb.settled_row);
+        for (int64_t q = q0; q <= q1; ++q) {
+          const int lo = (int)max(j0 - q * rb.sx, (int64_t)0), hi = (int)min(j1 - q * rb.sx, rb.sx) - 1;
+          const uint32_t need = (0xffffffffu >> (31 - (hi >> 5))) & (0xffffffffu << (lo >> 5));
+          settled = settled && (__ldg(sp + q) & need) == need;
+        }
+      }
+      if (__syncthreads_and(settled)) return;
+    }
+  }
   // Float tile by TMA, border-term table, chunk mask.  (kDecoupled) together with the mbarrier the
   // table and the mask are the only things a warp needs from other warps before the votes at the end
   // of stage 1, so the one barrier comes here, early, while no warp has loads in flight yet; the tile
@@ -1375,7 +1464,12 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
       sts_u32(ln.hull + (uint32_t)c * ROW, hb);
     }
   }
-  if (!__syncthreads_or(any_cross)) return;                // every run was finished inside its chunk
+  if (!__syncthreads_or(any_cross)) {                      // every run was finished inside its chunk
+    if constexpr (Bits && !Epilogue) {
+      if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
+    }
+    return;
+  }
   // Tiles with crossing runs: one bit per chunk that holds a run start, per line, so that the ends
   // of a crossing run are two look-ups instead of a walk over the chunks (made visible by the vote below).
   if (live && use_nz) {
@@ -1589,6 +1683,9 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
         }
       }
     }
+  }
+  if constexpr (Bits && !Epilogue) {
+    if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
   }
 }
 

@@ -320,6 +320,12 @@ int launch_later(const void* labels, const RunBits* bits, float* f, const LineGe
     RunBits rb;
     memset(&rb, 0, sizeof(rb));
     if (use_bits) rb = *bits;
+    // Settled tiles are skipped (and the Y pass refreshes the Z pass's plane) only where a skipped
+    // tile provably equals what the pass would store: integer samples (int_hull; with float hull tests
+    // the read-out may return a candidate within rounding of the minimum, DESIGN.md section 8) and no
+    // epilogue, whose sqrt / sign rewrites every row.
+    p.settled = use_bits && rb.settled && p.int_hull && flags == 0;
+    if (!p.settled) { rb.settled = nullptr; rb.refresh = nullptr; }
     const TileKernel<Bytes> kern =
         use_bits ? tile_kernel_bits<Bytes>(p)
         : p.epilogue ? (p.tma ? tile_kernel<Bytes, true, true>(p) : tile_kernel<Bytes, true, false>(p))

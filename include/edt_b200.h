@@ -38,7 +38,9 @@ extern "C" {
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather)
  * keep the number: every 202-level entry point
- * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up. */
+ * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
+ * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
+ * info[0..8) before), so its buffer must hold 9 ints. */
 #define EDTB200_VERSION 202
 
 /* flags */
@@ -596,10 +598,11 @@ int edtb200_pass_ms(int steps_back, float *ms3);
 
 /* Which kernel variant the last later-axis (Y or Z) pass launched by the calling thread used, so
  * that tests can tell which code paths they reached.  Read-only: it changes no launch.  Fills
- * info[0..8): kernel (0 = shared-memory tile, 1 = long-line, 2 = the bounded transforms' window
+ * info[0..9): kernel (0 = shared-memory tile, 1 = long-line, 2 = the bounded transforms' window
  * kernel, with its radius in place of the tile width), tile width TX, TMA staging, wide
  * CTA, CTAs per SM the tile kernel is compiled for, integer hull tests, epilogue (sqrt / sign in
- * the store), every candidate formed in double.  EDTB200_EINVAL before any such launch. */
+ * the store), every candidate formed in double, tiles left settled by the X pass skipped.
+ * EDTB200_EINVAL before any such launch. */
 int edtb200_last_later_launch(int *info);
 
 /* Free every cached device buffer / stream this library holds on all devices. */

@@ -1135,32 +1135,14 @@ int edtb200_transform_batch(const void* const* labels, float* const* outs, int c
 namespace {
 
 // One phase of edtb200_transform_chunked / edtb200_feature_transform_chunked (the plans of
-// include/edt_b200.h): `extent` slices of `slice_bytes` device bytes each, in `count` chunks of at
-// most `most` slices (count 0: the budget is below `need`, the least that works).
+// include/edt_b200.h): `extent` slices of `slice_vox` voxels and `slice_bytes` device bytes each, in
+// `count` chunks of at most `most` slices (count 0: the budget is below `need`, the least that works).
 struct PhasePlan {
-  int64_t extent = 0, count = 0, most = 0;
+  int64_t extent = 0, slice_vox = 0, count = 0, most = 0;
   size_t slice_bytes = 0, need = 0;
   int64_t start(int64_t k) const { return extent * k / count; }        // chunk sizes differ by one at most
   int64_t size(int64_t k) const { return start(k + 1) - start(k); }
 };
-
-// extent slices of slice_vox voxels that cost voxel_bytes device bytes per voxel each (a slot's
-// buffers and the phase's per-launch scratch); a chunk holds at most `cap` slices.
-PhasePlan plan_phase(int64_t extent, int64_t slice_vox, size_t voxel_bytes, int64_t cap, size_t budget) {
-  PhasePlan p;
-  p.extent = extent;
-  p.slice_bytes = (size_t)slice_vox * voxel_bytes;
-  p.need = (size_t)(extent < 2 ? extent : 2) * p.slice_bytes;
-  if (extent <= cap && (size_t)extent <= budget / p.slice_bytes) {
-    p.count = 1;
-  } else {
-    const int64_t c = std::min<int64_t>(cap, (int64_t)(budget / (2 * p.slice_bytes)));
-    if (c == 0) return p;
-    p.count = (extent + c - 1) / c;
-  }
-  p.most = (extent + p.count - 1) / p.count;
-  return p;
-}
 
 // Frees this device's cached whole-volume buffers and trims its private pool (the caller holds
 // host_call), so that a chunked call after a one-shot call that ran out of memory finds it free.
@@ -1179,53 +1161,134 @@ struct ChunkSlots {
   Scratch buf[2];
   void* labels[2] = {nullptr, nullptr};
   size_t lab = 0, vox = 0;
-  int take(DeviceCache& dc, const PhasePlan& p, int64_t slice_vox, int label_bytes, int planes) {
-    vox = (size_t)p.most * (size_t)slice_vox;
-    lab = (vox * (size_t)label_bytes + 255) & ~size_t(255);
-    const size_t bytes = lab + (size_t)planes * vox * 4;
-    for (int i = 0; i < (p.count > 1 ? 2 : 1); ++i) {
-      if (buf[i].alloc(dc, bytes, dc.stream) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(EDTB200_ENOMEM, "no device memory for a chunk slot of %zu bytes: give a smaller device_bytes",
-                    bytes);
-      }
-      labels[i] = buf[i].get();
-    }
-    CUDA_TRY(cudaStreamSynchronize(dc.stream));   // allocated on the passes' stream, used on all three
-    return 0;
-  }
   // volume j of slot `slot`
   template <class T = float>
   T* plane(int slot, int j) const { return reinterpret_cast<T*>(buf[slot].get<char>() + lab + (size_t)j * vox * 4); }
 };
 
-// The budget of a chunked call on a device whose host_call the caller holds: `device_bytes`, or with
-// 0 the memory free once the device's cached whole-volume buffers are dropped, less
-// EDTB200_CHUNK_RESERVE.  The buffers are dropped either way.
-int chunk_budget(DeviceCache& dc, size_t device_bytes, size_t* budget) {
-  drop_volume_buffers(dc);
-  *budget = device_bytes;
-  if (device_bytes == 0) {
-    size_t free_bytes = 0, total_bytes = 0;
-    CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
-    *budget = free_bytes > EDTB200_CHUNK_RESERVE ? free_bytes - EDTB200_CHUNK_RESERVE : 0;
+// Runs the chunks of plan p through run_pipeline; fill(slots, steps) sets the steps, which work on
+// the phase's slots of label_bytes and `planes` volumes.  The slots are taken on dc.stream and freed
+// on it when the phase returns, so that a next phase's slots reuse their memory instead of competing
+// with them for the budget.  Returns when every download has landed.
+template <class Fill>
+int run_phase(DeviceCache& dc, int device, const PhasePlan& p, int label_bytes, int planes, Fill fill) {
+  if (const int rc = pipeline_streams(dc)) return rc;   // dc.stream, which the slots are taken on
+  ChunkSlots slots;
+  slots.vox = (size_t)p.most * (size_t)p.slice_vox;
+  slots.lab = (slots.vox * (size_t)label_bytes + 255) & ~size_t(255);
+  const size_t bytes = slots.lab + (size_t)planes * slots.vox * 4;
+  for (int i = 0; i < (p.count > 1 ? 2 : 1); ++i) {
+    if (slots.buf[i].alloc(dc, bytes, dc.stream) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(EDTB200_ENOMEM, "no device memory for a chunk slot of %zu bytes: give a smaller device_bytes", bytes);
+    }
+    slots.labels[i] = slots.buf[i].get();
   }
+  CUDA_TRY(cudaStreamSynchronize(dc.stream));   // allocated on the passes' stream, used on all three
+  PipelineSteps steps;
+  fill(slots, steps);
+  return run_pipeline(dc, device, (int)p.count, steps);
+}
+
+// A host buffer of a streaming call; `written`: the call writes it.
+struct HostRange { const void* p; size_t bytes; const char* name; bool written; };
+
+// Fails with "<a> and <b> overlap" on the first pair, in list order, of non-null buffers that share a
+// byte where the call writes at least one of the two (inputs may overlap each other).
+int check_overlap(std::initializer_list<HostRange> ranges) {
+  for (const HostRange* a = ranges.begin(); a != ranges.end(); ++a)
+    for (const HostRange* b = a + 1; b != ranges.end(); ++b) {
+      const char *pa = static_cast<const char*>(a->p), *pb = static_cast<const char*>(b->p);
+      if (pa && pb && (a->written || b->written) && pa < pb + b->bytes && pb < pa + a->bytes)
+        return fail(EDTB200_EINVAL, "%s and %s overlap", a->name, b->name);
+    }
   return 0;
 }
 
-// Phase-2 chunk k of plan p2 in a host volume of `bytes` per voxel: n_last rows of size(k) * unit
-// voxels, one row per index along the last axis, `plane` voxels apart.
-HostBox line_box(const void* base, const PhasePlan& p2, int64_t k, int64_t unit, int64_t plane, int64_t n_last,
-                 size_t bytes) {
-  return HostBox{static_cast<char*>(const_cast<void*>(base)) + (size_t)(p2.start(k) * unit) * bytes,
-                 (size_t)(p2.size(k) * unit) * bytes, (size_t)plane * bytes, (size_t)n_last};
-}
+// A call that streams host buffers through `device`, as HostIO serves a one-shot call: the caller's
+// current device is restored on return, and from lock() on the call holds the device's host_call
+// lock and its device budget: `device_bytes`, or with 0 the memory free once the device's cached
+// whole-volume buffers are dropped, less EDTB200_CHUNK_RESERVE.  The buffers are dropped either way.
+struct StreamingCall {
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  size_t budget = 0;
 
-// Whether host ranges [a, a + an) and [b, b + bn) share a byte.
-bool overlap(const void* a, size_t an, const void* b, size_t bn) {
-  const char *pa = static_cast<const char*>(a), *pb = static_cast<const char*>(b);
-  return pa < pb + bn && pb < pa + an;
-}
+  int open(int device) { return probe(device, &dc); }
+  int lock(size_t device_bytes) {
+    lock_ = std::unique_lock<std::mutex>(dc->host_call);
+    drop_volume_buffers(*dc);
+    budget = device_bytes;
+    if (device_bytes == 0) {
+      size_t free_bytes = 0, total_bytes = 0;
+      CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
+      budget = free_bytes > EDTB200_CHUNK_RESERVE ? free_bytes - EDTB200_CHUNK_RESERVE : 0;
+    }
+    return 0;
+  }
+  // A phase within the budget: extent slices of slice_vox voxels that cost voxel_bytes device bytes
+  // per voxel each (a slot's buffers and the phase's per-launch scratch); a chunk holds at most `cap`
+  // slices.
+  PhasePlan plan(int64_t extent, int64_t slice_vox, size_t voxel_bytes, int64_t cap) const {
+    PhasePlan p;
+    p.extent = extent;
+    p.slice_vox = slice_vox;
+    p.slice_bytes = (size_t)slice_vox * voxel_bytes;
+    p.need = (size_t)(extent < 2 ? extent : 2) * p.slice_bytes;
+    if (extent <= cap && (size_t)extent <= budget / p.slice_bytes) {
+      p.count = 1;
+    } else {
+      const int64_t c = std::min<int64_t>(cap, (int64_t)(budget / (2 * p.slice_bytes)));
+      if (c == 0) return p;
+      p.count = (extent + c - 1) / c;
+    }
+    p.most = (extent + p.count - 1) / p.count;
+    return p;
+  }
+
+ private:
+  std::unique_lock<std::mutex> lock_;
+};
+
+// The two phases of a chunked transform of an (sx, sy, sz) volume.  Phase 1 cuts the last axis (z
+// slabs in 3-D, row ranges in 2-D) into slices of `plane` voxels; phase 2 cuts the axis before it
+// into boxes of whole lines along the last axis, slices of `unit` voxels per index of the last axis
+// and `line_vox` in all.
+struct TwoPhase {
+  int64_t n_last, n_cut, unit, plane, line_vox;
+  PhasePlan p1, p2;
+
+  TwoPhase(int ndim, int64_t sx, int64_t sy, int64_t sz)
+      : n_last(ndim == 3 ? sz : sy), n_cut(ndim == 3 ? sy : sx), unit(ndim == 3 ? sx : 1), plane(unit * n_cut),
+        line_vox(unit * n_last) {}
+
+  // Plans both phases within the call's budget from their device bytes per voxel and the most slices
+  // of a phase-2 chunk, and reports the chunk counts; `what` names the transform where the budget
+  // cannot hold one chunk.
+  int plan(const StreamingCall& call, size_t voxel_bytes1, size_t voxel_bytes2, int64_t cap2, const char* what,
+           int64_t* chunks) {
+    p1 = call.plan(n_last, plane, voxel_bytes1, n_last);
+    p2 = call.plan(n_cut, line_vox, voxel_bytes2, cap2);
+    if (p1.count == 0 || p2.count == 0)
+      return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked %s needs at "
+                                  "least %zu bytes", call.budget, what, std::max(p1.need, p2.need));
+    if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
+    return 0;
+  }
+
+  // Chunk k of a host volume of `bytes` per voxel.  Phase 1: size(k) whole slices, one range.
+  HostBox slab(const void* base, int64_t k, size_t bytes) const {
+    const size_t n = (size_t)(p1.size(k) * plane) * bytes;
+    return HostBox{host(base) + (size_t)(p1.start(k) * plane) * bytes, n, n, 1};
+  }
+  // Phase 2: n_last rows of size(k) * unit voxels, one per index along the last axis, `plane` voxels
+  // apart.
+  HostBox lines(const void* base, int64_t k, size_t bytes) const {
+    return HostBox{host(base) + (size_t)(p2.start(k) * unit) * bytes, (size_t)(p2.size(k) * unit) * bytes,
+                   (size_t)plane * bytes, (size_t)n_last};
+  }
+  static char* host(const void* base) { return static_cast<char*>(const_cast<void*>(base)); }
+};
 
 }  // namespace
 
@@ -1246,96 +1309,75 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
   if (total == 0) return 0;
   if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
-  const char* lab_host = static_cast<const char*>(labels);
-  char* out_host = reinterpret_cast<char*>(out);
-  if (overlap(lab_host, lab_bytes, out_host, out_bytes)) return fail(EDTB200_EINVAL, "labels and out overlap");
+  if ((rc = check_overlap({{labels, lab_bytes, "labels", false}, {out, out_bytes, "out", true}}))) return rc;
 
-  DeviceGuard restore_device;
-  DeviceCache* dcp = nullptr;
-  if ((rc = probe(device, &dcp))) return rc;
-  DeviceCache& dc = *dcp;
-  std::lock_guard<std::mutex> host_call(dc.host_call);
-  size_t budget = 0;
-  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+  StreamingCall call;
+  if ((rc = call.open(device)) || (rc = call.lock(device_bytes))) return rc;
+  DeviceCache& dc = *call.dc;
 
-  // Phase 1 cuts the last axis (z slabs in 3-D, row ranges in 2-D): X pass, and in 3-D the Y pass.
-  // Phase 2 cuts the axis before it into boxes of whole lines along the last axis: the last pass.
+  // Phase 1 cuts the last axis: X pass, and in 3-D the Y pass.  Phase 2 cuts the axis before it: the
+  // last pass.
   const int border = black_border != 0;
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   const int last = ndim - 1;
-  const int64_t n_last = t.n[last], n_cut = t.n[last - 1];
-  const int64_t plane = total / n_last;                    // voxels of one phase-1 slice
-  const int64_t unit = ndim == 3 ? sx : 1;                 // voxels of one phase-2 slice per row
-  const int64_t line_vox = unit * n_last;                  // voxels of one phase-2 slice
-  const int64_t cap2 = std::max<int64_t>(1, (int64_t)((((int64_t)1 << 32) - 65) / line_vox));
+  TwoPhase two(ndim, sx, sy, sz);
+  const int64_t cap2 = std::max<int64_t>(1, (int64_t)((((int64_t)1 << 32) - 65) / two.line_vox));
   const bool long1 = ndim == 3 && later_pass_is_long(geom_for_axis(1, sx, sy, sz), transform_arith(t.w, t.n, 1),
                                                      dc.max_smem_optin);
-  const int64_t c2 = std::min(n_cut, cap2);
+  const int64_t c2 = std::min(two.n_cut, cap2);
   const edtb200::LineGeom g2 = ndim == 3 ? geom_for_axis(2, sx, c2, sz) : geom_for_axis(1, c2, sy, 1);
   const bool long2 = later_pass_is_long(g2, transform_arith(t.w, t.n, last), dc.max_smem_optin);
   // per voxel: the labels and the distances, and the long-line kernel's two scratch volumes
-  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes + 4 + (long1 ? 8 : 0), n_last, budget);
-  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes + 4 + (long2 ? 8 : 0), cap2, budget);
-  if (p1.count == 0 || p2.count == 0)
-    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked transform needs at "
-                                "least %zu bytes", budget, std::max(p1.need, p2.need));
-  if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
-  if ((rc = pipeline_streams(dc))) return rc;
+  if ((rc = two.plan(call, label_bytes + 4 + (long1 ? 8 : 0), label_bytes + 4 + (long2 ? 8 : 0), cap2, "transform",
+                     chunks)))
+    return rc;
 
   static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
   const auto t0 = std::chrono::steady_clock::now();
-  {
-    ChunkSlots slots;
-    if ((rc = slots.take(dc, p1, plane, label_bytes, 1))) return rc;
-    PipelineSteps steps;
+  rc = run_phase(dc, device, two.p1, label_bytes, 1, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-1 chunk";
     steps.upload = [&](int k, int slot, cudaStream_t s) {
-      return upload(slots.labels[slot], lab_host + (size_t)(p1.start(k) * plane) * label_bytes,
-                    (size_t)(p1.size(k) * plane) * label_bytes, device, s);
+      return upload_box(slots.labels[slot], two.slab(labels, k, label_bytes), device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      int r = x_pass(t, slots.labels[slot], slots.plane(slot, 0), plane / sx * p1.size(k), dc, s);
+      int r = x_pass(t, slots.labels[slot], slots.plane(slot, 0), two.plane / sx * two.p1.size(k), dc, s);
       if (!r && ndim == 3)                                  // behind our own X pass
-        r = later_pass(t, 1, slots.labels[slot], slots.plane(slot, 0), geom_for_axis(1, sx, sy, p1.size(k)), border,
-                       border, dc, s, /*pdl=*/true);
+        r = later_pass(t, 1, slots.labels[slot], slots.plane(slot, 0), geom_for_axis(1, sx, sy, two.p1.size(k)),
+                       border, border, dc, s, /*pdl=*/true);
       return r;
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      return download(out + p1.start(k) * plane, slots.plane(slot, 0), (size_t)(p1.size(k) * plane) * sizeof(float),
-                      device, s);
+      return download_box(two.slab(out, k, sizeof(float)), slots.plane(slot, 0), device, s);
     };
-    if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
-  }
+  });
+  if (rc) return rc;
   const auto t1 = std::chrono::steady_clock::now();
-  {
-    ChunkSlots slots;
-    if ((rc = slots.take(dc, p2, line_vox, label_bytes, 1))) return rc;
-    auto box = [&](const void* base, int64_t k, size_t bytes) { return line_box(base, p2, k, unit, plane, n_last, bytes); };
-    PipelineSteps steps;
+  rc = run_phase(dc, device, two.p2, label_bytes, 1, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-2 chunk";
     steps.upload_writes_results = true;            // the intermediate distances go up into the slot
     steps.upload = [&](int k, int slot, cudaStream_t s) {
-      int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
-      return r ? r : upload_box(slots.plane(slot, 0), box(out_host, k, sizeof(float)), device, s);
+      int r = upload_box(slots.labels[slot], two.lines(labels, k, label_bytes), device, s);
+      return r ? r : upload_box(slots.plane(slot, 0), two.lines(out, k, sizeof(float)), device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      const int64_t c = p2.size(k);
+      const int64_t c = two.p2.size(k);
       const edtb200::LineGeom g = ndim == 3 ? geom_for_axis(2, sx, c, sz) : geom_for_axis(1, c, sy, 1);
       return later_pass(t, last, slots.labels[slot], slots.plane(slot, 0), g, border, border, dc, s, /*pdl=*/false);
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      return download_box(box(out_host, k, sizeof(float)), slots.plane(slot, 0), device, s);
+      return download_box(two.lines(out, k, sizeof(float)), slots.plane(slot, 0), device, s);
     };
-    if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
-  }
+  });
+  if (rc) return rc;
   if (verbose) {
     const auto t2 = std::chrono::steady_clock::now();
     const double ms1 = std::chrono::duration<double, std::milli>(t1 - t0).count();
     const double ms2 = std::chrono::duration<double, std::milli>(t2 - t1).count();
     fprintf(stderr, "[edt_b200] chunked %lldx%lldx%lld L=%d  budget %zu  chunks %lld + %lld  up %.3f GB  down %.3f GB  "
                     "phase 1 %.1f ms  phase 2 %.1f ms\n",
-            (long long)sx, (long long)sy, (long long)sz, label_bytes, budget, (long long)p1.count, (long long)p2.count,
-            (2.0 * label_bytes + 4.0) * (double)total / 1e9, 8.0 * (double)total / 1e9, ms1, ms2);
+            (long long)sx, (long long)sy, (long long)sz, label_bytes, call.budget, (long long)two.p1.count,
+            (long long)two.p2.count, (2.0 * label_bytes + 4.0) * (double)total / 1e9, 8.0 * (double)total / 1e9, ms1,
+            ms2);
   }
   return 0;
 }
@@ -1358,23 +1400,15 @@ int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int n
   for (int k = 0; k < ndim; ++k)
     if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, vol_bytes = (size_t)total * sizeof(float);
-  {
-    struct { const void* p; size_t n; const char* name; } host[5] = {
-        {labels, lab_bytes, "labels"}, {dist_out, vol_bytes, "dist_out"}, {idx_out[0], vol_bytes, "index plane 0"},
-        {idx_out[1], vol_bytes, "index plane 1"}, {ndim == 3 ? idx_out[2] : nullptr, vol_bytes, "index plane 2"}};
-    for (int i = 0; i < 5; ++i)
-      for (int j = i + 1; j < 5; ++j)
-        if (host[i].p && host[j].p && overlap(host[i].p, host[i].n, host[j].p, host[j].n))
-          return fail(EDTB200_EINVAL, "%s and %s overlap", host[i].name, host[j].name);
-  }
+  if ((rc = check_overlap({{labels, lab_bytes, "labels", false}, {dist_out, vol_bytes, "dist_out", true},
+                           {idx_out[0], vol_bytes, "index plane 0", true},
+                           {idx_out[1], vol_bytes, "index plane 1", true},
+                           {ndim == 3 ? idx_out[2] : nullptr, vol_bytes, "index plane 2", true}})))
+    return rc;
 
-  DeviceGuard restore_device;
-  DeviceCache* dcp = nullptr;
-  if ((rc = probe(device, &dcp))) return rc;
-  DeviceCache& dc = *dcp;
-  std::lock_guard<std::mutex> host_call(dc.host_call);
-  size_t budget = 0;
-  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+  StreamingCall call;
+  if ((rc = call.open(device)) || (rc = call.lock(device_bytes))) return rc;
+  DeviceCache& dc = *call.dc;
 
   // The phases of edtb200_transform_chunked, on the site-tracking passes.  Phase 1 resolves every
   // voxel's site within its slice (3-D: (qx, qy); 2-D: the X code, qx), phase 2 follows the last
@@ -1383,10 +1417,7 @@ int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int n
   const bool zero_bg = !(flags & EDTB200_SIGNED);
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   const int last = ndim - 1;
-  const int64_t n_last = t.n[last], n_cut = t.n[last - 1];
-  const int64_t plane = total / n_last;                    // voxels of one phase-1 slice
-  const int64_t unit = ndim == 3 ? sx : 1;                 // voxels of one phase-2 slice per row
-  const int64_t line_vox = unit * n_last;                  // voxels of one phase-2 slice
+  TwoPhase two(ndim, sx, sy, sz);
   // Slot volumes (4 bytes per voxel each) beside the labels:
   //   phase 1, 3-D  0 X distances, then qx; 1 Y distances; 2 X codes; 3 Y codes, then qy
   //   phase 1, 2-D  0 X distances; 1 X codes (= qx)
@@ -1394,33 +1425,24 @@ int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int n
   //                 axis's codes, then its coordinate; 5 y (3-D)
   // and per launch of a later pass the long-line kernel's hull, 4 bytes per voxel of the chunk.
   const int planes1 = ndim == 3 ? 4 : 2, planes2 = ndim == 3 ? 6 : 4, codes = ndim == 3 ? 4 : 3;
-  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes + 4 * planes1 + (ndim == 3 ? 4 : 0), n_last, budget);
-  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes + 4 * planes2 + 4, n_cut, budget);
-  if (p1.count == 0 || p2.count == 0)
-    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked feature transform "
-                                "needs at least %zu bytes", budget, std::max(p1.need, p2.need));
-  if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
-  if ((rc = pipeline_streams(dc))) return rc;
+  if ((rc = two.plan(call, label_bytes + 4 * planes1 + (ndim == 3 ? 4 : 0), label_bytes + 4 * planes2 + 4, two.n_cut,
+                     "feature transform", chunks)))
+    return rc;
 
-  const char* lab_host = static_cast<const char*>(labels);
   // the intermediate distances: dist_out, or bit-cast in the last axis's index plane, which phase 2
   // reads them from before it writes that plane
   float* mid = dist_out ? dist_out : reinterpret_cast<float*>(idx_out[last]);
-  {
-    ChunkSlots slots;
-    if ((rc = slots.take(dc, p1, plane, label_bytes, planes1))) return rc;
-    PipelineSteps steps;
+  rc = run_phase(dc, device, two.p1, label_bytes, planes1, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-1 chunk";
     steps.upload = [&](int k, int slot, cudaStream_t s) {
-      return upload(slots.labels[slot], lab_host + (size_t)(p1.start(k) * plane) * label_bytes,
-                    (size_t)(p1.size(k) * plane) * label_bytes, device, s);
+      return upload_box(slots.labels[slot], two.slab(labels, k, label_bytes), device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      const int64_t c = p1.size(k);
+      const int64_t c = two.p1.size(k);
       const void* lab = slots.labels[slot];
       return with_label_width(label_bytes, [&](auto b) {
         int r = launch_first_sites<b>(lab, slots.plane(slot, 0), slots.plane<int>(slot, ndim == 3 ? 2 : 1),
-                                      plane / sx * c, sx, wx, border, kernel_flags(flags, true, false), dc, s);
+                                      two.plane / sx * c, sx, wx, border, kernel_flags(flags, true, false), dc, s);
         if (r || ndim == 2) return r;
         r = launch_later_sites<b>(lab, slots.plane(slot, 0), slots.plane(slot, 1), slots.plane<int>(slot, 3),
                                   geom_for_axis(1, sx, sy, c), wy, border, border, kernel_flags(flags, false, false),
@@ -1430,32 +1452,27 @@ int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int n
       });
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      const int64_t off = p1.start(k) * plane;
-      const size_t bytes = (size_t)(p1.size(k) * plane) * sizeof(float);
-      int r = download(mid + off, slots.plane(slot, ndim == 3 ? 1 : 0), bytes, device, s);
-      if (!r) r = download(idx_out[0] + off, slots.plane(slot, ndim == 3 ? 0 : 1), bytes, device, s);
-      if (!r && ndim == 3) r = download(idx_out[1] + off, slots.plane(slot, 3), bytes, device, s);
+      int r = download_box(two.slab(mid, k, 4), slots.plane(slot, ndim == 3 ? 1 : 0), device, s);
+      if (!r) r = download_box(two.slab(idx_out[0], k, 4), slots.plane(slot, ndim == 3 ? 0 : 1), device, s);
+      if (!r && ndim == 3) r = download_box(two.slab(idx_out[1], k, 4), slots.plane(slot, 3), device, s);
       return r;
     };
-    if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
-  }
-  {
-    ChunkSlots slots;
-    if ((rc = slots.take(dc, p2, line_vox, label_bytes, planes2))) return rc;
-    auto box = [&](const void* base, int64_t k, size_t bytes) { return line_box(base, p2, k, unit, plane, n_last, bytes); };
-    PipelineSteps steps;
+  });
+  if (rc) return rc;
+  return run_phase(dc, device, two.p2, label_bytes, planes2, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-2 chunk";
     steps.upload_writes_results = true;            // volume 0 goes up and comes back down as x
     steps.upload = [&](int k, int slot, cudaStream_t s) {
-      int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
-      if (!r) r = upload_box(slots.plane(slot, 0), box(mid, k, sizeof(float)), device, s);
-      for (int a = 0; !r && a < ndim - 1; ++a) r = upload_box(slots.plane(slot, 2 + a), box(idx_out[a], k, 4), device, s);
+      int r = upload_box(slots.labels[slot], two.lines(labels, k, label_bytes), device, s);
+      if (!r) r = upload_box(slots.plane(slot, 0), two.lines(mid, k, 4), device, s);
+      for (int a = 0; !r && a < ndim - 1; ++a)
+        r = upload_box(slots.plane(slot, 2 + a), two.lines(idx_out[a], k, 4), device, s);
       return r;
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      const int64_t c = p2.size(k);
+      const int64_t c = two.p2.size(k);
       const edtb200::LineGeom g = ndim == 3 ? geom_for_axis(2, sx, c, sz) : geom_for_axis(1, c, sy, 1);
-      const edtb200::SiteBox sb{ndim, ndim == 3 ? sx : c, unit * c, n_last, p2.start(k)};
+      const edtb200::SiteBox sb{ndim, ndim == 3 ? sx : c, two.unit * c, two.n_last, two.p2.start(k)};
       const void* lab = slots.labels[slot];
       return with_label_width(label_bytes, [&](auto b) {
         const int r = launch_later_sites<b>(lab, slots.plane(slot, 0), slots.plane(slot, 1),
@@ -1468,15 +1485,13 @@ int edtb200_feature_transform_chunked(const void* labels, int label_bytes, int n
       });
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      int r = dist_out ? download_box(box(dist_out, k, sizeof(float)), slots.plane(slot, 1), device, s) : 0;
-      if (!r) r = download_box(box(idx_out[0], k, 4), slots.plane(slot, 0), device, s);
-      if (!r && ndim == 3) r = download_box(box(idx_out[1], k, 4), slots.plane(slot, 5), device, s);
-      if (!r) r = download_box(box(idx_out[last], k, 4), slots.plane(slot, codes), device, s);
+      int r = dist_out ? download_box(two.lines(dist_out, k, 4), slots.plane(slot, 1), device, s) : 0;
+      if (!r) r = download_box(two.lines(idx_out[0], k, 4), slots.plane(slot, 0), device, s);
+      if (!r && ndim == 3) r = download_box(two.lines(idx_out[1], k, 4), slots.plane(slot, 5), device, s);
+      if (!r) r = download_box(two.lines(idx_out[last], k, 4), slots.plane(slot, codes), device, s);
       return r;
     };
-    if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
-  }
-  return 0;
+  });
 }
 
 // Slot bytes of one group of edtb200_transform_stack on host buffers (include/edt_b200.h).
@@ -1496,14 +1511,13 @@ int edtb200_transform_stack(const void* labels, int label_bytes, int ndim, int64
   if (in_dev != out_dev)
     return fail(EDTB200_EINVAL, "edtb200_transform_stack takes labels and out both on the device or both on the host");
   const size_t vol_lab = (size_t)vol * (size_t)label_bytes, vol_out = (size_t)vol * sizeof(float);
-  const char* lab_host = static_cast<const char*>(labels);
-  if (!in_dev && overlap(lab_host, vol_lab * (size_t)count, out, vol_out * (size_t)count))
-    return fail(EDTB200_EINVAL, "labels and out overlap");
+  if (!in_dev && (rc = check_overlap({{labels, vol_lab * (size_t)count, "labels", false},
+                                      {out, vol_out * (size_t)count, "out", true}})))
+    return rc;
 
-  DeviceGuard restore_device;
-  DeviceCache* dcp = nullptr;
-  if ((rc = probe(device, &dcp))) return rc;
-  DeviceCache& dc = *dcp;
+  StreamingCall call;
+  if ((rc = call.open(device))) return rc;
+  DeviceCache& dc = *call.dc;
   const int border = black_border != 0;
   if (in_dev) {                                  // asynchronous on the caller's stream, no lock
     rc = run_passes(labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags, out, dc,
@@ -1514,9 +1528,7 @@ int edtb200_transform_stack(const void* labels, int label_bytes, int ndim, int64
 
   // Host buffers: groups of whole volumes through two device slots, planned as a phase of
   // edtb200_transform_chunked whose slices are volumes.
-  std::lock_guard<std::mutex> host_call(dc.host_call);
-  size_t budget = 0;
-  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+  if ((rc = call.lock(device_bytes))) return rc;
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
   bool long_any = false;                         // a later pass takes the long-line kernel: its scratch
   for (int k = 1; k < ndim; ++k)
@@ -1526,27 +1538,27 @@ int edtb200_transform_stack(const void* labels, int label_bytes, int ndim, int64
   // uploads and downloads overlap each other's passes, as edtb200_transform_batch's volumes do.
   const size_t voxel_bytes = label_bytes + 4 + (long_any ? 8 : 0);
   const int64_t most = std::max<int64_t>(1, (int64_t)(kStackGroupBytes / ((size_t)vol * voxel_bytes)));
-  const PhasePlan p = plan_phase(count, vol, voxel_bytes, most, budget);
+  const PhasePlan p = call.plan(count, vol, voxel_bytes, most);
   if (p.count == 0)
     return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one group of volumes: the stack needs at "
-                                "least %zu bytes", budget, p.need);
+                                "least %zu bytes", call.budget, p.need);
   if (p.count > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many groups of volumes");
-  if ((rc = pipeline_streams(dc))) return rc;
-  ChunkSlots slots;
-  if ((rc = slots.take(dc, p, vol, label_bytes, 1))) return rc;
-  PipelineSteps steps;
-  steps.item = "group";
-  steps.upload = [&](int k, int slot, cudaStream_t s) {
-    return upload(slots.labels[slot], lab_host + (size_t)p.start(k) * vol_lab, (size_t)p.size(k) * vol_lab, device, s);
-  };
-  steps.passes = [&](int k, int slot, cudaStream_t s) {
-    return run_passes(slots.labels[slot], label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags,
-                      slots.plane(slot, 0), dc, s, p.size(k));
-  };
-  steps.download = [&](int k, int slot, cudaStream_t s) {
-    return download(out + p.start(k) * vol, slots.plane(slot, 0), (size_t)p.size(k) * vol_out, device, s);
-  };
-  if ((rc = run_pipeline(dc, device, (int)p.count, steps))) return rc;   // every download has landed
+  const char* lab_host = static_cast<const char*>(labels);
+  rc = run_phase(dc, device, p, label_bytes, 1, [&](const ChunkSlots& slots, PipelineSteps& steps) {
+    steps.item = "group";
+    steps.upload = [&](int k, int slot, cudaStream_t s) {
+      return upload(slots.labels[slot], lab_host + (size_t)p.start(k) * vol_lab, (size_t)p.size(k) * vol_lab,
+                    device, s);
+    };
+    steps.passes = [&](int k, int slot, cudaStream_t s) {
+      return run_passes(slots.labels[slot], label_bytes, ndim, sx, sy, sz, wx, wy, wz, border, flags,
+                        slots.plane(slot, 0), dc, s, p.size(k));
+    };
+    steps.download = [&](int k, int slot, cudaStream_t s) {
+      return download(out + p.start(k) * vol, slots.plane(slot, 0), (size_t)p.size(k) * vol_out, device, s);
+    };
+  });
+  if (rc) return rc;
   if (groups) *groups = p.count;
   return 0;
 }
@@ -1788,16 +1800,13 @@ int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, c
   int64_t sx2 = 2 * sx, sy2 = 2 * sy, sz2 = ndim == 3 ? 2 * sz : 1;
   if ((rc = check_dims(1, ndim, sx2, sy2, sz2))) return rc;
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
-  if (overlap(labels, lab_bytes, out, out_bytes)) return fail(EDTB200_EINVAL, "labels and out overlap");
-  if (overlap(graph, (size_t)total, out, out_bytes)) return fail(EDTB200_EINVAL, "graph and out overlap");
+  if ((rc = check_overlap({{labels, lab_bytes, "labels", false}, {graph, (size_t)total, "graph", false},
+                           {out, out_bytes, "out", true}})))
+    return rc;
 
-  DeviceGuard restore_device;
-  DeviceCache* dcp = nullptr;
-  if ((rc = probe(device, &dcp))) return rc;
-  DeviceCache& dc = *dcp;
-  std::lock_guard<std::mutex> host_call(dc.host_call);
-  size_t budget = 0;
-  if ((rc = chunk_budget(dc, device_bytes, &budget))) return rc;
+  StreamingCall call;
+  if ((rc = call.open(device)) || (rc = call.lock(device_bytes))) return rc;
+  DeviceCache& dc = *call.dc;
 
   // The doubled grid's passes couple the cells of one line and the result samples even cells only,
   // so after the passes along the first axes each voxel carries two cells into the last pass: those
@@ -1811,15 +1820,13 @@ int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, c
   const int border = black_border != 0, as_float = (flags & EDTB200_LABELS_FLOAT) ? 1 : 0;
   const Transform t{1, ndim, 0, border, {wx / 2, wy / 2, wz / 2}, {sx2, sy2, sz2}};
   const int last = ndim - 1;
-  const int64_t n_last = ndim == 3 ? sz : sy, n_cut = ndim == 3 ? sy : sx;
-  const int64_t plane = total / n_last;                    // voxels of one phase-1 slice
-  const int64_t unit = ndim == 3 ? sx : 1;                 // voxels of one phase-2 slice per row
-  const int64_t line_vox = unit * n_last;                  // voxels of one phase-2 slice
+  TwoPhase two(ndim, sx, sy, sz);                          // cut in voxels, not doubled cells
+  const int64_t plane = two.plane, n_last = two.n_last;
   const int cells = ndim == 3 ? 8 : 4;                     // doubled cells per voxel in phase 1
-  const int64_t cap2 = std::max<int64_t>(1, (int64_t)((((int64_t)1 << 32) - 65) / (2 * line_vox)));
+  const int64_t cap2 = std::max<int64_t>(1, (int64_t)((((int64_t)1 << 32) - 65) / (2 * two.line_vox)));
   const bool long1 = ndim == 3 && later_pass_is_long(geom_for_axis(1, sx2, sy2, sz2), transform_arith(t.w, t.n, 1),
                                                      dc.max_smem_optin);
-  const int64_t c2 = std::min(n_cut, cap2);
+  const int64_t c2 = std::min(two.n_cut, cap2);
   const LineGeom g2 = ndim == 3 ? geom_for_axis(2, sx, c2, sz2) : geom_for_axis(1, c2, sy2, 1);
   const bool long2 = later_pass_is_long(g2, transform_arith(t.w, t.n, last), dc.max_smem_optin);
   // Slot volumes (4 bytes per voxel each) beside the labels and the graph:
@@ -1828,35 +1835,26 @@ int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, c
   //   phase 2  0, 1 the doubled lines; 2 cell 2l, then the result; 3 cell 2l + 1; 4 the lines' mask
   // and per launch of a later pass the long-line kernel's two scratch volumes of the doubled cells.
   const int planes1 = cells + 2 + cells / 4, planes2 = 5;
-  const PhasePlan p1 = plan_phase(n_last, plane, label_bytes + 1 + 4 * planes1 + (long1 ? 8 * cells : 0), n_last,
-                                  budget);
-  const PhasePlan p2 = plan_phase(n_cut, line_vox, label_bytes + 1 + 4 * planes2 + (long2 ? 16 : 0), cap2, budget);
-  if (p1.count == 0 || p2.count == 0)
-    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one chunk: the chunked voxel-graph "
-                                "transform needs at least %zu bytes", budget, std::max(p1.need, p2.need));
-  if (chunks) { chunks[0] = p1.count; chunks[1] = p2.count; }
+  if ((rc = two.plan(call, label_bytes + 1 + 4 * planes1 + (long1 ? 8 * cells : 0),
+                     label_bytes + 1 + 4 * planes2 + (long2 ? 16 : 0), cap2, "voxel-graph transform", chunks)))
+    return rc;
   std::unique_ptr<float, decltype(&free)> odd_cells(static_cast<float*>(malloc(out_bytes)), &free);
   if (!odd_cells)
     return fail(EDTB200_ENOMEM, "no host memory for the %zu-byte scratch of the odd cells between the phases",
                 out_bytes);
-  if ((rc = pipeline_streams(dc))) return rc;
 
-  const char* lab_host = static_cast<const char*>(labels);
   const int threads = 256;
   auto blocks = [&](int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + threads - 1) / threads,
                                                                                       (int64_t)dc.sm_count * 32)); };
-  {
-    ChunkSlots slots;
-    if ((rc = slots.take(dc, p1, plane, label_bytes + 1, planes1))) return rc;
-    PipelineSteps steps;
+  rc = run_phase(dc, device, two.p1, label_bytes + 1, planes1, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-1 chunk";
     steps.upload = [&](int k, int slot, cudaStream_t s) {
-      const size_t off = (size_t)(p1.start(k) * plane), n = (size_t)(p1.size(k) * plane);
-      const int r = upload(slots.labels[slot], lab_host + off * label_bytes, n * label_bytes, device, s);
-      return r ? r : upload(static_cast<char*>(slots.labels[slot]) + slots.vox * label_bytes, graph + off, n, device, s);
+      const int r = upload_box(slots.labels[slot], two.slab(labels, k, label_bytes), device, s);
+      return r ? r : upload_box(static_cast<char*>(slots.labels[slot]) + slots.vox * label_bytes, two.slab(graph, k, 1),
+                                device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      const int64_t c = p1.size(k), z0 = p1.start(k);
+      const int64_t c = two.p1.size(k), z0 = two.p1.start(k);
       const int64_t cy = ndim == 3 ? sy : c, cz = ndim == 3 ? c : 1;              // the slab's extents
       const uint8_t* gr = reinterpret_cast<const uint8_t*>(slots.labels[slot]) + slots.vox * label_bytes;
       float* f = slots.plane(slot, 0);
@@ -1882,28 +1880,23 @@ int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, c
       return 0;
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      const int64_t off = p1.start(k) * plane;
-      const size_t bytes = (size_t)(p1.size(k) * plane) * sizeof(float);
-      const int r = download(out + off, slots.plane(slot, cells), bytes, device, s);
-      return r ? r : download(odd_cells.get() + off, slots.plane(slot, cells + 1), bytes, device, s);
+      const int r = download_box(two.slab(out, k, sizeof(float)), slots.plane(slot, cells), device, s);
+      return r ? r : download_box(two.slab(odd_cells.get(), k, sizeof(float)), slots.plane(slot, cells + 1), device, s);
     };
-    if ((rc = run_pipeline(dc, device, (int)p1.count, steps))) return rc;   // every download has landed
-  }
-  {
-    ChunkSlots slots;
-    if ((rc = slots.take(dc, p2, line_vox, label_bytes + 1, planes2))) return rc;
-    auto box = [&](const void* base, int64_t k, size_t bytes) { return line_box(base, p2, k, unit, plane, n_last, bytes); };
-    PipelineSteps steps;
+  });
+  if (rc) return rc;
+  return run_phase(dc, device, two.p2, label_bytes + 1, planes2, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-2 chunk";
     steps.upload_writes_results = true;            // cell 2l goes up into the volume the result comes down from
     steps.upload = [&](int k, int slot, cudaStream_t s) {
-      int r = upload_box(slots.labels[slot], box(lab_host, k, label_bytes), device, s);
-      if (!r) r = upload_box(static_cast<char*>(slots.labels[slot]) + slots.vox * label_bytes, box(graph, k, 1), device, s);
-      if (!r) r = upload_box(slots.plane(slot, 2), box(out, k, sizeof(float)), device, s);
-      return r ? r : upload_box(slots.plane(slot, 3), box(odd_cells.get(), k, sizeof(float)), device, s);
+      int r = upload_box(slots.labels[slot], two.lines(labels, k, label_bytes), device, s);
+      if (!r) r = upload_box(static_cast<char*>(slots.labels[slot]) + slots.vox * label_bytes, two.lines(graph, k, 1),
+                             device, s);
+      if (!r) r = upload_box(slots.plane(slot, 2), two.lines(out, k, sizeof(float)), device, s);
+      return r ? r : upload_box(slots.plane(slot, 3), two.lines(odd_cells.get(), k, sizeof(float)), device, s);
     };
     steps.passes = [&](int k, int slot, cudaStream_t s) {
-      const int64_t c = p2.size(k), bp = unit * c;          // bp: the box's voxels per index of the last axis
+      const int64_t c = two.p2.size(k), bp = two.unit * c;  // bp: the box's voxels per index of the last axis
       const uint8_t* gr = reinterpret_cast<const uint8_t*>(slots.labels[slot]) + slots.vox * label_bytes;
       float* f = slots.plane(slot, 0);
       uint8_t* mask = slots.plane<uint8_t>(slot, 4);
@@ -1923,11 +1916,9 @@ int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, c
       return 0;
     };
     steps.download = [&](int k, int slot, cudaStream_t s) {
-      return download_box(box(out, k, sizeof(float)), slots.plane(slot, 2), device, s);
+      return download_box(two.lines(out, k, sizeof(float)), slots.plane(slot, 2), device, s);
     };
-    if ((rc = run_pipeline(dc, device, (int)p2.count, steps))) return rc;
-  }
-  return 0;
+  });
 }
 
 int edtb200_pass_first(const void* labels_dev, int label_bytes, int64_t sx, int64_t sy, int64_t sz,

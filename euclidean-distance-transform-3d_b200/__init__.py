@@ -23,6 +23,7 @@ the transform on the device.
 above accepts device-resident input directly (a torch CUDA tensor or any object exposing
 ``__cuda_array_interface__``) and then returns a torch CUDA tensor.
 """
+import collections
 import ctypes
 import os
 
@@ -34,6 +35,7 @@ __all__ = [
   "edt1d", "edt1dsq", "edt2d", "edt2dsq", "edt3d", "edt3dsq",
   "edt_cuda", "transform_batch", "each", "each_cuda", "label_stats_cuda", "device_count", "library_path", "EDTError",
   "feature_transform", "expand_labels",
+  "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
 ]
 
 FLAG_SQRT = 1
@@ -107,6 +109,11 @@ def _lib():
   lib.edtb200_bounded_plan.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
+  lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
+  lib.edtb200_surface_count.restype = ci
+  lib.edtb200_surface_distances.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, vp, i64, ci, vp, vp,
+                                            ci, ctypes.c_size_t, vp, vp]
+  lib.edtb200_surface_distances.restype = ci
   lib.edtb200_transform_multi.argtypes = [vp, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci]
   lib.edtb200_transform_multi.restype = ci
   lib.edtb200_transform_batch.argtypes = [vp, vp, ci, ci, ci, i64, i64, i64, f32, f32, f32, ci, ci, ci]
@@ -1188,6 +1195,274 @@ def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device
   if max_device_bytes is not None:
     _chunk_budget(max_device_bytes, True, None, on_device.dim())
   return _expand_device(on_device, distance, anisotropy, False)
+
+
+# ---------------------------------------------------------------------------------------
+# surface distances between two label volumes: Hausdorff distance, average surface distance and
+# surface Dice (edtb200_surface_count, edtb200_surface_distances)
+# ---------------------------------------------------------------------------------------
+
+SurfaceDistances = collections.namedtuple("SurfaceDistances", "labels offsets values")
+SurfaceDistances.__doc__ = """What surface_distances returns.  labels: the keys, in the caller's dtype;
+offsets: int64, count * K * 2 + 1 entries, segment (volume * K + key) * 2 + direction from
+values[offsets[s]] to values[offsets[s + 1]]; values: float32, each segment sorted ascending."""
+
+
+def _surface_anisotropy(vnd, anisotropy):
+  """One weight per volume axis (a scalar for 1-D volumes); default 1."""
+  if anisotropy is None:
+    return (1.0,) * vnd
+  if np.ndim(anisotropy) == 0 and vnd == 1:
+    return (float(anisotropy),)
+  weights = tuple(float(w) for w in np.asarray(anisotropy).reshape(-1))
+  if len(weights) != vnd:
+    raise ValueError("anisotropy must have one entry per volume axis (%d), got %d" % (vnd, len(weights)))
+  return weights
+
+
+def _surface_keys(labels, dtype):
+  """labels= in the caller's dtype, checked: no 0 and no repeat."""
+  keys = np.asarray(labels, dtype=dtype).reshape(-1)
+  if np.any(keys == 0):
+    raise ValueError("labels must not contain 0 (background)")
+  raw = _label_view(keys)
+  if raw is None:
+    raise TypeError("unsupported label dtype %s" % dtype)
+  if np.unique(raw).size != raw.size:
+    raise ValueError("labels must be distinct")
+  return keys
+
+
+def _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes):
+  """The sorted surface distances of a against b: (keys, offsets, values, count, host) with torch CUDA
+  offsets and values.  Host arrays go up through torch, as expand_labels' do."""
+  import torch
+  da, db = _device_array(a), _device_array(b)
+  host = da is None and db is None
+  if host:
+    na = np.asarray(np.array(a) if isinstance(a, list) else a)
+    nb = np.asarray(np.array(b) if isinstance(b, list) else b)
+    shape, dtype, nd = na.shape, na.dtype, na.ndim
+    if nb.shape != shape:
+      raise ValueError("a and b must have one shape, got %s and %s" % (shape, nb.shape))
+    if nb.dtype != dtype:
+      raise TypeError("a and b must have one dtype, got %s and %s" % (dtype, nb.dtype))
+    if _label_view(na[:0]) is None:
+      raise TypeError("unsupported label dtype %s" % dtype)
+  else:
+    if da is None:
+      da = torch.as_tensor(np.asarray(a), device=db.device)
+    if db is None:
+      db = torch.as_tensor(np.asarray(b), device=da.device)
+    shape, nd = tuple(da.shape), da.dim()
+    if tuple(db.shape) != shape:
+      raise ValueError("a and b must have one shape, got %s and %s" % (shape, tuple(db.shape)))
+    if db.dtype != da.dtype or db.device != da.device:
+      raise TypeError("a and b must have one dtype and device, got %s on %s and %s on %s"
+                      % (da.dtype, da.device, db.dtype, db.device))
+    if _torch_label_bytes(torch).get(da.dtype) is None and da.dtype not in (torch.float32, torch.float64):
+      raise TypeError("unsupported label dtype %s" % da.dtype)
+    dtype = torch.empty(0, dtype=da.dtype).numpy().dtype
+  if stacked:
+    vnd = _stack_dims(nd)
+  elif nd < 1 or nd > 3:
+    raise TypeError("surface distances take 1-D to 3-D volumes, got %d-D" % nd)
+  else:
+    vnd = nd
+  anisotropy = _surface_anisotropy(vnd, anisotropy)
+  keys = None if labels is None else _surface_keys(labels, dtype)
+  budget = 0 if max_device_bytes is None else int(max_device_bytes)
+  if budget < 0:
+    raise ValueError("max_device_bytes must be non-negative (0: what the device has free)")
+  if host:
+    if np.prod(shape) == 0:
+      count = (int(shape[0] if na.flags.c_contiguous else shape[-1])) if stacked else 1
+      keys = np.zeros(0, dtype) if keys is None else keys
+      nseg = count * keys.size * 2
+      return keys, torch.zeros(nseg + 1, dtype=torch.int64), torch.zeros(0, dtype=torch.float32), count, host
+    if device_count() == 0:
+      raise EDTError("edt_b200 error %d: no usable CUDA device; this library has no CPU fallback" % ECUDA, ECUDA)
+    dev = torch.device("cuda", int(device))
+    up = []
+    for x in (na, nb):
+      if not x.flags.c_contiguous and not x.flags.f_contiguous:
+        x = np.ascontiguousarray(x)
+      raw = x if x.dtype.kind == "f" else x.view(np.uint8 if x.itemsize == 1 else np.dtype("i%d" % x.itemsize))
+      up.append(torch.from_numpy(raw).to(dev))
+    da, db = up
+  # raw label bits, as the transforms compare them: -0.0 folded onto +0.0, unsigned as signed of one width
+  raw_of = {torch.float32: torch.int32, torch.float64: torch.int64, torch.bool: torch.uint8}
+  for name in ("uint16", "uint32", "uint64"):
+    if hasattr(torch, name):
+      raw_of[getattr(torch, name)] = getattr(torch, name.replace("u", ""))
+  ta, tb = ((t + 0 if t.is_floating_point() else t).view(raw_of.get(t.dtype, t.dtype)) for t in (da, db))
+  fortran = nd > 1 and not ta.is_contiguous() and ta.permute(*reversed(range(nd))).is_contiguous()
+  if fortran:              # through the transposed (C-ordered) view, as _stack_device and _front_door_device
+    ta, tb = ta.permute(*reversed(range(nd))), tb.permute(*reversed(range(nd)))
+    anisotropy = tuple(reversed(anisotropy))
+  ta, tb = ta.contiguous(), tb.contiguous()
+  count = int(ta.shape[0]) if stacked else 1      # the slowest axis in memory indexes the volumes
+  rtype = np.dtype("u%d" % ta.element_size())
+  if keys is None:
+    if ta.numel():
+      raw = np.union1d(torch.unique(ta).cpu().numpy(), torch.unique(tb).cpu().numpy()).view(rtype)
+    else:
+      raw = np.zeros(0, rtype)
+    raw = raw[raw != 0]
+    keys = raw.view(dtype)[np.argsort(raw.view(dtype), kind="stable")]     # sorted by the caller's value
+  raw_keys = (keys + 0 if keys.dtype.kind == "f" else keys).view(rtype)
+  perm = np.argsort(raw_keys, kind="stable")             # the C ABI takes the keys ascending as raw bits
+  sorted_keys = np.ascontiguousarray(raw_keys[perm])
+  nkeys = keys.size
+  nseg = count * nkeys * 2
+  dev = ta.device
+  counts = torch.zeros(nseg, dtype=torch.int64, device=dev)
+  stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+  (sx, sy, sz), (wx, wy, wz) = _x_fastest(ta.shape[1:] if stacked else ta.shape, anisotropy, False)
+  both = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
+  lib = _lib()
+  _check(lib.edtb200_surface_count(ta.data_ptr(), tb.data_ptr(), ta.element_size(), vnd, sx, sy, sz, count,
+                                   sorted_keys.ctypes.data, nkeys, both, counts.data_ptr(), dev.index, stream))
+  offsets = torch.zeros(nseg + 1, dtype=torch.int64, device=dev)
+  torch.cumsum(counts, 0, out=offsets[1:])
+  total = int(offsets[-1].item())
+  values = torch.empty(max(total, 1), dtype=torch.float32, device=dev)
+  _check(lib.edtb200_surface_distances(
+    ta.data_ptr(), tb.data_ptr(), ta.element_size(), vnd, sx, sy, sz, count, wx, wy, wz, sorted_keys.ctypes.data,
+    nkeys, both, offsets.data_ptr(), values.data_ptr(), dev.index, budget, None, stream))
+  values = values[:total]
+  # Segment (v, r, d) of sorted key r is the caller's segment (v, perm[r], d).  One sort on
+  # (segment << 32 | distance bits) -- non-negative floats order like their bits -- groups the
+  # segments in the caller's order and sorts each ascending.
+  new_of_old = (np.arange(count)[:, None, None] * nkeys + perm[None, :, None]) * 2 + np.arange(2)[None, None, :]
+  new_of_old = torch.from_numpy(new_of_old.reshape(-1)).to(dev)
+  seg_ids = torch.repeat_interleave(new_of_old, counts, output_size=total)
+  key = (seg_ids << 32) | values.view(torch.int32).to(torch.int64)
+  values = (torch.sort(key).values & 0xffffffff).to(torch.int32).view(torch.float32)
+  new_counts = torch.zeros_like(counts)
+  new_counts[new_of_old] = counts
+  offsets = torch.zeros_like(offsets)
+  torch.cumsum(new_counts, 0, out=offsets[1:])
+  return keys, offsets, values, count, host
+
+
+def surface_distances(a, b, anisotropy=None, *, labels=None, stacked=False, device=0, max_device_bytes=None):
+  """The surface distances of two label volumes a (prediction) and b (reference) of one shape: what
+  the Hausdorff distance, the average surface distance and surface Dice are formed from, on the GPU.
+
+  For a volume v and key k, the surface S_v(k) is the voxels of label k with a face neighbour of
+  another label or on a face of the volume (scipy's mask ^ binary_erosion(mask), border_value 0; in
+  a stack neighbours never cross into the next volume).  d_v,k(q) is the float32 distance from q to
+  the nearest voxel of S_v(k) under `anisotropy`, exactly edt(mask) of the mask that is 0 on S_v(k)
+  and 1 elsewhere (+inf when S_v(k) is empty).  A->B for key k is {d_b,k(q) : q in S_a(k)}, B->A the
+  other way round.
+
+  `labels` (in the caller's dtype, distinct and non-zero) are the keys; the default is the sorted
+  union of the non-zero labels of a and b.  Labels compare as edt() compares them (floats by value).
+  `stacked=True` takes stacks of volumes along the slowest axis in memory, as edt(stacked=True) does.
+  `max_device_bytes` bounds the device memory of the transforms (None or 0: what the GPU has free).
+
+  Returns SurfaceDistances(labels, offsets, values): segment s = (volume * K + key) * 2 + direction
+  (0: A->B, 1: B->A; volume 0 without `stacked`) is values[offsets[s]:offsets[s + 1]], sorted
+  ascending.  numpy arrays for host input; torch CUDA tensors for device input, computed on the
+  current stream."""
+  import torch
+  keys, offsets, values, _, host = _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes)
+  if host:
+    return SurfaceDistances(keys, offsets.cpu().numpy(), values.cpu().numpy())
+  return SurfaceDistances(torch.from_numpy(np.ascontiguousarray(keys)).to(offsets.device), offsets, values)
+
+
+def _surface_metric(a, b, anisotropy, labels, stacked, device, max_device_bytes, reduce):
+  """reduce(offsets, values, n) -> float64 (count, K) tensor from the sorted segments, with n the
+  (count, K, 2) segment lengths; then the empty-surface rules and the caller's shape and type."""
+  import torch
+  keys, offsets, values, count, host = _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes)
+  nkeys = keys.size
+  n = (offsets[1:] - offsets[:-1]).reshape(count, nkeys, 2)
+  out = reduce(offsets, values.to(torch.float64), n) if values.numel() else \
+      torch.zeros((count, nkeys), dtype=torch.float64, device=offsets.device)
+  out = torch.where((n[..., 0] == 0) & (n[..., 1] == 0), torch.full_like(out, float("nan")), out)
+  if not stacked:
+    out = out[0]
+  return out.cpu().numpy() if host else out
+
+
+def _segment_sums(offsets, x):
+  import torch
+  return torch.segment_reduce(x, "sum", offsets=offsets, unsafe=True)
+
+
+def hausdorff_distance(a, b, anisotropy=None, *, percentile=None, directed=False, labels=None, stacked=False, device=0,
+                       max_device_bytes=None):
+  """The Hausdorff distance between the surfaces of a (prediction) and b (reference) per key (see
+  surface_distances for the definitions and arguments): the largest distance A->B, or with
+  `percentile=p` np.percentile(A->B, p, method="linear"); with `directed=False` the larger of that over
+  A->B and over B->A.  Per key it is NaN when both surfaces are empty and +inf when one is.
+
+  Returns float64 of shape (K,), or (count, K) with `stacked`, in the order of `labels` (default: the
+  sorted union of the non-zero labels): numpy for host input, a torch CUDA tensor for device input."""
+  if percentile is not None:
+    percentile = float(percentile)
+    if not 0.0 <= percentile <= 100.0:
+      raise ValueError("percentile must be within [0, 100], got %r" % (percentile,))
+
+  def reduce(offsets, v, n):
+    import torch
+    start, length = offsets[:-1].reshape(n.shape), n
+    if percentile is None:
+      at = (start + length - 1).clamp(min=0)
+      d = v[at.clamp(max=v.numel() - 1)]
+    else:       # numpy's linear rule, its two-sided lerp included
+      pos = (percentile / 100.0) * (length - 1).clamp(min=0).to(torch.float64)
+      lo = pos.floor()
+      t = pos - lo
+      lo = lo.to(torch.int64)
+      hi = torch.minimum(lo + 1, (length - 1).clamp(min=0))
+      xa = v[(start + lo).clamp(max=v.numel() - 1)]
+      xb = v[(start + hi).clamp(max=v.numel() - 1)]
+      diff = xb - xa
+      d = torch.where(t >= 0.5, xb - diff * (1 - t), xa + diff * t)
+    d = d[..., 0] if directed else torch.maximum(d[..., 0], d[..., 1])
+    return torch.where((n[..., 0] == 0) | (n[..., 1] == 0), torch.full_like(d, float("inf")), d)
+  return _surface_metric(a, b, anisotropy, labels, stacked, device, max_device_bytes, reduce)
+
+
+def average_surface_distance(a, b, anisotropy=None, *, symmetric=False, labels=None, stacked=False, device=0,
+                             max_device_bytes=None):
+  """The average surface distance per key (see surface_distances for the definitions and arguments):
+  the mean of A->B, or with `symmetric=True` the mean of A->B and B->A taken together.  Per key it is
+  NaN when both surfaces are empty and +inf when one is.  The sums are formed in float64 from the
+  sorted segments, so the result does not depend on the order the GPU found the distances in.
+
+  Returns float64 of shape (K,), or (count, K) with `stacked`, as hausdorff_distance does."""
+  def reduce(offsets, v, n):
+    import torch
+    sums = _segment_sums(offsets, v).reshape(n.shape)
+    if symmetric:
+      m = sums.sum(-1) / n.sum(-1).to(torch.float64)
+    else:
+      m = sums[..., 0] / n[..., 0].to(torch.float64)
+    return torch.where((n[..., 0] == 0) | (n[..., 1] == 0), torch.full_like(m, float("inf")), m)
+  return _surface_metric(a, b, anisotropy, labels, stacked, device, max_device_bytes, reduce)
+
+
+def surface_dice(a, b, tolerance, anisotropy=None, *, labels=None, stacked=False, device=0, max_device_bytes=None):
+  """Surface Dice at `tolerance` per key (see surface_distances for the definitions and arguments):
+  (#{A->B <= tolerance} + #{B->A <= tolerance}) / (|S_a| + |S_b|), the distances compared in float64.
+  Per key it is NaN when both surfaces are empty and 0 when one is.
+
+  Returns float64 of shape (K,), or (count, K) with `stacked`, as hausdorff_distance does."""
+  tau = float(tolerance)
+  if not tau >= 0.0:
+    raise ValueError("tolerance must be zero or more, got %r" % (tolerance,))
+
+  def reduce(offsets, v, n):
+    import torch
+    within = _segment_sums(offsets, (v <= tau).to(torch.float64)).reshape(n.shape)
+    dice = within.sum(-1) / n.sum(-1).to(torch.float64)
+    return torch.where((n[..., 0] == 0) | (n[..., 1] == 0), torch.zeros_like(dice), dice)
+  return _surface_metric(a, b, anisotropy, labels, stacked, device, max_device_bytes, reduce)
 
 
 # ---------------------------------------------------------------------------------------

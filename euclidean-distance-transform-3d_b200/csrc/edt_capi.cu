@@ -1713,6 +1713,154 @@ int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t
   });
 }
 
+}  // extern "C"
+
+namespace {
+
+constexpr int64_t kSurfaceGroupVoxels = int64_t(1) << 31;   // mask voxels of one group of surface slots
+
+// The checks edtb200_surface_count and edtb200_surface_distances share before their pointers: the
+// geometry, count, nkeys and the host keys (non-zero, strictly ascending as unsigned integers of
+// label_bytes).  *empty: nothing to do (no voxel, no volume or no key).
+int check_surface(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count, const void* keys,
+                  int64_t nkeys, bool* empty) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (nkeys < 0) return fail(EDTB200_EINVAL, "negative nkeys");
+  if (nkeys > 0 && !keys) return fail(EDTB200_EINVAL, "null pointer (keys)");
+  uint64_t prev = 0;
+  for (int64_t k = 0; k < nkeys; ++k) {
+    uint64_t key = 0;
+    memcpy(&key, static_cast<const char*>(keys) + k * label_bytes, (size_t)label_bytes);   // little-endian
+    if (key == 0) return fail(EDTB200_EINVAL, "key %lld is 0 (background)", (long long)k);
+    if (k > 0 && key <= prev) return fail(EDTB200_EINVAL, "keys must be strictly ascending (key %lld)", (long long)k);
+    prev = key;
+  }
+  if (nkeys > 0 && count > ((int64_t)1 << 60) / nkeys) return fail(EDTB200_ELIMIT, "too many (volume, key) pairs");
+  *empty = sx * sy * sz == 0 || count == 0 || nkeys == 0;
+  return 0;
+}
+
+int check_surface_flags(int flags, const char* name) {
+  const int both = EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE;
+  if (flags != both)
+    return fail(EDTB200_EINVAL, "%s works on device buffers only: flags must be EDTB200_LABELS_ON_DEVICE | "
+                                "EDTB200_OUT_ON_DEVICE (got %d)", name, flags);
+  return 0;
+}
+
+// The keys on the device, for the kernels' search.
+int upload_keys(Scratch& dev, const void* keys, int64_t nkeys, int label_bytes, DeviceCache& dc, cudaStream_t s) {
+  const size_t bytes = (size_t)nkeys * (size_t)label_bytes;
+  if (dev.alloc(dc, bytes, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the keys");
+  }
+  CUDA_TRY(cudaMemcpyAsync(dev.get(), keys, bytes, cudaMemcpyHostToDevice, s));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int edtb200_surface_count(const void* a, const void* b, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                          int64_t count, const void* keys, int64_t nkeys, int flags, int64_t* counts, int device,
+                          void* stream_v) {
+  bool empty = false;
+  int rc = check_surface(label_bytes, ndim, sx, sy, sz, count, keys, nkeys, &empty);
+  if (rc || empty) return rc;
+  if (!a || !b || !counts) return fail(EDTB200_EINVAL, "null pointer");
+  if ((rc = check_surface_flags(flags, "edtb200_surface_count"))) return rc;
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  if ((rc = probe(device, &dc))) return rc;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream_v);
+  const int64_t slots = count * nkeys * 2;
+  Scratch dev_keys;
+  if ((rc = upload_keys(dev_keys, keys, nkeys, label_bytes, *dc, s))) return rc;
+  CUDA_TRY(cudaMemsetAsync(counts, 0, sizeof(int64_t) * (size_t)slots, s));
+  const edtb200::SurfaceSlots g{ndim, sx, sy, sz, sx * sy * sz, nkeys, 0, slots, 0, count};
+  return with_label_width(label_bytes, [&](auto w) {
+    return launch_surface<w>(a, b, dev_keys.get(), g, nullptr, nullptr, reinterpret_cast<unsigned long long*>(counts),
+                             nullptr, *dc, s);
+  });
+}
+
+int edtb200_surface_distances(const void* a, const void* b, int label_bytes, int ndim, int64_t sx, int64_t sy,
+                              int64_t sz, int64_t count, float wx, float wy, float wz, const void* keys, int64_t nkeys,
+                              int flags, const int64_t* offsets, float* values, int device, size_t device_bytes,
+                              int64_t* groups, void* stream_v) {
+  if (groups) *groups = 0;
+  bool empty = false;
+  int rc = check_surface(label_bytes, ndim, sx, sy, sz, count, keys, nkeys, &empty);
+  if (rc || empty) return rc;
+  if (!a || !b || !offsets || !values) return fail(EDTB200_EINVAL, "null pointer");
+  if ((rc = check_surface_flags(flags, "edtb200_surface_distances"))) return rc;
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  if ((rc = probe(device, &dc))) return rc;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream_v);
+  const int64_t vol = sx * sy * sz, slots = count * nkeys * 2;
+  // A slot costs its mask, its distances and, where a later pass takes the long-line kernel, that
+  // kernel's two scratch volumes: the stack planner's rule (edtb200_transform_stack).
+  const float w[3] = {wx, wy, wz};
+  const int64_t n[3] = {sx, sy, sz};
+  bool long_any = false;
+  for (int k = 1; k < ndim; ++k)
+    long_any = long_any || later_pass_is_long(geom_for_axis(k, sx, sy, sz), transform_arith(w, n, k), dc->max_smem_optin);
+  const size_t slot_bytes = (size_t)vol * (1 + 4 + (long_any ? 8 : 0));
+  size_t budget = device_bytes;
+  if (budget == 0) {
+    size_t free_bytes = 0, total_bytes = 0;
+    CUDA_TRY(cudaMemGetInfo(&free_bytes, &total_bytes));
+    budget = free_bytes > EDTB200_CHUNK_RESERVE ? free_bytes - EDTB200_CHUNK_RESERVE : 0;
+  }
+  const int64_t fit = std::min<int64_t>(slots, (int64_t)(budget / slot_bytes));
+  if (fit == 0)
+    return fail(EDTB200_ENOMEM, "a device budget of %zu bytes cannot hold one slot: the surface distances need at "
+                                "least %zu bytes", budget, slot_bytes);
+  // A group's masks hold at most kSurfaceGroupVoxels voxels (at least one slot), so that a call takes
+  // no more memory than the transforms need to stream at full rate.
+  const int64_t cap = std::max<int64_t>(1, kSurfaceGroupVoxels / vol);
+  const int64_t fit_capped = std::min(fit, cap);
+  const int64_t ngroups = (slots + fit_capped - 1) / fit_capped, most = (slots + ngroups - 1) / ngroups;
+
+  Scratch dev_keys, cursor, buf;
+  if ((rc = upload_keys(dev_keys, keys, nkeys, label_bytes, *dc, s))) return rc;
+  // the distances of a group's slots, then their masks
+  const size_t dist_bytes = ((size_t)most * (size_t)vol * 4 + 255) & ~size_t(255);
+  if (cursor.alloc(*dc, sizeof(int64_t) * (size_t)slots, s) != cudaSuccess ||
+      buf.alloc(*dc, dist_bytes + (size_t)most * (size_t)vol, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for a group of %lld slots", (long long)most);
+  }
+  auto* cur = cursor.get<unsigned long long>();
+  float* dist = buf.get<float>();
+  uint8_t* mask = buf.get<uint8_t>() + dist_bytes;
+  CUDA_TRY(cudaMemcpyAsync(cur, offsets, sizeof(int64_t) * (size_t)slots, cudaMemcpyDeviceToDevice, s));
+  for (int64_t grp = 0; grp < ngroups; ++grp) {
+    const int64_t s0 = slots * grp / ngroups, s1 = slots * (grp + 1) / ngroups;
+    const edtb200::SurfaceSlots g{ndim, sx, sy, sz, vol, nkeys, s0, s1, s0 / (2 * nkeys), (s1 - 1) / (2 * nkeys) + 1};
+    CUDA_TRY(cudaMemsetAsync(mask, 1, (size_t)(s1 - s0) * (size_t)vol, s));
+    rc = with_label_width(label_bytes, [&](auto lw) {
+      return launch_surface<lw>(a, b, dev_keys.get(), g, mask, nullptr, nullptr, nullptr, *dc, s);
+    });
+    if (!rc) rc = run_passes(mask, 1, ndim, sx, sy, sz, wx, wy, wz, 0, EDTB200_SQRT, dist, *dc, s, s1 - s0);
+    if (!rc) {
+      rc = with_label_width(label_bytes, [&](auto lw) {
+        return launch_surface<lw>(a, b, dev_keys.get(), g, nullptr, dist, cur + s0, values, *dc, s);
+      });
+    }
+    if (rc) return rc;
+  }
+  if (groups) *groups = ngroups;
+  return 0;
+}
+
 int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const unsigned char* graph, int ndim,
                                   int64_t sx, int64_t sy, int64_t sz, float wx, float wy, float wz,
                                   int black_border, int flags, float* out, int device, void* stream_v) {

@@ -1,10 +1,10 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as seven translation units so that the kernel templates build in
+// The library is compiled as eight translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
-// later-axis plan for host code that launches nothing) and edt_bounded.cu (the bounded
-// transforms' kernels).  The run-time label width
+// later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
+// transforms' kernels) and edt_surface.cu (the surface distances' kernels).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -249,6 +249,27 @@ int launch_later_window(const void* labels, const float* fin, float* fout, int* 
 template <int Bytes>
 int launch_bounded_cut(const void* labels, float* f, int* codes, int64_t total, float bound, int flags,
                        DeviceCache& dc, cudaStream_t stream);
+
+}  // namespace host
+
+// The slots of the surface kernels (edt_surface.cuh): a stack of volumes of (sx, sy, sz), `vol` voxels
+// each, nkeys keys, slot s = (volume * nkeys + key) * 2 + direction.  A launch covers the slots
+// [s0, s1), and so the volumes [v0, v1).
+struct SurfaceSlots {
+  int ndim;
+  int64_t sx, sy, sz, vol, nkeys;
+  int64_t s0, s1, v0, v1;
+};
+
+namespace host {
+
+// The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
+// device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:
+// surface_gather_kernel of `dist` (the masks' distances) through `cursor` (one per slot of the range);
+// else surface_count_kernel, adding into `cursor`.
+template <int Bytes>
+int launch_surface(const void* a, const void* b, const void* keys, const SurfaceSlots& g, uint8_t* mask,
+                   const float* dist, unsigned long long* cursor, float* values, DeviceCache& dc, cudaStream_t stream);
 
 // Whether plan_later (edt_passes.cuh) sends a later-axis pass over geometry g with arithmetic
 // `arith` to the long-line kernel (edt_plan.cu).

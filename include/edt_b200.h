@@ -36,7 +36,7 @@ extern "C" {
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
- * edtb200_expand_gather)
+ * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -269,6 +269,61 @@ int edtb200_expand_gather(const void *labels, int label_bytes, int ndim,
                           int64_t sx, int64_t sy, int64_t sz, int64_t count,
                           const float *sqdist, const int32_t *const *idx,
                           double limit_sq, int flags, void *out, int device, void *stream);
+
+/* Surface distances between two label volumes a (prediction) and b (reference) of one geometry, the
+ * inputs of the Hausdorff distance, the average surface distance and surface Dice; `count` volumes of
+ * (sx, sy, sz) each, laid back to back as for edtb200_transform_stack.
+ *   surface S_v(k)  the voxels p of volume v with v[p] == k that have a face neighbour (2 ndim of them,
+ *                   never in the next volume of the stack) of another label or lie on a face of their
+ *                   volume: scipy's mask ^ binary_erosion(mask) with border_value 0
+ *   d_v,k(q)        the float32 distance from q to the nearest voxel of S_v(k): edtb200_transform with
+ *                   EDTB200_SQRT and no black_border of the 1-byte mask that is 0 on S_v(k) and 1
+ *                   elsewhere, bit for bit; +inf when S_v(k) is empty
+ *   segments        one per (volume, key, direction), numbered (volume * nkeys + key) * 2 + direction:
+ *                   direction 0 (A->B) holds d_b,k(q) for every q in S_a(k), direction 1 (B->A) holds
+ *                   d_a,k(q) for every q in S_b(k)
+ *   keys            HOST array of nkeys labels of `label_bytes` bytes, non-zero and strictly ascending
+ *                   as unsigned integers; read before the call returns
+ *   flags           EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE: every other buffer is on `device`
+ * Labels are compared as raw bits, as in the transforms.  Both calls are asynchronous on `stream`,
+ * take no lock and free what they allocate (stream-ordered) on every exit.  An empty volume, count 0
+ * or nkeys 0 returns 0 touching nothing.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, nkeys >= 0, the keys
+ * ("null pointer (keys)" when nkeys > 0; no key 0; strictly ascending), count * nkeys within 2^60,
+ * emptiness, pointers, residency (flags exactly the two residency flags), device. */
+
+/* counts: count * nkeys * 2 int64, the length of every segment (|S_a(k)| for A->B, |S_b(k)| for
+ * B->A), in segment order.  One pass over both volumes. */
+int edtb200_surface_count(const void *a, const void *b, int label_bytes, int ndim,
+                          int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                          const void *keys, int64_t nkeys, int flags, int64_t *counts,
+                          int device, void *stream);
+
+/* The distances of every segment.
+ *   wx, wy, wz    anisotropy, as for edtb200_transform
+ *   offsets       count * nkeys * 2 + 1 int64: the exclusive scan of edtb200_surface_count's counts,
+ *                 the total last; segment s is written to values[offsets[s] .. offsets[s + 1]) in
+ *                 unspecified order
+ *   values        offsets[last] float32
+ *   device_bytes  the budget of the call's device memory, 0 = the memory free on the device less
+ *                 EDTB200_CHUNK_RESERVE
+ *   groups        NULL, or int64_t[1] that receives the number of groups run (0 on an error or when
+ *                 there is nothing to do)
+ * The segments' slots go through the transform in groups: a group is a contiguous range of slots
+ * whose masks are one stack through the transform of edtb200_transform_stack (one launch per pass),
+ * one pass over the volumes writes the masks and one more gathers the distances.  A slot costs
+ * V (1 + 4 + s) bytes for V = sx*sy*sz, s as for edtb200_transform_stack (8 when a later pass takes
+ * the long-line kernel); a group holds at most floor(budget / slot) slots and at most 2^31 mask voxels
+ * (at least one slot), and the call runs the fewest such groups, their sizes differing by one at
+ * most (one group when every slot fits both); EDTB200_ENOMEM when not even one
+ * slot fits, and the message names that least budget.  Outside the budget: the keys and one int64
+ * cursor per segment. */
+int edtb200_surface_distances(const void *a, const void *b, int label_bytes, int ndim,
+                              int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                              float wx, float wy, float wz,
+                              const void *keys, int64_t nkeys, int flags,
+                              const int64_t *offsets, float *values,
+                              int device, size_t device_bytes, int64_t *groups, void *stream);
 
 /* The same transform of ONE host volume spread over several GPUs of this process
  * (`devices[0..ndevices)`, distinct ordinals): SURVEY.md section 8b's `devices[] / ndevices`.

@@ -102,6 +102,19 @@ for d, an in ((2.5, (1, 1, 1)), (7.9, (0.7, 1.3, 2.9)), (40.0, (1, 4, 1)), (24.0
   check("bounded sdf %g" % d, edt.sdf(blk, anisotropy=an, max_distance=d), banded(oracle.sdf(blk, anisotropy=an), sq, d))
   dist, _ = edt.feature_transform(blk, an, signed=True, return_distances=True, max_distance=d)
   check("bounded feature %g" % d, dist, banded(oracle.sdf(blk, anisotropy=an), sq, d))
+# surface distances: every kernel (mask, count, gather) on 1-D to 3-D volumes and a stack, keys in
+# shared memory, several groups, against the scipy restatement
+import surface_cases as sc  # noqa: E402
+for shape, an in (((33,), (2.0,)), ((14, 11), (1.0, 3.0)), ((9, 8, 10), (1.0, 2.0, 3.0))):
+  a, b = sc.random_pair(rng, shape, nlabels=4, dtype=np.uint16, flips=0.1)
+  keys = sc.default_keys(a, b)
+  sd = edt.surface_distances(a, b, an, max_device_bytes=3 * 5 * a.size)
+  for k, (ab, ba) in enumerate(sc.segments(a, b, keys, an)):
+    check("surface %dd key %d" % (len(shape), k), sd.values[sd.offsets[2 * k]:sd.offsets[2 * k + 2]],
+          np.concatenate([ab, ba]))
+a, b = sc.random_pair(rng, (3, 7, 9, 8), nlabels=5, dtype=np.int64, flips=0.1)
+check("surface stack", edt.hausdorff_distance(a, b, stacked=True),
+      np.stack([sc.metric(x, y, sc.default_keys(a, b), (1.0, 1.0, 1.0), sc.hausdorff) for x, y in zip(a, b)]))
 # per-label statistics and box-restricted extraction
 import torch  # noqa: E402
 lt = torch.from_numpy(np.ascontiguousarray(vor.astype(np.int32))).cuda()

@@ -36,6 +36,7 @@ __all__ = [
   "edt_cuda", "transform_batch", "each", "each_cuda", "label_stats_cuda", "device_count", "library_path", "EDTError",
   "feature_transform", "expand_labels",
   "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
+  "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
 ]
 
 FLAG_SQRT = 1
@@ -107,6 +108,9 @@ def _lib():
   lib.edtb200_feature_transform_bounded.restype = ci
   lib.edtb200_bounded_plan.argtypes = [ci, i64, i64, i64, f32, f32, f32, ctypes.c_double, vp, vp]
   lib.edtb200_bounded_plan.restype = ci
+  lib.edtb200_morphology.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ctypes.c_double, ci, ci, vp,
+                                     ci, vp]
+  lib.edtb200_morphology.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1195,6 +1199,132 @@ def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device
   if max_device_bytes is not None:
     _chunk_budget(max_device_bytes, True, None, on_device.dim())
   return _expand_device(on_device, distance, anisotropy, False)
+
+
+# ---------------------------------------------------------------------------------------
+# spherical morphology: erosion, dilation, opening and closing with a Euclidean ball, each a threshold
+# on a bounded transform whose last store writes labels (edtb200_morphology)
+# ---------------------------------------------------------------------------------------
+
+_ERODE, _DILATE, _OPEN, _CLOSE = 0, 1, 2, 3      # EDTB200_ERODE, _DILATE, _OPEN, _CLOSE
+
+
+def _morph_label_bytes(dtype):
+  """Label width of a numpy or torch dtype the morphology takes (None: not one)."""
+  if isinstance(dtype, np.dtype):
+    if dtype == np.bool_ or (dtype.kind in "iuf" and dtype.itemsize in (1, 2, 4, 8)):
+      return None if dtype.kind == "f" and dtype.itemsize < 4 else dtype.itemsize
+    return None
+  import torch
+  if dtype in (torch.float32, torch.float64):
+    return 4 if dtype == torch.float32 else 8
+  return _torch_label_bytes(torch).get(dtype)
+
+
+def _morphology(op, labels, radius, anisotropy, black_border, device, stacked, name):
+  """Every check before any device use, then one edtb200_morphology call: host arrays are staged whole
+  (numpy out), device arrays run on the current stream (torch out)."""
+  r = float(radius)
+  if not (r >= 0.0 and r != float("inf")):
+    raise ValueError("%s: radius must be finite and zero or more, got %r" % (name, radius))
+  on_device = _device_array(labels)
+  arr = None if on_device is not None else np.asarray(np.array(labels) if isinstance(labels, list) else labels)
+  nd = on_device.dim() if on_device is not None else arr.ndim
+  lo, hi = (2, 4) if stacked else (1, 3)
+  if not lo <= nd <= hi:
+    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
+  nbytes = _morph_label_bytes(on_device.dtype if on_device is not None else arr.dtype)
+  if nbytes is None:
+    raise TypeError("%s: unsupported label dtype %s" % (name, on_device.dtype if on_device is not None else arr.dtype))
+  vnd = nd - 1 if stacked else nd
+  weights = _surface_anisotropy(vnd, anisotropy)
+  mask_out = op in (_DILATE, _CLOSE)
+  border = int(bool(black_border))
+  lib = _lib()
+  if on_device is None:
+    arr, order = _stack_order(arr)
+    out = np.zeros(arr.shape, dtype=np.bool_ if mask_out else arr.dtype, order=order)
+    if arr.size == 0:
+      return out
+    if stacked:
+      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
+    else:
+      count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
+    flags = FLAG_LABELS_FLOAT if arr.dtype.kind == "f" else 0
+    _check(lib.edtb200_morphology(arr.ctypes.data, nbytes, vnd, sx, sy, sz, count, wx, wy, wz, op, r, border, flags,
+                                  out.ctypes.data, int(device), None))
+    return out
+  import torch
+  t = on_device
+  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
+  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
+    t = t.permute(*reversed(range(nd)))
+    weights = tuple(reversed(weights))
+  elif not t.is_contiguous():
+    t = t.contiguous()
+  out = torch.empty(t.shape, dtype=torch.bool if mask_out else t.dtype, device=t.device)
+  if t.numel():
+    count = int(t.shape[0]) if stacked else 1
+    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
+    flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE | (FLAG_LABELS_FLOAT if t.is_floating_point() else 0)
+    stream = torch.cuda.current_stream(t.device).cuda_stream
+    _check(lib.edtb200_morphology(t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, op, r, border, flags,
+                                  out.data_ptr(), t.device.index, ctypes.c_void_p(stream)))
+  return out.permute(*reversed(range(nd))) if fortran else out
+
+
+# Shared by the four functions below.  B is the ball {v in Z^n : sum_j (w_j v_j)^2 <= r^2}, w the
+# anisotropy (one entry per axis of a volume, as for edt()), r the radius in the same units.  "Within r"
+# compares the float32 squared distance that edtsq / sdfsq compute, in float64, with r * r -- the rule
+# of max_distance= and expand_labels -- so each result is a threshold on one bounded transform
+# (max_distance = r), whose last pass writes the labels directly.  Labels compare as edt() compares
+# them: floats by value, so -0.0 is background.  A kept voxel keeps its exact bits (NaN payloads
+# included); every other voxel is all-zero bits.  The result has the input's shape and memory order;
+# numpy in gives numpy out, a torch CUDA tensor (or any __cuda_array_interface__ array) gives a torch
+# CUDA tensor computed on the current stream without a host synchronisation.  `stacked=True` takes a 2-D
+# to 4-D array whose slowest axis in memory indexes same-shaped volumes, as edt(stacked=True) does: the
+# result equals np.stack of the per-volume calls, with one launch per pass for all of them; a host
+# stack is staged on the GPU whole.  A radius that is negative, NaN or infinite is a ValueError, an
+# unsupported dtype or number of dimensions a TypeError; a host array that does not fit on the GPU
+# raises EDTError with code ENOMEM (there is no chunked path).
+
+def spherical_erode(labels, radius, anisotropy=None, black_border=False, *, device=0, stacked=False):
+  """Multi-label erosion by the ball of `radius`: a voxel keeps its label iff it is labelled (non-zero)
+  and no voxel of another label (background included) lies within `radius`, i.e. its edtsq (with
+  `black_border`: the volume's faces count as background) is not within radius; every other voxel
+  becomes 0.  Per label k this is scipy.ndimage.binary_erosion(labels == k, B,
+  border_value=0 if black_border else 1).  Radius 0 is the identity, and so is any radius for a volume
+  of one label without black_border (it has no site at all).  Returns the input's dtype."""
+  return _morphology(_ERODE, labels, radius, anisotropy, black_border, device, stacked, "spherical_erode")
+
+
+def spherical_open(labels, radius, anisotropy=None, black_border=False, *, device=0, stacked=False):
+  """Multi-label opening by the ball of `radius`: with E the spherical_erode result (with
+  `black_border`), a voxel keeps its label iff it is labelled and the squared distance from it to the
+  nearest voxel of E is within radius (that transform has no black border: no kept voxel lies outside
+  the volume); every other voxel becomes 0.  Per label k this is
+  scipy.ndimage.binary_dilation(eroded_k, B, border_value=0) -- not scipy's binary_opening with
+  border_value=1, which dilates from outside the volume too.  Every label opens at once, without a
+  loop over labels: the voxel q of E nearest p, if within radius, carries p's label, because the ball
+  around q lies inside q's own label and contains p.  Both transforms run back to back on the GPU.
+  Returns the input's dtype."""
+  return _morphology(_OPEN, labels, radius, anisotropy, black_border, device, stacked, "spherical_open")
+
+
+def spherical_dilate(labels, radius, anisotropy=None, *, device=0, stacked=False):
+  """Binary dilation by the ball of `radius`: every non-zero voxel is foreground, and a voxel is set iff
+  it is foreground or |sdfsq(labels)| there (the squared distance to the nearest foreground voxel) is
+  within radius.  Equals scipy.ndimage.binary_dilation(labels != 0, B, border_value=0).  Returns a bool
+  mask.  For a dilation that keeps the labels, see expand_labels."""
+  return _morphology(_DILATE, labels, radius, anisotropy, False, device, stacked, "spherical_dilate")
+
+
+def spherical_close(labels, radius, anisotropy=None, black_border=False, *, device=0, stacked=False):
+  """Binary closing by the ball of `radius`: D = spherical_dilate(labels, radius), then D eroded as a
+  two-label volume (with `black_border`: the faces count as background).  Equals
+  scipy.ndimage.binary_erosion(D, B, border_value=0 if black_border else 1).  Both transforms run back to
+  back on the GPU.  Returns a bool mask."""
+  return _morphology(_CLOSE, labels, radius, anisotropy, black_border, device, stacked, "spherical_close")
 
 
 # ---------------------------------------------------------------------------------------

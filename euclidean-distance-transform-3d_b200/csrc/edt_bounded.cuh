@@ -34,13 +34,16 @@ inline size_t window_smem_bytes(int radius, int label_bytes) {
 // far.  A value above `bound` is written as +inf.  Sites: the codes later_axis_long_kernel writes
 // (the winning row, site_direct for a border term, kSiteNone for +inf), so the resolver is shared.
 // Epi: flags' sqrt / sign in the store (the last pass).
+// The walk is window_tiles below; the kernels differ in their store only: later_axis_window_kernel
+// writes the distance (and site code), later_axis_window_select_kernel the morphology's label or mask.
 // ---------------------------------------------------------------------------------------
-template <int Bytes, bool Sites, bool Epi>
-__global__ void __launch_bounds__(kWindowWarps * 32)
-later_axis_window_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, const float* __restrict__ fin,
-                         float* __restrict__ fout, int* __restrict__ codes, LineGeom g, float w2, int radius,
-                         int border_lo, int border_hi, int flags, int dbl_from, float bound, int64_t row_tiles,
-                         int64_t tiles) {
+// store(at, best, site, label): row `at` of the pass has the value `best` (+inf above bound), won by
+// `site`, and the label `label`.
+template <int Bytes, class Store>
+__device__ __forceinline__ void window_tiles(const typename LabelOf<Bytes>::type* __restrict__ labels,
+                                             const float* __restrict__ fin, const LineGeom& g, float w2, int radius,
+                                             int border_lo, int border_hi, int dbl_from, float bound,
+                                             int64_t row_tiles, int64_t tiles, Store&& store) {
   using LT = typename LabelOf<Bytes>::type;
   extern __shared__ __align__(16) unsigned char window_smem[];
   const int span = kWindowRows + 2 * radius;
@@ -102,12 +105,25 @@ later_axis_window_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
         }
       }
       if (!(best <= bound)) best = inf;
-      const int64_t at = base + (int64_t)i * stride;
-      if constexpr (Sites) codes[at] = best < inf ? site : kSiteNone;
-      if constexpr (Epi) best = finish_value(best, mine == 0, flags);
-      fout[at] = best;
+      store(base + (int64_t)i * stride, best, site, mine);
     }
   }
+}
+
+template <int Bytes, bool Sites, bool Epi>
+__global__ void __launch_bounds__(kWindowWarps * 32)
+later_axis_window_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, const float* __restrict__ fin,
+                         float* __restrict__ fout, int* __restrict__ codes, LineGeom g, float w2, int radius,
+                         int border_lo, int border_hi, int flags, int dbl_from, float bound, int64_t row_tiles,
+                         int64_t tiles) {
+  using LT = typename LabelOf<Bytes>::type;
+  const float inf = __int_as_float(0x7f800000);
+  window_tiles<Bytes>(labels, fin, g, w2, radius, border_lo, border_hi, dbl_from, bound, row_tiles, tiles,
+                      [&](int64_t at, float best, int site, LT mine) {
+                        if constexpr (Sites) codes[at] = best < inf ? site : kSiteNone;
+                        if constexpr (Epi) best = finish_value(best, mine == 0, flags);
+                        fout[at] = best;
+                      });
 }
 
 // The cut of a pass that did not take the window kernel (or of a 1-D transform's X pass): in place

@@ -846,14 +846,17 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
 // then each later pass in the window kernel where bp says so (out of place) and in launch_later
 // otherwise (in place, without its sqrt / sign), then -- unless the last pass was a window pass,
 // which cuts in its store -- the cut.  The X pass writes f or one scratch volume, whichever makes the
-// last window pass land in f.
+// last window pass that writes distances land in f.  `count` volumes of (sx, sy, sz) laid end to end
+// are transformed each on its own, as run_passes does.  sel: a morphology step (edt_morphology.cuh),
+// whose last store writes sel's labels or mask instead of distances -- in the last pass where it takes
+// the window kernel, else in the select that replaces the cut (f then holds scratch distances).
 int run_bounded_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                        float wx, float wy, float wz, int border, int flags, float* f, const BoundedPlan& bp,
-                       DeviceCache& dc, cudaStream_t s) {
+                       DeviceCache& dc, cudaStream_t s, int64_t count = 1, const edtb200::MorphSelect* sel = nullptr) {
   const Transform t{label_bytes, ndim, flags, border, {wx, wy, wz}, {sx, sy, sz}};
-  const int64_t total = sx * sy * sz;
-  int windows = 0;
-  for (int k = 1; k < ndim; ++k) windows += bp.windowed[k] ? 1 : 0;
+  const int64_t total = sx * sy * sz * count;
+  int windows = 0;                                // window passes that write distances
+  for (int k = 1; k < ndim; ++k) windows += bp.windowed[k] && !(sel && k == ndim - 1) ? 1 : 0;
   Scratch other;
   if (windows && other.alloc(dc, sizeof(float) * (size_t)total, s) != cudaSuccess) {
     cudaGetLastError();
@@ -861,12 +864,15 @@ int run_bounded_passes(const void* labels, int label_bytes, int ndim, int64_t sx
   }
   float* buf[2] = {f, other.get<float>()};
   int cur = windows % 2;
-  int rc = dispatch_first(label_bytes, labels, buf[cur], sy * sz, sx, wx, border, kernel_flags(flags, true, false),
-                          dc, s);
+  int rc = dispatch_first(label_bytes, labels, buf[cur], sy * sz * count, sx, wx, border,
+                          kernel_flags(flags, true, false), dc, s);
   for (int k = 1; !rc && k < ndim; ++k) {
-    const edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz);
+    const edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz, count);
     const PassArith arith = transform_arith(t.w, t.n, k);
-    if (bp.windowed[k]) {
+    if (bp.windowed[k] && sel && k == ndim - 1) {
+      rc = launch_window_select(labels, label_bytes, buf[cur], g, t.w[k], (int)bp.radius[k], border, border, arith,
+                                bp.bound, *sel, dc, s);
+    } else if (bp.windowed[k]) {
       rc = with_label_width(label_bytes, [&](auto b) {
         return launch_later_window<b>(labels, buf[cur], buf[cur ^ 1], nullptr, g, t.w[k], (int)bp.radius[k], border,
                                       border, kernel_flags(flags, false, k == ndim - 1), arith, bp.bound, dc, s);
@@ -877,6 +883,7 @@ int run_bounded_passes(const void* labels, int label_bytes, int ndim, int64_t sx
     }
   }
   if (rc || (ndim >= 2 && bp.windowed[ndim - 1])) return rc;
+  if (sel) return launch_morph_select(f, total, bp.bound, *sel, dc, s);
   return with_label_width(label_bytes, [&](auto b) {
     return launch_bounded_cut<b>(labels, f, nullptr, total, bp.bound, kernel_flags(flags, false, true), dc, s);
   });
@@ -1681,6 +1688,86 @@ int edtb200_bounded_plan(int ndim, int64_t sx, int64_t sy, int64_t sz, float wx,
     windowed[k] = k < ndim ? (bp.windowed[k] ? 1 : 0) | (sp.windowed[k] ? 2 : 0) : 0;
   }
   return 0;
+}
+
+int edtb200_morphology(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                       int64_t count, float wx, float wy, float wz, int op, double radius, int black_border, int flags,
+                       void* out, int device, void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (op < EDTB200_ERODE || op > EDTB200_CLOSE) return fail(EDTB200_EINVAL, "op must be EDTB200_ERODE, _DILATE, _OPEN or _CLOSE (got %d)", op);
+  if (!(radius >= 0.0) || std::isinf(radius))
+    return fail(EDTB200_EINVAL, "radius must be finite and zero or more (got %g)", radius);
+  const int known = EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE | EDTB200_LABELS_FLOAT;
+  if (flags & ~known)
+    return fail(EDTB200_EINVAL, "edtb200_morphology takes only the residency flags and EDTB200_LABELS_FLOAT (got %d)",
+                flags);
+  const bool as_float = flags & EDTB200_LABELS_FLOAT;
+  if (as_float && label_bytes != 4 && label_bytes != 8)
+    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
+  const int64_t vol = sx * sy * sz;
+  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const float w[3] = {wx, wy, wz};
+  const BoundedPlan bp = bounded_plan(ndim, w, radius, /*sites=*/false);
+  const bool mask_out = op == EDTB200_DILATE || op == EDTB200_CLOSE;
+  const int border = black_border != 0;
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  // host buffers are staged through this device's cached buffers, as edtb200_transform_bounded stages them
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
+  const size_t out_bytes = (size_t)total * (mask_out ? 1 : (size_t)label_bytes);
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
+  void* d_out = io.out(out, out_bytes, static_cast<void*>(dc->dist));
+  // scratch: the distances, the first step's mask (opening, closing) and the folded float labels
+  const bool two = op == EDTB200_OPEN || op == EDTB200_CLOSE;
+  Scratch dist, mask, folded;
+  if (dist.alloc(*dc, sizeof(float) * (size_t)total, s) != cudaSuccess ||
+      (two && mask.alloc(*dc, (size_t)total, s) != cudaSuccess) ||
+      (as_float && folded.alloc(*dc, lab_bytes, s) != cudaSuccess)) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the morphology's scratch");
+  }
+  const void* runs = d_labels;                   // the labels the transforms compare
+  if (as_float) {
+    if ((rc = launch_fold_float_labels(d_labels, label_bytes, folded.get(), total, *dc, s))) return rc;
+    runs = folded.get();
+  }
+  // select tables, bit (2 nz + near): erode keeps nz & !near (4), dilate sets nz | near (2, 4, 8), open's
+  // mask is 0 on the erosion E and 1 elsewhere (the complement of 4), open keeps nz & near (8)
+  constexpr int kErode = 0x4, kDilate = 0xE, kNotEroded = 0xB, kNear = 0x8;
+  auto step = [&](const void* lab, int lab_w, int bord, int fl, const edtb200::MorphSelect& sel) {
+    return run_bounded_passes(lab, lab_w, ndim, sx, sy, sz, wx, wy, wz, bord, fl, dist.get<float>(), bp, *dc, s,
+                              count, &sel);
+  };
+  uint8_t* m = mask.get<uint8_t>();
+  switch (op) {
+    case EDTB200_ERODE:
+      rc = step(runs, label_bytes, border, 0, {d_labels, d_out, label_bytes, kErode, false, as_float});
+      break;
+    case EDTB200_DILATE:
+      rc = step(runs, label_bytes, 0, EDTB200_SIGNED, {d_labels, d_out, label_bytes, kDilate, true, as_float});
+      break;
+    case EDTB200_OPEN:        // the erosion E as a mask, then d^2(p, E) = edtsq of that mask
+      rc = step(runs, label_bytes, border, 0, {d_labels, m, label_bytes, kNotEroded, true, as_float});
+      if (!rc) rc = step(m, 1, 0, 0, {d_labels, d_out, label_bytes, kNear, false, as_float});
+      break;
+    default:                  // EDTB200_CLOSE: the dilation D as a mask, then D eroded as a two-label volume
+      rc = step(runs, label_bytes, 0, EDTB200_SIGNED, {d_labels, m, label_bytes, kDilate, true, as_float});
+      if (!rc) rc = step(m, 1, border, 0, {m, d_out, 1, kErode, true, false});
+      break;
+  }
+  return rc ? rc : io.finish();
 }
 
 int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,

@@ -1,10 +1,11 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as eight translation units so that the kernel templates build in
+// The library is compiled as nine translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
-// transforms' kernels) and edt_surface.cu (the surface distances' kernels).  The run-time label width
+// transforms' kernels), edt_surface.cu (the surface distances' kernels) and edt_morphology.cu (the
+// spherical morphology's label-writing stores).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -261,7 +262,31 @@ struct SurfaceSlots {
   int64_t s0, s1, v0, v1;
 };
 
+// The last store of a spherical morphology step (edt_morphology.cuh): at voxel p, with nz = src[p] is
+// non-zero and near = p's squared distance is within the bound, bit (2 nz + near) of `table` says
+// whether p is kept (mask_out: out[p] = 1, else out[p] = src[p]) or not (out[p] = 0).
+struct MorphSelect {
+  const void* src;     // the caller's labels, src_bytes each, raw bits
+  void* out;           // 1 byte per voxel (mask_out) or src_bytes
+  int src_bytes;
+  int table;
+  bool mask_out;
+  bool as_float;       // 4- / 8-byte IEEE labels: -0.0 is zero
+};
+
 namespace host {
+
+// The morphology's kernels (edt_morphology.cu).  launch_window_select: the last later pass along g as
+// launch_later_window, with the select in its store (label_bytes: the transform's labels, 1 or
+// sel.src_bytes).  launch_morph_select: the select over `total` values f.  launch_fold_float_labels:
+// out = in with -0.0 as +0.0, for 4- / 8-byte float labels.
+int launch_window_select(const void* labels, int label_bytes, const float* fin, const LineGeom& g, float w,
+                         int radius, int border_lo, int border_hi, PassArith arith, float bound,
+                         const MorphSelect& sel, DeviceCache& dc, cudaStream_t stream);
+int launch_morph_select(const float* f, int64_t total, float bound, const MorphSelect& sel, DeviceCache& dc,
+                        cudaStream_t stream);
+int launch_fold_float_labels(const void* in, int label_bytes, void* out, int64_t total, DeviceCache& dc,
+                             cudaStream_t stream);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

@@ -36,7 +36,7 @@ extern "C" {
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
- * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances)
+ * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -190,6 +190,53 @@ int edtb200_feature_transform_bounded(const void *labels, int label_bytes, int n
 int edtb200_bounded_plan(int ndim, int64_t sx, int64_t sy, int64_t sz,
                          float wx, float wy, float wz, double max_distance,
                          int64_t radius[3], int windowed[3]);
+
+/* Spherical morphology of label volumes: erosion, dilation, opening and closing with the Euclidean
+ * ball B = {v : sum_j (w_j v_j)^2 <= radius^2}, each a threshold on a bounded transform with
+ * max_distance = radius.  "Within" is (double)d2 <= (double)radius * radius on the float32 squared
+ * distance d2 as edtb200_transform computes it (+inf where there is no site): the rule of the bounded
+ * transforms' cut and of expand_labels.  L is the labels, 0 background.
+ *   EDTB200_ERODE  multi-label: p keeps L(p) iff L(p) != 0 and its edtsq (with black_border) is not
+ *                  within radius; else 0.  Per label k: scipy binary_erosion(L == k, B,
+ *                  border_value = black_border ? 0 : 1).
+ *   EDTB200_OPEN   multi-label: with E the erosion above, p keeps L(p) iff L(p) != 0 and d2(p, E != 0)
+ *                  is within radius, that transform without black_border; else 0.  Per label k:
+ *                  binary_dilation(eroded_k, B, border_value = 0).  One transform of E opens every
+ *                  label at once: the ball around E's voxel nearest p lies in that voxel's own label.
+ *   EDTB200_DILATE binary: out[p] = 1 iff L(p) != 0 or |sdfsq(L)|(p) is within radius (no
+ *                  black_border; black_border is ignored); binary_dilation(L != 0, B, border_value = 0).
+ *   EDTB200_CLOSE  binary: D = the dilation above, then out[p] = 1 iff D(p) and the edtsq of D as a
+ *                  two-label volume (with black_border) is not within radius: binary_erosion(D, B,
+ *                  border_value = black_border ? 0 : 1).
+ * radius 0 is the identity for erosion and opening; a voxel with no site at all (one label, no
+ * black_border) is never within any radius.
+ *
+ *   labels   count * sx*sy*sz labels of label_bytes (1, 2, 4 or 8) bytes, volumes back to back as for
+ *            edtb200_transform_stack (count 1: one volume), each transformed on its own
+ *   flags    the residency flags, and EDTB200_LABELS_FLOAT for 4- / 8-byte IEEE labels: -0.0 is then
+ *            background and compares equal to +0.0; every other value compares by its bits
+ *   out      erode / open: count * sx*sy*sz labels of label_bytes, a kept voxel's bits copied exactly
+ *            and every other voxel all-zero bits; dilate / close: count * sx*sy*sz bytes, 0 or 1.
+ *            It must not overlap labels.
+ * Residency, staging and asynchrony as edtb200_transform_bounded: host buffers are staged whole (there
+ * is no chunked path; EDTB200_ENOMEM when they do not fit).  Each transform is the bounded transform's
+ * passes with one launch per pass for the whole stack; the last store writes the labels or mask -- in
+ * the window kernel where the last pass takes it (EDTB200_BOUNDED_WINDOW_MAX), else in one select kernel
+ * after it.  Opening and closing run their two transforms back to back on one stream, the first writing
+ * a 1-byte mask that the second transforms.  Device memory beyond the labels and out: 4 bytes per voxel
+ * of distances, 4 more when a pass other than the last takes the window kernel, 1 for the mask of
+ * opening and closing, and label_bytes for the folded labels with EDTB200_LABELS_FLOAT.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, op, radius (finite,
+ * >= 0), flags, EDTB200_LABELS_FLOAT width, the stack's size (within 2^62 voxels), emptiness (returns 0
+ * touching nothing), pointers, device. */
+#define EDTB200_ERODE  0
+#define EDTB200_DILATE 1
+#define EDTB200_OPEN   2
+#define EDTB200_CLOSE  3
+int edtb200_morphology(const void *labels, int label_bytes, int ndim,
+                       int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                       float wx, float wy, float wz, int op, double radius,
+                       int black_border, int flags, void *out, int device, void *stream);
 
 /* A stack of `count` volumes of one geometry (sx, sy, sz), laid back to back (volume b starts at
  * voxel b * sx * sy * sz), each transformed on its own as edtb200_transform would: its result is

@@ -115,6 +115,21 @@ for shape, an in (((33,), (2.0,)), ((14, 11), (1.0, 3.0)), ((9, 8, 10), (1.0, 2.
 a, b = sc.random_pair(rng, (3, 7, 9, 8), nlabels=5, dtype=np.int64, flips=0.1)
 check("surface stack", edt.hausdorff_distance(a, b, stacked=True),
       np.stack([sc.metric(x, y, sc.default_keys(a, b), (1.0, 1.0, 1.0), sc.hausdorff) for x, y in zip(a, b)]))
+# spherical morphology: the label- and mask-writing window store (every (runs, labels) width pair), the
+# select after an unbounded last pass, the float fold, the two-stage calls and a stack, against the
+# threshold restatement on the oracle
+import morphology_cases as mc  # noqa: E402
+for dtype in (np.uint8, np.uint16, np.uint32, np.uint64, np.float32):
+  lab = np.asfortranarray(cases.random_volume(rng, (21, 19, 17), "blocks", dtype))
+  for op in mc.OPS:
+    for r in (2.0, 4.5):
+      fn = getattr(edt, "spherical_" + op)
+      got = fn(lab, r) if op == "dilate" else fn(lab, r, None, True)
+      check("morphology %s %s r=%g" % (op, np.dtype(dtype).name, r), mc._raw(got),
+            mc._raw(mc.threshold(op, lab, r, None, op != "dilate")))
+vols = np.stack([cases.random_volume(rng, (12, 14, 9), "blocks", np.uint16) for _ in range(3)])
+check("morphology stack", edt.spherical_open(vols, 2.0, stacked=True),
+      np.stack([mc.threshold("open", v, 2.0) for v in vols]))
 # per-label statistics and box-restricted extraction
 import torch  # noqa: E402
 lt = torch.from_numpy(np.ascontiguousarray(vor.astype(np.int32))).cuda()

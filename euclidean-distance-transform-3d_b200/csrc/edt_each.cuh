@@ -89,10 +89,10 @@ label_stats_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels, con
     if (!fg) continue;
     if (key == 0ull) continue;                       // background lanes drop out; `fg` names the rest
     const unsigned same = __match_any_sync(fg, key);
-    const int64_t plane = (int64_t)sx * sy;
+    const int64_t plane = (int64_t)sx * sy;              // may exceed 2^31 (only each axis fits an int)
     const int z = (int)(idx / plane);
-    const int rem = (int)(idx - (int64_t)z * plane);
-    const int y = rem / sx, x = rem - y * sx;
+    const int64_t rem = idx - (int64_t)z * plane;
+    const int y = (int)(rem / sx), x = (int)(rem - (int64_t)y * sx);
     const unsigned int bits = ordered_bits(d);
     const unsigned int mx = __reduce_max_sync(same, bits);
     const int x0 = __reduce_min_sync(same, x), x1 = __reduce_max_sync(same, x);

@@ -669,7 +669,13 @@ int edtb200_slab_step(const void *labels_dev, int label_bytes, int64_t sx, int64
  *     (0 = empty slot; label 0 is background and skipped), count_dev[s] = its voxels,
  *     max_dev[s] = its largest distance, argmax_dev[s] = the smallest linear index (x fastest)
  *     where that maximum is attained, box_dev[6*s..] = bounding box x0 y0 z0 x1 y1 z1 (inclusive).
- *     *overflow_dev is raised when the table was too small (repeat with a larger capacity).
+ *     A label's key is its raw bits zero-extended to 64 bits (signed labels are never sign-extended);
+ *     distances may be negative or infinite (not NaN).  Only each axis has to fit an int: a plane
+ *     sx * sy of more than 2^31 voxels is supported.
+ *     *overflow_dev is raised when the table was too small (repeat with a larger capacity).  While it
+ *     is 0 the table is complete, even with every slot filled; once it is 1 the call still returns
+ *     0 and the only guarantee is that every filled slot holds a label of the volume, each label at
+ *     most once -- its statistics may be partial and other labels are missing.
  * edtb200_label_extract : out = (labels == key) ? dt : 0 inside `box` (6 host ints as above, NULL =
  *     whole volume), nothing outside it is touched -- the equivalent of transfer_run_voxels on a
  *     blank image; erase != 0 zeroes the box instead (the reference's erase()).

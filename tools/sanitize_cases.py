@@ -130,13 +130,20 @@ for dtype in (np.uint8, np.uint16, np.uint32, np.uint64, np.float32):
 vols = np.stack([cases.random_volume(rng, (12, 14, 9), "blocks", np.uint16) for _ in range(3)])
 check("morphology stack", edt.spherical_open(vols, 2.0, stacked=True),
       np.stack([mc.threshold("open", v, 2.0) for v in vols]))
-# per-label statistics and box-restricted extraction
-import torch  # noqa: E402
-lt = torch.from_numpy(np.ascontiguousarray(vor.astype(np.int32))).cuda()
-dt = edt.edt_cuda(lt, (1.0, 1.0, 1.0), False, sqrt=True)
-st = edt.label_stats_cuda(lt, dt)
-assert int(st["count"].sum().item()) == lt.numel()
-for key, img in edt.each_cuda(lt, dt, in_place=True):
-  assert torch.equal(img, torch.where(lt == key, dt, torch.zeros((), device=dt.device)))
-done += 1
+# per-label views: a nearly full table whose probe chain wraps past its end, a table that overflows, and
+# a sub-box drawn at a ragged row length; the helpers are the GPU tests' own
+import each_cases as ec  # noqa: E402
+import test_each_gpu as teg  # noqa: E402
+keys = np.union1d(ec.colliding_keys(64, 128, 127, 4), ec.random_keys(60, 4, 1))
+lab = ec.noise((6, 20, 37), keys, 2, np.int32)
+teg.check_table(edt, lab, ec.distances(lab, "signed", 3), 128)
+lab = ec.singletons((3, 5, 43), ec.random_keys(700, 8, 4, signed=True), 5, np.int64, background=0.2)
+rc, overflow, table = teg.c_stats(edt, lab, ec.distances(lab, "inf", 6), 64)
+assert rc == 0 and overflow == 1 and np.isin(table["keys"][table["keys"] != 0], ec.keys_of(lab)).all()
+lab = ec.voronoi_many((5, 7, 75), 6, 7, np.uint16)
+dist = ec.distances(lab, "ties", 8)
+out = teg.device_bytes(np.zeros(lab.shape, np.float32))
+key, box = int(ec.keys_of(lab).max()), (2, 1, 1, 68, 5, 3)
+assert teg.c_extract(edt, teg.device_bytes(lab), 2, teg.device_bytes(dist), ec.dims_of(lab.shape), key, box, 0, out) == 0
+check("each sub-box", out.cpu().numpy().view(np.float32).reshape(lab.shape), ec.extract(lab, dist, key, box))
 print("sanitize_cases: %d results equal to the oracle" % done)

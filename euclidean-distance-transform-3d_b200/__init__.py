@@ -37,6 +37,7 @@ __all__ = [
   "feature_transform", "expand_labels",
   "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
+  "parabolic_erode", "parabolic_dilate",
 ]
 
 FLAG_SQRT = 1
@@ -111,6 +112,8 @@ def _lib():
   lib.edtb200_morphology.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ctypes.c_double, ci, ci, vp,
                                      ci, vp]
   lib.edtb200_morphology.restype = ci
+  lib.edtb200_parabolic.argtypes = [vp, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp]
+  lib.edtb200_parabolic.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1325,6 +1328,114 @@ def spherical_close(labels, radius, anisotropy=None, black_border=False, *, devi
   scipy.ndimage.binary_erosion(D, B, border_value=0 if black_border else 1).  Both transforms run back to
   back on the GPU.  Returns a bool mask."""
   return _morphology(_CLOSE, labels, radius, anisotropy, black_border, device, stacked, "spherical_close")
+
+
+# ---------------------------------------------------------------------------------------
+# parabolic erosion and dilation of float volumes: the distance transform of a sampled function
+# (edtb200_parabolic)
+# ---------------------------------------------------------------------------------------
+
+_PARABOLIC_ERODE, _PARABOLIC_DILATE = 0, 1      # EDTB200_PARABOLIC_ERODE, _DILATE
+
+
+def _parabolic(op, f, anisotropy, device, stacked, name):
+  """Every check before any device use, then one edtb200_parabolic call: host arrays are staged whole
+  (numpy out), device arrays run on the current stream (torch out)."""
+  on_device = _device_array(f)
+  arr = None if on_device is not None else np.asarray(f)
+  nd = on_device.dim() if on_device is not None else arr.ndim
+  lo, hi = (2, 4) if stacked else (1, 3)
+  if not lo <= nd <= hi:
+    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
+  if on_device is not None:
+    if on_device.is_complex():
+      raise TypeError("%s: it takes real or bool samples, got %s" % (name, on_device.dtype))
+  elif arr.dtype != np.bool_ and arr.dtype.kind not in "iuf":
+    raise TypeError("%s: it takes real or bool samples, got %s" % (name, arr.dtype))
+  vnd = nd - 1 if stacked else nd
+  weights = _surface_anisotropy(vnd, anisotropy)
+  for w in weights:
+    if not (np.isfinite(w) and w > 0.0):
+      raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (name, anisotropy))
+  lib = _lib()
+  if on_device is None:
+    arr, order = _stack_order(arr)
+    arr = arr.astype(np.float32, order="K", copy=False)
+    out = np.empty(arr.shape, dtype=np.float32, order=order)
+    if arr.size == 0:
+      return out
+    if stacked:
+      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
+    else:
+      count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
+    _check(lib.edtb200_parabolic(arr.ctypes.data, vnd, sx, sy, sz, count, wx, wy, wz, op, 0, out.ctypes.data,
+                                 int(device), None))
+    return out
+  import torch
+  t = on_device
+  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
+  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
+    t = t.permute(*reversed(range(nd)))
+    weights = tuple(reversed(weights))
+  t = t.to(torch.float32).contiguous()
+  out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
+  if t.numel():
+    count = int(t.shape[0]) if stacked else 1
+    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
+    stream = torch.cuda.current_stream(t.device).cuda_stream
+    _check(lib.edtb200_parabolic(t.data_ptr(), vnd, sx, sy, sz, count, wx, wy, wz, op,
+                                 FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, out.data_ptr(), t.device.index,
+                                 ctypes.c_void_p(stream)))
+  return out.permute(*reversed(range(nd))) if fortran else out
+
+
+_PARABOLIC_DOC = """
+
+  Definition.  Volumes are x-fastest: for C-ordered input the last axis is x, as for edt().  Erosion
+  starts from g = f as float32 and runs one pass per axis in the order x, y, z; each pass replaces every
+  sample g(i) of a line by
+
+      min( g(i), min_{j != i} fl32(fl64(fl64(w2 * (i-j)^2) + g(j))) ),   w2 = float32(w * w)
+
+  -- w2 rounded in float32, the sum formed in float64 and rounded once to float32, which is what numpy
+  gives in float64 followed by .astype(np.float32).  Lines never leave the volume and there are no
+  border terms.  A NaN sample is never a site (read as +inf for erosion, -inf for dilation), every zero
+  result is +0.0, a weight whose square overflows float32 leaves its pass's samples as they are, and
+  (with a finite w2) one -inf sample makes its whole line -inf.  Dilation is -parabolic_erode(-f) with
+  the same rules.  The result equals this definition bit for bit.
+
+  Input and output.  Samples of any real dtype or bool are converted to float32 first (float64 rounds
+  to float32 first).  The result is float32 with the input's shape and memory order; numpy in gives
+  numpy out, a torch CUDA tensor (or any __cuda_array_interface__ array) gives a torch CUDA tensor
+  computed on the current stream without a host synchronisation.  `stacked=True` takes a 2-D to 4-D
+  array whose slowest axis in memory indexes same-shaped volumes, as edt(stacked=True) does: np.stack
+  of the per-volume calls, one launch per pass for all of them.  A weight that is not finite and > 0 is
+  a ValueError, a wrong number of dimensions or a non-real dtype a TypeError; a host array that does not
+  fit on the GPU raises EDTError with code ENOMEM (there is no chunked path).
+
+  Worked uses.
+    edtsq of a mask, with integer weights w:
+        parabolic_erode(np.where(mask, np.inf, 0), w) == edtsq(mask, w)          (bit for bit)
+    the reverse distance transform -- the union of the balls of radius r at the medial points:
+        parabolic_dilate(np.where(medial, r * r, -np.inf)) > 0
+    ITK's ParabolicErode / DilateImageFilter at scale t with voxel spacing s:
+        anisotropy = s / sqrt(2 t)
+  """
+
+
+def parabolic_erode(f, anisotropy=None, *, device=0, stacked=False):
+  return _parabolic(_PARABOLIC_ERODE, f, anisotropy, device, stacked, "parabolic_erode")
+
+
+def parabolic_dilate(f, anisotropy=None, *, device=0, stacked=False):
+  return _parabolic(_PARABOLIC_DILATE, f, anisotropy, device, stacked, "parabolic_dilate")
+
+
+parabolic_erode.__doc__ = """Parabolic (grayscale) erosion: g(p) = min_q f(q) + sum_a (w_a (p_a - q_a))^2, computed as
+  one exact lower envelope of parabolas per axis -- the distance transform of the sampled function f
+  (Felzenszwalb-Huttenlocher).  Its cost per voxel does not depend on the weights.""" + _PARABOLIC_DOC
+parabolic_dilate.__doc__ = """Parabolic (grayscale) dilation: g(p) = max_q f(q) - sum_a (w_a (p_a - q_a))^2, computed as
+  -parabolic_erode(-f); NaN is never a site and zero results are +0.0.""" + _PARABOLIC_DOC
 
 
 # ---------------------------------------------------------------------------------------

@@ -1770,6 +1770,74 @@ int edtb200_morphology(const void* labels, int label_bytes, int ndim, int64_t sx
   return rc ? rc : io.finish();
 }
 
+int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx,
+                      float wy, float wz, int op, int flags, float* out, int device, void* stream_v) {
+  int rc = check_dims(4, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (op != EDTB200_PARABOLIC_ERODE && op != EDTB200_PARABOLIC_DILATE)
+    return fail(EDTB200_EINVAL, "op must be EDTB200_PARABOLIC_ERODE or _DILATE (got %d)", op);
+  const float w[3] = {wx, wy, wz};
+  for (int k = 0; k < ndim; ++k)
+    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
+      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_parabolic takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!f || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t bytes = sizeof(float) * (size_t)total;
+  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
+  if (same_side && f != out && (const char*)f < (const char*)out + bytes && (const char*)out < (const char*)f + bytes)
+    return fail(EDTB200_EINVAL, "out overlaps f without being f");
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, bytes));
+  const float* d_f = nullptr;
+  if ((rc = io.in(f, bytes, dc->labels, &d_f))) return rc;
+  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, bytes));
+  float* d_out = io.out(out, bytes, dc->dist);
+  // EDT_B200_VERBOSE=1: per-pass device times and kernels on stderr (synchronises the stream)
+  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
+  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  if (verbose)
+    for (int k = 0; k <= ndim; ++k)
+      if (cudaEventCreate(&ev[k]) == cudaSuccess) cudaEventRecord(ev[k], s);
+  int kernel[3] = {-1, -1, -1};
+  const float* src = d_f;                      // the first pass out of place, the others in place
+  for (int k = 0; !rc && k < ndim; ++k) {
+    edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz, count);
+    if (k == 0) {                              // rows of sx contiguous samples
+      g.outer_count = sy * sz * count; g.outer_stride = sx; g.inner_count = 1; g.line_stride = 1; g.n = (int)sx;
+    }
+    rc = launch_parabolic_pass(src, d_out, g, k == 0, w[k], op == EDTB200_PARABOLIC_DILATE, *dc, s, &kernel[k]);
+    if (ev[k + 1]) cudaEventRecord(ev[k + 1], s);
+    src = d_out;
+  }
+  if (verbose) {
+    static const char* names[4] = {"tile", "long", "brute", "copy"};
+    float ms[3] = {0.0f, 0.0f, 0.0f};
+    if (!rc && cudaEventSynchronize(ev[ndim]) == cudaSuccess) {
+      for (int k = 0; k < ndim; ++k)
+        if (ev[k] && ev[k + 1]) cudaEventElapsedTime(&ms[k], ev[k], ev[k + 1]);
+      fprintf(stderr, "[edt_b200] parabolic %s %lldx%lldx%lld x%lld  x %.3f ms (%s)  y %.3f ms (%s)  z %.3f ms (%s)\n",
+              op == EDTB200_PARABOLIC_DILATE ? "dilate" : "erode", (long long)sx, (long long)sy, (long long)sz,
+              (long long)count, ms[0], names[kernel[0] < 0 ? 0 : kernel[0]], ms[1],
+              kernel[1] < 0 ? "-" : names[kernel[1]], ms[2], kernel[2] < 0 ? "-" : names[kernel[2]]);
+    }
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+    cudaGetLastError();
+  }
+  return rc ? rc : io.finish();
+}
+
 int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                           int64_t count, const float* sqdist, const int32_t* const* idx, double limit_sq, int flags,
                           void* out, int device, void* stream_v) {

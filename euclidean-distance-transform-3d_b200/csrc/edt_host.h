@@ -1,11 +1,12 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as nine translation units so that the kernel templates build in
+// The library is compiled as ten translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
-// transforms' kernels), edt_surface.cu (the surface distances' kernels) and edt_morphology.cu (the
-// spherical morphology's label-writing stores).  The run-time label width
+// transforms' kernels), edt_surface.cu (the surface distances' kernels), edt_morphology.cu (the
+// spherical morphology's label-writing stores) and edt_parabolic.cu (the parabolic erosion and
+// dilation passes).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -287,6 +288,13 @@ int launch_morph_select(const float* f, int64_t total, float bound, const MorphS
                         cudaStream_t stream);
 int launch_fold_float_labels(const void* in, int label_bytes, void* out, int64_t total, DeviceCache& dc,
                              cudaStream_t stream);
+
+// One pass of a parabolic erosion (dilate: dilation) along the lines of g, in -> out (in == out: in
+// place), with weight w (edt_parabolic.cu).  rows: the X pass, whose lines are g.outer_count rows of
+// g.n contiguous samples g.outer_stride apart (inner_count 1, line_stride 1).  *kernel: what ran --
+// 0 the tile kernel, 1 the long-line hull, 2 the brute-force minimum, 3 the copy of an overflowing w^2.
+int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool rows, float w, bool dilate,
+                          DeviceCache& dc, cudaStream_t stream, int* kernel);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

@@ -36,7 +36,8 @@ extern "C" {
  * 201: additions only -- edtb200_last_later_launch.  202: additions only -- edtb200_feature_transform.
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
- * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology)
+ * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
+ * edtb200_parabolic)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -237,6 +238,46 @@ int edtb200_morphology(const void *labels, int label_bytes, int ndim,
                        int64_t sx, int64_t sy, int64_t sz, int64_t count,
                        float wx, float wy, float wz, int op, double radius,
                        int black_border, int flags, void *out, int device, void *stream);
+
+/* Parabolic erosion and dilation of float volumes: the distance transform of a sampled function
+ * (Felzenszwalb-Huttenlocher), ITK's ParabolicErode / DilateImageFilter.  Volumes are x-fastest, as
+ * everywhere here.  Erosion: g0 = f as float32, then one pass per axis a in the order x, y, z:
+ *     g_a(i) = min over j on i's line of cand(i, j)
+ *     cand(i, i) = g_{a-1}(i)                                    (the sample itself, never w2 * 0)
+ *     cand(i, j) = fl32(fl64(fl64(w2 * fl64((i-j)^2)) + fl64(g_{a-1}(j)))),  j != i
+ *     w2 = fl64(fl32(w_a * w_a))
+ * -- w2 rounded in float, the sum formed in double and rounded once to float32: what numpy computes in
+ * float64 followed by .astype(np.float32).  Lines never cross the volume (nor one volume of a stack
+ * into the next) and there are no border terms.  A NaN sample is read as +inf (never a site), -0.0 is
+ * read and written as +0.0, so every zero result is +0.0.  When w_a * w_a overflows float32 (w2 = +inf)
+ * every j != i candidate is +inf and the pass leaves its samples as they are; with a finite w2, a -inf
+ * sample makes its whole line -inf.  Dilation is -erosion(-f), with the same NaN and zero rules.  The
+ * result equals this definition bit for bit for every input.
+ *
+ * Uses: with integer weights, f = 0 on sites and +inf elsewhere gives the edtsq of the mask; a dilation
+ * of r^2 (-inf off the medial points) gives the reverse distance transform, > 0 on the union of balls;
+ * ITK's scale t is the weight spacing / sqrt(2 t).
+ *
+ *   f, out   count * sx*sy*sz float32, volumes back to back as for edtb200_transform_stack (count 1:
+ *            one volume).  out == f is allowed (in place); any other overlap is EDTB200_EINVAL.
+ *   wx..wz   the weights of the first ndim axes: finite and > 0 (the others are ignored)
+ *   op       EDTB200_PARABOLIC_ERODE or EDTB200_PARABOLIC_DILATE
+ *   flags    EDTB200_LABELS_ON_DEVICE (f is a device pointer) and EDTB200_OUT_ON_DEVICE only.  Both on
+ *            the device: asynchronous on `stream`, no lock and no host wait.  Host buffers are staged
+ *            whole through the device (there is no chunked path; EDTB200_ENOMEM when they do not fit).
+ * One launch per pass for the whole stack; the first pass runs f -> out, the others in place on out.
+ * Lines of at most 1024 samples take tile kernels that read and write every value once per pass and
+ * need no device memory beyond f and out.  Longer lines of at most 23170 samples take a one-thread-
+ * per-line hull with 8 bytes of device scratch per sample of the lines in flight (at most about 1 GiB);
+ * longer lines than that take a brute-force minimum over every candidate (O(n^2) per line), which in
+ * place needs a copy of the volume.  The hull is exact: its predicates fall back to exact expansion
+ * arithmetic where a double evaluation cannot decide.
+ * Checks, in order: ndim, sizes (as edtb200_transform), count >= 0, op, weights, flags, the stack's size
+ * (within 2^62 voxels), emptiness (returns 0 touching nothing), pointers and overlap, device. */
+#define EDTB200_PARABOLIC_ERODE  0
+#define EDTB200_PARABOLIC_DILATE 1
+int edtb200_parabolic(const float *f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                      float wx, float wy, float wz, int op, int flags, float *out, int device, void *stream);
 
 /* A stack of `count` volumes of one geometry (sx, sy, sz), laid back to back (volume b starts at
  * voxel b * sx * sy * sz), each transformed on its own as edtb200_transform would: its result is

@@ -130,6 +130,14 @@ for dtype in (np.uint8, np.uint16, np.uint32, np.uint64, np.float32):
 vols = np.stack([cases.random_volume(rng, (12, 14, 9), "blocks", np.uint16) for _ in range(3)])
 check("morphology stack", edt.spherical_open(vols, 2.0, stacked=True),
       np.stack([mc.threshold("open", v, 2.0) for v in vols]))
+# parabolic erosion / dilation: the X and Y / Z tile kernels with ragged tiles, the long-line hull, the
+# brute-force minimum and the copy of an overflowing w^2, against the numpy restatement
+import parabolic_cases as pc  # noqa: E402
+for shape, w in (((5, 33, 37), (0.7, 1.3, 2.9)), ((3, 1100), (1.0, 0.7)), ((1100, 2), (1.3, 1.0)),
+                 ((23172,), (0.7,)), ((4, 6, 7), (1e20, 1.0, 2.0))):
+  for op in ("erode", "dilate"):
+    f = pc.values("special", shape, rng)
+    check("parabolic %s %s" % (op, shape), getattr(edt, "parabolic_" + op)(f, w), pc.restate(op, f, w))
 # per-label views: a nearly full table whose probe chain wraps past its end, a table that overflows, and
 # a sub-box drawn at a ragged row length; the helpers are the GPU tests' own
 import each_cases as ec  # noqa: E402

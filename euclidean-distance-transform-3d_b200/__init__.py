@@ -114,6 +114,8 @@ def _lib():
   lib.edtb200_morphology.restype = ci
   lib.edtb200_parabolic.argtypes = [vp, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp]
   lib.edtb200_parabolic.restype = ci
+  lib.edtb200_parabolic_sites.argtypes = [vp, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
+  lib.edtb200_parabolic_sites.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1338,9 +1340,13 @@ def spherical_close(labels, radius, anisotropy=None, black_border=False, *, devi
 _PARABOLIC_ERODE, _PARABOLIC_DILATE = 0, 1      # EDTB200_PARABOLIC_ERODE, _DILATE
 
 
-def _parabolic(op, f, anisotropy, device, stacked, name):
-  """Every check before any device use, then one edtb200_parabolic call: host arrays are staged whole
-  (numpy out), device arrays run on the current stream (torch out)."""
+def _parabolic(op, f, anisotropy, device, stacked, name, return_indices=False):
+  """Every check before any device use, then one edtb200_parabolic call (edtb200_parabolic_sites with
+  return_indices): host arrays are staged whole (numpy out), device arrays run on the current stream
+  (torch out).  The index planes come back x first; indices[k], the coordinate along array axis k, is
+  x-fastest plane vnd - 1 - k of a C-ordered array and plane k of an F-ordered one."""
+  if not isinstance(return_indices, (bool, np.bool_)):
+    raise TypeError("%s: return_indices must be True or False, got %r" % (name, return_indices))
   on_device = _device_array(f)
   arr = None if on_device is not None else np.asarray(f)
   nd = on_device.dim() if on_device is not None else arr.ndim
@@ -1362,15 +1368,21 @@ def _parabolic(op, f, anisotropy, device, stacked, name):
     arr, order = _stack_order(arr)
     arr = arr.astype(np.float32, order="K", copy=False)
     out = np.empty(arr.shape, dtype=np.float32, order=order)
-    if arr.size == 0:
+    planes = np.empty((vnd,) + (arr.shape if order == "C" else arr.shape[::-1]), np.int32) if return_indices else None
+    if arr.size:
+      if stacked:
+        count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
+      else:
+        count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
+      if return_indices:
+        _check(lib.edtb200_parabolic_sites(arr.ctypes.data, vnd, sx, sy, sz, count, wx, wy, wz, op, 0,
+                                           out.ctypes.data, planes.ctypes.data, int(device), None))
+      else:
+        _check(lib.edtb200_parabolic(arr.ctypes.data, vnd, sx, sy, sz, count, wx, wy, wz, op, 0, out.ctypes.data,
+                                     int(device), None))
+    if not return_indices:
       return out
-    if stacked:
-      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
-    else:
-      count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
-    _check(lib.edtb200_parabolic(arr.ctypes.data, vnd, sx, sy, sz, count, wx, wy, wz, op, 0, out.ctypes.data,
-                                 int(device), None))
-    return out
+    return out, (planes[::-1] if order == "C" else planes.transpose((0,) + tuple(range(nd, 0, -1))))
   import torch
   t = on_device
   fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
@@ -1379,14 +1391,24 @@ def _parabolic(op, f, anisotropy, device, stacked, name):
     weights = tuple(reversed(weights))
   t = t.to(torch.float32).contiguous()
   out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
+  planes = torch.empty((vnd,) + tuple(t.shape), dtype=torch.int32, device=t.device) if return_indices else None
   if t.numel():
     count = int(t.shape[0]) if stacked else 1
     (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
-    stream = torch.cuda.current_stream(t.device).cuda_stream
-    _check(lib.edtb200_parabolic(t.data_ptr(), vnd, sx, sy, sz, count, wx, wy, wz, op,
-                                 FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, out.data_ptr(), t.device.index,
-                                 ctypes.c_void_p(stream)))
-  return out.permute(*reversed(range(nd))) if fortran else out
+    stream = ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
+    both = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
+    if return_indices:
+      _check(lib.edtb200_parabolic_sites(t.data_ptr(), vnd, sx, sy, sz, count, wx, wy, wz, op, both, out.data_ptr(),
+                                         planes.data_ptr(), t.device.index, stream))
+    else:
+      _check(lib.edtb200_parabolic(t.data_ptr(), vnd, sx, sy, sz, count, wx, wy, wz, op, both, out.data_ptr(),
+                                   t.device.index, stream))
+  if fortran:
+    out = out.permute(*reversed(range(nd)))
+  if not return_indices:
+    return out
+  # x first as written: an F-ordered caller's axis k is plane k, a C-ordered caller's is plane vnd - 1 - k
+  return out, (planes.permute(0, *range(nd, 0, -1)) if fortran else planes.flip(0))
 
 
 _PARABOLIC_DOC = """
@@ -1413,6 +1435,20 @@ _PARABOLIC_DOC = """
   a ValueError, a wrong number of dimensions or a non-real dtype a TypeError; a host array that does not
   fit on the GPU raises EDTError with code ENOMEM (there is no chunked path).
 
+  return_indices=True returns (values, indices): the values bit for bit as without it, and the sample q
+  that gives each value, int32 of shape (vnd,) + f.shape in scipy's layout (indices[k] is the coordinate
+  along array axis k, each plane in the input's memory order; with stacked=True within each volume), as
+  feature_transform returns them.  Each pass picks a site on every line among the candidates above (j = i
+  included): on lines of at most 23170 samples the least j among the REAL minimisers of
+  w2 * (i-j)^2 + g(j); on longer lines the least j among the minimisers of the float64 sum before its
+  float32 rounding.  NaN and +inf samples are never sites; with a finite w2 a line holding -inf takes its
+  least -inf position; with w2 = +inf every sample is its own site.  Dilation is the erosion of -f, so it
+  names the least maximiser.  The sites compose as the feature transform's (q_z from the Z pass at p, q_y
+  from the Y pass at (p_x, p_y, q_z), q_x from the X pass at (p_x, q_y, q_z)); where a line has no
+  candidate at all every coordinate is -1 and the value +inf (-inf for dilation).  So f(q) is never NaN,
+  and the value at p is the chain of rounded candidates from f(q): the X pass's, then Y's, then Z's.  It
+  costs 4 bytes per voxel of device memory per pass but the last, and lines of more than 2^26 samples.
+
   Worked uses.
     edtsq of a mask, with integer weights w:
         parabolic_erode(np.where(mask, np.inf, 0), w) == edtsq(mask, w)          (bit for bit)
@@ -1420,15 +1456,24 @@ _PARABOLIC_DOC = """
         parabolic_dilate(np.where(medial, r * r, -np.inf)) > 0
     ITK's ParabolicErode / DilateImageFilter at scale t with voxel spacing s:
         anisotropy = s / sqrt(2 t)
+    the power (Laguerre) diagram of weighted seeds -- p's cell is the seed c least in |p - c|^2 - omega_c:
+        f = np.where(seed_labels != 0, -omega, np.inf)
+        _, idx = parabolic_erode(f, return_indices=True)
+        cells = seed_labels[tuple(idx)]
+    the best placement of a part (Felzenszwalb-Huttenlocher): q maximising score(q) - sum_a (w_a d_a)^2:
+        best, idx = parabolic_dilate(score, w, return_indices=True)
+    the medial ball that decides each voxel of the reverse distance transform (-1 off the union):
+        cover, idx = parabolic_dilate(np.where(medial, r * r, -np.inf), return_indices=True)
+        ball = np.where(cover > 0, ball_ids[tuple(idx)], -1)
   """
 
 
-def parabolic_erode(f, anisotropy=None, *, device=0, stacked=False):
-  return _parabolic(_PARABOLIC_ERODE, f, anisotropy, device, stacked, "parabolic_erode")
+def parabolic_erode(f, anisotropy=None, *, device=0, stacked=False, return_indices=False):
+  return _parabolic(_PARABOLIC_ERODE, f, anisotropy, device, stacked, "parabolic_erode", return_indices)
 
 
-def parabolic_dilate(f, anisotropy=None, *, device=0, stacked=False):
-  return _parabolic(_PARABOLIC_DILATE, f, anisotropy, device, stacked, "parabolic_dilate")
+def parabolic_dilate(f, anisotropy=None, *, device=0, stacked=False, return_indices=False):
+  return _parabolic(_PARABOLIC_DILATE, f, anisotropy, device, stacked, "parabolic_dilate", return_indices)
 
 
 parabolic_erode.__doc__ = """Parabolic (grayscale) erosion: g(p) = min_q f(q) + sum_a (w_a (p_a - q_a))^2, computed as

@@ -1770,8 +1770,11 @@ int edtb200_morphology(const void* labels, int label_bytes, int ndim, int64_t sx
   return rc ? rc : io.finish();
 }
 
-int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx,
-                      float wy, float wz, int op, int flags, float* out, int device, void* stream_v) {
+// edtb200_parabolic, and with sites edtb200_parabolic_sites.
+static int parabolic_any(const float* f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx,
+                         float wy, float wz, int op, int flags, float* out, bool sites, int32_t* idx, int device,
+                         void* stream_v) {
+  const char* name = sites ? "edtb200_parabolic_sites" : "edtb200_parabolic";
   int rc = check_dims(4, ndim, sx, sy, sz);
   if (rc) return rc;
   if (count < 0) return fail(EDTB200_EINVAL, "negative count");
@@ -1782,16 +1785,23 @@ int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t 
     if (!(std::isfinite(w[k]) && w[k] > 0.0f))
       return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
   if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
-    return fail(EDTB200_EINVAL, "edtb200_parabolic takes only the residency flags (got %d)", flags);
+    return fail(EDTB200_EINVAL, "%s takes only the residency flags (got %d)", name, flags);
   const int64_t vol = sx * sy * sz;
   if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  // with sites, (i-j)^2 must be exact in double on the brute-force lines
+  if (sites && (sx > kParabolicSitesN || sy > kParabolicSitesN || sz > kParabolicSitesN))
+    return fail(EDTB200_ELIMIT, "%s takes lines of at most 2^26 samples", name);
   const int64_t total = vol * count;
   if (total == 0) return 0;
-  if (!f || !out) return fail(EDTB200_EINVAL, "null pointer");
-  const size_t bytes = sizeof(float) * (size_t)total;
+  if (!f || !out || (sites && !idx)) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t bytes = sizeof(float) * (size_t)total, idx_bytes = (size_t)ndim * bytes;
   const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
-  if (same_side && f != out && (const char*)f < (const char*)out + bytes && (const char*)out < (const char*)f + bytes)
-    return fail(EDTB200_EINVAL, "out overlaps f without being f");
+  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
+  };
+  if (same_side && f != out && overlap(f, bytes, out, bytes)) return fail(EDTB200_EINVAL, "out overlaps f without being f");
+  if (idx && overlap(idx, idx_bytes, out, bytes)) return fail(EDTB200_EINVAL, "idx overlaps out");
+  if (idx && same_side && overlap(idx, idx_bytes, f, bytes)) return fail(EDTB200_EINVAL, "idx overlaps f");
 
   DeviceGuard restore_device;
   DeviceCache* dc = nullptr;
@@ -1803,6 +1813,23 @@ int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t 
   if ((rc = io.in(f, bytes, dc->labels, &d_f))) return rc;
   if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, bytes));
   float* d_out = io.out(out, bytes, dc->dist);
+  // sites: the index planes (staged for a host idx), and the code planes of every pass but the last,
+  // whose codes go straight into its own index plane (the resolver reads them only at their own voxel)
+  Scratch staged, planes;
+  int32_t* d_idx = nullptr;
+  int* codes[3] = {nullptr, nullptr, nullptr};
+  if (idx) {
+    if (!io.out_dev && staged.alloc(*dc, idx_bytes, s) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(EDTB200_ENOMEM, "no device memory for the index planes");
+    }
+    d_idx = io.out(idx, idx_bytes, io.out_dev ? nullptr : staged.get<int32_t>());
+    if (ndim > 1 && planes.alloc(*dc, (size_t)(ndim - 1) * bytes, s) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(EDTB200_ENOMEM, "no device memory for the site code planes");
+    }
+    for (int k = 0; k < ndim; ++k) codes[k] = (k == ndim - 1 ? d_idx : planes.get<int32_t>()) + (size_t)k * total;
+  }
   // EDT_B200_VERBOSE=1: per-pass device times and kernels on stderr (synchronises the stream)
   static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1816,9 +1843,14 @@ int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t 
     if (k == 0) {                              // rows of sx contiguous samples
       g.outer_count = sy * sz * count; g.outer_stride = sx; g.inner_count = 1; g.line_stride = 1; g.n = (int)sx;
     }
-    rc = launch_parabolic_pass(src, d_out, g, k == 0, w[k], op == EDTB200_PARABOLIC_DILATE, *dc, s, &kernel[k]);
+    rc = launch_parabolic_pass(src, d_out, g, k == 0, w[k], op == EDTB200_PARABOLIC_DILATE, *dc, s, &kernel[k],
+                               codes[k]);
     if (ev[k + 1]) cudaEventRecord(ev[k + 1], s);
     src = d_out;
+  }
+  if (!rc && idx) {
+    int32_t* const planes_out[3] = {d_idx, d_idx + total, d_idx + 2 * (size_t)total};
+    rc = launch_resolve_sites<1>(nullptr, codes, ndim, sx, sy, sz, count, false, planes_out, *dc, s);
   }
   if (verbose) {
     static const char* names[4] = {"tile", "long", "brute", "copy"};
@@ -1836,6 +1868,17 @@ int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t 
     cudaGetLastError();
   }
   return rc ? rc : io.finish();
+}
+
+int edtb200_parabolic(const float* f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx,
+                      float wy, float wz, int op, int flags, float* out, int device, void* stream_v) {
+  return parabolic_any(f, ndim, sx, sy, sz, count, wx, wy, wz, op, flags, out, false, nullptr, device, stream_v);
+}
+
+int edtb200_parabolic_sites(const float* f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx,
+                            float wy, float wz, int op, int flags, float* out, int32_t* idx, int device,
+                            void* stream_v) {
+  return parabolic_any(f, ndim, sx, sy, sz, count, wx, wy, wz, op, flags, out, true, idx, device, stream_v);
 }
 
 int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,

@@ -293,8 +293,12 @@ int launch_fold_float_labels(const void* in, int label_bytes, void* out, int64_t
 // place), with weight w (edt_parabolic.cu).  rows: the X pass, whose lines are g.outer_count rows of
 // g.n contiguous samples g.outer_stride apart (inner_count 1, line_stride 1).  *kernel: what ran --
 // 0 the tile kernel, 1 the long-line hull, 2 the brute-force minimum, 3 the copy of an overflowing w^2.
+// codes non-null: the site-tracking instances, which also write every sample's site code (its winning
+// row on its line, or kSiteNone) to codes, laid out like out; lines of at most kParabolicSitesN samples,
+// beyond which (i-j)^2 is not exact in double.
+constexpr int64_t kParabolicSitesN = (int64_t)1 << 26;
 int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool rows, float w, bool dilate,
-                          DeviceCache& dc, cudaStream_t stream, int* kernel);
+                          DeviceCache& dc, cudaStream_t stream, int* kernel, int* codes = nullptr);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

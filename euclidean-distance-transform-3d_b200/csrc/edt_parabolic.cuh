@@ -30,6 +30,14 @@
 // Each value is read once and written once per pass on the tile kernels, which need no device memory
 // beyond their input and output; in place (in == out) every kernel but the brute-force one reads a
 // line wholly before writing it, and that one reads a copy.
+//
+// Sites (edtb200_parabolic_sites): separate instances (Sites = true, and parabolic_copy_sites_kernel)
+// also write every sample's winning row to a code plane, kSiteNone where the line has no candidate; the
+// values are those of the other instances bit for bit.  On lines of at most kParabolicExactN samples the
+// row is the least REAL minimiser: the read-out moves to the next hull vertex only when it is strictly
+// lower (pb_below, exact), and the tile kernels merge their segments in order by the same exact test.
+// Longer lines take the least j with the least double candidate.  The X tile kernel sends the codes
+// through a second transpose buffer per warp, so its rows of 1009 to 1024 samples take 2 warps, not 4.
 #pragma once
 #include "edt_host.h"
 
@@ -115,6 +123,18 @@ __device__ __forceinline__ bool pb_not_above(float fa, int a, float fb, int b, i
   return pb_exact_sign<3>(t) <= 0;
 }
 
+// Whether vertex b is strictly lower than vertex a at row i (any a, b): pb_not_above without the tie,
+// so that a read-out or a merge that moves only on it keeps the least minimiser.
+__device__ __forceinline__ bool pb_below(float fa, int a, float fb, int b, int i, double w2) {
+  const double q = __dmul_rn(w2, (double)(b - a) * (double)(2 * i - a - b));
+  const double s = __dsub_rn(__dsub_rn((double)fb, (double)fa), q);
+  const double bound = __dmul_rn(fabs((double)fa) + fabs((double)fb) + fabs(q), 0x1p-50);
+  if (s < -bound) return true;
+  if (s > bound) return false;
+  const double t[3] = {(double)fb, -(double)fa, -q};
+  return pb_exact_sign<3>(t) < 0;
+}
+
 // The candidate of vertex (f, v) at row i, rounded as the definition rounds it (d^2 w2 exact).
 __device__ __forceinline__ float pb_value(float f, int v, int i, double w2) {
   const int d = i - v;
@@ -162,12 +182,51 @@ struct PbHull {
     }
     return pb_value(fa, a, i, w2);
   }
+  // at(i) with its site: the read-out stays on a vertex that ties with the next one, so the site is the
+  // least minimiser (the hull never drops it: a vertex hidden at E = 0 ties with a lower position).
+  // first_neg: the first -inf position pushed (kSiteNone: none), the site of a -inf line.
+  __device__ float at_site(int i, int first_neg, int* site) {
+    if (neg) { *site = first_neg; return -__int_as_float(0x7f800000); }
+    if (top < 0) { *site = kSiteNone; return __int_as_float(0x7f800000); }
+    while (k < top && pb_below(fa, a, fb, b, i, w2)) {
+      ++k;
+      fa = fb;
+      a = b;
+      if (k < top) { fb = sf[(k + 1) * fs]; b = (int)si[(k + 1) * is]; }
+    }
+    *site = a;
+    return pb_value(fa, a, i, w2);
+  }
 };
+
+// The site-tracking read-out of a tile: the minimum at row i over the S segment hulls and its site.
+// Segments are merged in order and a later one wins only when its REAL candidate is strictly lower
+// (fminf of the rounded minima could not tell two different reals that round alike), so the site is
+// the least minimiser of the line; an earlier -inf segment keeps its first -inf position.
+template <int S>
+__device__ __forceinline__ float pb_merge_sites(PbHull<uint16_t> (&r)[S], const int (&first_neg)[S], int i,
+                                                double w2, int* site) {
+  float v = r[0].at_site(i, first_neg[0], site);
+  float bf = r[0].fa;                 // the winning vertex, when it is one (not -inf, not none)
+  for (int q = 1; q < S; ++q) {
+    int sq;
+    const float vq = r[q].at_site(i, first_neg[q], &sq);
+    if (sq == kSiteNone || v == -__int_as_float(0x7f800000)) continue;
+    if (vq == -__int_as_float(0x7f800000) || *site == kSiteNone || pb_below(bf, *site, r[q].fa, sq, i, w2)) {
+      v = vq;
+      *site = sq;
+      bf = r[q].fa;
+    }
+  }
+  return v;
+}
 
 // Shared memory of one tile CTA of S warps: the staged samples / stack heights, the stack positions,
 // each segment's stack top and -inf flag and, for the X pass, one 32 x 33 transpose buffer per warp.
-__host__ __device__ constexpr size_t pb_tile_smem(int n, bool rows, int S) {
-  return (size_t)n * (rows ? 33 : 32) * 4 + (size_t)n * 32 * 2 + (size_t)S * 32 * 8 + (rows ? (size_t)S * 32 * 33 * 4 : 0);
+// With sites, the X pass has a second transpose buffer per warp for the site codes.
+__host__ __device__ constexpr size_t pb_tile_smem(int n, bool rows, int S, bool sites = false) {
+  return (size_t)n * (rows ? 33 : 32) * 4 + (size_t)n * 32 * 2 + (size_t)S * 32 * 8 +
+         (rows ? (size_t)S * 32 * 33 * 4 * (sites ? 2 : 1) : 0);
 }
 
 // rows = false: lines of g (Y / Z pass), a tile = 32 adjacent lines of one outer index.
@@ -178,9 +237,11 @@ __host__ __device__ constexpr size_t pb_tile_smem(int n, bool rows, int S) {
 // own segment as the minimum over the S segment hulls.  The minimum of the rounded minima of the
 // segments is the rounded minimum of the line, so the result does not depend on S; S trades a shorter
 // serial hull build (n / S per lane) and S times the warps per SM for S candidates per output row.
-template <bool Rows, int S>
+// Sites: also write every sample's site code (its winning row, or kSiteNone) to `codes`, laid out like
+// `out`: each segment's read-out keeps its least minimiser and pb_merge_sites merges them exactly.
+template <bool Rows, int S, bool Sites = false>
 __global__ void __launch_bounds__(32 * S)
-parabolic_tile_kernel(const float* in, float* out, LineGeom g, double w2, bool dilate, int64_t tiles) {
+parabolic_tile_kernel(const float* in, float* out, LineGeom g, double w2, bool dilate, int64_t tiles, int* codes) {
   extern __shared__ __align__(16) unsigned char pb_smem[];
   constexpr int fp = Rows ? 33 : 32;
   const int n = g.n, lane = threadIdx.x & 31, s = threadIdx.x >> 5;
@@ -190,6 +251,7 @@ parabolic_tile_kernel(const float* in, float* out, LineGeom g, double w2, bool d
   int* tops = reinterpret_cast<int*>(pb_smem + (size_t)n * fp * 4 + (size_t)n * 64);
   int* negs = tops + S * 32;
   float* ob = reinterpret_cast<float*>(negs + S * 32) + s * 32 * 33;
+  int* oc = reinterpret_cast<int*>(negs + S * 32) + (S + s) * 32 * 33;     // Sites, X pass: the codes' buffer
   const int64_t tpo = (g.inner_count + 31) >> 5;
   for (int64_t t = blockIdx.x; t < tiles; t += gridDim.x) {
     int64_t base;
@@ -213,17 +275,30 @@ parabolic_tile_kernel(const float* in, float* out, LineGeom g, double w2, bool d
     __pipeline_wait_prior(0);
     __syncwarp();                     // the warp's lanes staged each other's columns of its segment
     PbHull<uint16_t> h{sf + lo * fp + lane, si + lo * 32 + lane, fp, 32, w2};
+    int first_neg = kSiteNone;        // Sites: the segment's first -inf position
     if (on)
-      for (int j = lo; j < hi; ++j) h.push(pb_in(sf[j * fp + lane], dilate), j);
+      for (int j = lo; j < hi; ++j) {
+        const float v = pb_in(sf[j * fp + lane], dilate);
+        if constexpr (Sites)
+          if (first_neg == kSiteNone && v == -__int_as_float(0x7f800000)) first_neg = j;
+        h.push(v, j);
+      }
     tops[s * 32 + lane] = h.top;
-    negs[s * 32 + lane] = h.neg;
+    if constexpr (Sites) negs[s * 32 + lane] = first_neg;
+    else negs[s * 32 + lane] = h.neg;
     __syncthreads();                  // every segment's hull is built
     PbHull<uint16_t> r[S];
+    int rneg[S];
     for (int q = 0; q < S; ++q) {
       const int qlo = min(n, q * seg);
       r[q] = PbHull<uint16_t>{sf + qlo * fp + lane, si + qlo * 32 + lane, fp, 32, w2};
       r[q].top = tops[q * 32 + lane];
-      r[q].neg = negs[q * 32 + lane] != 0;
+      if constexpr (Sites) {
+        rneg[q] = negs[q * 32 + lane];
+        r[q].neg = rneg[q] != kSiteNone;
+      } else {
+        r[q].neg = negs[q * 32 + lane] != 0;
+      }
       r[q].start();
     }
     auto at = [&](int i) {
@@ -234,14 +309,33 @@ parabolic_tile_kernel(const float* in, float* out, LineGeom g, double w2, bool d
     if (Rows) {
       const int64_t r0 = t * 32;
       for (int c = lo; c < hi; c += 32) {
-        for (int q = 0; q < 32 && c + q < hi; ++q) ob[q * 33 + lane] = at(c + q);
+        for (int q = 0; q < 32 && c + q < hi; ++q) {
+          if constexpr (Sites) {
+            int site;
+            ob[q * 33 + lane] = pb_out(pb_merge_sites<S>(r, rneg, c + q, w2, &site), dilate);
+            oc[q * 33 + lane] = site;
+          } else {
+            ob[q * 33 + lane] = at(c + q);
+          }
+        }
         __syncwarp();
         if (c + lane < hi)
-          for (int rr = 0; rr < 32 && r0 + rr < g.outer_count; ++rr) out[(r0 + rr) * g.outer_stride + c + lane] = ob[lane * 33 + rr];
+          for (int rr = 0; rr < 32 && r0 + rr < g.outer_count; ++rr) {
+            out[(r0 + rr) * g.outer_stride + c + lane] = ob[lane * 33 + rr];
+            if constexpr (Sites) codes[(r0 + rr) * g.outer_stride + c + lane] = oc[lane * 33 + rr];
+          }
         __syncwarp();
       }
     } else if (on) {
-      for (int i = lo; i < hi; ++i) out[base + i * g.line_stride] = at(i);
+      for (int i = lo; i < hi; ++i) {
+        if constexpr (Sites) {
+          int site;
+          out[base + i * g.line_stride] = pb_out(pb_merge_sites<S>(r, rneg, i, w2, &site), dilate);
+          codes[base + i * g.line_stride] = site;
+        } else {
+          out[base + i * g.line_stride] = at(i);
+        }
+      }
     }
     __syncthreads();                  // the next tile's staging overwrites every segment's hull
   }
@@ -249,36 +343,73 @@ parabolic_tile_kernel(const float* in, float* out, LineGeom g, double w2, bool d
 
 // One thread per line of at most kParabolicExactN samples; stack slot m of thread `tid` at
 // [m * threads + tid] of sf / si (coalesced across threads).  Lines: outer_count x inner_count.
+// Sites: also the site codes, as parabolic_tile_kernel writes them.
+template <bool Sites = false>
 __global__ void __launch_bounds__(128)
-parabolic_long_kernel(const float* in, float* out, LineGeom g, double w2, bool dilate, float* sf, int* si) {
+parabolic_long_kernel(const float* in, float* out, LineGeom g, double w2, bool dilate, float* sf, int* si, int* codes) {
   const int64_t threads = (int64_t)gridDim.x * blockDim.x, tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t lines = g.outer_count * g.inner_count;
   for (int64_t l = tid; l < lines; l += threads) {
     const int64_t o = l / g.inner_count, base = o * g.outer_stride + (l - o * g.inner_count);
     PbHull<int> h{sf + tid, si + tid, (int)threads, (int)threads, w2};
-    for (int j = 0; j < g.n; ++j) h.push(pb_in(in[base + j * g.line_stride], dilate), j);
+    int first_neg = kSiteNone;
+    for (int j = 0; j < g.n; ++j) {
+      const float v = pb_in(in[base + j * g.line_stride], dilate);
+      if constexpr (Sites)
+        if (first_neg == kSiteNone && v == -__int_as_float(0x7f800000)) first_neg = j;
+      h.push(v, j);
+    }
     h.start();
-    for (int i = 0; i < g.n; ++i) out[base + i * g.line_stride] = pb_out(h.at(i), dilate);
+    for (int i = 0; i < g.n; ++i) {
+      if constexpr (Sites) {
+        int site;
+        out[base + i * g.line_stride] = pb_out(h.at_site(i, first_neg, &site), dilate);
+        codes[base + i * g.line_stride] = site;
+      } else {
+        out[base + i * g.line_stride] = pb_out(h.at(i), dilate);
+      }
+    }
   }
 }
 
 // One thread per output sample of lines longer than kParabolicExactN: every candidate, formed as the
 // definition forms it (fl64 of (i-j)^2, of its product with w2 and of the sum).  `in` is not `out`.
+// Sites: the least j with the least double candidate (j == i: the sample itself), which rounds to the
+// minimum of the rounded candidates; +inf samples are never sites.
+template <bool Sites = false>
 __global__ void __launch_bounds__(256)
-parabolic_brute_kernel(const float* __restrict__ in, float* __restrict__ out, LineGeom g, double w2, bool dilate) {
+parabolic_brute_kernel(const float* __restrict__ in, float* __restrict__ out, LineGeom g, double w2, bool dilate,
+                       int* __restrict__ codes) {
   const int64_t total = g.outer_count * g.inner_count * (int64_t)g.n;
   for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < total; v += (int64_t)gridDim.x * blockDim.x) {
     const int64_t l = v / g.n, i = v - l * g.n;
     const int64_t o = l / g.inner_count, base = o * g.outer_stride + (l - o * g.inner_count);
-    float best = pb_in(in[base + i * g.line_stride], dilate);
-    for (int64_t j = 0; j < g.n; ++j) {
-      if (j == i) continue;
-      const double d = (double)(i - j);
-      const float c = __double2float_rn(__dadd_rn(__dmul_rn(w2, __dmul_rn(d, d)),
-                                                  (double)pb_in(in[base + j * g.line_stride], dilate)));
-      best = fminf(best, c);
+    if constexpr (Sites) {
+      double best = __int_as_float(0x7f800000);
+      int site = kSiteNone;
+      for (int64_t j = 0; j < g.n; ++j) {
+        const float f = pb_in(in[base + j * g.line_stride], dilate);
+        if (f == __int_as_float(0x7f800000)) continue;
+        const double d = (double)(i - j);
+        const double c = j == i ? (double)f : __dadd_rn(__dmul_rn(w2, __dmul_rn(d, d)), (double)f);
+        if (site == kSiteNone || c < best) {
+          best = c;
+          site = (int)j;
+        }
+      }
+      out[base + i * g.line_stride] = pb_out(__double2float_rn(best), dilate);
+      codes[base + i * g.line_stride] = site;
+    } else {
+      float best = pb_in(in[base + i * g.line_stride], dilate);
+      for (int64_t j = 0; j < g.n; ++j) {
+        if (j == i) continue;
+        const double d = (double)(i - j);
+        const float c = __double2float_rn(__dadd_rn(__dmul_rn(w2, __dmul_rn(d, d)),
+                                                    (double)pb_in(in[base + j * g.line_stride], dilate)));
+        best = fminf(best, c);
+      }
+      out[base + i * g.line_stride] = pb_out(best, dilate);
     }
-    out[base + i * g.line_stride] = pb_out(best, dilate);
   }
 }
 
@@ -286,6 +417,18 @@ __global__ void __launch_bounds__(256)
 parabolic_copy_kernel(const float* in, float* out, int64_t total, bool dilate) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
     out[i] = pb_out(pb_in(in[i], dilate), dilate);
+}
+
+// parabolic_copy_kernel with the site codes: every sample is its own site (its row, (i / stride) % n
+// along lines of n samples `stride` apart), but +inf, which has none.
+__global__ void __launch_bounds__(256)
+parabolic_copy_sites_kernel(const float* in, float* out, int* codes, int64_t total, int64_t stride, int n,
+                            bool dilate) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const float v = pb_in(in[i], dilate);
+    out[i] = pb_out(v, dilate);
+    codes[i] = v == __int_as_float(0x7f800000) ? kSiteNone : (int)((i / stride) % n);
+  }
 }
 
 namespace host {
@@ -298,7 +441,7 @@ inline int64_t pb_long_threads(int64_t lines, int n) {
 }
 
 int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool rows, float w, bool dilate,
-                          DeviceCache& dc, cudaStream_t stream, int* kernel) {
+                          DeviceCache& dc, cudaStream_t stream, int* kernel, int* codes) {
   const float w2f = w * w;                     // rounded to float, as the definition rounds it
   const double w2 = (double)w2f;
   const int64_t lines = g.outer_count * g.inner_count, total = lines * (int64_t)g.n;
@@ -311,7 +454,13 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
   if (std::isinf(w2f)) {
     *kernel = 3;
     // lines are whole and cover the volume, so the pass is elementwise over it
-    parabolic_copy_kernel<<<blocks_for(total, 256), 256, 0, stream>>>(in, out, total, dilate);
+    if (codes) {
+      const int64_t stride = rows ? 1 : g.line_stride;       // the row of sample i is (i / stride) % n
+      parabolic_copy_sites_kernel<<<blocks_for(total, 256), 256, 0, stream>>>(in, out, codes, total, stride, g.n,
+                                                                              dilate);
+    } else {
+      parabolic_copy_kernel<<<blocks_for(total, 256), 256, 0, stream>>>(in, out, total, dilate);
+    }
     CUDA_TRY(cudaGetLastError());
     return 0;
   }
@@ -319,25 +468,30 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
     *kernel = 0;
     // warps per CTA (segments per line): the default from records/h100/parabolic_bench.txt, or
     // EDTB200_PARABOLIC_WARPS = 1, 2 or 4 (an A/B switch for measurements); fewer where the shared
-    // memory of S transpose buffers does not fit
+    // memory of S transpose buffers does not fit (with sites, X rows of more than 1008 samples take 2)
     int S = kParabolicWarps;
     if (const char* env = getenv("EDTB200_PARABOLIC_WARPS")) S = atoi(env);
     if (S != 1 && S != 2 && S != 4) return fail(EDTB200_EINVAL, "EDTB200_PARABOLIC_WARPS must be 1, 2 or 4 (got %d)", S);
-    while (S > 1 && pb_tile_smem(g.n, rows, S) > (size_t)dc.max_smem_optin) S >>= 1;
-    const size_t smem = pb_tile_smem(g.n, rows, S);
+    const bool sites = codes != nullptr;
+    while (S > 1 && pb_tile_smem(g.n, rows, S, sites) > (size_t)dc.max_smem_optin) S >>= 1;
+    const size_t smem = pb_tile_smem(g.n, rows, S, sites);
     if (smem > (size_t)dc.max_smem_optin) return fail(EDTB200_ELIMIT, "a parabolic tile of %d rows exceeds the shared memory", g.n);
     const int64_t tiles = rows ? (g.outer_count + 31) >> 5 : ((g.inner_count + 31) >> 5) * g.outer_count;
     const unsigned blocks = (unsigned)(tiles < ((int64_t)1 << 30) ? tiles : ((int64_t)1 << 30));
     auto go = [&](auto kern) {
       CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      kern<<<blocks, 32 * S, smem, stream>>>(in, out, g, w2, dilate, tiles);
+      kern<<<blocks, 32 * S, smem, stream>>>(in, out, g, w2, dilate, tiles, codes);
       CUDA_TRY(cudaGetLastError());
       return 0;
     };
-    if (rows) return S == 1 ? go(parabolic_tile_kernel<true, 1>) : S == 2 ? go(parabolic_tile_kernel<true, 2>)
-                                                                   : go(parabolic_tile_kernel<true, 4>);
-    return S == 1 ? go(parabolic_tile_kernel<false, 1>) : S == 2 ? go(parabolic_tile_kernel<false, 2>)
-                                                          : go(parabolic_tile_kernel<false, 4>);
+    auto pick = [&](auto with_sites) {
+      constexpr bool St = decltype(with_sites)::value;
+      if (rows) return S == 1 ? go(parabolic_tile_kernel<true, 1, St>) : S == 2 ? go(parabolic_tile_kernel<true, 2, St>)
+                                                                       : go(parabolic_tile_kernel<true, 4, St>);
+      return S == 1 ? go(parabolic_tile_kernel<false, 1, St>) : S == 2 ? go(parabolic_tile_kernel<false, 2, St>)
+                                                              : go(parabolic_tile_kernel<false, 4, St>);
+    };
+    return sites ? pick(std::true_type{}) : pick(std::false_type{});
   }
   if (g.n <= kParabolicExactN) {
     *kernel = 1;
@@ -349,8 +503,9 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
       return fail(EDTB200_ENOMEM, "no device memory for the long lines' hull stacks");
     }
     float* sf = stack.get<float>();
-    parabolic_long_kernel<<<(unsigned)blocks, 128, 0, stream>>>(in, out, g, w2, dilate, sf,
-                                                               reinterpret_cast<int*>(sf + slots * (int64_t)g.n));
+    int* si = reinterpret_cast<int*>(sf + slots * (int64_t)g.n);
+    if (codes) parabolic_long_kernel<true><<<(unsigned)blocks, 128, 0, stream>>>(in, out, g, w2, dilate, sf, si, codes);
+    else parabolic_long_kernel<false><<<(unsigned)blocks, 128, 0, stream>>>(in, out, g, w2, dilate, sf, si, nullptr);
     CUDA_TRY(cudaGetLastError());
     return 0;
   }
@@ -367,7 +522,8 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
     CUDA_TRY(cudaMemcpyAsync(copy.get(), in, sizeof(float) * (size_t)span, cudaMemcpyDeviceToDevice, stream));
     src = copy.get<float>();
   }
-  parabolic_brute_kernel<<<blocks_for(total, 256), 256, 0, stream>>>(src, out, g, w2, dilate);
+  if (codes) parabolic_brute_kernel<true><<<blocks_for(total, 256), 256, 0, stream>>>(src, out, g, w2, dilate, codes);
+  else parabolic_brute_kernel<false><<<blocks_for(total, 256), 256, 0, stream>>>(src, out, g, w2, dilate, nullptr);
   CUDA_TRY(cudaGetLastError());
   return 0;
 }

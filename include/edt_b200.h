@@ -37,7 +37,7 @@ extern "C" {
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
- * edtb200_parabolic)
+ * edtb200_parabolic, edtb200_parabolic_sites)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -278,6 +278,40 @@ int edtb200_morphology(const void *labels, int label_bytes, int ndim,
 #define EDTB200_PARABOLIC_DILATE 1
 int edtb200_parabolic(const float *f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
                       float wx, float wy, float wz, int op, int flags, float *out, int device, void *stream);
+
+/* edtb200_parabolic with the minimising sample q of every voxel p (the maximising one for a dilation):
+ * the seed of p's power (Laguerre) cell, the best placement of a part, the ball that decides p.
+ *
+ * Each pass a also picks a site s_a(i) on the line of every voxel i among its candidates (j = i
+ * included, with the value g_{a-1}(i)):
+ *   - lines of at most 23170 samples (tile kernels and the long-line hull): the least j among the REAL
+ *     minimisers of w2 (i-j)^2 + g_{a-1}(j);
+ *   - longer lines (the brute-force minimum): the least j among the minimisers of the double
+ *     fl64(fl64(w2 * fl64((i-j)^2)) + g_{a-1}(j)), the candidate before its float32 rounding;
+ *   - NaN and +inf samples are never sites; with a finite w2 a line holding -inf takes the least j with
+ *     g_{a-1}(j) = -inf; with w2 = +inf s_a(i) = i; a voxel whose whole line is +inf or NaN has no site.
+ * Rounding is monotone, so the value written is the site's own rounded candidate in both tiers.  A
+ * dilation is the erosion of -f and so names the least maximiser.  The passes' sites compose as the
+ * feature transform's: q_z = s_z(p), q_y = s_y at (p_x, p_y, q_z), q_x = s_x at (p_x, q_y, q_z).  A voxel
+ * without a site gets -1 in every coordinate; its value is +inf (-inf for a dilation).  (A value can also
+ * be +inf with a site, where a finite candidate rounds past the float32 range.)  So f(q) is finite or
+ * +-inf at every q returned, and the value at p is the chain of rounded candidates from f(q): the X
+ * pass's, then the Y pass's, then the Z pass's.
+ *
+ *   f, out, ..., flags, device, stream   as edtb200_parabolic; out is bit for bit its result
+ *   idx   ndim x-fastest int32 planes of count * sx*sy*sz voxels, back to back: idx[0 .. V) the x
+ *         coordinate, then y, then z (V = count * sx*sy*sz), each within its voxel's own volume.  It is on
+ *         the device with EDTB200_OUT_ON_DEVICE, on the host otherwise, and must not overlap f or out.
+ * Device memory beyond edtb200_parabolic's: the code planes of every pass but the last (4 bytes per voxel
+ * each, so 8 in 3-D, 4 in 2-D and none in 1-D; the last pass writes its codes into its index plane), and
+ * for a host idx the staged planes (4 ndim bytes per voxel).  With sites, X rows of 1009 to 1024 samples
+ * take 2 warps per tile CTA instead of 4 (the codes need a second transpose buffer).
+ * Checks, in order: as edtb200_parabolic up to the stack's size, then the line length (a line of more
+ * than 2^26 samples is EDTB200_ELIMIT: beyond it (i-j)^2 is not exact in double), emptiness, pointers
+ * (idx included) and overlap (idx with out, and with f when f is on the same side), device. */
+int edtb200_parabolic_sites(const float *f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                            float wx, float wy, float wz, int op, int flags, float *out,
+                            int32_t *idx, int device, void *stream);
 
 /* A stack of `count` volumes of one geometry (sx, sy, sz), laid back to back (volume b starts at
  * voxel b * sx * sy * sz), each transformed on its own as edtb200_transform would: its result is

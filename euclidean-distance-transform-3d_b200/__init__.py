@@ -37,7 +37,7 @@ __all__ = [
   "feature_transform", "expand_labels",
   "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
-  "parabolic_erode", "parabolic_dilate",
+  "parabolic_erode", "parabolic_dilate", "nearest_labels",
 ]
 
 FLAG_SQRT = 1
@@ -116,6 +116,11 @@ def _lib():
   lib.edtb200_parabolic.restype = ci
   lib.edtb200_parabolic_sites.argtypes = [vp, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
   lib.edtb200_parabolic_sites.restype = ci
+  lib.edtb200_nearest_labels.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ctypes.c_double, ci, ci, vp,
+                                         vp, ci, vp]
+  lib.edtb200_nearest_labels.restype = ci
+  lib.edtb200_nearest_labels_plan.argtypes = [ci, i64, i64, i64, f32, f32, f32, ctypes.c_double, ci, ci, vp, vp]
+  lib.edtb200_nearest_labels_plan.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1481,6 +1486,132 @@ parabolic_erode.__doc__ = """Parabolic (grayscale) erosion: g(p) = min_q f(q) + 
   (Felzenszwalb-Huttenlocher).  Its cost per voxel does not depend on the weights.""" + _PARABOLIC_DOC
 parabolic_dilate.__doc__ = """Parabolic (grayscale) dilation: g(p) = max_q f(q) - sum_a (w_a (p_a - q_a))^2, computed as
   -parabolic_erode(-f); NaN is never a site and zero results are +0.0.""" + _PARABOLIC_DOC
+
+
+# ---------------------------------------------------------------------------------------
+# the k nearest distinct labels of every voxel within a distance (edtb200_nearest_labels)
+# ---------------------------------------------------------------------------------------
+
+FLAG_NEAREST_SQUARED = 32      # EDTB200_NEAREST_SQUARED
+
+
+def _nearest_label_bytes(dtype):
+  """Label width of a numpy or torch integer / bool dtype; TypeError for anything else (floats included)."""
+  if isinstance(dtype, np.dtype):
+    if dtype == np.bool_ or (dtype.kind in "iu" and dtype.itemsize in (1, 2, 4, 8)):
+      return dtype.itemsize
+  else:
+    import torch
+    nbytes = _torch_label_bytes(torch).get(dtype)
+    if nbytes is not None:
+      return nbytes
+  raise TypeError("nearest_labels: labels must be an integer or bool dtype, got %s" % dtype)
+
+
+def nearest_labels(labels, max_distance, anisotropy=None, *, k=2, squared=False, stacked=False, device=0):
+  """The k nearest distinct labels of every voxel within max_distance, and how far away each is.
+
+  Returns (distances, nearest): float32 distances and labels of the input's dtype, both of shape
+  (k,) + labels.shape.  Entry q of a voxel is plane q, and each plane has the input's memory order (the
+  layout of feature_transform's indices).  Entries come in ascending distance; ties are ordered by the
+  label read as an unsigned integer of its width.  Where fewer than k labels lie within max_distance the
+  missing entries are distance +inf and label 0.  A labelled voxel's entry 0 is (0, its own label).
+
+  Definition.  Volumes are x-fastest: for C-ordered input the last axis is x, as for edt().  Every voxel
+  with a non-zero label is a site of that label; label 0 is background, whose voxels ask the query but are
+  never sites (there is no border term, so black_border does not apply).  For a voxel p and a label M,
+
+      D_M(p) = parabolic_erode(np.where(labels == M, 0, np.inf), anisotropy)[p]      (bit for bit)
+
+  -- one pass per axis in the order x, y, z, each candidate fl32(fl64(w2 * (i-j)^2) + fl64(g(j))) with
+  w2 = float32(w * w).  With integer weights and values below 2^24 it is exactly the squared Euclidean
+  distance from p to the nearest voxel of M.  B is the largest float32 with float64(B) <= max_distance^2
+  (the cut of the bounded transforms); only labels with D_M(p) <= B count.
+    values  the k distances of p are the k smallest D_M(p) over the distinct counted labels, exactly;
+            squared=True returns D, otherwise np.sqrt of it in float32 (correctly rounded, as edt).
+    labels  each pass keeps per voxel the k least (value, label) pairs with distinct labels: the X pass
+            sees the voxel itself at 0 and each labelled voxel j != i of its row at fl32(w2 * (i-j)^2),
+            every later pass its own row's list and row j's entries each raised to
+            fl32(fl64(w2 * (i-j)^2) + fl64(v)); a label keeps its least value, ties go to the smaller
+            unsigned label, pairs above B are dropped.  So the labels are the k least (D_M(p), M) pairs
+            wherever rounding merges no two candidates -- always, for integer weights and values below
+            2^24; otherwise a label can differ only among labels whose value equals the k-th value.
+  The values are exact although each pass keeps only k entries: a label dropped at an intermediate voxel
+  had k others no larger there, and each pass adds w2 * d^2 and rounds, which is monotone.
+
+  Worked use: the U-Net weight map of touching cells, w(p) = w0 * exp(-(d1 + d2)^2 / (2 sigma^2)) on the
+  background, d1 and d2 the distances to the nearest and second-nearest cell:
+      (d, _) = nearest_labels(cells, max_distance=3 * sigma, k=2)
+      w = np.where(cells == 0, w0 * np.exp(-(d[0] + d[1]) ** 2 / (2 * sigma ** 2)), 0)
+  (+inf beyond max_distance makes the weight 0 there, where it is below w0 * exp(-4.5) anyway.)  Contacts
+  between segments within r are the voxels where nearest[1] != 0 at max_distance=r, and Voronoi boundaries
+  between instances lie where d[1] - d[0] is small.
+
+  Arguments.  `labels`: 1-D to 3-D, or with stacked=True a 2-D to 4-D array whose slowest axis in memory
+  indexes same-shaped volumes, each on its own with one launch per pass for all of them.  Integer and bool
+  dtypes only: float labels raise TypeError.  `max_distance` must be finite and >= 0 (ValueError): each
+  pass costs O(R) per voxel, R = max_distance / w rows, and R may not exceed 256 rows (EDTError ELIMIT).
+  `anisotropy`: one weight per volume axis, finite and > 0.  `k`: 1 to 4.  numpy in gives numpy out, staged
+  through the GPU whole (a host array that does not fit raises EDTError with code ENOMEM; there is no
+  chunked path); a torch CUDA tensor (or any __cuda_array_interface__ array) gives torch CUDA tensors
+  computed on the current stream.  Device memory beyond the labels and the outputs: k * (4 + itemsize)
+  bytes per voxel in 2-D and 3-D, none in 1-D.
+  """
+  name = "nearest_labels"
+  if isinstance(k, (bool, np.bool_)) or not isinstance(k, (int, np.integer)) or not 1 <= int(k) <= 4:
+    raise ValueError("%s: k must be an integer from 1 to 4, got %r" % (name, k))
+  k = int(k)
+  d = float(max_distance)
+  if not (d >= 0.0 and d != float("inf")):
+    raise ValueError("%s: max_distance must be finite and zero or more, got %r" % (name, max_distance))
+  on_device = _device_array(labels)
+  arr = None if on_device is not None else np.asarray(labels)
+  nd = on_device.dim() if on_device is not None else arr.ndim
+  lo, hi = (2, 4) if stacked else (1, 3)
+  if not lo <= nd <= hi:
+    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
+  nbytes = _nearest_label_bytes(on_device.dtype if on_device is not None else arr.dtype)
+  vnd = nd - 1 if stacked else nd
+  weights = _surface_anisotropy(vnd, anisotropy)
+  for w in weights:
+    if not (np.isfinite(w) and w > 0.0):
+      raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (name, anisotropy))
+  flags = 0 if not squared else FLAG_NEAREST_SQUARED
+  lib = _lib()
+  if on_device is None:
+    arr, order = _stack_order(arr)
+    planes = arr.shape if order == "C" else arr.shape[::-1]
+    back = (0,) + (tuple(range(1, nd + 1)) if order == "C" else tuple(range(nd, 0, -1)))
+    dist = np.empty((k,) + planes, np.float32).transpose(back)
+    near = np.empty((k,) + planes, arr.dtype).transpose(back)
+    if arr.size:
+      if stacked:
+        count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
+      else:
+        count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
+      _check(lib.edtb200_nearest_labels(arr.ctypes.data, nbytes, vnd, sx, sy, sz, count, wx, wy, wz, d, k, flags,
+                                        dist.ctypes.data, near.ctypes.data, int(device), None))
+    return dist, near
+  import torch
+  t = on_device
+  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
+  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
+    t = t.permute(*reversed(range(nd)))
+    weights = tuple(reversed(weights))
+  else:
+    t = t.contiguous()
+  dist = torch.empty((k,) + tuple(t.shape), dtype=torch.float32, device=t.device)
+  near = torch.empty((k,) + tuple(t.shape), dtype=t.dtype, device=t.device)
+  if t.numel():
+    count = int(t.shape[0]) if stacked else 1
+    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
+    stream = ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
+    _check(lib.edtb200_nearest_labels(t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, d, k,
+                                      flags | FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, dist.data_ptr(),
+                                      near.data_ptr(), t.device.index, stream))
+  if fortran:
+    return dist.permute(0, *range(nd, 0, -1)), near.permute(0, *range(nd, 0, -1))
+  return dist, near
 
 
 # ---------------------------------------------------------------------------------------

@@ -1881,6 +1881,101 @@ int edtb200_parabolic_sites(const float* f, int ndim, int64_t sx, int64_t sy, in
   return parabolic_any(f, ndim, sx, sy, sz, count, wx, wy, wz, op, flags, out, true, idx, device, stream_v);
 }
 
+// The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
+static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
+                          const float w[3], int k, double max_distance) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  for (int a = 0; a < ndim; ++a)
+    if (!(std::isfinite(w[a]) && w[a] > 0.0f))
+      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", a, (double)w[a]);
+  if (k < 1 || k > 4) return fail(EDTB200_EINVAL, "k must be 1, 2, 3 or 4 (got %d)", k);
+  if (!(max_distance >= 0.0) || std::isinf(max_distance))
+    return fail(EDTB200_EINVAL, "max_distance must be finite and zero or more (got %g): the cost is O(R) per voxel "
+                "per pass, so an unbounded call is not offered", max_distance);
+  return 0;
+}
+
+int edtb200_nearest_labels_plan(int ndim, int64_t sx, int64_t sy, int64_t sz, float wx, float wy, float wz,
+                                double max_distance, int k, int label_bytes, int64_t radius[3], int variant[3]) {
+  const float w[3] = {wx, wy, wz};
+  int rc = nearest_checks(label_bytes, ndim, sx, sy, sz, 1, w, k, max_distance);
+  if (rc) return rc;
+  if (!radius || !variant) return fail(EDTB200_EINVAL, "null pointer");
+  const NearestPlan p = nearest_plan(ndim, w, max_distance, k, label_bytes);
+  for (int a = 0; a < 3; ++a) {
+    radius[a] = p.radius[a];
+    variant[a] = p.variant[a];
+  }
+  return 0;
+}
+
+int edtb200_nearest_labels(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                           int64_t count, float wx, float wy, float wz, double max_distance, int k, int flags,
+                           float* dist_out, void* label_out, int device, void* stream_v) {
+  const float w[3] = {wx, wy, wz};
+  int rc = nearest_checks(label_bytes, ndim, sx, sy, sz, count, w, k, max_distance);
+  if (rc) return rc;
+  const NearestPlan p = nearest_plan(ndim, w, max_distance, k, label_bytes);
+  for (int a = 0; a < ndim; ++a)
+    if (p.variant[a] < 0)
+      return fail(EDTB200_ELIMIT, "the pass along axis %d needs a radius of %lld rows; the limit is %lld", a,
+                  (long long)p.radius[a], (long long)kNearRadiusLimit);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE | EDTB200_NEAREST_SQUARED))
+    return fail(EDTB200_EINVAL, "edtb200_nearest_labels takes only the residency flags and EDTB200_NEAREST_SQUARED "
+                "(got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if (vol > 0 && count > ((int64_t)1 << 62) / (vol * k)) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !dist_out || !label_out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
+  const size_t dist_bytes = sizeof(float) * (size_t)total * (size_t)k, lout_bytes = lab_bytes * (size_t)k;
+  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
+  };
+  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
+  if (overlap(dist_out, dist_bytes, label_out, lout_bytes)) return fail(EDTB200_EINVAL, "dist_out overlaps label_out");
+  if (same_side && (overlap(labels, lab_bytes, dist_out, dist_bytes) || overlap(labels, lab_bytes, label_out, lout_bytes)))
+    return fail(EDTB200_EINVAL, "an output overlaps labels");
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  // host buffers are staged whole: the labels and distances through this device's cached buffers, the
+  // output labels through scratch
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, dist_bytes));
+  float* d_dist = io.out(dist_out, dist_bytes, dc->dist);
+  Scratch staged, planes;
+  if (!io.out_dev && staged.alloc(*dc, lout_bytes, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the output labels");
+  }
+  void* d_lab = io.out(label_out, lout_bytes, io.out_dev ? nullptr : staged.get());
+  // the scratch set of the passes: k value and label planes (2-D and 3-D)
+  float* sdist = nullptr;
+  void* slab = nullptr;
+  if (ndim > 1) {
+    // the value planes from a 16-byte boundary after the label planes, which may end anywhere
+    const size_t at = (lout_bytes + 15) & ~(size_t)15;
+    if (planes.alloc(*dc, at + dist_bytes, s) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(EDTB200_ENOMEM, "no device memory for the passes' scratch planes");
+    }
+    slab = planes.get();
+    sdist = reinterpret_cast<float*>(planes.get<char>() + at);
+  }
+  rc = nearest_passes(d_labels, label_bytes, ndim, sx, sy, sz, count, w, p, k, !(flags & EDTB200_NEAREST_SQUARED),
+                      d_dist, d_lab, sdist, slab, *dc, s);
+  return rc ? rc : io.finish();
+}
+
 int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                           int64_t count, const float* sqdist, const int32_t* const* idx, double limit_sq, int flags,
                           void* out, int device, void* stream_v) {

@@ -1,12 +1,12 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as ten translation units so that the kernel templates build in
+// The library is compiled as eleven translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
 // transforms' kernels), edt_surface.cu (the surface distances' kernels), edt_morphology.cu (the
-// spherical morphology's label-writing stores) and edt_parabolic.cu (the parabolic erosion and
-// dilation passes).  The run-time label width
+// spherical morphology's label-writing stores), edt_parabolic.cu (the parabolic erosion and
+// dilation passes) and edt_nearest.cu (the nearest-labels passes).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -251,6 +251,26 @@ int launch_later_window(const void* labels, const float* fin, float* fout, int* 
 template <int Bytes>
 int launch_bounded_cut(const void* labels, float* f, int* codes, int64_t total, float bound, int flags,
                        DeviceCache& dc, cudaStream_t stream);
+
+// The plan of edtb200_nearest_labels (edt_nearest.cu): the bound B and radii R_a of bounded_plan, and
+// per axis the kernel its pass takes -- kNearRowsPass (the X pass), kNearStaged or kNearGlobal (a later
+// pass whose window tile fits kNearSmemLimit bytes of shared memory, or not), -1 for an axis >= ndim or
+// a radius above kNearRadiusLimit.
+constexpr int kNearRowsPass = EDTB200_NEAREST_ROWS, kNearStaged = EDTB200_NEAREST_STAGED,
+              kNearGlobal = EDTB200_NEAREST_GLOBAL;
+constexpr int64_t kNearRadiusLimit = 256;
+constexpr size_t kNearSmemLimit = 232448;      // the opt-in shared memory of a CTA on sm_90
+struct NearestPlan {
+  float bound = 0.0f;
+  int64_t radius[3] = {0, 0, 0};
+  int variant[3] = {-1, -1, -1};
+};
+NearestPlan nearest_plan(int ndim, const float w[3], double max_distance, int k, int label_bytes);
+// The passes of edtb200_nearest_labels over `count` volumes on the device: k value and label planes to
+// dist / lab, through the scratch planes sdist / slab (2-D and 3-D); root: sqrtf in the last store.
+int nearest_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                   const float w[3], const NearestPlan& p, int k, bool root, float* dist, void* lab, float* sdist,
+                   void* slab, DeviceCache& dc, cudaStream_t stream);
 
 }  // namespace host
 

@@ -37,7 +37,7 @@ extern "C" {
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
- * edtb200_parabolic, edtb200_parabolic_sites)
+ * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -312,6 +312,70 @@ int edtb200_parabolic(const float *f, int ndim, int64_t sx, int64_t sy, int64_t 
 int edtb200_parabolic_sites(const float *f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
                             float wx, float wy, float wz, int op, int flags, float *out,
                             int32_t *idx, int device, void *stream);
+
+/* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
+ * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between
+ * segments, Voronoi boundaries where d2 - d1 is small).
+ *
+ * Sites: every voxel with a non-zero label is a site of that label; label 0 is background, whose voxels
+ * ask the query but are never sites.  There is no border term.  For a voxel p and a label M,
+ *     D_M(p) = edtb200_parabolic's erosion of (0 on the voxels of M, +inf elsewhere) at p, bit for bit:
+ * one pass per axis in the order x, y, z, each candidate fl32(fl64(w2 (i-j)^2) + fl64(g(j))) with
+ * w2 = fl64(fl32(w * w)).  With integer weights and values below 2^24 it is exactly the squared distance
+ * from p to the nearest voxel of M.  B is the largest float32 with (double)B <= (double)d * d, the B of the
+ * bounded transforms; only labels with D_M(p) <= B count.
+ *   values  the k distances of p, ascending, are the k smallest D_M(p) over the distinct counted labels M;
+ *           where fewer than k labels count, the missing entries are +inf with label 0.
+ *   labels  are fixed by the per-pass rule: the X pass sees the voxel itself at 0 (when its label is
+ *           non-zero) and each site j != i within its window at fl32(w2 (i-j)^2); every later pass sees its
+ *           own row's list unchanged and row j's entries each as fl32(fl64(w2 (i-j)^2) + fl64(v)); each pass
+ *           keeps per voxel the k least (value, label) pairs with distinct labels -- a label keeps its least
+ *           value, ties are ordered by the label read as an unsigned integer of its width, pairs above B are
+ *           dropped -- and stores them in that order.  So the labels are the k least (D_M(p), M) pairs
+ *           wherever no rounding merges two candidates, which always holds for integer weights with values
+ *           below 2^24; otherwise a label can differ only among labels whose value equals the k-th value.
+ * The values are exact because the per-pass truncation is: a label B dropped at an intermediate voxel q on
+ * the path of its least value at p had k other labels no larger at q, and each pass adds w2 d^2 and rounds,
+ * which is monotone, so those k are no larger at p either.  A voxel of label A has entry 0 = (0, A).
+ *
+ *   labels     count * sx*sy*sz labels of label_bytes (1, 2, 4 or 8) bytes, volumes back to back as for
+ *              edtb200_transform_stack (count 1: one volume), each on its own
+ *   wx..wz     the weights of the first ndim axes: finite and > 0
+ *   max_distance  d, finite and >= 0: the cost is O(R) per voxel per pass, so there is no unbounded call
+ *   k          1 to 4
+ *   flags      the residency flags (both on the device: asynchronous on `stream`; host buffers are staged
+ *              whole, EDTB200_ENOMEM when they do not fit -- there is no chunked path) and
+ *              EDTB200_NEAREST_SQUARED: the values D; without it sqrtf of each, correctly rounded, as edt
+ *   dist_out   k x-fastest float32 planes of count * sx*sy*sz voxels, back to back (entry q of every voxel
+ *              is plane q)
+ *   label_out  k planes of labels of label_bytes, laid out as dist_out; neither output may overlap the
+ *              other or the labels
+ * Kernels: the X pass stages runs of voxels with R_x labels either side in shared memory; each later pass
+ * walks a window of R_a rows either side with lanes on 32 adjacent lines, staged in shared memory when
+ * (64 + 2 R_a) 32 k (4 + label_bytes) bytes fit the 227 KB of a CTA and read from global memory otherwise
+ * (equal bit for bit).  R_a is the bounded transforms' radius (edtb200_bounded_plan) and may not exceed
+ * 256 rows.  The passes write out of place: 3-D X -> out, Y -> scratch, Z -> out; 2-D X -> scratch,
+ * Y -> out; 1-D X -> out.  So the device memory beyond the labels and the outputs is k (4 + label_bytes)
+ * bytes per voxel in 2-D and 3-D, and none in 1-D.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, weights, k, max_distance,
+ * a pass radius above 256 (EDTB200_ELIMIT), flags, the stack's size (within 2^62 values), emptiness
+ * (returns 0 touching nothing), pointers and overlap, device. */
+#define EDTB200_NEAREST_SQUARED 32
+int edtb200_nearest_labels(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                           int64_t count, float wx, float wy, float wz, double max_distance, int k, int flags,
+                           float *dist_out, void *label_out, int device, void *stream);
+
+/* The plan of edtb200_nearest_labels, pure host logic (no device needed): radius[a] = R_a, the bounded
+ * transforms' rule (the largest r with (double)w2_a r^2 < nextafterf(B, +inf), as edtb200_bounded_plan
+ * gives it), and variant[a] the kernel of the pass along axis a: EDTB200_NEAREST_ROWS (the X pass),
+ * EDTB200_NEAREST_STAGED or EDTB200_NEAREST_GLOBAL (a later pass with its window in shared memory or read
+ * from global memory), -1 for an axis a >= ndim (radius 0) or a radius above 256, which the call refuses.
+ * Checks, in order: as edtb200_nearest_labels up to max_distance, then the pointers. */
+#define EDTB200_NEAREST_ROWS   0
+#define EDTB200_NEAREST_STAGED 1
+#define EDTB200_NEAREST_GLOBAL 2
+int edtb200_nearest_labels_plan(int ndim, int64_t sx, int64_t sy, int64_t sz, float wx, float wy, float wz,
+                                double max_distance, int k, int label_bytes, int64_t radius[3], int variant[3]);
 
 /* A stack of `count` volumes of one geometry (sx, sy, sz), laid back to back (volume b starts at
  * voxel b * sx * sy * sz), each transformed on its own as edtb200_transform would: its result is

@@ -138,6 +138,15 @@ for shape, w in (((5, 33, 37), (0.7, 1.3, 2.9)), ((3, 1100), (1.0, 0.7)), ((1100
   for op in ("erode", "dilate"):
     f = pc.values("special", shape, rng)
     check("parabolic %s %s" % (op, shape), getattr(edt, "parabolic_" + op)(f, w), pc.restate(op, f, w))
+# nearest labels: the X kernel and both later-pass variants (staged, global) on ragged tiles, every k and
+# width, against the per-pass restatement
+import nearest_labels_cases as nlc  # noqa: E402
+for shape, d, k, dtype in (((5, 33, 37), 3.5, 2, np.uint32), ((3, 70, 9), 50.0, 4, np.uint64), ((70,), 6.0, 3, np.int8),
+                           ((9, 66), 4.0, 1, np.uint16)):
+  lab = nlc.volume("seeds", shape, dtype, rng)
+  got, want = edt.nearest_labels(lab, d, k=k, squared=True), nlc.per_pass(lab, d, None, k)
+  check("nearest_labels %s k=%d" % (shape, k), got[0], want[0])
+  check("nearest_labels labels %s k=%d" % (shape, k), got[1], want[1])
 # per-label views: a nearly full table whose probe chain wraps past its end, a table that overflows, and
 # a sub-box drawn at a ragged row length; the helpers are the GPU tests' own
 import each_cases as ec  # noqa: E402

@@ -1881,6 +1881,126 @@ int edtb200_parabolic_sites(const float* f, int ndim, int64_t sx, int64_t sy, in
   return parabolic_any(f, ndim, sx, sy, sz, count, wx, wy, wz, op, flags, out, true, idx, device, stream_v);
 }
 
+int edtb200_medial_axis(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                        int64_t count, float wx, float wy, float wz, int black_border, int flags, uint8_t* medial_out,
+                        float* dist_out, int device, void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  const float w[3] = {wx, wy, wz};
+  for (int k = 0; k < ndim; ++k)
+    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
+      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE | EDTB200_LABELS_FLOAT))
+    return fail(EDTB200_EINVAL, "edtb200_medial_axis takes only the residency flags and EDTB200_LABELS_FLOAT (got %d)",
+                flags);
+  const bool as_float = flags & EDTB200_LABELS_FLOAT;
+  if (as_float && label_bytes != 4 && label_bytes != 8)
+    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
+  const int64_t vol = sx * sy * sz;
+  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  // the sites' limit: beyond it (i-j)^2 is not exact in double on the brute-force lines
+  if (sx > kParabolicSitesN || sy > kParabolicSitesN || sz > kParabolicSitesN)
+    return fail(EDTB200_ELIMIT, "edtb200_medial_axis takes lines of at most 2^26 samples");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !medial_out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, dist_bytes = sizeof(float) * (size_t)total;
+  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
+  };
+  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
+  if (same_side && overlap(labels, lab_bytes, medial_out, (size_t)total)) return fail(EDTB200_EINVAL, "medial_out overlaps labels");
+  if (dist_out && same_side && overlap(labels, lab_bytes, dist_out, dist_bytes))
+    return fail(EDTB200_EINVAL, "dist_out overlaps labels");
+  if (dist_out && overlap(medial_out, (size_t)total, dist_out, dist_bytes))
+    return fail(EDTB200_EINVAL, "dist_out overlaps medial_out");
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  // host buffers are staged whole: the labels and distances through this device's cached buffers, the
+  // mask through scratch
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  Scratch staged, values, planes;
+  if (!io.out_dev && staged.alloc(*dc, (size_t)total, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the medial mask");
+  }
+  uint8_t* d_medial = io.out(medial_out, (size_t)total, staged.get<uint8_t>());
+  float* d_dist = nullptr;
+  if (dist_out) {
+    if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, dist_bytes));
+    d_dist = io.out(dist_out, dist_bytes, dc->dist);
+  }
+  // scratch: one value volume (D^2 without distances, the dilation's values with them) and the code
+  // planes, which hold the folded float labels until the edtsq has read them
+  const size_t plane_bytes = std::max(dist_bytes * (size_t)ndim, as_float ? lab_bytes : 0);
+  if (values.alloc(*dc, dist_bytes, s) != cudaSuccess || planes.alloc(*dc, plane_bytes, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the medial axis's scratch");
+  }
+  const void* runs = d_labels;                   // the labels the edtsq compares
+  if (as_float) {
+    if ((rc = launch_fold_float_labels(d_labels, label_bytes, planes.get(), total, *dc, s))) return rc;
+    runs = planes.get();
+  }
+  float* d2 = d_dist ? d_dist : values.get<float>();
+  int* codes[3] = {nullptr, nullptr, nullptr};
+  for (int k = 0; k < ndim; ++k) codes[k] = planes.get<int>() + (size_t)k * total;
+
+  // EDT_B200_VERBOSE=1: per-step device times and kernels on stderr (synchronises the stream)
+  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
+  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  if (verbose)
+    for (int k = 0; k < 6; ++k)
+      if (cudaEventCreate(&ev[k]) == cudaSuccess && k == 0) cudaEventRecord(ev[0], s);
+  rc = run_passes(runs, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2, *dc, s, count);
+  if (ev[1]) cudaEventRecord(ev[1], s);
+  int kernel[3] = {-1, -1, -1};
+  const float* src = d2;                         // with distances the first pass writes the value scratch
+  float* dst = values.get<float>();
+  for (int k = 0; !rc && k < ndim; ++k) {
+    edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz, count);
+    if (k == 0) {                                // rows of sx contiguous samples
+      g.outer_count = sy * sz * count; g.outer_stride = sx; g.inner_count = 1; g.line_stride = 1; g.n = (int)sx;
+    }
+    rc = launch_parabolic_pass(src, dst, g, k == 0, w[k], /*dilate=*/true, *dc, s, &kernel[k], codes[k]);
+    if (ev[k + 2]) cudaEventRecord(ev[k + 2], s);
+    src = dst;
+  }
+  if (!rc && cudaMemsetAsync(d_medial, 0, (size_t)total, s) != cudaSuccess)
+    rc = fail(EDTB200_ECUDA, "cudaMemsetAsync of the medial mask failed");
+  if (!rc)
+    rc = launch_medial_mark(d_labels, label_bytes, codes, ndim, sx, sy, sz, count, as_float, d_medial, d_dist, *dc, s);
+  if (ev[5]) cudaEventRecord(ev[5], s);
+  if (verbose) {
+    static const char* names[4] = {"tile", "long", "brute", "copy"};
+    float ms[5] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+    if (!rc && cudaEventSynchronize(ev[5]) == cudaSuccess) {
+      int at = 0;                                // the event before each step
+      for (int k = 1; k <= 5; ++k) {
+        if (k >= 2 && k <= 4 && k - 2 >= ndim) continue;
+        if (ev[at] && ev[k]) cudaEventElapsedTime(&ms[k - 1], ev[at], ev[k]);
+        at = k;
+      }
+      fprintf(stderr, "[edt_b200] medial_axis %lldx%lldx%lld x%lld L=%d  edtsq %.3f ms  x %.3f ms (%s)  y %.3f ms (%s)  "
+                      "z %.3f ms (%s)  mark %.3f ms\n",
+              (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, ms[0], ms[1],
+              names[kernel[0] < 0 ? 0 : kernel[0]], ms[2], kernel[1] < 0 ? "-" : names[kernel[1]], ms[3],
+              kernel[2] < 0 ? "-" : names[kernel[2]], ms[4]);
+    }
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+    cudaGetLastError();
+  }
+  return rc ? rc : io.finish();
+}
+
 // The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
 static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
                           const float w[3], int k, double max_distance) {

@@ -1,12 +1,13 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as eleven translation units so that the kernel templates build in
+// The library is compiled as twelve translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
 // transforms' kernels), edt_surface.cu (the surface distances' kernels), edt_morphology.cu (the
 // spherical morphology's label-writing stores), edt_parabolic.cu (the parabolic erosion and
-// dilation passes) and edt_nearest.cu (the nearest-labels passes).  The run-time label width
+// dilation passes), edt_nearest.cu (the nearest-labels passes) and edt_medial.cu (the medial
+// axis's mark kernel).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -319,6 +320,13 @@ int launch_fold_float_labels(const void* in, int label_bytes, void* out, int64_t
 constexpr int64_t kParabolicSitesN = (int64_t)1 << 26;
 int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool rows, float w, bool dilate,
                           DeviceCache& dc, cudaStream_t stream, int* kernel, int* codes = nullptr);
+
+// The medial axis's last step over `count` volumes of (sx, sy, sz) (edt_medial.cu): every labelled voxel
+// (as_float: 4- / 8-byte IEEE labels, -0.0 is background) follows the parabolic passes' codes to its site
+// and sets medial there; dist non-null: D^2 in place -> its correctly rounded sqrt.
+int launch_medial_mark(const void* labels, int label_bytes, const int* const codes[3], int ndim, int64_t sx,
+                       int64_t sy, int64_t sz, int64_t count, bool as_float, uint8_t* medial, float* dist,
+                       DeviceCache& dc, cudaStream_t stream);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

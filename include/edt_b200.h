@@ -37,7 +37,8 @@ extern "C" {
  * Entry points added since (edtb200_transform_chunked, edtb200_feature_transform_chunked,
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
- * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan)
+ * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
+ * edtb200_medial_axis)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -312,6 +313,60 @@ int edtb200_parabolic(const float *f, int ndim, int64_t sx, int64_t sy, int64_t 
 int edtb200_parabolic_sites(const float *f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
                             float wx, float wy, float wz, int op, int flags, float *out,
                             int32_t *idx, int device, void *stream);
+
+/* The medial axis of every label at once: the balls that rebuild each label exactly, the input of the
+ * reverse distance transform (edtb200_parabolic's dilation of D^2 on the medial voxels, -inf elsewhere).
+ * For labels L (0 is background) with weights w and black_border:
+ *   1. D2 = edtb200_transform's edtsq of L (with black_border), bit for bit;
+ *   2. (V, q) = edtb200_parabolic_sites' dilation of D2 as it is -- 0 on the background, not masked to
+ *      -inf -- so q(p) is p's power (Laguerre) site, the maximiser of D2(y) - |p - y|^2_w;
+ *   3. medial[y] = 1 iff y = q(p) for some voxel p with L(p) != 0.
+ * The tie rule is edtb200_parabolic_sites': on lines of at most 23170 samples each pass takes the least j
+ * among the REAL maximisers.  With integer weights and values below 2^24 nothing rounds, and q(p) is the
+ * lexicographically least (z, y, x) among the real maximisers of D2(y) - |p - y|^2_w over the volume, x
+ * the fastest axis in memory (so a caller's memory order decides which of tied maximisers is marked).  The
+ * marked set is the reduced discrete medial axis (Coeurjolly & Montanvert, 2007): the balls B(y, D(y))
+ * that are the power maximiser of at least one labelled voxel.  It is neither thin nor connected: not a
+ * topological skeleton and not the minimal medial axis.
+ *   reconstruction  for any weights, at every p with L(p) != 0, the dilation of (D2 on medial, -inf
+ *                   elsewhere) equals V(p) bit for bit and is > 0: it is <= V(p) because every pass is
+ *                   monotone, and >= the chain of rounded candidates from q(p), which is medial and, by the
+ *                   sites' definition, gives V(p).
+ *   integer weights the reconstruction is <= 0 on every background voxel, so "> 0" is exactly L != 0; q(p)
+ *                   carries L(p); per label M the balls of M's medial voxels rebuild exactly the voxels of M,
+ *                   so every non-empty label has a medial voxel.
+ * Examples (1-D, background on both sides): a run of 5 has D2 = 1 4 9 4 1 and medial {2}; a run of 4 has
+ * D2 = 1 4 4 1 and medial {1, 2}.  A volume of one non-zero label without black_border has D2 = +inf, and
+ * its only medial voxel is its first one (a -inf line takes its first -inf position).
+ *
+ *   labels      count * sx*sy*sz labels of label_bytes (1, 2, 4 or 8) bytes, volumes back to back as for
+ *               edtb200_transform_stack (count 1: one volume), each on its own; q(p) lies in p's volume
+ *   wx..wz      the weights of the first ndim axes: finite and > 0
+ *   flags       the residency flags (both on the device: asynchronous on `stream`, no lock and no host wait;
+ *               host buffers are staged whole, EDTB200_ENOMEM when they do not fit -- there is no chunked
+ *               path), and EDTB200_LABELS_FLOAT for 4- / 8-byte IEEE labels: -0.0 is then background and
+ *               compares equal to +0.0, as in edtb200_morphology
+ *   medial_out  count * sx*sy*sz bytes, 0 or 1
+ *   dist_out    NULL, or count * sx*sy*sz float32: edt (sqrt of D2, correctly rounded), bit for bit
+ *               edtb200_transform's with EDTB200_SQRT; on the same side as medial_out
+ * Kernels, on one stream: the edtsq of the stack (one launch per pass, into dist_out or scratch), the
+ * parabolic dilation with site codes (edtb200_parabolic_sites' instances; with distances the X pass runs
+ * out of place from D2 into a value scratch, without them every pass runs in place over the D2 scratch;
+ * the codes go to one plane per axis and no index plane is written), then the mask is zeroed and
+ * medial_mark_kernel has every labelled voxel follow its codes to q(p) and store 1 there, taking the
+ * square root of dist_out in the same pass.  Device memory beyond the labels and the outputs: 4 + 4 ndim
+ * bytes per voxel (16 in 3-D: one value volume and ndim code planes; the folded labels of
+ * EDTB200_LABELS_FLOAT live in the code planes until the edtsq has read them, so a 1-D call with 8-byte
+ * float labels takes 4 + 8), plus the edtsq's long-line scratch where its plan takes that kernel, the
+ * parabolic long-line hull on lines of 1025 to 23170 samples, and the staged host buffers.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, weights, flags,
+ * EDTB200_LABELS_FLOAT width, the stack's size (within 2^62 voxels), the line length (a line of more than
+ * 2^26 samples is EDTB200_ELIMIT, as for edtb200_parabolic_sites), emptiness (returns 0 touching nothing),
+ * pointers (labels, medial_out) and overlap (neither output may overlap the labels when on the same side,
+ * nor the other output), device.  EDT_B200_VERBOSE=1 prints each step's device time on stderr. */
+int edtb200_medial_axis(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                        int64_t count, float wx, float wy, float wz, int black_border, int flags,
+                        uint8_t *medial_out, float *dist_out, int device, void *stream);
 
 /* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
  * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between

@@ -147,6 +147,13 @@ for shape, d, k, dtype in (((5, 33, 37), 3.5, 2, np.uint32), ((3, 70, 9), 50.0, 
   got, want = edt.nearest_labels(lab, d, k=k, squared=True), nlc.per_pass(lab, d, None, k)
   check("nearest_labels %s k=%d" % (shape, k), got[0], want[0])
   check("nearest_labels labels %s k=%d" % (shape, k), got[1], want[1])
+# medial axis: the mark kernel over a stack, with and without distances, float labels, against the restatement
+import medial_axis_cases as mac  # noqa: E402
+for shape, dtype, stacked in (((4, 9, 11, 7), np.uint16, True), ((13, 30), np.float32, False), ((50,), np.int8, False)):
+  lab = (rng.integers(0, 3, shape) * (rng.random(shape) < 0.9)).astype(dtype)
+  got, dist = edt.medial_axis(lab, None, True, return_distance=True, stacked=stacked)
+  check("medial_axis %s" % (shape,), got, mac.restate(lab, None, True, stacked=stacked)[0])
+  check("medial_axis only %s" % (shape,), edt.medial_axis(lab, None, True, stacked=stacked), got)
 # per-label views: a nearly full table whose probe chain wraps past its end, a table that overflows, and
 # a sub-box drawn at a ragged row length; the helpers are the GPU tests' own
 import each_cases as ec  # noqa: E402

@@ -312,12 +312,15 @@ __device__ __forceinline__ uint32_t nibbles_to_word(uint32_t nib, int lane) {
 // Plain = false: behaviour selected by `flags` at run time.
 // Settled = true (first_axis_planes_kernel only): also clears bit b of set_y / set_z where a value
 // stored for the lane's four voxels of block b exceeds ty / tz (lanes past sx leave theirs set).
-template <int Bytes, int K, bool Plain, bool Settled = false, class Load>
+// OneRowY = true (first_axis_planes_kernel only): stores min(f, ty) for the voxels marked in one_row
+// (4 bits per block, like the masks below), before the settled compare: the voxels whose y-run is
+// one row long, which the Y pass would bring to exactly that value (DESIGN.md section 4.1).
+template <int Bytes, int K, bool Plain, bool Settled = false, bool OneRowY = false, class Load>
 __device__ __forceinline__ void first_axis_vec_row(Load load, float* __restrict__ dst, int sx, const float* table_s,
                                                    int border, int flags, bool keep_background, int lane,
                                                    unsigned lt_mask, unsigned gt_mask, unsigned int& nstarts,
                                                    float ty = 0.0f, float tz = 0.0f, uint32_t* set_y = nullptr,
-                                                   uint32_t* set_z = nullptr) {
+                                                   uint32_t* set_z = nullptr, uint32_t one_row = 0u) {
   using WT = typename LabelOf<Bytes>::wide;
   const unsigned full = 0xffffffffu;
 
@@ -415,6 +418,12 @@ __device__ __forceinline__ void first_axis_vec_row(Load load, float* __restrict_
       float val = table_s[k];
       if (!Plain) val = finish_value(val, background, flags);
       r[e] = val;
+    }
+    if constexpr (OneRowY) {
+      const uint32_t s = (one_row >> (4 * b)) & 15u;
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if ((s >> e) & 1u) r[e] = fminf(r[e], ty);
     }
     if constexpr (Settled) {                          // one compare per block and plane
       const float most = fmaxf(fmaxf(r[0], r[1]), fmaxf(r[2], r[3]));
@@ -618,6 +627,13 @@ __device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
 // z > 0, is preceded by one extra stage that is only compared against).  In 2-D every item is a
 // band of its own and the halo row is the previous band's last.  Items are split evenly over one
 // persistent wave of CTAs.
+// A voxel whose y-run is one row long (its label differs from rows y - 1 and y + 1, or the line ends
+// there) leaves the Y pass at exactly min(f, w2): the run's own sample and the border term w2 * 1^2 of
+// the label change or line end next to it, which a line of sy >= 2 rows always has on one side -- also
+// at rows 0 and sy - 1 without black_border.  The kernel stores that value already (ty = w2), so such
+// voxels end the X pass settled for the Y pass.  A band's last row does so only where it is the line's
+// last row: its row y + 1 is not staged, and the Y pass settles its runs (staging it as well, W+2 rows
+// per stage, was measured no faster on the 512^3 label-noise transform, DESIGN.md section 4.1).
 //
 // Shared memory: S mbarriers (64 bytes), the ring of S stages of (W+1)*sx labels, the step table.
 // ---------------------------------------------------------------------------------------
@@ -642,6 +658,12 @@ __device__ __forceinline__ void load4_shared(const typename LabelOf<Bytes>::type
 }
 
 constexpr int kPlaneBarBytes = 64;     // room for the ring's mbarriers (S <= 8)
+
+// Labels a[0..3] against b[0..3]: bit e set where they differ.
+template <class WT>
+__device__ __forceinline__ uint32_t label_changes(const WT a[4], const WT b[4]) {
+  return (a[0] != b[0] ? 1u : 0u) | (a[1] != b[1] ? 2u : 0u) | (a[2] != b[2] ? 4u : 0u) | (a[3] != b[3] ? 8u : 0u);
+}
 
 // Planes: 1 the y plane, 2 the y and z planes.  The ring's depth S is `stages`; W is blockDim.x / 32.
 // Registers capped at the CTAs per SM that the ring leaves room for with 8 warps, 3 stages and 512-voxel
@@ -717,10 +739,29 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
       // this row is row warp + 1 of its stage (row 0: the halo row y - 1)
       const LT* cur = ring + (size_t)slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
       const LT* back = ring + (size_t)prev_slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
+      // ---- the row against rows y - 1 and y + 1, 4 bits per block: a y-run starts here (the y
+      // plane's bits) / at the next row (the line end counts); both: a y-run of one row.  Row y + 1
+      // is in the stage except for the band's last row ----
+      const bool next_staged = y + 1 < sy && warp + 1 < warps;
+      uint32_t ystart = 0u, ynext = 0u;
+#pragma unroll
+      for (int b = 0; b < K; ++b) {
+        const int q0 = (b << 7) + (lane << 2);
+        if (q0 >= sx) continue;
+        WT here[4], u[4];
+        load4_shared<Bytes>(cur + q0, here);
+        uint32_t s = 15u, e = (y + 1 == sy) ? 15u : 0u;            // first row along y: all start
+        if (y > 0) { load4_shared<Bytes>(cur - sx + q0, u); s = label_changes<WT>(u, here); }
+        if (next_staged) { load4_shared<Bytes>(cur + sx + q0, u); e = label_changes<WT>(u, here); }
+        ystart |= s << (4 * b);
+        ynext |= e << (4 * b);
+      }
+      const uint32_t one_row = sy > 1 ? (ystart & ynext) : 0u;     // lines of one row have no border term
       uint32_t set_y = 0xffffffffu, set_z = 0xffffffffu;
-      first_axis_vec_row<Bytes, K, Plain, true>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); },
-                                                out + line * sx, sx, table_s, border, flags, keep_background, lane,
-                                                lt_mask, gt_mask, nstarts, planes.ty, planes.tz, &set_y, &set_z);
+      first_axis_vec_row<Bytes, K, Plain, true, true>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); },
+                                                      out + line * sx, sx, table_s, border, flags, keep_background,
+                                                      lane, lt_mask, gt_mask, nstarts, planes.ty, planes.tz, &set_y,
+                                                      &set_z, one_row);
       // ---- settled planes: segment 4 b + w of the row is lanes 8 w .. 8 w + 7 of block b ----
       uint32_t seg_y = 0u, seg_z = 0u;
 #pragma unroll
@@ -738,25 +779,28 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
         planes.settled_y[line] = seg_y | (0xffffffffu << (4 * K));
         if (Planes == 2) planes.settled_z[line] = seg_z | (0xffffffffu << (4 * K));
       }
-      // ---- run-start planes: compare with rows (y - 1, z) and (y, z - 1); one nibble per lane and
-      // block -> the row's wpr words, word c in lane c, stored by one instruction per plane ----
+      // ---- run-start planes: the y nibbles from above, the z ones compare with row (y, z - 1); one
+      // nibble per lane and block -> the row's wpr words, word c in lane c, stored by one instruction
+      // per plane ----
       uint32_t word[Planes] = {};
 #pragma unroll
       for (int b = 0; b < K; ++b) {
         const int q0 = (b << 7) + (lane << 2);
         const bool in_row = q0 < sx;
-        WT here[4], u[Planes][4];
-        if (in_row) {
-          load4_shared<Bytes>(cur + q0, here);
-          load4_shared<Bytes>(cur - sx + q0, u[0]);
-          if (Planes == 2) load4_shared<Bytes>(back + q0, u[Planes - 1]);
+        uint32_t nibs[Planes];
+        nibs[0] = (ystart >> (4 * b)) & 15u;
+        if (Planes == 2) {
+          nibs[Planes - 1] = in_row ? 15u : 0u;                   // first slice of a volume: all start
+          if (in_row && vz != 0) {
+            WT here[4], u[4];
+            load4_shared<Bytes>(cur + q0, here);
+            load4_shared<Bytes>(back + q0, u);
+            nibs[Planes - 1] = label_changes<WT>(u, here);
+          }
         }
 #pragma unroll
         for (int a = 0; a < Planes; ++a) {
-          uint32_t nib = in_row ? 15u : 0u;                       // first row along the axis: all start
-          if (in_row && (a == 0 ? y > 0 : vz != 0))
-            nib = (u[a][0] != here[0] ? 1u : 0u) | (u[a][1] != here[1] ? 2u : 0u) |
-                  (u[a][2] != here[2] ? 4u : 0u) | (u[a][3] != here[3] ? 8u : 0u);
+          const uint32_t nib = nibs[a];
           // word w of block b sits in lanes 8w .. 8w + 7; lane c takes word c = 4 b + w
           const uint32_t got = __shfl_sync(full, nibbles_to_word(nib, lane), (lane & 3) << 3);
           if ((lane >> 2) == b) word[a] = got;

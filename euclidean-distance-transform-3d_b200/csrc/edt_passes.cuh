@@ -72,6 +72,10 @@ int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, c
     // three CTAs per SM, each with one to two stages (18 KB) of labels in flight.  Measured on the
     // 512^3 label-noise transform, 6 or 4 rows per band and rings of 4 or 6 stages were slower.
     // Fewer rows per band where the ring does not fit (it always does for rows of at most 512 voxels).
+    // A stage holds no row after its band, so the band's last row leaves its y-runs of one row to the
+    // Y pass (about 6 % of its label-noise tiles then still run).  Staging that row too (62 KB, still
+    // three CTAs per SM for 4-byte labels; one for 8-byte ones) settled them all but made the X pass as
+    // much slower as it made the Y pass faster (DESIGN.md section 4.1).
     int warps = 8;
     const int stages = 3;
     while (warps > 1 && planes_smem_bytes(sx, Bytes, warps, stages) > (size_t)dc.max_smem_optin) warps >>= 1;

@@ -2001,6 +2001,112 @@ int edtb200_medial_axis(const void* labels, int label_bytes, int ndim, int64_t s
   return rc ? rc : io.finish();
 }
 
+int edtb200_skeletonize(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                        int64_t count, float wx, float wy, float wz, int black_border, int flags,
+                        uint8_t* skeleton_out, float* dist_out, int device, void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (ndim < 2) return fail(EDTB200_EINVAL, "edtb200_skeletonize takes 2-D and 3-D volumes (got ndim %d)", ndim);
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  const float w[3] = {wx, wy, wz};
+  for (int k = 0; k < ndim; ++k)
+    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
+      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_skeletonize takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  // one list segment holds the voxels of one subfield: 4-byte entries
+  const int64_t cap = count * ((sx + 1) / 2) * ((sy + 1) / 2) * ((sz + 1) / 2);
+  if (cap >= ((int64_t)1 << 32))
+    return fail(EDTB200_ELIMIT, "edtb200_skeletonize takes stacks of fewer than 2^32 voxels per subfield");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !skeleton_out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, dist_bytes = sizeof(float) * (size_t)total;
+  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
+    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
+  };
+  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
+  if (same_side && overlap(labels, lab_bytes, skeleton_out, (size_t)total))
+    return fail(EDTB200_EINVAL, "skeleton_out overlaps labels");
+  if (dist_out && same_side && overlap(labels, lab_bytes, dist_out, dist_bytes))
+    return fail(EDTB200_EINVAL, "dist_out overlaps labels");
+  if (dist_out && overlap(skeleton_out, (size_t)total, dist_out, dist_bytes))
+    return fail(EDTB200_EINVAL, "dist_out overlaps skeleton_out");
+
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  HostIO io;
+  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  // host buffers are staged whole: the labels and distances through this device's cached buffers, the
+  // skeleton through scratch
+  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  const void* d_labels = nullptr;
+  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  Scratch staged, values, list, control;
+  if (!io.out_dev && staged.alloc(*dc, (size_t)total, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the skeleton");
+  }
+  uint8_t* d_skel = io.out(skeleton_out, (size_t)total, staged.get<uint8_t>());
+  float* d_dist = nullptr;
+  if (dist_out) {
+    if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, dist_bytes));
+    d_dist = io.out(dist_out, dist_bytes, dc->dist);
+  }
+  // scratch: the edtsq when no distances are wanted, then -- once the edtsq has returned its own scratch to
+  // the pool -- the two list buffers of one segment per subfield and the control block (the state plane is
+  // the skeleton's buffer)
+  if (!d_dist && values.alloc(*dc, dist_bytes, s) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for the skeleton's edtsq");
+  }
+  SkeletonScratch sk;
+  sk.segments = ndim == 3 ? 8 : 4;
+  sk.cap = (uint32_t)cap;
+  const size_t list_bytes = 2 * (size_t)sk.segments * (size_t)cap * sizeof(uint32_t);
+  float* d2 = d_dist ? d_dist : values.get<float>();
+  float h = wx;
+  for (int k = 1; k < ndim; ++k) h = std::min(h, w[k]);
+
+  // EDT_B200_VERBOSE=1: per-step device times and the thinning's counts on stderr (synchronises the stream)
+  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
+  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+  if (verbose)
+    for (int k = 0; k < 3; ++k)
+      if (cudaEventCreate(&ev[k]) == cudaSuccess && k == 0) cudaEventRecord(ev[0], s);
+  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2, *dc, s, count);
+  if (ev[1]) cudaEventRecord(ev[1], s);
+  if (!rc && (list.alloc(*dc, list_bytes, s) != cudaSuccess ||
+              control.alloc(*dc, skeleton_control_bytes(), s) != cudaSuccess)) {
+    cudaGetLastError();
+    rc = fail(EDTB200_ENOMEM, "no device memory for the skeleton's lists");
+  }
+  sk.list = list.get<uint32_t>();
+  sk.control = control.get();
+  if (!rc) rc = launch_skeleton_thin(d_labels, label_bytes, ndim, sx, sy, sz, count, h, d2, sk, d_skel, d_dist, *dc, s);
+  if (ev[2]) cudaEventRecord(ev[2], s);
+  if (verbose) {
+    float ms[2] = {0.0f, 0.0f};
+    unsigned long long n[3] = {0, 0, 0};
+    if (!rc && cudaEventSynchronize(ev[2]) == cudaSuccess) {
+      if (ev[0] && ev[1]) cudaEventElapsedTime(&ms[0], ev[0], ev[1]);
+      if (ev[1] && ev[2]) cudaEventElapsedTime(&ms[1], ev[1], ev[2]);
+      skeleton_stats(sk.control, n);
+      fprintf(stderr, "[edt_b200] skeletonize %lldx%lldx%lld x%lld L=%d  edtsq %.3f ms  thin %.3f ms  rounds %llu  "
+                      "cycles %llu  steps %llu  scratch %zu bytes\n",
+              (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, ms[0], ms[1], n[0], n[1],
+              n[2], (d_dist ? 0 : dist_bytes) + list_bytes + skeleton_control_bytes());
+    }
+    for (cudaEvent_t e : ev)
+      if (e) cudaEventDestroy(e);
+    cudaGetLastError();
+  }
+  return rc ? rc : io.finish();
+}
+
 // The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
 static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
                           const float w[3], int k, double max_distance) {

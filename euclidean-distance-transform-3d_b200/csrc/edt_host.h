@@ -1,13 +1,13 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as twelve translation units so that the kernel templates build in
+// The library is compiled as thirteen translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
 // transforms' kernels), edt_surface.cu (the surface distances' kernels), edt_morphology.cu (the
 // spherical morphology's label-writing stores), edt_parabolic.cu (the parabolic erosion and
-// dilation passes), edt_nearest.cu (the nearest-labels passes) and edt_medial.cu (the medial
-// axis's mark kernel).  The run-time label width
+// dilation passes), edt_nearest.cu (the nearest-labels passes), edt_medial.cu (the medial
+// axis's mark kernel) and edt_skeleton.cu (the skeleton's thinning kernel).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -327,6 +327,26 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
 int launch_medial_mark(const void* labels, int label_bytes, const int* const codes[3], int ndim, int64_t sx,
                        int64_t sy, int64_t sz, int64_t count, bool as_float, uint8_t* medial, float* dist,
                        DeviceCache& dc, cudaStream_t stream);
+
+// The skeleton's scratch (edt_skeleton.cu): two list buffers of `segments` segments of `cap` 4-byte entries
+// each, and the control block (skeleton_control_bytes()).
+struct SkeletonScratch {
+  uint32_t* list = nullptr;
+  void* control = nullptr;
+  int segments = 0;
+  uint32_t cap = 0;
+};
+
+// The thinning of skeletonize over `count` volumes of (sx, sy, sz) (edt_skeleton.cu): one cooperative
+// launch of skeleton_thin_kernel on the edtsq r, h the least weight; keeps its state plane in skeleton and
+// leaves the result there (0 / 1); dist
+// non-null, the correctly rounded sqrt of r into dist (which may be r itself).
+int launch_skeleton_thin(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                         int64_t count, float h, const float* r, const SkeletonScratch& scratch, uint8_t* skeleton,
+                         float* dist, DeviceCache& dc, cudaStream_t stream);
+size_t skeleton_control_bytes();
+// The rounds, cycles and steps of the last thinning on `control` (synchronous copy).
+int skeleton_stats(const void* control, unsigned long long out[3]);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

@@ -38,7 +38,7 @@ extern "C" {
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
- * edtb200_medial_axis)
+ * edtb200_medial_axis, edtb200_skeletonize)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -367,6 +367,72 @@ int edtb200_parabolic_sites(const float *f, int ndim, int64_t sx, int64_t sy, in
 int edtb200_medial_axis(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                         int64_t count, float wx, float wy, float wz, int black_border, int flags,
                         uint8_t *medial_out, float *dist_out, int device, void *stream);
+
+/* Topology-preserving curve skeletons of every label at once, thinned in the order of the distance
+ * transform, so that the skeleton is centred in physical units even on anisotropic voxels.
+ * Terms.  Coordinates are taken within one volume (x the fastest axis in memory).  The voxels of a label
+ * M are 26-connected (2-D: 8-); everything that is not M -- background, other labels, and the voxels
+ * outside the volume -- is 6-connected (2-D: 4-).  All labels are thinned at once; deleting a voxel of M
+ * never changes the topology of another label N, for which it was already "not N".
+ *   simple     p of label M is simple iff the M-voxels of N26(p) \ {p} form exactly one 26-component
+ *              and the non-M voxels of N18(p) \ {p} (6-connected within that set) have exactly one
+ *              6-component that contains a 6-neighbour of p.  2-D: the M-pixels of N8(p) \ {p} form
+ *              exactly one 8-component and the non-M pixels of N8(p) \ {p} have exactly one 4-component
+ *              4-adjacent to p.
+ *   end point  p of label M is an end point iff exactly one voxel of N26(p) \ {p} (2-D: N8) is of M.
+ *   subfield   k = (x & 1) | (y & 1) << 1 | (z & 1) << 2 (2-D: (x & 1) | (y & 1) << 1).
+ * Rounds.  R = edtb200_transform's edtsq of the labels (with black_border), float32, bit for bit; h = the
+ * least weight of the first ndim axes; theta_t = (t h)^2 in double for t = 1, 2, ... (t below 2^53).
+ * Round t admits the labelled voxels still present whose (double) R <= theta_t.  Rounds run up to the
+ * first t with theta_t >= the largest finite R of a labelled voxel; then one final round admits every
+ * voxel still present, R = +inf included (a label that touches the volume's edge without black_border).
+ * A round that admits no new voxel changes nothing, and the kernel skips it.
+ * Inside a round cycles repeat; a cycle runs the steps k = 0, 1, ..., 7 (2-D: 0 .. 3) in order, and step
+ * k deletes, all at once, every present admitted voxel of subfield k that is simple on the image at the
+ * start of the step and was not an end point at the start of the CYCLE.  The round ends after the first
+ * cycle that deletes nothing.  The skeleton is the set of voxels present after the final round.  No two
+ * voxels of one subfield are 26-neighbours, so a step equals any sequential order of its deletions.
+ *   topology   each label keeps its number of 26-components (2-D: 8-), the number of 6-components of its
+ *              complement (2-D: 4-) and its Euler characteristic, so also its cavities and tunnels.
+ *   thinness   no voxel of the result is simple and not an end point.
+ *   order      the result depends on which axis is fastest in memory, through the subfield order: an
+ *              F-ordered array gives the C-ordered call on its transpose with the weights reversed, and
+ *              the same labels in the two orders can give different, equally valid skeletons.
+ * Examples: a straight line one voxel thick is its own skeleton; an isolated voxel stays; a 3x3x3 cube
+ * in background gives exactly its centre; a hollow spherical shell keeps a closed surface around its
+ * cavity; a 4x6x12 box (z, y, x) in background gives the line x = 4 .. 10 at (z, y) = (3, 4) of the box
+ * padded by one voxel, along its long axis; a 2-D disc of radius 6 gives its centre pixel.
+ *
+ *   labels        count * sx*sy*sz labels of label_bytes (1, 2, 4 or 8) bytes, integers (no float
+ *                 labels), volumes back to back as for edtb200_transform_stack (count 1: one volume),
+ *                 each thinned on its own
+ *   ndim          2 or 3; wx..wz the weights of the first ndim axes: finite and > 0
+ *   flags         the residency flags only (both on the device: asynchronous on `stream`, no lock and no
+ *                 host wait; host buffers are staged whole, EDTB200_ENOMEM when they do not fit -- there
+ *                 is no chunked path)
+ *   skeleton_out  count * sx*sy*sz bytes, 0 or 1
+ *   dist_out      NULL, or count * sx*sy*sz float32: edt (sqrt of R, correctly rounded), bit for bit
+ *                 edtb200_transform's with EDTB200_SQRT; on the same side as skeleton_out
+ * Kernels, on one stream: the edtsq of the stack (one launch per pass, into dist_out or scratch), then
+ * ONE cooperative launch of skeleton_thin_kernel, which runs every round, cycle and step with a grid
+ * barrier between them: a sweep per round admits voxels into a compact list with one segment per
+ * subfield, each cycle's first pass drops the deleted entries and the end points (an end point at the
+ * start of a cycle can never be deleted later, so it is retired for good), each step tests only its
+ * segment, and the last sweep writes the skeleton and the square roots.  Device memory beyond the labels
+ * and the outputs: 4 + 8 bytes per voxel for volumes of even sides (12 in 2-D and 3-D; 8 with dist_out,
+ * which holds R): R (4, without dist_out) and two list buffers of one 4-byte entry per voxel (a segment
+ * holds count * ceil(sx/2) * ceil(sy/2) * ceil(sz/2) entries); the state byte of each voxel lives in
+ * skeleton_out's device buffer.  The lists are taken after the edtsq has returned its long-line scratch
+ * (where its plan takes that kernel), so the two do not add up; plus the staged host buffers.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), ndim of 2 or 3, count >= 0, weights,
+ * flags, the stack's size (within 2^62 voxels), a subfield's size (below 2^32 voxels, else
+ * EDTB200_ELIMIT), emptiness (returns 0 touching nothing), pointers (labels, skeleton_out) and overlap
+ * (neither output may overlap the labels when on the same side, nor the other output), device.
+ * EDT_B200_VERBOSE=1 prints the edtsq's and the thinning's device times, and the rounds, cycles and
+ * steps run, on stderr. */
+int edtb200_skeletonize(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                        int64_t count, float wx, float wy, float wz, int black_border, int flags,
+                        uint8_t *skeleton_out, float *dist_out, int device, void *stream);
 
 /* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
  * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between

@@ -154,6 +154,15 @@ for shape, dtype, stacked in (((4, 9, 11, 7), np.uint16, True), ((13, 30), np.fl
   got, dist = edt.medial_axis(lab, None, True, return_distance=True, stacked=stacked)
   check("medial_axis %s" % (shape,), got, mac.restate(lab, None, True, stacked=stacked)[0])
   check("medial_axis only %s" % (shape,), edt.medial_axis(lab, None, True, stacked=stacked), got)
+# skeleton: the cooperative thinning kernel over a stack, 2-D and 3-D, with and without distances, against
+# the restatement
+import skeleton_cases as skc  # noqa: E402
+for shape, dtype, stacked, w in (((3, 9, 11, 7), np.uint16, True, (1.0, 1.0, 2.0)), ((13, 30), np.int64, False, None),
+                                 ((6, 10, 12), np.uint8, False, (4.0, 4.0, 40.0))):
+  lab = (rng.integers(0, 3, shape) * (rng.random(shape) < 0.9)).astype(dtype)
+  got, dist = edt.skeletonize(lab, w, True, return_distance=True, stacked=stacked)
+  check("skeletonize %s" % (shape,), got, skc.restate(lab, w, True, stacked=stacked))
+  check("skeletonize only %s" % (shape,), edt.skeletonize(lab, w, True, stacked=stacked), got)
 # per-label views: a nearly full table whose probe chain wraps past its end, a table that overflows, and
 # a sub-box drawn at a ragged row length; the helpers are the GPU tests' own
 import each_cases as ec  # noqa: E402

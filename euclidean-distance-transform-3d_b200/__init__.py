@@ -573,7 +573,7 @@ def _stack_dims(dims, voxel_graph=None):
   return dims - 1
 
 
-def _stack_anisotropy(vnd, anisotropy):
+def _volume_anisotropy(vnd, anisotropy):
   """One weight per volume axis (a scalar for 1-D volumes); default 1."""
   if anisotropy is None:
     return (1.0,) * vnd
@@ -581,7 +581,7 @@ def _stack_anisotropy(vnd, anisotropy):
     return (float(anisotropy),)
   weights = tuple(float(a) for a in np.asarray(anisotropy).reshape(-1))
   if len(weights) != vnd:
-    raise ValueError("stacked=True: anisotropy must have one entry per volume axis (%d), got %d" % (vnd, len(weights)))
+    raise ValueError("anisotropy must have one entry per volume axis (%d), got %d" % (vnd, len(weights)))
   return weights
 
 
@@ -607,7 +607,7 @@ def _stack_front_door(data, anisotropy, black_border, voxel_graph, flags, device
   if on_device is None:
     data = np.asarray(np.array(data) if isinstance(data, list) else data)
   vnd = _stack_dims(on_device.dim() if on_device is not None else data.ndim, voxel_graph)
-  anisotropy = _stack_anisotropy(vnd, anisotropy)
+  anisotropy = _volume_anisotropy(vnd, anisotropy)
   if on_device is not None:
     if max_device_bytes is not None:
       raise ValueError("max_device_bytes streams a host array through the GPU; a device-resident array already fits")
@@ -939,7 +939,7 @@ def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_
   nd = data.ndim
   vnd = nd - 1 if stacked else nd           # index planes: one per (volume) axis
   if stacked:
-    anisotropy = _stack_anisotropy(vnd, anisotropy)
+    anisotropy = _volume_anisotropy(vnd, anisotropy)
     data, order = _stack_order(data)
   else:
     anisotropy = _feature_anisotropy(nd, anisotropy)
@@ -993,7 +993,7 @@ def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False
   import torch
   dims = t.dim()
   vnd = dims - 1 if stacked else dims       # index planes: one per (volume) axis
-  anisotropy = _stack_anisotropy(vnd, anisotropy) if stacked else _feature_anisotropy(dims, anisotropy)
+  anisotropy = _volume_anisotropy(vnd, anisotropy) if stacked else _feature_anisotropy(dims, anisotropy)
   if t.dtype in (torch.float32, torch.float64):
     t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)     # -0.0 == +0.0
   nbytes = _torch_label_bytes(torch).get(t.dtype)
@@ -1146,7 +1146,7 @@ def _expand_stack(labels, on_device, distance, anisotropy, device, max_device_by
   if max_device_bytes is not None:
     raise ValueError("stacked=True stages the whole stack on the GPU at once; it cannot be combined with "
                      "max_device_bytes")
-  anisotropy = _stack_anisotropy(vnd, anisotropy)
+  anisotropy = _volume_anisotropy(vnd, anisotropy)
   if on_device is not None:
     return _expand_device(on_device, distance, anisotropy, True)
   arr, order = _stack_order(arr)
@@ -1217,6 +1217,99 @@ def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device
 
 
 # ---------------------------------------------------------------------------------------
+# whole-volume operations: one C ABI call on the whole input, host or device
+# ---------------------------------------------------------------------------------------
+
+class _WholeVolume:
+  """The input of one whole-volume operation, resolved for its C ABI call.  A numpy array is staged on
+  the GPU whole and gives numpy results; a device array (a torch CUDA tensor or any
+  __cuda_array_interface__ object) gives torch CUDA results computed on its current stream.  `arr` is
+  C- or F-contiguous (C where both apply; a strided array is copied to C order), and the C ABI reads an
+  F-ordered one as its C-ordered transpose, with the weights reversed.  With `stacked` the slowest axis
+  in memory indexes same-shaped volumes.  Outputs are allocated in the input's shape and memory order,
+  so nothing is mapped back afterwards."""
+
+  def __init__(self, name, data, stacked, dims, device):
+    """`dims`: the (least, most) dimensions of one volume; a stack has one more."""
+    t = _device_array(data)
+    self.on_device = t is not None
+    arr = t if self.on_device else np.asarray(data)
+    nd = arr.dim() if self.on_device else arr.ndim
+    self.stacked = 1 if stacked else 0
+    lo, hi = dims[0] + self.stacked, dims[1] + self.stacked
+    if not lo <= nd <= hi:
+      raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D"
+                      % (name, "stacked=True" if stacked else "it", lo, hi, nd))
+    if self.on_device:
+      self.fortran = nd > 1 and not arr.is_contiguous() and arr.permute(*reversed(range(nd))).is_contiguous()
+      if not self.fortran:
+        arr = arr.contiguous()
+    else:
+      arr, order = _stack_order(arr)
+      self.fortran = order == "F"
+    self.name, self.arr, self.dtype, self.shape = name, arr, arr.dtype, tuple(arr.shape)
+    self.vnd = nd - self.stacked
+    self.size = arr.numel() if self.on_device else arr.size
+    self.flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE if self.on_device else 0
+    self._device = device
+
+  def set_weights(self, anisotropy, positive=True):
+    """One weight per volume axis, and with `positive` each finite and > 0; sets `geometry`, the
+    vnd, sx, sy, sz, count, wx, wy, wz of the C ABI call."""
+    weights = _volume_anisotropy(self.vnd, anisotropy)
+    if positive:
+      for w in weights:
+        if not (np.isfinite(w) and w > 0.0):
+          raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (self.name, anisotropy))
+    shape = self.shape
+    if self.fortran:
+      shape, weights = shape[::-1], weights[::-1]
+    (sx, sy, sz), (wx, wy, wz) = _x_fastest(shape[1:] if self.stacked else shape, weights, False)
+    self.geometry = (self.vnd, sx, sy, sz, int(shape[0]) if self.stacked else 1, wx, wy, wz)
+
+  @property
+  def floating(self):
+    return self.dtype.is_floating_point if self.on_device else self.dtype.kind == "f"
+
+  @property
+  def ptr(self):
+    return self.ptr_of(self.arr)
+
+  @staticmethod
+  def ptr_of(x):
+    if x is None:
+      return None
+    return x.ctypes.data if isinstance(x, np.ndarray) else x.data_ptr()
+
+  @property
+  def where(self):
+    """The device and stream of the C ABI call."""
+    if not self.on_device:
+      return int(self._device), None
+    import torch
+    return self.arr.device.index, ctypes.c_void_p(torch.cuda.current_stream(self.arr.device).cuda_stream)
+
+  def empty(self, dtype=None, planes=None):
+    """An output in the input's shape and memory order, or with `planes=k` k of them as one array of
+    shape (k,) + shape.  `dtype`: a name numpy and torch share ("bool", "int32", "float32"), None for the
+    input's."""
+    lead = () if planes is None else (planes,)
+    shape = lead + (self.shape[::-1] if self.fortran else self.shape)     # as the C ABI reads the input
+    if not self.on_device:
+      dtype = self.dtype if dtype is None else dtype
+      if not lead:
+        return np.empty(self.shape, dtype, order="F" if self.fortran else "C")
+      out = np.empty(shape, dtype)
+    else:
+      import torch
+      out = torch.empty(shape, dtype=self.dtype if dtype is None else getattr(torch, dtype), device=self.arr.device)
+    if not self.fortran:
+      return out
+    back = tuple(range(len(lead))) + tuple(range(out.ndim - 1, len(lead) - 1, -1))
+    return out.permute(*back) if self.on_device else out.transpose(back)
+
+
+# ---------------------------------------------------------------------------------------
 # spherical morphology: erosion, dilation, opening and closing with a Euclidean ball, each a threshold
 # on a bounded transform whose last store writes labels (edtb200_morphology)
 # ---------------------------------------------------------------------------------------
@@ -1242,50 +1335,17 @@ def _morphology(op, labels, radius, anisotropy, black_border, device, stacked, n
   r = float(radius)
   if not (r >= 0.0 and r != float("inf")):
     raise ValueError("%s: radius must be finite and zero or more, got %r" % (name, radius))
-  on_device = _device_array(labels)
-  arr = None if on_device is not None else np.asarray(np.array(labels) if isinstance(labels, list) else labels)
-  nd = on_device.dim() if on_device is not None else arr.ndim
-  lo, hi = (2, 4) if stacked else (1, 3)
-  if not lo <= nd <= hi:
-    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
-  nbytes = _morph_label_bytes(on_device.dtype if on_device is not None else arr.dtype)
+  v = _WholeVolume(name, labels, stacked, (1, 3), device)
+  nbytes = _morph_label_bytes(v.dtype)
   if nbytes is None:
-    raise TypeError("%s: unsupported label dtype %s" % (name, on_device.dtype if on_device is not None else arr.dtype))
-  vnd = nd - 1 if stacked else nd
-  weights = _surface_anisotropy(vnd, anisotropy)
-  mask_out = op in (_DILATE, _CLOSE)
-  border = int(bool(black_border))
-  lib = _lib()
-  if on_device is None:
-    arr, order = _stack_order(arr)
-    out = np.zeros(arr.shape, dtype=np.bool_ if mask_out else arr.dtype, order=order)
-    if arr.size == 0:
-      return out
-    if stacked:
-      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
-    else:
-      count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
-    flags = FLAG_LABELS_FLOAT if arr.dtype.kind == "f" else 0
-    _check(lib.edtb200_morphology(arr.ctypes.data, nbytes, vnd, sx, sy, sz, count, wx, wy, wz, op, r, border, flags,
-                                  out.ctypes.data, int(device), None))
-    return out
-  import torch
-  t = on_device
-  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
-  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
-    t = t.permute(*reversed(range(nd)))
-    weights = tuple(reversed(weights))
-  elif not t.is_contiguous():
-    t = t.contiguous()
-  out = torch.empty(t.shape, dtype=torch.bool if mask_out else t.dtype, device=t.device)
-  if t.numel():
-    count = int(t.shape[0]) if stacked else 1
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
-    flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE | (FLAG_LABELS_FLOAT if t.is_floating_point() else 0)
-    stream = torch.cuda.current_stream(t.device).cuda_stream
-    _check(lib.edtb200_morphology(t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, op, r, border, flags,
-                                  out.data_ptr(), t.device.index, ctypes.c_void_p(stream)))
-  return out.permute(*reversed(range(nd))) if fortran else out
+    raise TypeError("%s: unsupported label dtype %s" % (name, v.dtype))
+  v.set_weights(anisotropy, positive=False)        # taken as edtb200_transform takes them
+  out = v.empty("bool" if op in (_DILATE, _CLOSE) else None)
+  if v.size:
+    flags = v.flags | (FLAG_LABELS_FLOAT if v.floating else 0)
+    _check(_lib().edtb200_morphology(v.ptr, nbytes, *v.geometry, op, r, int(bool(black_border)), flags,
+                                     v.ptr_of(out), *v.where))
+  return out
 
 
 # Shared by the four functions below.  B is the ball {v in Z^n : sum_j (w_j v_j)^2 <= r^2}, w the
@@ -1357,68 +1417,26 @@ def _parabolic(op, f, anisotropy, device, stacked, name, return_indices=False):
   x-fastest plane vnd - 1 - k of a C-ordered array and plane k of an F-ordered one."""
   if not isinstance(return_indices, (bool, np.bool_)):
     raise TypeError("%s: return_indices must be True or False, got %r" % (name, return_indices))
-  on_device = _device_array(f)
-  arr = None if on_device is not None else np.asarray(f)
-  nd = on_device.dim() if on_device is not None else arr.ndim
-  lo, hi = (2, 4) if stacked else (1, 3)
-  if not lo <= nd <= hi:
-    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
-  if on_device is not None:
-    if on_device.is_complex():
-      raise TypeError("%s: it takes real or bool samples, got %s" % (name, on_device.dtype))
-  elif arr.dtype != np.bool_ and arr.dtype.kind not in "iuf":
-    raise TypeError("%s: it takes real or bool samples, got %s" % (name, arr.dtype))
-  vnd = nd - 1 if stacked else nd
-  weights = _surface_anisotropy(vnd, anisotropy)
-  for w in weights:
-    if not (np.isfinite(w) and w > 0.0):
-      raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (name, anisotropy))
-  lib = _lib()
-  if on_device is None:
-    arr, order = _stack_order(arr)
-    arr = arr.astype(np.float32, order="K", copy=False)
-    out = np.empty(arr.shape, dtype=np.float32, order=order)
-    planes = np.empty((vnd,) + (arr.shape if order == "C" else arr.shape[::-1]), np.int32) if return_indices else None
-    if arr.size:
-      if stacked:
-        count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
-      else:
-        count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
-      if return_indices:
-        _check(lib.edtb200_parabolic_sites(arr.ctypes.data, vnd, sx, sy, sz, count, wx, wy, wz, op, 0,
-                                           out.ctypes.data, planes.ctypes.data, int(device), None))
-      else:
-        _check(lib.edtb200_parabolic(arr.ctypes.data, vnd, sx, sy, sz, count, wx, wy, wz, op, 0, out.ctypes.data,
-                                     int(device), None))
-    if not return_indices:
-      return out
-    return out, (planes[::-1] if order == "C" else planes.transpose((0,) + tuple(range(nd, 0, -1))))
-  import torch
-  t = on_device
-  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
-  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
-    t = t.permute(*reversed(range(nd)))
-    weights = tuple(reversed(weights))
-  t = t.to(torch.float32).contiguous()
-  out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
-  planes = torch.empty((vnd,) + tuple(t.shape), dtype=torch.int32, device=t.device) if return_indices else None
-  if t.numel():
-    count = int(t.shape[0]) if stacked else 1
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
-    stream = ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
-    both = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
+  v = _WholeVolume(name, f, stacked, (1, 3), device)
+  if v.on_device:
+    if v.arr.is_complex():
+      raise TypeError("%s: it takes real or bool samples, got %s" % (name, v.dtype))
+  elif v.dtype != np.bool_ and v.dtype.kind not in "iuf":
+    raise TypeError("%s: it takes real or bool samples, got %s" % (name, v.dtype))
+  v.set_weights(anisotropy)
+  v.arr = v.arr.float() if v.on_device else v.arr.astype(np.float32, order="K", copy=False)   # memory order kept
+  out = v.empty("float32")
+  planes = v.empty("int32", planes=v.vnd) if return_indices else None
+  if v.size:
     if return_indices:
-      _check(lib.edtb200_parabolic_sites(t.data_ptr(), vnd, sx, sy, sz, count, wx, wy, wz, op, both, out.data_ptr(),
-                                         planes.data_ptr(), t.device.index, stream))
+      _check(_lib().edtb200_parabolic_sites(v.ptr, *v.geometry, op, v.flags, v.ptr_of(out), v.ptr_of(planes),
+                                            *v.where))
     else:
-      _check(lib.edtb200_parabolic(t.data_ptr(), vnd, sx, sy, sz, count, wx, wy, wz, op, both, out.data_ptr(),
-                                   t.device.index, stream))
-  if fortran:
-    out = out.permute(*reversed(range(nd)))
+      _check(_lib().edtb200_parabolic(v.ptr, *v.geometry, op, v.flags, v.ptr_of(out), *v.where))
   if not return_indices:
     return out
   # x first as written: an F-ordered caller's axis k is plane k, a C-ordered caller's is plane vnd - 1 - k
-  return out, (planes.permute(0, *range(nd, 0, -1)) if fortran else planes.flip(0))
+  return out, (planes if v.fortran else planes.flip(0) if v.on_device else planes[::-1])
 
 
 _PARABOLIC_DOC = """
@@ -1538,57 +1556,17 @@ def medial_axis(labels, anisotropy=None, black_border=False, *, return_distance=
   name = "medial_axis"
   if not isinstance(return_distance, (bool, np.bool_)):
     raise TypeError("%s: return_distance must be True or False, got %r" % (name, return_distance))
-  on_device = _device_array(labels)
-  arr = None if on_device is not None else np.asarray(np.array(labels) if isinstance(labels, list) else labels)
-  nd = on_device.dim() if on_device is not None else arr.ndim
-  lo, hi = (2, 4) if stacked else (1, 3)
-  if not lo <= nd <= hi:
-    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
-  nbytes = _morph_label_bytes(on_device.dtype if on_device is not None else arr.dtype)
+  v = _WholeVolume(name, labels, stacked, (1, 3), device)
+  nbytes = _morph_label_bytes(v.dtype)
   if nbytes is None:
-    raise TypeError("%s: unsupported label dtype %s" % (name, on_device.dtype if on_device is not None else arr.dtype))
-  vnd = nd - 1 if stacked else nd
-  weights = _surface_anisotropy(vnd, anisotropy)
-  for w in weights:
-    if not (np.isfinite(w) and w > 0.0):
-      raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (name, anisotropy))
-  border = int(bool(black_border))
-  lib = _lib()
-  if on_device is None:
-    arr, order = _stack_order(arr)
-    medial = np.empty(arr.shape, dtype=np.bool_, order=order)
-    dist = np.empty(arr.shape, dtype=np.float32, order=order) if return_distance else None
-    if arr.size:
-      if stacked:
-        count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
-      else:
-        count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
-      flags = FLAG_LABELS_FLOAT if arr.dtype.kind == "f" else 0
-      _check(lib.edtb200_medial_axis(arr.ctypes.data, nbytes, vnd, sx, sy, sz, count, wx, wy, wz, border, flags,
-                                     medial.ctypes.data, None if dist is None else dist.ctypes.data, int(device),
-                                     None))
-    return (medial, dist) if return_distance else medial
-  import torch
-  t = on_device
-  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
-  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
-    t = t.permute(*reversed(range(nd)))
-    weights = tuple(reversed(weights))
-  elif not t.is_contiguous():
-    t = t.contiguous()
-  medial = torch.empty(t.shape, dtype=torch.bool, device=t.device)
-  dist = torch.empty(t.shape, dtype=torch.float32, device=t.device) if return_distance else None
-  if t.numel():
-    count = int(t.shape[0]) if stacked else 1
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
-    flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE | (FLAG_LABELS_FLOAT if t.is_floating_point() else 0)
-    stream = torch.cuda.current_stream(t.device).cuda_stream
-    _check(lib.edtb200_medial_axis(t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, border, flags,
-                                   medial.data_ptr(), None if dist is None else dist.data_ptr(), t.device.index,
-                                   ctypes.c_void_p(stream)))
-  if fortran:
-    medial = medial.permute(*reversed(range(nd)))
-    dist = None if dist is None else dist.permute(*reversed(range(nd)))
+    raise TypeError("%s: unsupported label dtype %s" % (name, v.dtype))
+  v.set_weights(anisotropy)
+  medial = v.empty("bool")
+  dist = v.empty("float32") if return_distance else None
+  if v.size:
+    flags = v.flags | (FLAG_LABELS_FLOAT if v.floating else 0)
+    _check(_lib().edtb200_medial_axis(v.ptr, nbytes, *v.geometry, int(bool(black_border)), flags, v.ptr_of(medial),
+                                      v.ptr_of(dist), *v.where))
   return (medial, dist) if return_distance else medial
 
 
@@ -1642,57 +1620,18 @@ def skeletonize(labels, anisotropy=None, black_border=False, *, return_distance=
   name = "skeletonize"
   if not isinstance(return_distance, (bool, np.bool_)):
     raise TypeError("%s: return_distance must be True or False, got %r" % (name, return_distance))
-  on_device = _device_array(labels)
-  arr = None if on_device is not None else np.asarray(np.array(labels) if isinstance(labels, list) else labels)
-  nd = on_device.dim() if on_device is not None else arr.ndim
-  lo, hi = (3, 4) if stacked else (2, 3)
-  if not lo <= nd <= hi:
-    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
-  dtype = on_device.dtype if on_device is not None else arr.dtype
+  v = _WholeVolume(name, labels, stacked, (2, 3), device)
   try:
-    nbytes = _nearest_label_bytes(dtype)
+    nbytes = _nearest_label_bytes(v.dtype)
   except TypeError:
-    raise TypeError("%s: unsupported label dtype %s: labels must be an integer or bool dtype" % (name, dtype)) from None
-  vnd = nd - 1 if stacked else nd
-  weights = _surface_anisotropy(vnd, anisotropy)
-  for w in weights:
-    if not (np.isfinite(w) and w > 0.0):
-      raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (name, anisotropy))
-  border = int(bool(black_border))
-  lib = _lib()
-  if on_device is None:
-    arr, order = _stack_order(arr)
-    skel = np.empty(arr.shape, dtype=np.bool_, order=order)
-    dist = np.empty(arr.shape, dtype=np.float32, order=order) if return_distance else None
-    if arr.size:
-      if stacked:
-        count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
-      else:
-        count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
-      _check(lib.edtb200_skeletonize(arr.ctypes.data, nbytes, vnd, sx, sy, sz, count, wx, wy, wz, border, 0,
-                                     skel.ctypes.data, None if dist is None else dist.ctypes.data, int(device),
-                                     None))
-    return (skel, dist) if return_distance else skel
-  import torch
-  t = on_device
-  fortran = not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
-  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
-    t = t.permute(*reversed(range(nd)))
-    weights = tuple(reversed(weights))
-  elif not t.is_contiguous():
-    t = t.contiguous()
-  skel = torch.empty(t.shape, dtype=torch.bool, device=t.device)
-  dist = torch.empty(t.shape, dtype=torch.float32, device=t.device) if return_distance else None
-  if t.numel():
-    count = int(t.shape[0]) if stacked else 1
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
-    stream = torch.cuda.current_stream(t.device).cuda_stream
-    _check(lib.edtb200_skeletonize(t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, border,
-                                   FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, skel.data_ptr(),
-                                   None if dist is None else dist.data_ptr(), t.device.index, ctypes.c_void_p(stream)))
-  if fortran:
-    skel = skel.permute(*reversed(range(nd)))
-    dist = None if dist is None else dist.permute(*reversed(range(nd)))
+    raise TypeError("%s: unsupported label dtype %s: labels must be an integer or bool dtype"
+                    % (name, v.dtype)) from None
+  v.set_weights(anisotropy)
+  skel = v.empty("bool")
+  dist = v.empty("float32") if return_distance else None
+  if v.size:
+    _check(_lib().edtb200_skeletonize(v.ptr, nbytes, *v.geometry, int(bool(black_border)), v.flags, v.ptr_of(skel),
+                                      v.ptr_of(dist), *v.where))
   return (skel, dist) if return_distance else skel
 
 
@@ -1772,53 +1711,15 @@ def nearest_labels(labels, max_distance, anisotropy=None, *, k=2, squared=False,
   d = float(max_distance)
   if not (d >= 0.0 and d != float("inf")):
     raise ValueError("%s: max_distance must be finite and zero or more, got %r" % (name, max_distance))
-  on_device = _device_array(labels)
-  arr = None if on_device is not None else np.asarray(labels)
-  nd = on_device.dim() if on_device is not None else arr.ndim
-  lo, hi = (2, 4) if stacked else (1, 3)
-  if not lo <= nd <= hi:
-    raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D" % (name, "stacked=True" if stacked else "it", lo, hi, nd))
-  nbytes = _nearest_label_bytes(on_device.dtype if on_device is not None else arr.dtype)
-  vnd = nd - 1 if stacked else nd
-  weights = _surface_anisotropy(vnd, anisotropy)
-  for w in weights:
-    if not (np.isfinite(w) and w > 0.0):
-      raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (name, anisotropy))
-  flags = 0 if not squared else FLAG_NEAREST_SQUARED
-  lib = _lib()
-  if on_device is None:
-    arr, order = _stack_order(arr)
-    planes = arr.shape if order == "C" else arr.shape[::-1]
-    back = (0,) + (tuple(range(1, nd + 1)) if order == "C" else tuple(range(nd, 0, -1)))
-    dist = np.empty((k,) + planes, np.float32).transpose(back)
-    near = np.empty((k,) + planes, arr.dtype).transpose(back)
-    if arr.size:
-      if stacked:
-        count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(arr.shape, order == "C", weights)
-      else:
-        count, ((sx, sy, sz), (wx, wy, wz)) = 1, _x_fastest(arr.shape, weights, order == "F")
-      _check(lib.edtb200_nearest_labels(arr.ctypes.data, nbytes, vnd, sx, sy, sz, count, wx, wy, wz, d, k, flags,
-                                        dist.ctypes.data, near.ctypes.data, int(device), None))
-    return dist, near
-  import torch
-  t = on_device
-  fortran = nd > 1 and not t.is_contiguous() and t.permute(*reversed(range(nd))).is_contiguous()
-  if fortran:                                    # its transposed (C-ordered) view, the weights reversed
-    t = t.permute(*reversed(range(nd)))
-    weights = tuple(reversed(weights))
-  else:
-    t = t.contiguous()
-  dist = torch.empty((k,) + tuple(t.shape), dtype=torch.float32, device=t.device)
-  near = torch.empty((k,) + tuple(t.shape), dtype=t.dtype, device=t.device)
-  if t.numel():
-    count = int(t.shape[0]) if stacked else 1
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape[1:] if stacked else t.shape, weights, False)
-    stream = ctypes.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
-    _check(lib.edtb200_nearest_labels(t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, d, k,
-                                      flags | FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE, dist.data_ptr(),
-                                      near.data_ptr(), t.device.index, stream))
-  if fortran:
-    return dist.permute(0, *range(nd, 0, -1)), near.permute(0, *range(nd, 0, -1))
+  v = _WholeVolume(name, labels, stacked, (1, 3), device)
+  nbytes = _nearest_label_bytes(v.dtype)
+  v.set_weights(anisotropy)
+  dist = v.empty("float32", planes=k)
+  near = v.empty(planes=k)
+  if v.size:
+    flags = v.flags | (FLAG_NEAREST_SQUARED if squared else 0)
+    _check(_lib().edtb200_nearest_labels(v.ptr, nbytes, *v.geometry, d, k, flags, v.ptr_of(dist), v.ptr_of(near),
+                                         *v.where))
   return dist, near
 
 
@@ -1831,18 +1732,6 @@ SurfaceDistances = collections.namedtuple("SurfaceDistances", "labels offsets va
 SurfaceDistances.__doc__ = """What surface_distances returns.  labels: the keys, in the caller's dtype;
 offsets: int64, count * K * 2 + 1 entries, segment (volume * K + key) * 2 + direction from
 values[offsets[s]] to values[offsets[s + 1]]; values: float32, each segment sorted ascending."""
-
-
-def _surface_anisotropy(vnd, anisotropy):
-  """One weight per volume axis (a scalar for 1-D volumes); default 1."""
-  if anisotropy is None:
-    return (1.0,) * vnd
-  if np.ndim(anisotropy) == 0 and vnd == 1:
-    return (float(anisotropy),)
-  weights = tuple(float(w) for w in np.asarray(anisotropy).reshape(-1))
-  if len(weights) != vnd:
-    raise ValueError("anisotropy must have one entry per volume axis (%d), got %d" % (vnd, len(weights)))
-  return weights
 
 
 def _surface_keys(labels, dtype):
@@ -1894,7 +1783,7 @@ def _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes):
     raise TypeError("surface distances take 1-D to 3-D volumes, got %d-D" % nd)
   else:
     vnd = nd
-  anisotropy = _surface_anisotropy(vnd, anisotropy)
+  anisotropy = _volume_anisotropy(vnd, anisotropy)
   keys = None if labels is None else _surface_keys(labels, dtype)
   budget = 0 if max_device_bytes is None else int(max_device_bytes)
   if budget < 0:

@@ -16,9 +16,11 @@ SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE = 1, 2, 4, 8
 PROBE = "probe"
 BIG = (1 << 30) + 1
 
-# two separate host blocks: the checks only test for NULL and for overlap
-_LABELS = np.zeros(512, np.uint64)
-_OUT = np.zeros(512, np.uint64)
+# two separate host blocks: the checks only test for NULL and for overlap.  Each holds the largest extent a
+# case passes (valid_1d: 300 volumes of 4 voxels, 4800 bytes), so that whether two valid extents overlap never
+# depends on where the allocator placed the blocks
+_LABELS = np.zeros(1024, np.uint64)
+_OUT = np.zeros(1024, np.uint64)
 L, O = _LABELS.ctypes.data, _OUT.ctypes.data
 
 

@@ -450,58 +450,6 @@ cudaError_t private_stream(DeviceCache& dc) {
   return dc.stream ? cudaSuccess : cudaStreamCreateWithFlags(&dc.stream, cudaStreamNonBlocking);
 }
 
-// The residency contract of include/edt_b200.h for one call whose inputs and outputs may lie in
-// host memory: open() takes the device's host_call lock unless every buffer is on the device and
-// picks the stream; in() / out() give the device address of each buffer, uploading a host input
-// into the caller's staging buffer or noting a download from it; finish() runs the downloads in
-// order and, when host memory is involved, waits for them.
-struct HostIO {
-  bool in_dev = false, out_dev = false;
-  cudaStream_t stream = nullptr;
-
-  int open(DeviceCache& dc, int device, int flags, void* stream_v) {
-    in_dev = flags & EDTB200_LABELS_ON_DEVICE;
-    out_dev = flags & EDTB200_OUT_ON_DEVICE;
-    device_ = device;
-    stream = static_cast<cudaStream_t>(stream_v);
-    if (in_dev && out_dev) return 0;         // asynchronous on the caller's stream, no lock
-    lock_ = std::unique_lock<std::mutex>(dc.host_call);
-    // Both sides on the host and no stream given: the private stream.  With one side on the device
-    // the legacy default stream (NULL) is kept: it is ordered after the work the caller queued on
-    // the default / blocking streams that produced that buffer.
-    if (!stream && !in_dev && !out_dev) {
-      CUDA_TRY(private_stream(dc));
-      stream = dc.stream;
-    }
-    return 0;
-  }
-  template <class T>
-  int in(const T* src, size_t bytes, void* staging, const T** dev) {
-    *dev = in_dev ? src : static_cast<const T*>(staging);
-    return in_dev ? 0 : upload(staging, src, bytes, device_, stream);
-  }
-  template <class T>
-  T* out(T* dst, size_t bytes, T* staging) {
-    if (out_dev) return dst;
-    downloads_[count_++] = {dst, staging, bytes};
-    return staging;
-  }
-  int finish() {
-    for (int i = 0; i < count_; ++i) {
-      const int rc = download(downloads_[i].dst, downloads_[i].src, downloads_[i].bytes, device_, stream);
-      if (rc) return rc;
-    }
-    if (!(in_dev && out_dev)) CUDA_TRY(cudaStreamSynchronize(stream));
-    return 0;
-  }
-
- private:
-  struct Download { void* dst; const void* src; size_t bytes; };
-  Download downloads_[4];                    // at most the distances and three index planes
-  int count_ = 0, device_ = 0;
-  std::unique_lock<std::mutex> lock_;
-};
-
 // Restores the calling thread's current CUDA device when an entry point returns (callers such as
 // PyTorch rely on "their" current device staying put).
 struct DeviceGuard {
@@ -577,6 +525,33 @@ int check_dims(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz)
   return 0;
 }
 
+int check_weights(int ndim, const float w[3]) {
+  for (int k = 0; k < ndim; ++k)
+    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
+      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  return 0;
+}
+
+// A stack of `count` volumes of `vol` voxels, `per_voxel` values each, holds at most 2^62 values.
+int check_stack(int64_t vol, int64_t count, int64_t per_voxel) {
+  if (vol > 0 && count > ((int64_t)1 << 62) / (vol * per_voxel))
+    return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  return 0;
+}
+
+int check_float_labels(int flags, int label_bytes) {
+  if ((flags & EDTB200_LABELS_FLOAT) && label_bytes != 4 && label_bytes != 8)
+    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
+  return 0;
+}
+
+bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
+  return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
+}
+
+// Inputs and outputs in the same memory space: an address in one may alias the other.
+bool same_side(int flags) { return !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE); }
+
 int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines, int64_t sx, float w,
                    int border, int flags, DeviceCache& dc, cudaStream_t s, const edtb200::XPlanes* planes = nullptr) {
   return with_label_width(label_bytes, [&](auto b) {
@@ -602,6 +577,83 @@ cudaError_t grow(T*& p, size_t& have, size_t need) {
   if (e == cudaSuccess) have = need;
   return e;
 }
+
+// The residency contract of include/edt_b200.h for one call whose inputs and outputs may lie in
+// host memory: open() probes the device, takes its host_call lock unless every buffer is on the
+// device and picks the stream; in() / out() give the device address of each buffer, uploading a host
+// input into the caller's staging buffer or noting a download from it; finish() runs the downloads
+// in order and, when host memory is involved, waits for them.  The caller's current device is
+// restored last, so the Scratch a call declares after its HostIO is freed while the call still
+// holds the lock and the device.
+struct HostIO {
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  bool in_dev = false, out_dev = false;
+  cudaStream_t stream = nullptr;
+
+  int open(int device, int flags, void* stream_v) {
+    if (const int rc = probe(device, &dc)) return rc;
+    in_dev = flags & EDTB200_LABELS_ON_DEVICE;
+    out_dev = flags & EDTB200_OUT_ON_DEVICE;
+    device_ = device;
+    stream = static_cast<cudaStream_t>(stream_v);
+    if (in_dev && out_dev) return 0;         // asynchronous on the caller's stream, no lock
+    lock_ = std::unique_lock<std::mutex>(dc->host_call);
+    // Both sides on the host and no stream given: the private stream.  With one side on the device
+    // the legacy default stream (NULL) is kept: it is ordered after the work the caller queued on
+    // the default / blocking streams that produced that buffer.
+    if (!stream && !in_dev && !out_dev) {
+      CUDA_TRY(private_stream(*dc));
+      stream = dc->stream;
+    }
+    return 0;
+  }
+  template <class T>
+  int in(const T* src, size_t bytes, void* staging, const T** dev) {
+    *dev = in_dev ? src : static_cast<const T*>(staging);
+    return in_dev ? 0 : upload(staging, src, bytes, device_, stream);
+  }
+  template <class T>
+  T* out(T* dst, size_t bytes, T* staging) {
+    if (out_dev) return dst;
+    downloads_[count_++] = {dst, staging, bytes};
+    return staging;
+  }
+  // in() / out() staged through the device's cached labels / distances buffer, grown for a host buffer
+  template <class T>
+  int in_labels(const T* src, size_t bytes, const T** dev) {
+    if (!in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, bytes));
+    return in(src, bytes, dc->labels, dev);
+  }
+  template <class T>
+  int out_dist(T* dst, size_t bytes, T** dev) {
+    if (!out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, bytes));
+    *dev = out(dst, bytes, static_cast<T*>(static_cast<void*>(dc->dist)));
+    return 0;
+  }
+  // out() staged through `scratch`, taken for a host buffer ("no device memory for <what>")
+  template <class T>
+  int out_staged(T* dst, size_t bytes, Scratch& scratch, const char* what, T** dev) {
+    if (!out_dev)
+      if (const int rc = scratch.take(*dc, bytes, stream, what)) return rc;
+    *dev = out(dst, bytes, scratch.get<T>());
+    return 0;
+  }
+  int finish() {
+    for (int i = 0; i < count_; ++i) {
+      const int rc = download(downloads_[i].dst, downloads_[i].src, downloads_[i].bytes, device_, stream);
+      if (rc) return rc;
+    }
+    if (!(in_dev && out_dev)) CUDA_TRY(cudaStreamSynchronize(stream));
+    return 0;
+  }
+
+ private:
+  struct Download { void* dst; const void* src; size_t bytes; };
+  Download downloads_[4];                    // at most the distances and three index planes
+  int count_ = 0, device_ = 0;
+  std::unique_lock<std::mutex> lock_;
+};
 
 // Kernel flags of a pass from the ABI flags: sqrt and sign act in the store of the last pass;
 // background-as-label (sdf) changes the first pass only -- later passes treat every run alike.
@@ -784,6 +836,50 @@ void nvtx_init() {
 void nvtx_push(const char* name) { nvtx_init(); if (g_nvtx_push) g_nvtx_push(name); }
 void nvtx_pop() { if (g_nvtx_pop) g_nvtx_pop(); }
 
+// EDT_B200_VERBOSE=1: the calls report their device times on stderr, one "[edt_b200] ..." line each
+// (SURVEY.md section 5).  A verbose call synchronises its stream to read them.
+bool verbose() {
+  static const bool on = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
+  return on;
+}
+
+// The device times between the steps of one verbose call: stamp() after each step records an event on
+// the stream, synchronize() waits for the last one, ms(a, b) is the time between stamps a and b (0 where
+// an event is missing).  Off unless verbose(): no events, and synchronize() is false.  The events are
+// destroyed on every exit.
+class StepTimer {
+ public:
+  explicit StepTimer(cudaStream_t s) : s_(s) {}
+  StepTimer(const StepTimer&) = delete;
+  StepTimer& operator=(const StepTimer&) = delete;
+  ~StepTimer() {
+    if (!on_) return;
+    for (int i = 0; i < n_; ++i)
+      if (ev_[i]) cudaEventDestroy(ev_[i]);
+    cudaGetLastError();
+  }
+  bool on() const { return on_; }
+  void stamp() {
+    if (!on_ || n_ == kMax) return;
+    cudaEvent_t& e = ev_[n_++];
+    if (cudaEventCreate(&e) != cudaSuccess) { e = nullptr; cudaGetLastError(); return; }
+    if (cudaEventRecord(e, s_) != cudaSuccess) cudaGetLastError();
+  }
+  bool synchronize() const { return n_ > 0 && ev_[n_ - 1] && cudaEventSynchronize(ev_[n_ - 1]) == cudaSuccess; }
+  float ms(int a, int b) const {
+    float t = 0.0f;
+    if (a < n_ && b < n_ && ev_[a] && ev_[b]) cudaEventElapsedTime(&t, ev_[a], ev_[b]);
+    return t;
+  }
+
+ private:
+  static constexpr int kMax = 6;
+  cudaStream_t s_;
+  bool on_ = verbose();
+  int n_ = 0;
+  cudaEvent_t ev_[kMax] = {};
+};
+
 // All passes of one transform on device-resident buffers: of `count` volumes of (sx, sy, sz) laid end
 // to end, each transformed on its own with one launch per pass for all of them.  Every pass keeps one
 // volume's extents for its arithmetic (transform_arith over t.n), so each volume gets the plan it
@@ -802,11 +898,9 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   RunPlanes planes;
   int rc = take_run_planes(planes, t, labels, f, sy, sz, count, dc, stream);
   if (rc) return rc;
-  // EDT_B200_VERBOSE=1: per-pass device times of every transform on stderr (SURVEY.md section 5).
-  // The dump needs the passes to have finished, so a verbose transform synchronises its stream.
-  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
+  // verbose: per-pass device times of every transform, read from the mark_pass ring
   const bool profile_was = g_profile;
-  if (verbose) g_profile = true;
+  if (verbose()) g_profile = true;
   mark_pass(0, stream);
   nvtx_push("edt.x");
   rc = x_pass(t, labels, f, sy * sz * count, dc, stream, &planes);
@@ -826,7 +920,7 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
     nvtx_pop();
     mark_pass(3, stream);
   }
-  if (verbose) {
+  if (verbose()) {
     g_profile = profile_was;
     float ms[3] = {0.0f, 0.0f, 0.0f};
     if (!rc && edtb200_pass_ms(0, ms) == 0) {
@@ -838,6 +932,26 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
               total > 0 ? nvox / total / 1e3 : 0.0,
               total > 0 ? nvox * (3.0 * label_bytes + 20.0) / total / 1e6 : 0.0);
     }
+  }
+  return rc;
+}
+
+// The parabolic passes (dilate: dilation) along every axis of `count` volumes of (sx, sy, sz) laid end
+// to end: the first from `in` into `out`, the others in place on `out`; codes[k] non-null: pass k also
+// writes its site codes there.  kernel[k] is what pass k ran (launch_parabolic_pass), -1 for none; the
+// timer is stamped after each pass.
+int parabolic_passes(const float* in, float* out, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                     const float w[3], bool dilate, int* const codes[3], int kernel[3], StepTimer& timer,
+                     DeviceCache& dc, cudaStream_t s) {
+  kernel[0] = kernel[1] = kernel[2] = -1;
+  int rc = 0;
+  for (int k = 0; !rc && k < ndim; ++k) {
+    edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz, count);
+    if (k == 0) {                              // rows of sx contiguous samples
+      g.outer_count = sy * sz * count; g.outer_stride = sx; g.inner_count = 1; g.line_stride = 1; g.n = (int)sx;
+    }
+    rc = launch_parabolic_pass(k == 0 ? in : out, out, g, k == 0, w[k], dilate, dc, s, &kernel[k], codes[k]);
+    timer.stamp();
   }
   return rc;
 }
@@ -858,10 +972,9 @@ int run_bounded_passes(const void* labels, int label_bytes, int ndim, int64_t sx
   int windows = 0;                                // window passes that write distances
   for (int k = 1; k < ndim; ++k) windows += bp.windowed[k] && !(sel && k == ndim - 1) ? 1 : 0;
   Scratch other;
-  if (windows && other.alloc(dc, sizeof(float) * (size_t)total, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the bounded transform's scratch volume");
-  }
+  if (windows)
+    if (const int rc = other.take(dc, sizeof(float) * (size_t)total, s, "the bounded transform's scratch volume"))
+      return rc;
   float* buf[2] = {f, other.get<float>()};
   int cur = windows % 2;
   int rc = dispatch_first(label_bytes, labels, buf[cur], sy * sz * count, sx, wx, border,
@@ -1072,18 +1185,14 @@ int edtb200_transform(const void* labels, int label_bytes, int ndim, int64_t sx,
   if (total == 0) return 0;
   if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
-  // host buffers are staged through this device's cached buffers
-  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
-  float* d_out = io.out(out, out_bytes, dc->dist);
-  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_out, *dc,
+  float* d_out = nullptr;
+  if ((rc = io.in_labels(labels, (size_t)total * (size_t)label_bytes, &d_labels)) ||
+      (rc = io.out_dist(out, (size_t)total * sizeof(float), &d_out)))
+    return rc;
+  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_out, *io.dc,
                   io.stream);
   return rc ? rc : io.finish();
 }
@@ -1339,7 +1448,6 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
                      chunks)))
     return rc;
 
-  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
   const auto t0 = std::chrono::steady_clock::now();
   rc = run_phase(dc, device, two.p1, label_bytes, 1, [&](const ChunkSlots& slots, PipelineSteps& steps) {
     steps.item = "phase-1 chunk";
@@ -1376,7 +1484,7 @@ int edtb200_transform_chunked(const void* labels, int label_bytes, int ndim, int
     };
   });
   if (rc) return rc;
-  if (verbose) {
+  if (verbose()) {
     const auto t2 = std::chrono::steady_clock::now();
     const double ms1 = std::chrono::duration<double, std::milli>(t1 - t0).count();
     const double ms2 = std::chrono::duration<double, std::milli>(t2 - t1).count();
@@ -1598,30 +1706,23 @@ int feature_transform_any(const void* labels, int label_bytes, int ndim, int64_t
   }
   const int64_t total = vol * count;
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
-  // host buffers are staged through the cached labels and distances and one scratch for the planes;
-  // a distance volume and an index plane are 4 bytes per voxel
-  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, vol_bytes = (size_t)total * sizeof(float);
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  // host index planes are staged through one scratch; a distance volume and an index plane are 4 bytes
+  // per voxel
+  const size_t vol_bytes = (size_t)total * sizeof(float);
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
+  float* d_dist = nullptr;
+  if ((rc = io.in_labels(labels, (size_t)total * (size_t)label_bytes, &d_labels)) ||
+      (dist_out && (rc = io.out_dist(dist_out, vol_bytes, &d_dist))))
+    return rc;
   Scratch planes;
-  if (!io.out_dev) {
-    if (dist_out) CUDA_TRY(grow(dc->dist, dc->dist_bytes, vol_bytes));
-    if (planes.alloc(*dc, (size_t)ndim * vol_bytes, io.stream) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the index planes");
-    }
-  }
-  float* d_dist = dist_out ? io.out(dist_out, vol_bytes, dc->dist) : nullptr;
+  if (!io.out_dev && (rc = planes.take(*io.dc, (size_t)ndim * vol_bytes, io.stream, "the index planes"))) return rc;
   int32_t* d_idx[3] = {nullptr, nullptr, nullptr};
   for (int k = 0; k < ndim; ++k)
     d_idx[k] = io.out(idx_out[k], vol_bytes, io.out_dev ? nullptr : planes.get<int32_t>() + (size_t)k * total);
   rc = run_feature_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_dist,
-                          d_idx, *dc, io.stream, count, bp);
+                          d_idx, *io.dc, io.stream, count, bp);
   return rc ? rc : io.finish();
 }
 
@@ -1659,19 +1760,15 @@ int edtb200_transform_bounded(const void* labels, int label_bytes, int ndim, int
   const float w[3] = {wx, wy, wz};
   const BoundedPlan bp = bounded_plan(ndim, w, max_distance, /*sites=*/false);
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
-  // host buffers are staged through this device's cached buffers, as edtb200_transform stages them
-  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = (size_t)total * sizeof(float);
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
-  float* d_out = io.out(out, out_bytes, dc->dist);
+  float* d_out = nullptr;
+  if ((rc = io.in_labels(labels, (size_t)total * (size_t)label_bytes, &d_labels)) ||
+      (rc = io.out_dist(out, (size_t)total * sizeof(float), &d_out)))
+    return rc;
   rc = run_bounded_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, flags, d_out, bp,
-                          *dc, io.stream);
+                          *io.dc, io.stream);
   return rc ? rc : io.finish();
 }
 
@@ -1703,11 +1800,10 @@ int edtb200_morphology(const void* labels, int label_bytes, int ndim, int64_t sx
   if (flags & ~known)
     return fail(EDTB200_EINVAL, "edtb200_morphology takes only the residency flags and EDTB200_LABELS_FLOAT (got %d)",
                 flags);
+  if ((rc = check_float_labels(flags, label_bytes))) return rc;
   const bool as_float = flags & EDTB200_LABELS_FLOAT;
-  if (as_float && label_bytes != 4 && label_bytes != 8)
-    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
   const int64_t vol = sx * sy * sz;
-  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  if ((rc = check_stack(vol, count, 1))) return rc;
   const int64_t total = vol * count;
   if (total == 0) return 0;
   if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
@@ -1716,38 +1812,33 @@ int edtb200_morphology(const void* labels, int label_bytes, int ndim, int64_t sx
   const bool mask_out = op == EDTB200_DILATE || op == EDTB200_CLOSE;
   const int border = black_border != 0;
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const cudaStream_t s = io.stream;
-  // host buffers are staged through this device's cached buffers, as edtb200_transform_bounded stages them
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
-  const size_t out_bytes = (size_t)total * (mask_out ? 1 : (size_t)label_bytes);
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, out_bytes));
-  void* d_out = io.out(out, out_bytes, static_cast<void*>(dc->dist));
+  void* d_out = nullptr;
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) ||
+      (rc = io.out_dist(out, (size_t)total * (mask_out ? 1 : (size_t)label_bytes), &d_out)))
+    return rc;
   // scratch: the distances, the first step's mask (opening, closing) and the folded float labels
   const bool two = op == EDTB200_OPEN || op == EDTB200_CLOSE;
+  const char* what = "the morphology's scratch";
   Scratch dist, mask, folded;
-  if (dist.alloc(*dc, sizeof(float) * (size_t)total, s) != cudaSuccess ||
-      (two && mask.alloc(*dc, (size_t)total, s) != cudaSuccess) ||
-      (as_float && folded.alloc(*dc, lab_bytes, s) != cudaSuccess)) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the morphology's scratch");
-  }
+  if ((rc = dist.take(*io.dc, sizeof(float) * (size_t)total, s, what)) ||
+      (two && (rc = mask.take(*io.dc, (size_t)total, s, what))) ||
+      (as_float && (rc = folded.take(*io.dc, lab_bytes, s, what))))
+    return rc;
   const void* runs = d_labels;                   // the labels the transforms compare
   if (as_float) {
-    if ((rc = launch_fold_float_labels(d_labels, label_bytes, folded.get(), total, *dc, s))) return rc;
+    if ((rc = launch_fold_float_labels(d_labels, label_bytes, folded.get(), total, *io.dc, s))) return rc;
     runs = folded.get();
   }
   // select tables, bit (2 nz + near): erode keeps nz & !near (4), dilate sets nz | near (2, 4, 8), open's
   // mask is 0 on the erosion E and 1 elsewhere (the complement of 4), open keeps nz & near (8)
   constexpr int kErode = 0x4, kDilate = 0xE, kNotEroded = 0xB, kNear = 0x8;
   auto step = [&](const void* lab, int lab_w, int bord, int fl, const edtb200::MorphSelect& sel) {
-    return run_bounded_passes(lab, lab_w, ndim, sx, sy, sz, wx, wy, wz, bord, fl, dist.get<float>(), bp, *dc, s,
+    return run_bounded_passes(lab, lab_w, ndim, sx, sy, sz, wx, wy, wz, bord, fl, dist.get<float>(), bp, *io.dc, s,
                               count, &sel);
   };
   uint8_t* m = mask.get<uint8_t>();
@@ -1781,13 +1872,11 @@ static int parabolic_any(const float* f, int ndim, int64_t sx, int64_t sy, int64
   if (op != EDTB200_PARABOLIC_ERODE && op != EDTB200_PARABOLIC_DILATE)
     return fail(EDTB200_EINVAL, "op must be EDTB200_PARABOLIC_ERODE or _DILATE (got %d)", op);
   const float w[3] = {wx, wy, wz};
-  for (int k = 0; k < ndim; ++k)
-    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
-      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  if ((rc = check_weights(ndim, w))) return rc;
   if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
     return fail(EDTB200_EINVAL, "%s takes only the residency flags (got %d)", name, flags);
   const int64_t vol = sx * sy * sz;
-  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  if ((rc = check_stack(vol, count, 1))) return rc;
   // with sites, (i-j)^2 must be exact in double on the brute-force lines
   if (sites && (sx > kParabolicSitesN || sy > kParabolicSitesN || sz > kParabolicSitesN))
     return fail(EDTB200_ELIMIT, "%s takes lines of at most 2^26 samples", name);
@@ -1795,77 +1884,43 @@ static int parabolic_any(const float* f, int ndim, int64_t sx, int64_t sy, int64
   if (total == 0) return 0;
   if (!f || !out || (sites && !idx)) return fail(EDTB200_EINVAL, "null pointer");
   const size_t bytes = sizeof(float) * (size_t)total, idx_bytes = (size_t)ndim * bytes;
-  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
-  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
-    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
-  };
-  if (same_side && f != out && overlap(f, bytes, out, bytes)) return fail(EDTB200_EINVAL, "out overlaps f without being f");
-  if (idx && overlap(idx, idx_bytes, out, bytes)) return fail(EDTB200_EINVAL, "idx overlaps out");
-  if (idx && same_side && overlap(idx, idx_bytes, f, bytes)) return fail(EDTB200_EINVAL, "idx overlaps f");
+  if (same_side(flags) && f != out && overlaps(f, bytes, out, bytes))
+    return fail(EDTB200_EINVAL, "out overlaps f without being f");
+  if (idx && overlaps(idx, idx_bytes, out, bytes)) return fail(EDTB200_EINVAL, "idx overlaps out");
+  if (idx && same_side(flags) && overlaps(idx, idx_bytes, f, bytes)) return fail(EDTB200_EINVAL, "idx overlaps f");
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const cudaStream_t s = io.stream;
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, bytes));
   const float* d_f = nullptr;
-  if ((rc = io.in(f, bytes, dc->labels, &d_f))) return rc;
-  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, bytes));
-  float* d_out = io.out(out, bytes, dc->dist);
+  float* d_out = nullptr;
+  if ((rc = io.in_labels(f, bytes, &d_f)) || (rc = io.out_dist(out, bytes, &d_out))) return rc;
   // sites: the index planes (staged for a host idx), and the code planes of every pass but the last,
   // whose codes go straight into its own index plane (the resolver reads them only at their own voxel)
   Scratch staged, planes;
   int32_t* d_idx = nullptr;
   int* codes[3] = {nullptr, nullptr, nullptr};
   if (idx) {
-    if (!io.out_dev && staged.alloc(*dc, idx_bytes, s) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the index planes");
-    }
-    d_idx = io.out(idx, idx_bytes, io.out_dev ? nullptr : staged.get<int32_t>());
-    if (ndim > 1 && planes.alloc(*dc, (size_t)(ndim - 1) * bytes, s) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the site code planes");
-    }
+    if ((rc = io.out_staged(idx, idx_bytes, staged, "the index planes", &d_idx)) ||
+        (ndim > 1 && (rc = planes.take(*io.dc, (size_t)(ndim - 1) * bytes, s, "the site code planes"))))
+      return rc;
     for (int k = 0; k < ndim; ++k) codes[k] = (k == ndim - 1 ? d_idx : planes.get<int32_t>()) + (size_t)k * total;
   }
-  // EDT_B200_VERBOSE=1: per-pass device times and kernels on stderr (synchronises the stream)
-  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  if (verbose)
-    for (int k = 0; k <= ndim; ++k)
-      if (cudaEventCreate(&ev[k]) == cudaSuccess) cudaEventRecord(ev[k], s);
-  int kernel[3] = {-1, -1, -1};
-  const float* src = d_f;                      // the first pass out of place, the others in place
-  for (int k = 0; !rc && k < ndim; ++k) {
-    edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz, count);
-    if (k == 0) {                              // rows of sx contiguous samples
-      g.outer_count = sy * sz * count; g.outer_stride = sx; g.inner_count = 1; g.line_stride = 1; g.n = (int)sx;
-    }
-    rc = launch_parabolic_pass(src, d_out, g, k == 0, w[k], op == EDTB200_PARABOLIC_DILATE, *dc, s, &kernel[k],
-                               codes[k]);
-    if (ev[k + 1]) cudaEventRecord(ev[k + 1], s);
-    src = d_out;
-  }
+  StepTimer timer(s);
+  timer.stamp();
+  int kernel[3];
+  rc = parabolic_passes(d_f, d_out, ndim, sx, sy, sz, count, w, op == EDTB200_PARABOLIC_DILATE, codes, kernel, timer,
+                        *io.dc, s);
   if (!rc && idx) {
     int32_t* const planes_out[3] = {d_idx, d_idx + total, d_idx + 2 * (size_t)total};
-    rc = launch_resolve_sites<1>(nullptr, codes, ndim, sx, sy, sz, count, false, planes_out, *dc, s);
+    rc = launch_resolve_sites<1>(nullptr, codes, ndim, sx, sy, sz, count, false, planes_out, *io.dc, s);
   }
-  if (verbose) {
+  if (!rc && timer.synchronize()) {
     static const char* names[4] = {"tile", "long", "brute", "copy"};
-    float ms[3] = {0.0f, 0.0f, 0.0f};
-    if (!rc && cudaEventSynchronize(ev[ndim]) == cudaSuccess) {
-      for (int k = 0; k < ndim; ++k)
-        if (ev[k] && ev[k + 1]) cudaEventElapsedTime(&ms[k], ev[k], ev[k + 1]);
-      fprintf(stderr, "[edt_b200] parabolic %s %lldx%lldx%lld x%lld  x %.3f ms (%s)  y %.3f ms (%s)  z %.3f ms (%s)\n",
-              op == EDTB200_PARABOLIC_DILATE ? "dilate" : "erode", (long long)sx, (long long)sy, (long long)sz,
-              (long long)count, ms[0], names[kernel[0] < 0 ? 0 : kernel[0]], ms[1],
-              kernel[1] < 0 ? "-" : names[kernel[1]], ms[2], kernel[2] < 0 ? "-" : names[kernel[2]]);
-    }
-    for (cudaEvent_t e : ev)
-      if (e) cudaEventDestroy(e);
-    cudaGetLastError();
+    fprintf(stderr, "[edt_b200] parabolic %s %lldx%lldx%lld x%lld  x %.3f ms (%s)  y %.3f ms (%s)  z %.3f ms (%s)\n",
+            op == EDTB200_PARABOLIC_DILATE ? "dilate" : "erode", (long long)sx, (long long)sy, (long long)sz,
+            (long long)count, timer.ms(0, 1), names[kernel[0] < 0 ? 0 : kernel[0]], timer.ms(1, 2),
+            kernel[1] < 0 ? "-" : names[kernel[1]], timer.ms(2, 3), kernel[2] < 0 ? "-" : names[kernel[2]]);
   }
   return rc ? rc : io.finish();
 }
@@ -1888,17 +1943,14 @@ int edtb200_medial_axis(const void* labels, int label_bytes, int ndim, int64_t s
   if (rc) return rc;
   if (count < 0) return fail(EDTB200_EINVAL, "negative count");
   const float w[3] = {wx, wy, wz};
-  for (int k = 0; k < ndim; ++k)
-    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
-      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  if ((rc = check_weights(ndim, w))) return rc;
   if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE | EDTB200_LABELS_FLOAT))
     return fail(EDTB200_EINVAL, "edtb200_medial_axis takes only the residency flags and EDTB200_LABELS_FLOAT (got %d)",
                 flags);
+  if ((rc = check_float_labels(flags, label_bytes))) return rc;
   const bool as_float = flags & EDTB200_LABELS_FLOAT;
-  if (as_float && label_bytes != 4 && label_bytes != 8)
-    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
   const int64_t vol = sx * sy * sz;
-  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  if ((rc = check_stack(vol, count, 1))) return rc;
   // the sites' limit: beyond it (i-j)^2 is not exact in double on the brute-force lines
   if (sx > kParabolicSitesN || sy > kParabolicSitesN || sz > kParabolicSitesN)
     return fail(EDTB200_ELIMIT, "edtb200_medial_axis takes lines of at most 2^26 samples");
@@ -1906,97 +1958,65 @@ int edtb200_medial_axis(const void* labels, int label_bytes, int ndim, int64_t s
   if (total == 0) return 0;
   if (!labels || !medial_out) return fail(EDTB200_EINVAL, "null pointer");
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, dist_bytes = sizeof(float) * (size_t)total;
-  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
-    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
-  };
-  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
-  if (same_side && overlap(labels, lab_bytes, medial_out, (size_t)total)) return fail(EDTB200_EINVAL, "medial_out overlaps labels");
-  if (dist_out && same_side && overlap(labels, lab_bytes, dist_out, dist_bytes))
+  if (same_side(flags) && overlaps(labels, lab_bytes, medial_out, (size_t)total))
+    return fail(EDTB200_EINVAL, "medial_out overlaps labels");
+  if (dist_out && same_side(flags) && overlaps(labels, lab_bytes, dist_out, dist_bytes))
     return fail(EDTB200_EINVAL, "dist_out overlaps labels");
-  if (dist_out && overlap(medial_out, (size_t)total, dist_out, dist_bytes))
+  if (dist_out && overlaps(medial_out, (size_t)total, dist_out, dist_bytes))
     return fail(EDTB200_EINVAL, "dist_out overlaps medial_out");
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const cudaStream_t s = io.stream;
   // host buffers are staged whole: the labels and distances through this device's cached buffers, the
   // mask through scratch
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  Scratch staged, values, planes;
-  if (!io.out_dev && staged.alloc(*dc, (size_t)total, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the medial mask");
-  }
-  uint8_t* d_medial = io.out(medial_out, (size_t)total, staged.get<uint8_t>());
+  uint8_t* d_medial = nullptr;
   float* d_dist = nullptr;
-  if (dist_out) {
-    if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, dist_bytes));
-    d_dist = io.out(dist_out, dist_bytes, dc->dist);
-  }
+  Scratch staged, values, planes;
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) ||
+      (rc = io.out_staged(medial_out, (size_t)total, staged, "the medial mask", &d_medial)) ||
+      (dist_out && (rc = io.out_dist(dist_out, dist_bytes, &d_dist))))
+    return rc;
   // scratch: one value volume (D^2 without distances, the dilation's values with them) and the code
   // planes, which hold the folded float labels until the edtsq has read them
   const size_t plane_bytes = std::max(dist_bytes * (size_t)ndim, as_float ? lab_bytes : 0);
-  if (values.alloc(*dc, dist_bytes, s) != cudaSuccess || planes.alloc(*dc, plane_bytes, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the medial axis's scratch");
-  }
+  if ((rc = values.take(*io.dc, dist_bytes, s, "the medial axis's scratch")) ||
+      (rc = planes.take(*io.dc, plane_bytes, s, "the medial axis's scratch")))
+    return rc;
   const void* runs = d_labels;                   // the labels the edtsq compares
   if (as_float) {
-    if ((rc = launch_fold_float_labels(d_labels, label_bytes, planes.get(), total, *dc, s))) return rc;
+    if ((rc = launch_fold_float_labels(d_labels, label_bytes, planes.get(), total, *io.dc, s))) return rc;
     runs = planes.get();
   }
   float* d2 = d_dist ? d_dist : values.get<float>();
   int* codes[3] = {nullptr, nullptr, nullptr};
   for (int k = 0; k < ndim; ++k) codes[k] = planes.get<int>() + (size_t)k * total;
 
-  // EDT_B200_VERBOSE=1: per-step device times and kernels on stderr (synchronises the stream)
-  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
-  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  if (verbose)
-    for (int k = 0; k < 6; ++k)
-      if (cudaEventCreate(&ev[k]) == cudaSuccess && k == 0) cudaEventRecord(ev[0], s);
-  rc = run_passes(runs, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2, *dc, s, count);
-  if (ev[1]) cudaEventRecord(ev[1], s);
-  int kernel[3] = {-1, -1, -1};
-  const float* src = d2;                         // with distances the first pass writes the value scratch
-  float* dst = values.get<float>();
-  for (int k = 0; !rc && k < ndim; ++k) {
-    edtb200::LineGeom g = geom_for_axis(k, sx, sy, sz, count);
-    if (k == 0) {                                // rows of sx contiguous samples
-      g.outer_count = sy * sz * count; g.outer_stride = sx; g.inner_count = 1; g.line_stride = 1; g.n = (int)sx;
-    }
-    rc = launch_parabolic_pass(src, dst, g, k == 0, w[k], /*dilate=*/true, *dc, s, &kernel[k], codes[k]);
-    if (ev[k + 2]) cudaEventRecord(ev[k + 2], s);
-    src = dst;
-  }
+  // steps: the edtsq, a pass per axis, the mark
+  StepTimer timer(s);
+  timer.stamp();
+  rc = run_passes(runs, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2, *io.dc, s, count);
+  timer.stamp();
+  int kernel[3];
+  // with distances the first pass writes the value scratch
+  if (!rc)
+    rc = parabolic_passes(d2, values.get<float>(), ndim, sx, sy, sz, count, w, /*dilate=*/true, codes, kernel, timer,
+                          *io.dc, s);
   if (!rc && cudaMemsetAsync(d_medial, 0, (size_t)total, s) != cudaSuccess)
     rc = fail(EDTB200_ECUDA, "cudaMemsetAsync of the medial mask failed");
   if (!rc)
-    rc = launch_medial_mark(d_labels, label_bytes, codes, ndim, sx, sy, sz, count, as_float, d_medial, d_dist, *dc, s);
-  if (ev[5]) cudaEventRecord(ev[5], s);
-  if (verbose) {
+    rc = launch_medial_mark(d_labels, label_bytes, codes, ndim, sx, sy, sz, count, as_float, d_medial, d_dist, *io.dc,
+                            s);
+  timer.stamp();
+  if (!rc && timer.synchronize()) {
     static const char* names[4] = {"tile", "long", "brute", "copy"};
-    float ms[5] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
-    if (!rc && cudaEventSynchronize(ev[5]) == cudaSuccess) {
-      int at = 0;                                // the event before each step
-      for (int k = 1; k <= 5; ++k) {
-        if (k >= 2 && k <= 4 && k - 2 >= ndim) continue;
-        if (ev[at] && ev[k]) cudaEventElapsedTime(&ms[k - 1], ev[at], ev[k]);
-        at = k;
-      }
-      fprintf(stderr, "[edt_b200] medial_axis %lldx%lldx%lld x%lld L=%d  edtsq %.3f ms  x %.3f ms (%s)  y %.3f ms (%s)  "
-                      "z %.3f ms (%s)  mark %.3f ms\n",
-              (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, ms[0], ms[1],
-              names[kernel[0] < 0 ? 0 : kernel[0]], ms[2], kernel[1] < 0 ? "-" : names[kernel[1]], ms[3],
-              kernel[2] < 0 ? "-" : names[kernel[2]], ms[4]);
-    }
-    for (cudaEvent_t e : ev)
-      if (e) cudaEventDestroy(e);
-    cudaGetLastError();
+    fprintf(stderr, "[edt_b200] medial_axis %lldx%lldx%lld x%lld L=%d  edtsq %.3f ms  x %.3f ms (%s)  y %.3f ms (%s)  "
+                    "z %.3f ms (%s)  mark %.3f ms\n",
+            (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, timer.ms(0, 1), timer.ms(1, 2),
+            names[kernel[0] < 0 ? 0 : kernel[0]], ndim > 1 ? timer.ms(2, 3) : 0.0f,
+            kernel[1] < 0 ? "-" : names[kernel[1]], ndim > 2 ? timer.ms(3, 4) : 0.0f,
+            kernel[2] < 0 ? "-" : names[kernel[2]], timer.ms(ndim + 1, ndim + 2));
   }
   return rc ? rc : io.finish();
 }
@@ -2009,13 +2029,11 @@ int edtb200_skeletonize(const void* labels, int label_bytes, int ndim, int64_t s
   if (ndim < 2) return fail(EDTB200_EINVAL, "edtb200_skeletonize takes 2-D and 3-D volumes (got ndim %d)", ndim);
   if (count < 0) return fail(EDTB200_EINVAL, "negative count");
   const float w[3] = {wx, wy, wz};
-  for (int k = 0; k < ndim; ++k)
-    if (!(std::isfinite(w[k]) && w[k] > 0.0f))
-      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", k, (double)w[k]);
+  if ((rc = check_weights(ndim, w))) return rc;
   if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
     return fail(EDTB200_EINVAL, "edtb200_skeletonize takes only the residency flags (got %d)", flags);
   const int64_t vol = sx * sy * sz;
-  if (vol > 0 && count > ((int64_t)1 << 62) / vol) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  if ((rc = check_stack(vol, count, 1))) return rc;
   // one list segment holds the voxels of one subfield: 4-byte entries
   const int64_t cap = count * ((sx + 1) / 2) * ((sy + 1) / 2) * ((sz + 1) / 2);
   if (cap >= ((int64_t)1 << 32))
@@ -2024,45 +2042,30 @@ int edtb200_skeletonize(const void* labels, int label_bytes, int ndim, int64_t s
   if (total == 0) return 0;
   if (!labels || !skeleton_out) return fail(EDTB200_EINVAL, "null pointer");
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes, dist_bytes = sizeof(float) * (size_t)total;
-  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
-    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
-  };
-  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
-  if (same_side && overlap(labels, lab_bytes, skeleton_out, (size_t)total))
+  if (same_side(flags) && overlaps(labels, lab_bytes, skeleton_out, (size_t)total))
     return fail(EDTB200_EINVAL, "skeleton_out overlaps labels");
-  if (dist_out && same_side && overlap(labels, lab_bytes, dist_out, dist_bytes))
+  if (dist_out && same_side(flags) && overlaps(labels, lab_bytes, dist_out, dist_bytes))
     return fail(EDTB200_EINVAL, "dist_out overlaps labels");
-  if (dist_out && overlap(skeleton_out, (size_t)total, dist_out, dist_bytes))
+  if (dist_out && overlaps(skeleton_out, (size_t)total, dist_out, dist_bytes))
     return fail(EDTB200_EINVAL, "dist_out overlaps skeleton_out");
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const cudaStream_t s = io.stream;
   // host buffers are staged whole: the labels and distances through this device's cached buffers, the
   // skeleton through scratch
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  Scratch staged, values, list, control;
-  if (!io.out_dev && staged.alloc(*dc, (size_t)total, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the skeleton");
-  }
-  uint8_t* d_skel = io.out(skeleton_out, (size_t)total, staged.get<uint8_t>());
+  uint8_t* d_skel = nullptr;
   float* d_dist = nullptr;
-  if (dist_out) {
-    if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, dist_bytes));
-    d_dist = io.out(dist_out, dist_bytes, dc->dist);
-  }
+  Scratch staged, values, list, control;
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) ||
+      (rc = io.out_staged(skeleton_out, (size_t)total, staged, "the skeleton", &d_skel)) ||
+      (dist_out && (rc = io.out_dist(dist_out, dist_bytes, &d_dist))))
+    return rc;
   // scratch: the edtsq when no distances are wanted, then -- once the edtsq has returned its own scratch to
   // the pool -- the two list buffers of one segment per subfield and the control block (the state plane is
   // the skeleton's buffer)
-  if (!d_dist && values.alloc(*dc, dist_bytes, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the skeleton's edtsq");
-  }
+  if (!d_dist && (rc = values.take(*io.dc, dist_bytes, s, "the skeleton's edtsq"))) return rc;
   SkeletonScratch sk;
   sk.segments = ndim == 3 ? 8 : 4;
   sk.cap = (uint32_t)cap;
@@ -2071,38 +2074,25 @@ int edtb200_skeletonize(const void* labels, int label_bytes, int ndim, int64_t s
   float h = wx;
   for (int k = 1; k < ndim; ++k) h = std::min(h, w[k]);
 
-  // EDT_B200_VERBOSE=1: per-step device times and the thinning's counts on stderr (synchronises the stream)
-  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
-  cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  if (verbose)
-    for (int k = 0; k < 3; ++k)
-      if (cudaEventCreate(&ev[k]) == cudaSuccess && k == 0) cudaEventRecord(ev[0], s);
-  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2, *dc, s, count);
-  if (ev[1]) cudaEventRecord(ev[1], s);
-  if (!rc && (list.alloc(*dc, list_bytes, s) != cudaSuccess ||
-              control.alloc(*dc, skeleton_control_bytes(), s) != cudaSuccess)) {
-    cudaGetLastError();
-    rc = fail(EDTB200_ENOMEM, "no device memory for the skeleton's lists");
-  }
+  // steps: the edtsq, the thinning
+  StepTimer timer(s);
+  timer.stamp();
+  rc = run_passes(d_labels, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2, *io.dc, s, count);
+  timer.stamp();
+  if (!rc) rc = list.take(*io.dc, list_bytes, s, "the skeleton's lists");
+  if (!rc) rc = control.take(*io.dc, skeleton_control_bytes(), s, "the skeleton's lists");
   sk.list = list.get<uint32_t>();
   sk.control = control.get();
-  if (!rc) rc = launch_skeleton_thin(d_labels, label_bytes, ndim, sx, sy, sz, count, h, d2, sk, d_skel, d_dist, *dc, s);
-  if (ev[2]) cudaEventRecord(ev[2], s);
-  if (verbose) {
-    float ms[2] = {0.0f, 0.0f};
+  if (!rc)
+    rc = launch_skeleton_thin(d_labels, label_bytes, ndim, sx, sy, sz, count, h, d2, sk, d_skel, d_dist, *io.dc, s);
+  timer.stamp();
+  if (!rc && timer.synchronize()) {
     unsigned long long n[3] = {0, 0, 0};
-    if (!rc && cudaEventSynchronize(ev[2]) == cudaSuccess) {
-      if (ev[0] && ev[1]) cudaEventElapsedTime(&ms[0], ev[0], ev[1]);
-      if (ev[1] && ev[2]) cudaEventElapsedTime(&ms[1], ev[1], ev[2]);
-      skeleton_stats(sk.control, n);
-      fprintf(stderr, "[edt_b200] skeletonize %lldx%lldx%lld x%lld L=%d  edtsq %.3f ms  thin %.3f ms  rounds %llu  "
-                      "cycles %llu  steps %llu  scratch %zu bytes\n",
-              (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, ms[0], ms[1], n[0], n[1],
-              n[2], (d_dist ? 0 : dist_bytes) + list_bytes + skeleton_control_bytes());
-    }
-    for (cudaEvent_t e : ev)
-      if (e) cudaEventDestroy(e);
-    cudaGetLastError();
+    skeleton_stats(sk.control, n);
+    fprintf(stderr, "[edt_b200] skeletonize %lldx%lldx%lld x%lld L=%d  edtsq %.3f ms  thin %.3f ms  rounds %llu  "
+                    "cycles %llu  steps %llu  scratch %zu bytes\n",
+            (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, timer.ms(0, 1), timer.ms(1, 2),
+            n[0], n[1], n[2], (d_dist ? 0 : dist_bytes) + list_bytes + skeleton_control_bytes());
   }
   return rc ? rc : io.finish();
 }
@@ -2113,9 +2103,7 @@ static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, i
   int rc = check_dims(label_bytes, ndim, sx, sy, sz);
   if (rc) return rc;
   if (count < 0) return fail(EDTB200_EINVAL, "negative count");
-  for (int a = 0; a < ndim; ++a)
-    if (!(std::isfinite(w[a]) && w[a] > 0.0f))
-      return fail(EDTB200_EINVAL, "the weight of axis %d must be finite and > 0 (got %g)", a, (double)w[a]);
+  if ((rc = check_weights(ndim, w))) return rc;
   if (k < 1 || k > 4) return fail(EDTB200_EINVAL, "k must be 1, 2, 3 or 4 (got %d)", k);
   if (!(max_distance >= 0.0) || std::isinf(max_distance))
     return fail(EDTB200_EINVAL, "max_distance must be finite and zero or more (got %g): the cost is O(R) per voxel "
@@ -2152,53 +2140,41 @@ int edtb200_nearest_labels(const void* labels, int label_bytes, int ndim, int64_
     return fail(EDTB200_EINVAL, "edtb200_nearest_labels takes only the residency flags and EDTB200_NEAREST_SQUARED "
                 "(got %d)", flags);
   const int64_t vol = sx * sy * sz;
-  if (vol > 0 && count > ((int64_t)1 << 62) / (vol * k)) return fail(EDTB200_ELIMIT, "too many voxels in the stack");
+  if ((rc = check_stack(vol, count, k))) return rc;
   const int64_t total = vol * count;
   if (total == 0) return 0;
   if (!labels || !dist_out || !label_out) return fail(EDTB200_EINVAL, "null pointer");
   const size_t lab_bytes = (size_t)total * (size_t)label_bytes;
   const size_t dist_bytes = sizeof(float) * (size_t)total * (size_t)k, lout_bytes = lab_bytes * (size_t)k;
-  auto overlap = [](const void* a, size_t na, const void* b, size_t nb) {
-    return (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
-  };
-  const bool same_side = !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE);
-  if (overlap(dist_out, dist_bytes, label_out, lout_bytes)) return fail(EDTB200_EINVAL, "dist_out overlaps label_out");
-  if (same_side && (overlap(labels, lab_bytes, dist_out, dist_bytes) || overlap(labels, lab_bytes, label_out, lout_bytes)))
+  if (overlaps(dist_out, dist_bytes, label_out, lout_bytes)) return fail(EDTB200_EINVAL, "dist_out overlaps label_out");
+  if (same_side(flags) &&
+      (overlaps(labels, lab_bytes, dist_out, dist_bytes) || overlaps(labels, lab_bytes, label_out, lout_bytes)))
     return fail(EDTB200_EINVAL, "an output overlaps labels");
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
   const cudaStream_t s = io.stream;
   // host buffers are staged whole: the labels and distances through this device's cached buffers, the
   // output labels through scratch
-  if (!io.in_dev) CUDA_TRY(grow(dc->labels, dc->labels_bytes, lab_bytes));
   const void* d_labels = nullptr;
-  if ((rc = io.in(labels, lab_bytes, dc->labels, &d_labels))) return rc;
-  if (!io.out_dev) CUDA_TRY(grow(dc->dist, dc->dist_bytes, dist_bytes));
-  float* d_dist = io.out(dist_out, dist_bytes, dc->dist);
+  float* d_dist = nullptr;
+  void* d_lab = nullptr;
   Scratch staged, planes;
-  if (!io.out_dev && staged.alloc(*dc, lout_bytes, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the output labels");
-  }
-  void* d_lab = io.out(label_out, lout_bytes, io.out_dev ? nullptr : staged.get());
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) || (rc = io.out_dist(dist_out, dist_bytes, &d_dist)) ||
+      (rc = io.out_staged(label_out, lout_bytes, staged, "the output labels", &d_lab)))
+    return rc;
   // the scratch set of the passes: k value and label planes (2-D and 3-D)
   float* sdist = nullptr;
   void* slab = nullptr;
   if (ndim > 1) {
     // the value planes from a 16-byte boundary after the label planes, which may end anywhere
     const size_t at = (lout_bytes + 15) & ~(size_t)15;
-    if (planes.alloc(*dc, at + dist_bytes, s) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the passes' scratch planes");
-    }
+    if ((rc = planes.take(*io.dc, at + dist_bytes, s, "the passes' scratch planes"))) return rc;
     slab = planes.get();
     sdist = reinterpret_cast<float*>(planes.get<char>() + at);
   }
   rc = nearest_passes(d_labels, label_bytes, ndim, sx, sy, sz, count, w, p, k, !(flags & EDTB200_NEAREST_SQUARED),
-                      d_dist, d_lab, sdist, slab, *dc, s);
+                      d_dist, d_lab, sdist, slab, *io.dc, s);
   return rc ? rc : io.finish();
 }
 
@@ -2218,9 +2194,8 @@ int edtb200_expand_gather(const void* labels, int label_bytes, int ndim, int64_t
     return fail(EDTB200_EINVAL, "edtb200_expand_gather works on device buffers only: flags must be "
                                 "EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE, optionally with EDTB200_LABELS_FLOAT "
                                 "(got %d)", flags);
+  if ((rc = check_float_labels(flags, label_bytes))) return rc;
   const bool as_float = flags & EDTB200_LABELS_FLOAT;
-  if (as_float && label_bytes != 4 && label_bytes != 8)
-    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
 
   DeviceGuard restore_device;
   DeviceCache* dc = nullptr;
@@ -2272,10 +2247,7 @@ int check_surface_flags(int flags, const char* name) {
 // The keys on the device, for the kernels' search.
 int upload_keys(Scratch& dev, const void* keys, int64_t nkeys, int label_bytes, DeviceCache& dc, cudaStream_t s) {
   const size_t bytes = (size_t)nkeys * (size_t)label_bytes;
-  if (dev.alloc(dc, bytes, s) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the keys");
-  }
+  if (const int rc = dev.take(dc, bytes, s, "the keys")) return rc;
   CUDA_TRY(cudaMemcpyAsync(dev.get(), keys, bytes, cudaMemcpyHostToDevice, s));
   return 0;
 }
@@ -2388,10 +2360,9 @@ int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const uns
     return fail(EDTB200_EINVAL, "a voxel graph needs a 2-D or 3-D volume (got ndim %d)", ndim);
   if (flags & EDTB200_SIGNED)
     return fail(EDTB200_EINVAL, "EDTB200_SIGNED is not defined with a voxel graph: subtract two transforms");
-  if ((flags & EDTB200_LABELS_FLOAT) && label_bytes != 4 && label_bytes != 8)
-    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
-  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  int rc = check_float_labels(flags, label_bytes);
   if (rc) return rc;
+  if ((rc = check_dims(label_bytes, ndim, sx, sy, sz))) return rc;
   const int64_t total = sx * sy * sz;
   if (total == 0) return 0;
   if (!labels || !graph || !out) return fail(EDTB200_EINVAL, "null pointer");
@@ -2400,10 +2371,9 @@ int edtb200_transform_voxel_graph(const void* labels, int label_bytes, const uns
   if (rc) return rc;
   const int64_t total2 = sx2 * sy2 * sz2;
 
-  DeviceGuard restore_device;
-  DeviceCache* dc = nullptr;
   HostIO io;
-  if ((rc = probe(device, &dc)) || (rc = io.open(*dc, device, flags, stream_v))) return rc;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  DeviceCache* dc = io.dc;
   const cudaStream_t stream = io.stream;
   // stream-ordered scratch: the inputs when they come from the host, the doubled byte mask, the
   // doubled distance volume, and the result when it goes back to the host.  It is freed when the
@@ -2457,10 +2427,9 @@ int edtb200_transform_voxel_graph_chunked(const void* labels, int label_bytes, c
     return fail(EDTB200_EINVAL, "a voxel graph needs a 2-D or 3-D volume (got ndim %d)", ndim);
   if (flags & EDTB200_SIGNED)
     return fail(EDTB200_EINVAL, "EDTB200_SIGNED is not defined with a voxel graph: subtract two transforms");
-  if ((flags & EDTB200_LABELS_FLOAT) && label_bytes != 4 && label_bytes != 8)
-    return fail(EDTB200_EINVAL, "EDTB200_LABELS_FLOAT needs 4- or 8-byte labels");
-  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  int rc = check_float_labels(flags, label_bytes);
   if (rc) return rc;
+  if ((rc = check_dims(label_bytes, ndim, sx, sy, sz))) return rc;
   const int64_t total = sx * sy * sz;
   if (total == 0) return 0;
   if (!labels || !graph || !out) return fail(EDTB200_EINVAL, "null pointer");
@@ -2941,29 +2910,24 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   const int border = black_border != 0;
   const Transform t{label_bytes, 3, flags, border, {wx, wy, wz}, {sx, sy, sz}};
 
-  // EDT_B200_VERBOSE=1: device time of every phase of the step on stderr (synchronises the stream)
-  static const bool verbose = getenv("EDT_B200_VERBOSE") != nullptr && atoi(getenv("EDT_B200_VERBOSE")) != 0;
-  cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  auto stamp = [&](int i) {
-    if (!verbose) return;
-    if (cudaEventCreate(&ev[i]) == cudaSuccess) cudaEventRecord(ev[i], stream);
-    cudaGetLastError();
-  };
-  stamp(0);
+  // verbose: the device time of every phase of the step, with the launches serialised
+  StepTimer timer(stream);
+  const bool verbose = timer.on();
+  timer.stamp();
   mark_pass(0, stream);              // per-pass events for bench.py (edtb200_profile_passes), as in run_passes
   // X and Y passes: slab-local
   nvtx_push("edt.x");
   rc = x_pass(t, labels_dev, f_dev, sy * sz, *dc, stream);
   nvtx_pop();
   if (rc) return rc;
-  stamp(1);
+  timer.stamp();
   mark_pass(1, stream);
   nvtx_push("edt.y");
   rc = later_pass(t, 1, labels_dev, f_dev, geom_for_axis(1, sx, sy, sz), border, border, *dc, stream,
                   /*pdl=*/!verbose);
   nvtx_pop();
   if (rc) return rc;
-  stamp(2);
+  timer.stamp();
 
   const int64_t plane = sx * sy;
   const SlabStageLayout L = slab_stage_layout(plane, label_bytes, halo);
@@ -2991,7 +2955,7 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
     nvtx_pop();
   }
 
-  stamp(3);
+  timer.stamp();
   mark_pass(2, stream);              // "second pass" = Y plus the face staging kernel
   // Z pass on the slab, interior faces open
   nvtx_push("edt.z");
@@ -3000,7 +2964,7 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
   nvtx_pop();
   if (rc) return rc;
 
-  stamp(4);
+  timer.stamp();
   mark_pass(3, stream);
   if (has_lo || has_hi) {
     nvtx_push("edt.halo.fixup");
@@ -3029,15 +2993,13 @@ int edtb200_slab_step(const void* labels_dev, int label_bytes, int64_t sx, int64
     if (rc) return rc;
     nvtx_pop();
   }
-  stamp(5);
+  timer.stamp();
   if (verbose) {
     float ms[5] = {0, 0, 0, 0, 0};
-    if (ev[5] && cudaEventSynchronize(ev[5]) == cudaSuccess)
-      for (int i = 0; i < 5; ++i) if (ev[i] && ev[i + 1]) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
+    if (timer.synchronize())
+      for (int i = 0; i < 5; ++i) ms[i] = timer.ms(i, i + 1);
     fprintf(stderr, "[edt_b200] slab step %llu dev %d: x %.3f  y %.3f  stage %.3f  z %.3f  fixup %.3f ms\n", step, device,
             ms[0], ms[1], ms[2], ms[3], ms[4]);
-    for (auto& e : ev) if (e) cudaEventDestroy(e);
-    cudaGetLastError();
   }
   return 0;
 }

@@ -123,6 +123,12 @@ class Scratch {
     if (e != cudaSuccess) p_ = nullptr;
     return e;
   }
+  // alloc, failing with "no device memory for <what>" (and the sticky error cleared) when it cannot.
+  int take(DeviceCache& dc, size_t bytes, cudaStream_t stream, const char* what) {
+    if (alloc(dc, bytes, stream) == cudaSuccess) return 0;
+    cudaGetLastError();
+    return fail(EDTB200_ENOMEM, "no device memory for %s", what);
+  }
   template <class T = void>
   T* get() const { return static_cast<T*>(p_); }
 

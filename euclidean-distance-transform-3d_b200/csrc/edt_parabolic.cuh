@@ -498,10 +498,7 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
     const int64_t threads = pb_long_threads(lines, g.n);
     const int64_t blocks = (threads + 127) / 128, slots = blocks * 128;
     Scratch stack;
-    if (stack.alloc(dc, (size_t)slots * (size_t)g.n * 8, stream) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the long lines' hull stacks");
-    }
+    if (const int rc = stack.take(dc, (size_t)slots * (size_t)g.n * 8, stream, "the long lines' hull stacks")) return rc;
     float* sf = stack.get<float>();
     int* si = reinterpret_cast<int*>(sf + slots * (int64_t)g.n);
     if (codes) parabolic_long_kernel<true><<<(unsigned)blocks, 128, 0, stream>>>(in, out, g, w2, dilate, sf, si, codes);
@@ -515,10 +512,7 @@ int launch_parabolic_pass(const float* in, float* out, const LineGeom& g, bool r
   if (in == out) {
     // lines cover the volume from its first sample to its last
     const int64_t span = (g.outer_count - 1) * g.outer_stride + (g.inner_count - 1) + (int64_t)(g.n - 1) * g.line_stride + 1;
-    if (copy.alloc(dc, sizeof(float) * (size_t)span, stream) != cudaSuccess) {
-      cudaGetLastError();
-      return fail(EDTB200_ENOMEM, "no device memory for the copy of the long lines");
-    }
+    if (const int rc = copy.take(dc, sizeof(float) * (size_t)span, stream, "the copy of the long lines")) return rc;
     CUDA_TRY(cudaMemcpyAsync(copy.get(), in, sizeof(float) * (size_t)span, cudaMemcpyDeviceToDevice, stream));
     src = copy.get<float>();
   }

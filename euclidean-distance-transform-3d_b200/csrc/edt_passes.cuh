@@ -346,10 +346,7 @@ int launch_later(const void* labels, const RunBits* bits, float* f, const LineGe
   const size_t bytes = sizeof(float) * (size_t)lines * (size_t)g.n;
   Scratch tmp, hull;                            // freed on every exit, hull first
   CUDA_TRY(tmp.alloc(dc, bytes, stream));
-  if (hull.alloc(dc, bytes, stream) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the long-line scratch volumes");
-  }
+  if (const int rc = hull.take(dc, bytes, stream, "the long-line scratch volumes")) return rc;
   const int64_t blocks = (lines + 127) / 128;
   if (blocks > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many lines");
   later_axis_long_kernel<Bytes><<<(unsigned)blocks, 128, 0, stream>>>(
@@ -373,10 +370,8 @@ int launch_later_sites(const void* labels, const float* fin, float* fout, int* c
   const int64_t blocks = (lines + 127) / 128;
   if (blocks > 0x7fffffffLL) return fail(EDTB200_ELIMIT, "too many lines");
   Scratch hull;
-  if (hull.alloc(dc, sizeof(int) * (size_t)lines * (size_t)g.n, stream) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(EDTB200_ENOMEM, "no device memory for the long-line hull scratch");
-  }
+  if (const int rc = hull.take(dc, sizeof(int) * (size_t)lines * (size_t)g.n, stream, "the long-line hull scratch"))
+    return rc;
   later_axis_long_kernel<Bytes, true><<<(unsigned)blocks, 128, 0, stream>>>(
       static_cast<const LT*>(labels), fin, fout, hull.get<int>(), g, w * w, border_lo, border_hi, flags,
       arith.exact ? 4096 : 0, codes);

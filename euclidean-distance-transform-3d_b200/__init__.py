@@ -25,6 +25,7 @@ above accepts device-resident input directly (a torch CUDA tensor or any object 
 """
 import collections
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -50,6 +51,9 @@ FLAG_LABELS_FLOAT = 16
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
+
+_TOO_MANY_DIMS = "Multi-Label EDT library only supports up to 3 dimensions got {}."
+_GRAPH_DIMS = "Voxel connectivity graph is only supported for 2D and 3D. Got {}."
 
 ECUDA = -2                # EDTB200_ECUDA
 ENOMEM = -3               # EDTB200_ENOMEM
@@ -334,88 +338,11 @@ def _result_buffer(count):
   return np.frombuffer(block, dtype=np.float32, count=count)
 
 
-def _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes=None, bound=None):
-  """`max_device_bytes` (an int) streams the volume through one GPU in chunks within that budget
-  (edtb200_transform_chunked).  With None, a 2-D / 3-D volume whose one-shot transform runs out of
-  device memory is retried once that way, with the budget the device has free.  `bound`: the
-  bounded transform's max_distance (edtb200_transform_bounded, one shot only)."""
-  nd = data.ndim
-  order = "F" if data.flags.f_contiguous else "C"
-  if not data.flags.c_contiguous and not data.flags.f_contiguous:
-    data = np.ascontiguousarray(data)
-  labels = _label_view(data)
-  if labels is None:
-    return np.zeros(data.shape, dtype=np.float32, order=order)
-  (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
-  out = _result_buffer(data.size)
-  lib = _lib()
-  if isinstance(device, (list, tuple, range)) or (isinstance(device, np.ndarray) and device.ndim == 1):
-    # several GPUs of this process share ONE host volume (edtb200_transform_multi): Z slabs for the
-    # X / Y passes, Y slabs for the Z pass, re-partitioned over NVLink; exact for any input
-    devs = [int(d) for d in device]
-    arr = (ctypes.c_int * len(devs))(*devs)
-    _check(lib.edtb200_transform_multi(
-      labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz,
-      int(bool(black_border)), int(flags), out.ctypes.data, arr, len(devs)))
-    return out.reshape(data.shape, order=order)
-  args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), int(flags),
-          out.ctypes.data, int(device))
-  if bound is not None:
-    _check(lib.edtb200_transform_bounded(*args, None, bound))
-    return out.reshape(data.shape, order=order)
-  if max_device_bytes is None:
-    try:
-      _check(lib.edtb200_transform(*args, None))
-      return out.reshape(data.shape, order=order)
-    except EDTError as e:
-      if e.code != ENOMEM or nd not in (2, 3):
-        raise
-    max_device_bytes = 0                    # too large for the device: stream it through in chunks
-  _check(lib.edtb200_transform_chunked(*args, int(max_device_bytes), None))
-  return out.reshape(data.shape, order=order)
-
-
 def _graph_bytes(voxel_graph, order):
   """The graph as uint8 in the data's memory order (src/edt.pyx:294-298, 527-530)."""
   g = np.asarray(voxel_graph)
   g = np.ascontiguousarray(g) if order == "C" else np.asfortranarray(g)
   return g.view(np.uint8) if g.dtype in (np.uint8, np.int8) else g.astype(np.uint8)
-
-
-def _transform_voxel_graph_host(data, voxel_graph, anisotropy, black_border, flags, device):
-  """__edt2dsq_voxel_graph / __edt3dsq_voxel_graph, src/edt.pyx:514-620, 736-844.  A one-shot call
-  that runs out of device memory is retried once through edtb200_transform_voxel_graph_chunked, with
-  the budget the device has free."""
-  order = "F" if data.flags.f_contiguous else "C"
-  if not data.flags.c_contiguous and not data.flags.f_contiguous:
-    data = np.ascontiguousarray(data)
-  graph = _graph_bytes(voxel_graph, order)
-  if graph.shape != data.shape:
-    raise ValueError("voxel_graph must have the shape of data")
-  dt = data.dtype
-  if dt == np.bool_:
-    labels = data.view(np.uint8)
-  elif dt.kind in "iu" and dt.itemsize in (1, 2, 4, 8):
-    labels = data.view(np.dtype("u%d" % dt.itemsize))
-  elif dt in (np.float32, np.float64):
-    labels, flags = data, flags | FLAG_LABELS_FLOAT
-  else:
-    return np.zeros(data.shape, dtype=np.float32, order=order)   # no branch in the reference either
-  (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
-  out = np.empty(data.size, dtype=np.float32)
-  if isinstance(device, (list, tuple)):
-    device = device[0]                      # the graph transform runs on one GPU
-  lib = _lib()
-  args = (labels.ctypes.data, labels.dtype.itemsize, graph.ctypes.data, data.ndim, sx, sy, sz, wx, wy, wz,
-          int(bool(black_border)), int(flags), out.ctypes.data, int(device))
-  try:
-    _check(lib.edtb200_transform_voxel_graph(*args, None))
-  except EDTError as e:
-    if e.code != ENOMEM:
-      raise
-    # the doubled grid does not fit the device: stream it through in chunks
-    _check(lib.edtb200_transform_voxel_graph_chunked(*args, 0, None))
-  return out.reshape(data.shape, order=order)
 
 
 def _device_array(data):
@@ -444,124 +371,191 @@ def _device_array(data):
   return None
 
 
-def _front_door_device(t, anisotropy, black_border, voxel_graph, flags, fixed_dims, bound=None):
-  """Device-resident input to the reference-named functions: same semantics, result returned as a
-  torch CUDA tensor (which itself exports DLPack and `__cuda_array_interface__`).  A Fortran-ordered
-  array is transformed through its transposed (C-ordered) view with the anisotropy reversed, which
-  is exactly the axis mapping of src/edt.pyx:651-664, so the memory order is preserved without a copy."""
-  import torch
-  dims = t.dim()
-  if fixed_dims is not None and dims != fixed_dims:
-    raise ValueError("expected a %d-D array, got %d-D" % (fixed_dims, dims))
-  if dims > 3:
-    raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
-  if voxel_graph is not None and dims not in (2, 3):
-    raise TypeError("Voxel connectivity graph is only supported for 2D and 3D. Got {}.".format(dims))
-  if t.numel() == 0:
-    return torch.zeros(t.shape, dtype=torch.float32, device=t.device)
-  if t.dtype in (torch.float32, torch.float64):
-    if voxel_graph is not None:
-      # with a graph the labels only say foreground / background, and for floats the reference
-      # tests `labels[loc] > 0` (src/edt_voxel_graph.hpp:76, 151): negative values and NaN are
-      # background, exactly as on the host path (EDTB200_LABELS_FLOAT)
-      t = (t > 0).to(torch.uint8)
-    else:
-      # labels compare by value (src/edt.pyx:704-722): fold -0.0 onto +0.0, then use the raw bits
-      t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)
+def _weights(n, anisotropy, rule="volume"):
+  """One float weight for each of `n` axes; None gives 1.0 each.  How a scalar and a sequence count is the
+  caller's `rule`:
+    "volume"  stacks and the whole-volume operations: a scalar for one axis, else the entries of any shape;
+    "first"   a single host volume, and feature_transform, as src/edt.pyx takes them: a 1-D volume takes a
+              scalar or the first entry, more axes iterate the entries (a scalar is a TypeError);
+    "wrap"    a single device volume of the edt family: a scalar is one entry;
+    "cuda"    edt_cuda and transform_batch: a scalar for one axis, more axes iterate the entries."""
   if anisotropy is None:
-    anisotropy = (1.0,) * dims
-  elif np.ndim(anisotropy) == 0:
-    anisotropy = (float(anisotropy),)
-  else:
-    anisotropy = tuple(float(a) for a in anisotropy)
-  if len(anisotropy) != dims:
+    return (1.0,) * n
+  if rule == "volume":
+    if np.ndim(anisotropy) == 0 and n == 1:
+      return (float(anisotropy),)
+    weights = tuple(float(a) for a in np.asarray(anisotropy).reshape(-1))
+    if len(weights) != n:
+      raise ValueError("anisotropy must have one entry per volume axis (%d), got %d" % (n, len(weights)))
+    return weights
+  if np.ndim(anisotropy) == 0 and (n == 1 or rule == "wrap"):
+    anisotropy = (anisotropy,)
+  elif n == 1 and rule == "first":
+    anisotropy = (np.asarray(anisotropy).reshape(-1)[0],)
+  weights = tuple(float(a) for a in anisotropy)
+  if len(weights) != n:
     raise ValueError("anisotropy must have one entry per dimension")
-  fortran = dims > 1 and not t.is_contiguous() and t.permute(*reversed(range(dims))).is_contiguous()
-  if fortran:
-    t = t.permute(*reversed(range(dims)))
-    anisotropy = tuple(reversed(anisotropy))
-  graph = None
-  if voxel_graph is not None:
-    graph = _device_array(voxel_graph)
-    if graph is None:
-      graph = torch.as_tensor(np.ascontiguousarray(voxel_graph), device=t.device)
-    if graph.dtype not in (torch.uint8, torch.int8):
-      graph = graph.to(torch.uint8)
-    if fortran:
-      graph = graph.permute(*reversed(range(dims)))
-    graph = graph.contiguous()
-  sqrt, signed = bool(flags & FLAG_SQRT), bool(flags & FLAG_SIGNED)
-  if graph is not None and signed:       # f(data) - f(data == 0), src/edt.pyx:147-158
-    out = edt_cuda(t, anisotropy, black_border, sqrt=sqrt, voxel_graph=graph)
-    out -= edt_cuda(t == 0, anisotropy, black_border, sqrt=sqrt, voxel_graph=graph)
-  else:
-    out = edt_cuda(t, anisotropy, black_border, sqrt=sqrt, signed=signed, voxel_graph=graph, max_distance=bound)
-  return out.permute(*reversed(range(dims))) if fortran else out
+  return weights
 
 
-def _chunk_budget(max_device_bytes, on_device, voxel_graph, dims):
-  """max_device_bytes as an int, after rejecting what the chunked transform does not cover."""
+class _Volume:
+  """The input of one transform or whole-volume operation, resolved for its C ABI call.  A numpy array (or a
+  list) gives numpy results; a device array (a torch CUDA tensor or any __cuda_array_interface__ object)
+  gives torch CUDA results computed on its current stream.  With `stacked` the slowest axis in memory
+  indexes same-shaped volumes.  Given `dims`, the (least, most) dimensions of one volume, the number of
+  dimensions is checked as the whole-volume operations check it and the memory order is fixed at once;
+  the transforms check the dimensions with their own messages and then call order()."""
+
+  def __init__(self, name, data, stacked=False, dims=None, device=0):
+    t = _device_array(data)
+    self.on_device = t is not None
+    self.arr = t if self.on_device else np.asarray(data)
+    self.nd = self.arr.dim() if self.on_device else self.arr.ndim
+    self.stacked = 1 if stacked else 0
+    self.vnd = self.nd - self.stacked
+    self.name, self._device = name, device
+    if dims is not None:
+      lo, hi = dims[0] + self.stacked, dims[1] + self.stacked
+      if not lo <= self.nd <= hi:
+        raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D"
+                        % (name, "stacked=True" if stacked else "it", lo, hi, self.nd))
+      self.order()
+
+  def order(self, f_first=False, c_only=False):
+    """Make `arr` C- or F-contiguous: C where both apply (F with `f_first`, as a single host volume of the
+    transforms is read), a strided array copied to C order (any non-C tensor, with `c_only`).  The C ABI
+    reads an F-ordered one as its C-ordered transpose, with the weights reversed."""
+    arr, self.shape = self.arr, tuple(self.arr.shape)
+    if self.on_device:
+      contiguous = arr.is_contiguous()
+      self.fortran = (not (contiguous or c_only) and self.nd > 1
+                      and arr.permute(*reversed(range(self.nd))).is_contiguous())
+      if not contiguous and not self.fortran:
+        arr = arr.contiguous()
+      self.size, self.flags = math.prod(self.shape), FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
+    else:
+      flags = arr.flags
+      if not (flags.c_contiguous or flags.f_contiguous):
+        arr = np.ascontiguousarray(arr)
+        flags = arr.flags
+      self.fortran = flags.f_contiguous and (f_first or not flags.c_contiguous)
+      self.size, self.flags = arr.size, 0
+    self.arr, self.dtype = arr, arr.dtype
+    return self
+
+  def set_weights(self, anisotropy, positive=True, rule="volume"):
+    """One weight per volume axis by `rule` (see _weights; None: `anisotropy` is that tuple already), and with
+    `positive` each finite and > 0; sets `geometry`, the vnd, sx, sy, sz, count, wx, wy, wz of the C ABI call."""
+    weights = anisotropy if rule is None else _weights(self.vnd, anisotropy, rule)
+    if positive:
+      for w in weights:
+        if not (np.isfinite(w) and w > 0.0):
+          raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (self.name, anisotropy))
+    dims, count = self.shape, 1
+    if not self.fortran:                    # x-fastest: the last axis of a C-ordered array first
+      dims, weights = dims[::-1], weights[::-1]
+    if self.stacked:                        # the slowest axis in memory indexes the volumes
+      dims, count = dims[:-1], dims[-1]
+    pad = 3 - self.vnd
+    (sx, sy, sz), (wx, wy, wz) = dims + (1,) * pad, tuple(weights) + (1.0,) * pad
+    self.geometry = (self.vnd, sx, sy, sz, count, wx, wy, wz)
+    self.volume_geometry = (self.vnd, sx, sy, sz, wx, wy, wz)       # of a C ABI call on one volume
+
+  def labels(self):
+    """(raw, nbytes): the label bits the C ABI compares -- floats by value (-0.0 folded onto +0.0),
+    unsigned and bool labels as the integers of their width -- or None for a dtype it does not take."""
+    if not self.on_device:
+      raw = _label_view(self.arr)
+      return None if raw is None else (raw, raw.dtype.itemsize)
+    import torch
+    t = self.arr
+    raw = _torch_raw_labels(torch).get(t.dtype)
+    if raw is None:
+      return None
+    if t.dtype in (torch.float32, torch.float64):
+      t = t + 0
+    return (t if raw is t.dtype else t.view(raw)), t.element_size()
+
+  @property
+  def floating(self):
+    return self.dtype.is_floating_point if self.on_device else self.dtype.kind == "f"
+
+  @property
+  def ptr(self):
+    return self.ptr_of(self.arr)
+
+  def ptr_of(self, x):
+    """The address of `x`, an array on the input's side (None: None)."""
+    if x is None:
+      return None
+    return x.data_ptr() if self.on_device else x.ctypes.data
+
+  @property
+  def where(self):
+    """The device and stream of the C ABI call."""
+    if not self.on_device:
+      return int(self._device), None
+    import torch
+    device = self.arr.device
+    return device.index, ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+  def empty(self, dtype=None, planes=None):
+    """An output in the input's shape and memory order, or with `planes=k` k of them as one array of
+    shape (k,) + shape.  `dtype`: a name numpy and torch share ("bool", "int32", "float32"), None for the
+    input's."""
+    lead = () if planes is None else (planes,)
+    shape = lead + (self.shape[::-1] if self.fortran else self.shape)     # as the C ABI reads the input
+    if not self.on_device:
+      dtype = self.dtype if dtype is None else dtype
+      if not lead:
+        return np.empty(self.shape, dtype, order="F" if self.fortran else "C")
+      out = np.empty(shape, dtype)
+    else:
+      import torch
+      out = torch.empty(shape, dtype=self.dtype if dtype is None else getattr(torch, dtype), device=self.arr.device)
+    if not self.fortran:
+      return out
+    back = tuple(range(len(lead))) + tuple(range(out.ndim - 1, len(lead) - 1, -1))
+    return out.permute(*back) if self.on_device else out.transpose(back)
+
+  def upload(self, device):
+    """The ordered host array as a torch tensor on `device`, in its memory order: float labels as they are,
+    others as the integers of their width that torch takes (uint8 for one byte, else signed)."""
+    import torch
+    arr = self.arr
+    raw = arr if self.floating else arr.view(np.uint8 if arr.itemsize == 1 else np.dtype("i%d" % arr.itemsize))
+    return torch.from_numpy(raw).to(device)
+
+  def shaped(self, flat):
+    """A flat host buffer of `size` elements viewed in the input's shape and memory order."""
+    return flat.reshape(self.shape, order="F" if self.fortran else "C")
+
+  def plane_ptrs(self, planes):
+    """The C ABI's x-fastest index planes of `planes` (made by empty(planes=vnd)): plane j is the caller's
+    axis j of an F-ordered input and axis vnd - 1 - j of a C-ordered one (within a volume, for a stack)."""
+    axes = range(self.vnd) if self.fortran else range(self.vnd - 1, -1, -1)
+    ptrs = [planes[k].data_ptr() for k in axes] if self.on_device else [planes[k].ctypes.data for k in axes]
+    return (ctypes.c_void_p * self.vnd)(*ptrs)
+
+
+def _chunk_budget(max_device_bytes, on_device=False, voxel_graph=None, dims=None, staged=False):
+  """max_device_bytes as an int, after rejecting what the chunked and stacked transforms do not cover: a
+  budget for a device-resident array or with a voxel graph, for a single volume (`dims`) not of 2 or 3
+  dimensions, and any budget for a stack that is `staged` on the GPU whole."""
+  if staged:
+    raise ValueError("stacked=True stages the whole stack on the GPU at once; it cannot be combined with "
+                     "max_device_bytes")
   if on_device:
     raise ValueError("max_device_bytes streams a host array through the GPU; a device-resident array already fits")
   if voxel_graph is not None:
     raise ValueError("max_device_bytes cannot be combined with voxel_graph")
-  if dims not in (2, 3):
+  if dims is not None and dims not in (2, 3):
     raise ValueError("max_device_bytes needs a 2-D or 3-D array, got %d-D" % dims)
   budget = int(max_device_bytes)
   if budget < 0:
     raise ValueError("max_device_bytes must be non-negative (0: what the device has free)")
   return budget
 
-
-def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None, max_device_bytes=None,
-                stacked=False, bound=None):
-  """Argument handling of edtsq(), src/edt.pyx:276-310.  bound: max_distance after _bound."""
-  if stacked:
-    return _stack_front_door(data, anisotropy, black_border, voxel_graph, flags, device, max_device_bytes)
-  on_device = _device_array(data)
-  if on_device is not None:
-    if max_device_bytes is not None:
-      _chunk_budget(max_device_bytes, True, voxel_graph, on_device.dim())
-    return _front_door_device(on_device, anisotropy, black_border, voxel_graph, flags, fixed_dims, bound)
-  if isinstance(data, list):
-    data = np.array(data)
-  data = np.asarray(data)
-  dims = data.ndim
-  if fixed_dims is not None and dims != fixed_dims:
-    raise ValueError("expected a %d-D array, got %d-D" % (fixed_dims, dims))
-  if max_device_bytes is not None:
-    max_device_bytes = _chunk_budget(max_device_bytes, False, voxel_graph, dims)
-  if data.size == 0:
-    return np.zeros(shape=data.shape, dtype=np.float32)
-  if voxel_graph is not None:
-    if dims not in (2, 3):
-      raise TypeError("Voxel connectivity graph is only supported for 2D and 3D. Got {}.".format(dims))
-    anisotropy = nvl(anisotropy, (1.0,) * dims)
-    if flags & FLAG_SIGNED:
-      # sdf / sdfsq with a graph: f(data) - f(data == 0), both under the graph (src/edt.pyx:147-158)
-      dt = _transform_voxel_graph_host(data, voxel_graph, anisotropy, black_border, flags & ~FLAG_SIGNED, device)
-      dt -= _transform_voxel_graph_host(data == 0, voxel_graph, anisotropy, black_border, flags & ~FLAG_SIGNED,
-                                        device)
-      return dt
-    return _transform_voxel_graph_host(data, voxel_graph, anisotropy, black_border, flags, device)
-  if dims == 1:
-    anisotropy = nvl(anisotropy, 1.0)
-    if np.ndim(anisotropy) != 0:
-      anisotropy = np.asarray(anisotropy).reshape(-1)[0]
-    anisotropy = (float(anisotropy),)
-  elif dims == 2:
-    anisotropy = nvl(anisotropy, (1.0, 1.0))
-  elif dims == 3:
-    anisotropy = nvl(anisotropy, (1.0, 1.0, 1.0))
-  else:
-    raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
-  return _transform_host(data, anisotropy, black_border, flags, device, max_device_bytes, bound)
-
-
-# ---------------------------------------------------------------------------------------
-# stacks: same-shaped volumes along the slowest axis in memory, each transformed on its own with
-# one launch per pass for all of them (edtb200_transform_stack, edtb200_feature_transform_stack)
-# ---------------------------------------------------------------------------------------
 
 def _stack_dims(dims, voxel_graph=None):
   """The volume ndim of a stacked array of `dims` dimensions, after rejecting what stacks do not cover."""
@@ -573,76 +567,148 @@ def _stack_dims(dims, voxel_graph=None):
   return dims - 1
 
 
-def _volume_anisotropy(vnd, anisotropy):
-  """One weight per volume axis (a scalar for 1-D volumes); default 1."""
-  if anisotropy is None:
-    return (1.0,) * vnd
-  if np.ndim(anisotropy) == 0 and vnd == 1:
-    return (float(anisotropy),)
-  weights = tuple(float(a) for a in np.asarray(anisotropy).reshape(-1))
-  if len(weights) != vnd:
-    raise ValueError("anisotropy must have one entry per volume axis (%d), got %d" % (vnd, len(weights)))
-  return weights
+def _transform(v, labels, nbytes, black_border, flags, out, budget=None, bound=None, graph=None):
+  """The distance transform of the resolved volume `v` from the raw label bits `labels` into `out`,
+  through the entry point the arguments ask for: edtb200_transform_multi for a single host volume
+  on several GPUs, _stack for a stack (budget: its groups' device memory), _voxel_graph with a
+  graph, _bounded with a bound, _chunked with a budget, else edtb200_transform.  A one-shot host
+  transform that runs out of device memory (of a 2-D / 3-D volume, or any voxel graph) is
+  streamed through one GPU in chunks instead."""
+  lib = _lib()
+  bb, flags, device = int(bool(black_border)), int(flags) | v.flags, v._device
+  if not (v.on_device or v.stacked or graph is not None) and (
+      isinstance(device, (list, tuple, range)) or (isinstance(device, np.ndarray) and device.ndim == 1)):
+    # several GPUs of this process share ONE host volume (edtb200_transform_multi): Z slabs for the
+    # X / Y passes, Y slabs for the Z pass, re-partitioned over NVLink; exact for any input
+    devs = [int(d) for d in device]
+    _check(lib.edtb200_transform_multi(v.ptr_of(labels), nbytes, *v.volume_geometry, bb, flags, v.ptr_of(out),
+                                       (ctypes.c_int * len(devs))(*devs), len(devs)))
+    return
+  device, stream = v.where
+  if v.stacked:
+    _check(lib.edtb200_transform_stack(v.ptr_of(labels), nbytes, *v.geometry, bb, flags, v.ptr_of(out), device,
+                                       budget, None, stream))
+    return
+  if graph is not None:
+    one_shot, chunked = lib.edtb200_transform_voxel_graph, lib.edtb200_transform_voxel_graph_chunked
+    args = (v.ptr_of(labels), nbytes, v.ptr_of(graph)) + v.volume_geometry + (bb, flags, v.ptr_of(out), device)
+  else:
+    one_shot, chunked = lib.edtb200_transform, lib.edtb200_transform_chunked
+    args = (v.ptr_of(labels), nbytes) + v.volume_geometry + (bb, flags, v.ptr_of(out), device)
+  if bound is not None:
+    _check(lib.edtb200_transform_bounded(*args, stream, bound))
+    return
+  if budget is None:
+    try:
+      _check(one_shot(*args, stream))
+      return
+    except EDTError as e:
+      if e.code != ENOMEM or v.on_device or (graph is None and v.nd not in (2, 3)):
+        raise
+    budget = 0                              # too large for the device: stream it through in chunks
+  _check(chunked(*args, budget, stream))
 
 
-def _stack_layout(shape, c_order, anisotropy):
-  """count, (sx, sy, sz), (wx, wy, wz) of a stack of `shape`: the slowest axis in memory (axis 0 in C
-  order, the last axis in F order) indexes the volumes, the others are one volume."""
-  count = int(shape[0] if c_order else shape[-1])
-  dims, weights = _x_fastest(shape[1:] if c_order else shape[:-1], anisotropy, not c_order)
-  return count, dims, weights
+def _voxel_graph(v, voxel_graph, anisotropy, rule, black_border, flags):
+  """__edt2dsq_voxel_graph / __edt3dsq_voxel_graph, src/edt.pyx:514-620, 736-844, of a resolved volume; with
+  FLAG_SIGNED f(data) - f(data == 0), both under the graph (src/edt.pyx:147-158).  The labels only say
+  foreground / background, and for floats the reference tests `labels[loc] > 0`
+  (src/edt_voxel_graph.hpp:76, 151): negative values and NaN are background, on the host through
+  EDTB200_LABELS_FLOAT and on the device as a uint8 mask."""
+  signed = bool(flags & FLAG_SIGNED)
+  flags &= ~FLAG_SIGNED
+  if v.on_device:
+    import torch
+    labels = ((v.arr > 0).to(torch.uint8), 1) if v.dtype in (torch.float32, torch.float64) else v.labels()
+    if labels is None:
+      raise TypeError("edt_cuda: unsupported label dtype %s" % v.dtype)
+    graph = _device_array(voxel_graph)
+    if graph is None:
+      graph = torch.as_tensor(np.ascontiguousarray(voxel_graph), device=v.arr.device)
+    if graph.dtype not in (torch.uint8, torch.int8):
+      graph = graph.to(torch.uint8)
+    if not (graph.device == v.arr.device and tuple(graph.shape) == v.shape):
+      raise ValueError("edt_cuda: voxel_graph must be a uint8/int8 CUDA tensor shaped like labels")
+    graph = (graph.permute(*reversed(range(v.nd))) if v.fortran else graph).contiguous()
+    new = lambda: v.empty("float32")
+    background = lambda: (labels[0] == 0).view(torch.uint8)
+  else:
+    graph = _graph_bytes(voxel_graph, "F" if v.fortran else "C")
+    if graph.shape != v.shape:
+      raise ValueError("voxel_graph must have the shape of data")
+    if v.dtype in (np.float32, np.float64):
+      labels, flags = (v.arr, v.arr.itemsize), flags | FLAG_LABELS_FLOAT
+    else:
+      labels = v.labels()
+    new = lambda: v.shaped(np.empty(v.size, dtype=np.float32))
+    background = lambda: (v.arr == 0).view(np.uint8)
+  if labels is None:                        # no branch in the reference: f(data) is zeros
+    out = np.zeros(v.shape, dtype=np.float32, order="F" if v.fortran else "C")
+    if not signed:
+      return out
+  v.set_weights(anisotropy, positive=False, rule=rule)
+  if labels is not None:
+    out = new()
+    _transform(v, *labels, black_border, flags, out, graph=graph)
+  if signed:
+    other = new()
+    _transform(v, background(), 1, black_border, flags & ~FLAG_LABELS_FLOAT, other, graph=graph)
+    out -= other
+  return out
 
 
-def _stack_order(data):
-  """Memory order of a stacked numpy array ("C" wins where both apply), made contiguous if it is neither."""
-  if not data.flags.c_contiguous and not data.flags.f_contiguous:
-    data = np.ascontiguousarray(data)
-  return data, ("C" if data.flags.c_contiguous else "F")
-
-
-def _stack_front_door(data, anisotropy, black_border, voxel_graph, flags, device, max_device_bytes):
-  """edtsq(..., stacked=True) and friends: host arrays go through the GPU in groups of whole volumes
-  within `max_device_bytes` (None or 0: what the GPU has free); device arrays in one call."""
-  on_device = _device_array(data)
-  if on_device is None:
-    data = np.asarray(np.array(data) if isinstance(data, list) else data)
-  vnd = _stack_dims(on_device.dim() if on_device is not None else data.ndim, voxel_graph)
-  anisotropy = _volume_anisotropy(vnd, anisotropy)
-  if on_device is not None:
+def _front_door(data, anisotropy, black_border, voxel_graph, flags, device, fixed_dims=None, max_device_bytes=None,
+                stacked=False, bound=None):
+  """Argument handling of edtsq(), src/edt.pyx:276-310, for host and device arrays and stacks.  bound:
+  max_distance after _bound.  `max_device_bytes` streams a 2-D / 3-D host volume through one GPU in chunks
+  within that budget, and with None a one-shot transform that runs out of device memory is retried once
+  that way; for a host stack it is the budget of the groups of whole volumes that go through the GPU."""
+  v = _Volume("edt", data, stacked, device=device[0] if voxel_graph is not None and isinstance(device, (list, tuple))
+              else device)
+  nd, rule = v.nd, "first"                 # a single host volume takes its weights as src/edt.pyx does
+  if stacked:
+    _stack_dims(nd, voxel_graph)
+    anisotropy, rule = _weights(v.vnd, anisotropy), None
+    max_device_bytes = 0 if max_device_bytes is None else _chunk_budget(max_device_bytes, v.on_device)
+  else:
+    if v.on_device and max_device_bytes is not None:
+      _chunk_budget(max_device_bytes, True)
+    if fixed_dims is not None and nd != fixed_dims:
+      raise ValueError("expected a %d-D array, got %d-D" % (fixed_dims, nd))
     if max_device_bytes is not None:
-      raise ValueError("max_device_bytes streams a host array through the GPU; a device-resident array already fits")
-    return _stack_device(on_device, anisotropy, black_border, flags)
-  budget = 0 if max_device_bytes is None else int(max_device_bytes)
-  if budget < 0:
-    raise ValueError("max_device_bytes must be non-negative (0: what the device has free)")
-  data, order = _stack_order(data)
-  labels = _label_view(data) if data.size else None
+      max_device_bytes = _chunk_budget(max_device_bytes, False, voxel_graph, nd)
+  if v.on_device:
+    import torch
+    if not stacked:
+      if nd > 3:
+        raise TypeError(_TOO_MANY_DIMS.format(nd))
+      if voxel_graph is not None and nd not in (2, 3):
+        raise TypeError(_GRAPH_DIMS.format(nd))
+    if v.arr.numel() == 0:
+      return torch.zeros(v.arr.shape, dtype=torch.float32, device=v.arr.device)
+    if not stacked:
+      anisotropy, rule = _weights(nd, anisotropy, "wrap"), None
+      if nd < 1:
+        raise TypeError(_TOO_MANY_DIMS.format(nd))
+  elif not stacked:
+    if v.arr.size == 0:
+      return np.zeros(shape=v.arr.shape, dtype=np.float32)
+    if voxel_graph is not None and nd not in (2, 3):
+      raise TypeError(_GRAPH_DIMS.format(nd))
+    if voxel_graph is None and not 1 <= nd <= 3:
+      raise TypeError(_TOO_MANY_DIMS.format(nd))
+  v.order(f_first=not (stacked or v.on_device))
+  if voxel_graph is not None:
+    return _voxel_graph(v, voxel_graph, anisotropy, rule, black_border, flags)
+  labels = v.labels() if v.size else None
   if labels is None:
-    return np.zeros(data.shape, dtype=np.float32, order=order)
-  count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(data.shape, order == "C", anisotropy)
-  out = _result_buffer(data.size)
-  _check(_lib().edtb200_transform_stack(
-    labels.ctypes.data, labels.dtype.itemsize, vnd, sx, sy, sz, count, wx, wy, wz, int(bool(black_border)),
-    int(flags), out.ctypes.data, int(device), budget, None, None))
-  return out.reshape(data.shape, order=order)
-
-
-def _stack_device(t, anisotropy, black_border, flags):
-  """A device-resident stack: an F-ordered one goes through its transposed (C-ordered) view, whose axis 0
-  is then the volume index, with the volume's anisotropy reversed."""
-  import torch
-  dims = t.dim()
-  if t.numel() == 0:
-    return torch.zeros(t.shape, dtype=torch.float32, device=t.device)
-  if t.dtype in (torch.float32, torch.float64):
-    t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)     # -0.0 == +0.0
-  fortran = not t.is_contiguous() and t.permute(*reversed(range(dims))).is_contiguous()
-  if fortran:
-    t = t.permute(*reversed(range(dims)))
-    anisotropy = tuple(reversed(anisotropy))
-  out = edt_cuda(t, anisotropy, black_border, sqrt=bool(flags & FLAG_SQRT), signed=bool(flags & FLAG_SIGNED),
-                 stacked=True)
-  return out.permute(*reversed(range(dims))) if fortran else out
+    if v.on_device:
+      raise TypeError("edt_cuda: unsupported label dtype %s" % v.dtype)
+    return np.zeros(v.shape, dtype=np.float32, order="F" if v.fortran else "C")
+  v.set_weights(anisotropy, positive=False, rule=rule)
+  out = v.empty("float32") if v.on_device else v.shaped(_result_buffer(v.size))
+  _transform(v, *labels, black_border, flags, out, max_device_bytes, bound)
+  return out
 
 
 # ---------------------------------------------------------------------------------------
@@ -666,7 +732,7 @@ def _pick(device, devices, max_device_bytes=None, stacked=False):
 # `max_device_bytes=N` (every function below but the 1-D ones) streams a 2-D / 3-D host array
 # through one GPU in chunks that fit N bytes of device memory (0: what the GPU has free), with the
 # result of the one-shot transform bit for bit; with None a one-shot transform that runs out of
-# device memory falls back to that once (see _transform_host).
+# device memory falls back to that once (see _transform).
 #
 # `stacked=True` (edt, edtsq, sdf, sdfsq, edt_cuda, feature_transform, expand_labels) takes a 2-D to
 # 4-D array whose slowest axis in memory (axis 0 of a C-ordered array, the last of an F-ordered one) indexes
@@ -687,7 +753,7 @@ def _pick(device, devices, max_device_bytes=None, stacked=False):
 def edtsq(data, anisotropy=None, black_border=False, parallel=1, voxel_graph=None, order=None,
           *, device=0, devices=None, max_device_bytes=None, stacked=False, max_distance=None):
   """Squared anisotropic multi-label EDT of a 1-D, 2-D or 3-D array (src/edt.pyx:245-310).
-  `devices=[0, 1, ...]` spreads one host volume over several GPUs (see _transform_host)."""
+  `devices=[0, 1, ...]` spreads one host volume over several GPUs (see _transform)."""
   bound = _bound(max_distance, voxel_graph, devices, stacked, max_device_bytes)
   return _front_door(data, anisotropy, black_border, voxel_graph, 0, _pick(device, devices, max_device_bytes, stacked),
                      max_device_bytes=max_device_bytes, stacked=stacked, bound=bound)
@@ -763,6 +829,7 @@ def edt3d(data, anisotropy=(1.0, 1.0, 1.0), black_border=False, parallel=1, voxe
 # ---------------------------------------------------------------------------------------
 
 _TORCH_LABEL_BYTES = None
+_TORCH_RAW_LABELS = None
 
 
 def _torch_label_bytes(torch):
@@ -775,6 +842,18 @@ def _torch_label_bytes(torch):
         table[getattr(torch, name)] = size
     _TORCH_LABEL_BYTES = table
   return _TORCH_LABEL_BYTES
+
+
+def _torch_raw_labels(torch):
+  """The dtype whose bits the C ABI compares, for each torch label dtype: floats by value (folded first),
+  unsigned and bool labels as the integers of their width."""
+  global _TORCH_RAW_LABELS
+  if _TORCH_RAW_LABELS is None:
+    signed = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}
+    table = {d: (d if d == torch.int8 else signed[n]) for d, n in _torch_label_bytes(torch).items()}
+    table.update({torch.float32: torch.int32, torch.float64: torch.int64})
+    _TORCH_RAW_LABELS = table
+  return _TORCH_RAW_LABELS
 
 
 def edt_cuda(labels, anisotropy=None, black_border=False, *, sqrt=False, signed=False, out=None,
@@ -790,60 +869,36 @@ def edt_cuda(labels, anisotropy=None, black_border=False, *, sqrt=False, signed=
   if not (isinstance(labels, torch.Tensor) and labels.is_cuda):
     raise TypeError("edt_cuda expects a torch CUDA tensor")
   bound = _bound(max_distance, voxel_graph, stacked=stacked)
-  nd = labels.dim()
+  v = _Volume("edt_cuda", labels, stacked)
+  nd = v.nd
   if stacked:
-    vnd = _stack_dims(nd, voxel_graph)
+    _stack_dims(nd, voxel_graph)
   elif nd < 1 or nd > 3:
-    raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(nd))
-  else:
-    vnd = nd
-  if not labels.is_contiguous():
-    labels = labels.contiguous()
-  nbytes = _torch_label_bytes(torch).get(labels.dtype)
+    raise TypeError(_TOO_MANY_DIMS.format(nd))
+  labels = v.order(c_only=True).arr
+  nbytes = _torch_label_bytes(torch).get(v.dtype)
   if nbytes is None:
-    raise TypeError("edt_cuda: unsupported label dtype %s" % labels.dtype)
+    raise TypeError("edt_cuda: unsupported label dtype %s" % v.dtype)
   if out is None:
-    out = torch.empty(labels.shape, dtype=torch.float32, device=labels.device)
+    out = torch.empty(v.shape, dtype=torch.float32, device=labels.device)
   elif not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()
             and out.shape == labels.shape and out.device == labels.device):
     raise ValueError("edt_cuda: `out` must be a contiguous float32 CUDA tensor of the same shape/device")
-  if labels.numel() == 0:
+  if v.size == 0:
     return out
-  if anisotropy is None:
-    anisotropy = (1.0,) * vnd
-  elif vnd == 1 and np.ndim(anisotropy) == 0:
-    anisotropy = (float(anisotropy),)
-  (sx, sy, sz), (wx, wy, wz) = _x_fastest(labels.shape[1:] if stacked else labels.shape, anisotropy, False)
-  flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
-  if sqrt:
-    flags |= FLAG_SQRT
-  if signed:
-    flags |= FLAG_SIGNED
-  stream = torch.cuda.current_stream(labels.device).cuda_stream
-  if stacked:
-    _check(_lib().edtb200_transform_stack(
-      labels.data_ptr(), nbytes, vnd, sx, sy, sz, int(labels.shape[0]), wx, wy, wz, int(bool(black_border)), flags,
-      out.data_ptr(), labels.device.index, 0, None, ctypes.c_void_p(stream)))
-    return out
+  v.set_weights(anisotropy, positive=False, rule="cuda")
   if voxel_graph is not None:
     if nd not in (2, 3):
-      raise TypeError("Voxel connectivity graph is only supported for 2D and 3D. Got {}.".format(nd))
+      raise TypeError(_GRAPH_DIMS.format(nd))
     if signed:
       raise ValueError("edt_cuda: with voxel_graph, form f(labels) - f(labels == 0) from two calls")
     if not (isinstance(voxel_graph, torch.Tensor) and voxel_graph.device == labels.device
             and voxel_graph.dtype in (torch.uint8, torch.int8) and voxel_graph.shape == labels.shape):
       raise ValueError("edt_cuda: voxel_graph must be a uint8/int8 CUDA tensor shaped like labels")
     voxel_graph = voxel_graph.contiguous()
-    _check(_lib().edtb200_transform_voxel_graph(
-      labels.data_ptr(), nbytes, voxel_graph.data_ptr(), nd, sx, sy, sz, wx, wy, wz,
-      int(bool(black_border)), flags, out.data_ptr(), labels.device.index, ctypes.c_void_p(stream)))
-    return out
-  args = (labels.data_ptr(), nbytes, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags, out.data_ptr(),
-          labels.device.index, ctypes.c_void_p(stream))
-  if bound is not None:
-    _check(_lib().edtb200_transform_bounded(*args, bound))
-  else:
-    _check(_lib().edtb200_transform(*args))
+  flags = (FLAG_SQRT if sqrt else 0) | (FLAG_SIGNED if signed else 0)
+  _transform(v, labels, nbytes, black_border, flags, out, budget=0 if stacked else None, bound=bound,
+             graph=voxel_graph)
   return out
 
 
@@ -860,7 +915,7 @@ def transform_batch(volumes, anisotropy=None, black_border=False, *, sqrt=False,
     return []
   first = vols[0]
   if first.ndim < 1 or first.ndim > 3:
-    raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(first.ndim))
+    raise TypeError(_TOO_MANY_DIMS.format(first.ndim))
   order = "F" if first.flags.f_contiguous else "C"
   fixed = []
   for v in vols:
@@ -892,11 +947,7 @@ def transform_batch(volumes, anisotropy=None, black_border=False, *, sqrt=False,
       o[...] = 0
     return outs
   nd = first.ndim
-  if anisotropy is None:
-    anisotropy = (1.0,) * nd
-  elif nd == 1 and np.ndim(anisotropy) == 0:
-    anisotropy = (float(anisotropy),)
-  (sx, sy, sz), (wx, wy, wz) = _x_fastest(first.shape, anisotropy, order == "F")
+  (sx, sy, sz), (wx, wy, wz) = _x_fastest(first.shape, _weights(nd, anisotropy, "cuda"), order == "F")
   n = len(views)
   lab_ptrs = (ctypes.c_void_p * n)(*[v.ctypes.data for v in views])
   out_ptrs = (ctypes.c_void_p * n)(*[o.ctypes.data for o in outs])
@@ -910,125 +961,36 @@ def transform_batch(volumes, anisotropy=None, black_border=False, *, sqrt=False,
 # feature transform: WHERE the nearest boundary is (scipy's return_indices), and expand_labels
 # ---------------------------------------------------------------------------------------
 
-def _feature_anisotropy(dims, anisotropy):
-  """Default and 1-D anisotropy handling of _front_door."""
-  if dims == 1:
-    anisotropy = nvl(anisotropy, 1.0)
-    if np.ndim(anisotropy) != 0:
-      anisotropy = np.asarray(anisotropy).reshape(-1)[0]
-    return (float(anisotropy),)
-  if dims in (2, 3):
-    anisotropy = tuple(float(a) for a in nvl(anisotropy, (1.0,) * dims))
-    if len(anisotropy) != dims:
-      raise ValueError("anisotropy must have one entry per dimension")
-    return anisotropy
-  raise TypeError("Multi-Label EDT library only supports up to 3 dimensions got {}.".format(dims))
-
-
-def _feature_host(data, anisotropy, black_border, flags, want_dist, device, max_device_bytes=None, stacked=False,
-                  bound=None):
-  """(distances or None, indices) of a numpy array through host buffers (edtb200_feature_transform).
-  `max_device_bytes` (an int) streams a 2-D / 3-D array through one GPU in chunks within that budget
-  (edtb200_feature_transform_chunked); with None a one-shot call that runs out of device memory is
-  retried once that way, as _transform_host does.  stacked: a stack of volumes along the slowest axis
-  in memory (edtb200_feature_transform_stack), one index plane per volume axis.  bound: the bounded
-  feature transform's max_distance (edtb200_feature_transform_bounded, one shot only)."""
-  if isinstance(data, list):
-    data = np.array(data)
-  data = np.asarray(data)
-  nd = data.ndim
-  vnd = nd - 1 if stacked else nd           # index planes: one per (volume) axis
-  if stacked:
-    anisotropy = _volume_anisotropy(vnd, anisotropy)
-    data, order = _stack_order(data)
-  else:
-    anisotropy = _feature_anisotropy(nd, anisotropy)
-    if not data.flags.c_contiguous and not data.flags.f_contiguous:
-      data = np.ascontiguousarray(data)
-    order = "F" if data.flags.f_contiguous else "C"
-  labels = _label_view(data)
+def _feature(v, black_border, flags, want_dist, budget=None, bound=None):
+  """(distances or None, indices) of the resolved volume `v`, its order and weights set: the index planes
+  from empty(planes=vnd), the distances zeroed first.  The entry point follows the arguments as in
+  _transform, a one-shot host call that runs out of device memory included."""
+  labels = v.labels()
   if labels is None:
-    raise TypeError("feature_transform: unsupported label dtype %s" % data.dtype)
-  # one plane per array axis, each in the input's memory order: for F order the planes are
-  # allocated with the axes reversed and viewed back
-  planes = np.empty((vnd,) + (data.shape if order == "C" else data.shape[::-1]), dtype=np.int32)
-  dist = np.zeros(data.size, dtype=np.float32) if want_dist else None
-  if data.size:
-    if stacked:
-      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(data.shape, order == "C", anisotropy)
-    else:
-      (sx, sy, sz), (wx, wy, wz) = _x_fastest(data.shape, anisotropy, order == "F")
-    # x-fastest axis j is array axis j in F order, array axis nd - 1 - j in C order (of a stack: its
-    # plane vnd - 1 - j, the volume index being array axis 0)
-    ptrs = (ctypes.c_void_p * vnd)(*[planes[j if order == "F" else vnd - 1 - j].ctypes.data for j in range(vnd)])
+    raise TypeError("feature_transform: unsupported label dtype %s" % v.dtype)
+  planes = v.empty("int32", planes=v.vnd)
+  dist = None
+  if want_dist:
+    dist = v.empty("float32").zero_() if v.on_device else v.shaped(np.zeros(v.size, dtype=np.float32))
+  if v.size:
     lib = _lib()
-    dist_ptr = dist.ctypes.data if want_dist else None
-    if stacked:
-      _check(lib.edtb200_feature_transform_stack(
-        labels.ctypes.data, labels.dtype.itemsize, vnd, sx, sy, sz, count, wx, wy, wz, int(bool(black_border)),
-        int(flags), dist_ptr, ptrs, int(device), None))
-    else:
-      args = (labels.ctypes.data, labels.dtype.itemsize, nd, sx, sy, sz, wx, wy, wz, int(bool(black_border)),
-              int(flags), dist_ptr, ptrs, int(device))
-      if bound is not None:
-        _check(lib.edtb200_feature_transform_bounded(*args, None, bound))
-      elif max_device_bytes is None:
-        try:
-          _check(lib.edtb200_feature_transform(*args, None))
-        except EDTError as e:
-          if e.code != ENOMEM or nd not in (2, 3):
-            raise
-          max_device_bytes = 0                # too large for the device: stream it through in chunks
-      if max_device_bytes is not None:
-        _check(lib.edtb200_feature_transform_chunked(*args, int(max_device_bytes), None))
-  indices = planes if order == "C" else planes.transpose((0,) + tuple(range(nd, 0, -1)))
-  return (dist.reshape(data.shape, order=order) if want_dist else None), indices
-
-
-def _feature_device(t, anisotropy, black_border, flags, want_dist, stacked=False, bound=None):
-  """(distances or None, indices) of a torch CUDA tensor as torch CUDA tensors on its current
-  stream, without host copies.  A Fortran-ordered tensor goes through its transposed view, as in
-  _front_door_device, and its results are returned in its order.  stacked: a stack of volumes
-  along the slowest axis in memory, one index plane per volume axis."""
-  import torch
-  dims = t.dim()
-  vnd = dims - 1 if stacked else dims       # index planes: one per (volume) axis
-  anisotropy = _volume_anisotropy(vnd, anisotropy) if stacked else _feature_anisotropy(dims, anisotropy)
-  if t.dtype in (torch.float32, torch.float64):
-    t = (t + 0).view(torch.int32 if t.dtype == torch.float32 else torch.int64)     # -0.0 == +0.0
-  nbytes = _torch_label_bytes(torch).get(t.dtype)
-  if nbytes is None:
-    raise TypeError("feature_transform: unsupported label dtype %s" % t.dtype)
-  fortran = dims > 1 and not t.is_contiguous() and t.permute(*reversed(range(dims))).is_contiguous()
-  if fortran:
-    t = t.permute(*reversed(range(dims)))
-    anisotropy = tuple(reversed(anisotropy))
-  t = t.contiguous()
-  planes = torch.empty((vnd,) + tuple(t.shape), dtype=torch.int32, device=t.device)
-  dist = torch.zeros(t.shape, dtype=torch.float32, device=t.device) if want_dist else None
-  if t.numel():
-    # x-fastest axis j is the caller's array axis j when it was F-ordered, else axis dims - 1 - j (of
-    # a stack: its plane vnd - 1 - j, the volume index being axis 0)
-    ptrs = (ctypes.c_void_p * vnd)(*[planes[j if fortran else vnd - 1 - j].data_ptr() for j in range(vnd)])
-    stream = torch.cuda.current_stream(t.device).cuda_stream
-    dist_ptr = dist.data_ptr() if want_dist else None
-    flags = int(flags) | FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
-    if stacked:
-      count, (sx, sy, sz), (wx, wy, wz) = _stack_layout(t.shape, True, anisotropy)
-      _check(_lib().edtb200_feature_transform_stack(
-        t.data_ptr(), nbytes, vnd, sx, sy, sz, count, wx, wy, wz, int(bool(black_border)), flags, dist_ptr, ptrs,
-        t.device.index, ctypes.c_void_p(stream)))
-    else:
-      (sx, sy, sz), (wx, wy, wz) = _x_fastest(t.shape, anisotropy, False)
-      args = (t.data_ptr(), nbytes, dims, sx, sy, sz, wx, wy, wz, int(bool(black_border)), flags, dist_ptr, ptrs,
-              t.device.index, ctypes.c_void_p(stream))
-      if bound is not None:
-        _check(_lib().edtb200_feature_transform_bounded(*args, bound))
-      else:
-        _check(_lib().edtb200_feature_transform(*args))
-  if fortran:
-    planes = planes.permute(0, *range(dims, 0, -1))
-    dist = dist.permute(*reversed(range(dims))) if want_dist else None
+    device, stream = v.where
+    tail = (int(bool(black_border)), int(flags) | v.flags, v.ptr_of(dist), v.plane_ptrs(planes), device)
+    if v.stacked:
+      _check(lib.edtb200_feature_transform_stack(v.ptr_of(labels[0]), labels[1], *v.geometry, *tail, stream))
+      return dist, planes
+    args = (v.ptr_of(labels[0]), labels[1]) + v.volume_geometry + tail
+    if bound is not None:
+      _check(lib.edtb200_feature_transform_bounded(*args, stream, bound))
+    elif budget is None:
+      try:
+        _check(lib.edtb200_feature_transform(*args, stream))
+      except EDTError as e:
+        if e.code != ENOMEM or v.on_device or v.nd not in (2, 3):
+          raise
+        budget = 0                          # too large for the device: stream it through in chunks
+    if budget is not None:
+      _check(lib.edtb200_feature_transform_chunked(*args, budget, stream))
   return dist, planes
 
 
@@ -1066,32 +1028,37 @@ def feature_transform(data, anisotropy=None, black_border=False, *, signed=False
   or max_device_bytes."""
   bound = _bound(max_distance, stacked=stacked, max_device_bytes=max_device_bytes)
   flags = FLAG_SQRT | (FLAG_SIGNED if signed else 0)
-  on_device = _device_array(data)
-  if stacked:
-    _stack_dims(on_device.dim() if on_device is not None else np.ndim(data))
-    if max_device_bytes is not None:
-      raise ValueError("stacked=True stages the whole stack on the GPU at once; it cannot be combined with "
-                       "max_device_bytes")
-    if on_device is not None:
-      dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances, stacked=True)
-    else:
-      dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device, stacked=True)
-    return (dist, idx) if return_distances else idx
-  if max_device_bytes is not None:
-    dims = on_device.dim() if on_device is not None else np.ndim(data)
-    max_device_bytes = _chunk_budget(max_device_bytes, on_device is not None, None, dims)
-  if on_device is not None:
-    dist, idx = _feature_device(on_device, anisotropy, black_border, flags, return_distances, bound=bound)
-  else:
-    dist, idx = _feature_host(data, anisotropy, black_border, flags, return_distances, device, max_device_bytes,
-                              bound=bound)
+  v = _Volume("feature_transform", data, stacked, device=device)
+  max_device_bytes = _feature_budget(v, max_device_bytes)
+  anisotropy = _weights(v.vnd, anisotropy) if stacked else _single_weights(v, anisotropy)
+  v.order(f_first=not (stacked or v.on_device))
+  v.set_weights(anisotropy, positive=False, rule=None)
+  dist, idx = _feature(v, black_border, flags, return_distances, max_device_bytes, bound)
   return (dist, idx) if return_distances else idx
 
 
-def _expand_host(arr, distance, anisotropy, device, max_device_bytes):
-  """expand_labels of a contiguous numpy array through the chunked feature transform: the labels are
+def _feature_budget(v, max_device_bytes):
+  """max_device_bytes of feature_transform and expand_labels, after rejecting a budget for a stack, which is
+  staged on the GPU whole, and a stack of the wrong number of dimensions."""
+  if v.stacked:
+    _stack_dims(v.nd)
+    return _chunk_budget(max_device_bytes, staged=True) if max_device_bytes is not None else None
+  return None if max_device_bytes is None else _chunk_budget(max_device_bytes, v.on_device, None, v.nd)
+
+
+def _single_weights(v, anisotropy):
+  """The weights of one volume of feature_transform and expand_labels, taken as edt takes a host array."""
+  if not 1 <= v.nd <= 3:
+    raise TypeError(_TOO_MANY_DIMS.format(v.nd))
+  return _weights(v.nd, anisotropy, "first")
+
+
+def _expand_host(v, distance, anisotropy, max_device_bytes):
+  """expand_labels of a resolved host volume through the chunked feature transform: the labels are
   gathered on the host, a bounded range of voxels at a time, at the background voxels that grow."""
-  dist, idx = _feature_host(arr, anisotropy, False, FLAG_SIGNED, True, device, max_device_bytes)
+  v.set_weights(_single_weights(v, anisotropy), positive=False, rule=None)
+  dist, idx = _feature(v, False, FLAG_SIGNED, True, max_device_bytes)
+  arr = v.arr
   order = "F" if arr.flags.f_contiguous and not arr.flags.c_contiguous else "C"
   out = arr.copy(order=order)
   # every array here is contiguous in `order`, so these flat views follow memory
@@ -1108,61 +1075,22 @@ def _expand_host(arr, distance, anisotropy, device, max_device_bytes):
   return out
 
 
-def _expand_device(t, distance, anisotropy, stacked):
-  """expand_labels of a torch CUDA tensor (with `stacked`, a stack of volumes along its slowest axis in
-  memory) on its current stream: the signed feature transform, then one gather kernel
-  (edtb200_expand_gather) over the memory-order view and the x-fastest index planes the transform
-  used.  The result keeps t's strides."""
-  import torch
-  dims = t.dim()
-  if not t.is_contiguous() and not t.permute(*reversed(range(dims))).is_contiguous():
-    t = t.contiguous()
-  dist, idx = _feature_device(t, anisotropy, False, FLAG_SIGNED, True, stacked=stacked)
-  if t.numel() == 0:
-    return t.clone()
-  # _feature_device returns F-ordered planes where it ran on the transposed view
-  fortran = dims > 1 and not idx[0].is_contiguous()
-  lab = (t.permute(*reversed(range(dims))) if fortran else t).contiguous()
-  vnd = dims - 1 if stacked else dims
-  count = int(lab.shape[0]) if stacked else 1
-  (sx, sy, sz), _ = _x_fastest(lab.shape[1:] if stacked else lab.shape, (1.0,) * vnd, False)
-  # x-fastest axis j is the caller's axis j when F-ordered, else axis vnd - 1 - j (as in _feature_device)
-  ptrs = (ctypes.c_void_p * vnd)(*[idx[j if fortran else vnd - 1 - j].data_ptr() for j in range(vnd)])
-  flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE | (FLAG_LABELS_FLOAT if lab.is_floating_point() else 0)
-  out = torch.empty_like(lab)
-  stream = torch.cuda.current_stream(lab.device).cuda_stream
-  _check(_lib().edtb200_expand_gather(
-    lab.data_ptr(), lab.element_size(), vnd, sx, sy, sz, count, dist.data_ptr(), ptrs, float(distance) ** 2, flags,
-    out.data_ptr(), lab.device.index, ctypes.c_void_p(stream)))
-  return out.permute(*reversed(range(dims))) if fortran else out
-
-
-def _expand_stack(labels, on_device, distance, anisotropy, device, max_device_bytes):
-  """expand_labels(stacked=True).  A host stack is uploaded whole, grown on the device and copied back,
-  as a host volume is; one that does not fit raises EDTError with code ENOMEM."""
-  import torch
-  arr = None if on_device is not None else np.asarray(np.array(labels) if isinstance(labels, list) else labels)
-  vnd = _stack_dims(on_device.dim() if on_device is not None else arr.ndim)
-  if max_device_bytes is not None:
-    raise ValueError("stacked=True stages the whole stack on the GPU at once; it cannot be combined with "
-                     "max_device_bytes")
-  anisotropy = _volume_anisotropy(vnd, anisotropy)
-  if on_device is not None:
-    return _expand_device(on_device, distance, anisotropy, True)
-  arr, order = _stack_order(arr)
-  if _label_view(arr) is None:
-    raise TypeError("expand_labels: unsupported label dtype %s" % arr.dtype)
-  if arr.size == 0:
-    return arr.copy(order=order)
-  if device_count() == 0:
-    raise EDTError("edt_b200 error %d: no usable CUDA device; this library has no CPU fallback" % ECUDA, ECUDA)
-  raw = arr if arr.dtype.kind == "f" else arr.view(np.uint8 if arr.itemsize == 1 else np.dtype("i%d" % arr.itemsize))
-  try:
-    out = _expand_device(torch.from_numpy(raw).to(torch.device("cuda", int(device))), distance, anisotropy, True)
-  except torch.cuda.OutOfMemoryError as e:
-    raise EDTError("edt_b200 error %d: the stack of %d bytes does not fit on the GPU (%s)" % (ENOMEM, arr.nbytes, e),
-                   ENOMEM) from e
-  return out.cpu().numpy().view(arr.dtype)
+def _expand_device(v, distance, anisotropy):
+  """expand_labels of a device volume (with `stacked`, a stack of volumes along its slowest axis in memory) on
+  its current stream: the signed feature transform, then one gather kernel (edtb200_expand_gather) over the
+  labels and index planes in the layout the transform used.  The result has the input's memory order."""
+  if not v.stacked:
+    anisotropy = _single_weights(v, anisotropy)
+  v.order()
+  v.set_weights(anisotropy, positive=False, rule=None)
+  dist, idx = _feature(v, False, FLAG_SIGNED, True)
+  if v.size == 0:
+    return v.arr.clone()
+  out = v.empty()
+  flags = v.flags | (FLAG_LABELS_FLOAT if v.floating else 0)
+  _check(_lib().edtb200_expand_gather(v.ptr, v.arr.element_size(), *v.geometry[:5], v.ptr_of(dist),
+                                      v.plane_ptrs(idx), float(distance) ** 2, flags, v.ptr_of(out), *v.where))
+  return out
 
 
 def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device_bytes=None, stacked=False):
@@ -1185,128 +1113,39 @@ def expand_labels(labels, distance=1.0, anisotropy=None, *, device=0, max_device
   volume axis.  The whole stack is staged on the GPU at once: it cannot be combined with
   max_device_bytes, and a host stack that does not fit raises EDTError with code ENOMEM."""
   import torch
-  on_device = _device_array(labels)
+  v = _Volume("expand_labels", labels, stacked, device=device)
+  max_device_bytes = _feature_budget(v, max_device_bytes)
   if stacked:
-    return _expand_stack(labels, on_device, distance, anisotropy, device, max_device_bytes)
-  if on_device is None:
-    arr = np.asarray(labels)
-    if not arr.flags.c_contiguous and not arr.flags.f_contiguous:
-      arr = np.ascontiguousarray(arr)
-    if max_device_bytes is not None:
-      max_device_bytes = _chunk_budget(max_device_bytes, False, None, arr.ndim)
-    if _label_view(arr) is None:
-      raise TypeError("expand_labels: unsupported label dtype %s" % arr.dtype)
-    if max_device_bytes is None:
-      raw = arr.view(np.uint8 if arr.dtype.itemsize == 1 else np.dtype("i%d" % arr.dtype.itemsize))
-      if arr.dtype.kind == "f":
-        raw = arr                            # folded by _feature_device and compared by value below
-      try:
-        out = expand_labels(torch.from_numpy(raw).to(torch.device("cuda", int(device))), distance, anisotropy)
-        return out.cpu().numpy().view(arr.dtype)
-      except (EDTError, torch.cuda.OutOfMemoryError) as e:
-        if getattr(e, "code", ENOMEM) != ENOMEM or arr.ndim not in (2, 3):
+    anisotropy = _weights(v.vnd, anisotropy)
+  if v.on_device:
+    return _expand_device(v, distance, anisotropy)
+  v.order(f_first=not stacked)
+  if v.labels() is None:
+    raise TypeError("expand_labels: unsupported label dtype %s" % v.dtype)
+  if max_device_bytes is None:
+    # host arrays go up through torch, are grown on the device and come back
+    if stacked:
+      if v.size == 0:
+        return v.arr.copy(order="F" if v.fortran else "C")
+      if device_count() == 0:
+        raise EDTError("edt_b200 error %d: no usable CUDA device; this library has no CPU fallback" % ECUDA, ECUDA)
+    arr = v.arr
+    try:
+      up = _Volume("expand_labels", v.upload(torch.device("cuda", int(device))), stacked)
+      return _expand_device(up, distance, anisotropy).cpu().numpy().view(arr.dtype)
+    except (EDTError, torch.cuda.OutOfMemoryError) as e:
+      if stacked:
+        if isinstance(e, EDTError):
           raise
-      torch.cuda.empty_cache()               # what the one-shot attempt left cached goes back to the device
-      max_device_bytes = 0                   # too large for the device: the chunked path
-    if arr.size == 0:
-      return arr.copy()
-    return _expand_host(arr, distance, anisotropy, device, max_device_bytes)
-  if max_device_bytes is not None:
-    _chunk_budget(max_device_bytes, True, None, on_device.dim())
-  return _expand_device(on_device, distance, anisotropy, False)
-
-
-# ---------------------------------------------------------------------------------------
-# whole-volume operations: one C ABI call on the whole input, host or device
-# ---------------------------------------------------------------------------------------
-
-class _WholeVolume:
-  """The input of one whole-volume operation, resolved for its C ABI call.  A numpy array is staged on
-  the GPU whole and gives numpy results; a device array (a torch CUDA tensor or any
-  __cuda_array_interface__ object) gives torch CUDA results computed on its current stream.  `arr` is
-  C- or F-contiguous (C where both apply; a strided array is copied to C order), and the C ABI reads an
-  F-ordered one as its C-ordered transpose, with the weights reversed.  With `stacked` the slowest axis
-  in memory indexes same-shaped volumes.  Outputs are allocated in the input's shape and memory order,
-  so nothing is mapped back afterwards."""
-
-  def __init__(self, name, data, stacked, dims, device):
-    """`dims`: the (least, most) dimensions of one volume; a stack has one more."""
-    t = _device_array(data)
-    self.on_device = t is not None
-    arr = t if self.on_device else np.asarray(data)
-    nd = arr.dim() if self.on_device else arr.ndim
-    self.stacked = 1 if stacked else 0
-    lo, hi = dims[0] + self.stacked, dims[1] + self.stacked
-    if not lo <= nd <= hi:
-      raise TypeError("%s: %s takes %d-D to %d-D arrays, got %d-D"
-                      % (name, "stacked=True" if stacked else "it", lo, hi, nd))
-    if self.on_device:
-      self.fortran = nd > 1 and not arr.is_contiguous() and arr.permute(*reversed(range(nd))).is_contiguous()
-      if not self.fortran:
-        arr = arr.contiguous()
-    else:
-      arr, order = _stack_order(arr)
-      self.fortran = order == "F"
-    self.name, self.arr, self.dtype, self.shape = name, arr, arr.dtype, tuple(arr.shape)
-    self.vnd = nd - self.stacked
-    self.size = arr.numel() if self.on_device else arr.size
-    self.flags = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE if self.on_device else 0
-    self._device = device
-
-  def set_weights(self, anisotropy, positive=True):
-    """One weight per volume axis, and with `positive` each finite and > 0; sets `geometry`, the
-    vnd, sx, sy, sz, count, wx, wy, wz of the C ABI call."""
-    weights = _volume_anisotropy(self.vnd, anisotropy)
-    if positive:
-      for w in weights:
-        if not (np.isfinite(w) and w > 0.0):
-          raise ValueError("%s: every anisotropy weight must be finite and > 0, got %r" % (self.name, anisotropy))
-    shape = self.shape
-    if self.fortran:
-      shape, weights = shape[::-1], weights[::-1]
-    (sx, sy, sz), (wx, wy, wz) = _x_fastest(shape[1:] if self.stacked else shape, weights, False)
-    self.geometry = (self.vnd, sx, sy, sz, int(shape[0]) if self.stacked else 1, wx, wy, wz)
-
-  @property
-  def floating(self):
-    return self.dtype.is_floating_point if self.on_device else self.dtype.kind == "f"
-
-  @property
-  def ptr(self):
-    return self.ptr_of(self.arr)
-
-  @staticmethod
-  def ptr_of(x):
-    if x is None:
-      return None
-    return x.ctypes.data if isinstance(x, np.ndarray) else x.data_ptr()
-
-  @property
-  def where(self):
-    """The device and stream of the C ABI call."""
-    if not self.on_device:
-      return int(self._device), None
-    import torch
-    return self.arr.device.index, ctypes.c_void_p(torch.cuda.current_stream(self.arr.device).cuda_stream)
-
-  def empty(self, dtype=None, planes=None):
-    """An output in the input's shape and memory order, or with `planes=k` k of them as one array of
-    shape (k,) + shape.  `dtype`: a name numpy and torch share ("bool", "int32", "float32"), None for the
-    input's."""
-    lead = () if planes is None else (planes,)
-    shape = lead + (self.shape[::-1] if self.fortran else self.shape)     # as the C ABI reads the input
-    if not self.on_device:
-      dtype = self.dtype if dtype is None else dtype
-      if not lead:
-        return np.empty(self.shape, dtype, order="F" if self.fortran else "C")
-      out = np.empty(shape, dtype)
-    else:
-      import torch
-      out = torch.empty(shape, dtype=self.dtype if dtype is None else getattr(torch, dtype), device=self.arr.device)
-    if not self.fortran:
-      return out
-    back = tuple(range(len(lead))) + tuple(range(out.ndim - 1, len(lead) - 1, -1))
-    return out.permute(*back) if self.on_device else out.transpose(back)
+        raise EDTError("edt_b200 error %d: the stack of %d bytes does not fit on the GPU (%s)"
+                       % (ENOMEM, arr.nbytes, e), ENOMEM) from e
+      if getattr(e, "code", ENOMEM) != ENOMEM or v.nd not in (2, 3):
+        raise
+    torch.cuda.empty_cache()                 # what the one-shot attempt left cached goes back to the device
+    max_device_bytes = 0                     # too large for the device: the chunked path
+  if v.size == 0:
+    return v.arr.copy()
+  return _expand_host(v, distance, anisotropy, max_device_bytes)
 
 
 # ---------------------------------------------------------------------------------------
@@ -1335,7 +1174,7 @@ def _morphology(op, labels, radius, anisotropy, black_border, device, stacked, n
   r = float(radius)
   if not (r >= 0.0 and r != float("inf")):
     raise ValueError("%s: radius must be finite and zero or more, got %r" % (name, radius))
-  v = _WholeVolume(name, labels, stacked, (1, 3), device)
+  v = _Volume(name, labels, stacked, (1, 3), device)
   nbytes = _morph_label_bytes(v.dtype)
   if nbytes is None:
     raise TypeError("%s: unsupported label dtype %s" % (name, v.dtype))
@@ -1417,7 +1256,7 @@ def _parabolic(op, f, anisotropy, device, stacked, name, return_indices=False):
   x-fastest plane vnd - 1 - k of a C-ordered array and plane k of an F-ordered one."""
   if not isinstance(return_indices, (bool, np.bool_)):
     raise TypeError("%s: return_indices must be True or False, got %r" % (name, return_indices))
-  v = _WholeVolume(name, f, stacked, (1, 3), device)
+  v = _Volume(name, f, stacked, (1, 3), device)
   if v.on_device:
     if v.arr.is_complex():
       raise TypeError("%s: it takes real or bool samples, got %s" % (name, v.dtype))
@@ -1556,7 +1395,7 @@ def medial_axis(labels, anisotropy=None, black_border=False, *, return_distance=
   name = "medial_axis"
   if not isinstance(return_distance, (bool, np.bool_)):
     raise TypeError("%s: return_distance must be True or False, got %r" % (name, return_distance))
-  v = _WholeVolume(name, labels, stacked, (1, 3), device)
+  v = _Volume(name, labels, stacked, (1, 3), device)
   nbytes = _morph_label_bytes(v.dtype)
   if nbytes is None:
     raise TypeError("%s: unsupported label dtype %s" % (name, v.dtype))
@@ -1620,7 +1459,7 @@ def skeletonize(labels, anisotropy=None, black_border=False, *, return_distance=
   name = "skeletonize"
   if not isinstance(return_distance, (bool, np.bool_)):
     raise TypeError("%s: return_distance must be True or False, got %r" % (name, return_distance))
-  v = _WholeVolume(name, labels, stacked, (2, 3), device)
+  v = _Volume(name, labels, stacked, (2, 3), device)
   try:
     nbytes = _nearest_label_bytes(v.dtype)
   except TypeError:
@@ -1711,7 +1550,7 @@ def nearest_labels(labels, max_distance, anisotropy=None, *, k=2, squared=False,
   d = float(max_distance)
   if not (d >= 0.0 and d != float("inf")):
     raise ValueError("%s: max_distance must be finite and zero or more, got %r" % (name, max_distance))
-  v = _WholeVolume(name, labels, stacked, (1, 3), device)
+  v = _Volume(name, labels, stacked, (1, 3), device)
   nbytes = _nearest_label_bytes(v.dtype)
   v.set_weights(anisotropy)
   dist = v.empty("float32", planes=k)
@@ -1751,23 +1590,22 @@ def _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes):
   """The sorted surface distances of a against b: (keys, offsets, values, count, host) with torch CUDA
   offsets and values.  Host arrays go up through torch, as expand_labels' do."""
   import torch
-  da, db = _device_array(a), _device_array(b)
-  host = da is None and db is None
+  va, vb = (_Volume("surface_distances", x, stacked, device=device) for x in (a, b))
+  host = not va.on_device and not vb.on_device
   if host:
-    na = np.asarray(np.array(a) if isinstance(a, list) else a)
-    nb = np.asarray(np.array(b) if isinstance(b, list) else b)
-    shape, dtype, nd = na.shape, na.dtype, na.ndim
-    if nb.shape != shape:
-      raise ValueError("a and b must have one shape, got %s and %s" % (shape, nb.shape))
-    if nb.dtype != dtype:
-      raise TypeError("a and b must have one dtype, got %s and %s" % (dtype, nb.dtype))
-    if _label_view(na[:0]) is None:
+    shape, dtype, nd = va.arr.shape, va.arr.dtype, va.nd
+    if vb.arr.shape != shape:
+      raise ValueError("a and b must have one shape, got %s and %s" % (shape, vb.arr.shape))
+    if vb.arr.dtype != dtype:
+      raise TypeError("a and b must have one dtype, got %s and %s" % (dtype, vb.arr.dtype))
+    if _label_view(va.arr[:0]) is None:
       raise TypeError("unsupported label dtype %s" % dtype)
   else:
-    if da is None:
-      da = torch.as_tensor(np.asarray(a), device=db.device)
-    if db is None:
-      db = torch.as_tensor(np.asarray(b), device=da.device)
+    if not va.on_device:
+      va = _Volume(va.name, torch.as_tensor(va.arr, device=vb.arr.device), stacked)
+    if not vb.on_device:
+      vb = _Volume(vb.name, torch.as_tensor(vb.arr, device=va.arr.device), stacked)
+    da, db = va.arr, vb.arr
     shape, nd = tuple(da.shape), da.dim()
     if tuple(db.shape) != shape:
       raise ValueError("a and b must have one shape, got %s and %s" % (shape, tuple(db.shape)))
@@ -1778,44 +1616,30 @@ def _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes):
       raise TypeError("unsupported label dtype %s" % da.dtype)
     dtype = torch.empty(0, dtype=da.dtype).numpy().dtype
   if stacked:
-    vnd = _stack_dims(nd)
+    _stack_dims(nd)
   elif nd < 1 or nd > 3:
     raise TypeError("surface distances take 1-D to 3-D volumes, got %d-D" % nd)
-  else:
-    vnd = nd
-  anisotropy = _volume_anisotropy(vnd, anisotropy)
+  anisotropy = _weights(va.vnd, anisotropy)
   keys = None if labels is None else _surface_keys(labels, dtype)
-  budget = 0 if max_device_bytes is None else int(max_device_bytes)
-  if budget < 0:
-    raise ValueError("max_device_bytes must be non-negative (0: what the device has free)")
+  budget = 0 if max_device_bytes is None else _chunk_budget(max_device_bytes)
   if host:
     if np.prod(shape) == 0:
-      count = (int(shape[0] if na.flags.c_contiguous else shape[-1])) if stacked else 1
+      count = (int(shape[0] if va.arr.flags.c_contiguous else shape[-1])) if stacked else 1
       keys = np.zeros(0, dtype) if keys is None else keys
       nseg = count * keys.size * 2
       return keys, torch.zeros(nseg + 1, dtype=torch.int64), torch.zeros(0, dtype=torch.float32), count, host
     if device_count() == 0:
       raise EDTError("edt_b200 error %d: no usable CUDA device; this library has no CPU fallback" % ECUDA, ECUDA)
+    # host arrays go up through torch, as expand_labels' do
     dev = torch.device("cuda", int(device))
-    up = []
-    for x in (na, nb):
-      if not x.flags.c_contiguous and not x.flags.f_contiguous:
-        x = np.ascontiguousarray(x)
-      raw = x if x.dtype.kind == "f" else x.view(np.uint8 if x.itemsize == 1 else np.dtype("i%d" % x.itemsize))
-      up.append(torch.from_numpy(raw).to(dev))
-    da, db = up
-  # raw label bits, as the transforms compare them: -0.0 folded onto +0.0, unsigned as signed of one width
-  raw_of = {torch.float32: torch.int32, torch.float64: torch.int64, torch.bool: torch.uint8}
-  for name in ("uint16", "uint32", "uint64"):
-    if hasattr(torch, name):
-      raw_of[getattr(torch, name)] = getattr(torch, name.replace("u", ""))
-  ta, tb = ((t + 0 if t.is_floating_point() else t).view(raw_of.get(t.dtype, t.dtype)) for t in (da, db))
-  fortran = nd > 1 and not ta.is_contiguous() and ta.permute(*reversed(range(nd))).is_contiguous()
-  if fortran:              # through the transposed (C-ordered) view, as _stack_device and _front_door_device
-    ta, tb = ta.permute(*reversed(range(nd))), tb.permute(*reversed(range(nd)))
-    anisotropy = tuple(reversed(anisotropy))
-  ta, tb = ta.contiguous(), tb.contiguous()
-  count = int(ta.shape[0]) if stacked else 1      # the slowest axis in memory indexes the volumes
+    va, vb = (_Volume(v.name, v.order().upload(dev), stacked) for v in (va, vb))
+  # a's memory order decides the layout the C ABI reads; b is laid out the same way
+  va.order()
+  va.set_weights(anisotropy, positive=False, rule=None)
+  rev = tuple(reversed(range(nd)))
+  vb.arr = vb.arr.permute(*rev).contiguous().permute(*rev) if va.fortran else vb.arr.contiguous()
+  (ta, nbytes), (tb, _) = va.labels(), vb.labels()
+  vnd, sx, sy, sz, count, wx, wy, wz = va.geometry
   rtype = np.dtype("u%d" % ta.element_size())
   if keys is None:
     if ta.numel():
@@ -1832,7 +1656,6 @@ def _surface_run(a, b, anisotropy, labels, stacked, device, max_device_bytes):
   dev = ta.device
   counts = torch.zeros(nseg, dtype=torch.int64, device=dev)
   stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-  (sx, sy, sz), (wx, wy, wz) = _x_fastest(ta.shape[1:] if stacked else ta.shape, anisotropy, False)
   both = FLAG_LABELS_ON_DEVICE | FLAG_OUT_ON_DEVICE
   lib = _lib()
   _check(lib.edtb200_surface_count(ta.data_ptr(), tb.data_ptr(), ta.element_size(), vnd, sx, sy, sz, count,

@@ -209,7 +209,7 @@ def test_stacked_rejects_budget_for_device_input(edt):
     def dim(self):
       return 3
   with pytest.raises(ValueError, match="device-resident"):
-    edt._front_door(FakeDeviceArray(), None, False, None, 0, 0, max_device_bytes=1 << 20, stacked=True)
+    edt.edtsq(FakeDeviceArray(), max_device_bytes=1 << 20, stacked=True)
 
 
 def test_stacked_empty_stack_touches_no_device(edt):

@@ -1,5 +1,7 @@
-"""GPU tests: the input layouts every whole-volume operation accepts -- the spherical morphology, parabolic
-erosion and dilation with and without return_indices, medial_axis, skeletonize and nearest_labels.  A device
+"""GPU tests: the input layouts every whole-volume operation and transform accepts -- the spherical
+morphology, parabolic erosion and dilation with and without return_indices, medial_axis, skeletonize,
+nearest_labels, edt and sdf (max_distance= applies to single volumes only, so their stacked rows run
+unbounded), feature_transform with distances and expand_labels.  A device
 tensor that is neither C- nor F-contiguous, a __cuda_array_interface__ object that is not a torch tensor, an
 F-ordered device stack and a strided host array each give, bit for bit, what the host call gives on a numpy
 array of the same values in the same memory order (a strided one: its C-contiguous copy; a wrapper: the
@@ -21,6 +23,12 @@ CALLS = {
   "medial_axis": lambda edt, x, w, s: edt.medial_axis(x, w, True, return_distance=True, stacked=s),
   "skeletonize": lambda edt, x, w, s: edt.skeletonize(x, w, return_distance=True, stacked=s),
   "nearest_labels": lambda edt, x, w, s: edt.nearest_labels(x, 2.0, w, k=2, stacked=s),
+  "edt": lambda edt, x, w, s: (edt.edt(x, w, True, stacked=s),),
+  "sdf": lambda edt, x, w, s: (edt.sdf(x, w, stacked=s),),
+  "edt_max_distance": lambda edt, x, w, s: (edt.edt(x, w, True, stacked=s, max_distance=None if s else 2.5),),
+  "sdf_max_distance": lambda edt, x, w, s: (edt.sdf(x, w, stacked=s, max_distance=None if s else 2.5),),
+  "feature_transform": lambda edt, x, w, s: edt.feature_transform(x, w, True, return_distances=True, stacked=s),
+  "expand_labels": lambda edt, x, w, s: (edt.expand_labels(x, 2.0, w, stacked=s),),
 }
 WEIGHTS = (1.0, 2.0, 3.0)
 

@@ -78,6 +78,13 @@ def torch_gather(t, dist, idx, distance):
   return out
 
 
+def signed_features(t, anisotropy):
+  """(squared signed distances, index planes) of a device volume: the feature transform expand_labels runs."""
+  v = edt._Volume("expand_bench", t).order()
+  v.set_weights(anisotropy, positive=False, rule="first")
+  return edt._feature(v, False, edt.FLAG_SIGNED, True)
+
+
 def kernel_gather(t, dist, idx, distance):
   """edtb200_expand_gather on a C-contiguous volume and the feature transform's planes."""
   nd = t.dim()
@@ -129,14 +136,13 @@ def volume_rows(args):
   ok = True
   for name in WORKLOADS:
     lab, an, _ = workloads.generate(name, args.n, "cuda")
-    dist, idx = edt._feature_device(lab, an, False, edt.FLAG_SIGNED, True)
+    dist, idx = signed_features(lab, an)
     torch.cuda.synchronize()
     parts = (
       ("gather", (("kernel", lambda: kernel_gather(lab, dist, idx, DISTANCE)),
                   ("torch ops", lambda: torch_gather(lab, dist, idx, DISTANCE)))),
       ("whole", (("expand_labels", lambda: edt.expand_labels(lab, DISTANCE, an)),
-                 ("feature+torch", lambda: torch_gather(lab, *edt._feature_device(lab, an, False, edt.FLAG_SIGNED,
-                                                                                   True), DISTANCE)))),
+                 ("feature+torch", lambda: torch_gather(lab, *signed_features(lab, an), DISTANCE)))),
     )
     for part, sides in parts:
       results = [fn() for _, fn in sides]

@@ -2573,6 +2573,30 @@ int edtb200_pass_first(const void* labels_dev, int label_bytes, int64_t sx, int6
                         static_cast<cudaStream_t>(stream));
 }
 
+// The arithmetic of a later pass with weight w along lines of n rows over `count` samples the caller
+// gave (edtb200_pass_later, edtb200_pass_window): one reduction over them on s, and a wait for it,
+// tells whether the candidate sums are exact in double, and whether the integer hull tests apply.
+int caller_samples_arith(const float* f_dev, int64_t count, float w, int64_t n, DeviceCache& dc, cudaStream_t s,
+                         PassArith* arith) {
+  const int init[2] = {0, 1024};
+  int range[2] = {0, 1024};
+  {
+    Scratch range_dev;                                           // freed before the wait below
+    CUDA_TRY(range_dev.alloc(dc, 2 * sizeof(int), s));
+    CUDA_TRY(cudaMemcpyAsync(range_dev.get(), init, sizeof(init), cudaMemcpyHostToDevice, s));
+    int64_t blocks = (count + 255) / 256;
+    if (blocks > (int64_t)dc.sm_count * 8) blocks = (int64_t)dc.sm_count * 8;
+    sample_range_kernel<<<(unsigned)blocks, 256, 0, s>>>(f_dev, count, range_dev.get<int>());
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(range, range_dev.get(), sizeof(range), cudaMemcpyDeviceToHost, s));
+  }
+  CUDA_TRY(cudaStreamSynchronize(s));
+  float fmax;
+  memcpy(&fmax, &range[0], sizeof(float));
+  *arith = sampled_arith(fmax, range[1], w, n);
+  return 0;
+}
+
 int edtb200_pass_later(const void* labels_dev, int label_bytes, int axis, int64_t sx, int64_t sy, int64_t sz,
                        float w, int border_lo, int border_hi, int flags, float* f_dev, int device,
                        void* stream) {
@@ -2585,29 +2609,47 @@ int edtb200_pass_later(const void* labels_dev, int label_bytes, int axis, int64_
   DeviceCache* dc = nullptr;
   rc = probe(device, &dc);
   if (rc) return rc;
-  // The samples come from the caller: one reduction over them (and a wait for it) tells whether
-  // the pass's candidate sums are exact in double, and whether the integer hull tests apply.
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int64_t count = sx * sy * sz;
-  const int init[2] = {0, 1024};
-  int range[2] = {0, 1024};
-  {
-    Scratch range_dev;                                           // freed before the wait below
-    CUDA_TRY(range_dev.alloc(*dc, 2 * sizeof(int), s));
-    CUDA_TRY(cudaMemcpyAsync(range_dev.get(), init, sizeof(init), cudaMemcpyHostToDevice, s));
-    int64_t blocks = (count + 255) / 256;
-    if (blocks > (int64_t)dc->sm_count * 8) blocks = (int64_t)dc->sm_count * 8;
-    sample_range_kernel<<<(unsigned)blocks, 256, 0, s>>>(f_dev, count, range_dev.get<int>());
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(range, range_dev.get(), sizeof(range), cudaMemcpyDeviceToHost, s));
-  }
-  CUDA_TRY(cudaStreamSynchronize(s));
-  float fmax;
-  memcpy(&fmax, &range[0], sizeof(float));
   const edtb200::LineGeom g = geom_for_axis(axis, sx, sy, sz);
+  PassArith arith;
+  rc = caller_samples_arith(f_dev, sx * sy * sz, w, g.n, *dc, s, &arith);
+  if (rc) return rc;
   return dispatch_later(label_bytes, labels_dev, f_dev, g, w, border_lo != 0, border_hi != 0,
-                        kernel_flags(flags, /*first=*/false, /*last=*/true), sampled_arith(fmax, range[1], w, g.n),
-                        *dc, s, /*pdl=*/false);
+                        kernel_flags(flags, /*first=*/false, /*last=*/true), arith, *dc, s, /*pdl=*/false);
+}
+
+int edtb200_pass_window(const void* labels_dev, int label_bytes, int axis, int64_t sx, int64_t sy, int64_t sz,
+                        float w, int border_lo, int border_hi, int flags, double max_distance, const float* fin_dev,
+                        float* fout_dev, int* codes_dev, int device, void* stream) {
+  int rc = check_dims(label_bytes, 3, sx, sy, sz);
+  if (rc) return rc;
+  if (axis != 1 && axis != 2) return fail(EDTB200_EINVAL, "axis must be 1 (Y) or 2 (Z)");
+  if ((rc = check_weights(1, &w))) return rc;
+  if (!(max_distance >= 0.0)) return fail(EDTB200_EINVAL, "max_distance must be zero or more (got %g)", max_distance);
+  const BoundedPlan bp = window_pass_plan(w, max_distance);
+  if (bp.radius[0] > kWindowRadiusLimit)
+    return fail(EDTB200_EINVAL, "window radius %lld out of range", (long long)bp.radius[0]);
+  const int64_t count = sx * sy * sz;
+  if (count == 0) return 0;
+  if (!labels_dev || !fin_dev || !fout_dev) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t bytes = sizeof(float) * (size_t)count;
+  if (overlaps(fin_dev, bytes, fout_dev, bytes) || (codes_dev && (overlaps(codes_dev, bytes, fin_dev, bytes) ||
+                                                                  overlaps(codes_dev, bytes, fout_dev, bytes))))
+    return fail(EDTB200_EINVAL, "fin, fout and codes must not overlap");
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  rc = probe(device, &dc);
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const edtb200::LineGeom g = geom_for_axis(axis, sx, sy, sz);
+  PassArith arith;
+  rc = caller_samples_arith(fin_dev, count, w, g.n, *dc, s, &arith);
+  if (rc) return rc;
+  return with_label_width(label_bytes, [&](auto b) {
+    return launch_later_window<b>(labels_dev, fin_dev, fout_dev, codes_dev, g, w, (int)bp.radius[0], border_lo != 0,
+                                  border_hi != 0, kernel_flags(flags, /*first=*/false, /*last=*/true), arith,
+                                  bp.bound, *dc, s);
+  });
 }
 
 int edtb200_last_later_launch(int* info) {

@@ -244,6 +244,9 @@ constexpr int kWindowRadiusLimit = 128;
 // transform's EDTB200_BOUNDED_SITES_WINDOW_MAX), or EDTB200_BOUNDED_RMAX for both (an A/B switch for
 // measurements; -1: no pass is windowed) (edt_plan.cu).  max_distance >= 0.
 BoundedPlan bounded_plan(int ndim, const float w[3], double max_distance, bool sites);
+// The B and R (in radius[0]) of one later pass with weight w that edtb200_pass_window runs: the plan
+// above for that axis, every radius up to kWindowRadiusLimit windowed (edt_plan.cu).
+BoundedPlan window_pass_plan(float w, double max_distance);
 
 // The bounded transforms' kernels (edt_bounded.cuh, one instantiation per label width in
 // edt_bounded.cu).  launch_later_window: the later pass along g out of place (fin -> fout) over the

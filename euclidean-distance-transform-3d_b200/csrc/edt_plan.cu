@@ -22,5 +22,10 @@ BoundedPlan bounded_plan(int ndim, const float w[3], double max_distance, bool s
   return plan_bounded(ndim, w, max_distance, rmax);
 }
 
+BoundedPlan window_pass_plan(float w, double max_distance) {
+  const float ws[3] = {w, w, w};
+  return plan_bounded(1, ws, max_distance, kWindowRadiusLimit);
+}
+
 }  // namespace host
 }  // namespace edtb200

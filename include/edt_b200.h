@@ -38,7 +38,7 @@ extern "C" {
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
- * edtb200_medial_axis, edtb200_skeletonize)
+ * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -850,6 +850,22 @@ int edtb200_pass_later(const void *labels_dev, int label_bytes, int axis,
                        int64_t sx, int64_t sy, int64_t sz, float w,
                        int border_lo, int border_hi, int flags,
                        float *f_dev, int device, void *stream);
+
+/* edtb200_pass_window : one later pass of the bounded transforms (edtb200_transform_bounded) in their
+ *     window kernel, for tests of that kernel alone.  B and R are the bounded transforms' for an axis of
+ *     weight w and max_distance (edtb200_bounded_plan), and the window kernel runs whatever R is, up to
+ *     its limit of 128 rows.  Out of place: fout_dev = the pass over the samples fin_dev (any
+ *     non-negative floats), with every row above B written as +inf; codes_dev (may be NULL) = the
+ *     feature transform's site codes of the pass.  axis, borders and flags as edtb200_pass_later; the
+ *     arithmetic is decided from the samples as there (one reduction, and a wait for it).
+ *     edtb200_last_later_launch reports the launch (kernel 2, R in info[1]).  Checks, in order: label
+ *     width and sizes, axis, w (finite and > 0), max_distance (>= 0), R (at most 128), emptiness,
+ *     pointers, fin / fout / codes overlapping, then the device. */
+int edtb200_pass_window(const void *labels_dev, int label_bytes, int axis,
+                        int64_t sx, int64_t sy, int64_t sz, float w,
+                        int border_lo, int border_hi, int flags, double max_distance,
+                        const float *fin_dev, float *fout_dev, int *codes_dev,
+                        int device, void *stream);
 
 /* Z-slab decomposition across GPUs (DESIGN.md section 8): a rank runs edtb200_pass_later(axis=2)
  * on its slab with the interior faces open (border flags 0 there) and then folds the

@@ -64,6 +64,15 @@ def _pass_later(labels=P, label_bytes=4, axis=1, sx=4, sy=4, sz=4, w=1.0, lo=0, 
   return (labels, label_bytes, axis, sx, sy, sz, w, lo, hi, flags, f, device, stream)
 
 
+_FIN, _FOUT, _CODES = (np.zeros(64, np.float32) for _ in range(3))   # three disjoint buffers
+FIN, FOUT, CODES = _FIN.ctypes.data, _FOUT.ctypes.data, _CODES.ctypes.data
+
+
+def _pass_window(labels=P, label_bytes=4, axis=1, sx=4, sy=4, sz=4, w=1.0, lo=0, hi=0, flags=0, d=3.0, fin=FIN,
+                 fout=FOUT, codes=None, device=63, stream=None):
+  return (labels, label_bytes, axis, sx, sy, sz, w, lo, hi, flags, d, fin, fout, codes, device, stream)
+
+
 def _face_runs(labels=P, label_bytes=4, sx=4, sy=4, sz=4, high_face=0, halo=2, flags=0, m=P, overflow=P, device=63,
                stream=None):
   return (labels, label_bytes, sx, sy, sz, high_face, halo, flags, m, overflow, device, stream)
@@ -208,6 +217,41 @@ CASES = {
     ("empty_before_null", dict(sy=0, f=None), 0, ""),
     ("valid_y", dict(), PROBE, ""),
     ("valid_z", dict(axis=2), PROBE, ""),
+  ]),
+  "edtb200_pass_window": (_pass_window, [
+    ("label_bytes", dict(label_bytes=3), EINVAL, "label_bytes"),
+    ("negative_size", dict(sz=-1), EINVAL, "negative size"),
+    ("axis_too_long", dict(sy=BIG), ELIMIT, "axis longer than 2^30"),
+    ("axis_0", dict(axis=0), EINVAL, "axis must be 1 (Y) or 2 (Z)"),
+    ("weight_0", dict(w=0.0), EINVAL, "weight"),
+    ("weight_nan", dict(w=float("nan")), EINVAL, "weight"),
+    ("weight_inf", dict(w=float("inf")), EINVAL, "weight"),
+    ("negative_distance", dict(d=-1.0), EINVAL, "max_distance"),
+    ("nan_distance", dict(d=float("nan")), EINVAL, "max_distance"),
+    ("no_bound", dict(d=float("inf")), EINVAL, "window radius 4611686018427387904 out of range"),
+    ("radius_129", dict(d=129.0), EINVAL, "window radius 129 out of range"),
+    ("radius_129_weight", dict(w=0.5, d=64.5), EINVAL, "window radius 129 out of range"),
+    ("null_labels", dict(labels=None), EINVAL, "null pointer"),
+    ("null_fin", dict(fin=None), EINVAL, "null pointer"),
+    ("null_fout", dict(fout=None), EINVAL, "null pointer"),
+    ("in_place", dict(fout=FIN), EINVAL, "must not overlap"),
+    ("fout_inside_fin", dict(fout=FIN + 16), EINVAL, "must not overlap"),
+    ("codes_on_fin", dict(codes=FIN + 60), EINVAL, "must not overlap"),
+    ("codes_on_fout", dict(codes=FOUT), EINVAL, "must not overlap"),
+    # order: label width, sizes, axis, weight, distance, radius, emptiness, pointers, overlap
+    ("label_bytes_before_axis", dict(label_bytes=5, axis=3), EINVAL, "label_bytes"),
+    ("size_before_axis", dict(sx=-1, axis=0), EINVAL, "negative size"),
+    ("axis_before_weight", dict(axis=0, w=0.0), EINVAL, "axis must be"),
+    ("weight_before_distance", dict(w=-1.0, d=-1.0), EINVAL, "weight"),
+    ("distance_before_empty", dict(d=-1.0, sx=0), EINVAL, "max_distance"),
+    ("radius_before_empty", dict(d=200.0, sx=0), EINVAL, "window radius 200 out of range"),
+    ("empty_before_null", dict(sy=0, labels=None, fin=None), 0, ""),
+    ("null_before_overlap", dict(labels=None, fout=FIN), EINVAL, "null pointer"),
+    ("valid", dict(), PROBE, ""),
+    ("valid_radius_0", dict(d=0.0), PROBE, ""),
+    ("valid_radius_128", dict(d=128.0, axis=2, flags=3), PROBE, ""),
+    ("valid_radius_128_weight", dict(w=0.5, d=64.0), PROBE, ""),
+    ("valid_with_codes", dict(codes=CODES, lo=1, hi=1), PROBE, ""),
   ]),
   "edtb200_slab_face_runs": (_face_runs, [
     ("label_bytes", dict(label_bytes=3), EINVAL, "label_bytes"),

@@ -518,6 +518,7 @@ struct TileBoxes {
 // it loads anything: for the line (o, j) and row i the bit (j % sx) / 32 of word o * settled_outer +
 // j / sx + i * settled_row.  With `refresh` (the Y pass: the Z pass's settled plane, same layout)
 // every tile that runs sets the bits of its rows that it leaves at f <= refresh_t.
+// `group` (1 to 32): consecutive tiles per CTA of the grouped kernel (later_axis_tile_kernel).
 struct RunBits {
   const uint32_t* start;   // a run of equal labels starts at this row (always at row 0)
   int64_t row_words;
@@ -529,6 +530,7 @@ struct RunBits {
   int64_t settled_outer;
   uint32_t* refresh;
   float refresh_t;
+  int group;               // (in the tail padding: the struct keeps its size and layout)
 };
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
@@ -1164,6 +1166,61 @@ __device__ __forceinline__ void refresh_settled(const RunBits& rb, const float* 
   }
 }
 
+// The settled check of the grouped tile kernel: bit k of the result is set when tile t0 + k (of the
+// cnt tiles from t0) has a segment that is not settled -- the per-tile check of later_axis_tile_kernel
+// over the whole group in one read of the plane.  Thread t takes row t and walks the tiles from t0
+// without a division per tile: tile k covers the lines [j0, j0 + TX) of its outer, which reach rows
+// q, q + 1, ... of the plane, cut at multiples of sx (r: j0's place in row q).  Consecutive tiles share
+// their word (the x-segments of one row), which is loaded once.  The masks are OR-ed over the CTA
+// through `slots` (one word per warp), so the result is CTA-uniform.
+template <int TX>
+__device__ __forceinline__ uint32_t unsettled_tiles(const RunBits& rb, const LineGeom& g, int64_t t0, int cnt, int n,
+                                                    uint32_t* slots) {
+  const int64_t outer0 = t0 / g.tiles_per_outer;
+  const int64_t j00 = (t0 - outer0 * g.tiles_per_outer) * TX;
+  const int64_t q00 = j00 / rb.sx;
+  uint32_t m = 0u;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    int64_t outer = outer0, j0 = j00, q = q00, r = j00 - q00 * rb.sx;
+    int64_t last = -1;                                 // the index of the word in w
+    uint32_t w = 0u;
+    for (int k = 0; k < cnt; ++k) {
+      bool settled = true;
+      int64_t left = min((int64_t)TX, g.inner_count - j0), qq = q, rr = r;
+      while (left > 0) {
+        const int64_t take = min(left, rb.sx - rr);   // lines [rr, rr + take) of row qq
+        const int lo = (int)rr, hi = (int)(rr + take) - 1;
+        const uint32_t need = (0xffffffffu >> (31 - (hi >> 5))) & (0xffffffffu << (lo >> 5));
+        const int64_t at = outer * rb.settled_outer + qq + (int64_t)i * rb.settled_row;
+        if (at != last) { w = __ldg(rb.settled + at); last = at; }
+        settled = settled && (w & need) == need;
+        left -= take; rr = 0; ++qq;
+      }
+      if (!settled) m |= 1u << k;
+      j0 += TX;
+      if (j0 >= g.inner_count) {                       // the next tile starts the next outer
+        ++outer; j0 = 0; q = 0; r = 0;
+      } else {
+        for (r += TX; r >= rb.sx; r -= rb.sx) ++q;
+      }
+    }
+  }
+  m = __reduce_or_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0) slots[threadIdx.x >> 5] = m;
+  __syncthreads();
+  for (int wi = 0; wi < (int)(blockDim.x >> 5); ++wi) m |= slots[wi];
+  return m;
+}
+
+// The grouped tile kernel's step to its next tile: false when none is left; otherwise the barrier
+// that frees the shared memory of the tile that ended, and the parity of the next mbarrier phase.
+__device__ __forceinline__ bool next_group_tile(uint32_t todo, uint32_t& phase) {
+  if (!todo) return false;
+  __syncthreads();
+  phase ^= 1u;
+  return true;
+}
+
 // MinCtas: CTAs of 512 threads per SM the kernel is compiled for.  3 (40 registers, a few spills)
 // is what the envelope stages want -- they are latency-bound and the third CTA's warps hide it;
 // 2 (60 registers, no spills) is faster when nearly every run is one row long (label noise), where
@@ -1177,6 +1234,11 @@ __device__ __forceinline__ void refresh_settled(const RunBits& rb, const float* 
 // label-noise shape only (2 CTAs per SM, TMA, 32-wide tiles, no background bits: unsigned transforms).
 // It also skips settled tiles and refreshes the Z pass's settled plane, where the host passes those
 // planes in rb (launch_later).
+// Grouped (Bits with IntHull and no epilogue, the instance that skips settled tiles): a CTA owns the
+// rb.group consecutive tiles from blockIdx.x * rb.group.  It reads the settled words of the whole
+// group once, then runs the tiles that are not settled one after another, with the border table and
+// the mbarrier set up once: a pass that skips nearly every tile costs one read per CTA instead of a
+// CTA launch and an L2 round trip per tile (DESIGN.md section 4.1).
 template <int Bytes, int TX, bool Epilogue, bool UseTMA, bool Wide, int MinCtas, bool IntHull, bool Bits = false>
 __global__ void __launch_bounds__(Wide ? 1024 : 512, Wide ? 1 : MinCtas)
 later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
@@ -1216,521 +1278,557 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
   const int x = lane & (TX - 1);
   const int chunk0 = (threadIdx.x >> 5) * SUBS + (lane / TX);
   const int chunk_step = (blockDim.x >> 5) * SUBS;
+  constexpr bool kGrouped = Bits && IntHull && !Epilogue;
 
-  const int64_t tile = blockIdx.x;
-  const int64_t outer = tile / g.tiles_per_outer;
-  const int64_t inner0 = (tile - outer * g.tiles_per_outer) * TX;
-  const bool live = (inner0 + x) < g.inner_count;
-  // CTA-uniform tile origin + 32-bit element offsets (the host guarantees n * line_stride < 2^32)
-  const LT* __restrict__ tl = labels + (outer * g.outer_stride + inner0);
-  float* __restrict__ tf = f + (outer * g.outer_stride + inner0);
-  const uint32_t ls = (uint32_t)g.line_stride;
-  const size_t pitch = (size_t)ls * sizeof(float);
-  const float inf = __int_as_float(0x7f800000);
-  const double w2d = (double)w2;
-
-  pdl_launch_dependents();             // the next pass may start staging its labels during our tail
-  if (!UseTMA) pdl_wait_for_previous_grid();           // plain loads of f happen in the staging loop
-  // (Bits) A tile whose voxels all have f <= w2 keeps every value (DESIGN.md section 4.1): it ends
-  // here, before its mbarrier, tile load or border table.  Thread t checks row t, in every row q of
-  // the settled plane that the tile's lines [j0, j1) reach, the x-segments they cover.
-  if constexpr (Bits && !Epilogue) {
+  // (kGrouped) bit k of `todo`: tile t0 + k is still to run.  The group's settled tiles are dropped
+  // here, before the mbarrier, any tile load or the border table.  The hull words hold the check's
+  // per-warp masks: they are first written in stage 1, behind the barrier that ends stage 0.
+  int64_t t0 = 0;
+  uint32_t todo = 0u, phase = 0u;      // phase: the parity of the mbarrier phase of the current tile
+  if constexpr (kGrouped) {
+    pdl_launch_dependents();
+    t0 = (int64_t)blockIdx.x * rb.group;
+    const int cnt = (int)min((int64_t)rb.group, (int64_t)g.tiles_per_outer * g.outer_count - t0);
+    todo = cnt >= 32 ? 0xffffffffu : (1u << cnt) - 1u;
     if (rb.settled) {
       pdl_wait_for_previous_grid();    // the plane is complete (Z pass: and refreshed by the Y pass)
-      const int64_t j0 = inner0, j1 = min(inner0 + TX, g.inner_count);
-      const int64_t q0 = j0 / rb.sx, q1 = (j1 - 1) / rb.sx;
-      bool settled = true;
-      for (int i = threadIdx.x; i < n; i += blockDim.x) {
-        const uint32_t* sp = rb.settled + (outer * rb.settled_outer + (int64_t)i * rb.settled_row);
-        for (int64_t q = q0; q <= q1; ++q) {
-          const int lo = (int)max(j0 - q * rb.sx, (int64_t)0), hi = (int)min(j1 - q * rb.sx, rb.sx) - 1;
-          const uint32_t need = (0xffffffffu >> (31 - (hi >> 5))) & (0xffffffffu << (lo >> 5));
-          settled = settled && (__ldg(sp + q) & need) == need;
+      todo &= unsettled_tiles<TX>(rb, g, t0, cnt, n, reinterpret_cast<uint32_t*>(smem_tile + (hullw_a - fs_a)));
+    }
+    if (!todo) return;
+    for (int i = threadIdx.x; i < n + 2; i += blockDim.x) {
+      const float e = (float)i;
+      sts_f32(sq_a + (uint32_t)i * 4u, __fmul_rn(w2, __fmul_rn(e, e)));
+    }
+    if (threadIdx.x == 0) {
+      pdl_wait_for_previous_grid();
+      mbar_init(bar, 1);               // made visible by the barrier that ends stage 0
+    }
+  }
+  // One tile per pass of this loop; only the grouped kernel takes a second pass (`continue` ends a tile).
+  do {
+    int64_t tile = blockIdx.x;
+    if constexpr (kGrouped) {
+      tile = t0 + __ffs(todo) - 1;
+      todo &= todo - 1u;
+    }
+    const int64_t outer = tile / g.tiles_per_outer;
+    const int64_t inner0 = (tile - outer * g.tiles_per_outer) * TX;
+    const bool live = (inner0 + x) < g.inner_count;
+    // CTA-uniform tile origin + 32-bit element offsets (the host guarantees n * line_stride < 2^32)
+    const LT* __restrict__ tl = labels + (outer * g.outer_stride + inner0);
+    float* __restrict__ tf = f + (outer * g.outer_stride + inner0);
+    const uint32_t ls = (uint32_t)g.line_stride;
+    const size_t pitch = (size_t)ls * sizeof(float);
+    const float inf = __int_as_float(0x7f800000);
+    const double w2d = (double)w2;
+
+    if (!kGrouped) pdl_launch_dependents();  // the next pass may start staging its labels during our tail
+    if (!UseTMA) pdl_wait_for_previous_grid();           // plain loads of f happen in the staging loop
+    // (Bits) A tile whose voxels all have f <= w2 keeps every value (DESIGN.md section 4.1): it ends
+    // here, before its mbarrier, tile load or border table.  Thread t checks row t, in every row q of
+    // the settled plane that the tile's lines [j0, j1) reach, the x-segments they cover.
+    if constexpr (Bits && !Epilogue && !kGrouped) {
+      if (rb.settled) {
+        pdl_wait_for_previous_grid();    // the plane is complete (Z pass: and refreshed by the Y pass)
+        const int64_t j0 = inner0, j1 = min(inner0 + TX, g.inner_count);
+        const int64_t q0 = j0 / rb.sx, q1 = (j1 - 1) / rb.sx;
+        bool settled = true;
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+          const uint32_t* sp = rb.settled + (outer * rb.settled_outer + (int64_t)i * rb.settled_row);
+          for (int64_t q = q0; q <= q1; ++q) {
+            const int lo = (int)max(j0 - q * rb.sx, (int64_t)0), hi = (int)min(j1 - q * rb.sx, rb.sx) - 1;
+            const uint32_t need = (0xffffffffu >> (31 - (hi >> 5))) & (0xffffffffu << (lo >> 5));
+            settled = settled && (__ldg(sp + q) & need) == need;
+          }
+        }
+        if (__syncthreads_and(settled)) continue;
+      }
+    }
+    // Float tile by TMA, border-term table, chunk mask.  (kDecoupled) together with the mbarrier the
+    // table and the mask are the only things a warp needs from other warps before the votes at the end
+    // of stage 1, so the one barrier comes here, early, while no warp has loads in flight yet; the tile
+    // is requested right behind it, together with the first label loads.
+    if (UseTMA && threadIdx.x == 0) {
+      if (!kGrouped) {
+        if (!kDecoupled) pdl_wait_for_previous_grid();    // f is complete only when the previous pass has finished
+        mbar_init(bar, 1);
+      }
+      if (!kDecoupled) {
+        mbar_expect_tx(bar, (unsigned)rows_alloc * ROW);
+        for (int bx = 0; bx < tb.nboxes; ++bx)
+          tma_load_3d(smem_tile + (size_t)bx * tb.box_rows * ROW, &fmap, (int)inner0, bx * tb.box_rows, (int)outer, bar);
+      }
+    }
+    if (threadIdx.x < TX) sts_u32(nz_a + threadIdx.x * 4u, 0u);
+    for (int i = threadIdx.x; !kGrouped && i < n + 2; i += blockDim.x) {
+      const float e = (float)i;
+      sts_f32(sq_a + (uint32_t)i * 4u, __fmul_rn(w2, __fmul_rn(e, e)));
+    }
+    if (kDecoupled) {
+      __syncthreads();
+      if (UseTMA && threadIdx.x == 0) {
+        pdl_wait_for_previous_grid();
+        mbar_expect_tx(bar, (unsigned)rows_alloc * ROW);
+        for (int bx = 0; bx < tb.nboxes; ++bx)
+          tma_load_3d(smem_tile + (size_t)bx * tb.box_rows * ROW, &fmap, (int)inner0, bx * tb.box_rows, (int)outer, bar);
+      }
+    }
+
+    // ============ stage 0 (Bits): run-start bits -> one word per (chunk, line) ============
+    if constexpr (Bits) {
+      pdl_wait_for_previous_grid();      // the plane is complete (written by the X pass)
+      if (live) {
+        const int64_t j = inner0 + x, q = j / rb.sx, rj = j - q * rb.sx;
+        const uint32_t* bstart = rb.start + (outer * rb.outer_words + q * rb.wpr + (rj >> 5));
+        const int bit = (int)(rj & 31);
+        const size_t rw = (size_t)rb.row_words;
+        for (int c = chunk0; c < nchunks; c += chunk_step) {
+          const int i0 = c << 5;
+          const uint32_t* sp = bstart + (size_t)i0 * rw;
+          uint32_t wstart = 0;
+          if (i0 + 32 <= n) {
+  #pragma unroll
+            for (int r = 0; r < 32; ++r) wstart |= ((__ldg(sp + r * rw) >> bit) & 1u) << r;
+          } else {
+            for (int r = 0; r < n - i0; ++r) wstart |= ((__ldg(sp + r * rw) >> bit) & 1u) << r;
+            wstart |= 1u << (n - i0);        // pretend a run starts at row n (line end)
+          }
+          if (i0 == 0) wstart |= 1u;         // a run starts at row 0 by definition
+          sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wstart);
+          if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);   // no sign: not read
+        }
+      } else {
+        for (int c = chunk0; c < nchunks; c += chunk_step) {
+          sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);
+          if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);
         }
       }
-      if (__syncthreads_and(settled)) return;
     }
-  }
-  // Float tile by TMA, border-term table, chunk mask.  (kDecoupled) together with the mbarrier the
-  // table and the mask are the only things a warp needs from other warps before the votes at the end
-  // of stage 1, so the one barrier comes here, early, while no warp has loads in flight yet; the tile
-  // is requested right behind it, together with the first label loads.
-  if (UseTMA && threadIdx.x == 0) {
-    if (!kDecoupled) pdl_wait_for_previous_grid();      // f is complete only when the previous pass has finished
-    mbar_init(bar, 1);
-    if (!kDecoupled) {
-      mbar_expect_tx(bar, (unsigned)rows_alloc * ROW);
-      for (int bx = 0; bx < tb.nboxes; ++bx)
-        tma_load_3d(smem_tile + (size_t)bx * tb.box_rows * ROW, &fmap, (int)inner0, bx * tb.box_rows, (int)outer, bar);
-    }
-  }
-  if (threadIdx.x < TX) sts_u32(nz_a + threadIdx.x * 4u, 0u);
-  for (int i = threadIdx.x; i < n + 2; i += blockDim.x) {
-    const float e = (float)i;
-    sts_f32(sq_a + (uint32_t)i * 4u, __fmul_rn(w2, __fmul_rn(e, e)));
-  }
-  if (kDecoupled) {
-    __syncthreads();
-    if (UseTMA && threadIdx.x == 0) {
-      pdl_wait_for_previous_grid();
-      mbar_expect_tx(bar, (unsigned)rows_alloc * ROW);
-      for (int bx = 0; bx < tb.nboxes; ++bx)
-        tma_load_3d(smem_tile + (size_t)bx * tb.box_rows * ROW, &fmap, (int)inner0, bx * tb.box_rows, (int)outer, bar);
-    }
-  }
 
-  // ============ stage 0 (Bits): run-start bits -> one word per (chunk, line) ============
-  if constexpr (Bits) {
-    pdl_wait_for_previous_grid();      // the plane is complete (written by the X pass)
+    // ============ stage 0: labels -> run-start / background words ============
+    for (int c = chunk0; !Bits && c < nchunks; c += chunk_step) {
+      const int i0 = c << 5;
+      uint32_t wstart = 0, wzero = 0, ext = 1u;      // ext: a run starts at row i0 + 32 (or the line ends there)
+      if (live) {
+        uint32_t idx = (uint32_t)i0 * ls + (uint32_t)x;
+        const LT* lp = tl + idx;               // (kRoomy) stepped by one line stride per row
+        LT prev = (i0 > 0) ? tl[idx - ls] : (LT)0;
+        uint32_t fdst = fs_a + (uint32_t)i0 * ROW + (uint32_t)x * 4u;
+        if (i0 + 32 <= n) {
+  #pragma unroll
+          for (int r = 0; r < 32; ++r) {
+            const LT here = kRoomy ? *lp : tl[idx];
+            if (kRoomy) lp += ls;
+            if (!UseTMA) sts_f32(fdst + r * ROW, tf[idx]);
+            if (!UseTMA || !kRoomy) idx += ls;
+            if (here != prev) wstart |= (1u << r);
+            if (Epilogue && here == 0) wzero |= (1u << r);
+            prev = here;
+          }
+          if (kDecoupled && i0 + 32 < n) ext = (kRoomy ? *lp : tl[idx]) != prev;
+        } else {
+          for (int r = 0; r < n - i0; ++r) {
+            const LT here = kRoomy ? *lp : tl[idx];
+            if (kRoomy) lp += ls;
+            if (!UseTMA) sts_f32(fdst + r * ROW, tf[idx]);
+            if (!UseTMA || !kRoomy) idx += ls;
+            if (here != prev) wstart |= (1u << r);
+            if (Epilogue && here == 0) wzero |= (1u << r);
+            prev = here;
+          }
+          wstart |= 1u << (n - i0);          // pretend a run starts at row n (line end)
+        }
+        if (i0 == 0) wstart |= 1u;           // a run starts at row 0 by definition
+      }
+      sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wstart);
+      if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wzero);
+      if (kDecoupled) sts_u8(cflag_a + (uint32_t)(c * TX + x), ext << 2);   // bit 2 of the chunk's flag byte, for stage 1
+    }
+    pdl_wait_for_previous_grid();        // nobody may store into f before the previous pass is done
+    if (!UseTMA || !kDecoupled) __syncthreads();   // words, table (and plain-loaded tile) visible; orders the mbarrier init
+    if (UseTMA) mbar_wait(bar, phase);   // float tile has landed
+
+    // every shared address used from here on carries the token, so no (non-volatile) load of the
+    // staged tile can be scheduled above the barrier / the TMA completion wait
+    const uint32_t tok = smem_token();
+    TileLine<TX> ln;
+    ln.f = fs_a + (uint32_t)x * 4u + tok;
+    ln.hull = hullw_a + (uint32_t)x * 4u + tok;
+    const uint32_t startcol = startw_a + (uint32_t)x * 4u + tok;
+    const uint32_t zerocol = zerow_a + (uint32_t)x * 4u + tok;
+    const uint32_t sq_t = sq_a + tok;
+    // per (chunk, line): bit 0 = the long-run segment entering from below is constant,
+    //                    bit 1 = the long-run segment leaving above is constant
+    const uint32_t cflagcol = cflag_a + (uint32_t)x;
+    const uint32_t nzcol = nz_a + (uint32_t)x * 4u;
+    char* const line0 = reinterpret_cast<char*>(tf + x);
+
+    // ============ stage 1: everything that can be finished inside a chunk ============
+    // Per chunk (32 rows of one line): the rows are cut into segments by the run starts; a segment
+    // is LOCAL when its run lies inside the chunk and CROSSING when the run goes on in the chunk
+    // below and / or above.
+    //   (1a) runs of length one: min(f, w2), straight-line predicated code;
+    //   (1b) which segments are constant (no scan needed), from one pass over the samples;
+    //   (1c) hulls of all non-constant segments, ONE loop over their rows (build_hull_rows);
+    //   (1d) outputs of the local runs, ONE loop over their rows (read_out_rows_local).
+    // The hull bits of the crossing segments go to hullw for stages 2 and 3.
+    int any_cross = 0;
     if (live) {
-      const int64_t j = inner0 + x, q = j / rb.sx, rj = j - q * rb.sx;
-      const uint32_t* bstart = rb.start + (outer * rb.outer_words + q * rb.wpr + (rj >> 5));
-      const int bit = (int)(rj & 31);
-      const size_t rw = (size_t)rb.row_words;
       for (int c = chunk0; c < nchunks; c += chunk_step) {
         const int i0 = c << 5;
-        const uint32_t* sp = bstart + (size_t)i0 * rw;
-        uint32_t wstart = 0;
-        if (i0 + 32 <= n) {
-#pragma unroll
-          for (int r = 0; r < 32; ++r) wstart |= ((__ldg(sp + r * rw) >> bit) & 1u) << r;
-        } else {
-          for (int r = 0; r < n - i0; ++r) wstart |= ((__ldg(sp + r * rw) >> bit) & 1u) << r;
-          wstart |= 1u << (n - i0);        // pretend a run starts at row n (line end)
-        }
-        if (i0 == 0) wstart |= 1u;         // a run starts at row 0 by definition
-        sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wstart);
-        if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);   // no sign: not read
-      }
-    } else {
-      for (int c = chunk0; c < nchunks; c += chunk_step) {
-        sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);
-        if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, 0u);
-      }
-    }
-  }
+        const int rows = min(32, n - i0);
+        const uint32_t rowmask = rows == 32 ? 0xffffffffu : ((1u << rows) - 1u);
+        const uint32_t wstart = lds_u32(startcol + (uint32_t)c * ROW);
+        const uint32_t wzero = Epilogue ? lds_u32(zerocol + (uint32_t)c * ROW) : 0u;
+        // bit r of `nextw`: a run starts at row i0 + r + 1 (the line end counts as a start)
+        // ext: a run starts at row i0 + 32 (the line end counts as a start)
+        uint32_t ext = 1u;
+        if (kDecoupled) ext = (lds_u8_volatile(cflagcol + (uint32_t)c * TX) >> 2) & 1u;     // (this thread's own store)
+        else if (i0 + 32 < n) ext = lds_u32(startcol + (uint32_t)(c + 1) * ROW) & 1u;
+        const uint32_t nextw = (wstart >> 1) | (ext << 31);
+        uint32_t single = wstart & nextw & rowmask;          // runs of length one
+        if (!border_lo && c == 0) single &= ~1u;             // rows lacking a border term go the long way
+        if (!border_hi && i0 + 32 >= n) single &= ~(1u << (n - 1 - i0));
 
-  // ============ stage 0: labels -> run-start / background words ============
-  for (int c = chunk0; !Bits && c < nchunks; c += chunk_step) {
-    const int i0 = c << 5;
-    uint32_t wstart = 0, wzero = 0, ext = 1u;      // ext: a run starts at row i0 + 32 (or the line ends there)
-    if (live) {
-      uint32_t idx = (uint32_t)i0 * ls + (uint32_t)x;
-      const LT* lp = tl + idx;               // (kRoomy) stepped by one line stride per row
-      LT prev = (i0 > 0) ? tl[idx - ls] : (LT)0;
-      uint32_t fdst = fs_a + (uint32_t)i0 * ROW + (uint32_t)x * 4u;
-      if (i0 + 32 <= n) {
-#pragma unroll
-        for (int r = 0; r < 32; ++r) {
-          const LT here = kRoomy ? *lp : tl[idx];
-          if (kRoomy) lp += ls;
-          if (!UseTMA) sts_f32(fdst + r * ROW, tf[idx]);
-          if (!UseTMA || !kRoomy) idx += ls;
-          if (here != prev) wstart |= (1u << r);
-          if (Epilogue && here == 0) wzero |= (1u << r);
-          prev = here;
-        }
-        if (kDecoupled && i0 + 32 < n) ext = (kRoomy ? *lp : tl[idx]) != prev;
-      } else {
-        for (int r = 0; r < n - i0; ++r) {
-          const LT here = kRoomy ? *lp : tl[idx];
-          if (kRoomy) lp += ls;
-          if (!UseTMA) sts_f32(fdst + r * ROW, tf[idx]);
-          if (!UseTMA || !kRoomy) idx += ls;
-          if (here != prev) wstart |= (1u << r);
-          if (Epilogue && here == 0) wzero |= (1u << r);
-          prev = here;
-        }
-        wstart |= 1u << (n - i0);          // pretend a run starts at row n (line end)
-      }
-      if (i0 == 0) wstart |= 1u;           // a run starts at row 0 by definition
-    }
-    sts_u32(startw_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wstart);
-    if (Epilogue) sts_u32(zerow_a + (uint32_t)c * ROW + (uint32_t)x * 4u, wzero);
-    if (kDecoupled) sts_u8(cflag_a + (uint32_t)(c * TX + x), ext << 2);   // bit 2 of the chunk's flag byte, for stage 1
-  }
-  pdl_wait_for_previous_grid();        // nobody may store into f before the previous pass is done
-  if (!UseTMA || !kDecoupled) __syncthreads();   // words, table (and plain-loaded tile) visible; orders the mbarrier init
-  if (UseTMA) mbar_wait(bar, 0);       // float tile has landed
-
-  // every shared address used from here on carries the token, so no (non-volatile) load of the
-  // staged tile can be scheduled above the barrier / the TMA completion wait
-  const uint32_t tok = smem_token();
-  TileLine<TX> ln;
-  ln.f = fs_a + (uint32_t)x * 4u + tok;
-  ln.hull = hullw_a + (uint32_t)x * 4u + tok;
-  const uint32_t startcol = startw_a + (uint32_t)x * 4u + tok;
-  const uint32_t zerocol = zerow_a + (uint32_t)x * 4u + tok;
-  const uint32_t sq_t = sq_a + tok;
-  // per (chunk, line): bit 0 = the long-run segment entering from below is constant,
-  //                    bit 1 = the long-run segment leaving above is constant
-  const uint32_t cflagcol = cflag_a + (uint32_t)x;
-  const uint32_t nzcol = nz_a + (uint32_t)x * 4u;
-  char* const line0 = reinterpret_cast<char*>(tf + x);
-
-  // ============ stage 1: everything that can be finished inside a chunk ============
-  // Per chunk (32 rows of one line): the rows are cut into segments by the run starts; a segment
-  // is LOCAL when its run lies inside the chunk and CROSSING when the run goes on in the chunk
-  // below and / or above.
-  //   (1a) runs of length one: min(f, w2), straight-line predicated code;
-  //   (1b) which segments are constant (no scan needed), from one pass over the samples;
-  //   (1c) hulls of all non-constant segments, ONE loop over their rows (build_hull_rows);
-  //   (1d) outputs of the local runs, ONE loop over their rows (read_out_rows_local).
-  // The hull bits of the crossing segments go to hullw for stages 2 and 3.
-  int any_cross = 0;
-  if (live) {
-    for (int c = chunk0; c < nchunks; c += chunk_step) {
-      const int i0 = c << 5;
-      const int rows = min(32, n - i0);
-      const uint32_t rowmask = rows == 32 ? 0xffffffffu : ((1u << rows) - 1u);
-      const uint32_t wstart = lds_u32(startcol + (uint32_t)c * ROW);
-      const uint32_t wzero = Epilogue ? lds_u32(zerocol + (uint32_t)c * ROW) : 0u;
-      // bit r of `nextw`: a run starts at row i0 + r + 1 (the line end counts as a start)
-      // ext: a run starts at row i0 + 32 (the line end counts as a start)
-      uint32_t ext = 1u;
-      if (kDecoupled) ext = (lds_u8_volatile(cflagcol + (uint32_t)c * TX) >> 2) & 1u;     // (this thread's own store)
-      else if (i0 + 32 < n) ext = lds_u32(startcol + (uint32_t)(c + 1) * ROW) & 1u;
-      const uint32_t nextw = (wstart >> 1) | (ext << 31);
-      uint32_t single = wstart & nextw & rowmask;          // runs of length one
-      if (!border_lo && c == 0) single &= ~1u;             // rows lacking a border term go the long way
-      if (!border_hi && i0 + 32 >= n) single &= ~(1u << (n - 1 - i0));
-
-      // (1a) runs of length one: out = min(f, w2).  The pass works in place, so a row that keeps its
-      // value (f <= w2 -- with label noise nearly every row of the later passes) is not stored at
-      // all: one pass over the chunk's samples marks the rows that change (`chg`) and, for (1b),
-      // the rows whose sample differs from the row below (`breaks`).  The square root / sign of the
-      // last pass rewrites every row.
-      uint32_t breaks = 0u;
-      bool have_breaks = false;
-      const uint32_t multi = rowmask & ~single;
-      {
-        const uint32_t at = ln.f + (uint32_t)i0 * ROW;
-        if (single && !Epilogue && kRoomy) {
-          have_breaks = true;
-          uint32_t chg = 0u;
-          float prev = lds_f32(at);
-          if (prev > w2) chg = 1u;
-          if (rows == 32) {
-#pragma unroll
-            for (int r = 1; r < 32; ++r) {
-              const float cur = lds_f32(at + r * ROW);
-              if (cur != prev) breaks |= 1u << r;
-              if (cur > w2) chg |= 1u << r;
-              prev = cur;
-            }
-          } else {
-            for (int r = 1; r < rows; ++r) {
-              const float cur = lds_f32(at + r * ROW);
-              if (cur != prev) breaks |= 1u << r;
-              if (cur > w2) chg |= 1u << r;
-              prev = cur;
-            }
-          }
-          for (chg &= single; chg; chg &= chg - 1u)
-            *reinterpret_cast<float*>(line0 + (size_t)(i0 + __ffs(chg) - 1) * pitch) = w2;
-        } else {
-          if (single) {                     // value computed unconditionally, store predicated
-            char* op = line0 + (size_t)i0 * pitch;
+        // (1a) runs of length one: out = min(f, w2).  The pass works in place, so a row that keeps its
+        // value (f <= w2 -- with label noise nearly every row of the later passes) is not stored at
+        // all: one pass over the chunk's samples marks the rows that change (`chg`) and, for (1b),
+        // the rows whose sample differs from the row below (`breaks`).  The square root / sign of the
+        // last pass rewrites every row.
+        uint32_t breaks = 0u;
+        bool have_breaks = false;
+        const uint32_t multi = rowmask & ~single;
+        {
+          const uint32_t at = ln.f + (uint32_t)i0 * ROW;
+          if (single && !Epilogue && kRoomy) {
+            have_breaks = true;
+            uint32_t chg = 0u;
+            float prev = lds_f32(at);
+            if (prev > w2) chg = 1u;
             if (rows == 32) {
-#pragma unroll
-              for (int r = 0; r < 32; ++r) {
-                const float fv = lds_f32(at + r * ROW);
-                if (Epilogue) {
-                  const float v = finish_value(fminf(fv, w2), (wzero >> r) & 1u, flags);
-                  if (single & (1u << r)) *reinterpret_cast<float*>(op) = v;
-                } else {
-                  if ((single & (1u << r)) && fv > w2) *reinterpret_cast<float*>(op) = w2;
-                }
-                op += pitch;
+  #pragma unroll
+              for (int r = 1; r < 32; ++r) {
+                const float cur = lds_f32(at + r * ROW);
+                if (cur != prev) breaks |= 1u << r;
+                if (cur > w2) chg |= 1u << r;
+                prev = cur;
               }
             } else {
-              for (int r = 0; r < rows; ++r) {
-                const float fv = lds_f32(at + r * ROW);
-                float v = fminf(fv, w2);
-                if (Epilogue) v = finish_value(v, (wzero >> r) & 1u, flags);
-                if ((single & (1u << r)) && (Epilogue || fv > w2)) *reinterpret_cast<float*>(op) = v;
-                op += pitch;
+              for (int r = 1; r < rows; ++r) {
+                const float cur = lds_f32(at + r * ROW);
+                if (cur != prev) breaks |= 1u << r;
+                if (cur > w2) chg |= 1u << r;
+                prev = cur;
+              }
+            }
+            for (chg &= single; chg; chg &= chg - 1u)
+              *reinterpret_cast<float*>(line0 + (size_t)(i0 + __ffs(chg) - 1) * pitch) = w2;
+          } else {
+            if (single) {                     // value computed unconditionally, store predicated
+              char* op = line0 + (size_t)i0 * pitch;
+              if (rows == 32) {
+  #pragma unroll
+                for (int r = 0; r < 32; ++r) {
+                  const float fv = lds_f32(at + r * ROW);
+                  if (Epilogue) {
+                    const float v = finish_value(fminf(fv, w2), (wzero >> r) & 1u, flags);
+                    if (single & (1u << r)) *reinterpret_cast<float*>(op) = v;
+                  } else {
+                    if ((single & (1u << r)) && fv > w2) *reinterpret_cast<float*>(op) = w2;
+                  }
+                  op += pitch;
+                }
+              } else {
+                for (int r = 0; r < rows; ++r) {
+                  const float fv = lds_f32(at + r * ROW);
+                  float v = fminf(fv, w2);
+                  if (Epilogue) v = finish_value(v, (wzero >> r) & 1u, flags);
+                  if ((single & (1u << r)) && (Epilogue || fv > w2)) *reinterpret_cast<float*>(op) = v;
+                  op += pitch;
+                }
               }
             }
           }
         }
-      }
 
-      uint32_t hb = 0u;
-      if (multi) {
-        const uint32_t wreal = wstart & rowmask;
-        const uint32_t starts = wreal | 1u;                // the segment entering from below starts at row 0
-        const bool entering = !(wstart & 1u), leaving = !ext;
-        const uint32_t ent_mask = entering ? (wreal ? ((1u << (__ffs(wreal) - 1)) - 1u) : rowmask) : 0u;
-        const int s2 = 31 - __clz(starts);                 // first row of the last segment
-        const uint32_t lea_mask = (leaving && wreal) ? (0xffffffffu << s2) : 0u;
-        const uint32_t cross_mask = ent_mask | lea_mask;
+        uint32_t hb = 0u;
+        if (multi) {
+          const uint32_t wreal = wstart & rowmask;
+          const uint32_t starts = wreal | 1u;                // the segment entering from below starts at row 0
+          const bool entering = !(wstart & 1u), leaving = !ext;
+          const uint32_t ent_mask = entering ? (wreal ? ((1u << (__ffs(wreal) - 1)) - 1u) : rowmask) : 0u;
+          const int s2 = 31 - __clz(starts);                 // first row of the last segment
+          const uint32_t lea_mask = (leaving && wreal) ? (0xffffffffu << s2) : 0u;
+          const uint32_t cross_mask = ent_mask | lea_mask;
 
-        // (1b) rows whose sample differs from the row below, then the rows of non-constant segments
-        if (!have_breaks) {
-          const uint32_t at = ln.f + (uint32_t)i0 * ROW;
-          float prev = lds_f32(at);
-          if (rows == 32) {
-#pragma unroll
-            for (int r = 1; r < 32; ++r) {
-              const float cur = lds_f32(at + r * ROW);
-              if (cur != prev) breaks |= 1u << r;
-              prev = cur;
+          // (1b) rows whose sample differs from the row below, then the rows of non-constant segments
+          if (!have_breaks) {
+            const uint32_t at = ln.f + (uint32_t)i0 * ROW;
+            float prev = lds_f32(at);
+            if (rows == 32) {
+  #pragma unroll
+              for (int r = 1; r < 32; ++r) {
+                const float cur = lds_f32(at + r * ROW);
+                if (cur != prev) breaks |= 1u << r;
+                prev = cur;
+              }
+            } else {
+              for (int r = 1; r < rows; ++r) {
+                const float cur = lds_f32(at + r * ROW);
+                if (cur != prev) breaks |= 1u << r;
+                prev = cur;
+              }
             }
-          } else {
-            for (int r = 1; r < rows; ++r) {
-              const float cur = lds_f32(at + r * ROW);
-              if (cur != prev) breaks |= 1u << r;
-              prev = cur;
+          }
+          const uint32_t noncst = nonconstant_rows(starts, breaks & ~starts & rowmask) & multi;
+          // a constant crossing segment is its own hull: equal heights never hide one another
+          if (cross_mask) {
+            uint32_t cflags = 0u;
+            if (ent_mask && !(noncst & ent_mask)) { cflags |= 1u; if (ln.fval(i0) < inf) hb |= ent_mask; }
+            if (lea_mask && !(noncst & lea_mask)) { cflags |= 2u; if (ln.fval(i0 + s2) < inf) hb |= lea_mask; }
+            sts_u8(cflagcol + (uint32_t)c * TX, cflags);
+            any_cross |= 1;
+            // bit 1: a crossing run that is not constant here, or across the boundary below
+            if ((noncst & cross_mask) || (entering && ln.fval(i0) != ln.fval(i0 - 1))) any_cross |= 2;
+          }
+          // (1c) hulls of the non-constant segments
+          if (noncst) hb = IntHull ? build_hull_rows_int<TX>(ln, i0, noncst, starts, w2i, hb)
+                                   : build_hull_rows<TX>(ln, i0, noncst, starts, w2d, hb);
+          // (1d) the local runs are finished here
+          const uint32_t local = multi & ~cross_mask;
+          if (local)
+            read_out_rows_local<TX, Epilogue>(ln, i0, local, starts, nextw, noncst, hb, wzero, n, w2, border_lo,
+                                              border_hi, sq_t, line0, pitch, flags);
+        }
+        sts_u32(ln.hull + (uint32_t)c * ROW, hb);
+      }
+    }
+    if (!__syncthreads_or(any_cross)) {                      // every run was finished inside its chunk
+      if constexpr (Bits && !Epilogue) {
+        if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
+      }
+      continue;
+    }
+    // Tiles with crossing runs: one bit per chunk that holds a run start, per line, so that the ends
+    // of a crossing run are two look-ups instead of a walk over the chunks (made visible by the vote below).
+    if (live && use_nz) {
+      for (int c = chunk0; c < nchunks; c += chunk_step) {
+        const uint32_t rowmask = (n - (c << 5) >= 32) ? 0xffffffffu : ((1u << (n - (c << 5))) - 1u);
+        if (lds_u32(startcol + (uint32_t)c * ROW) & rowmask) red_shared_or(nzcol, 1u << c);
+      }
+    }
+    // every crossing run of the tile constant (blocky labels, solid objects along this axis)?  Then
+    // nothing needs stitching and stage 3 writes min(f, border terms) without looking at any hull.
+    const bool all_const = !__syncthreads_or(any_cross & 2);
+
+    // ============ stage 2: stitch the hulls of runs that cross chunk boundaries ============
+    // Divide and conquer over the chunk segments of every run: the boundaries of a run are numbered
+    // j = 1, 2, ... from the chunk the run starts in; in the round with group size `half` every
+    // boundary with j = half (mod 2 half) merges the `half` segments left of it with the (up to)
+    // `half` segments right of it, all runs, boundaries and lines in parallel.  Left of a boundary
+    // stands the finished hull of the run's rows in the left group (A), right of it the finished hull
+    // of its rows in the right group (B).  All of A lies left of all of B, so the hull of the union
+    // is a prefix of A plus a suffix of B: drop A's top while it is hidden by (the vertex below it,
+    // B's first), drop B's first while it is hidden by (A's top, B's second), until neither applies.
+    // Numbering the boundaries per run (not per line) keeps the number of rounds -- each ends in a
+    // CTA-wide barrier -- at log2 of the longest run's chunk count instead of log2 of the line's:
+    // two rounds for runs of up to 128 rows.  Boundaries of different runs may meet in one hull word,
+    // so bits are dropped with an atomic AND.
+    if (!all_const) {
+      for (int half = 1; half < nchunks; half <<= 1) {
+        int more = 0;
+        if (live) {
+          for (int c = chunk0; c < nchunks; c += chunk_step) {
+            if (c == 0) continue;                              // no boundary below the first chunk
+            const int i0 = c << 5;
+            const uint32_t wc = lds_u32(startcol + (uint32_t)c * ROW);
+            if (wc & 1u) continue;                             // a run starts exactly here: nothing crosses
+            int a = 0;                                         // start of the run that crosses
+            int b = n;                                         // its end (exclusive)
+            if (use_nz) {
+              const uint32_t nzw = lds_u32_volatile(nzcol);
+              const uint32_t below = nzw & ((1u << c) - 1u), above = nzw & (0xffffffffu << c);
+              if (below) {
+                const int cc = 31 - __clz(below);
+                a = (cc << 5) + 31 - __clz(lds_u32(startcol + (uint32_t)cc * ROW));
+              }
+              if (above) {
+                const int cc = __ffs(above) - 1;
+                b = min(n, (cc << 5) + __ffs(lds_u32(startcol + (uint32_t)cc * ROW)) - 1);
+              }
+            } else {
+              for (int cc = c - 1; cc >= 0; --cc) {
+                const uint32_t w = lds_u32(startcol + (uint32_t)cc * ROW);
+                if (w) { a = (cc << 5) + 31 - __clz(w); break; }
+              }
+              for (int cc = c; cc < nchunks; ++cc) {
+                const uint32_t w = lds_u32(startcol + (uint32_t)cc * ROW);
+                if (w) { b = min(n, (cc << 5) + __ffs(w) - 1); break; }
+              }
+            }
+            const int ca = a >> 5, cb = (b - 1) >> 5;          // the run has boundaries 1 .. cb - ca
+            if (cb - ca >= 2 * half) more = 1;                 // some boundary of it waits for a later round
+            if (((c - ca) & (2 * half - 1)) != half) continue; // not this boundary's round
+            if (half == 1) {
+              // (first round only: later rounds see hulls that earlier merges may have thinned out)
+              // equal-height rows on both sides of the boundary cannot hide one another: when the two
+              // adjacent chunk segments are constant and equal there is nothing to drop here
+              const uint32_t fl_hi = lds_u8_volatile(cflagcol + (uint32_t)c * TX);
+              const uint32_t fl_lo = lds_u8_volatile(cflagcol + (uint32_t)(c - 1) * TX);
+              const bool lo_const = (a >= ((c - 1) << 5)) ? (fl_lo & 2u) != 0 : (fl_lo & 1u) != 0;
+              if ((fl_hi & 1u) && lo_const && ln.fval(i0) == ln.fval(i0 - 1)) continue;
+            }
+            const int alo = max(a, (c - half) << 5);           // the run's rows inside the two groups
+            const int bhi = min(b, min(n, (c + half) << 5));
+            int av = prev_vertex<TX>(ln, i0, alo);
+            int bv = next_vertex<TX>(ln, i0 - 1, bhi);
+            if (av < 0 || bv < 0) continue;
+            int ap = prev_vertex<TX>(ln, av, alo);
+            int bn = next_vertex<TX>(ln, bv, bhi);
+            float fa = ln.fval(av), fb = ln.fval(bv);
+            float fap = ap >= 0 ? ln.fval(ap) : 0.0f, fbn = bn >= 0 ? ln.fval(bn) : 0.0f;
+            for (;;) {
+              if (ap >= 0 && (IntHull ? vertex_hidden_int(ap, fap, av, fa, bv, fb, w2i)
+                                      : vertex_hidden(ap, fap, av, fa, bv, fb, w2d))) {   // A's top is hidden
+                ln.drop(av);
+                av = ap; fa = fap;
+                ap = prev_vertex<TX>(ln, av, alo);
+                if (ap >= 0) fap = ln.fval(ap);
+                continue;
+              }
+              if (bn >= 0 && (IntHull ? vertex_hidden_int(av, fa, bv, fb, bn, fbn, w2i)
+                                      : vertex_hidden(av, fa, bv, fb, bn, fbn, w2d))) {   // B's first is hidden
+                ln.drop(bv);
+                bv = bn; fb = fbn;
+                bn = next_vertex<TX>(ln, bv, bhi);
+                if (bn >= 0) fbn = ln.fval(bn);
+                continue;
+              }
+              break;
             }
           }
         }
-        const uint32_t noncst = nonconstant_rows(starts, breaks & ~starts & rowmask) & multi;
-        // a constant crossing segment is its own hull: equal heights never hide one another
-        if (cross_mask) {
-          uint32_t cflags = 0u;
-          if (ent_mask && !(noncst & ent_mask)) { cflags |= 1u; if (ln.fval(i0) < inf) hb |= ent_mask; }
-          if (lea_mask && !(noncst & lea_mask)) { cflags |= 2u; if (ln.fval(i0 + s2) < inf) hb |= lea_mask; }
-          sts_u8(cflagcol + (uint32_t)c * TX, cflags);
-          any_cross |= 1;
-          // bit 1: a crossing run that is not constant here, or across the boundary below
-          if ((noncst & cross_mask) || (entering && ln.fval(i0) != ln.fval(i0 - 1))) any_cross |= 2;
-        }
-        // (1c) hulls of the non-constant segments
-        if (noncst) hb = IntHull ? build_hull_rows_int<TX>(ln, i0, noncst, starts, w2i, hb)
-                                 : build_hull_rows<TX>(ln, i0, noncst, starts, w2d, hb);
-        // (1d) the local runs are finished here
-        const uint32_t local = multi & ~cross_mask;
-        if (local)
-          read_out_rows_local<TX, Epilogue>(ln, i0, local, starts, nextw, noncst, hb, wzero, n, w2, border_lo,
-                                            border_hi, sq_t, line0, pitch, flags);
+        if (!__syncthreads_or(more)) break;                    // (the barrier of the round)
       }
-      sts_u32(ln.hull + (uint32_t)c * ROW, hb);
     }
-  }
-  if (!__syncthreads_or(any_cross)) {                      // every run was finished inside its chunk
+
+    // ============ stage 3: outputs of the crossing segments, ONE loop over their rows per chunk ============
+    if (live) {
+      for (int c = chunk0; c < nchunks; c += chunk_step) {
+        const int i0 = c << 5;
+        const int rows = min(32, n - i0);
+        const uint32_t rowmask = rows == 32 ? 0xffffffffu : ((1u << rows) - 1u);
+        const uint32_t wstart = lds_u32(startcol + (uint32_t)c * ROW);
+        const uint32_t wzero = Epilogue ? lds_u32(zerocol + (uint32_t)c * ROW) : 0u;
+        const bool entering = !(wstart & 1u);                             // only possible for c > 0
+        bool leaving = false;
+        if (i0 + 32 < n) leaving = !(lds_u32(startcol + (uint32_t)(c + 1) * ROW) & 1u);
+        if (!entering && !leaving) continue;
+        const uint32_t wreal = wstart & rowmask;
+        const int s2 = 31 - __clz(wreal | 1u);                            // first row of the last segment
+        const uint32_t ent_mask = entering ? (wreal ? ((1u << (__ffs(wreal) - 1)) - 1u) : rowmask) : 0u;
+        const uint32_t lea_mask = (leaving && wreal) ? (0xffffffffu << s2) : 0u;
+
+        // the runs of the two segments: [a_ent, b_ent) came in from below, [i0 + s2, b_up) leaves above
+        int a_ent = 0, b_up = n;
+        if (use_nz) {                  // nearest chunks with a run start, from the line's chunk mask
+          const uint32_t nzw = lds_u32_volatile(nzcol);
+          const uint32_t below = entering ? (nzw & ((1u << c) - 1u)) : 0u;
+          const uint32_t above = leaving ? (nzw & (0xfffffffeu << c)) : 0u;
+          if (below) {
+            const int cc = 31 - __clz(below);
+            a_ent = (cc << 5) + 31 - __clz(lds_u32(startcol + (uint32_t)cc * ROW));
+          }
+          if (above) {
+            const int cc = __ffs(above) - 1;
+            b_up = min(n, (cc << 5) + __ffs(lds_u32(startcol + (uint32_t)cc * ROW)) - 1);
+          }
+        } else {
+          if (entering) {
+            for (int cc = c - 1; cc >= 0; --cc) {
+              const uint32_t ws = lds_u32(startcol + (uint32_t)cc * ROW);
+              if (ws) { a_ent = (cc << 5) + 31 - __clz(ws); break; }
+            }
+          }
+          if (leaving) {
+            for (int cc = c + 1; cc < nchunks; ++cc) {
+              const uint32_t ws = lds_u32(startcol + (uint32_t)cc * ROW);
+              if (ws) { b_up = min(n, (cc << 5) + __ffs(ws) - 1); break; }
+            }
+          }
+        }
+        const int b_ent = wreal ? (i0 + __ffs(wreal) - 1) : (leaving ? b_up : min(n, i0 + 32));
+        const bool cst_ent = ent_mask && (all_const || run_is_constant<TX>(ln, cflagcol, a_ent, b_ent));
+        const bool cst_lea = lea_mask && (all_const || run_is_constant<TX>(ln, cflagcol, i0 + s2, b_up));
+
+        // one straight loop per crossing segment (the rows of a segment are adjacent), running addresses
+        for (int seg = 0; seg < 2; ++seg) {
+          const uint32_t mask = seg ? lea_mask : ent_mask;
+          if (!mask) continue;
+          const int rlo = __ffs(mask) - 1, rhi = 32 - __clz(mask);      // rows [rlo, rhi) of the chunk
+          const int a = seg ? i0 + s2 : a_ent, b = seg ? b_up : b_ent;
+          const bool cst = seg ? cst_lea : cst_ent;
+          const bool lo_b = a > 0 || border_lo, hi_b = b < n || border_hi, bg = (wzero >> rlo) & 1u;
+          uint32_t sq_lo = sq_t + (uint32_t)(i0 + rlo - a + 1) * 4u;   // sq[i - a + 1]
+          uint32_t sq_hi = sq_t + (uint32_t)(b - i0 - rlo) * 4u;       // sq[b - i]
+          char* dst = line0 + (size_t)(i0 + rlo) * pitch;
+          if (cst) {
+            // a constant run: out = min(f, border terms) (solid objects, blocky labels, background).
+            // The run's one value against the smallest border terms these rows can see (those of the
+            // rows nearest to a and to b): when it is not above them every row keeps its value, and as
+            // the pass works in place nothing has to be stored at all
+            uint32_t f_at = ln.f + (uint32_t)(i0 + rlo) * ROW;
+            const float f0 = lds_f32(f_at);
+            const float lo_min = lo_b ? lds_f32(sq_lo) : inf;
+            const float hi_min = hi_b ? lds_f32(sq_t + (uint32_t)(b - i0 - rhi + 1) * 4u) : inf;
+            if (f0 <= fminf(lo_min, hi_min)) {
+              if (!Epilogue) continue;
+              const float v = finish_value(f0, bg, flags);
+              if (__float_as_uint(v) == __float_as_uint(f0)) continue;
+              for (int r = rlo; r < rhi; ++r) { *reinterpret_cast<float*>(dst) = v; dst += pitch; }
+              continue;
+            }
+  #pragma unroll 4
+            for (int r = rlo; r < rhi; ++r) {
+              float best = lds_f32(f_at);
+              if (lo_b) best = fminf(best, lds_f32(sq_lo));
+              if (hi_b) best = fminf(best, lds_f32(sq_hi));
+              if (Epilogue) best = finish_value(best, bg, flags);
+              *reinterpret_cast<float*>(dst) = best;
+              f_at += ROW; sq_lo += 4u; sq_hi -= 4u; dst += pitch;
+            }
+            continue;
+          }
+          HullWalk w;
+          walk_begin<TX>(w, ln, i0 + rlo, a, b, w2);
+          for (int i = i0 + rlo; i < i0 + rhi; ++i) {
+            float best = inf;
+            if (w.v >= 0) {
+              best = __fmaf_rn(w2, __fmul_rn(w.dv, w.dv), w.fv);
+              while (w.v1 >= 0) {
+                const float cand = __fmaf_rn(w2, __fmul_rn(w.dv1, w.dv1), w.fv1);
+                if (!(cand <= best)) break;
+                if (cand == best && !tie_not_above(w2, w.dv1, w.fv1, w.dv, w.fv)) break;
+                best = cand; w.v = w.v1; w.fv = w.fv1; w.dv = w.dv1;
+                walk_advance<TX>(w, ln, i);
+              }
+              w.dv += 1.0f; w.dv1 += 1.0f;
+            }
+            if (lo_b) best = fminf(best, lds_f32(sq_lo));
+            if (hi_b) best = fminf(best, lds_f32(sq_hi));
+            if (Epilogue) best = finish_value(best, bg, flags);             // a run has one label
+            *reinterpret_cast<float*>(dst) = best;
+            sq_lo += 4u; sq_hi -= 4u; dst += pitch;
+          }
+        }
+      }
+    }
     if constexpr (Bits && !Epilogue) {
       if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
     }
-    return;
-  }
-  // Tiles with crossing runs: one bit per chunk that holds a run start, per line, so that the ends
-  // of a crossing run are two look-ups instead of a walk over the chunks (made visible by the vote below).
-  if (live && use_nz) {
-    for (int c = chunk0; c < nchunks; c += chunk_step) {
-      const uint32_t rowmask = (n - (c << 5) >= 32) ? 0xffffffffu : ((1u << (n - (c << 5))) - 1u);
-      if (lds_u32(startcol + (uint32_t)c * ROW) & rowmask) red_shared_or(nzcol, 1u << c);
-    }
-  }
-  // every crossing run of the tile constant (blocky labels, solid objects along this axis)?  Then
-  // nothing needs stitching and stage 3 writes min(f, border terms) without looking at any hull.
-  const bool all_const = !__syncthreads_or(any_cross & 2);
-
-  // ============ stage 2: stitch the hulls of runs that cross chunk boundaries ============
-  // Divide and conquer over the chunk segments of every run: the boundaries of a run are numbered
-  // j = 1, 2, ... from the chunk the run starts in; in the round with group size `half` every
-  // boundary with j = half (mod 2 half) merges the `half` segments left of it with the (up to)
-  // `half` segments right of it, all runs, boundaries and lines in parallel.  Left of a boundary
-  // stands the finished hull of the run's rows in the left group (A), right of it the finished hull
-  // of its rows in the right group (B).  All of A lies left of all of B, so the hull of the union
-  // is a prefix of A plus a suffix of B: drop A's top while it is hidden by (the vertex below it,
-  // B's first), drop B's first while it is hidden by (A's top, B's second), until neither applies.
-  // Numbering the boundaries per run (not per line) keeps the number of rounds -- each ends in a
-  // CTA-wide barrier -- at log2 of the longest run's chunk count instead of log2 of the line's:
-  // two rounds for runs of up to 128 rows.  Boundaries of different runs may meet in one hull word,
-  // so bits are dropped with an atomic AND.
-  if (!all_const) {
-    for (int half = 1; half < nchunks; half <<= 1) {
-      int more = 0;
-      if (live) {
-        for (int c = chunk0; c < nchunks; c += chunk_step) {
-          if (c == 0) continue;                              // no boundary below the first chunk
-          const int i0 = c << 5;
-          const uint32_t wc = lds_u32(startcol + (uint32_t)c * ROW);
-          if (wc & 1u) continue;                             // a run starts exactly here: nothing crosses
-          int a = 0;                                         // start of the run that crosses
-          int b = n;                                         // its end (exclusive)
-          if (use_nz) {
-            const uint32_t nzw = lds_u32_volatile(nzcol);
-            const uint32_t below = nzw & ((1u << c) - 1u), above = nzw & (0xffffffffu << c);
-            if (below) {
-              const int cc = 31 - __clz(below);
-              a = (cc << 5) + 31 - __clz(lds_u32(startcol + (uint32_t)cc * ROW));
-            }
-            if (above) {
-              const int cc = __ffs(above) - 1;
-              b = min(n, (cc << 5) + __ffs(lds_u32(startcol + (uint32_t)cc * ROW)) - 1);
-            }
-          } else {
-            for (int cc = c - 1; cc >= 0; --cc) {
-              const uint32_t w = lds_u32(startcol + (uint32_t)cc * ROW);
-              if (w) { a = (cc << 5) + 31 - __clz(w); break; }
-            }
-            for (int cc = c; cc < nchunks; ++cc) {
-              const uint32_t w = lds_u32(startcol + (uint32_t)cc * ROW);
-              if (w) { b = min(n, (cc << 5) + __ffs(w) - 1); break; }
-            }
-          }
-          const int ca = a >> 5, cb = (b - 1) >> 5;          // the run has boundaries 1 .. cb - ca
-          if (cb - ca >= 2 * half) more = 1;                 // some boundary of it waits for a later round
-          if (((c - ca) & (2 * half - 1)) != half) continue; // not this boundary's round
-          if (half == 1) {
-            // (first round only: later rounds see hulls that earlier merges may have thinned out)
-            // equal-height rows on both sides of the boundary cannot hide one another: when the two
-            // adjacent chunk segments are constant and equal there is nothing to drop here
-            const uint32_t fl_hi = lds_u8_volatile(cflagcol + (uint32_t)c * TX);
-            const uint32_t fl_lo = lds_u8_volatile(cflagcol + (uint32_t)(c - 1) * TX);
-            const bool lo_const = (a >= ((c - 1) << 5)) ? (fl_lo & 2u) != 0 : (fl_lo & 1u) != 0;
-            if ((fl_hi & 1u) && lo_const && ln.fval(i0) == ln.fval(i0 - 1)) continue;
-          }
-          const int alo = max(a, (c - half) << 5);           // the run's rows inside the two groups
-          const int bhi = min(b, min(n, (c + half) << 5));
-          int av = prev_vertex<TX>(ln, i0, alo);
-          int bv = next_vertex<TX>(ln, i0 - 1, bhi);
-          if (av < 0 || bv < 0) continue;
-          int ap = prev_vertex<TX>(ln, av, alo);
-          int bn = next_vertex<TX>(ln, bv, bhi);
-          float fa = ln.fval(av), fb = ln.fval(bv);
-          float fap = ap >= 0 ? ln.fval(ap) : 0.0f, fbn = bn >= 0 ? ln.fval(bn) : 0.0f;
-          for (;;) {
-            if (ap >= 0 && (IntHull ? vertex_hidden_int(ap, fap, av, fa, bv, fb, w2i)
-                                    : vertex_hidden(ap, fap, av, fa, bv, fb, w2d))) {   // A's top is hidden
-              ln.drop(av);
-              av = ap; fa = fap;
-              ap = prev_vertex<TX>(ln, av, alo);
-              if (ap >= 0) fap = ln.fval(ap);
-              continue;
-            }
-            if (bn >= 0 && (IntHull ? vertex_hidden_int(av, fa, bv, fb, bn, fbn, w2i)
-                                    : vertex_hidden(av, fa, bv, fb, bn, fbn, w2d))) {   // B's first is hidden
-              ln.drop(bv);
-              bv = bn; fb = fbn;
-              bn = next_vertex<TX>(ln, bv, bhi);
-              if (bn >= 0) fbn = ln.fval(bn);
-              continue;
-            }
-            break;
-          }
-        }
-      }
-      if (!__syncthreads_or(more)) break;                    // (the barrier of the round)
-    }
-  }
-
-  // ============ stage 3: outputs of the crossing segments, ONE loop over their rows per chunk ============
-  if (live) {
-    for (int c = chunk0; c < nchunks; c += chunk_step) {
-      const int i0 = c << 5;
-      const int rows = min(32, n - i0);
-      const uint32_t rowmask = rows == 32 ? 0xffffffffu : ((1u << rows) - 1u);
-      const uint32_t wstart = lds_u32(startcol + (uint32_t)c * ROW);
-      const uint32_t wzero = Epilogue ? lds_u32(zerocol + (uint32_t)c * ROW) : 0u;
-      const bool entering = !(wstart & 1u);                             // only possible for c > 0
-      bool leaving = false;
-      if (i0 + 32 < n) leaving = !(lds_u32(startcol + (uint32_t)(c + 1) * ROW) & 1u);
-      if (!entering && !leaving) continue;
-      const uint32_t wreal = wstart & rowmask;
-      const int s2 = 31 - __clz(wreal | 1u);                            // first row of the last segment
-      const uint32_t ent_mask = entering ? (wreal ? ((1u << (__ffs(wreal) - 1)) - 1u) : rowmask) : 0u;
-      const uint32_t lea_mask = (leaving && wreal) ? (0xffffffffu << s2) : 0u;
-
-      // the runs of the two segments: [a_ent, b_ent) came in from below, [i0 + s2, b_up) leaves above
-      int a_ent = 0, b_up = n;
-      if (use_nz) {                  // nearest chunks with a run start, from the line's chunk mask
-        const uint32_t nzw = lds_u32_volatile(nzcol);
-        const uint32_t below = entering ? (nzw & ((1u << c) - 1u)) : 0u;
-        const uint32_t above = leaving ? (nzw & (0xfffffffeu << c)) : 0u;
-        if (below) {
-          const int cc = 31 - __clz(below);
-          a_ent = (cc << 5) + 31 - __clz(lds_u32(startcol + (uint32_t)cc * ROW));
-        }
-        if (above) {
-          const int cc = __ffs(above) - 1;
-          b_up = min(n, (cc << 5) + __ffs(lds_u32(startcol + (uint32_t)cc * ROW)) - 1);
-        }
-      } else {
-        if (entering) {
-          for (int cc = c - 1; cc >= 0; --cc) {
-            const uint32_t ws = lds_u32(startcol + (uint32_t)cc * ROW);
-            if (ws) { a_ent = (cc << 5) + 31 - __clz(ws); break; }
-          }
-        }
-        if (leaving) {
-          for (int cc = c + 1; cc < nchunks; ++cc) {
-            const uint32_t ws = lds_u32(startcol + (uint32_t)cc * ROW);
-            if (ws) { b_up = min(n, (cc << 5) + __ffs(ws) - 1); break; }
-          }
-        }
-      }
-      const int b_ent = wreal ? (i0 + __ffs(wreal) - 1) : (leaving ? b_up : min(n, i0 + 32));
-      const bool cst_ent = ent_mask && (all_const || run_is_constant<TX>(ln, cflagcol, a_ent, b_ent));
-      const bool cst_lea = lea_mask && (all_const || run_is_constant<TX>(ln, cflagcol, i0 + s2, b_up));
-
-      // one straight loop per crossing segment (the rows of a segment are adjacent), running addresses
-      for (int seg = 0; seg < 2; ++seg) {
-        const uint32_t mask = seg ? lea_mask : ent_mask;
-        if (!mask) continue;
-        const int rlo = __ffs(mask) - 1, rhi = 32 - __clz(mask);      // rows [rlo, rhi) of the chunk
-        const int a = seg ? i0 + s2 : a_ent, b = seg ? b_up : b_ent;
-        const bool cst = seg ? cst_lea : cst_ent;
-        const bool lo_b = a > 0 || border_lo, hi_b = b < n || border_hi, bg = (wzero >> rlo) & 1u;
-        uint32_t sq_lo = sq_t + (uint32_t)(i0 + rlo - a + 1) * 4u;   // sq[i - a + 1]
-        uint32_t sq_hi = sq_t + (uint32_t)(b - i0 - rlo) * 4u;       // sq[b - i]
-        char* dst = line0 + (size_t)(i0 + rlo) * pitch;
-        if (cst) {
-          // a constant run: out = min(f, border terms) (solid objects, blocky labels, background).
-          // The run's one value against the smallest border terms these rows can see (those of the
-          // rows nearest to a and to b): when it is not above them every row keeps its value, and as
-          // the pass works in place nothing has to be stored at all
-          uint32_t f_at = ln.f + (uint32_t)(i0 + rlo) * ROW;
-          const float f0 = lds_f32(f_at);
-          const float lo_min = lo_b ? lds_f32(sq_lo) : inf;
-          const float hi_min = hi_b ? lds_f32(sq_t + (uint32_t)(b - i0 - rhi + 1) * 4u) : inf;
-          if (f0 <= fminf(lo_min, hi_min)) {
-            if (!Epilogue) continue;
-            const float v = finish_value(f0, bg, flags);
-            if (__float_as_uint(v) == __float_as_uint(f0)) continue;
-            for (int r = rlo; r < rhi; ++r) { *reinterpret_cast<float*>(dst) = v; dst += pitch; }
-            continue;
-          }
-#pragma unroll 4
-          for (int r = rlo; r < rhi; ++r) {
-            float best = lds_f32(f_at);
-            if (lo_b) best = fminf(best, lds_f32(sq_lo));
-            if (hi_b) best = fminf(best, lds_f32(sq_hi));
-            if (Epilogue) best = finish_value(best, bg, flags);
-            *reinterpret_cast<float*>(dst) = best;
-            f_at += ROW; sq_lo += 4u; sq_hi -= 4u; dst += pitch;
-          }
-          continue;
-        }
-        HullWalk w;
-        walk_begin<TX>(w, ln, i0 + rlo, a, b, w2);
-        for (int i = i0 + rlo; i < i0 + rhi; ++i) {
-          float best = inf;
-          if (w.v >= 0) {
-            best = __fmaf_rn(w2, __fmul_rn(w.dv, w.dv), w.fv);
-            while (w.v1 >= 0) {
-              const float cand = __fmaf_rn(w2, __fmul_rn(w.dv1, w.dv1), w.fv1);
-              if (!(cand <= best)) break;
-              if (cand == best && !tie_not_above(w2, w.dv1, w.fv1, w.dv, w.fv)) break;
-              best = cand; w.v = w.v1; w.fv = w.fv1; w.dv = w.dv1;
-              walk_advance<TX>(w, ln, i);
-            }
-            w.dv += 1.0f; w.dv1 += 1.0f;
-          }
-          if (lo_b) best = fminf(best, lds_f32(sq_lo));
-          if (hi_b) best = fminf(best, lds_f32(sq_hi));
-          if (Epilogue) best = finish_value(best, bg, flags);             // a run has one label
-          *reinterpret_cast<float*>(dst) = best;
-          sq_lo += 4u; sq_hi -= 4u; dst += pitch;
-        }
-      }
-    }
-  }
-  if constexpr (Bits && !Epilogue) {
-    if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
-  }
+    // (kGrouped) the next tile's TMA and stage 0 overwrite the tile, the words and the chunk mask: every
+    // thread must be done with them
+  } while (kGrouped && next_group_tile(todo, phase));
 }
 
 // ---------------------------------------------------------------------------------------

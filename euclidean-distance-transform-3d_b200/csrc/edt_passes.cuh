@@ -309,7 +309,6 @@ int launch_later(const void* labels, const RunBits* bits, float* f, const LineGe
     // Programmatic dependent launch: this pass may begin (label staging) while the previous pass of
     // the stream drains its last wave; the kernel itself waits before touching the distances.
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)tiles);
     cfg.blockDim = dim3((unsigned)((warps > 32 ? 32 : warps) * 32));
     cfg.dynamicSmemBytes = tile_smem_bytes(g.n, p.tx, p.tma ? tb.box_rows * tb.nboxes : g.n);
     cfg.stream = stream;
@@ -335,6 +334,22 @@ int launch_later(const void* labels, const RunBits* bits, float* f, const LineGe
         : p.epilogue ? (p.tma ? tile_kernel<Bytes, true, true>(p) : tile_kernel<Bytes, true, false>(p))
                      : (p.tma ? tile_kernel<Bytes, false, true>(p) : tile_kernel<Bytes, false, false>(p));
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
+    // With `settled` armed, each CTA of the Bits kernel checks and runs a group of consecutive tiles:
+    // as many as make the grid three to four waves of resident CTAs (at most 32, one bit per tile), so
+    // that a pass which skips nearly every tile costs a few reads per SM and not one CTA per tile.
+    // Fewer, larger groups (two waves: 16 tiles at 512^3) skip no faster and serialise the tiles that
+    // run where they cluster, as the Z tiles of the X pass's band rows do (DESIGN.md section 4.1).
+    // Resident CTAs: the plan's CTAs per SM (p.ctas, what the kernel is compiled for), so that sizing
+    // the grid adds no runtime query to the launch.  EDTB200_SETTLED_GROUP forces the group size (A/B
+    // switch for measurements).
+    rb.group = 1;
+    if (p.settled) {
+      static const int forced_group = getenv("EDTB200_SETTLED_GROUP") ? atoi(getenv("EDTB200_SETTLED_GROUP")) : 0;
+      const int64_t waves4 = 4 * (int64_t)dc.sm_count * p.ctas;
+      const int64_t group = forced_group > 0 ? forced_group : (tiles + waves4 - 1) / waves4;
+      rb.group = (int)(group < 1 ? 1 : group > 32 ? 32 : group);
+    }
+    cfg.gridDim = dim3((unsigned)((tiles + rb.group - 1) / rb.group));
     CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, static_cast<const LT*>(labels), rb, f, g, tb, w2, border_lo,
                                 border_hi, flags, p.int_hull ? (int)w2 : 0));
     g_last_later = p;

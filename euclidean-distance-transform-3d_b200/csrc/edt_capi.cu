@@ -679,7 +679,8 @@ edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz, in
 // of scope.  They pay where the later passes only stream -- label noise (predicted from the previous
 // transform's run statistic, as the later passes' CTA count is) with labels of 4 or 8 bytes: there a
 // later pass moves 4 + 1/8 bytes per voxel instead of 8 or 12, for 1/4 byte more written by the X pass
-// (which stages its label rows in shared memory to compare neighbouring rows).  On narrower labels
+// (which stages its label rows in shared memory, bands of slices marching along y, to compare
+// neighbouring rows).  On narrower labels
 // and on structured volumes the dearer
 // X pass costs more than the later passes gain (DESIGN.md section 4.1), so none are taken there;
 // nor for signed transforms, whose last pass needs the labels' background bits as well.
@@ -697,7 +698,8 @@ int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const
                     int64_t count, DeviceCache& dc, cudaStream_t s) {
   const int64_t sx = t.n[0];
   if (t.ndim < 2 || t.label_bytes < 4 || (t.flags & EDTB200_SIGNED) || sx > 512 ||
-      !first_is_vec(labels, t.label_bytes, f, sx) || !label_noise_predicted(dc) || sz * count > 0x7fffffffLL)
+      !first_is_vec(labels, t.label_bytes, f, sx) || !label_noise_predicted(dc) || sz * count > 0x7fffffffLL ||
+      sy > 0x3fffffffLL)                // that X pass counts slices and rows in 32 bits
     return 0;
   bool tile = false;
   for (int k = 1; k < t.ndim; ++k)

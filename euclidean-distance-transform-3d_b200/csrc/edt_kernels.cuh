@@ -620,22 +620,26 @@ __device__ __forceinline__ void sts_f32(uint32_t addr, float v) {
 // First-axis pass that also writes the run-start planes (XPlanes), for rows of sx <= 128*K
 // voxels on which first_axis_vec_kernel runs, labels of 4 or 8 bytes.
 //
-// A CTA of W warps owns bands of W consecutive rows y0 .. y0+W-1 (warp w: row y0 + w).  A *stage*
-// is one band at one z together with its halo row y0 - 1 (none when y0 = 0): (W+1) rows that are
-// contiguous in memory, so one thread stages them with one 1-D bulk copy completed on an mbarrier.
-// The CTA walks a contiguous range of (band, z) items, z fastest, through a ring of S stages issued
-// S - 1 ahead, so that every label is read from HBM once: the y plane compares a row with its
-// stage's previous row, the z plane with the same row one stage back (the range's first item, if
-// z > 0, is preceded by one extra stage that is only compared against).  In 2-D every item is a
-// band of its own and the halo row is the previous band's last.  Items are split evenly over one
-// persistent wave of CTAs.
-// A voxel whose y-run is one row long (its label differs from rows y - 1 and y + 1, or the line ends
-// there) leaves the Y pass at exactly min(f, w2): the run's own sample and the border term w2 * 1^2 of
-// the label change or line end next to it, which a line of sy >= 2 rows always has on one side -- also
-// at rows 0 and sy - 1 without black_border.  The kernel stores that value already (ty = w2), so such
-// voxels end the X pass settled for the Y pass.  A band's last row does so only where it is the line's
-// last row: its row y + 1 is not staged, and the Y pass settles its runs (staging it as well, W+2 rows
-// per stage, was measured no faster on the 512^3 label-noise transform, DESIGN.md section 4.1).
+// The warps march along y.  In 3-D a CTA of W warps owns a band of W consecutive slices z0 .. z0+W-1
+// (warp w: slice z0 + w) and a chunk of rows ya .. yb.  A *stage* is one row y of every slice of the
+// band plus the halo row (y, z0 - 1): W + 1 rows of sx labels, one 1-D bulk copy each, completed on
+// the stage's mbarrier.  The z plane compares warp w's row with the stage's row of slice z0 + w - 1
+// (the halo for warp 0); a slice that starts a volume (vz = 0, also inside a band of a stack) has all
+// its z bits set, and a band that starts a volume loads no halo.  In 2-D the W warps take W
+// independent (image, y-chunk) sequences, and there is no halo.
+// Row y + 1 is the same warp's row in the next stage, so a stage is processed once it and its
+// successor have landed; the compare of row y - 1 with row y is the previous row's compare with its
+// successor, kept in a register.  Each chunk also stages the rows ya - 1 and yb + 1 (where they
+// exist), which are only compared with.  So every row sees rows y - 1 and y + 1, and a voxel whose
+// y-run is one row long (its label differs from rows y - 1 and y + 1, or the line ends there) gets
+// min(f, w2) here: that is exactly what the Y pass would leave, its own sample and the border term
+// w2 * 1^2 of the label change or line end next to it, which a line of sy >= 2 rows always has on one
+// side -- also at rows 0 and sy - 1 without black_border.  Such voxels end the X pass settled for the
+// Y pass (ty = w2).  Lines of one row have no border term and never take it.
+// The stages pass through a ring of S slots, issued S ahead: two are read while the other S - 2 load.
+// The (band, chunk) items are numbered band fastest and dealt out round robin over one persistent
+// wave, so the CTAs of neighbouring bands and the same chunk start together and march at one rate:
+// a halo row is staged by the band below at about the same time, and is expected to come from L2.
 //
 // Shared memory: S mbarriers (64 bytes), the ring of S stages of (W+1)*sx labels, the step table.
 // ---------------------------------------------------------------------------------------
@@ -660,6 +664,10 @@ __device__ __forceinline__ void load4_shared(const typename LabelOf<Bytes>::type
 }
 
 constexpr int kPlaneBarBytes = 64;     // room for the ring's mbarriers (S <= 8)
+// W slices per band, S stages in the ring.  Four stages of 9 rows of 512 4-byte labels (72 KB) leave
+// room for 3 CTAs per SM; three of 9 rows of 8-byte labels (108 KB) for 2.
+constexpr int kPlaneWarps = 8;
+__host__ __device__ constexpr int planes_stages(int label_bytes) { return label_bytes == 8 ? 3 : 4; }
 
 // Labels a[0..3] against b[0..3]: bit e set where they differ.
 template <class WT>
@@ -667,59 +675,102 @@ __device__ __forceinline__ uint32_t label_changes(const WT a[4], const WT b[4]) 
   return (a[0] != b[0] ? 1u : 0u) | (a[1] != b[1] ? 2u : 0u) | (a[2] != b[2] ? 4u : 0u) | (a[3] != b[3] ? 8u : 0u);
 }
 
-// Planes: 1 the y plane, 2 the y and z planes.  The ring's depth S is `stages`; W is blockDim.x / 32.
-// Registers capped at the CTAs per SM that the ring leaves room for with 8 warps, 3 stages and 512-voxel
-// rows: 3 for 4-byte labels (57 KB), 2 for 8-byte ones (110 KB).
+// One row source of the march: row source r of item j (0: the halo, 1 + w: warp w's slice) is slice z,
+// rows ya .. yb; ok = false: none.  Planes: 2 in 3-D (items are (band, chunk), band fastest), 1 in 2-D
+// (warp w of item j takes the (image, chunk) sequence j * W + w, chunk fastest).  Slices and rows are
+// counted in 32 bits (take_run_planes), lines and voxels in 64.
+struct MarchSource {
+  int z, ya, yb;
+  bool ok;
+};
+template <int W, int Planes>
+__device__ __forceinline__ MarchSource march_source(int64_t j, int r, int nz, int sy, int depth, int nchunks) {
+  MarchSource m;
+  int k;
+  if constexpr (Planes == 2) {
+    const int nbands = (nz + W - 1) / W, z0 = (int)(j % nbands) * W;
+    k = (int)(j / nbands);
+    m.z = z0 + r - 1;
+    m.ok = r == 0 ? (z0 % depth) != 0 : m.z < nz;
+  } else {
+    const int64_t q = j * W + r - 1;
+    m.z = (int)(q / nchunks);
+    k = (int)(q - (int64_t)m.z * nchunks);
+    m.ok = r > 0 && m.z < nz;
+  }
+  m.ya = (int)((int64_t)k * sy / nchunks);
+  m.yb = (int)((int64_t)(k + 1) * sy / nchunks) - 1;
+  return m;
+}
+
+// Items of the march over nz slices in nchunks y-chunks each (see march_source).
+template <int W, int Planes>
+__host__ __device__ __forceinline__ int64_t march_items(int64_t nz, int64_t nchunks) {
+  return Planes == 2 ? (nz + W - 1) / W * nchunks : (nz * nchunks + W - 1) / W;
+}
+
+// Planes: 1 the y plane, 2 the y and z planes.  nchunks: y-chunks per slice (launch_first_vec).
+// Registers capped at the CTAs per SM that the ring leaves room for: 3 for 4-byte labels, 2 for 8-byte ones.
 template <int Bytes, int K, bool Plain, int Planes>
-__global__ void __launch_bounds__(256, Bytes == 8 ? 2 : 3)
+__global__ void __launch_bounds__(32 * kPlaneWarps, Bytes == 8 ? 2 : 3)
 first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
                          float* __restrict__ out, int64_t nlines, int sx,
                          const float* __restrict__ table, int border, int flags, RunStat stat, XPlanes planes,
-                         int stages) {
+                         int nchunks) {
   static_assert(Bytes >= 4 && Planes >= 1 && Planes <= 2, "the bulk copies need 16-byte label rows");
   using LT = typename LabelOf<Bytes>::type;
   using WT = typename LabelOf<Bytes>::wide;
+  constexpr int W = kPlaneWarps, S = planes_stages(Bytes);
   extern __shared__ __align__(16) unsigned char planes_smem[];
   pdl_launch_dependents();                           // the second-axis pass may start staging labels
 
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
-  const int warps = blockDim.x >> 5;
-  const int64_t sy = planes.sy, nz = nlines / sy;
-  const int64_t nbands = (sy + warps - 1) / warps;
-  const size_t row_bytes = (size_t)sx * Bytes;
-  const size_t stage_bytes = (size_t)(warps + 1) * row_bytes;
+  const int sy = (int)planes.sy, nz = (int)(nlines / planes.sy), depth = (int)planes.depth;
+  const unsigned row_bytes = (unsigned)sx * Bytes;
+  const int stage_labels = (W + 1) * sx;
   uint64_t* bar = reinterpret_cast<uint64_t*>(planes_smem);
   LT* ring = reinterpret_cast<LT*>(planes_smem + kPlaneBarBytes);
-  float* table_s = reinterpret_cast<float*>(planes_smem + kPlaneBarBytes + stages * stage_bytes);
+  float* table_s = reinterpret_cast<float*>(planes_smem + kPlaneBarBytes + (size_t)S * stage_labels * Bytes);
 
-  // this CTA's items [j0, j1); stage i holds item first + i, and stage 0 only serves as the z
-  // neighbour of stage 1 when it is the extra one (pro = 1)
-  const int64_t items = nbands * nz;
-  const int64_t j0 = items * blockIdx.x / gridDim.x, j1 = items * (blockIdx.x + 1) / gridDim.x;
-  const int pro = (Planes == 2 && j0 < j1 && j0 % nz != 0) ? 1 : 0;
-  const int64_t first = j0 - pro, count = j1 - first;
-  int band = (int)(first / nz), z = (int)(first - band * nz);     // item of stage i, advanced per stage
-  int vz = (int)(z % planes.depth);                  // z within its volume, advanced with z
-  // thread 0: the next stage to issue, its item and its slot
-  int64_t issued = 0;
-  int issue_band = band, issue_z = z, issue_slot = 0;
-  auto issue_next = [&]() {
-    const int64_t y0 = (int64_t)issue_band * warps;
-    const int halo = y0 > 0 ? 1 : 0;
-    const unsigned bytes = (unsigned)((halo + min((int64_t)warps, sy - y0)) * row_bytes);
-    uint64_t* b = bar + issue_slot;
-    mbar_expect_tx(b, bytes);
-    bulk_load(reinterpret_cast<unsigned char*>(ring) + issue_slot * stage_bytes + (1 - halo) * row_bytes,
-              labels + ((int64_t)issue_z * sy + y0 - halo) * sx, bytes, b);
-    if (++issue_z == nz) { issue_z = 0; ++issue_band; }
-    if (++issue_slot == stages) issue_slot = 0;
-    ++issued;
+  // this CTA's items blockIdx.x + n * gridDim.x; every item takes nst stages (the longest chunk, its
+  // leading and trailing rows), stage i holding row ya - 1 + i of each source
+  const int64_t items = march_items<W, Planes>(nz, nchunks);
+  const int nst = (sy + nchunks - 1) / nchunks + 2;
+  // warp 0: the item and stage to issue next; lane r <= W: row source r's next row (src_y, at src_row)
+  // and the last row it stages (-1: none)
+  int64_t issue_j = blockIdx.x;
+  int issue_i = 0, issue_slot = 0, src_y = 0, src_last = -1;
+  const LT* src_row = labels;
+  auto issue_source = [&]() {
+    const MarchSource m = march_source<W, Planes>(issue_j, lane, nz, sy, depth, nchunks);
+    src_y = m.ya - 1;
+    src_last = m.ok && lane <= W ? min(m.yb + 1, sy - 1) : -1;
+    src_row = labels + ((int64_t)m.z * sy + src_y) * sx;
   };
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < stages; ++s) mbar_init(bar + s, 1);
-    while (issued < stages - 1 && issued < count) issue_next();
+  auto issue_next = [&]() {
+    const bool load = src_y >= 0 && src_y <= src_last;
+    const unsigned rows = __ballot_sync(full, load);
+    uint64_t* b = bar + issue_slot;
+    if (lane == 0) mbar_expect_tx(b, __popc(rows) * row_bytes);
+    __syncwarp();
+    if (load) bulk_load(ring + issue_slot * stage_labels + lane * sx, src_row, row_bytes, b);
+    ++src_y;
+    src_row += sx;
+    if (++issue_slot == S) issue_slot = 0;
+    if (++issue_i == nst) {
+      issue_i = 0;
+      issue_j += gridDim.x;
+      issue_source();
+    }
+  };
+  if (threadIdx.x == 0)
+    for (int s = 0; s < S; ++s) mbar_init(bar + s, 1);
+  __syncwarp();
+  if (warp == 0) {
+    issue_source();
+    for (int s = 0; s < S && issue_j < items; ++s) issue_next();
   }
   for (int i = threadIdx.x; i <= sx; i += blockDim.x) table_s[i] = __ldg(table + i);
   if (threadIdx.x == 0) table_s[sx + 1] = __int_as_float(0x7f800000);
@@ -728,97 +779,110 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
   const unsigned lt_mask = (1u << lane) - 1u;
   const unsigned gt_mask = (lane == 31) ? 0u : (0xfffffffeu << lane);
   const bool keep_background = Plain ? false : (flags & kZeroLabel) != 0;
-  const int64_t wpr = (sx + 31) >> 5;
+  const int wpr = (sx + 31) >> 5;
+  uint32_t in_row = 0u;                              // the nibbles of the lane's voxels inside the row
+#pragma unroll
+  for (int b = 0; b < K; ++b)
+    if ((b << 7) + (lane << 2) < sx) in_row |= 15u << (4 * b);
   unsigned int nstarts = 0;                          // label changes along x seen by this lane
 
-  int slot = 0, prev_slot = stages - 1;
-  unsigned phase = 0;
-  for (int64_t i = 0; i < count; ++i) {
+  int slot = 0;                                      // the slot and phase parity of the item's stage i
+  unsigned phase = 0u;
+  for (int64_t j = blockIdx.x; j < items; j += gridDim.x) {
+    const MarchSource me = march_source<W, Planes>(j, warp + 1, nz, sy, depth, nchunks);
+    const bool zfirst = Planes == 2 && me.z % depth == 0;       // the warp's slice starts a volume
+    const int ylast = me.ok ? me.yb : -2;                       // the last row it processes
+    uint32_t ystart = 0u;                            // y-runs that start at row y (the previous ynext)
     mbar_wait(bar + slot, phase);
-    const int64_t y = (int64_t)band * warps + warp;
-    if (i >= pro && y < sy) {
-      const int64_t line = z * sy + y;
-      // this row is row warp + 1 of its stage (row 0: the halo row y - 1)
-      const LT* cur = ring + (size_t)slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
-      const LT* back = ring + (size_t)prev_slot * (stage_bytes / Bytes) + (size_t)(warp + 1) * sx;
-      // ---- the row against rows y - 1 and y + 1, 4 bits per block: a y-run starts here (the y
-      // plane's bits) / at the next row (the line end counts); both: a y-run of one row.  Row y + 1
-      // is in the stage except for the band's last row ----
-      const bool next_staged = y + 1 < sy && warp + 1 < warps;
-      uint32_t ystart = 0u, ynext = 0u;
+    for (int i = 0; i < nst; ++i) {
+      const int next_slot = slot + 1 == S ? 0 : slot + 1;
+      const unsigned next_phase = next_slot == 0 ? phase ^ 1u : phase;
+      const int y = me.ya - 1 + i;
+      if (i + 1 < nst) {
+        mbar_wait(bar + next_slot, next_phase);
+        if (y <= ylast) {
+          const LT* cur = ring + slot * stage_labels + (warp + 1) * sx;
+          const LT* next = ring + next_slot * stage_labels + (warp + 1) * sx;
+          // ---- y-runs that start at row y + 1, 4 bits per block (the line end counts; row -1 stands
+          // for the line's start, so row 0 gets all bits) ----
+          uint32_t ynext = in_row;
+          if (y >= 0 && y + 1 < sy) {
+            ynext = 0u;
 #pragma unroll
-      for (int b = 0; b < K; ++b) {
-        const int q0 = (b << 7) + (lane << 2);
-        if (q0 >= sx) continue;
-        WT here[4], u[4];
-        load4_shared<Bytes>(cur + q0, here);
-        uint32_t s = 15u, e = (y + 1 == sy) ? 15u : 0u;            // first row along y: all start
-        if (y > 0) { load4_shared<Bytes>(cur - sx + q0, u); s = label_changes<WT>(u, here); }
-        if (next_staged) { load4_shared<Bytes>(cur + sx + q0, u); e = label_changes<WT>(u, here); }
-        ystart |= s << (4 * b);
-        ynext |= e << (4 * b);
-      }
-      const uint32_t one_row = sy > 1 ? (ystart & ynext) : 0u;     // lines of one row have no border term
-      uint32_t set_y = 0xffffffffu, set_z = 0xffffffffu;
-      first_axis_vec_row<Bytes, K, Plain, true, true>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); },
-                                                      out + line * sx, sx, table_s, border, flags, keep_background,
-                                                      lane, lt_mask, gt_mask, nstarts, planes.ty, planes.tz, &set_y,
-                                                      &set_z, one_row);
-      // ---- settled planes: segment 4 b + w of the row is lanes 8 w .. 8 w + 7 of block b ----
-      uint32_t seg_y = 0u, seg_z = 0u;
-#pragma unroll
-      for (int b = 0; b < K; ++b) {
-        uint32_t v = __ballot_sync(full, (set_y >> b) & 1u);
-        v &= v >> 4; v &= v >> 2; v &= v >> 1;               // bit 8 w: all of lanes 8 w .. 8 w + 7
-        seg_y |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
-        if (Planes == 2) {
-          v = __ballot_sync(full, (set_z >> b) & 1u);
-          v &= v >> 4; v &= v >> 2; v &= v >> 1;
-          seg_z |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
-        }
-      }
-      if (lane == 0) {
-        planes.settled_y[line] = seg_y | (0xffffffffu << (4 * K));
-        if (Planes == 2) planes.settled_z[line] = seg_z | (0xffffffffu << (4 * K));
-      }
-      // ---- run-start planes: the y nibbles from above, the z ones compare with row (y, z - 1); one
-      // nibble per lane and block -> the row's wpr words, word c in lane c, stored by one instruction
-      // per plane ----
-      uint32_t word[Planes] = {};
-#pragma unroll
-      for (int b = 0; b < K; ++b) {
-        const int q0 = (b << 7) + (lane << 2);
-        const bool in_row = q0 < sx;
-        uint32_t nibs[Planes];
-        nibs[0] = (ystart >> (4 * b)) & 15u;
-        if (Planes == 2) {
-          nibs[Planes - 1] = in_row ? 15u : 0u;                   // first slice of a volume: all start
-          if (in_row && vz != 0) {
-            WT here[4], u[4];
-            load4_shared<Bytes>(cur + q0, here);
-            load4_shared<Bytes>(back + q0, u);
-            nibs[Planes - 1] = label_changes<WT>(u, here);
+            for (int b = 0; b < K; ++b) {
+              const int q0 = (b << 7) + (lane << 2);
+              if (q0 >= sx) continue;
+              WT here[4], u[4];
+              load4_shared<Bytes>(cur + q0, here);
+              load4_shared<Bytes>(next + q0, u);
+              ynext |= label_changes<WT>(here, u) << (4 * b);
+            }
           }
-        }
+          if (y >= me.ya) {                          // not the leading row: this row's outputs
+            const int64_t line = (int64_t)me.z * sy + y;
+            const uint32_t one_row = sy > 1 ? (ystart & ynext) : 0u;   // lines of one row have no border term
+            uint32_t set_y = 0xffffffffu, set_z = 0xffffffffu;
+            first_axis_vec_row<Bytes, K, Plain, true, true>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); },
+                                                            out + line * sx, sx, table_s, border, flags,
+                                                            keep_background, lane, lt_mask, gt_mask, nstarts,
+                                                            planes.ty, planes.tz, &set_y, &set_z, one_row);
+            // ---- settled planes: segment 4 b + w of the row is lanes 8 w .. 8 w + 7 of block b ----
+            uint32_t seg_y = 0u, seg_z = 0u;
 #pragma unroll
-        for (int a = 0; a < Planes; ++a) {
-          const uint32_t nib = nibs[a];
-          // word w of block b sits in lanes 8w .. 8w + 7; lane c takes word c = 4 b + w
-          const uint32_t got = __shfl_sync(full, nibbles_to_word(nib, lane), (lane & 3) << 3);
-          if ((lane >> 2) == b) word[a] = got;
+            for (int b = 0; b < K; ++b) {
+              uint32_t v = __ballot_sync(full, (set_y >> b) & 1u);
+              v &= v >> 4; v &= v >> 2; v &= v >> 1;             // bit 8 w: all of lanes 8 w .. 8 w + 7
+              seg_y |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
+              if (Planes == 2) {
+                v = __ballot_sync(full, (set_z >> b) & 1u);
+                v &= v >> 4; v &= v >> 2; v &= v >> 1;
+                seg_z |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
+              }
+            }
+            if (lane == 0) {
+              planes.settled_y[line] = seg_y | (0xffffffffu << (4 * K));
+              if (Planes == 2) planes.settled_z[line] = seg_z | (0xffffffffu << (4 * K));
+            }
+            // ---- run-start planes: the y nibbles from ystart, the z ones compare with the stage's row
+            // of slice z - 1; one nibble per lane and block -> the row's wpr words, word c in lane c,
+            // stored by one instruction per plane ----
+            const LT* below = cur - sx;
+            uint32_t word[Planes] = {};
+#pragma unroll
+            for (int b = 0; b < K; ++b) {
+              const int q0 = (b << 7) + (lane << 2);
+              uint32_t nibs[Planes];
+              nibs[0] = (ystart >> (4 * b)) & 15u;
+              if (Planes == 2) {
+                nibs[Planes - 1] = (in_row >> (4 * b)) & 15u;     // first slice of a volume: all start
+                if (q0 < sx && !zfirst) {
+                  WT here[4], u[4];
+                  load4_shared<Bytes>(cur + q0, here);
+                  load4_shared<Bytes>(below + q0, u);
+                  nibs[Planes - 1] = label_changes<WT>(u, here);
+                }
+              }
+#pragma unroll
+              for (int a = 0; a < Planes; ++a) {
+                const uint32_t nib = nibs[a];
+                // word w of block b sits in lanes 8w .. 8w + 7; lane c takes word c = 4 b + w
+                const uint32_t got = __shfl_sync(full, nibbles_to_word(nib, lane), (lane & 3) << 3);
+                if ((lane >> 2) == b) word[a] = got;
+              }
+            }
+            if (lane < wpr) {
+              planes.y[line * wpr + lane] = word[0];
+              if (Planes == 2) planes.z[line * wpr + lane] = word[Planes - 1];
+            }
+          }
+          ystart = ynext;
         }
       }
-      if (lane < wpr) {
-        planes.y[line * wpr + lane] = word[0];
-        if (Planes == 2) planes.z[line * wpr + lane] = word[Planes - 1];
-      }
+      __syncthreads();                               // stage i is read by no one any more
+      if (warp == 0 && issue_j < items) issue_next();    // the stage S later, into its slot
+      slot = next_slot;
+      phase = next_phase;
     }
-    __syncthreads();                                 // stage i - 1 is read by no one any more
-    if (threadIdx.x == 0 && issued < count) issue_next();   // stage i + S - 1, into the slot of i - 1
-    prev_slot = slot;
-    if (++slot == stages) { slot = 0; phase ^= 1u; }
-    if (++vz == planes.depth) vz = 0;                // nz is a whole number of volumes: wraps with z
-    if (++z == nz) { z = 0; ++band; }
   }
   if (stat.counter) {
 #pragma unroll

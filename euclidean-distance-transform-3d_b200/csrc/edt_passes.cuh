@@ -9,6 +9,7 @@
 #include "edt_host.h"
 #include "edt_feature.cuh"
 
+#include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <cstdlib>
@@ -43,9 +44,9 @@ int launch_first_generic(const void* labels, float* f, int* codes, int64_t nline
   return 0;
 }
 
-// Shared memory of first_axis_planes_kernel with `warps` rows per band and a ring of `stages`.
-inline size_t planes_smem_bytes(int64_t sx, int label_bytes, int warps, int stages) {
-  return kPlaneBarBytes + (size_t)stages * (size_t)(warps + 1) * (size_t)sx * label_bytes +
+// Shared memory of first_axis_planes_kernel: its ring of stages of W + 1 rows, the step table.
+inline size_t planes_smem_bytes(int64_t sx, int label_bytes) {
+  return kPlaneBarBytes + (size_t)planes_stages(label_bytes) * (size_t)(kPlaneWarps + 1) * (size_t)sx * label_bytes +
          sizeof(float) * (size_t)(sx + 2);
 }
 
@@ -68,31 +69,29 @@ int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, c
     return 0;
   }
   if constexpr (Bytes >= 4 && K <= 4) {
-    // Bands of 8 rows through a ring of 3 stages: 57 KB for 512-voxel rows of 4-byte labels, so
-    // three CTAs per SM, each with one to two stages (18 KB) of labels in flight.  Measured on the
-    // 512^3 label-noise transform, 6 or 4 rows per band and rings of 4 or 6 stages were slower.
-    // Fewer rows per band where the ring does not fit (it always does for rows of at most 512 voxels).
-    // A stage holds no row after its band, so the band's last row leaves its y-runs of one row to the
-    // Y pass (about 6 % of its label-noise tiles then still run).  Staging that row too (62 KB, still
-    // three CTAs per SM for 4-byte labels; one for 8-byte ones) settled them all but made the X pass as
-    // much slower as it made the Y pass faster (DESIGN.md section 4.1).
-    int warps = 8;
-    const int stages = 3;
-    while (warps > 1 && planes_smem_bytes(sx, Bytes, warps, stages) > (size_t)dc.max_smem_optin) warps >>= 1;
-    const size_t smem = planes_smem_bytes(sx, Bytes, warps, stages);
+    // Bands of 8 slices that march along y through a ring of stages of 9 rows: 4 stages (74 KB) for
+    // 512-voxel rows of 4-byte labels, so three CTAs per SM, each reading two stages with two more
+    // (36 KB) in flight; 3 stages (110 KB) for 8-byte ones, two CTAs per SM, one stage in flight.
+    constexpr int W = kPlaneWarps;
+    const size_t smem = planes_smem_bytes(sx, Bytes);
     if (smem > (size_t)dc.max_smem_optin)
       return fail(EDTB200_ELIMIT, "run-start planes of %lld-voxel rows exceed the shared memory", (long long)sx);
-    auto kern = planes->z ? first_axis_planes_kernel<Bytes, K, Plain, 2> : first_axis_planes_kernel<Bytes, K, Plain, 1>;
+    const bool z = planes->z != nullptr;
+    auto kern = z ? first_axis_planes_kernel<Bytes, K, Plain, 2> : first_axis_planes_kernel<Bytes, K, Plain, 1>;
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, warps * 32, smem));
-    // one persistent wave, the (band, z) items split evenly over it
-    const int64_t items = (planes->sy + warps - 1) / warps * (nlines / planes->sy);
-    int64_t blocks = (int64_t)dc.sm_count * (per_sm > 0 ? per_sm : 1);
-    if (blocks > items) blocks = items;
-    if (blocks < 1) blocks = 1;
-    kern<<<(unsigned)blocks, warps * 32, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table,
-                                                         border, flags, stat, *planes, stages);
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, W * 32, smem));
+    // One persistent wave.  The slices are cut into y-chunks so that the items -- (band, chunk) in 3-D,
+    // W (image, chunk) sequences in 2-D -- fill the wave without a second one, but into no chunk shorter
+    // than 67 rows, so that each chunk's leading and trailing rows, read once more, stay within 3 % of
+    // its labels.
+    const int64_t sy = planes->sy, nz = nlines / sy, wave = (int64_t)dc.sm_count * (per_sm > 0 ? per_sm : 1);
+    const int64_t fill = z ? wave / ((nz + W - 1) / W) : wave * W / nz;
+    const int64_t nchunks = std::max<int64_t>(1, std::min(fill, sy * 3 / 200));
+    const int64_t items = z ? march_items<W, 2>(nz, nchunks) : march_items<W, 1>(nz, nchunks);
+    const int64_t blocks = std::max<int64_t>(1, std::min(wave, items));
+    kern<<<(unsigned)blocks, W * 32, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table, border,
+                                                     flags, stat, *planes, (int)nchunks);
     CUDA_TRY(cudaGetLastError());
     return 0;
   }

@@ -561,9 +561,9 @@ int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines
 
 int dispatch_later(int label_bytes, const void* labels, float* f, const edtb200::LineGeom& g, float w,
                    int lo, int hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t s, bool pdl,
-                   const edtb200::RunBits* bits = nullptr) {
+                   const LaterNoise* planned = nullptr) {
   return with_label_width(label_bytes, [&](auto b) {
-    return launch_later<b>(labels, bits, f, g, w, lo, hi, flags, arith, dc, s, pdl);
+    return launch_later<b>(labels, planned, f, g, w, lo, hi, flags, arith, dc, s, pdl);
   });
 }
 
@@ -655,60 +655,29 @@ struct HostIO {
   std::unique_lock<std::mutex> lock_;
 };
 
-// Kernel flags of a pass from the ABI flags: sqrt and sign act in the store of the last pass;
-// background-as-label (sdf) changes the first pass only -- later passes treat every run alike.
-int kernel_flags(int flags, bool first, bool last) {
-  const int epilogue = ((flags & EDTB200_SQRT) ? edtb200::kSqrt : 0) | ((flags & EDTB200_SIGNED) ? edtb200::kNegate : 0);
-  return (last ? epilogue : 0) | (first && (flags & EDTB200_SIGNED) ? edtb200::kZeroLabel : 0);
-}
-
-// One transform: each of its passes derives its kernel flags and arithmetic from these.  w and n
-// are the weights and extents of the whole volume, whatever part of it a pass covers.
-struct Transform {
-  int label_bytes, ndim, flags, border;
-  float w[3];
-  int64_t n[3];
-};
-
-// The lines of the later pass along `axis` over `count` volumes of (sx, sy, sz) laid end to end: the
-// outer dimension walks the volumes, so that no line crosses from one volume into the next.
-edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz, int64_t count = 1);
-
-// The run-start planes that the X pass of one transform writes for its later passes (XPlanes): one
-// bit per voxel and later axis, stream-ordered scratch freed on the stream when the owner goes out
-// of scope.  They pay where the later passes only stream -- label noise (predicted from the previous
-// transform's run statistic, as the later passes' CTA count is) with labels of 4 or 8 bytes: there a
-// later pass moves 4 + 1/8 bytes per voxel instead of 8 or 12, for 1/4 byte more written by the X pass
-// (which stages its label rows in shared memory, bands of slices marching along y, to compare
-// neighbouring rows).  On narrower labels
-// and on structured volumes the dearer
-// X pass costs more than the later passes gain (DESIGN.md section 4.1), so none are taken there;
-// nor for signed transforms, whose last pass needs the labels' background bits as well.
+// The label-noise plan of one transform (noise_plan) and the run-start planes that its X pass writes for
+// its later passes (XPlanes): one bit per voxel and later axis, stream-ordered scratch freed on the
+// stream when the owner goes out of scope.
 struct RunPlanes {
   Scratch mem;
   edtb200::XPlanes x{};             // x.y null: none
-  edtb200::RunBits bits[3] = {};    // the later pass along axis k reads bits[k] (start null: none)
+  LaterNoise later[3];              // the later pass along axis k as planned (bits.start null: no plane)
   const edtb200::XPlanes* for_x() const { return x.y ? &x : nullptr; }
-  const edtb200::RunBits* for_axis(int k) const { return bits[k].start ? &bits[k] : nullptr; }
 };
 
-// Takes the planes for transform t over `count` volumes (t.n[0], sy, sz) laid end to end at labels / f
-// where they pay; taking none costs nothing (the later passes then read the labels).
+// Plans transform t over `count` volumes (t.n[0], sy, sz) laid end to end at labels / f, and takes the
+// planes the plan asks for; where there is no room for them the later passes read the labels.
 int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const float* f, int64_t sy, int64_t sz,
                     int64_t count, DeviceCache& dc, cudaStream_t s) {
-  const int64_t sx = t.n[0];
-  if (t.ndim < 2 || t.label_bytes < 4 || (t.flags & EDTB200_SIGNED) || sx > 512 ||
-      !first_is_vec(labels, t.label_bytes, f, sx) || !label_noise_predicted(dc) || sz * count > 0x7fffffffLL ||
-      sy > 0x3fffffffLL)                // that X pass counts slices and rows in 32 bits
-    return 0;
-  bool tile = false;
-  for (int k = 1; k < t.ndim; ++k)
-    tile = tile ||
-           !later_pass_is_long(geom_for_axis(k, sx, sy, sz, count), transform_arith(t.w, t.n, k), dc.max_smem_optin);
-  if (!tile) return 0;
+  const NoisePlan np = noise_plan(t, count, labels, f, dc);
+  for (int k = 1; k < 3; ++k) {
+    rp.later[k].noise = np.noise;
+    rp.later[k].plan = np.later[k];
+  }
+  if (!np.planes) return 0;
   // per later axis: the run-start plane (wpr words per row), then the settled plane (one word per row)
-  const int64_t wpr = (sx + 31) >> 5, rows = sy * sz * count, words = rows * wpr;
-  if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)(words + rows) * (size_t)(t.ndim - 1), s) != cudaSuccess) {
+  const int64_t sx = t.n[0], wpr = (sx + 31) >> 5, rows = sy * sz * count, words = rows * wpr;
+  if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)(words + rows) * (size_t)np.planes, s) != cudaSuccess) {
     cudaGetLastError();
     return 0;                        // no room: the later passes read the labels
   }
@@ -717,22 +686,20 @@ int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const
   rp.x.depth = sz;
   rp.x.y = p;
   rp.x.settled_y = p + words;
-  rp.x.z = t.ndim == 3 ? p + words + rows : nullptr;
-  rp.x.settled_z = t.ndim == 3 ? p + 2 * words + rows : nullptr;
+  rp.x.z = np.planes == 2 ? p + words + rows : nullptr;
+  rp.x.settled_z = np.planes == 2 ? p + 2 * words + rows : nullptr;
   rp.x.ty = t.w[1] * t.w[1];         // the float products the later passes compare with (launch_later)
-  rp.x.tz = t.ndim == 3 ? t.w[2] * t.w[2] : 0.0f;
+  rp.x.tz = np.planes == 2 ? t.w[2] * t.w[2] : 0.0f;
   // Y pass: outer = z (of every volume), inner = x; Z pass: outer = volume, inner = y * sx + x, rows
   // sy * wpr words apart.  Settled words: Y pass at z * sy + y, Z pass at volume * sz * sy + z * sy + y.
-  rp.bits[1] = edtb200::RunBits{rp.x.y, wpr, sy * wpr, sx, wpr, rp.x.settled_y, 1, sy, nullptr, 0.0f};
-  if (t.ndim == 3) {
-    rp.bits[2] = edtb200::RunBits{rp.x.z, sy * wpr, sz * sy * wpr, sx, wpr, rp.x.settled_z, sy, sz * sy, nullptr, 0.0f};
-    // the Y pass refreshes the Z pass's settled plane only where the Z pass may skip tiles (no
-    // epilogue, integer hull: see launch_later)
-    if (kernel_flags(t.flags, false, true) == 0 && transform_arith(t.w, t.n, 2).int_hull) {
-      rp.bits[1].refresh = rp.x.settled_z;
-      rp.bits[1].refresh_t = rp.x.tz;
-    }
-  }
+  if (np.reads[1])
+    rp.later[1].bits = edtb200::RunBits{rp.x.y, wpr, sy * wpr, sx, wpr, np.later[1].settled ? rp.x.settled_y : nullptr,
+                                        1, sy, np.refresh ? rp.x.settled_z : nullptr, np.refresh ? rp.x.tz : 0.0f,
+                                        np.group[1]};
+  if (np.reads[2])
+    rp.later[2].bits = edtb200::RunBits{rp.x.z, sy * wpr, sz * sy * wpr, sx, wpr,
+                                        np.later[2].settled ? rp.x.settled_z : nullptr, sy, sz * sy, nullptr, 0.0f,
+                                        np.group[2]};
   return 0;
 }
 
@@ -748,7 +715,7 @@ int x_pass(const Transform& t, const void* labels, float* f, int64_t nlines, Dev
 int later_pass(const Transform& t, int k, const void* labels, float* f, const edtb200::LineGeom& g, int lo, int hi,
                DeviceCache& dc, cudaStream_t s, bool pdl, const RunPlanes* planes = nullptr) {
   return dispatch_later(t.label_bytes, labels, f, g, t.w[k], lo, hi, kernel_flags(t.flags, false, k == t.ndim - 1),
-                        transform_arith(t.w, t.n, k), dc, s, pdl, planes ? planes->for_axis(k) : nullptr);
+                        transform_arith(t.w, t.n, k), dc, s, pdl, planes ? &planes->later[k] : nullptr);
 }
 
 // Largest finite |f| (as float bits: non-negative floats order like their bits) and the exponent
@@ -773,18 +740,6 @@ __global__ void __launch_bounds__(256) sample_range_kernel(const float* __restri
     atomicMax(reinterpret_cast<unsigned int*>(range), hi);
     atomicMin(range + 1, low);
   }
-}
-
-edtb200::LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz, int64_t count) {
-  edtb200::LineGeom g;
-  if (axis == 1) {
-    g.outer_count = sz * count; g.outer_stride = sx * sy; g.inner_count = sx; g.line_stride = sx; g.n = (int)sy;
-  } else {
-    g.outer_count = count; g.outer_stride = count > 1 ? sx * sy * sz : 0; g.inner_count = sx * sy;
-    g.line_stride = sx * sy; g.n = (int)sz;
-  }
-  g.tiles_per_outer = 0;
-  return g;
 }
 
 // Optional per-pass timing for bench.py: with profiling on, every transform of this thread records
@@ -894,9 +849,9 @@ int run_passes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_
   // in the stream is our own previous pass, which never writes the labels, so their label staging
   // (before griddepcontrol.wait) may overlap its tail.  The per-axis entry points do not do this:
   // there the previous kernel is the caller's and may be the one producing the labels.
-  // On predicted label noise with wide labels the X pass also writes run-start bit planes, and the
-  // later passes read those instead of the labels (RunPlanes); a later pass reads its plane only
-  // after griddepcontrol.wait.
+  // Every pass plans with one reading of the noise prediction (RunPlanes).  On predicted label noise
+  // with wide labels the X pass also writes run-start bit planes, and the later passes read those
+  // instead of the labels; a later pass reads its plane only after griddepcontrol.wait.
   RunPlanes planes;
   int rc = take_run_planes(planes, t, labels, f, sy, sz, count, dc, stream);
   if (rc) return rc;

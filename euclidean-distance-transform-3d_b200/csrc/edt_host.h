@@ -180,6 +180,35 @@ PassArith transform_arith(const float* w, const int64_t* n, int k);
 // lowest set bit over the finite non-zero samples is 2^low (1024: there is none).
 PassArith sampled_arith(float fmax, int low, float w, int64_t n);
 
+// One transform: each of its passes derives its kernel flags and arithmetic from these.  w and n
+// are the weights and extents of the whole volume, whatever part of it a pass covers.
+struct Transform {
+  int label_bytes, ndim, flags, border;
+  float w[3];
+  int64_t n[3];
+};
+
+// Kernel flags of a pass from the ABI flags: sqrt and sign act in the store of the last pass;
+// background-as-label (sdf) changes the first pass only -- later passes treat every run alike.
+inline int kernel_flags(int flags, bool first, bool last) {
+  const int epilogue = ((flags & EDTB200_SQRT) ? kSqrt : 0) | ((flags & EDTB200_SIGNED) ? kNegate : 0);
+  return (last ? epilogue : 0) | (first && (flags & EDTB200_SIGNED) ? kZeroLabel : 0);
+}
+
+// The lines of the later pass along `axis` over `count` volumes of (sx, sy, sz) laid end to end: the
+// outer dimension walks the volumes, so that no line crosses from one volume into the next.
+inline LineGeom geom_for_axis(int axis, int64_t sx, int64_t sy, int64_t sz, int64_t count = 1) {
+  LineGeom g;
+  if (axis == 1) {
+    g.outer_count = sz * count; g.outer_stride = sx * sy; g.inner_count = sx; g.line_stride = sx; g.n = (int)sy;
+  } else {
+    g.outer_count = count; g.outer_stride = count > 1 ? sx * sy * sz : 0; g.inner_count = sx * sy;
+    g.line_stride = sx * sy; g.n = (int)sz;
+  }
+  g.tiles_per_outer = 0;
+  return g;
+}
+
 // Whether launch_first runs the register-resident X kernels (rows of at most 1024 voxels, a multiple
 // of 4, labels and distances aligned for vector access) -- the only ones that write XPlanes.
 inline bool first_is_vec(const void* labels, int label_bytes, const float* f, int64_t sx) {
@@ -188,18 +217,17 @@ inline bool first_is_vec(const void* labels, int label_bytes, const float* f, in
 }
 
 // Axis-pass launchers, one instantiation per label width (edt_passes.cuh).  planes: the run-start
-// planes the X pass writes (null: none; only for labels of 4 or 8 bytes and rows of at most 512
-// voxels where first_is_vec holds).
-// bits: the later pass's run-start plane from such an X pass (null: none); it is read only where the
-// pass takes the label-noise tile kernel, otherwise the labels are.
+// planes the X pass writes (null: none), where noise_plan takes them.
+// planned: what noise_plan planned for the later pass (null: it reads the noise prediction at launch
+// and no plane).
+struct LaterNoise;
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
                  const XPlanes* planes, DeviceCache& dc, cudaStream_t stream);
 template <int Bytes>
-int launch_later(const void* labels, const RunBits* bits, float* f, const LineGeom& g0, float w, int border_lo,
-                 int border_hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl);
-// noise_predicted (edt_passes.cuh) for host code that launches nothing (edt_plan.cu).
-bool label_noise_predicted(const DeviceCache& dc);
+int launch_later(const void* labels, const LaterNoise* planned, float* f, const LineGeom& g0, float w,
+                 int border_lo, int border_hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream,
+                 bool pdl);
 // The site-tracking passes of the feature transform and the kernel that resolves their codes
 // into coordinate planes (edt_passes.cuh, edt_feature.cuh).
 template <int Bytes>
@@ -375,9 +403,31 @@ struct LaterLaunch {
   int kernel = -1;      // 0 = tile kernel, 1 = long-line kernel, 2 = window kernel, -1 = no launch yet
   // tx: the tile width, or the window kernel's radius
   int tx = 0, tma = 0, wide = 0, ctas = 0, int_hull = 0, epilogue = 0, all_double = 0;
-  int settled = 0;      // tiles whose voxels the X pass left settled are skipped (launch_later)
+  int settled = 0;      // tiles whose voxels the X pass left settled are skipped (plan_noise)
 };
 extern thread_local LaterLaunch g_last_later;
+
+// The label-noise plan of one transform (plan_noise, edt_passes.cuh): the run-start planes its X pass
+// writes (XPlanes) and how each later pass k >= 1 uses them.
+struct NoisePlan {
+  bool noise = false;          // the one reading of the noise prediction that every pass plans with
+  int planes = 0;              // later axes the X pass writes planes for: 0 none, 1 y, 2 y and z
+  LaterLaunch later[3];        // what launch_later plans for axis k; settled: it skips settled tiles
+  bool reads[3] = {false, false, false};   // axis k reads its run-start plane instead of the labels
+  int group[3] = {1, 1, 1};    // tiles per CTA of axis k
+  bool refresh = false;        // the Y pass refreshes the Z pass's settled plane
+};
+// plan_noise for transform t over `count` volumes laid end to end at labels / f on this device, with
+// one reading of the noise prediction and the A/B switches of the later passes (edt_plan.cu).
+NoisePlan noise_plan(const Transform& t, int64_t count, const void* labels, const float* f, const DeviceCache& dc);
+
+// One later pass of run_passes as noise_plan planned it: the prediction it plans with and, where it
+// reads its run-start plane (bits.start non-null), the plan that plane was armed for.
+struct LaterNoise {
+  bool noise = false;
+  RunBits bits = {};
+  LaterLaunch plan;
+};
 
 }  // namespace host
 }  // namespace edtb200

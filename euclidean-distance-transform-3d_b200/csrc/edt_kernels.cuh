@@ -514,11 +514,11 @@ struct TileBoxes {
 // The run-start plane of one later-axis pass written by the X pass (XPlanes): for the line (outer o,
 // inner j) and row i the bit (j % sx) & 31 of word  o * outer_words + (j / sx) * wpr + (j % sx) / 32
 // + i * row_words.  Y pass: outer = z, inner = x; Z pass: inner = y * sx + x.
-// With `settled` (the pass's settled plane, XPlanes) a tile whose voxels all have f <= w2 ends before
-// it loads anything: for the line (o, j) and row i the bit (j % sx) / 32 of word o * settled_outer +
-// j / sx + i * settled_row.  With `refresh` (the Y pass: the Z pass's settled plane, same layout)
-// every tile that runs sets the bits of its rows that it leaves at f <= refresh_t.
-// `group` (1 to 32): consecutive tiles per CTA of the grouped kernel (later_axis_tile_kernel).
+// The grouped kernel (skips_settled) reads `settled`, the pass's settled plane (XPlanes), and skips
+// every tile whose voxels all have f <= w2: for the line (o, j) and row i the bit (j % sx) / 32 of word
+// o * settled_outer + j / sx + i * settled_row.  With `refresh` (the Y pass: the Z pass's settled
+// plane, same layout) every tile that it runs sets the bits of its rows that it leaves at
+// f <= refresh_t.  `group` (1 to 32): consecutive tiles per CTA of the grouped kernel.
 struct RunBits {
   const uint32_t* start;   // a run of equal labels starts at this row (always at row 0)
   int64_t row_words;
@@ -532,6 +532,15 @@ struct RunBits {
   float refresh_t;
   int group;               // (in the tail padding: the struct keeps its size and layout)
 };
+
+// Whether the tile kernel instance <Bits, IntHull, Epilogue> is the grouped one that skips settled
+// tiles and refreshes the Z pass's settled plane: only there does a skipped tile provably equal what
+// the pass would store -- integer samples (with float hull tests the read-out may return a candidate
+// within rounding of the minimum, DESIGN.md section 8) and no epilogue, whose sqrt / sign rewrites
+// every row.  The host arms the skip by the same rule (plan_noise).
+constexpr __host__ __device__ bool skips_settled(bool bits, bool int_hull, bool epilogue) {
+  return bits && int_hull && !epilogue;
+}
 
 __device__ __forceinline__ uint32_t smem_addr(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -1296,9 +1305,8 @@ __device__ __forceinline__ bool next_group_tile(uint32_t todo, uint32_t& phase) 
 // plane is read only after griddepcontrol.wait: the Z pass may start while the X pass is still
 // running (the Y pass lets its dependents start before it waits itself).  Compiled for the
 // label-noise shape only (2 CTAs per SM, TMA, 32-wide tiles, no background bits: unsigned transforms).
-// It also skips settled tiles and refreshes the Z pass's settled plane, where the host passes those
-// planes in rb (launch_later).
-// Grouped (Bits with IntHull and no epilogue, the instance that skips settled tiles): a CTA owns the
+// Grouped (skips_settled: Bits with IntHull and no epilogue, the only instance that skips settled
+// tiles and refreshes the Z pass's settled plane): a CTA owns the
 // rb.group consecutive tiles from blockIdx.x * rb.group.  It reads the settled words of the whole
 // group once, then runs the tiles that are not settled one after another, with the border table and
 // the mbarrier set up once: a pass that skips nearly every tile costs one read per CTA instead of a
@@ -1342,7 +1350,7 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
   const int x = lane & (TX - 1);
   const int chunk0 = (threadIdx.x >> 5) * SUBS + (lane / TX);
   const int chunk_step = (blockDim.x >> 5) * SUBS;
-  constexpr bool kGrouped = Bits && IntHull && !Epilogue;
+  constexpr bool kGrouped = skips_settled(Bits, IntHull, Epilogue);
 
   // (kGrouped) bit k of `todo`: tile t0 + k is still to run.  The group's settled tiles are dropped
   // here, before the mbarrier, any tile load or the border table.  The hull words hold the check's
@@ -1388,26 +1396,6 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
 
     if (!kGrouped) pdl_launch_dependents();  // the next pass may start staging its labels during our tail
     if (!UseTMA) pdl_wait_for_previous_grid();           // plain loads of f happen in the staging loop
-    // (Bits) A tile whose voxels all have f <= w2 keeps every value (DESIGN.md section 4.1): it ends
-    // here, before its mbarrier, tile load or border table.  Thread t checks row t, in every row q of
-    // the settled plane that the tile's lines [j0, j1) reach, the x-segments they cover.
-    if constexpr (Bits && !Epilogue && !kGrouped) {
-      if (rb.settled) {
-        pdl_wait_for_previous_grid();    // the plane is complete (Z pass: and refreshed by the Y pass)
-        const int64_t j0 = inner0, j1 = min(inner0 + TX, g.inner_count);
-        const int64_t q0 = j0 / rb.sx, q1 = (j1 - 1) / rb.sx;
-        bool settled = true;
-        for (int i = threadIdx.x; i < n; i += blockDim.x) {
-          const uint32_t* sp = rb.settled + (outer * rb.settled_outer + (int64_t)i * rb.settled_row);
-          for (int64_t q = q0; q <= q1; ++q) {
-            const int lo = (int)max(j0 - q * rb.sx, (int64_t)0), hi = (int)min(j1 - q * rb.sx, rb.sx) - 1;
-            const uint32_t need = (0xffffffffu >> (31 - (hi >> 5))) & (0xffffffffu << (lo >> 5));
-            settled = settled && (__ldg(sp + q) & need) == need;
-          }
-        }
-        if (__syncthreads_and(settled)) continue;
-      }
-    }
     // Float tile by TMA, border-term table, chunk mask.  (kDecoupled) together with the mbarrier the
     // table and the mask are the only things a warp needs from other warps before the votes at the end
     // of stage 1, so the one barrier comes here, early, while no warp has loads in flight yet; the tile
@@ -1668,7 +1656,7 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
       }
     }
     if (!__syncthreads_or(any_cross)) {                      // every run was finished inside its chunk
-      if constexpr (Bits && !Epilogue) {
+      if constexpr (kGrouped) {
         if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
       }
       continue;
@@ -1887,7 +1875,7 @@ later_axis_tile_kernel(const __grid_constant__ CUtensorMap fmap,
         }
       }
     }
-    if constexpr (Bits && !Epilogue) {
+    if constexpr (kGrouped) {
       if (rb.refresh) refresh_settled(rb, f, g, outer, inner0, n);
     }
     // (kGrouped) the next tile's TMA and stage 0 overwrite the tile, the words and the chunk mask: every

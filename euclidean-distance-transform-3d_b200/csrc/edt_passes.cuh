@@ -101,7 +101,7 @@ int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, c
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
                  const XPlanes* planes, DeviceCache& dc, cudaStream_t stream) {
-  if (planes && (Bytes < 4 || sx > 512 || !first_is_vec(labels, Bytes, f, sx)))
+  if (planes && !first_is_vec(labels, Bytes, f, sx))   // launch_first_vec refuses the rest
     return fail(EDTB200_EINVAL, "run-start planes asked of an X launch that cannot write them");
   StepTable step(dc, stream);
   int trc = step.get(w, (int)sx + 1);
@@ -150,6 +150,12 @@ inline bool noise_predicted(const DeviceCache& dc) {
   if (!p) return false;
   const unsigned long long starts = p[0], voxels = p[1];
   return voxels > 0 && starts * 10ull >= voxels * 9ull;
+}
+
+// EDTB200_NO_INT_HULL: the later passes test their hulls in double only (A/B switch for measurements).
+inline bool no_int_hull() {
+  static const bool off = getenv("EDTB200_NO_INT_HULL") != nullptr;
+  return off;
 }
 
 // Tensor map over the distance volume for one later-axis pass: dims (adjacent lines, line
@@ -220,6 +226,66 @@ inline LaterLaunch plan_later(const LineGeom& g, bool epilogue, PassArith arith,
   return LaterLaunch{1, 0, 0, 0, 0, 0, epilogue, !arith.exact};
 }
 
+// plan_later's tma_ok before the tensor map is encoded: the distances 16-byte aligned (f16) and every
+// line and outer stride of g a multiple of 4 floats.
+inline bool tma_aligned(bool f16, const LineGeom& g) {
+  return f16 && g.line_stride % 4 == 0 && (g.outer_count <= 1 || g.outer_stride % 4 == 0);
+}
+
+// The label-noise plan of transform t over `count` volumes laid end to end (run_passes).  Pure host
+// logic.  f16: the distances are 16-byte aligned; first_vec: first_is_vec holds for its X pass; noise:
+// the one reading of noise_predicted; int_hull_off, forced_group: EDTB200_NO_INT_HULL and
+// EDTB200_SETTLED_GROUP.
+// The run-start planes pay where the later passes only stream -- label noise with labels of 4 or 8
+// bytes: there a later pass moves 4 + 1/8 bytes per voxel instead of 8 or 12, for 1/4 byte more
+// written by the X pass (which stages its label rows in shared memory, bands of slices marching along
+// y, to compare neighbouring rows).  On narrower labels and on structured volumes the dearer X pass
+// costs more than the later passes gain (DESIGN.md section 4.1), so none are taken there; nor for
+// signed transforms, whose last pass needs the labels' background bits as well.  The X pass writes a
+// plane for every later axis once one later pass takes a tile kernel; a later pass reads its plane
+// where it takes the label-noise tile kernel (2 CTAs per SM), otherwise the labels.
+inline NoisePlan plan_noise(const Transform& t, int64_t count, bool f16, bool first_vec, bool noise, bool int_hull_off,
+                            int forced_group, int max_smem_optin, int sm_count) {
+  NoisePlan np;
+  np.noise = noise;
+  const int64_t sx = t.n[0], sy = t.n[1], sz = t.n[2];
+  bool tile = false;
+  for (int k = 1; k < t.ndim; ++k) {
+    const LineGeom g = geom_for_axis(k, sx, sy, sz, count);
+    np.later[k] = plan_later(g, kernel_flags(t.flags, false, k == t.ndim - 1) != 0, transform_arith(t.w, t.n, k),
+                             max_smem_optin, tma_aligned(f16, g), noise, int_hull_off);
+    tile = tile || np.later[k].kernel == 0;
+  }
+  if (t.ndim < 2 || t.label_bytes < 4 || (t.flags & EDTB200_SIGNED) || sx > 512 || !first_vec || !noise ||
+      sz * count > 0x7fffffffLL || sy > 0x3fffffffLL || !tile)   // that X pass counts slices and rows in 32 bits
+    return np;
+  np.planes = t.ndim - 1;
+  for (int k = 1; k < t.ndim; ++k) {
+    LaterLaunch& p = np.later[k];
+    np.reads[k] = p.ctas == 2;       // the label-noise variant (tile_kernel_bits)
+    p.settled = np.reads[k] && skips_settled(true, p.int_hull, p.epilogue);
+    // With `settled` armed, each CTA checks and runs a group of consecutive tiles: as many as make the
+    // grid three to four waves of resident CTAs (at most 32, one bit per tile), so that a pass which
+    // skips nearly every tile costs a few reads per SM and not one CTA per tile.  Fewer, larger groups
+    // (two waves: 16 tiles at 512^3) skip no faster and serialise the tiles that run where they
+    // cluster, as the Z tiles of the X pass's band rows do (DESIGN.md section 4.1).  Resident CTAs: the
+    // plan's CTAs per SM (what the kernel is compiled for), so that sizing the grid adds no runtime
+    // query to the launch.
+    if (p.settled) {
+      const LineGeom g = geom_for_axis(k, sx, sy, sz, count);
+      const int64_t tiles = (g.inner_count + p.tx - 1) / p.tx * g.outer_count;
+      const int64_t waves4 = 4 * (int64_t)sm_count * p.ctas;
+      const int64_t group = forced_group > 0 ? forced_group : (tiles + waves4 - 1) / waves4;
+      np.group[k] = (int)(group < 1 ? 1 : group > 32 ? 32 : group);
+    }
+  }
+  // the Y pass refreshes the Z pass's settled plane where it skips tiles itself and the Z pass has
+  // no epilogue and integer samples
+  np.refresh = t.ndim == 3 && np.later[1].settled && kernel_flags(t.flags, false, true) == 0 &&
+               transform_arith(t.w, t.n, 2).int_hull;
+  return np;
+}
+
 // The plan of a bounded transform with max_distance d >= 0 (include/edt_b200.h, DESIGN.md section 5).
 // Pure host logic.  B is the largest float32 with (double)B <= d^2; a later pass along axis k needs
 // only the samples v with (double)w2 (i - v)^2 < nextafterf(B, +inf), i.e. within R_k rows, and takes
@@ -283,16 +349,14 @@ TileKernel<Bytes> tile_kernel_bits(const LaterLaunch& p) {
 }
 
 template <int Bytes>
-int launch_later(const void* labels, const RunBits* bits, float* f, const LineGeom& g0, float w, int border_lo,
+int launch_later(const void* labels, const LaterNoise* planned, float* f, const LineGeom& g0, float w, int border_lo,
                  int border_hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream, bool pdl) {
   using LT = typename LabelOf<Bytes>::type;
   LineGeom g = g0;
   const float w2 = w * w;                       // float product, as src/edt.hpp:181
-  static const bool int_hull_off = getenv("EDTB200_NO_INT_HULL") != nullptr;     // A/B switch for measurements
-  const bool aligned = reinterpret_cast<uintptr_t>(f) % 16 == 0 && g.line_stride % 4 == 0 &&
-                       (g.outer_count <= 1 || g.outer_stride % 4 == 0);
-  const bool noise = noise_predicted(dc);
-  LaterLaunch p = plan_later(g, flags != 0, arith, dc.max_smem_optin, aligned, noise, int_hull_off);
+  const bool aligned = tma_aligned(reinterpret_cast<uintptr_t>(f) % 16 == 0, g);
+  const bool noise = planned ? planned->noise : noise_predicted(dc);
+  LaterLaunch p = plan_later(g, flags != 0, arith, dc.max_smem_optin, aligned, noise, no_int_hull());
 
   if (p.kernel == 0) {
     TileBoxes tb;
@@ -303,7 +367,7 @@ int launch_later(const void* labels, const RunBits* bits, float* f, const LineGe
     CUtensorMap map;
     memset(&map, 0, sizeof(map));
     if (p.tma && !make_tile_map(&map, f, g, p.tx, tb.box_rows))
-      p = plan_later(g, flags != 0, arith, dc.max_smem_optin, false, noise, int_hull_off);
+      p = plan_later(g, flags != 0, arith, dc.max_smem_optin, false, noise, no_int_hull());
     const int warps = tile_warps(g.n, p.tx);
     // Programmatic dependent launch: this pass may begin (label staging) while the previous pass of
     // the stream drains its last wave; the kernel itself waits before touching the distances.
@@ -316,38 +380,22 @@ int launch_later(const void* labels, const RunBits* bits, float* f, const LineGe
     pdl_attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = pdl_attr;
     cfg.numAttrs = pdl ? 1 : 0;   // only when the previous kernel of the stream is our own pass
-    // the X pass's run-start plane is read where the plan is the label-noise variant (the prediction
-    // the plane was written for); any other plan reads the labels, and the plane goes unused
-    const bool use_bits = bits && Bytes >= 4 && p.tx == 32 && p.tma && !p.wide && p.ctas == 2 && !(flags & kNegate);
+    // The run-start plane, its settled skip and its group as plan_noise armed them; only where the
+    // tensor map could not be encoded is the plan another one, and the pass reads the labels.
     RunBits rb;
     memset(&rb, 0, sizeof(rb));
-    if (use_bits) rb = *bits;
-    // Settled tiles are skipped (and the Y pass refreshes the Z pass's plane) only where a skipped
-    // tile provably equals what the pass would store: integer samples (int_hull; with float hull tests
-    // the read-out may return a candidate within rounding of the minimum, DESIGN.md section 8) and no
-    // epilogue, whose sqrt / sign rewrites every row.
-    p.settled = use_bits && rb.settled && p.int_hull && flags == 0;
-    if (!p.settled) { rb.settled = nullptr; rb.refresh = nullptr; }
+    rb.group = 1;
+    if (planned && planned->bits.start) {
+      LaterLaunch armed = planned->plan;
+      armed.settled = 0;
+      if (!memcmp(&p, &armed, sizeof(p))) rb = planned->bits;
+    }
+    p.settled = rb.settled != nullptr;
     const TileKernel<Bytes> kern =
-        use_bits ? tile_kernel_bits<Bytes>(p)
+        rb.start ? tile_kernel_bits<Bytes>(p)
         : p.epilogue ? (p.tma ? tile_kernel<Bytes, true, true>(p) : tile_kernel<Bytes, true, false>(p))
                      : (p.tma ? tile_kernel<Bytes, false, true>(p) : tile_kernel<Bytes, false, false>(p));
     CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cfg.dynamicSmemBytes));
-    // With `settled` armed, each CTA of the Bits kernel checks and runs a group of consecutive tiles:
-    // as many as make the grid three to four waves of resident CTAs (at most 32, one bit per tile), so
-    // that a pass which skips nearly every tile costs a few reads per SM and not one CTA per tile.
-    // Fewer, larger groups (two waves: 16 tiles at 512^3) skip no faster and serialise the tiles that
-    // run where they cluster, as the Z tiles of the X pass's band rows do (DESIGN.md section 4.1).
-    // Resident CTAs: the plan's CTAs per SM (p.ctas, what the kernel is compiled for), so that sizing
-    // the grid adds no runtime query to the launch.  EDTB200_SETTLED_GROUP forces the group size (A/B
-    // switch for measurements).
-    rb.group = 1;
-    if (p.settled) {
-      static const int forced_group = getenv("EDTB200_SETTLED_GROUP") ? atoi(getenv("EDTB200_SETTLED_GROUP")) : 0;
-      const int64_t waves4 = 4 * (int64_t)dc.sm_count * p.ctas;
-      const int64_t group = forced_group > 0 ? forced_group : (tiles + waves4 - 1) / waves4;
-      rb.group = (int)(group < 1 ? 1 : group > 32 ? 32 : group);
-    }
     cfg.gridDim = dim3((unsigned)((tiles + rb.group - 1) / rb.group));
     CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, map, static_cast<const LT*>(labels), rb, f, g, tb, w2, border_lo,
                                 border_hi, flags, p.int_hull ? (int)w2 : 0));
@@ -466,7 +514,7 @@ int launch_expand_gather(const void* labels, const float* sqdist, const int32_t*
   template int edtb200::host::launch_first<B>(const void*, float*, int64_t, int64_t, float, int, int,    \
                                               const edtb200::XPlanes*, edtb200::host::DeviceCache&,      \
                                               cudaStream_t);                                             \
-  template int edtb200::host::launch_later<B>(const void*, const edtb200::RunBits*, float*,              \
+  template int edtb200::host::launch_later<B>(const void*, const edtb200::host::LaterNoise*, float*,     \
                                               const edtb200::LineGeom&, float, int, int, int,            \
                                               edtb200::host::PassArith, edtb200::host::DeviceCache&,     \
                                               cudaStream_t, bool);                                       \

@@ -1,6 +1,6 @@
-// edt_plan.cu -- the later-axis plan (plan_later, edt_passes.cuh) for host code that only needs to
-// know which kernel a pass would take, not launch it.  It instantiates no launcher: those live in
-// edt_passes_b{1,2,4,8}.cu.
+// edt_plan.cu -- the later-axis and label-noise plans (plan_later, plan_noise, edt_passes.cuh) for host
+// code that only needs to know what the passes would take, not launch them.  It instantiates no
+// launcher: those live in edt_passes_b{1,2,4,8}.cu.
 #include "edt_passes.cuh"
 
 namespace edtb200 {
@@ -11,7 +11,12 @@ bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin) 
   return plan_later(g, false, arith, max_smem_optin, true, false, false).kernel == 1;
 }
 
-bool label_noise_predicted(const DeviceCache& dc) { return noise_predicted(dc); }
+NoisePlan noise_plan(const Transform& t, int64_t count, const void* labels, const float* f, const DeviceCache& dc) {
+  // EDTB200_SETTLED_GROUP forces the later passes' group size (A/B switch for measurements)
+  static const int forced_group = getenv("EDTB200_SETTLED_GROUP") ? atoi(getenv("EDTB200_SETTLED_GROUP")) : 0;
+  return plan_noise(t, count, reinterpret_cast<uintptr_t>(f) % 16 == 0, first_is_vec(labels, t.label_bytes, f, t.n[0]),
+                    noise_predicted(dc), no_int_hull(), forced_group, dc.max_smem_optin, dc.sm_count);
+}
 
 BoundedPlan bounded_plan(int ndim, const float w[3], double max_distance, bool sites) {
   int64_t rmax = sites ? EDTB200_BOUNDED_SITES_WINDOW_MAX : EDTB200_BOUNDED_WINDOW_MAX;

@@ -16,22 +16,18 @@ import sys
 import numpy as np
 import pytest
 
+from noise_cases import FRESH, WIDE, twice
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HERE = os.path.dirname(os.path.abspath(__file__))
-WIDE = (np.uint32, np.uint64)
-FRESH = 1 << 21                        # planted labels: above every noise label
 # (sz, sy, sx) in array order; Y tiles sz * ceil(sx / 32), Z tiles ceil(sx * sy / 32)
 SHAPES = [(20, 33, 32), (12, 40, 48), (10, 37, 96), (6, 24, 512)]
 STACK = (3, 5, 21, 48)                 # 3 volumes: 32 Z tiles each, the last one half full
 # array order (w_z, w_y, w_x): with w_z = 2 the Z pass takes voxels at f <= 4 as settled, so the Y
 # pass's refresh settles the Z tiles of x-runs of five (f = 9 after X, 2 after Y)
 ANISO = [(1.0, 1.0, 1.0), (2.0, 1.0, 1.0)]
-
-
-def noise(shape, dtype, rng):
-  return rng.integers(1, 1 << 20, shape).astype(dtype)
 
 
 def pattern(group_index, group, rng):
@@ -52,7 +48,7 @@ def planted(shape, dtype, seed, group):
   tiles (z, x-segment): an x-run of three inside the segment (f = 4 after X), and in every fourth
   such tile an x-run of five, whose middle voxel only the Y pass settles for the Z pass."""
   rng = np.random.default_rng(seed)
-  lab = noise(shape, dtype, rng)
+  lab = rng.integers(1, 1 << 20, shape).astype(dtype)
   vols = lab.reshape((-1,) + shape[-3:])
   nv = vols.shape[0]
   sz, sy, sx = shape[-3:]
@@ -86,11 +82,6 @@ def planted(shape, dtype, seed, group):
       if x0 + width <= sx:
         vols[v, z, y, x0:x0 + width] = next(fresh)
   return lab
-
-
-def twice(fn, labels, **kw):
-  fn(labels, **kw)                     # leaves the run statistic of this volume behind
-  return fn(labels, **kw)
 
 
 def run_cases(edt, oracle, group):

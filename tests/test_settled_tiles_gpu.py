@@ -10,17 +10,9 @@ The plan's `settled` field says whether the skip was armed: on int_hull passes w
 import numpy as np
 import pytest
 
+from noise_cases import FRESH, WIDE, noise, twice
+
 pytestmark = pytest.mark.gpu
-
-WIDE = (np.uint32, np.uint64)
-FRESH = 1 << 21                        # planted labels: above every noise label
-
-
-def noise(shape, dtype, seed, background=0.02):
-  rng = np.random.default_rng(seed)
-  lab = rng.integers(1, 1 << 20, shape).astype(dtype)
-  lab[rng.random(shape) < background] = 0
-  return lab
 
 
 def planted(shape, dtype, seed):
@@ -80,13 +72,6 @@ def unsettled_everywhere(shape, dtype, seed):
       rows[np.arange(rows.shape[0]), x0 + d] = np.arange(fresh, fresh + rows.shape[0])
     fresh += rows.shape[0]
   return lab
-
-
-def twice(fn, labels, **kw):
-  # leaves the run statistic of this volume behind; under a black border the row's first voxel
-  # counts as a run start, so that narrow rows (sx = 4) are label noise too
-  fn(labels, **dict(kw, black_border=True))
-  return fn(labels, **kw)
 
 
 # (sz, sy, sx): sx in 4, 36, 132, 500, 512; sy and sz not multiples of 8.  Rows of fewer than 32

@@ -2,7 +2,11 @@
 """Device times of the 512^3 label-noise edtsq (iid labels 0..255, anisotropy (1, 1, 1), no black
 border: the bench.py workload) for labels of 4 and 8 bytes, whole transform and per pass (GPU only):
 
-  python tools/noise_bench.py [--size 512] [--steps 20] [--reps 3]    (EDTB200_LIBRARY=... for another build)
+  python tools/noise_bench.py [--size 512] [--steps 20] [--reps 3] [--anisotropy 1,0.7,1]
+                              (EDTB200_LIBRARY=... for another build)
+
+--anisotropy (array order) picks other weights: with a non-integer one the later passes read their
+run-start planes without skipping settled tiles.
 
 Each label width is transformed twice before timing, so that the run statistic predicts label noise
 and the X pass writes the run-start planes.  A rep times `steps` transforms between two CUDA events,
@@ -39,7 +43,9 @@ def main():
   ap.add_argument("--size", type=int, default=512)
   ap.add_argument("--steps", type=int, default=20)
   ap.add_argument("--reps", type=int, default=3)
+  ap.add_argument("--anisotropy", type=lambda v: tuple(float(x) for x in v.split(",")), default=(1.0, 1.0, 1.0))
   args = ap.parse_args()
+  w = args.anisotropy
   dev = torch.device("cuda", 0)
   lib = edt._lib()
   n = args.size
@@ -51,20 +57,20 @@ def main():
     lab = base.to(dtype)
     out = torch.empty(lab.shape, dtype=torch.float32, device=dev)
     for _ in range(2):
-      edt.edt_cuda(lab, (1, 1, 1), False, out=out)
+      edt.edt_cuda(lab, w, False, out=out)
     torch.cuda.synchronize()
     totals, passes = [], []
     for _ in range(args.reps):
       e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
       e0.record()
       for _ in range(args.steps):
-        edt.edt_cuda(lab, (1, 1, 1), False, out=out)
+        edt.edt_cuda(lab, w, False, out=out)
       e1.record()
       torch.cuda.synchronize()
       totals.append(e0.elapsed_time(e1) / args.steps)
       lib.edtb200_profile_passes(1)
       for _ in range(args.steps):
-        edt.edt_cuda(lab, (1, 1, 1), False, out=out)
+        edt.edt_cuda(lab, w, False, out=out)
       torch.cuda.synchronize()
       lib.edtb200_profile_passes(0)
       buf = (ctypes.c_float * 3)()
@@ -74,7 +80,7 @@ def main():
           raise RuntimeError("edtb200_pass_ms failed")
         smp.append([float(v) for v in buf])
       passes.append([statistics.mean(s[i] for s in smp) for i in range(3)])
-    print(json.dumps({"label_bytes": lab.element_size(), "size": n, "steps": args.steps,
+    print(json.dumps({"label_bytes": lab.element_size(), "size": n, "anisotropy": w, "steps": args.steps,
                       "ms": [round(t, 4) for t in totals], "ms_median": round(statistics.median(totals), 4),
                       "pass_ms_xyz": [[round(v, 4) for v in p] for p in passes], "clocks": card()}), flush=True)
     del lab, out

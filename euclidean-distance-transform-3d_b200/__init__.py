@@ -39,7 +39,7 @@ __all__ = [
   "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
   "parabolic_erode", "parabolic_dilate", "nearest_labels", "medial_axis",
-  "skeletonize",
+  "skeletonize", "local_thickness",
 ]
 
 FLAG_SQRT = 1
@@ -117,6 +117,9 @@ def _lib():
   lib.edtb200_morphology.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ctypes.c_double, ci, ci, vp,
                                      ci, vp]
   lib.edtb200_morphology.restype = ci
+  lib.edtb200_local_thickness.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp, vp, ci,
+                                          vp]
+  lib.edtb200_local_thickness.restype = ci
   lib.edtb200_parabolic.argtypes = [vp, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, ci, vp]
   lib.edtb200_parabolic.restype = ci
   lib.edtb200_parabolic_sites.argtypes = [vp, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
@@ -1242,6 +1245,112 @@ def spherical_close(labels, radius, anisotropy=None, black_border=False, *, devi
   scipy.ndimage.binary_erosion(D, B, border_value=0 if black_border else 1).  Both transforms run back to
   back on the GPU.  Returns a bool mask."""
   return _morphology(_CLOSE, labels, radius, anisotropy, black_border, device, stacked, "spherical_close")
+
+
+# ---------------------------------------------------------------------------------------
+# local thickness: the largest opening of a ladder of radii that still covers each voxel
+# (edtb200_local_thickness)
+# ---------------------------------------------------------------------------------------
+
+THICKNESS_MAX_SIZES = 4096      # EDTB200_THICKNESS_MAX_SIZES
+
+
+def _thickness_sizes(sizes, name):
+  """An int n (default levels, as n) or the given radii as float64, sorted descending without repeats."""
+  if isinstance(sizes, (bool, np.bool_)):
+    raise TypeError("%s: sizes must be an integer or a 1-D sequence of radii, got %r" % (name, sizes))
+  if isinstance(sizes, (int, np.integer)):
+    if not 1 <= sizes <= THICKNESS_MAX_SIZES:
+      raise ValueError("%s: sizes must be 1 to %d levels, got %d" % (name, THICKNESS_MAX_SIZES, sizes))
+    return int(sizes)
+  arr = np.asarray(sizes)
+  if arr.dtype.kind not in "iuf":
+    raise TypeError("%s: sizes must be an integer or a 1-D sequence of radii, got %r" % (name, sizes))
+  if arr.ndim != 1 or arr.size == 0:
+    raise ValueError("%s: sizes must be a non-empty 1-D sequence of radii, got shape %s" % (name, arr.shape))
+  arr = arr.astype(np.float64)
+  if not (np.all(np.isfinite(arr)) and np.all(arr >= 0.0)):
+    raise ValueError("%s: every size must be finite and zero or more, got %r" % (name, sizes))
+  arr = np.unique(arr)[::-1].copy()
+  if arr.size > THICKNESS_MAX_SIZES:
+    raise ValueError("%s: at most %d distinct sizes, got %d" % (name, THICKNESS_MAX_SIZES, arr.size))
+  return arr
+
+
+def local_thickness(labels, anisotropy=None, black_border=False, *, sizes=25, return_sizes=False, device=0,
+                    stacked=False):
+  """Local thickness of every label at once: for each labelled voxel, the largest radius of a ladder of sizes
+  whose ball lies inside the voxel's own label and covers the voxel, as porespy's local_thickness defines it.
+
+  Definition.  For labels L (0 is background), anisotropy w, black_border and levels r_1 > ... > r_m:
+    1. D2 = edtsq(L, w, black_border), bit for bit;
+    2. the seeds of level r are the voxels whose D2 is not within r ((double)D2 > r * r): the voxels
+       spherical_erode(L, r, w, black_border) keeps;
+    3. d2_r = edtsq of the mask that is 0 on the seeds and 1 elsewhere, without black border;
+    4. out[p] = float32(max r_i with L(p) != 0 and (double)d2_r_i(p) <= r_i * r_i), or 0 where there is none.
+  So out == max_i(np.where(spherical_open(L, r_i, w, black_border) != 0, r_i, 0)) bit for bit: every label is
+  handled in one pass because the ball around a seed lies inside the seed's label.  The value is a RADIUS in
+  the units of w; Hildebrand & Ruegsegger's thickness (BoneJ's Thickness) is twice it.  Labels compare as
+  edt() compares them: floats by value, so -0.0 is background.  Exact Hildebrand thickness, with every
+  distinct D2 as a level, is not offered: each level costs one transform of a 1-byte mask.
+
+  Levels.  `sizes` is either
+    - a sequence of radii, finite and >= 0: sorted descending without repeats, the same for every volume;
+    - an integer n (default 25): per volume, in float64, with R = sqrt(the largest finite D2 over its
+      labelled voxels) and h = min(w) (the least weight, rounded to float32 as every weight is),
+      r_i = (h/2) * (2R/h)^(i/n) for i = 0 .. n-1.  Every labelled voxel gets at least h/2 and the top level
+      stays below R; a volume with no finite labelled D2 (no labelled
+      voxel, or one label without black_border) takes R = h/2.  These levels are computed on the GPU (pow
+      may differ from numpy's in the last bit), so the result is defined relative to the levels used, which
+      return_sizes=True returns: as out, sizes (shape (m,) descending, or (count, m) for a stack with
+      default levels, whose volumes have their own levels).
+
+  Input and output.  Labels of bool, any integer dtype, float32 or float64, 1-D to 3-D (2-D to 4-D with
+  stacked=True, whose slowest axis in memory indexes same-shaped volumes as edt(stacked=True): the result
+  equals np.stack of the per-volume calls).  Returns float32 with the input's shape and memory order.  numpy
+  in gives numpy out; a torch CUDA tensor (or any __cuda_array_interface__ array) gives torch CUDA tensors
+  computed on the current stream without a host synchronisation, default levels included.  Sizes that are
+  empty, not 1-D, NaN, infinite or negative, an n below 1 or above THICKNESS_MAX_SIZES, and a weight that
+  is not finite and > 0 are ValueErrors; an unsupported dtype or number of dimensions, or sizes of a
+  non-numeric type, TypeErrors.  A host array that does not fit on the GPU raises EDTError with code ENOMEM
+  (there is no chunked path).  Device memory beyond the input and output: 9 bytes per voxel (label bytes
+  more for float labels)."""
+  name = "local_thickness"
+  levels = _thickness_sizes(sizes, name)
+  if not isinstance(return_sizes, (bool, np.bool_)):
+    raise TypeError("%s: return_sizes must be True or False, got %r" % (name, return_sizes))
+  v = _Volume(name, labels, stacked, (1, 3), device)
+  nbytes = _morph_label_bytes(v.dtype)
+  if nbytes is None:
+    raise TypeError("%s: unsupported label dtype %s" % (name, v.dtype))
+  v.set_weights(anisotropy)
+  out = v.empty("float32")
+  count = v.geometry[4]
+  by_default = isinstance(levels, int)
+  m = levels if by_default else levels.size
+  # the levels the C ABI writes: every default level, and the given ones only on the device (the host has them)
+  used = None
+  if return_sizes and (by_default or v.on_device):
+    if v.on_device:
+      import torch
+      used = torch.empty((count, m), dtype=torch.float64, device=v.arr.device)
+    else:
+      used = np.empty((count, m), np.float64)
+  if v.size:
+    flags = v.flags | (FLAG_LABELS_FLOAT if v.floating else 0)
+    _check(_lib().edtb200_local_thickness(v.ptr, nbytes, *v.geometry, int(bool(black_border)), flags,
+                                          None if by_default else levels.ctypes.data, m, v.ptr_of(out),
+                                          v.ptr_of(used), *v.where))
+  elif used is not None:            # no voxel: every default level is h/2, and the given ones as they are
+    used[...] = 0.5 * float(min(np.float32(x) for x in v.geometry[5:5 + v.vnd])) if by_default else \
+        used.new_tensor(levels)
+  if not return_sizes:
+    return out
+  if by_default:
+    return out, (used if v.stacked else used[0])
+  if not v.on_device:
+    return out, levels
+  return out, (used[0] if count else used.new_tensor(levels))
 
 
 # ---------------------------------------------------------------------------------------

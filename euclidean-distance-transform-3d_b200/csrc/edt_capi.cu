@@ -1818,6 +1818,118 @@ int edtb200_morphology(const void* labels, int label_bytes, int ndim, int64_t sx
   return rc ? rc : io.finish();
 }
 
+int edtb200_local_thickness(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                            int64_t count, float wx, float wy, float wz, int black_border, int flags,
+                            const double* sizes, int nsizes, float* out, double* sizes_out, int device,
+                            void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  const float w[3] = {wx, wy, wz};
+  if ((rc = check_weights(ndim, w))) return rc;
+  if (nsizes < 1 || nsizes > EDTB200_THICKNESS_MAX_SIZES)
+    return fail(EDTB200_EINVAL, "nsizes must be 1 to %d (got %d)", EDTB200_THICKNESS_MAX_SIZES, nsizes);
+  if (sizes)
+    for (int i = 0; i < nsizes; ++i)
+      if (!(sizes[i] >= 0.0) || std::isinf(sizes[i]))
+        return fail(EDTB200_EINVAL, "sizes[%d] must be finite and zero or more (got %g)", i, sizes[i]);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE | EDTB200_LABELS_FLOAT))
+    return fail(EDTB200_EINVAL,
+                "edtb200_local_thickness takes only the residency flags and EDTB200_LABELS_FLOAT (got %d)", flags);
+  if ((rc = check_float_labels(flags, label_bytes))) return rc;
+  const bool as_float = flags & EDTB200_LABELS_FLOAT;
+  const int64_t vol = sx * sy * sz;
+  if ((rc = check_stack(vol, count, 1))) return rc;
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, out_bytes = sizeof(float) * (size_t)total;
+  const size_t levels_bytes = sizeof(double) * (size_t)count * (size_t)nsizes;
+  if (same_side(flags) && overlaps(labels, lab_bytes, out, out_bytes)) return fail(EDTB200_EINVAL, "out overlaps labels");
+  if (sizes_out && overlaps(sizes_out, levels_bytes, out, out_bytes))
+    return fail(EDTB200_EINVAL, "sizes_out overlaps out");
+  if (sizes_out && same_side(flags) && overlaps(sizes_out, levels_bytes, labels, lab_bytes))
+    return fail(EDTB200_EINVAL, "sizes_out overlaps labels");
+  // the levels a caller gave, descending; a repeated level is run once
+  std::vector<double> given;
+  if (sizes) given.assign(sizes, sizes + nsizes);
+  std::sort(given.begin(), given.end(), [](double a, double b) { return a > b; });
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  const void* d_labels = nullptr;
+  float* d_out = nullptr;
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) || (rc = io.out_dist(out, out_bytes, &d_out))) return rc;
+  // scratch: D2, the mask and the mask's distances (9 bytes per voxel), the folded float labels, and with
+  // default levels their table (r staged for a host sizes_out, or kept in scratch without one), cuts and tops
+  Scratch d2, mask, d2r, folded, table, staged;
+  const char* what = "local thickness's scratch";
+  const bool by_default = !sizes;
+  double* d_levels = nullptr;
+  if ((rc = d2.take(*io.dc, sizeof(float) * (size_t)total, s, what)) ||
+      (rc = mask.take(*io.dc, (size_t)total, s, what)) ||
+      (rc = d2r.take(*io.dc, sizeof(float) * (size_t)total, s, what)) ||
+      (as_float && (rc = folded.take(*io.dc, lab_bytes, s, what))))
+    return rc;
+  if (sizes_out && (by_default || io.out_dev) &&
+      (rc = io.out_staged(sizes_out, levels_bytes, staged, "the levels", &d_levels)))
+    return rc;
+  const size_t cuts_bytes = sizeof(float) * (size_t)count * (size_t)nsizes;
+  if (by_default &&
+      (rc = table.take(*io.dc, (d_levels ? 0 : levels_bytes) + cuts_bytes + sizeof(unsigned) * (size_t)count, s, what)))
+    return rc;
+  const void* runs = d_labels;                   // the labels the edtsq compares
+  if (as_float) {
+    if ((rc = launch_fold_float_labels(d_labels, label_bytes, folded.get(), total, *io.dc, s))) return rc;
+    runs = folded.get();
+  }
+  StepTimer timer(s);
+  timer.stamp();
+  rc = run_passes(runs, label_bytes, ndim, sx, sy, sz, wx, wy, wz, black_border != 0, 0, d2.get<float>(), *io.dc, s,
+                  count);
+  float* cuts = nullptr;
+  if (!rc && by_default) {
+    char* base = table.get<char>();
+    if (!d_levels) { d_levels = reinterpret_cast<double*>(base); base += levels_bytes; }
+    cuts = reinterpret_cast<float*>(base);
+    unsigned* top = reinterpret_cast<unsigned*>(base + cuts_bytes);
+    const double h = (double)*std::min_element(w, w + ndim);
+    rc = launch_thickness_top(d_labels, label_bytes, as_float, d2.get<float>(), vol, count, top, *io.dc, s);
+    if (!rc) rc = launch_thickness_levels(top, count, nsizes, h, d_levels, cuts, *io.dc, s);
+  }
+  timer.stamp();
+  // per level: the seeds, the edtsq of the mask, the store
+  bool first = true;
+  for (int i = 0; !rc && i < nsizes; ++i) {
+    edtb200::ThicknessLevel level{nullptr, nullptr, 0, 0.0, 0.0f};
+    if (by_default) {
+      level = {d_levels + i, cuts + i, nsizes, 0.0, 0.0f};
+    } else {
+      level.r0 = given[i];
+      level.b0 = edtb200::cut_bound(given[i]);
+      if (sizes_out && !io.out_dev)
+        for (int64_t v = 0; v < count; ++v) sizes_out[v * nsizes + i] = given[i];
+      else if (sizes_out && (rc = launch_thickness_fill(d_levels, count, nsizes, i, given[i], *io.dc, s)))
+        break;
+      if (i > 0 && given[i] == given[i - 1]) continue;
+    }
+    rc = launch_thickness_seed(d2.get<float>(), vol, count, level, mask.get<uint8_t>(), *io.dc, s);
+    if (!rc)
+      rc = run_passes(mask.get(), 1, ndim, sx, sy, sz, wx, wy, wz, 0, 0, d2r.get<float>(), *io.dc, s, count);
+    if (!rc)
+      rc = launch_thickness_store(d_labels, label_bytes, as_float, d2r.get<float>(), vol, count, level, first, d_out,
+                                  *io.dc, s);
+    first = false;
+  }
+  timer.stamp();
+  if (!rc && timer.synchronize())
+    fprintf(stderr, "[edt_b200] local_thickness %lldx%lldx%lld x%lld L=%d  edtsq and levels %.3f ms  %d levels %.3f ms\n",
+            (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, timer.ms(0, 1), nsizes,
+            timer.ms(1, 2));
+  return rc ? rc : io.finish();
+}
+
 // edtb200_parabolic, and with sites edtb200_parabolic_sites.
 static int parabolic_any(const float* f, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx,
                          float wy, float wz, int op, int flags, float* out, bool sites, int32_t* idx, int device,

@@ -1,25 +1,40 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as thirteen translation units so that the kernel templates build in
+// The library is compiled as fourteen translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
 // transforms' kernels), edt_surface.cu (the surface distances' kernels), edt_morphology.cu (the
 // spherical morphology's label-writing stores), edt_parabolic.cu (the parabolic erosion and
 // dilation passes), edt_nearest.cu (the nearest-labels passes), edt_medial.cu (the medial
-// axis's mark kernel) and edt_skeleton.cu (the skeleton's thinning kernel).  The run-time label width
+// axis's mark kernel), edt_skeleton.cu (the skeleton's thinning kernel) and edt_thickness.cu
+// (local thickness's levels, seeds and stores).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
 #include "edt_kernels.cuh"
 #include "edt_feature.cuh"       // SiteBox
 
+#include <cfloat>
+#include <cmath>
 #include <condition_variable>
 #include <cstdint>
 #include <mutex>
 #include <type_traits>
 
 namespace edtb200 {
+
+// The cut B of max_distance d >= 0: the largest float32 whose double is at most d^2 (FLT_MAX where d^2
+// reaches it), so that a float32 squared distance v is within d iff v <= B.  Also on the device, where
+// local thickness derives the cut of each level it computes there.
+__host__ __device__ inline float cut_bound(double d) {
+  const double L = d * d;
+  if (L >= (double)FLT_MAX) return FLT_MAX;
+  float b = (float)L;
+  if ((double)b > L) b = nextafterf(b, -INFINITY);
+  return b;
+}
+
 namespace host {
 
 // Sets the calling thread's error message (edtb200_last_error) and returns `code`.
@@ -333,7 +348,45 @@ struct MorphSelect {
   bool as_float;       // 4- / 8-byte IEEE labels: -0.0 is zero
 };
 
+// Whether a raw label is non-zero; as_float: 4- / 8-byte IEEE labels, where -0.0 is zero too.
+template <int SrcBytes>
+__device__ __forceinline__ bool label_nonzero(typename LabelOf<SrcBytes>::type v, bool as_float) {
+  if constexpr (SrcBytes >= 4) {
+    using LT = typename LabelOf<SrcBytes>::type;
+    if (as_float) return (LT)(v << 1) != 0;                // every bit but the sign
+  }
+  return v != 0;
+}
+
+// One level of local thickness (edt_thickness.cuh): its radius r and cut B = cut_bound(r), for volume v at
+// r[v * vstride] and bound[v * vstride] (the default levels, computed on the device), or r0 and b0 for every
+// volume when r is null (levels the caller gave).
+struct ThicknessLevel {
+  const double* r;
+  const float* bound;
+  int64_t vstride;
+  double r0;
+  float b0;
+};
+
 namespace host {
+
+// The kernels of local thickness over `count` volumes of `vol` voxels (edt_thickness.cu).
+// launch_thickness_top: top[v] = 1 + the bits of v's largest finite labelled D2 (0: none; top zeroed
+// here).  launch_thickness_levels: the n default levels of every volume from top, descending, and their
+// cuts.  launch_thickness_fill: out[v * m + j] = r for every volume.  launch_thickness_seed: mask = 0 where
+// D2 > B, else 1.  launch_thickness_store: out = fl32(r) where the voxel is labelled and d2r <= B, taking
+// the maximum with out unless `first` (then 0 elsewhere).
+int launch_thickness_top(const void* labels, int label_bytes, bool as_float, const float* d2, int64_t vol,
+                         int64_t count, unsigned* top, DeviceCache& dc, cudaStream_t stream);
+int launch_thickness_levels(const unsigned* top, int64_t count, int n, double h, double* r, float* bound,
+                            DeviceCache& dc, cudaStream_t stream);
+int launch_thickness_fill(double* out, int64_t count, int m, int j, double r, DeviceCache& dc, cudaStream_t stream);
+int launch_thickness_seed(const float* d2, int64_t vol, int64_t count, const ThicknessLevel& level, uint8_t* mask,
+                          DeviceCache& dc, cudaStream_t stream);
+int launch_thickness_store(const void* labels, int label_bytes, bool as_float, const float* d2r, int64_t vol,
+                           int64_t count, const ThicknessLevel& level, bool first, float* out, DeviceCache& dc,
+                           cudaStream_t stream);
 
 // The morphology's kernels (edt_morphology.cu).  launch_window_select: the last later pass along g as
 // launch_later_window, with the select in its store (label_bytes: the transform's labels, 1 or

@@ -11,16 +11,6 @@
 
 namespace edtb200 {
 
-// Whether a raw label is non-zero; as_float: 4- / 8-byte IEEE labels, where -0.0 is zero too.
-template <int SrcBytes>
-__device__ __forceinline__ bool label_nonzero(typename LabelOf<SrcBytes>::type v, bool as_float) {
-  if constexpr (SrcBytes >= 4) {
-    using LT = typename LabelOf<SrcBytes>::type;
-    if (as_float) return (LT)(v << 1) != 0;                // every bit but the sign
-  }
-  return v != 0;
-}
-
 // The select of voxel `at`: near = its value is within the bound.
 template <int SrcBytes>
 __device__ __forceinline__ void morph_store(const MorphSelect& sel, int64_t at, bool near) {

@@ -293,13 +293,7 @@ inline NoisePlan plan_noise(const Transform& t, int64_t count, bool f16, bool fi
 // capped at 2^62, which also stands for "no bound" (B = FLT_MAX, or w2 = 0).
 inline BoundedPlan plan_bounded(int ndim, const float w[3], double d, int64_t rmax) {
   BoundedPlan p;
-  const double L = d * d;
-  if (L >= (double)FLT_MAX) {
-    p.bound = FLT_MAX;
-  } else {
-    p.bound = (float)L;
-    if ((double)p.bound > L) p.bound = nextafterf(p.bound, -INFINITY);
-  }
+  p.bound = cut_bound(d);
   const double above = (double)nextafterf(p.bound, INFINITY);
   for (int k = 0; k < ndim; ++k) {
     const double w2 = (double)(w[k] * w[k]);          // the float product the passes use

@@ -38,7 +38,7 @@ extern "C" {
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
- * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window)
+ * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -239,6 +239,60 @@ int edtb200_morphology(const void *labels, int label_bytes, int ndim,
                        int64_t sx, int64_t sy, int64_t sz, int64_t count,
                        float wx, float wy, float wz, int op, double radius,
                        int black_border, int flags, void *out, int device, void *stream);
+
+/* Local thickness of every label at once: for each labelled voxel, the radius of the largest ball of a
+ * given ladder of levels that lies inside the voxel's own label and covers it (Hildebrand & Ruegsegger's
+ * thickness is twice this value, BoneJ's included; porespy's local_thickness returns the radius).  For
+ * labels L (0 is background), weights w, black_border and levels r_1 > ... > r_m of a volume:
+ *   1. D2 = edtb200_transform's edtsq of L with black_border, bit for bit;
+ *   2. the seeds of level r are S_r = { x : (double)D2(x) > r*r } -- exactly the voxels EDTB200_ERODE at
+ *      radius r keeps; background has D2 = 0 and is never a seed;
+ *   3. d2_r = the edtsq of the 1-byte mask that is 0 on S_r and 1 elsewhere, WITHOUT black border (the
+ *      second transform of EDTB200_OPEN);
+ *   4. out[p] = fl32(max{ r_i : L(p) != 0 and (double)d2_r_i(p) <= r_i*r_i }), and 0 where no level
+ *      qualifies or L(p) == 0.
+ * So out equals the maximum over i of (r_i where edtb200_morphology's EDTB200_OPEN at r_i is non-zero), bit
+ * for bit: the ball around a seed lies inside the seed's own label, so one pass handles every label.
+ * Exact Hildebrand thickness (every distinct D2 as a level) is not offered: each level costs a transform.
+ *
+ *   labels     count * sx*sy*sz labels of label_bytes (1, 2, 4 or 8) bytes, volumes back to back as for
+ *              edtb200_transform_stack (count 1: one volume), each on its own
+ *   wx..wz     the weights of the first ndim axes: finite and > 0
+ *   flags      the residency flags, and EDTB200_LABELS_FLOAT for 4- / 8-byte IEEE labels (-0.0 is then
+ *              background), as edtb200_morphology takes them
+ *   sizes      a host array of nsizes radii, finite and >= 0, in any order and with repeats: the levels of
+ *              every volume (sorted descending; a repeat is run once).  NULL: nsizes default levels per
+ *              volume, computed on the device in double from R = sqrt(the largest finite D2 over the
+ *              volume's labelled voxels) -- R = h/2 where there is none (no labelled voxel, or one label
+ *              without black_border) -- and h = the least weight of the first ndim axes (a float):
+ *                  r_i = (h/2) * (2R/h)^(i/n),  i = 0 .. n-1,  n = nsizes
+ *              so every labelled voxel gets at least h/2 (it is its own seed) and the top level stays
+ *              below R, which leaves it seeds.  pow may differ from another library's in the last bit:
+ *              the result is defined relative to the levels sizes_out returns.
+ *   nsizes     1 .. EDTB200_THICKNESS_MAX_SIZES
+ *   out        count * sx*sy*sz float32 radii in the units of w; must not overlap labels
+ *   sizes_out  NULL, or count * nsizes doubles on the side of out: the levels volume v used, descending, at
+ *              sizes_out[v * nsizes ...] (repeats kept)
+ * Residency, staging and asynchrony as edtb200_morphology: both sides on the device run asynchronously on
+ * `stream` with no host wait, default levels included; host buffers are staged whole (EDTB200_ENOMEM when
+ * they do not fit; there is no chunked path).  Kernels, on one stream, one launch per pass for the whole
+ * stack: the edtsq (edtb200_transform's passes); with default levels a per-volume maximum of the finite
+ * labelled D2 and one kernel that writes the levels and their float cuts B = the largest float32 whose
+ * double is at most r*r to the device; then per level a seed kernel (D2 > B -> 0), the unbounded passes on
+ * the mask, and a store that keeps the maximum (d2_r <= B -- the rule of the bounded transforms' cut, so
+ * equal to them bit for bit).  Device memory beyond the labels and out: 9 bytes per voxel (D2, the mask,
+ * its distances), label_bytes more with EDTB200_LABELS_FLOAT, 12 bytes per default level and volume plus 4
+ * per volume, the staged levels of a host sizes_out, and the edtsq's own scratch where its plan takes it.
+ * Checks, in order: label width, ndim, sizes (as edtb200_transform), count >= 0, weights, nsizes, each
+ * radius (finite, >= 0), flags, EDTB200_LABELS_FLOAT width, the stack's size (within 2^62 voxels),
+ * emptiness (returns 0 touching nothing), pointers (labels, out) and overlap (out with labels on the same
+ * side; sizes_out with out, and with labels on the same side), device.  EDT_B200_VERBOSE=1 prints the
+ * device time of the edtsq and of the levels on stderr. */
+#define EDTB200_THICKNESS_MAX_SIZES 4096
+int edtb200_local_thickness(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                            int64_t count, float wx, float wy, float wz, int black_border, int flags,
+                            const double *sizes, int nsizes, float *out, double *sizes_out,
+                            int device, void *stream);
 
 /* Parabolic erosion and dilation of float volumes: the distance transform of a sampled function
  * (Felzenszwalb-Huttenlocher), ITK's ParabolicErode / DilateImageFilter.  Volumes are x-fastest, as

@@ -294,20 +294,45 @@ struct XPlanes {
   float ty, tz;
 };
 
-// A lane's 4-bit nibble of a 128-voxel block (voxels 4 lane .. 4 lane + 3) -> the block's 32-bit
-// word that holds it, in natural x order: word w of the block ends up in lanes 8w .. 8w + 7.
-__device__ __forceinline__ uint32_t nibbles_to_word(uint32_t nib, int lane) {
-  uint32_t v = nib << (4 * (lane & 7));
-  v |= __shfl_xor_sync(0xffffffffu, v, 1);
-  v |= __shfl_xor_sync(0xffffffffu, v, 2);
-  v |= __shfl_xor_sync(0xffffffffu, v, 4);
-  return v;
+// Bit i of the low byte of x -> bit 4 i.
+__device__ __forceinline__ uint32_t spread_nibble_bits(uint32_t x) {
+  x &= 0xffu;
+  x = (x | (x << 12)) & 0x000f000fu;
+  x = (x | (x << 6)) & 0x03030303u;
+  return (x | (x << 3)) & 0x11111111u;
 }
 
-// One row of the register-resident X kernels, from its labels to its distances at dst: the lane's
-// labels v (voxels 128 b + 4 lane .. + 3 of block b; load(q0, v[b]) fetches the four at q0, zeros
-// past sx), run-start / background masks, nearest boundaries, table lookups from table_s (T[0..sx],
-// +inf at sx + 1) and float4 stores.  Adds the row's label changes along x to the lane's nstarts.
+// The run-start words of one row of at most 512 voxels, in natural x order, from every lane's nibbles
+// (bits 4 b .. 4 b + 3 of the y plane, 16 + 4 b .. of the z plane: its voxels 128 b + 4 lane .. + 3 of
+// block b): lane c = 4 b + w gets word c, which holds nibble b of lanes 8 w .. 8 w + 7.  One shuffle
+// per source lane serves both planes.
+__device__ __forceinline__ void gather_plane_words(uint32_t nibs, int lane, uint32_t& word_y, uint32_t& word_z) {
+  const int src = (lane & 3) << 3, sh = lane & 12;   // sh = 4 b for lanes 0 .. 15 (the rest store nothing)
+  word_y = word_z = 0u;
+#pragma unroll
+  for (int l = 0; l < 8; ++l) {
+    const uint32_t g = __shfl_sync(0xffffffffu, nibs, src + l) >> sh;
+    const uint32_t at = 15u << (4 * l);
+    word_y |= (g << (4 * l)) & at;
+    word_z |= (l < 4 ? g >> (16 - 4 * l) : g << (4 * l - 16)) & at;
+  }
+}
+
+// The lane's labels of one row for the register-resident X kernels: v[b] = voxels 128 b + 4 lane .. + 3
+// of block b, which load(q0, v[b]) fetches from q0; zeros past sx.
+template <int Bytes, int K, class Load>
+__device__ __forceinline__ void load_vec_row(Load load, int sx, int lane, typename LabelOf<Bytes>::wide v[K][4]) {
+#pragma unroll
+  for (int b = 0; b < K; ++b) {
+    const int q0 = (b << 7) + (lane << 2);
+    if (q0 < sx) load(q0, v[b]);
+    else { v[b][0] = v[b][1] = v[b][2] = v[b][3] = 0; }
+  }
+}
+
+// One row of the register-resident X kernels, from the lane's labels v (load_vec_row) to its
+// distances at dst: run-start / background masks, nearest boundaries, table lookups from table_s
+// (T[0..sx], +inf at sx + 1) and float4 stores.  Adds the row's label changes along x to the lane's nstarts.
 // Plain = true: squared EDT, background forced to 0, no sqrt / sign (the hot configuration);
 // Plain = false: behaviour selected by `flags` at run time.
 // Settled = true (first_axis_planes_kernel only): also clears bit b of set_y / set_z where a value
@@ -315,23 +340,17 @@ __device__ __forceinline__ uint32_t nibbles_to_word(uint32_t nib, int lane) {
 // OneRowY = true (first_axis_planes_kernel only): stores min(f, ty) for the voxels marked in one_row
 // (4 bits per block, like the masks below), before the settled compare: the voxels whose y-run is
 // one row long, which the Y pass would bring to exactly that value (DESIGN.md section 4.1).
-template <int Bytes, int K, bool Plain, bool Settled = false, bool OneRowY = false, class Load>
-__device__ __forceinline__ void first_axis_vec_row(Load load, float* __restrict__ dst, int sx, const float* table_s,
-                                                   int border, int flags, bool keep_background, int lane,
-                                                   unsigned lt_mask, unsigned gt_mask, unsigned int& nstarts,
-                                                   float ty = 0.0f, float tz = 0.0f, uint32_t* set_y = nullptr,
-                                                   uint32_t* set_z = nullptr, uint32_t one_row = 0u) {
+template <int Bytes, int K, bool Plain, bool Settled = false, bool OneRowY = false>
+__device__ __forceinline__ void first_axis_vec_row(const typename LabelOf<Bytes>::wide v[K][4], float* __restrict__ dst,
+                                                   int sx, const float* table_s, int border, int flags,
+                                                   bool keep_background, int lane, unsigned lt_mask, unsigned gt_mask,
+                                                   unsigned int& nstarts, float ty = 0.0f, float tz = 0.0f,
+                                                   uint32_t* set_y = nullptr, uint32_t* set_z = nullptr,
+                                                   uint32_t one_row = 0u) {
   using WT = typename LabelOf<Bytes>::wide;
   const unsigned full = 0xffffffffu;
 
   // ---- labels -> per-block 4-bit "label changes here" / "is background" masks ----
-  WT v[K][4];
-#pragma unroll
-  for (int b = 0; b < K; ++b) {
-    const int q0 = (b << 7) + (lane << 2);
-    if (q0 < sx) load(q0, v[b]);
-    else { v[b][0] = v[b][1] = v[b][2] = v[b][3] = 0; }
-  }
   uint32_t edges = 0, zeros = 0;                   // 4 bits per block
   uint32_t occ[K];                                 // lanes owning at least one boundary
 #pragma unroll
@@ -463,8 +482,10 @@ first_axis_vec_kernel(const typename LabelOf<Bytes>::type* __restrict__ labels,
   for (int64_t line = (int64_t)blockIdx.x * warps + warp; line < nlines; line += step) {
     const LT* __restrict__ src = labels + line * sx;
     float* __restrict__ dst = out + line * sx;
-    first_axis_vec_row<Bytes, K, Plain>([&](int q0, WT* v) { Vec4Labels<Bytes>::load(src + q0, v); }, dst, sx,
-                                        table_s, border, flags, keep_background, lane, lt_mask, gt_mask, nstarts);
+    WT v[K][4];
+    load_vec_row<Bytes, K>([&](int q0, WT* r) { Vec4Labels<Bytes>::load(src + q0, r); }, sx, lane, v);
+    first_axis_vec_row<Bytes, K, Plain>(v, dst, sx, table_s, border, flags, keep_background, lane, lt_mask, gt_mask,
+                                        nstarts);
   }
   if (stat.counter) {
 #pragma unroll
@@ -727,6 +748,7 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
                          const float* __restrict__ table, int border, int flags, RunStat stat, XPlanes planes,
                          int nchunks) {
   static_assert(Bytes >= 4 && Planes >= 1 && Planes <= 2, "the bulk copies need 16-byte label rows");
+  static_assert(K <= 4, "a lane's nibbles of both planes share one word (gather_plane_words)");
   using LT = typename LabelOf<Bytes>::type;
   using WT = typename LabelOf<Bytes>::wide;
   constexpr int W = kPlaneWarps, S = planes_stages(Bytes);
@@ -812,6 +834,9 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
         if (y <= ylast) {
           const LT* cur = ring + slot * stage_labels + (warp + 1) * sx;
           const LT* next = ring + next_slot * stage_labels + (warp + 1) * sx;
+          // row y's labels, read from the stage once for all three compares and the distances
+          WT v[K][4];
+          load_vec_row<Bytes, K>([&](int q0, WT* r) { load4_shared<Bytes>(cur + q0, r); }, sx, lane, v);
           // ---- y-runs that start at row y + 1, 4 bits per block (the line end counts; row -1 stands
           // for the line's start, so row 0 gets all bits) ----
           uint32_t ynext = in_row;
@@ -821,67 +846,49 @@ first_axis_planes_kernel(const typename LabelOf<Bytes>::type* __restrict__ label
             for (int b = 0; b < K; ++b) {
               const int q0 = (b << 7) + (lane << 2);
               if (q0 >= sx) continue;
-              WT here[4], u[4];
-              load4_shared<Bytes>(cur + q0, here);
+              WT u[4];
               load4_shared<Bytes>(next + q0, u);
-              ynext |= label_changes<WT>(here, u) << (4 * b);
+              ynext |= label_changes<WT>(v[b], u) << (4 * b);
             }
           }
           if (y >= me.ya) {                          // not the leading row: this row's outputs
             const int64_t line = (int64_t)me.z * sy + y;
+            // ---- z-runs that start at row y: compare with the stage's row of slice z - 1 (a first slice
+            // of a volume: all start) ----
+            uint32_t zstart = in_row;
+            if (Planes == 2 && !zfirst) {
+              const LT* below = cur - sx;
+              zstart = 0u;
+#pragma unroll
+              for (int b = 0; b < K; ++b) {
+                const int q0 = (b << 7) + (lane << 2);
+                if (q0 >= sx) continue;
+                WT u[4];
+                load4_shared<Bytes>(below + q0, u);
+                zstart |= label_changes<WT>(u, v[b]) << (4 * b);
+              }
+            }
             const uint32_t one_row = sy > 1 ? (ystart & ynext) : 0u;   // lines of one row have no border term
             uint32_t set_y = 0xffffffffu, set_z = 0xffffffffu;
-            first_axis_vec_row<Bytes, K, Plain, true, true>([&](int q0, WT* v) { load4_shared<Bytes>(cur + q0, v); },
-                                                            out + line * sx, sx, table_s, border, flags,
+            first_axis_vec_row<Bytes, K, Plain, true, true>(v, out + line * sx, sx, table_s, border, flags,
                                                             keep_background, lane, lt_mask, gt_mask, nstarts,
                                                             planes.ty, planes.tz, &set_y, &set_z, one_row);
-            // ---- settled planes: segment 4 b + w of the row is lanes 8 w .. 8 w + 7 of block b ----
-            uint32_t seg_y = 0u, seg_z = 0u;
-#pragma unroll
-            for (int b = 0; b < K; ++b) {
-              uint32_t v = __ballot_sync(full, (set_y >> b) & 1u);
-              v &= v >> 4; v &= v >> 2; v &= v >> 1;             // bit 8 w: all of lanes 8 w .. 8 w + 7
-              seg_y |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
-              if (Planes == 2) {
-                v = __ballot_sync(full, (set_z >> b) & 1u);
-                v &= v >> 4; v &= v >> 2; v &= v >> 1;
-                seg_z |= ((v & 1u) | ((v >> 7) & 2u) | ((v >> 14) & 4u) | ((v >> 21) & 8u)) << (4 * b);
-              }
-            }
+            // ---- settled planes: segment 4 b + w of the row is lanes 8 w .. 8 w + 7 of block b.  The lane's
+            // unsettled blocks (y in bits 0 .. 3, z in 4 .. 7) go to bits 4 b + w (y) and 16 + 4 b + w (z);
+            // one OR over the warp gives the segments that hold an unsettled voxel ----
+            const uint32_t open = ~(set_y & 15u | (set_z & 15u) << 4) & 0xffu;
+            const uint32_t open_seg = __reduce_or_sync(full, spread_nibble_bits(open) << (lane >> 3));
             if (lane == 0) {
-              planes.settled_y[line] = seg_y | (0xffffffffu << (4 * K));
-              if (Planes == 2) planes.settled_z[line] = seg_z | (0xffffffffu << (4 * K));
+              planes.settled_y[line] = ~open_seg | 0xffff0000u;
+              if (Planes == 2) planes.settled_z[line] = ~(open_seg >> 16);
             }
-            // ---- run-start planes: the y nibbles from ystart, the z ones compare with the stage's row
-            // of slice z - 1; one nibble per lane and block -> the row's wpr words, word c in lane c,
-            // stored by one instruction per plane ----
-            const LT* below = cur - sx;
-            uint32_t word[Planes] = {};
-#pragma unroll
-            for (int b = 0; b < K; ++b) {
-              const int q0 = (b << 7) + (lane << 2);
-              uint32_t nibs[Planes];
-              nibs[0] = (ystart >> (4 * b)) & 15u;
-              if (Planes == 2) {
-                nibs[Planes - 1] = (in_row >> (4 * b)) & 15u;     // first slice of a volume: all start
-                if (q0 < sx && !zfirst) {
-                  WT here[4], u[4];
-                  load4_shared<Bytes>(cur + q0, here);
-                  load4_shared<Bytes>(below + q0, u);
-                  nibs[Planes - 1] = label_changes<WT>(u, here);
-                }
-              }
-#pragma unroll
-              for (int a = 0; a < Planes; ++a) {
-                const uint32_t nib = nibs[a];
-                // word w of block b sits in lanes 8w .. 8w + 7; lane c takes word c = 4 b + w
-                const uint32_t got = __shfl_sync(full, nibbles_to_word(nib, lane), (lane & 3) << 3);
-                if ((lane >> 2) == b) word[a] = got;
-              }
-            }
+            // ---- run-start planes: the y nibbles from ystart, the z ones from zstart -> the row's wpr
+            // words, word c in lane c, stored by one instruction per plane ----
+            uint32_t word_y, word_z;
+            gather_plane_words(ystart | zstart << 16, lane, word_y, word_z);
             if (lane < wpr) {
-              planes.y[line * wpr + lane] = word[0];
-              if (Planes == 2) planes.z[line * wpr + lane] = word[Planes - 1];
+              planes.y[line * wpr + lane] = word_y;
+              if (Planes == 2) planes.z[line * wpr + lane] = word_z;
             }
           }
           ystart = ynext;

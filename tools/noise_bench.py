@@ -2,8 +2,10 @@
 """Device times of the 512^3 label-noise edtsq (iid labels 0..255, anisotropy (1, 1, 1), no black
 border: the bench.py workload) for labels of 4 and 8 bytes, whole transform and per pass (GPU only):
 
-  python tools/noise_bench.py [--size 512] [--steps 20] [--reps 3] [--anisotropy 1,0.7,1]
+  python tools/noise_bench.py [--size 512] [--steps 20] [--reps 3] [--anisotropy 1,0.7,1] [--image 262144,512]
                               (EDTB200_LIBRARY=... for another build)
+
+--image SY,SX times an SY x SX image of the same label noise instead (the Z pass time reads 0).
 
 --anisotropy (array order) picks other weights: with a non-integer one the later passes read their
 run-start planes without skipping settled tiles.
@@ -43,15 +45,17 @@ def main():
   ap.add_argument("--size", type=int, default=512)
   ap.add_argument("--steps", type=int, default=20)
   ap.add_argument("--reps", type=int, default=3)
-  ap.add_argument("--anisotropy", type=lambda v: tuple(float(x) for x in v.split(",")), default=(1.0, 1.0, 1.0))
+  ap.add_argument("--anisotropy", type=lambda v: tuple(float(x) for x in v.split(",")), default=None)
+  ap.add_argument("--image", type=lambda v: tuple(int(x) for x in v.split(",")), default=None,
+                  help="SY,SX: a 2-D image instead of the 3-D volume")
   args = ap.parse_args()
-  w = args.anisotropy
+  shape = args.image or (args.size,) * 3
+  w = args.anisotropy or (1.0,) * len(shape)
   dev = torch.device("cuda", 0)
   lib = edt._lib()
-  n = args.size
   g = torch.Generator(device=dev)
   g.manual_seed(0)
-  base = torch.randint(0, 256, (n, n, n), dtype=torch.int32, device=dev, generator=g)
+  base = torch.randint(0, 256, shape, dtype=torch.int32, device=dev, generator=g)
   print(json.dumps({"card": card(), "library": os.path.basename(edt.library_path())}), flush=True)
   for dtype in (torch.int32, torch.int64):
     lab = base.to(dtype)
@@ -80,7 +84,7 @@ def main():
           raise RuntimeError("edtb200_pass_ms failed")
         smp.append([float(v) for v in buf])
       passes.append([statistics.mean(s[i] for s in smp) for i in range(3)])
-    print(json.dumps({"label_bytes": lab.element_size(), "size": n, "anisotropy": w, "steps": args.steps,
+    print(json.dumps({"label_bytes": lab.element_size(), "shape": list(shape), "anisotropy": w, "steps": args.steps,
                       "ms": [round(t, 4) for t in totals], "ms_median": round(statistics.median(totals), 4),
                       "pass_ms_xyz": [[round(v, 4) for v in p] for p in passes], "clocks": card()}), flush=True)
     del lab, out

@@ -39,7 +39,7 @@ __all__ = [
   "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
   "parabolic_erode", "parabolic_dilate", "nearest_labels", "medial_axis",
-  "skeletonize", "local_thickness",
+  "skeletonize", "local_thickness", "geodesic_distance",
 ]
 
 FLAG_SQRT = 1
@@ -133,6 +133,8 @@ def _lib():
   lib.edtb200_medial_axis.restype = ci
   lib.edtb200_skeletonize.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, vp, vp, ci, vp]
   lib.edtb200_skeletonize.restype = ci
+  lib.edtb200_geodesic.argtypes = [vp, ci, vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, vp, vp, ci, vp]
+  lib.edtb200_geodesic.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1584,6 +1586,112 @@ def skeletonize(labels, anisotropy=None, black_border=False, *, return_distance=
     _check(_lib().edtb200_skeletonize(v.ptr, nbytes, *v.geometry, int(bool(black_border)), v.flags, v.ptr_of(skel),
                                       v.ptr_of(dist), *v.where))
   return (skel, dist) if return_distance else skel
+
+
+# ---------------------------------------------------------------------------------------
+# shortest-path distances inside each label from seed voxels (edtb200_geodesic)
+# ---------------------------------------------------------------------------------------
+
+def _integer_bytes(dtype, what):
+  """Width of a numpy or torch bool / integer dtype of 1, 2, 4 or 8 bytes; TypeError for anything else."""
+  try:
+    return _nearest_label_bytes(dtype)
+  except TypeError:
+    raise TypeError("geodesic_distance: unsupported %s dtype %s: it must be an integer or bool dtype"
+                    % (what, dtype)) from None
+
+
+def geodesic_distance(labels, seeds, anisotropy=None, *, return_indices=False, stacked=False, device=0):
+  """Geodesic distance: the length of the shortest path from a seed to each voxel that stays inside the
+  voxel's own label, on the GPU.
+
+  Definition.  Volumes are x-fastest, as for edt(): x is the last axis of a C-ordered array and the first of
+  an F-ordered one; coordinates are taken within one volume.
+    graph     every voxel with a non-zero label is a node; two nodes are joined when they are 26-neighbours
+              (2-D: 8, 1-D: 2) with the same label.  Label 0 and the outside of the volume cannot be crossed
+              (there is no black_border).  A step (dx, dy, dz), each in {-1, 0, 1}, has the length
+              sqrt((dx*wx)^2 + (dy*wy)^2 + (dz*wz)^2): each weight rounded to float32 (as the C ABI takes
+              it) and promoted to double, the squares summed in double in the order x, y, z, the square root
+              correctly rounded.
+    seeds     a voxel is a seed when its seed value and its label are both non-zero; seeds on background are
+              ignored.
+    distance  D is the least fixed point of D[v] = min(D[v], fl64(D[u] + w(u, v))) over the graph neighbours
+              u of v, from 0 on the seeds and +inf elsewhere -- exactly what Dijkstra computes in double
+              (scipy.sparse.csgraph.dijkstra(G, indices=seeds, min_only=True) on this graph).  The result is
+              float32(D), rounded once to nearest; label-0 voxels and voxels with no seed in their component
+              are +inf.
+    indices   with return_indices=True, S[v] is the least linear seed index c (x-fastest within the volume)
+              with a tight path c = u0 .. uk = v, every step satisfying D[u_{i+1}] == fl64(D[u_i] + w): the
+              seed v is reached from first, ties going to the least index, independent of any evaluation order.
+  The result equals this definition bit for bit on every run.
+
+  Examples.  A straight corridor: D is the number of steps times the step's weight,
+      labels = np.zeros((3, 9), np.uint8); labels[1, 1:8] = 1
+      seeds = np.zeros((3, 9), bool); seeds[1, 1] = True
+      geodesic_distance(labels, seeds, (1.0, 0.5))[1, 1:8]  ->  [0, 0.5, 1, 1.5, 2, 2.5, 3]
+  and +inf everywhere off the corridor.  An L-shaped corridor, where D is larger than the edt:
+      labels = np.zeros((5, 5), np.uint8); labels[0, :] = 1; labels[:, 4] = 1
+      seeds = np.zeros((5, 5), bool); seeds[0, 0] = True
+      geodesic_distance(labels, seeds)[4, 4]  ->  np.float32(6 + np.sqrt(2)) = 7.4142137,
+  three steps along the top, one diagonal step across the corner and three down, where the straight line
+  is sqrt(32) = 5.656854.
+  Seed splitting of touching objects: every voxel of a mask gets the marker it reaches first without
+  leaving the mask (-1 indices, where no marker is reachable, masked to 0):
+      dist, idx = geodesic_distance(mask, markers != 0, return_indices=True)
+      split = np.where(idx[0] >= 0, markers[tuple(idx)], 0)
+
+  Input and output.  `labels`: bool or integer dtypes of 1, 2, 4 or 8 bytes (float labels are a TypeError),
+  1-D to 3-D, or with stacked=True 2-D to 4-D whose slowest axis in memory indexes same-shaped volumes, as
+  edt(stacked=True); the result equals np.stack of the per-volume calls.  `seeds`: bool or integer dtypes (a
+  TypeError otherwise) of the labels' shape (a ValueError otherwise); it is read in the labels' memory
+  order, copied into it where its own differs, and moved to the labels' GPU when they are device-resident.
+  `anisotropy`: one weight per volume axis, each finite and > 0 (a ValueError otherwise).  Returns `dist`,
+  float32 with the input's shape and memory order, or with return_indices=True `(dist, indices)`, indices
+  int32 of shape (vnd,) + labels.shape in scipy's return_indices layout (indices[k] is the coordinate along
+  array axis k, each plane in the input's memory order, within each voxel's own volume for a stack), as
+  feature_transform returns them, -1 in every plane where dist is +inf.  numpy in gives numpy out; a torch
+  CUDA tensor (or any __cuda_array_interface__ array) gives torch CUDA tensors computed on the current stream
+  without a host synchronisation: each phase is one cooperative kernel.  A host array that does not fit on
+  the GPU raises EDTError with code ENOMEM (there is no chunked path).
+
+  Cost.  The GPU relaxes 8x8x8 tiles (2-D 16x16, 1-D 256) in rounds, each round re-relaxing the tiles whose
+  halo changed; the number of rounds grows with how often shortest paths turn across tile boundaries -- a
+  handful for a convex object, thousands for a maze.  Device memory beyond the input and the outputs: 8 bytes
+  per voxel for D, 8 more with return_indices, and 12 bytes per tile."""
+  name = "geodesic_distance"
+  if not isinstance(return_indices, (bool, np.bool_)):
+    raise TypeError("%s: return_indices must be True or False, got %r" % (name, return_indices))
+  v = _Volume(name, labels, stacked, (1, 3), device)
+  nbytes = _integer_bytes(v.dtype, "label")
+  sd = _device_array(seeds)
+  if v.on_device:
+    import torch
+    sd = torch.as_tensor(seeds if sd is None else sd, device=v.arr.device)
+  elif sd is not None:
+    raise TypeError("%s: seeds are a GPU array but labels are a host array; pass both on the same side" % name)
+  else:
+    sd = np.asarray(seeds)
+  seed_bytes = _integer_bytes(sd.dtype, "seed")
+  if tuple(sd.shape) != v.shape:
+    raise ValueError("%s: seeds must have the labels' shape %s, got %s" % (name, v.shape, tuple(sd.shape)))
+  v.set_weights(anisotropy)
+  # the seeds in the labels' memory order
+  if not v.on_device:
+    sd = np.asfortranarray(sd) if v.fortran else np.ascontiguousarray(sd)
+  elif v.fortran:
+    back = tuple(range(v.nd - 1, -1, -1))
+    sd = sd.permute(*back).contiguous().permute(*back)
+  else:
+    sd = sd.contiguous()
+  dist = v.empty("float32")
+  planes = v.empty("int32", planes=v.vnd) if return_indices else None
+  if v.size:
+    ptrs = v.plane_ptrs(planes) if return_indices else None
+    _check(_lib().edtb200_geodesic(v.ptr, nbytes, v.ptr_of(sd), seed_bytes, *v.geometry, v.flags, v.ptr_of(dist),
+                                   ptrs, *v.where))
+  if not return_indices:
+    return dist
+  return dist, planes
 
 
 # ---------------------------------------------------------------------------------------

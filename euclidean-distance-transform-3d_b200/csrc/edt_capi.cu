@@ -2166,6 +2166,113 @@ int edtb200_skeletonize(const void* labels, int label_bytes, int ndim, int64_t s
   return rc ? rc : io.finish();
 }
 
+int edtb200_geodesic(const void* labels, int label_bytes, const void* seeds, int seed_bytes, int ndim, int64_t sx,
+                     int64_t sy, int64_t sz, int64_t count, float wx, float wy, float wz, int flags, float* dist_out,
+                     int32_t* const* idx_out, int device, void* stream_v) {
+  if (!(label_bytes == 1 || label_bytes == 2 || label_bytes == 4 || label_bytes == 8))
+    return fail(EDTB200_EINVAL, "label_bytes must be 1, 2, 4 or 8 (got %d)", label_bytes);
+  if (!(seed_bytes == 1 || seed_bytes == 2 || seed_bytes == 4 || seed_bytes == 8))
+    return fail(EDTB200_EINVAL, "seed_bytes must be 1, 2, 4 or 8 (got %d)", seed_bytes);
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  const float w[3] = {wx, wy, wz};
+  if ((rc = check_weights(ndim, w))) return rc;
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_geodesic takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if ((rc = check_stack(vol, count, 1))) return rc;
+  // the worklists hold 4-byte tile numbers
+  const int64_t ntiles = geodesic_tiles(ndim, sx, sy, sz, count);
+  if (ntiles >= ((int64_t)1 << 32)) return fail(EDTB200_ELIMIT, "edtb200_geodesic takes stacks of fewer than 2^32 tiles");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !seeds || !dist_out) return fail(EDTB200_EINVAL, "null pointer");
+  if (idx_out)
+    for (int k = 0; k < ndim; ++k)
+      if (!idx_out[k]) return fail(EDTB200_EINVAL, "null index plane %d", k);
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, seed_size = (size_t)total * (size_t)seed_bytes;
+  const size_t dist_bytes = sizeof(float) * (size_t)total, plane_bytes = sizeof(int32_t) * (size_t)total;
+  // outputs against the inputs (on the same side) and against each other
+  const void* outs[4] = {dist_out, idx_out ? idx_out[0] : nullptr, idx_out && ndim > 1 ? idx_out[1] : nullptr,
+                         idx_out && ndim > 2 ? idx_out[2] : nullptr};
+  const size_t out_bytes[4] = {dist_bytes, plane_bytes, plane_bytes, plane_bytes};
+  static const char* names[4] = {"dist_out", "index plane 0", "index plane 1", "index plane 2"};
+  for (int i = 0; i < 4; ++i) {
+    if (!outs[i]) continue;
+    if (same_side(flags) && overlaps(labels, lab_bytes, outs[i], out_bytes[i]))
+      return fail(EDTB200_EINVAL, "%s overlaps labels", names[i]);
+    if (same_side(flags) && overlaps(seeds, seed_size, outs[i], out_bytes[i]))
+      return fail(EDTB200_EINVAL, "%s overlaps seeds", names[i]);
+    for (int j = 0; j < i; ++j)
+      if (outs[j] && overlaps(outs[j], out_bytes[j], outs[i], out_bytes[i]))
+        return fail(EDTB200_EINVAL, "%s overlaps %s", names[i], names[j]);
+  }
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  // host buffers are staged whole: the labels and distances through this device's cached buffers, the
+  // seeds and index planes through scratch
+  const void* d_labels = nullptr;
+  const void* d_seeds = nullptr;
+  float* d_dist = nullptr;
+  int32_t* d_planes[3] = {nullptr, nullptr, nullptr};
+  Scratch seed_stage, plane_stage[3], values, indices, tiles;
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) || (rc = io.out_dist(dist_out, dist_bytes, &d_dist)))
+    return rc;
+  if (!io.in_dev && (rc = seed_stage.take(*io.dc, seed_size, s, "the staged seeds"))) return rc;
+  if ((rc = io.in(seeds, seed_size, seed_stage.get(), &d_seeds))) return rc;
+  for (int k = 0; idx_out && k < ndim; ++k)
+    if ((rc = io.out_staged(idx_out[k], plane_bytes, plane_stage[k], "the index planes", &d_planes[k]))) return rc;
+  // scratch: D, S with indices, one flag and two list entries per tile, and the two control blocks
+  GeodesicScratch g;
+  g.ntiles = ntiles;
+  const size_t tile_bytes = 3 * sizeof(uint32_t) * (size_t)ntiles, d_bytes = sizeof(double) * (size_t)total;
+  const size_t s_bytes = idx_out ? sizeof(unsigned long long) * (size_t)total : 0;
+  if ((rc = values.take(*io.dc, d_bytes, s, "the geodesic distances")) ||
+      (idx_out && (rc = indices.take(*io.dc, s_bytes, s, "the geodesic seed indices"))) ||
+      (rc = tiles.take(*io.dc, tile_bytes + geodesic_control_bytes(), s, "the geodesic worklists")))
+    return rc;
+  g.d = values.get<double>();
+  g.s = indices.get<unsigned long long>();
+  // the control blocks first: they hold 8-byte counters, and 3 * ntiles words may end off an 8-byte boundary
+  g.control = tiles.get();
+  g.flag = reinterpret_cast<uint32_t*>(tiles.get<char>() + geodesic_control_bytes());
+  g.list = g.flag + ntiles;
+  // the step lengths: each weight promoted to double, the squares summed in the order x, y, z, sqrt
+  double step[8] = {0.0};
+  for (int m = 1; m < 8; ++m) {
+    double sum = 0.0;
+    for (int k = 0; k < 3; ++k)
+      if (m >> k & 1) sum += (double)w[k] * (double)w[k];
+    step[m] = std::sqrt(sum);
+  }
+
+  // steps: the distances, the indices, the store
+  StepTimer timer(s);
+  timer.stamp();
+  rc = launch_geodesic_phase(d_labels, label_bytes, d_seeds, seed_bytes, ndim, sx, sy, sz, count, step, g, false,
+                             *io.dc, s);
+  timer.stamp();
+  if (!rc && idx_out)
+    rc = launch_geodesic_phase(d_labels, label_bytes, d_seeds, seed_bytes, ndim, sx, sy, sz, count, step, g, true,
+                               *io.dc, s);
+  timer.stamp();
+  if (!rc) rc = launch_geodesic_store(ndim, sx, sy, sz, count, g, d_dist, idx_out ? d_planes : nullptr, *io.dc, s);
+  timer.stamp();
+  if (!rc && timer.synchronize()) {
+    unsigned long long n[4] = {0, 0, 0, 0};
+    geodesic_stats(g.control, n);
+    fprintf(stderr, "[edt_b200] geodesic %lldx%lldx%lld x%lld L=%d  distances %.3f ms (rounds %llu, tile visits %llu)  "
+                    "indices %.3f ms (rounds %llu, tile visits %llu)  store %.3f ms  tiles %lld  scratch %zu bytes\n",
+            (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, timer.ms(0, 1), n[0], n[1],
+            timer.ms(1, 2), n[2], n[3], timer.ms(2, 3), (long long)ntiles,
+            d_bytes + s_bytes + tile_bytes + geodesic_control_bytes());
+  }
+  return rc ? rc : io.finish();
+}
+
 // The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
 static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
                           const float w[3], int k, double max_distance) {

@@ -1,14 +1,15 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as fourteen translation units so that the kernel templates build in
+// The library is compiled as fifteen translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
 // transforms' kernels), edt_surface.cu (the surface distances' kernels), edt_morphology.cu (the
 // spherical morphology's label-writing stores), edt_parabolic.cu (the parabolic erosion and
 // dilation passes), edt_nearest.cu (the nearest-labels passes), edt_medial.cu (the medial
-// axis's mark kernel), edt_skeleton.cu (the skeleton's thinning kernel) and edt_thickness.cu
-// (local thickness's levels, seeds and stores).  The run-time label width
+// axis's mark kernel), edt_skeleton.cu (the skeleton's thinning kernel), edt_thickness.cu
+// (local thickness's levels, seeds and stores) and edt_geodesic.cu (geodesic_distance's relaxation
+// passes).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -437,6 +438,33 @@ int launch_skeleton_thin(const void* labels, int label_bytes, int ndim, int64_t 
 size_t skeleton_control_bytes();
 // The rounds, cycles and steps of the last thinning on `control` (synchronous copy).
 int skeleton_stats(const void* control, unsigned long long out[3]);
+
+// The scratch of geodesic_distance (edt_geodesic.cu): D (one double per voxel), S (one 8-byte index per
+// voxel, with indices), one flag per tile, two worklists of `ntiles` 4-byte entries and the control blocks of
+// the two phases (geodesic_control_bytes()).
+struct GeodesicScratch {
+  double* d = nullptr;
+  unsigned long long* s = nullptr;
+  uint32_t* flag = nullptr;
+  uint32_t* list = nullptr;
+  void* control = nullptr;
+  int64_t ntiles = 0;
+};
+
+// The tiles of `count` volumes of (sx, sy, sz) (3-D 8x8x8, 2-D 16x16, 1-D 256 voxels each).
+int64_t geodesic_tiles(int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count);
+// One phase of geodesic_distance (edt_geodesic.cu): its seed kernel, then ONE cooperative launch of
+// geodesic_relax_kernel that runs every round.  index false: D from the seeds; true: S over the tight edges
+// of the fixed D.  step[|dx| | |dy| << 1 | |dz| << 2]: the step lengths the host formed.
+int launch_geodesic_phase(const void* labels, int label_bytes, const void* seeds, int seed_bytes, int ndim,
+                          int64_t sx, int64_t sy, int64_t sz, int64_t count, const double step[8],
+                          const GeodesicScratch& g, bool index, DeviceCache& dc, cudaStream_t stream);
+// float32(D) into dist and, with planes (null: none), S as int32 coordinate planes within each volume.
+int launch_geodesic_store(int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, const GeodesicScratch& g,
+                          float* dist, int32_t* const planes[3], DeviceCache& dc, cudaStream_t stream);
+size_t geodesic_control_bytes();
+// The rounds and tile visits of the distance and index phases of the last call on `control` (synchronous).
+int geodesic_stats(const void* control, unsigned long long out[4]);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

@@ -38,7 +38,8 @@ extern "C" {
  * edtb200_transform_voxel_graph_chunked, edtb200_transform_stack, edtb200_feature_transform_stack,
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
- * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness)
+ * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness,
+ * edtb200_geodesic)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -487,6 +488,66 @@ int edtb200_medial_axis(const void *labels, int label_bytes, int ndim, int64_t s
 int edtb200_skeletonize(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
                         int64_t count, float wx, float wy, float wz, int black_border, int flags,
                         uint8_t *skeleton_out, float *dist_out, int device, void *stream);
+
+/* Geodesic distance: the length of the shortest path from a seed to each voxel that stays inside the
+ * voxel's own label (connectomics path lengths, seed splitting of touching objects, geodesic maps from clicks,
+ * tortuosity).  Volumes are x-fastest, as everywhere here; coordinates are taken within one volume.
+ *   graph     every voxel with a non-zero label is a node; two nodes are joined when they are 26-neighbours
+ *             (2-D: 8, 1-D: 2) with the SAME label.  Label 0 and the outside of the volume cannot be crossed
+ *             (there is no black_border).  A step (dx, dy, dz), each in {-1, 0, 1}, has the length
+ *             w = sqrt((dx*wx)^2 + (dy*wy)^2 + (dz*wz)^2): each (float) weight promoted to double, the squares summed
+ *             in double in the order x, y, z, the square root correctly rounded.  The host forms the 7
+ *             distinct lengths (one per non-zero (|dx|, |dy|, |dz|)) once; no device code forms a weight.
+ *   seeds     a voxel is a seed when its seed value AND its label are non-zero (seeds on background are
+ *             ignored).
+ *   distance  D is the least fixed point of D[v] = min(D[v], fl64(D[u] + w(u, v))) over the graph neighbours u
+ *             of v, from D = 0 on the seeds and +inf elsewhere -- what Dijkstra computes in double.  dist_out
+ *             = float32(D), rounded once to nearest; label-0 voxels and voxels with no seed in their component
+ *             get +inf.
+ *   indices   S[v] is the least linear seed index c (x-fastest within the volume) with a TIGHT path c = u0 ..
+ *             uk = v: every step has D[u_{i+1}] == fl64(D[u_i] + w).  Deterministic, independent of the order of
+ *             evaluation.  idx_out holds S as ndim int32 coordinate planes laid out like the labels (idx_out[0]
+ *             the x coordinate, idx_out[1] y, idx_out[2] z), -1 in every plane where D is +inf.
+ * Examples: along a straight one-voxel corridor D is the number of steps times its axis weight; in an
+ * L-shaped corridor D at the far end is the sum of both legs, larger than the edt's straight line.
+ *
+ *   labels, label_bytes  count * sx*sy*sz labels of 1, 2, 4 or 8 bytes (integers: compared by their bits),
+ *                        volumes back to back as for edtb200_transform_stack (count 1: one volume)
+ *   seeds, seed_bytes    count * sx*sy*sz values of 1, 2, 4 or 8 bytes, laid out like the labels and on the
+ *                        same side (EDTB200_LABELS_ON_DEVICE covers both)
+ *   wx..wz               the weights of the first ndim axes: finite and > 0
+ *   flags                the residency flags only (both on the device: asynchronous on `stream`, no lock and
+ *                        no host wait; host buffers are staged whole, EDTB200_ENOMEM when they do not fit --
+ *                        there is no chunked path)
+ *   dist_out             count * sx*sy*sz float32
+ *   idx_out              NULL, or ndim pointers to count * sx*sy*sz int32 planes on the side of dist_out
+ * Kernels, on one stream.  The distances: a seed kernel writes D as doubles (0 / +inf) and queues the tiles
+ * that hold a seed; then ONE cooperative launch of geodesic_relax_kernel runs every round with a grid barrier
+ * between them.  Tiles are 8x8x8 voxels (2-D 16x16, 1-D 256).  A round's CTAs each take tiles of the
+ * worklist, stage a tile and a one-voxel halo of D and labels in shared memory, relax it in sweeps until a
+ * sweep lowers nothing, write back the voxels that went down, and queue each neighbour tile (up to 26) that a
+ * lowered voxel on a face, edge or corner touches (in round 1, whose tiles are those the seed kernel queued,
+ * the seeds count as lowered, so a seed on a tile's border reaches past it); a per-tile flag holding the round it is queued for makes
+ * each list hold a tile at most once.  The rounds end when one queues nothing.  A halo value read while its
+ * owner writes it is an 8-byte load, never torn; D only decreases, so a stale value is an upper bound and the
+ * owner's write queues the reader again.  Termination follows from monotone decrease over finitely many
+ * doubles; there is no round cap.  With idx_out the same rounds then run on S with D fixed: S starts at the
+ * seed's own index and relaxes by min over tight edges only, evaluated with the same double add.  A store
+ * kernel writes float32(D) and the coordinate planes.  The rounds grow with how often shortest paths turn
+ * across tile boundaries: a handful for a convex object, thousands for a maze.
+ * Device memory beyond the labels, seeds and outputs: 8 bytes per voxel for D, 8 more for S with idx_out,
+ * 12 bytes per tile (its flag and its entries in the two worklists), 64 bytes of control blocks, and the
+ * staged seeds and index planes of a host call.
+ * Checks, in order: label width, seed width, ndim and sizes (as edtb200_transform), count >= 0, weights,
+ * flags, the stack's size (within 2^62 voxels, so that a linear seed index fits S's 8 bytes), its tiles
+ * (fewer than 2^32, else EDTB200_ELIMIT: the worklists hold 4-byte tile numbers), emptiness (returns 0
+ * touching nothing), pointers (labels, seeds, dist_out, and each of the ndim planes when idx_out is given),
+ * overlaps (no output may overlap the labels or seeds when on the same side, nor another output), device.
+ * EDT_B200_VERBOSE=1 prints the device time of the distances, indices and store, and the rounds and tile
+ * visits of each phase, on stderr. */
+int edtb200_geodesic(const void *labels, int label_bytes, const void *seeds, int seed_bytes, int ndim,
+                     int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx, float wy, float wz,
+                     int flags, float *dist_out, int32_t *const *idx_out, int device, void *stream);
 
 /* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
  * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between

@@ -12,7 +12,8 @@ import math
 import numpy as np
 import pytest
 
-EINVAL = -1
+from abi_checks import ABI_VERSION, EINVAL
+
 WINDOW_MAX = 2           # EDTB200_BOUNDED_WINDOW_MAX (edtb200_transform_bounded)
 SITES_WINDOW_MAX = 32    # EDTB200_BOUNDED_SITES_WINDOW_MAX (edtb200_feature_transform_bounded)
 CAP = 1 << 62
@@ -65,7 +66,7 @@ def test_symbols_and_version(edt):
   lib = edt._lib()
   for name in ("edtb200_transform_bounded", "edtb200_feature_transform_bounded", "edtb200_bounded_plan"):
     assert hasattr(lib, name)
-  assert lib.edtb200_version() == 202
+  assert lib.edtb200_version() == ABI_VERSION
 
 
 def _ds_around(b):

@@ -3,22 +3,18 @@
 Every entry point rejects a bad argument with a return code and a message before it touches a
 device, so these checks run on any machine.  For each entry point the table below gives its
 argument checks, the order of those checks where one call can fail two of them, and a fully
-valid call, which must get past every check and stop at the device probe: device 63 is "no
-usable CUDA device" on a machine without a GPU and "out of range" on one with a GPU, device 64
-is a "bad device" everywhere.  Nothing here launches a kernel or copies a byte.
+valid call, which must get past every check and stop at the device probe (abi_checks.expect_probe).
+Nothing here launches a kernel or copies a byte.
 """
 import ctypes
 
 import numpy as np
 import pytest
 
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 2, 4, 8, 16
-PROBE = "probe"                    # expected outcome of a call that passes every argument check
+from abi_checks import BIG, EINVAL, ELIMIT, LABELS_FLOAT, LABELS_ON_DEVICE, OUT_ON_DEVICE, PROBE, SIGNED, check_case
 
 _HOST = np.zeros(64, np.uint64)    # stands in for every data pointer: the checks only test for NULL
 P = _HOST.ctypes.data
-BIG = (1 << 30) + 1
 
 
 def ptrs(*values):
@@ -49,7 +45,10 @@ def _batch(labels=None, outs=None, count=2, label_bytes=4, ndim=3, sx=4, sy=4, s
 
 
 def _multi(labels=P, label_bytes=4, ndim=3, sx=4, sy=4, sz=4, w=(1.0, 1.0, 1.0), border=0, flags=0, out=P,
-           devices=(63,), ndevices=None):
+           devices=(63,), ndevices=None, device=63):
+  """`device` takes the place of device 63 in the list."""
+  if devices is not None:
+    devices = tuple(device if d == 63 else d for d in devices)
   arr = (ctypes.c_int * len(devices))(*devices) if devices is not None else None
   n = len(devices) if ndevices is None else ndevices
   return (labels, label_bytes, ndim, sx, sy, sz, *w, border, flags, out, arr, n)
@@ -345,41 +344,9 @@ TABLE = [(name, case, overrides, rc, msg)
          for name, (_, cases) in CASES.items() for case, overrides, rc, msg in cases]
 
 
-def _call(lib, name, overrides):
-  build = CASES[name][0]
-  return getattr(lib, name)(*build(**overrides)), lib.edtb200_last_error() or b""
-
-
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
-def _with_device(name, overrides, device):
-  over = dict(overrides)
-  if name == "edtb200_transform_multi":
-    devs = over.get("devices", (63,))
-    over["devices"] = tuple(device if d == 63 else d for d in devs)
-  else:
-    over["device"] = device
-  return over
-
-
 @pytest.mark.parametrize("name,case,overrides,rc,msg", TABLE, ids=["%s-%s" % (t[0][8:], t[1]) for t in TABLE])
 def test_argument_check(edt, name, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got_rc, err = _call(lib, name, overrides)
-    assert got_rc == rc, (got_rc, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got_rc, err = _call(lib, name, _with_device(name, overrides, device))
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got_rc == want_rc and want_msg in err, (device, got_rc, err)
+  check_case(edt, getattr(edt._lib(), name), CASES[name][0], overrides, rc, msg)
 
 
 @pytest.mark.parametrize("name", sorted(CASES))

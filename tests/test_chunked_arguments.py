@@ -2,8 +2,7 @@
 max_device_bytes.
 
 As in test_capi_arguments.py, every rejection comes with a return code and a message before any
-device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing
+device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing
 here launches a kernel or copies a byte.
 """
 import ctypes
@@ -11,10 +10,8 @@ import ctypes
 import numpy as np
 import pytest
 
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE = 1, 2, 4, 8
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, ECUDA, EINVAL, ELIMIT, HEADER, LABELS_ON_DEVICE, OUT_ON_DEVICE, PROBE, SIGNED,
+                        SQRT, check_case)
 
 # two separate host blocks: the checks only test for NULL and for overlap
 _LABELS = np.zeros(256, np.uint64)
@@ -60,45 +57,27 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_chunked_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  chunks = (ctypes.c_int64 * 2)(-7, -7)
-  if rc != PROBE:
-    got = lib.edtb200_transform_chunked(*_chunked(**overrides, chunks=chunks))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    assert list(chunks) == [0, 0]                        # cleared before any check
-    return
-  for device in (63, 64):
-    got = lib.edtb200_transform_chunked(*_chunked(**dict(overrides, device=device), chunks=chunks))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  chunks = []
+
+  def build(**kw):
+    chunks.append((ctypes.c_int64 * 2)(-7, -7))
+    return _chunked(**kw, chunks=chunks[-1])
+  check_case(edt, edt._lib().edtb200_transform_chunked, build, overrides, rc, msg)
+  assert all(list(c) == [0, 0] for c in chunks)          # each call cleared its chunks before any check
 
 
 def test_chunked_is_an_addition_at_the_same_version(edt):
   """edtb200_transform_chunked is exported next to the 202-level entry points, which keep the number."""
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
+  assert lib.edtb200_version() == ABI_VERSION
   assert hasattr(lib, "edtb200_transform_chunked") and hasattr(lib, "edtb200_feature_transform")
 
 
 def test_chunk_reserve_is_declared():
-  import os
   import re
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  header = open(os.path.join(root, "include", "edt_b200.h")).read()
-  assert int(re.search(r"#define EDTB200_CHUNK_RESERVE (\d+)", header).group(1)) == 512 << 20
+  assert int(re.search(r"#define EDTB200_CHUNK_RESERVE (\d+)", HEADER).group(1)) == 512 << 20
 
 
 # ---- Python: max_device_bytes ----------------------------------------------------------------

@@ -2,8 +2,7 @@
 expand_labels(stacked=True).
 
 As in test_stack_arguments.py, every rejection comes with a return code and a message before any
-device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing
+device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing
 here launches a kernel or copies a byte.
 """
 import ctypes
@@ -12,11 +11,8 @@ import inspect
 import numpy as np
 import pytest
 
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 1, 2, 4, 8, 16
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, BOTH, ECUDA, EINVAL, ELIMIT, LABELS_FLOAT, LABELS_ON_DEVICE, OUT_ON_DEVICE,
+                        PROBE, SIGNED, SQRT, check_case)
 
 # separate host blocks: the checks only test for NULL
 _LABELS = np.zeros(512, np.uint64)
@@ -82,33 +78,14 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_expand_gather_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_expand_gather(*_gather(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_expand_gather(*_gather(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, edt._lib().edtb200_expand_gather, _gather, overrides, rc, msg)
 
 
 def test_expand_gather_is_an_addition_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
+  assert lib.edtb200_version() == ABI_VERSION
   assert hasattr(lib, "edtb200_expand_gather")
   assert lib.edtb200_expand_gather.argtypes[9] is ctypes.c_double
 

@@ -2,8 +2,7 @@
 max_device_bytes on feature_transform / expand_labels.
 
 As in test_chunked_arguments.py, every rejection comes with a return code and a message before any
-device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing
+device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing
 here launches a kernel or copies a byte.
 """
 import ctypes
@@ -12,10 +11,8 @@ import itertools
 import numpy as np
 import pytest
 
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE = 1, 2, 4, 8
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, ECUDA, EINVAL, ELIMIT, LABELS_ON_DEVICE, OUT_ON_DEVICE, PROBE, SIGNED, SQRT,
+                        check_case)
 
 # separate host blocks: the checks only test for NULL and for overlap.  64 voxels: 256 label bytes
 # (label_bytes 4), 256 bytes per distance volume and index plane.
@@ -82,31 +79,15 @@ def _overlap_cases():
   return out
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_feature_chunked_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  chunks = (ctypes.c_int64 * 2)(-7, -7)
-  if rc != PROBE:
-    got = lib.edtb200_feature_transform_chunked(*_call(**overrides, chunks=chunks))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    assert list(chunks) == [0, 0]                        # cleared before any check
-    return
-  for device in (63, 64):
-    got = lib.edtb200_feature_transform_chunked(*_call(**dict(overrides, device=device), chunks=chunks))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
-    assert list(chunks) == [0, 0]
+  chunks = []
+
+  def build(**kw):
+    chunks.append((ctypes.c_int64 * 2)(-7, -7))
+    return _call(**kw, chunks=chunks[-1])
+  check_case(edt, edt._lib().edtb200_feature_transform_chunked, build, overrides, rc, msg)
+  assert all(list(c) == [0, 0] for c in chunks)          # each call cleared its chunks before any check
 
 
 @pytest.mark.parametrize("case,ptrs,msg", _overlap_cases(), ids=[c[0] for c in _overlap_cases()])
@@ -121,7 +102,7 @@ def test_feature_chunked_overlap(edt, case, ptrs, msg):
 
 def test_feature_chunked_is_an_addition_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
+  assert lib.edtb200_version() == ABI_VERSION
   assert hasattr(lib, "edtb200_feature_transform_chunked") and hasattr(lib, "edtb200_transform_chunked")
 
 

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 
 import feature_cases as fc
+from abi_checks import ABI_VERSION
 
 ANISOTROPIES = ((1.0, 1.0, 1.0), (1.0, 2.0, 3.0), (0.7, 1.3, 2.9), (3.3, 3.3, 40.7))
 
@@ -187,4 +188,4 @@ def test_feature_abi_argument_checks(edt):
 
 
 def test_feature_abi_version(edt):
-  assert edt._lib().edtb200_version() == 202
+  assert edt._lib().edtb200_version() == ABI_VERSION

@@ -1,25 +1,17 @@
-"""CPU tests: the argument checks of edtb200_geodesic in their documented order, the header's prototype and
-version comment against the ctypes binding, the Python rejections of geodesic_distance -- each before any
-device is touched -- and the statements of its docstring and the header, with the docstring's examples
-checked on the CPU restatement.  A fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere."""
+"""CPU tests: the argument checks of edtb200_geodesic in their documented order, the header's parameter
+names and version comment, the Python rejections of geodesic_distance -- each before any device is touched
+-- and the statements of its docstring and the header, with the docstring's examples checked on the CPU
+restatement.  A fully valid call stops at the device probe (abi_checks.expect_probe)."""
 import ctypes
 import inspect
-import os
 import re
 
 import numpy as np
 import pytest
 
 import geodesic_cases as gc
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 1, 4, 8, 16
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
-PROBE = "probe"
-BIG = (1 << 30) + 1
-INF, NAN = float("inf"), float("nan")
+from abi_checks import (ABI_VERSION, BIG, BOTH, EINVAL, ELIMIT, HEADER, INF, LABELS_FLOAT, LABELS_ON_DEVICE, NAN,
+                        PROBE, SQRT, check_case, header_doc, no_device_use, prototypes)
 
 _LAB = np.zeros(128, np.uint32)          # 2 volumes of 4 x 4 x 4
 _SEED = np.zeros(128, np.uint8)
@@ -96,57 +88,23 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_geodesic_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_geodesic(*_args(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_geodesic(*_args(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, edt._lib().edtb200_geodesic, _args, overrides, rc, msg)
 
 
-_CTYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "float": ctypes.c_float}
-
-
-def test_the_header_prototype_matches_the_binding(edt):
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  proto = re.search(r"int edtb200_geodesic\(([^)]*)\);", header)
-  assert proto
-  params = [" ".join(p.split()) for p in proto.group(1).split(",")]
-  want = []
-  for p in params:
-    typ = p.rsplit(" ", 1)[0]
-    want.append(ctypes.c_void_p if "*" in p else _CTYPES[typ])
+def test_the_header_names_the_parameters():
+  params = prototypes()["edtb200_geodesic"][1]
   names = [re.sub(r"[*\s]", "", p.rsplit(" ", 1)[1]) for p in params]
   assert names == ["labels", "label_bytes", "seeds", "seed_bytes", "ndim", "sx", "sy", "sz", "count", "wx", "wy", "wz",
                    "flags", "dist_out", "idx_out", "device", "stream"]
   assert "float *dist_out" in params[13] and "int32_t *const *idx_out" in params[14]
-  lib = edt._lib()
-  assert list(lib.edtb200_geodesic.argtypes) == want
-  assert lib.edtb200_geodesic.restype is ctypes.c_int
 
 
 def test_the_header_documents_an_addition_at_the_same_version(edt):
-  assert edt._lib().edtb200_version() == 202
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  assert "edtb200_geodesic" in header[:header.index("#define EDTB200_VERSION")]
-  at = header.index("int edtb200_geodesic(")
-  doc = " ".join(header[header.rindex("/*", 0, at):at].replace("\n *", " ").split())
+  assert edt._lib().edtb200_version() == ABI_VERSION
+  assert "edtb200_geodesic" in HEADER[:HEADER.index("#define EDTB200_VERSION")]
+  doc = header_doc("edtb200_geodesic")
   for text in ("26-neighbours (2-D: 8, 1-D: 2) with the SAME label", "in the order x, y, z",
                "D[v] = min(D[v], fl64(D[u] + w(u, v)))", "float32(D), rounded once to nearest",
                "least linear seed index c (x-fastest within the volume)", "D[u_{i+1}] == fl64(D[u_i] + w)",
@@ -159,15 +117,6 @@ def test_the_header_documents_an_addition_at_the_same_version(edt):
 
 
 # ---- Python ---------------------------------------------------------------------------------------------
-
-@pytest.fixture
-def no_device_use(edt, monkeypatch):
-  class Tripwire:
-    def __getattr__(self, name):
-      raise AssertionError("the library was used (%s) before the arguments were checked" % name)
-  monkeypatch.setattr(edt, "_lib", lambda: Tripwire())
-  return edt
-
 
 def test_signature(edt):
   p = inspect.signature(edt.geodesic_distance).parameters

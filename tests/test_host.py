@@ -4,17 +4,16 @@ No compute call is made here -- there is no GPU -- but the library must load, ex
 symbol include/edt_b200.h declares, and refuse loudly to run without a device.
 """
 import ctypes
-import os
 import re
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import abi_checks
 
 
 def test_library_exports_every_declared_symbol(edt):
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
+  header = abi_checks.HEADER
   declared = set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", header))
   assert {"edtb200_transform", "edtb200_pass_first", "edtb200_pass_later", "edtb200_release",
           "edtb200_last_error", "edtb200_device_count", "edtb200_version"} <= declared
@@ -25,12 +24,34 @@ def test_library_exports_every_declared_symbol(edt):
 
 
 def test_header_flag_values_match_python(edt):
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  vals = dict(re.findall(r"#define (EDTB200_[A-Z_]+)\s+(\d+)", header))
+  vals = dict(re.findall(r"#define (EDTB200_[A-Z_]+)\s+(\d+)", abi_checks.HEADER))
   assert int(vals["EDTB200_SQRT"]) == edt.FLAG_SQRT
   assert int(vals["EDTB200_SIGNED"]) == edt.FLAG_SIGNED
   assert int(vals["EDTB200_LABELS_ON_DEVICE"]) == edt.FLAG_LABELS_ON_DEVICE
   assert int(vals["EDTB200_OUT_ON_DEVICE"]) == edt.FLAG_OUT_ON_DEVICE
+
+
+_PARAM_TYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "float": ctypes.c_float, "double": ctypes.c_double,
+                "size_t": ctypes.c_size_t, "unsigned long long": ctypes.c_uint64, "uint64_t": ctypes.c_uint64}
+_RESULT_TYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "const char *": ctypes.c_char_p,
+                 "void *": ctypes.c_void_p, "void": None}
+
+
+def test_every_binding_matches_its_header_prototype(edt):
+  """ctypes passes a value of the wrong width without complaint, so each binding must match the header."""
+  lib = edt._lib()
+  for name, (result, params) in abi_checks.prototypes().items():
+    want = []
+    for p in params:
+      if name == "edtb200_slab_pack" and p.endswith("*y_start"):
+        want.append(ctypes.POINTER(ctypes.c_int64))
+      elif "*" in p or "[" in p:
+        want.append(ctypes.c_void_p)
+      else:
+        want.append(_PARAM_TYPES[p.rsplit(" ", 1)[0]])
+    fn = getattr(lib, name)
+    assert list(fn.argtypes or []) == want, (name, fn.argtypes, want)
+    assert fn.restype is _RESULT_TYPES[result], (name, fn.restype, result)
 
 
 def test_no_silent_cpu_fallback(edt):

@@ -2,24 +2,19 @@
 rejections of local_thickness.
 
 As in test_morphology_arguments.py, every rejection comes with a return code and a message before any
-device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA device"
-without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing here launches a
-kernel or copies a byte.
+device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing here
+launches a kernel or copies a byte.
 """
 import ctypes
 import inspect
-import os
 import re
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 1, 2, 4, 8, 16
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, BOTH, EINVAL, ELIMIT, HEADER, LABELS_FLOAT, LABELS_ON_DEVICE, PROBE, SIGNED,
+                        SQRT, check_case, no_device_use)
+
 MAX_SIZES = 4096
 
 _IN = np.zeros(512, np.uint64)
@@ -97,55 +92,25 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_local_thickness_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_local_thickness(*_args(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_local_thickness(*_args(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, edt._lib().edtb200_local_thickness, _args, overrides, rc, msg)
 
 
 def test_local_thickness_is_an_addition_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  assert "edtb200_local_thickness" in set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", header))
-  version_comment = header[:header.index("#define EDTB200_VERSION")]
+  assert lib.edtb200_version() == ABI_VERSION
+  assert "edtb200_local_thickness" in set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", HEADER))
+  version_comment = HEADER[:HEADER.index("#define EDTB200_VERSION")]
   assert "edtb200_local_thickness" in version_comment
-  assert re.search(r"#define EDTB200_THICKNESS_MAX_SIZES\s+%d\b" % MAX_SIZES, header)
+  assert re.search(r"#define EDTB200_THICKNESS_MAX_SIZES\s+%d\b" % MAX_SIZES, HEADER)
   assert edt.THICKNESS_MAX_SIZES == MAX_SIZES
   assert hasattr(ctypes.CDLL(edt.library_path()), "edtb200_local_thickness")
-  proto = re.search(r"int edtb200_local_thickness\(([^)]*)\)", header).group(1)
+  proto = re.search(r"int edtb200_local_thickness\(([^)]*)\)", HEADER).group(1)
   assert len(proto.split(",")) == len(lib.edtb200_local_thickness.argtypes) == 18
 
 
 # ---- Python ---------------------------------------------------------------------------------------------
-
-@pytest.fixture
-def no_device_use(edt, monkeypatch):
-  """Fails the test if a call reaches the C library."""
-  class Tripwire:
-    def __getattr__(self, name):
-      raise AssertionError("the library was used (%s) before the arguments were checked" % name)
-  monkeypatch.setattr(edt, "_lib", lambda: Tripwire())
-  return edt
-
 
 def test_exported(edt):
   assert "local_thickness" in edt.__all__

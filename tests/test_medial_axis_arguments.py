@@ -1,24 +1,16 @@
-"""CPU tests: the argument checks of edtb200_medial_axis in their documented order, the header's prototype
-against the ctypes binding, the Python rejections of medial_axis -- each before any device is touched --
-and the identities its docstring and the header state.  A fully valid call stops at the device probe:
-device 63 is "no usable CUDA device" without a GPU and "out of range" with one, device 64 is a "bad
-device" everywhere."""
-import ctypes
+"""CPU tests: the argument checks of edtb200_medial_axis in their documented order, the header's parameter
+names, the Python rejections of medial_axis -- each before any device is touched -- and the identities its
+docstring and the header state.  A fully valid call stops at the device probe (abi_checks.expect_probe)."""
 import inspect
-import os
 import re
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 1, 4, 8, 16
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, BOTH, EINVAL, ELIMIT, HEADER, INF, LABELS_FLOAT, LABELS_ON_DEVICE, NAN,
+                        PROBE, SQRT, check_case, header_doc, no_device_use, prototypes)
+
 LINE = (1 << 26) + 1
-INF, NAN = float("inf"), float("nan")
 
 _LAB = np.zeros(128, np.uint32)          # 2 volumes of 4 x 4 x 4
 _MED = np.zeros(128, np.uint8)
@@ -95,57 +87,23 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_medial_axis_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_medial_axis(*_args(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_medial_axis(*_args(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, edt._lib().edtb200_medial_axis, _args, overrides, rc, msg)
 
 
-_CTYPES = {"int": ctypes.c_int, "int64_t": ctypes.c_int64, "float": ctypes.c_float}
-
-
-def test_the_header_prototype_matches_the_binding(edt):
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  proto = re.search(r"int edtb200_medial_axis\(([^)]*)\);", header)
-  assert proto
-  params = [" ".join(p.split()) for p in proto.group(1).split(",")]
-  want = []
-  for p in params:
-    typ = p.rsplit(" ", 1)[0]
-    want.append(ctypes.c_void_p if "*" in p else _CTYPES[typ])
+def test_the_header_names_the_parameters():
+  params = prototypes()["edtb200_medial_axis"][1]
   names = [re.sub(r"[*\s]", "", p.rsplit(" ", 1)[1]) for p in params]
   assert names == ["labels", "label_bytes", "ndim", "sx", "sy", "sz", "count", "wx", "wy", "wz", "black_border",
                    "flags", "medial_out", "dist_out", "device", "stream"]
   assert "uint8_t *medial_out" in params[12] and "float *dist_out" in params[13]
-  lib = edt._lib()
-  assert list(lib.edtb200_medial_axis.argtypes) == want
-  assert lib.edtb200_medial_axis.restype is ctypes.c_int
 
 
 def test_the_header_documents_an_addition_at_the_same_version(edt):
-  assert edt._lib().edtb200_version() == 202
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  assert "edtb200_medial_axis" in header[:header.index("#define EDTB200_VERSION")]
-  at = header.index("int edtb200_medial_axis(")
-  doc = " ".join(header[header.rindex("/*", 0, at):at].replace("\n *", " ").split())
+  assert edt._lib().edtb200_version() == ABI_VERSION
+  assert "edtb200_medial_axis" in HEADER[:HEADER.index("#define EDTB200_VERSION")]
+  doc = header_doc("edtb200_medial_axis")
   for text in ("least j", "REAL maximisers", "lexicographically least (z, y, x)", "not masked to",
                "-inf", "reduced discrete medial axis", "4 + 4 ndim", "16 in 3-D", "2^26", "EDTB200_ELIMIT",
                "D2 = 1 4 9 4 1", "medial {2}", "medial {1, 2}", "its first one", "not a topological skeleton",
@@ -154,15 +112,6 @@ def test_the_header_documents_an_addition_at_the_same_version(edt):
 
 
 # ---- Python ---------------------------------------------------------------------------------------------
-
-@pytest.fixture
-def no_device_use(edt, monkeypatch):
-  class Tripwire:
-    def __getattr__(self, name):
-      raise AssertionError("the library was used (%s) before the arguments were checked" % name)
-  monkeypatch.setattr(edt, "_lib", lambda: Tripwire())
-  return edt
-
 
 def test_signature(edt):
   p = inspect.signature(edt.medial_axis).parameters

@@ -1,23 +1,17 @@
 """CPU tests: the argument checks of edtb200_parabolic in their documented order, and the Python
 rejections of parabolic_erode and parabolic_dilate -- each before any device is touched.  A fully valid
-call stops at the device probe: device 63 is "no usable CUDA device" without a GPU and "out of range"
-with one, device 64 is a "bad device" everywhere."""
+call stops at the device probe (abi_checks.expect_probe)."""
 import ctypes
 import inspect
-import os
 import re
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 1, 4, 8, 16
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
+from abi_checks import (ABI_VERSION, BIG, BOTH, EINVAL, ELIMIT, HEADER, INF, LABELS_FLOAT, LABELS_ON_DEVICE, NAN,
+                        PROBE, SQRT, check_case, no_device_use)
+
 ERODE, DILATE = 0, 1
-PROBE = "probe"
-BIG = (1 << 30) + 1
-INF, NAN = float("inf"), float("nan")
 
 _IN = np.zeros(512, np.float32)
 _OUT = np.zeros(512, np.float32)
@@ -71,54 +65,24 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_parabolic_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_parabolic(*_args(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_parabolic(*_args(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, edt._lib().edtb200_parabolic, _args, overrides, rc, msg)
 
 
 def test_parabolic_is_an_addition_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  assert "edtb200_parabolic" in set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", header))
-  assert "edtb200_parabolic" in header[:header.index("#define EDTB200_VERSION")]
+  assert lib.edtb200_version() == ABI_VERSION
+  assert "edtb200_parabolic" in set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", HEADER))
+  assert "edtb200_parabolic" in HEADER[:HEADER.index("#define EDTB200_VERSION")]
   for name, value in (("PARABOLIC_ERODE", 0), ("PARABOLIC_DILATE", 1)):
-    assert re.search(r"#define EDTB200_%s\s+%d\b" % (name, value), header), name
+    assert re.search(r"#define EDTB200_%s\s+%d\b" % (name, value), HEADER), name
   assert hasattr(ctypes.CDLL(edt.library_path()), "edtb200_parabolic")
 
 
 # ---- Python ---------------------------------------------------------------------------------------------
 
 FNS = ["parabolic_erode", "parabolic_dilate"]
-
-
-@pytest.fixture
-def no_device_use(edt, monkeypatch):
-  """Fails the test if a call reaches the C library."""
-  class Tripwire:
-    def __getattr__(self, name):
-      raise AssertionError("the library was used (%s) before the arguments were checked" % name)
-  monkeypatch.setattr(edt, "_lib", lambda: Tripwire())
-  return edt
 
 
 def test_exported(edt):

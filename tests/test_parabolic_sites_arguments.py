@@ -1,14 +1,14 @@
 """CPU tests: the argument checks of edtb200_parabolic_sites in their documented order (those of
 edtb200_parabolic, then the 2^26 line limit, then idx with the pointers and overlaps), the Python
-rejections of return_indices, and the docstrings.  A fully valid call stops at the device probe: device 63
-is "no usable CUDA device" without a GPU and "out of range" with one, device 64 is a "bad device"."""
-import os
+rejections of return_indices, and the docstrings.  A fully valid call stops at the device probe
+(abi_checks.expect_probe)."""
 import re
 
 import numpy as np
 import pytest
 
-from test_parabolic_arguments import BOTH, CASES, ECUDA, EINVAL, ELIMIT, IN, LABELS_ON_DEVICE, OUT, PROBE, ROOT
+from abi_checks import ABI_VERSION, BOTH, EINVAL, ELIMIT, HEADER, LABELS_ON_DEVICE, PROBE, check_case, no_device_use
+from test_parabolic_arguments import CASES, IN, OUT
 
 _IDX = np.zeros(3 * 512, np.int32)
 IDX = _IDX.ctypes.data
@@ -42,55 +42,27 @@ SITES_CASES = [(name.replace("parabolic", "parabolic_sites"), kw, rc, msg) for n
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", SITES_CASES, ids=[c[0] for c in SITES_CASES])
 def test_parabolic_sites_argument_check(edt, case, overrides, rc, msg):
   lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_parabolic_sites(*_args(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    if msg == "residency flags":
-      assert b"edtb200_parabolic_sites" in err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_parabolic_sites(*_args(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, lib.edtb200_parabolic_sites, _args, overrides, rc, msg)
+  if msg == "residency flags":
+    assert b"edtb200_parabolic_sites" in lib.edtb200_last_error()
 
 
 def test_the_header_documents_an_addition_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  assert "edtb200_parabolic_sites" in header[:header.index("#define EDTB200_VERSION")]
-  proto = re.search(r"int edtb200_parabolic_sites\(([^)]*)\);", header)
+  assert lib.edtb200_version() == ABI_VERSION
+  assert "edtb200_parabolic_sites" in HEADER[:HEADER.index("#define EDTB200_VERSION")]
+  proto = re.search(r"int edtb200_parabolic_sites\(([^)]*)\);", HEADER)
   assert proto and "int32_t *idx" in proto.group(1)
   for text in ("least j among the REAL", "2^26", "EDTB200_ELIMIT", "-1 in every coordinate", "8 in 3-D"):
-    assert text in header, text
+    assert text in HEADER, text
 
 
 # ---- Python ---------------------------------------------------------------------------------------------
 
 FNS = ["parabolic_erode", "parabolic_dilate"]
-
-
-@pytest.fixture
-def no_device_use(edt, monkeypatch):
-  class Tripwire:
-    def __getattr__(self, name):
-      raise AssertionError("the library was used (%s) before the arguments were checked" % name)
-  monkeypatch.setattr(edt, "_lib", lambda: Tripwire())
-  return edt
 
 
 @pytest.mark.parametrize("name", FNS)

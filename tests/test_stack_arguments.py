@@ -2,8 +2,7 @@
 the Python rejections of stacked=True.
 
 As in test_chunked_arguments.py, every rejection comes with a return code and a message before any
-device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing
+device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing
 here launches a kernel or copies a byte.
 """
 import ctypes
@@ -11,10 +10,8 @@ import ctypes
 import numpy as np
 import pytest
 
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE = 1, 2, 4, 8
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, BOTH, ECUDA, EINVAL, ELIMIT, LABELS_ON_DEVICE, OUT_ON_DEVICE, PROBE, SIGNED,
+                        SQRT, check_case)
 
 # two separate host blocks: the checks only test for NULL and for overlap.  Each holds the largest extent a
 # case passes (valid_1d: 300 volumes of 4 voxels, 4800 bytes), so that whether two valid extents overlap never
@@ -38,8 +35,6 @@ def _feature_stack(labels=L, label_bytes=4, ndim=3, sx=4, sy=4, sz=4, count=2, w
   idx = ptrs(O, O, O) if idx is None else idx
   return (labels, label_bytes, ndim, sx, sy, sz, count, *w, border, flags, dist, idx, device, stream)
 
-
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
 
 STACK_CASES = [
   ("label_bytes_3", dict(label_bytes=3), EINVAL, "label_bytes"),
@@ -98,52 +93,25 @@ FEATURE_CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", STACK_CASES, ids=[c[0] for c in STACK_CASES])
 def test_transform_stack_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  groups = (ctypes.c_int64 * 1)(-7)
-  if rc != PROBE:
-    got = lib.edtb200_transform_stack(*_stack(**overrides, groups=groups))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    assert groups[0] == 0                                # cleared before any check
-    return
-  for device in (63, 64):
-    got = lib.edtb200_transform_stack(*_stack(**dict(overrides, device=device), groups=groups))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
-    assert groups[0] == 0
+  groups = []
+
+  def build(**kw):
+    groups.append((ctypes.c_int64 * 1)(-7))
+    return _stack(**kw, groups=groups[-1])
+  check_case(edt, edt._lib().edtb200_transform_stack, build, overrides, rc, msg)
+  assert all(g[0] == 0 for g in groups)                  # each call cleared its groups before any check
 
 
 @pytest.mark.parametrize("case,overrides,rc,msg", FEATURE_CASES, ids=[c[0] for c in FEATURE_CASES])
 def test_feature_transform_stack_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  if rc != PROBE:
-    got = lib.edtb200_feature_transform_stack(*_feature_stack(**overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = lib.edtb200_feature_transform_stack(*_feature_stack(**dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, edt._lib().edtb200_feature_transform_stack, _feature_stack, overrides, rc, msg)
 
 
 def test_stack_entry_points_are_additions_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
+  assert lib.edtb200_version() == ABI_VERSION
   assert hasattr(lib, "edtb200_transform_stack") and hasattr(lib, "edtb200_feature_transform_stack")
 
 

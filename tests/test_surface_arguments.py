@@ -2,24 +2,19 @@
 rejections of surface_distances, hausdorff_distance, average_surface_distance and surface_dice.
 
 As in test_expand_stack_arguments.py, every rejection comes with a return code and a message before
-any device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing
+any device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing
 here launches a kernel or copies a byte.
 """
 import ctypes
+import functools
 import inspect
-import os
 import re
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, LABELS_ON_DEVICE, OUT_ON_DEVICE = 1, 4, 8
-BOTH = LABELS_ON_DEVICE | OUT_ON_DEVICE
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, BOTH, ECUDA, EINVAL, ELIMIT, HEADER, LABELS_ON_DEVICE, OUT_ON_DEVICE, PROBE,
+                        SQRT, check_case)
 
 # separate host blocks: the checks only test for NULL (the keys are read: they are host memory)
 _A = np.zeros(512, np.uint64)
@@ -93,20 +88,10 @@ CASES = [
 ]
 
 
-def _args(fn, overrides):
-  o = dict(overrides)
-  out = o.pop("out", OUT)
+def _args(fn, out=OUT, **o):
   if fn == "count":
     return _count(counts=out, **o)
   return _dist(offsets=out, values=out, **o)
-
-
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
 
 
 @pytest.mark.parametrize("fn", ["count", "distances"])
@@ -114,17 +99,7 @@ def _expect_probe(edt, device):
 def test_surface_argument_check(edt, fn, case, overrides, rc, msg):
   lib = edt._lib()
   call = lib.edtb200_surface_count if fn == "count" else lib.edtb200_surface_distances
-  if rc != PROBE:
-    got = call(*_args(fn, overrides))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    return
-  for device in (63, 64):
-    got = call(*_args(fn, dict(overrides, device=device)))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
+  check_case(edt, call, functools.partial(_args, fn), overrides, rc, msg)
 
 
 def test_distances_null_offsets_and_values(edt):
@@ -144,9 +119,8 @@ def test_distances_groups_zeroed_on_error_and_empty(edt):
 
 def test_surface_entry_points_are_additions_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
-  header = open(os.path.join(ROOT, "include", "edt_b200.h")).read()
-  declared = set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", header))
+  assert lib.edtb200_version() == ABI_VERSION
+  declared = set(re.findall(r"\b(edtb200_[a-z0-9_]+)\s*\(", HEADER))
   assert {"edtb200_surface_count", "edtb200_surface_distances"} <= declared
   raw = ctypes.CDLL(edt.library_path())
   assert hasattr(raw, "edtb200_surface_count") and hasattr(raw, "edtb200_surface_distances")

@@ -1,19 +1,18 @@
 """CPU tests: the argument checks of edtb200_transform_voxel_graph_chunked.
 
 As in test_chunked_arguments.py, every rejection comes with a return code and a message before any
-device is touched, and a fully valid call stops at the device probe: device 63 is "no usable CUDA
-device" without a GPU and "out of range" with one, device 64 is a "bad device" everywhere.  Nothing
+device is touched, and a fully valid call stops at the device probe (abi_checks.expect_probe).  Nothing
 here launches a kernel or copies a byte.
 """
 import ctypes
+import os
 
 import numpy as np
 import pytest
 
-EINVAL, ECUDA, ELIMIT = -1, -2, -4
-SQRT, SIGNED, LABELS_ON_DEVICE, OUT_ON_DEVICE, LABELS_FLOAT = 1, 2, 4, 8, 16
-PROBE = "probe"
-BIG = (1 << 30) + 1
+from abi_checks import (ABI_VERSION, BIG, ECUDA, EINVAL, ELIMIT, HEADER, LABELS_FLOAT, LABELS_ON_DEVICE, OUT_ON_DEVICE,
+                        PROBE, ROOT, SIGNED, SQRT, check_case)
+
 HALF = (1 << 29) + 1                    # fits one axis, but its doubled axis is longer than 2^30
 
 # separate host blocks: the checks only test for NULL and for overlap.  64 voxels: 256 label bytes
@@ -81,45 +80,26 @@ CASES = [
 ]
 
 
-def _expect_probe(edt, device):
-  if device >= 64:
-    return EINVAL, b"bad device %d" % device
-  if edt.device_count() == 0:
-    return ECUDA, b"no usable CUDA device"
-  return EINVAL, b"device %d out of range" % device
-
-
 @pytest.mark.parametrize("case,overrides,rc,msg", CASES, ids=[c[0] for c in CASES])
 def test_voxel_graph_chunked_argument_check(edt, case, overrides, rc, msg):
-  lib = edt._lib()
-  chunks = (ctypes.c_int64 * 2)(-7, -7)
-  if rc != PROBE:
-    got = lib.edtb200_transform_voxel_graph_chunked(*_call(**overrides, chunks=chunks))
-    err = lib.edtb200_last_error() or b""
-    assert got == rc, (got, err)
-    assert msg.encode() in err, err
-    assert list(chunks) == [0, 0]                        # cleared before any check
-    return
-  for device in (63, 64):
-    got = lib.edtb200_transform_voxel_graph_chunked(*_call(**dict(overrides, device=device), chunks=chunks))
-    err = lib.edtb200_last_error() or b""
-    want_rc, want_msg = _expect_probe(edt, device)
-    assert got == want_rc and want_msg in err, (device, got, err)
-    assert list(chunks) == [0, 0]
+  chunks = []
+
+  def build(**kw):
+    chunks.append((ctypes.c_int64 * 2)(-7, -7))
+    return _call(**kw, chunks=chunks[-1])
+  check_case(edt, edt._lib().edtb200_transform_voxel_graph_chunked, build, overrides, rc, msg)
+  assert all(list(c) == [0, 0] for c in chunks)          # each call cleared its chunks before any check
 
 
 def test_voxel_graph_chunked_is_an_addition_at_the_same_version(edt):
   lib = edt._lib()
-  assert lib.edtb200_version() == 202
+  assert lib.edtb200_version() == ABI_VERSION
   assert hasattr(lib, "edtb200_transform_voxel_graph_chunked") and hasattr(lib, "edtb200_transform_voxel_graph")
 
 
 def test_voxel_graph_chunked_is_declared():
-  import os
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  header = open(os.path.join(root, "include", "edt_b200.h")).read()
-  assert "int edtb200_transform_voxel_graph_chunked(" in header
-  shim = open(os.path.join(root, "include", "edt_voxel_graph.hpp")).read()
+  assert "int edtb200_transform_voxel_graph_chunked(" in HEADER
+  shim = open(os.path.join(ROOT, "include", "edt_voxel_graph.hpp")).read()
   assert "edtb200_transform_voxel_graph_chunked(" in shim
 
 

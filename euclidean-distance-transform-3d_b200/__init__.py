@@ -158,6 +158,9 @@ def _lib():
   lib.edtb200_pass_window.argtypes = [vp, ci, ci, i64, i64, i64, f32, ci, ci, ci, ctypes.c_double, vp, vp, vp, ci,
                                       vp]
   lib.edtb200_pass_window.restype = ci
+  lib.edtb200_noise_planes.argtypes = [vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, ci, ci, ci, ci, vp, vp, vp,
+                                       ci, vp]
+  lib.edtb200_noise_planes.restype = ci
   lib.edtb200_slab_pack.argtypes = [vp, vp, i64, i64, i64, ci, ctypes.POINTER(ctypes.c_int64), ci, ci, vp]
   lib.edtb200_slab_pack.restype = ci
   lib.edtb200_slab_face_runs.argtypes = [vp, ci, i64, i64, i64, ci, ci, ci, vp, vp, ci, vp]

@@ -553,9 +553,10 @@ bool overlaps(const void* a, size_t na, const void* b, size_t nb) {
 bool same_side(int flags) { return !(flags & EDTB200_LABELS_ON_DEVICE) == !(flags & EDTB200_OUT_ON_DEVICE); }
 
 int dispatch_first(int label_bytes, const void* labels, float* f, int64_t nlines, int64_t sx, float w,
-                   int border, int flags, DeviceCache& dc, cudaStream_t s, const edtb200::XPlanes* planes = nullptr) {
+                   int border, int flags, DeviceCache& dc, cudaStream_t s, const edtb200::XPlanes* planes = nullptr,
+                   PlanesMarch* march = nullptr) {
   return with_label_width(label_bytes, [&](auto b) {
-    return launch_first<b>(labels, f, nlines, sx, w, border, flags, planes, dc, s);
+    return launch_first<b>(labels, f, nlines, sx, w, border, flags, planes, dc, s, march);
   });
 }
 
@@ -665,23 +666,24 @@ struct RunPlanes {
   const edtb200::XPlanes* for_x() const { return x.y ? &x : nullptr; }
 };
 
-// Plans transform t over `count` volumes (t.n[0], sy, sz) laid end to end at labels / f, and takes the
-// planes the plan asks for; where there is no room for them the later passes read the labels.
-int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const float* f, int64_t sy, int64_t sz,
-                    int64_t count, DeviceCache& dc, cudaStream_t s) {
-  const NoisePlan np = noise_plan(t, count, labels, f, dc);
+// The 32-bit words of the planes that plan np asks of transform t over `count` volumes (t.n[0], sy, sz):
+// per later axis, the run-start plane (wpr = ceil(sx / 32) words per row), then the settled plane (one
+// word per row); [y plane | settled_y | z plane | settled_z].
+int64_t run_planes_words(const NoisePlan& np, const Transform& t, int64_t sy, int64_t sz, int64_t count) {
+  const int64_t rows = sy * sz * count;
+  return (rows * ((t.n[0] + 31) >> 5) + rows) * np.planes;
+}
+
+// Arms the later passes of rp as plan np says, with the planes (if any) laid out at p, run_planes_words
+// of them.
+void arm_run_planes(RunPlanes& rp, const NoisePlan& np, const Transform& t, uint32_t* p, int64_t sy, int64_t sz,
+                    int64_t count) {
   for (int k = 1; k < 3; ++k) {
     rp.later[k].noise = np.noise;
     rp.later[k].plan = np.later[k];
   }
-  if (!np.planes) return 0;
-  // per later axis: the run-start plane (wpr words per row), then the settled plane (one word per row)
+  if (!np.planes || !p) return;
   const int64_t sx = t.n[0], wpr = (sx + 31) >> 5, rows = sy * sz * count, words = rows * wpr;
-  if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)(words + rows) * (size_t)np.planes, s) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;                        // no room: the later passes read the labels
-  }
-  uint32_t* p = rp.mem.get<uint32_t>();
   rp.x.sy = sy;
   rp.x.depth = sz;
   rp.x.y = p;
@@ -700,14 +702,30 @@ int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const
     rp.later[2].bits = edtb200::RunBits{rp.x.z, sy * wpr, sz * sy * wpr, sx, wpr,
                                         np.later[2].settled ? rp.x.settled_z : nullptr, sy, sz * sy, nullptr, 0.0f,
                                         np.group[2]};
+}
+
+// Plans transform t over `count` volumes (t.n[0], sy, sz) laid end to end at labels / f, and takes the
+// planes the plan asks for; where there is no room for them the later passes read the labels.
+int take_run_planes(RunPlanes& rp, const Transform& t, const void* labels, const float* f, int64_t sy, int64_t sz,
+                    int64_t count, DeviceCache& dc, cudaStream_t s) {
+  const NoisePlan np = noise_plan(t, count, labels, f, dc);
+  uint32_t* p = nullptr;
+  if (np.planes) {
+    if (rp.mem.alloc(dc, sizeof(uint32_t) * (size_t)run_planes_words(np, t, sy, sz, count), s) == cudaSuccess)
+      p = rp.mem.get<uint32_t>();
+    else
+      cudaGetLastError();            // no room: the later passes read the labels
+  }
+  arm_run_planes(rp, np, t, p, sy, sz, count);
   return 0;
 }
 
-// The X pass over nlines rows; planes: the run-start planes it writes (null: none).
+// The X pass over nlines rows; planes: the run-start planes it writes (null: none); march: the march
+// of the plane-writing kernel asked for and launched (PlanesMarch, null: its own rule).
 int x_pass(const Transform& t, const void* labels, float* f, int64_t nlines, DeviceCache& dc, cudaStream_t s,
-           const RunPlanes* planes = nullptr) {
+           const RunPlanes* planes = nullptr, PlanesMarch* march = nullptr) {
   return dispatch_first(t.label_bytes, labels, f, nlines, t.n[0], t.w[0], t.border,
-                        kernel_flags(t.flags, true, t.ndim == 1), dc, s, planes ? planes->for_x() : nullptr);
+                        kernel_flags(t.flags, true, t.ndim == 1), dc, s, planes ? planes->for_x() : nullptr, march);
 }
 
 // The later pass along axis k over geometry g, with the borders lo / hi at the ends of its lines;
@@ -2826,6 +2844,68 @@ int edtb200_pass_window(const void* labels_dev, int label_bytes, int axis, int64
                                   border_hi != 0, kernel_flags(flags, /*first=*/false, /*last=*/true), arith,
                                   bp.bound, *dc, s);
   });
+}
+
+int edtb200_noise_planes(const void* labels_dev, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                         int64_t count, float wx, float wy, float wz, int black_border, int flags, int passes,
+                         int nchunks, int ctas, float* f_dev, uint32_t* planes_dev, int* info, int device,
+                         void* stream) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (label_bytes < 4) return fail(EDTB200_EINVAL, "the run-start planes need labels of 4 or 8 bytes (got %d)", label_bytes);
+  if (ndim < 2) return fail(EDTB200_EINVAL, "the run-start planes need 2-D or 3-D volumes (got ndim %d)", ndim);
+  if (count < 1) return fail(EDTB200_EINVAL, "count must be 1 or more (got %lld)", (long long)count);
+  if ((rc = check_stack(sx * sy * sz, count, 1))) return rc;
+  const float w[3] = {wx, wy, wz};
+  if ((rc = check_weights(ndim, w))) return rc;
+  if (flags & EDTB200_SIGNED) return fail(EDTB200_EINVAL, "a signed transform (EDTB200_SIGNED) takes no run-start planes");
+  if (flags & ~EDTB200_SQRT) return fail(EDTB200_EINVAL, "flags may only hold EDTB200_SQRT (got %d)", flags);
+  if (passes != 1 && passes != 2) return fail(EDTB200_EINVAL, "passes must be 1 or 2 (got %d)", passes);
+  if (sx > 512 || sx % 4 != 0)
+    return fail(EDTB200_EINVAL, "the run-start planes need rows of at most 512 voxels, a multiple of 4 (got %lld)",
+                (long long)sx);
+  if (sz * count > 0x7fffffffLL || sy > 0x3fffffffLL)
+    return fail(EDTB200_EINVAL, "more slices or rows than the plane-writing X pass counts in 32 bits");
+  if (nchunks < 0 || nchunks > sy)
+    return fail(EDTB200_EINVAL, "nchunks must be 0 or 1..sy = %lld (got %d)", (long long)sy, nchunks);
+  if (ctas < 0 || (ctas > 0 && nchunks == 0))
+    return fail(EDTB200_EINVAL, "ctas must be 0, or 1..items with nchunks given (got %d)", ctas);
+  if (ctas > 0) {
+    using edtb200::kPlaneWarps;
+    const int64_t items = ndim == 3 ? edtb200::march_items<kPlaneWarps, 2>(sz * count, nchunks)
+                                    : edtb200::march_items<kPlaneWarps, 1>(count, nchunks);
+    if (ctas > items) return fail(EDTB200_EINVAL, "ctas must be 0 or 1..items = %lld (got %d)", (long long)items, ctas);
+  }
+  if (sx * sy * sz == 0) return 0;
+  if (!labels_dev || !f_dev || !planes_dev || !info) return fail(EDTB200_EINVAL, "null pointer");
+  if (!first_is_vec(labels_dev, label_bytes, f_dev, sx) || reinterpret_cast<uintptr_t>(planes_dev) % 4 != 0)
+    return fail(EDTB200_EINVAL, "labels, distances and planes must be aligned for vector access");
+  DeviceGuard restore_device;
+  DeviceCache* dc = nullptr;
+  rc = probe(device, &dc);
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const Transform t{label_bytes, ndim, flags, black_border != 0, {wx, wy, wz}, {sx, sy, sz}};
+  // the plan of the second call on label noise; the X pass writes the planes whatever the later passes take
+  NoisePlan np = noise_plan(t, count, labels_dev, f_dev, *dc, /*noise=*/1);
+  if (passes == 2 && !np.planes)
+    return fail(EDTB200_EINVAL, "the transform takes no run-start planes for these extents and weights");
+  np.planes = ndim - 1;
+  RunPlanes rp;
+  arm_run_planes(rp, np, t, planes_dev, sy, sz, count);
+  PlanesMarch march;
+  march.want_chunks = nchunks;
+  march.want_ctas = ctas;
+  rc = x_pass(t, labels_dev, f_dev, sy * sz * count, *dc, s, &rp, &march);
+  if (!rc && passes == 2)
+    rc = later_pass(t, 1, labels_dev, f_dev, geom_for_axis(1, sx, sy, sz, count), t.border, t.border, *dc, s,
+                    /*pdl=*/true, &rp);
+  if (rc) return rc;
+  const int v[10] = {label_bytes, march.k, march.plain, march.planes, (int)march.nchunks, (int)march.items,
+                     (int)march.grid, passes == 2 && np.reads[1], passes == 2 && np.later[1].settled,
+                     passes == 2 && np.refresh};
+  memcpy(info, v, sizeof(v));
+  return 0;
 }
 
 int edtb200_last_later_launch(int* info) {

@@ -237,9 +237,16 @@ inline bool first_is_vec(const void* labels, int label_bytes, const float* f, in
 // planned: what noise_plan planned for the later pass (null: it reads the noise prediction at launch
 // and no plane).
 struct LaterNoise;
+// The march of the plane-writing X pass (first_axis_planes_kernel), for edtb200_noise_planes: the y-chunks
+// per slice and the CTAs a caller asks for (0: launch_first_vec's own rule), then what was launched.
+struct PlanesMarch {
+  int64_t want_chunks = 0, want_ctas = 0;
+  int k = 0, plain = 0, planes = 0;            // the instance <Bytes, K, Plain, Planes>
+  int64_t nchunks = 0, items = 0, grid = 0;
+};
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
-                 const XPlanes* planes, DeviceCache& dc, cudaStream_t stream);
+                 const XPlanes* planes, DeviceCache& dc, cudaStream_t stream, PlanesMarch* march = nullptr);
 template <int Bytes>
 int launch_later(const void* labels, const LaterNoise* planned, float* f, const LineGeom& g0, float w,
                  int border_lo, int border_hi, int flags, PassArith arith, DeviceCache& dc, cudaStream_t stream,
@@ -499,8 +506,10 @@ struct NoisePlan {
   bool refresh = false;        // the Y pass refreshes the Z pass's settled plane
 };
 // plan_noise for transform t over `count` volumes laid end to end at labels / f on this device, with
-// one reading of the noise prediction and the A/B switches of the later passes (edt_plan.cu).
-NoisePlan noise_plan(const Transform& t, int64_t count, const void* labels, const float* f, const DeviceCache& dc);
+// one reading of the noise prediction and the A/B switches of the later passes (edt_plan.cu).  noise
+// 0 / 1: plan as if the prediction were that instead (edtb200_noise_planes); -1: read it.
+NoisePlan noise_plan(const Transform& t, int64_t count, const void* labels, const float* f, const DeviceCache& dc,
+                     int noise = -1);
 
 // One later pass of run_passes as noise_plan planned it: the prediction it plans with and, where it
 // reads its run-start plane (bits.start non-null), the plan that plane was armed for.

@@ -51,11 +51,14 @@ inline size_t planes_smem_bytes(int64_t sx, int label_bytes) {
 }
 
 // The register-resident X kernel for K 128-voxel blocks per row; with `planes` (planes->y non-null)
-// the kernel that also writes them, compiled for labels of 4 and 8 bytes and rows of at most 512
-// voxels only, where run_passes takes them.
+// the kernel that also writes them, compiled for labels of 4 and 8 bytes, rows of at most 512 voxels
+// and the plain kernel flags only, where run_passes takes them: plan_noise takes no planes for a
+// signed transform, and the X pass of any other transform of two or more axes has flags 0.
+// march (may be null): the chunk count and grid asked for and launched (PlanesMarch).
 template <int Bytes, int K, bool Plain>
 int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, const float* table, int border,
-                     int flags, RunStat stat, const XPlanes* planes, DeviceCache& dc, cudaStream_t stream) {
+                     int flags, RunStat stat, const XPlanes* planes, DeviceCache& dc, cudaStream_t stream,
+                     PlanesMarch* march) {
   using LT = typename LabelOf<Bytes>::type;
   if (!planes) {
     const size_t smem = sizeof(float) * (size_t)(sx + 2);
@@ -68,7 +71,7 @@ int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, c
     CUDA_TRY(cudaGetLastError());
     return 0;
   }
-  if constexpr (Bytes >= 4 && K <= 4) {
+  if constexpr (Bytes >= 4 && K <= 4 && Plain) {
     // Bands of 8 slices that march along y through a ring of stages of 9 rows: 4 stages (74 KB) for
     // 512-voxel rows of 4-byte labels, so three CTAs per SM, each reading two stages with two more
     // (36 KB) in flight; 3 stages (110 KB) for 8-byte ones, two CTAs per SM, one stage in flight.
@@ -87,12 +90,22 @@ int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, c
     // its labels.
     const int64_t sy = planes->sy, nz = nlines / sy, wave = (int64_t)dc.sm_count * (per_sm > 0 ? per_sm : 1);
     const int64_t fill = z ? wave / ((nz + W - 1) / W) : wave * W / nz;
-    const int64_t nchunks = std::max<int64_t>(1, std::min(fill, sy * 3 / 200));
+    // A march may ask for another chunk count (1 .. sy) and grid (1 .. items), checked by its caller.
+    const int64_t nchunks = march && march->want_chunks ? march->want_chunks
+                                                        : std::max<int64_t>(1, std::min(fill, sy * 3 / 200));
     const int64_t items = z ? march_items<W, 2>(nz, nchunks) : march_items<W, 1>(nz, nchunks);
-    const int64_t blocks = std::max<int64_t>(1, std::min(wave, items));
+    const int64_t blocks = march && march->want_ctas ? march->want_ctas : std::max<int64_t>(1, std::min(wave, items));
     kern<<<(unsigned)blocks, W * 32, smem, stream>>>(static_cast<const LT*>(labels), f, nlines, (int)sx, table, border,
                                                      flags, stat, *planes, (int)nchunks);
     CUDA_TRY(cudaGetLastError());
+    if (march) {
+      march->k = K;
+      march->plain = Plain;
+      march->planes = z ? 2 : 1;
+      march->nchunks = nchunks;
+      march->items = items;
+      march->grid = blocks;
+    }
     return 0;
   }
   return fail(EDTB200_EINVAL, "run-start planes asked of an X launch that cannot write them");
@@ -100,7 +113,7 @@ int launch_first_vec(const void* labels, float* f, int64_t nlines, int64_t sx, c
 
 template <int Bytes>
 int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float w, int border, int flags,
-                 const XPlanes* planes, DeviceCache& dc, cudaStream_t stream) {
+                 const XPlanes* planes, DeviceCache& dc, cudaStream_t stream, PlanesMarch* march) {
   if (planes && !first_is_vec(labels, Bytes, f, sx))   // launch_first_vec refuses the rest
     return fail(EDTB200_EINVAL, "run-start planes asked of an X launch that cannot write them");
   StepTable step(dc, stream);
@@ -112,8 +125,9 @@ int launch_first(const void* labels, float* f, int64_t nlines, int64_t sx, float
   // register-resident vector kernel when rows are short and 16-byte aligned
   if (first_is_vec(labels, Bytes, f, sx)) {
 #define EDT_LAUNCH_VEC(KK)                                                                                        \
-  (flags == 0 ? launch_first_vec<Bytes, KK, true>(labels, f, nlines, sx, table, border, flags, stat, planes, dc, stream) \
-              : launch_first_vec<Bytes, KK, false>(labels, f, nlines, sx, table, border, flags, stat, planes, dc, stream))
+  (flags == 0                                                                                                    \
+       ? launch_first_vec<Bytes, KK, true>(labels, f, nlines, sx, table, border, flags, stat, planes, dc, stream, march) \
+       : launch_first_vec<Bytes, KK, false>(labels, f, nlines, sx, table, border, flags, stat, planes, dc, stream, march))
     const int rc = sx <= 128 ? EDT_LAUNCH_VEC(1) : sx <= 256 ? EDT_LAUNCH_VEC(2) : sx <= 512 ? EDT_LAUNCH_VEC(4)
                                                                                             : EDT_LAUNCH_VEC(8);
 #undef EDT_LAUNCH_VEC
@@ -507,7 +521,7 @@ int launch_expand_gather(const void* labels, const float* sqdist, const int32_t*
 #define EDT_INSTANTIATE_PASSES(B)                                                                        \
   template int edtb200::host::launch_first<B>(const void*, float*, int64_t, int64_t, float, int, int,    \
                                               const edtb200::XPlanes*, edtb200::host::DeviceCache&,      \
-                                              cudaStream_t);                                             \
+                                              cudaStream_t, edtb200::host::PlanesMarch*);                \
   template int edtb200::host::launch_later<B>(const void*, const edtb200::host::LaterNoise*, float*,     \
                                               const edtb200::LineGeom&, float, int, int, int,            \
                                               edtb200::host::PassArith, edtb200::host::DeviceCache&,     \

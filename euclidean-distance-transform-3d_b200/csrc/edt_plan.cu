@@ -11,11 +11,13 @@ bool later_pass_is_long(const LineGeom& g, PassArith arith, int max_smem_optin) 
   return plan_later(g, false, arith, max_smem_optin, true, false, false).kernel == 1;
 }
 
-NoisePlan noise_plan(const Transform& t, int64_t count, const void* labels, const float* f, const DeviceCache& dc) {
+NoisePlan noise_plan(const Transform& t, int64_t count, const void* labels, const float* f, const DeviceCache& dc,
+                     int noise) {
   // EDTB200_SETTLED_GROUP forces the later passes' group size (A/B switch for measurements)
   static const int forced_group = getenv("EDTB200_SETTLED_GROUP") ? atoi(getenv("EDTB200_SETTLED_GROUP")) : 0;
   return plan_noise(t, count, reinterpret_cast<uintptr_t>(f) % 16 == 0, first_is_vec(labels, t.label_bytes, f, t.n[0]),
-                    noise_predicted(dc), no_int_hull(), forced_group, dc.max_smem_optin, dc.sm_count);
+                    noise < 0 ? noise_predicted(dc) : noise != 0, no_int_hull(), forced_group, dc.max_smem_optin,
+                    dc.sm_count);
 }
 
 BoundedPlan bounded_plan(int ndim, const float w[3], double max_distance, bool sites) {

@@ -39,7 +39,7 @@ extern "C" {
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
  * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness,
- * edtb200_geodesic)
+ * edtb200_geodesic, edtb200_noise_planes)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -981,6 +981,39 @@ int edtb200_pass_window(const void *labels_dev, int label_bytes, int axis,
                         int border_lo, int border_hi, int flags, double max_distance,
                         const float *fin_dev, float *fout_dev, int *codes_dev,
                         int device, void *stream);
+
+/* edtb200_noise_planes : the X pass that a transform runs on label noise, for tests of that pass alone:
+ *     the pass that also writes the run-start and settled planes of the later passes (DESIGN.md section
+ *     4.1), over `count` volumes of (sx, sy, sz) laid end to end (2-D: images of (sx, sy)), on device
+ *     buffers, asynchronous on `stream`.  f_dev gets the distances, planes_dev the planes, in the layout
+ *     the transform uses, per later axis (y; in 3-D then z) the run-start plane and its settled plane:
+ *       [y plane | settled_y | z plane | settled_z]     rows = sy * sz * count, wpr = ceil(sx / 32)
+ *       run-start plane   wpr words per row (y, z), bit x % 32 of word x / 32: a y-run (z-run) starts
+ *                         at the voxel -- y == 0 or its label differs from row y - 1's (z within its
+ *                         own volume: z == 0 or its label differs from slice z - 1's); 0 past sx
+ *       settled plane     one word per row: bit s set when every voxel of x-segment s (32 voxels, padding
+ *                         voxels past sx counting as settled) ends the pass at f <= w_y^2 (w_z^2)
+ *     passes 1: the X pass.  passes 2: then the Y pass as a transform on predicted label noise plans it
+ *     (reading its plane, skipping settled tiles and refreshing settled_z where it does), so that f and
+ *     the planes are what the Z pass would find.  flags: 0 or EDTB200_SQRT (its sqrt applies in the Y
+ *     pass of a 2-D transform).  nchunks: y-chunks per slice of the pass's march, 1..sy (0: the
+ *     transform's own rule); ctas: its grid, 1..items, only with nchunks given (0: one persistent wave).
+ *     info (10 ints): label bytes, K (128-voxel blocks per row), Plain, planes written (1 or 2), the
+ *     march's nchunks, items and grid, and for passes 2 whether the Y pass read its plane, skipped
+ *     settled tiles and refreshed settled_z.  edtb200_last_later_launch reports the Y launch.  Refused
+ *     (EDTB200_EINVAL, before any device is touched) is every call a transform never sends down this
+ *     path: labels of 1 or 2 bytes, ndim 1, EDTB200_SIGNED or another flag, rows longer than 512 or not
+ *     a multiple of 4, more than 2^31 - 1 slices or 2^30 - 1 rows, nchunks or ctas out of range, and
+ *     pointers not aligned for vector access; passes 2 also where the transform would take no planes
+ *     (EDTB200_EINVAL after the probe).  Checks, in order: label width and sizes, label width >= 4,
+ *     ndim, count, weights, flags, passes, sx, counters, nchunks, ctas, emptiness, pointers, alignment,
+ *     then the device. */
+int edtb200_noise_planes(const void *labels_dev, int label_bytes, int ndim,
+                         int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                         float wx, float wy, float wz, int black_border, int flags,
+                         int passes, int nchunks, int ctas,
+                         float *f_dev, uint32_t *planes_dev, int *info,
+                         int device, void *stream);
 
 /* Z-slab decomposition across GPUs (DESIGN.md section 8): a rank runs edtb200_pass_later(axis=2)
  * on its slab with the interior faces open (border flags 0 there) and then folds the

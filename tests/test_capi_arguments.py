@@ -72,6 +72,16 @@ def _pass_window(labels=P, label_bytes=4, axis=1, sx=4, sy=4, sz=4, w=1.0, lo=0,
   return (labels, label_bytes, axis, sx, sy, sz, w, lo, hi, flags, d, fin, fout, codes, device, stream)
 
 
+_ALIGNED = np.zeros(32, np.uint64)
+PA = (_ALIGNED.ctypes.data + 63) // 64 * 64          # aligned for vector access by every label width
+
+
+def _noise_planes(labels=PA, label_bytes=4, ndim=3, sx=64, sy=8, sz=8, count=1, w=(1.0, 1.0, 1.0), border=0,
+                  flags=0, passes=1, nchunks=0, ctas=0, f=PA, planes=PA, info=P, device=63, stream=None):
+  return (labels, label_bytes, ndim, sx, sy, sz, count, *w, border, flags, passes, nchunks, ctas, f, planes, info,
+          device, stream)
+
+
 def _face_runs(labels=P, label_bytes=4, sx=4, sy=4, sz=4, high_face=0, halo=2, flags=0, m=P, overflow=P, device=63,
                stream=None):
   return (labels, label_bytes, sx, sy, sz, high_face, halo, flags, m, overflow, device, stream)
@@ -251,6 +261,58 @@ CASES = {
     ("valid_radius_128", dict(d=128.0, axis=2, flags=3), PROBE, ""),
     ("valid_radius_128_weight", dict(w=0.5, d=64.0), PROBE, ""),
     ("valid_with_codes", dict(codes=CODES, lo=1, hi=1), PROBE, ""),
+  ]),
+  "edtb200_noise_planes": (_noise_planes, [
+    ("label_bytes", dict(label_bytes=3), EINVAL, "label_bytes"),
+    ("label_bytes_1", dict(label_bytes=1), EINVAL, "labels of 4 or 8 bytes"),
+    ("label_bytes_2", dict(label_bytes=2), EINVAL, "labels of 4 or 8 bytes"),
+    ("ndim_1", dict(ndim=1), EINVAL, "2-D or 3-D"),
+    ("axis_too_long", dict(sz=BIG), ELIMIT, "axis longer than 2^30"),
+    ("count_0", dict(count=0), EINVAL, "count must be 1 or more"),
+    ("weight_0", dict(w=(1.0, 0.0, 1.0)), EINVAL, "weight"),
+    ("weight_nan", dict(w=(1.0, 1.0, float("nan"))), EINVAL, "weight"),
+    ("signed", dict(flags=SIGNED), EINVAL, "EDTB200_SIGNED"),
+    ("signed_sqrt", dict(flags=SIGNED | 1), EINVAL, "EDTB200_SIGNED"),
+    ("other_flag", dict(flags=LABELS_ON_DEVICE), EINVAL, "flags may only hold EDTB200_SQRT"),
+    ("passes_0", dict(passes=0), EINVAL, "passes must be 1 or 2"),
+    ("passes_3", dict(passes=3), EINVAL, "passes must be 1 or 2"),
+    ("sx_516", dict(sx=516), EINVAL, "rows of at most 512 voxels"),
+    ("sx_6", dict(sx=6), EINVAL, "a multiple of 4"),
+    ("slices_beyond_32_bits", dict(sz=1 << 30, count=2), EINVAL, "counts in 32 bits"),
+    ("rows_beyond_32_bits", dict(sy=1 << 30), EINVAL, "counts in 32 bits"),
+    ("nchunks_negative", dict(nchunks=-1), EINVAL, "nchunks must be 0 or 1..sy = 8"),
+    ("nchunks_above_sy", dict(nchunks=9), EINVAL, "nchunks must be 0 or 1..sy = 8"),
+    ("ctas_negative", dict(nchunks=2, ctas=-1), EINVAL, "ctas must be 0"),
+    ("ctas_without_nchunks", dict(ctas=1), EINVAL, "with nchunks given"),
+    ("ctas_above_items", dict(nchunks=2, ctas=3), EINVAL, "ctas must be 0 or 1..items = 2"),
+    ("ctas_above_items_3d_stack", dict(sz=3, count=3, nchunks=2, ctas=5), EINVAL, "1..items = 4"),
+    ("ctas_above_items_2d", dict(ndim=2, count=20, nchunks=1, ctas=4), EINVAL, "1..items = 3"),
+    ("null_labels", dict(labels=None), EINVAL, "null pointer"),
+    ("null_f", dict(f=None), EINVAL, "null pointer"),
+    ("null_planes", dict(planes=None), EINVAL, "null pointer"),
+    ("null_info", dict(info=None), EINVAL, "null pointer"),
+    ("labels_misaligned", dict(labels=PA + 4), EINVAL, "aligned for vector access"),
+    ("labels_misaligned_8", dict(labels=PA + 16, label_bytes=8), EINVAL, "aligned for vector access"),
+    ("f_misaligned", dict(f=PA + 4), EINVAL, "aligned for vector access"),
+    ("planes_misaligned", dict(planes=PA + 2), EINVAL, "aligned for vector access"),
+    # order: label width and sizes, label width >= 4, ndim, count, weights, flags, passes, sx, counters,
+    # nchunks, ctas, emptiness, pointers, alignment
+    ("label_bytes_before_ndim", dict(label_bytes=2, ndim=1), EINVAL, "labels of 4 or 8 bytes"),
+    ("ndim_before_count", dict(ndim=1, count=0), EINVAL, "2-D or 3-D"),
+    ("count_before_weight", dict(count=0, w=(0.0, 1.0, 1.0)), EINVAL, "count"),
+    ("weight_before_flags", dict(w=(0.0, 1.0, 1.0), flags=SIGNED), EINVAL, "weight"),
+    ("flags_before_passes", dict(flags=SIGNED, passes=0), EINVAL, "EDTB200_SIGNED"),
+    ("passes_before_sx", dict(passes=0, sx=6), EINVAL, "passes"),
+    ("sx_before_nchunks", dict(sx=516, nchunks=-1), EINVAL, "rows of at most 512 voxels"),
+    ("nchunks_before_ctas", dict(nchunks=9, ctas=1), EINVAL, "nchunks"),
+    ("ctas_before_empty", dict(nchunks=1, ctas=2, sx=0), EINVAL, "ctas"),
+    ("empty_before_null", dict(sx=0, labels=None, info=None), 0, ""),
+    ("null_before_alignment", dict(labels=None, f=PA + 4), EINVAL, "null pointer"),
+    # the weight of a missing axis is not read
+    ("valid", dict(), PROBE, ""),
+    ("valid_2d", dict(ndim=2, sz=-1, w=(1.0, 1.0, 0.0), count=20, nchunks=1, ctas=3), PROBE, ""),
+    ("valid_overrides", dict(nchunks=8, ctas=8, passes=2, flags=1, border=1), PROBE, ""),
+    ("valid_8_bytes", dict(label_bytes=8, sx=512, count=5), PROBE, ""),
   ]),
   "edtb200_slab_face_runs": (_face_runs, [
     ("label_bytes", dict(label_bytes=3), EINVAL, "label_bytes"),

@@ -39,7 +39,7 @@ __all__ = [
   "surface_distances", "SurfaceDistances", "hausdorff_distance", "average_surface_distance", "surface_dice",
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
   "parabolic_erode", "parabolic_dilate", "nearest_labels", "medial_axis",
-  "skeletonize", "local_thickness", "geodesic_distance",
+  "skeletonize", "local_thickness", "geodesic_distance", "watershed",
 ]
 
 FLAG_SQRT = 1
@@ -135,6 +135,8 @@ def _lib():
   lib.edtb200_skeletonize.restype = ci
   lib.edtb200_geodesic.argtypes = [vp, ci, vp, ci, ci, i64, i64, i64, i64, f32, f32, f32, ci, vp, vp, ci, vp]
   lib.edtb200_geodesic.restype = ci
+  lib.edtb200_watershed.argtypes = [vp, ci, vp, ci, vp, ci, i64, i64, i64, i64, ci, ci, vp, vp, ci, vp]
+  lib.edtb200_watershed.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1595,13 +1597,13 @@ def skeletonize(labels, anisotropy=None, black_border=False, *, return_distance=
 # shortest-path distances inside each label from seed voxels (edtb200_geodesic)
 # ---------------------------------------------------------------------------------------
 
-def _integer_bytes(dtype, what):
+def _integer_bytes(dtype, what, name="geodesic_distance"):
   """Width of a numpy or torch bool / integer dtype of 1, 2, 4 or 8 bytes; TypeError for anything else."""
   try:
     return _nearest_label_bytes(dtype)
   except TypeError:
-    raise TypeError("geodesic_distance: unsupported %s dtype %s: it must be an integer or bool dtype"
-                    % (what, dtype)) from None
+    raise TypeError("%s: unsupported %s dtype %s: it must be an integer or bool dtype"
+                    % (name, what, dtype)) from None
 
 
 def geodesic_distance(labels, seeds, anisotropy=None, *, return_indices=False, stacked=False, device=0):
@@ -1695,6 +1697,136 @@ def geodesic_distance(labels, seeds, anisotropy=None, *, return_indices=False, s
   if not return_indices:
     return dist
   return dist, planes
+
+
+# ---------------------------------------------------------------------------------------
+# marker-controlled flooding of an altitude image inside each label (edtb200_watershed)
+# ---------------------------------------------------------------------------------------
+
+def _like_volume(v, data, what, name):
+  """`data` on the side and in the memory order of the volume `v`: host data is moved to v's GPU when v is
+  device-resident; device data with a host volume is a TypeError; a shape other than v's a ValueError."""
+  t = _device_array(data)
+  if v.on_device:
+    import torch
+    x = torch.as_tensor(data if t is None else t, device=v.arr.device)
+  elif t is not None:
+    raise TypeError("%s: %s is a GPU array but the volume is a host array; pass every array on the same side"
+                    % (name, what))
+  else:
+    x = np.asarray(data)
+  if tuple(x.shape) != v.shape:
+    raise ValueError("%s: %s must have the volume's shape %s, got %s" % (name, what, v.shape, tuple(x.shape)))
+  return x
+
+
+def _in_volume_order(v, x):
+  """x (already on v's side and of v's shape) in v's memory order, contiguous."""
+  if not v.on_device:
+    return np.asfortranarray(x) if v.fortran else np.ascontiguousarray(x)
+  if v.fortran:
+    back = tuple(range(v.nd - 1, -1, -1))
+    return x.permute(*back).contiguous().permute(*back)
+  return x.contiguous()
+
+
+def _real_float32(x, name):
+  """x as float32 (once, where it is another real dtype); a TypeError for complex and non-numeric dtypes."""
+  if isinstance(x, np.ndarray):
+    if x.dtype.kind not in "biuf":
+      raise TypeError("%s: unsupported image dtype %s: it must be a real dtype" % (name, x.dtype))
+    return x if x.dtype == np.float32 else x.astype(np.float32)
+  import torch
+  if x.dtype.is_complex:
+    raise TypeError("%s: unsupported image dtype %s: it must be a real dtype" % (name, x.dtype))
+  return x if x.dtype == torch.float32 else x.to(torch.float32)
+
+
+def watershed(image, markers, labels=None, *, connectivity=1, return_level=False, stacked=False, device=0):
+  """Watershed: marker-controlled flooding of an altitude image inside each label, on the GPU.  The usual
+  split of touching objects is
+      dist = edt(mask); markers = <one marker per maximum of dist>; watershed(-dist, markers, mask)
+  (skimage.segmentation.watershed's mask=m is labels=m here: flooding stays inside each label).
+
+  Definition.  Volumes are x-fastest, as for edt(): x is the last axis of a C-ordered array and the first of
+  an F-ordered one.
+    graph     every voxel with a non-zero label is a node (labels=None: every voxel, all with one label); two
+              nodes are joined when they are neighbours under `connectivity` with the same label: an offset
+              counts when at most `connectivity` of its components are non-zero (3-D 1/2/3: 6/18/26
+              neighbours, 2-D 1/2: 4/8), as in scipy and skimage.  Label 0 and the outside of the volume
+              cannot be crossed.
+    altitude  f = image as float32; NaN is read as +inf and -0.0 as +0.0; +inf and -inf are valid altitudes.
+    seeds     a voxel is a seed when its marker and its label are both non-zero; markers on label 0 are
+              ignored.  Marker values are compared as unsigned integers of the markers' width.
+    level     L is the least fixed point of L[v] = min(L[v], max(f[v], L[u])) over the graph neighbours u of
+              v, from f on the seeds and +inf elsewhere: the lowest flood level at which water from some seed
+              reaches v.  It is exact: min and max round nothing.
+    result    an edge u -> v is tight when v is not a seed and L[v] == max(f[v], L[u]).  W = the marker on
+              the seeds; elsewhere W[v] is the least marker m with a tight path from a seed of marker m to v
+              whose voxels after the first are non-seeds, and 0 where there is none and on label 0.
+  The result equals this definition bit for bit on every run, whatever order the GPU floods in.  Ties: a
+  voxel reached at the same level from two markers goes to the smaller marker value, and plateaus are not
+  split by distance.  skimage breaks such ties by the order of its queue, so the two agree on every voxel
+  but the tied ones.
+
+  Examples.  Two basins in 1-D split at the ridge between them:
+      image = np.array([0, 3, 1, 5, 2, 0], np.float32)
+      markers = np.array([1, 0, 0, 0, 0, 2], np.uint8)
+      watershed(image, markers)  ->  [1, 1, 1, 1, 2, 2]
+  (the ridge voxel is reached at level 5 from both sides and goes to the smaller marker), and
+      watershed(image, markers, return_level=True)[1]  ->  [0, 3, 3, 5, 2, 0]
+  (the pit of altitude 1 fills up to the 3 that water from marker 1 must pass).
+  Two touching discs split at the neck:
+      dist = edt(mask); split = watershed(-dist, markers, mask)
+
+  Input and output.  `image`: any real dtype, 1-D to 3-D, or with stacked=True 2-D to 4-D whose slowest axis
+  in memory indexes same-shaped volumes, as edt(stacked=True); the result equals np.stack of the per-volume
+  calls.  Anything but float32 is converted to float32 once (float64 altitudes that differ only below
+  float32's precision become equal, and may tie).  `markers`: bool or integer dtypes of 1, 2, 4 or 8 bytes.
+  `labels`: None, or bool or integer dtypes of 1, 2, 4 or 8 bytes (float labels are a TypeError).  Every
+  array has the same shape (a ValueError otherwise) and is read in the memory order of `labels` (of `image`
+  when labels is None), copied into it where its own differs.  `connectivity`: an int from 1 to the number
+  of volume axes.  Returns W in the markers' dtype (bool markers give uint8) with the volume's shape and
+  memory order, or with return_level=True `(W, level)`, level float32 (+inf on label 0 and where no seed
+  is reachable at a finite level).  numpy in gives numpy out; a torch CUDA tensor (or any
+  __cuda_array_interface__ array) gives torch CUDA tensors computed on the current stream without a host
+  synchronisation: each phase is one cooperative kernel; host arrays passed with it are moved to its GPU.
+  A host array that does not fit on the GPU raises EDTError with code ENOMEM (there is no chunked path).
+
+  Cost.  The GPU floods 8x8x8 tiles (2-D 16x16, 1-D 256) in rounds, each round re-relaxing the tiles whose
+  halo changed, first for the level and then for the markers over the tight edges.  Device memory beyond
+  the inputs and the outputs: 4 bytes per voxel for the level, 4 for the markers (8 for 8-byte markers), and
+  12 bytes per tile."""
+  name = "watershed"
+  if not isinstance(return_level, (bool, np.bool_)):
+    raise TypeError("%s: return_level must be True or False, got %r" % (name, return_level))
+  if isinstance(connectivity, (bool, np.bool_)) or not isinstance(connectivity, (int, np.integer)):
+    raise TypeError("%s: connectivity must be an int, got %r" % (name, connectivity))
+  ref = image if labels is None else labels
+  v = _Volume(name, ref, stacked, (1, 3), device)
+  if not 1 <= connectivity <= v.vnd:
+    raise ValueError("%s: connectivity must be 1 to %d for %d-D volumes, got %d" % (name, v.vnd, v.vnd, connectivity))
+  nbytes = 0 if labels is None else _integer_bytes(v.dtype, "label", name)
+  mk = _like_volume(v, markers, "markers", name)
+  marker_bytes = _integer_bytes(mk.dtype, "marker", name)
+  img = v.arr if labels is None else _like_volume(v, image, "image", name)
+  img = _in_volume_order(v, _real_float32(img, name))
+  mk = _in_volume_order(v, mk)
+  v.set_weights(None, positive=False)
+  # W in the markers' dtype, bool as uint8
+  if v.on_device:
+    import torch
+    out_dtype = "uint8" if mk.dtype == torch.bool else str(mk.dtype).split(".")[-1]
+  else:
+    out_dtype = "uint8" if mk.dtype == np.bool_ else mk.dtype.name
+  out = v.empty(out_dtype)
+  level = v.empty("float32") if return_level else None
+  if v.size:
+    vnd, sx, sy, sz, count = v.geometry[:5]
+    _check(_lib().edtb200_watershed(None if labels is None else v.ptr, nbytes, v.ptr_of(mk), marker_bytes,
+                                    v.ptr_of(img), vnd, sx, sy, sz, count, int(connectivity), v.flags, v.ptr_of(out),
+                                    v.ptr_of(level), *v.where))
+  return (out, level) if return_level else out
 
 
 # ---------------------------------------------------------------------------------------

@@ -2291,6 +2291,106 @@ int edtb200_geodesic(const void* labels, int label_bytes, const void* seeds, int
   return rc ? rc : io.finish();
 }
 
+int edtb200_watershed(const void* labels, int label_bytes, const void* markers, int marker_bytes, const float* image,
+                      int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, int connectivity, int flags,
+                      void* out, float* level_out, int device, void* stream_v) {
+  if (!(label_bytes == 0 || label_bytes == 1 || label_bytes == 2 || label_bytes == 4 || label_bytes == 8))
+    return fail(EDTB200_EINVAL, "label_bytes must be 0 (no labels), 1, 2, 4 or 8 (got %d)", label_bytes);
+  if (!(marker_bytes == 1 || marker_bytes == 2 || marker_bytes == 4 || marker_bytes == 8))
+    return fail(EDTB200_EINVAL, "marker_bytes must be 1, 2, 4 or 8 (got %d)", marker_bytes);
+  int rc = check_dims(label_bytes ? label_bytes : 1, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (connectivity < 1 || connectivity > ndim)
+    return fail(EDTB200_EINVAL, "connectivity must be 1 to ndim (%d) (got %d)", ndim, connectivity);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_watershed takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if ((rc = check_stack(vol, count, 1))) return rc;
+  // the worklists hold 4-byte tile numbers
+  const int64_t ntiles = geodesic_tiles(ndim, sx, sy, sz, count);
+  if (ntiles >= ((int64_t)1 << 32)) return fail(EDTB200_ELIMIT, "edtb200_watershed takes stacks of fewer than 2^32 tiles");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if ((label_bytes && !labels) || !markers || !image || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, marker_size = (size_t)total * (size_t)marker_bytes;
+  const size_t image_bytes = sizeof(float) * (size_t)total, out_bytes = marker_size;
+  // outputs against the inputs (on the same side) and against each other
+  const void* outs[2] = {out, level_out};
+  const size_t outs_bytes[2] = {out_bytes, image_bytes};
+  static const char* names[2] = {"out", "level_out"};
+  for (int i = 0; i < 2; ++i) {
+    if (!outs[i]) continue;
+    if (same_side(flags) && label_bytes && overlaps(labels, lab_bytes, outs[i], outs_bytes[i]))
+      return fail(EDTB200_EINVAL, "%s overlaps labels", names[i]);
+    if (same_side(flags) && overlaps(markers, marker_size, outs[i], outs_bytes[i]))
+      return fail(EDTB200_EINVAL, "%s overlaps markers", names[i]);
+    if (same_side(flags) && overlaps(image, image_bytes, outs[i], outs_bytes[i]))
+      return fail(EDTB200_EINVAL, "%s overlaps image", names[i]);
+  }
+  if (level_out && overlaps(out, out_bytes, level_out, image_bytes))
+    return fail(EDTB200_EINVAL, "level_out overlaps out");
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  const cudaStream_t s = io.stream;
+  // host buffers are staged whole: the labels and levels through this device's cached buffers, the markers,
+  // the image and the result through scratch
+  const void* d_labels = nullptr;
+  const void* d_markers = nullptr;
+  const float* d_image = nullptr;
+  void* d_out = nullptr;
+  float* d_level = nullptr;
+  Scratch marker_stage, image_stage, out_stage, values, wsheds, tiles;
+  if (label_bytes && (rc = io.in_labels(labels, lab_bytes, &d_labels))) return rc;
+  if (level_out && (rc = io.out_dist(level_out, image_bytes, &d_level))) return rc;
+  if (!io.in_dev && ((rc = marker_stage.take(*io.dc, marker_size, s, "the staged markers")) ||
+                     (rc = image_stage.take(*io.dc, image_bytes, s, "the staged image"))))
+    return rc;
+  if ((rc = io.in(markers, marker_size, marker_stage.get(), &d_markers)) ||
+      (rc = io.in(image, image_bytes, image_stage.get(), &d_image)) ||
+      (rc = io.out_staged(out, out_bytes, out_stage, "the watershed labels", &d_out)))
+    return rc;
+  // scratch: L, W, one flag and two list entries per tile, and the two control blocks
+  WatershedScratch g;
+  g.ntiles = ntiles;
+  const size_t tile_bytes = 3 * sizeof(uint32_t) * (size_t)ntiles, l_bytes = sizeof(float) * (size_t)total;
+  const size_t w_bytes = (marker_bytes == 8 ? 8 : 4) * (size_t)total;
+  if ((rc = values.take(*io.dc, l_bytes, s, "the watershed levels")) ||
+      (rc = wsheds.take(*io.dc, w_bytes, s, "the watershed markers")) ||
+      (rc = tiles.take(*io.dc, tile_bytes + watershed_control_bytes(), s, "the watershed worklists")))
+    return rc;
+  g.level = values.get<float>();
+  g.w = wsheds.get();
+  // the control blocks first: they hold 8-byte counters, and 3 * ntiles words may end off an 8-byte boundary
+  g.control = tiles.get();
+  g.flag = reinterpret_cast<uint32_t*>(tiles.get<char>() + watershed_control_bytes());
+  g.list = g.flag + ntiles;
+
+  // steps: the levels, the labels, the store
+  StepTimer timer(s);
+  timer.stamp();
+  rc = launch_watershed_phase(d_labels, label_bytes, d_markers, marker_bytes, d_image, ndim, sx, sy, sz, count,
+                              connectivity, g, false, *io.dc, s);
+  timer.stamp();
+  if (!rc)
+    rc = launch_watershed_phase(d_labels, label_bytes, d_markers, marker_bytes, d_image, ndim, sx, sy, sz, count,
+                                connectivity, g, true, *io.dc, s);
+  timer.stamp();
+  if (!rc) rc = launch_watershed_store(ndim, sx, sy, sz, count, marker_bytes, g, d_out, d_level, *io.dc, s);
+  timer.stamp();
+  if (!rc && timer.synchronize()) {
+    unsigned long long n[4] = {0, 0, 0, 0};
+    watershed_stats(g.control, n);
+    fprintf(stderr, "[edt_b200] watershed %lldx%lldx%lld x%lld L=%d M=%d c=%d  levels %.3f ms (rounds %llu, tile visits "
+                    "%llu)  labels %.3f ms (rounds %llu, tile visits %llu)  store %.3f ms  tiles %lld  scratch %zu bytes\n",
+            (long long)sx, (long long)sy, (long long)sz, (long long)count, label_bytes, marker_bytes, connectivity,
+            timer.ms(0, 1), n[0], n[1], timer.ms(1, 2), n[2], n[3], timer.ms(2, 3), (long long)ntiles,
+            l_bytes + w_bytes + tile_bytes + watershed_control_bytes());
+  }
+  return rc ? rc : io.finish();
+}
+
 // The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
 static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
                           const float w[3], int k, double max_distance) {

@@ -1,6 +1,6 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as fifteen translation units so that the kernel templates build in
+// The library is compiled as sixteen translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
@@ -8,8 +8,8 @@
 // spherical morphology's label-writing stores), edt_parabolic.cu (the parabolic erosion and
 // dilation passes), edt_nearest.cu (the nearest-labels passes), edt_medial.cu (the medial
 // axis's mark kernel), edt_skeleton.cu (the skeleton's thinning kernel), edt_thickness.cu
-// (local thickness's levels, seeds and stores) and edt_geodesic.cu (geodesic_distance's relaxation
-// passes).  The run-time label width
+// (local thickness's levels, seeds and stores), edt_geodesic.cu (geodesic_distance's relaxation
+// passes) and edt_watershed.cu (watershed's relaxation passes).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -472,6 +472,33 @@ int launch_geodesic_store(int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t 
 size_t geodesic_control_bytes();
 // The rounds and tile visits of the distance and index phases of the last call on `control` (synchronous).
 int geodesic_stats(const void* control, unsigned long long out[4]);
+
+// The scratch of watershed (edt_watershed.cu): L (one float per voxel), W (4 bytes per voxel, 8 for 8-byte
+// markers), one flag per tile and two worklists of `ntiles` (geodesic_tiles) 4-byte entries, and the control
+// blocks of the two phases (watershed_control_bytes()).
+struct WatershedScratch {
+  float* level = nullptr;
+  void* w = nullptr;
+  uint32_t* flag = nullptr;
+  uint32_t* list = nullptr;
+  void* control = nullptr;
+  int64_t ntiles = 0;
+};
+
+// One phase of watershed (edt_watershed.cu): its seed kernel, then ONE cooperative launch of
+// watershed_relax_kernel that runs every round.  label_phase false: L from the seeds; true: W over the tight
+// edges of the fixed L.  label_bytes 0: no labels.
+int launch_watershed_phase(const void* labels, int label_bytes, const void* markers, int marker_bytes,
+                           const float* image, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                           int connectivity, const WatershedScratch& g, bool label_phase, DeviceCache& dc,
+                           cudaStream_t stream);
+// W into `out` in the markers' width (0 where there is none) and, with level_out (null: none), L.
+int launch_watershed_store(int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count, int marker_bytes,
+                           const WatershedScratch& g, void* out, float* level_out, DeviceCache& dc,
+                           cudaStream_t stream);
+size_t watershed_control_bytes();
+// The rounds and tile visits of the level and label phases of the last call on `control` (synchronous).
+int watershed_stats(const void* control, unsigned long long out[4]);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

@@ -39,7 +39,7 @@ extern "C" {
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
  * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness,
- * edtb200_geodesic, edtb200_noise_planes)
+ * edtb200_geodesic, edtb200_noise_planes, edtb200_watershed)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -548,6 +548,62 @@ int edtb200_skeletonize(const void *labels, int label_bytes, int ndim, int64_t s
 int edtb200_geodesic(const void *labels, int label_bytes, const void *seeds, int seed_bytes, int ndim,
                      int64_t sx, int64_t sy, int64_t sz, int64_t count, float wx, float wy, float wz,
                      int flags, float *dist_out, int32_t *const *idx_out, int device, void *stream);
+
+/* Watershed: marker-controlled flooding of an altitude image inside each label (splitting touching objects:
+ * markers at the maxima of edt(mask), then the watershed of -edt).  Volumes are x-fastest, as everywhere here.
+ *   graph     every voxel with a non-zero label is a node (label_bytes 0: every voxel, all with one label);
+ *             two nodes are joined when they are neighbours under `connectivity` with the SAME label: an
+ *             offset in {-1, 0, 1}^ndim counts when at most `connectivity` of its components are non-zero
+ *             (3-D 1/2/3: 6/18/26 neighbours, 2-D 1/2: 4/8, 1-D 1: 2), as in scipy and skimage.  Label 0 and
+ *             the outside of the volume cannot be crossed.
+ *   altitude  f = image as float32, NaN read as +inf and -0.0 as +0.0; +inf and -inf are valid altitudes.
+ *   seeds     a voxel is a seed when its marker AND its label are non-zero (markers on label 0 are ignored).
+ *             Marker values are compared as unsigned integers of marker_bytes.
+ *   level     L is the least fixed point of L[v] = min(L[v], max(f[v], L[u])) over the graph neighbours u of
+ *             v, from f on the seeds and +inf elsewhere: the lowest flood level at which water from some seed
+ *             reaches v.  min and max round nothing, so L is exact.
+ *   result    an edge u -> v is TIGHT when v is not a seed and L[v] == max(f[v], L[u]).  W[s] = marker[s] on
+ *             the seeds; elsewhere W[v] is the least marker m with a tight path from a seed of marker m to
+ *             v whose voxels after the first are non-seeds, and 0 where there is none and on label 0.
+ *             Deterministic, independent of the order of evaluation, also on plateaus.  Ties (a voxel reached
+ *             at the same level from two markers) go to the smaller marker; plateaus are not split by
+ *             distance.
+ *
+ *   labels, label_bytes    count * sx*sy*sz labels of 1, 2, 4 or 8 bytes (integers: compared by their bits),
+ *                          volumes back to back as for edtb200_transform_stack; label_bytes 0: no labels
+ *                          (labels is not read)
+ *   markers, marker_bytes  count * sx*sy*sz markers of 1, 2, 4 or 8 bytes, laid out like the volume
+ *   image                  count * sx*sy*sz float32 altitudes, laid out like the volume
+ *   connectivity           1 to ndim
+ *   flags                  the residency flags only (EDTB200_LABELS_ON_DEVICE covers every input; both on
+ *                          the device: asynchronous on `stream`, no lock and no host wait; host buffers are
+ *                          staged whole, EDTB200_ENOMEM when they do not fit -- there is no chunked path)
+ *   out                    count * sx*sy*sz markers of marker_bytes: W
+ *   level_out              NULL, or count * sx*sy*sz float32 on the side of out: L (+inf on label 0)
+ * Kernels, on one stream, on the tiles and worklists of edtb200_geodesic (8x8x8 voxels, 2-D 16x16, 1-D 256).
+ * The levels: a seed kernel writes L (f / +inf) and queues the tiles that hold a seed; then ONE cooperative
+ * launch of watershed_relax_kernel runs every round with a grid barrier between them.  A round's CTAs each
+ * stage a tile and a one-voxel halo of L and labels in shared memory, relax it in sweeps of min over the
+ * neighbours of max(f[v], L[u]) until a sweep lowers nothing, write back the voxels that went down and queue
+ * each neighbour tile that a lowered voxel on a face, edge or corner touches through the connectivity (in
+ * round 1 the seeds count as lowered, so a seed on a tile's border reaches past it).  The labels: the same
+ * rounds on W = marker - 1 (all ones: none) with L fixed, by min over the tight edges, queued on changes of W
+ * (a voxel of altitude +inf has L = +inf and can still take a W); the seeds are never written.  A store kernel
+ * writes W in the markers' width and L.  Every halo read is an aligned 4- or 8-byte load (W is 4 bytes for
+ * markers of up to 4 bytes, 8 for 8-byte markers), never torn; values only decrease, so a stale value is an
+ * upper bound and the owner's write queues the reader again; there is no round cap.
+ * Device memory beyond the inputs and outputs: 4 bytes per voxel for L, 4 for W (8 with 8-byte markers),
+ * 12 bytes per tile, 64 bytes of control blocks, and the staged markers, image and result of a host call.
+ * Checks, in order: label width, marker width, ndim and sizes (as edtb200_transform), count >= 0,
+ * connectivity, flags, the stack's size (within 2^62 voxels), its tiles (fewer than 2^32, else
+ * EDTB200_ELIMIT: the worklists hold 4-byte tile numbers), emptiness (returns 0 touching nothing), pointers
+ * (labels unless label_bytes is 0, markers, image, out), overlaps (no output may overlap an input when on the
+ * same side, nor the other output), device.
+ * EDT_B200_VERBOSE=1 prints the device time of the levels, labels and store, and the rounds and tile visits
+ * of each phase, on stderr. */
+int edtb200_watershed(const void *labels, int label_bytes, const void *markers, int marker_bytes,
+                      const float *image, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                      int connectivity, int flags, void *out, float *level_out, int device, void *stream);
 
 /* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
  * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between

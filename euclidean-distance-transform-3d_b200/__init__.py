@@ -40,6 +40,7 @@ __all__ = [
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
   "parabolic_erode", "parabolic_dilate", "nearest_labels", "medial_axis",
   "skeletonize", "local_thickness", "geodesic_distance", "watershed",
+  "connected_components", "extended_maxima",
 ]
 
 FLAG_SQRT = 1
@@ -137,6 +138,10 @@ def _lib():
   lib.edtb200_geodesic.restype = ci
   lib.edtb200_watershed.argtypes = [vp, ci, vp, ci, vp, ci, i64, i64, i64, i64, ci, ci, vp, vp, ci, vp]
   lib.edtb200_watershed.restype = ci
+  lib.edtb200_connected_components.argtypes = [vp, ci, ci, i64, i64, i64, i64, ci, ci, vp, ci, ci, vp]
+  lib.edtb200_connected_components.restype = ci
+  lib.edtb200_extended_maxima.argtypes = [vp, ci, vp, ci, i64, i64, i64, i64, ctypes.c_double, ci, ci, vp, ci, ci, vp]
+  lib.edtb200_extended_maxima.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1827,6 +1832,141 @@ def watershed(image, markers, labels=None, *, connectivity=1, return_level=False
                                     v.ptr_of(img), vnd, sx, sy, sz, count, int(connectivity), v.flags, v.ptr_of(out),
                                     v.ptr_of(level), *v.where))
   return (out, level) if return_level else out
+
+
+# ---------------------------------------------------------------------------------------
+# connected components and extended maxima (edtb200_connected_components, edtb200_extended_maxima)
+# ---------------------------------------------------------------------------------------
+
+_COMPONENTS_GRAPH = """
+    graph      every voxel with a non-zero label is a node (extended_maxima with labels=None: every voxel, all
+               with one label); two nodes are joined when they are neighbours under `connectivity` with the
+               same label: an offset counts when at most `connectivity` of its components are non-zero (3-D
+               1/2/3: 6/18/26 neighbours, 2-D 1/2: 4/8), as in scipy and skimage.  Label 0 and the outside of
+               the volume cannot be crossed.
+    numbering  each component is numbered 1..n in increasing order of its least voxel index in memory order,
+               everything else 0.  For a C-ordered array this is scipy.ndimage.label's numbering; for an
+               F-ordered one it is that numbering of a.T, transposed back."""
+
+_COMPONENTS_IO = """
+  Input and output.  Volumes are x-fastest, as for edt(): x is the last axis of a C-ordered array and the first
+  of an F-ordered one.  1-D to 3-D arrays, or with stacked=True 2-D to 4-D whose slowest axis in memory indexes
+  same-shaped volumes; each volume is numbered on its own from 1, so the result equals np.stack of the
+  per-volume calls bit for bit.  Labels are bool or integer dtypes of 1, 2, 4 or 8 bytes (float labels are a
+  TypeError).  The result is int32 when each volume has fewer than 2^31 voxels, else int64, with the volume's
+  shape and memory order.  numpy in gives numpy out; a torch CUDA tensor (or any __cuda_array_interface__
+  array) gives a torch CUDA tensor computed on the current stream without a host synchronisation.  A host
+  array that does not fit on the GPU raises EDTError with code ENOMEM (there is no chunked path)."""
+
+
+def _components_out(v):
+  """The result of a components call on the volume v (after set_weights): int32 when each volume has fewer
+  than 2^31 voxels, else int64; and its width."""
+  sx, sy, sz = v.geometry[1:4]
+  out_bytes = 4 if sx * sy * sz < (1 << 31) else 8
+  return v.empty("int32" if out_bytes == 4 else "int64"), out_bytes
+
+
+def _connectivity(name, connectivity, v):
+  if isinstance(connectivity, (bool, np.bool_)) or not isinstance(connectivity, (int, np.integer)):
+    raise TypeError("%s: connectivity must be an int, got %r" % (name, connectivity))
+  if not 1 <= connectivity <= v.vnd:
+    raise ValueError("%s: connectivity must be 1 to %d for %d-D volumes, got %d" % (name, v.vnd, v.vnd, connectivity))
+  return int(connectivity)
+
+
+_CONNECTED_COMPONENTS_DOC = ("""Connected components of every label, numbered, on the GPU: cc3d.connected_components, or
+  scipy.ndimage.label applied to each label at once.
+
+  Definition.""" + _COMPONENTS_GRAPH + """
+  The default connectivity=1 is scipy's and watershed's; cc3d's default of 26 is connectivity=3.
+
+  Examples (2-D, C order):
+      connected_components(np.array([[1, 1, 0, 2], [0, 1, 0, 2], [3, 0, 0, 1]]))
+        ->  [[1, 1, 0, 2], [0, 1, 0, 2], [3, 0, 0, 4]]
+      connected_components(np.array([[1, 0], [0, 1]]))                   ->  [[1, 0], [0, 2]]
+      connected_components(np.array([[1, 0], [0, 1]]), connectivity=2)   ->  [[1, 0], [0, 1]]
+""" + _COMPONENTS_IO + """
+
+  Cost.  Union-find whose cost does not grow with a component's diameter: a tile pass in shared memory, a
+  border pass of lock-free unions in global memory, a flatten pass, a prefix sum and a number pass.  Device
+  memory beyond the input and the output: 4 bytes per voxel of parents and the scan's scratch.""")
+
+
+def connected_components(labels, *, connectivity=1, stacked=False, device=0):
+  name = "connected_components"
+  v = _Volume(name, labels, stacked, (1, 3), device)
+  conn = _connectivity(name, connectivity, v)
+  nbytes = _integer_bytes(v.dtype, "label", name)
+  v.set_weights(None, positive=False)
+  out, out_bytes = _components_out(v)
+  if v.size:
+    vnd, sx, sy, sz, count = v.geometry[:5]
+    _check(_lib().edtb200_connected_components(v.ptr, nbytes, vnd, sx, sy, sz, count, conn, v.flags, v.ptr_of(out),
+                                               out_bytes, *v.where))
+  return out
+
+
+connected_components.__doc__ = _CONNECTED_COMPONENTS_DOC
+
+
+_EXTENDED_MAXIMA_DOC = ("""Extended maxima: the regional maxima of the h-maxima transform (Soille's EMAX_h, MATLAB's imextendedmax),
+  numbered, on the GPU.  They are the markers of the usual split of touching objects:
+      dist = edt(mask); markers = extended_maxima(dist, h, mask); watershed(-dist, markers, mask)
+  and extended_maxima(-f, h) gives the minima markers of an unseeded watershed(f, ...) (NaN, read as -inf here
+  and as +inf by watershed, never becomes a marker).
+
+  Definition.""" + _COMPONENTS_GRAPH + """
+    image      f = image as float32, NaN read as -inf and -0.0 as +0.0.  `h` is a finite real >= 0 (a
+               ValueError otherwise); m = fl32(fl64(f) - fl64(h)), -0.0 read as +0.0, so m <= f and h = 0
+               gives m = f.
+    R          the least fixed point of R[v] = max(R[v], min(f[v], R[u])) over the joined neighbours u of v,
+               from m: the reconstruction by dilation of m under f.  It is exact: min and max round nothing.
+    plateau    a component of the graph restricted to the edges with R[u] == R[v]; it is a maximum when no
+               node in it has a joined neighbour with a larger R, and its R is not -inf.
+    result     the maximum plateaus, numbered as above.
+  When f - h is exact in float32, a peak survives exactly when its dynamic -- its height above the highest
+  pass to a higher voxel of its label -- exceeds h.  skimage.morphology.h_maxima keeps dynamics >= h and
+  returns only the top plateau of each survivor; here a peak whose dynamic equals h is merged, and a survivor
+  is marked by the whole plateau of R at its top, which reaches h below the peak.
+
+  Examples (1-D):
+      extended_maxima(np.array([0, 3, 1, 5, 2, 0.]))         ->  [0, 1, 0, 2, 0, 0]   (h=1.9 the same)
+      extended_maxima(np.array([0, 3, 1, 5, 2, 0.]), h=2)    ->  [0, 0, 0, 1, 0, 0]   (the peak at 1 has dynamic 2)
+      extended_maxima(np.array([0, 4, 3.5, 4, 0.]), h=0.4)   ->  [0, 1, 0, 2, 0]
+      extended_maxima(np.array([0, 4, 3.5, 4, 0.]), h=0.5)   ->  [0, 1, 1, 1, 0]
+""" + _COMPONENTS_IO + """  The image may be any real dtype and is converted
+  to float32 once; it is read in the memory order of `labels` (of `image` when labels is None).
+
+  Cost.  With h = 0, R = f and the plateaus are labelled by the union-find passes of connected_components with
+  the key (label, R), then a mark pass drops the plateaus with a larger neighbour.  With h > 0, R first comes
+  from watershed's level phase on negated values, which floods 8x8x8 tiles in rounds (its cost grows with the
+  distance R has to travel).  Device memory beyond the inputs and the output: 4 bytes per voxel of parents and
+  the scan's scratch, and with h > 0 another 4 + 4 bytes per voxel and 12 bytes per tile.""")
+
+
+def extended_maxima(image, h=0.0, labels=None, *, connectivity=1, stacked=False, device=0):
+  name = "extended_maxima"
+  if isinstance(h, (bool, np.bool_)) or not isinstance(h, (int, float, np.integer, np.floating)):
+    raise TypeError("%s: h must be a real number, got %r" % (name, h))
+  if not (math.isfinite(float(h)) and float(h) >= 0.0):
+    raise ValueError("%s: h must be finite and >= 0, got %r" % (name, h))
+  ref = image if labels is None else labels
+  v = _Volume(name, ref, stacked, (1, 3), device)
+  conn = _connectivity(name, connectivity, v)
+  nbytes = 0 if labels is None else _integer_bytes(v.dtype, "label", name)
+  img = v.arr if labels is None else _like_volume(v, image, "image", name)
+  img = _in_volume_order(v, _real_float32(img, name))
+  v.set_weights(None, positive=False)
+  out, out_bytes = _components_out(v)
+  if v.size:
+    vnd, sx, sy, sz, count = v.geometry[:5]
+    _check(_lib().edtb200_extended_maxima(None if labels is None else v.ptr, nbytes, v.ptr_of(img), vnd, sx, sy, sz,
+                                          count, float(h), conn, v.flags, v.ptr_of(out), out_bytes, *v.where))
+  return out
+
+
+extended_maxima.__doc__ = _EXTENDED_MAXIMA_DOC
 
 
 # ---------------------------------------------------------------------------------------

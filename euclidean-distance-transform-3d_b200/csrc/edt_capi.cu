@@ -2391,6 +2391,164 @@ int edtb200_watershed(const void* labels, int label_bytes, const void* markers, 
   return rc ? rc : io.finish();
 }
 
+// The checks edtb200_connected_components and edtb200_extended_maxima share after their own, in their
+// documented order: out_bytes, the stack's size, the volume's size (parents are 4-byte indices within a volume)
+// and the output width against it.
+static int components_checks(const char* name, int64_t vol, int64_t count, int out_bytes) {
+  if (out_bytes != 4 && out_bytes != 8) return fail(EDTB200_EINVAL, "out_bytes must be 4 or 8 (got %d)", out_bytes);
+  if (const int rc = check_stack(vol, count, 1)) return rc;
+  if (vol >= ((int64_t)1 << 32)) return fail(EDTB200_ELIMIT, "%s takes volumes of fewer than 2^32 voxels", name);
+  if (out_bytes == 4 && vol >= ((int64_t)1 << 31))
+    return fail(EDTB200_EINVAL, "out_bytes 4 needs volumes of fewer than 2^31 voxels (got %lld)", (long long)vol);
+  return 0;
+}
+
+// The union-find passes and the numbering of one call, device buffers in place; h > 0 first reconstructs -R
+// from the image.  Prints the phases with EDT_B200_VERBOSE.
+static int components_run(const char* name, ComponentsJob j, const float* image, double h, void* out, HostIO& io) {
+  const cudaStream_t s = io.stream;
+  const int64_t total = j.sx * j.sy * j.sz * j.count;
+  const size_t temp_bytes = components_temp_bytes(total, j.count, j.out_bytes);
+  const size_t p_bytes = sizeof(uint32_t) * (size_t)total;
+  Scratch parents, temp, values, tiles;
+  int rc;
+  if ((rc = parents.take(*io.dc, p_bytes, s, "the component parents")) ||
+      (rc = temp.take(*io.dc, temp_bytes, s, "the component numbering")))
+    return rc;
+  j.parent = parents.get<uint32_t>();
+  size_t extra = 0;
+  WatershedScratch g;
+  if (image && h > 0.0) {
+    // -R and -f, one flag and two list entries per tile, and the control blocks
+    g.ntiles = geodesic_tiles(j.ndim, j.sx, j.sy, j.sz, j.count);
+    const size_t tile_bytes = 3 * sizeof(uint32_t) * (size_t)g.ntiles;
+    extra = 2 * sizeof(float) * (size_t)total + tile_bytes + watershed_control_bytes();
+    if ((rc = values.take(*io.dc, 2 * sizeof(float) * (size_t)total, s, "the reconstruction")) ||
+        (rc = tiles.take(*io.dc, tile_bytes + watershed_control_bytes(), s, "the reconstruction worklists")))
+      return rc;
+    g.level = values.get<float>();
+    g.control = tiles.get();
+    g.flag = reinterpret_cast<uint32_t*>(tiles.get<char>() + watershed_control_bytes());
+    g.list = g.flag + g.ntiles;
+  }
+  // steps: [the reconstruction,] the union, the flatten (and mark), the numbering
+  StepTimer timer(s);
+  timer.stamp();
+  rc = 0;
+  if (g.level) {
+    rc = launch_hmax_phase(j.labels, j.label_bytes, image, h, g.level + total, j.ndim, j.sx, j.sy, j.sz, j.count,
+                           j.connectivity, g, *io.dc, s);
+    j.value = g.level;
+    j.negated = true;
+    timer.stamp();
+  } else {
+    j.value = image;
+  }
+  if (!rc) rc = launch_components_union(j, *io.dc, s);
+  timer.stamp();
+  if (!rc) rc = launch_components_flatten(j, out, *io.dc, s);
+  timer.stamp();
+  if (!rc) rc = launch_components_number(j, out, temp.get(), temp_bytes, *io.dc, s);
+  timer.stamp();
+  if (!rc && timer.synchronize()) {
+    const int k = g.level ? 1 : 0;
+    unsigned long long n[4] = {0, 0, 0, 0};
+    if (g.level) watershed_stats(g.control, n);
+    fprintf(stderr, "[edt_b200] %s %lldx%lldx%lld x%lld L=%d c=%d  reconstruction %.3f ms (rounds %llu, tile visits "
+                    "%llu)  union %.3f ms  flatten%s %.3f ms  numbering %.3f ms  scratch %zu bytes\n",
+            name, (long long)j.sx, (long long)j.sy, (long long)j.sz, (long long)j.count, j.label_bytes, j.connectivity,
+            k ? timer.ms(0, 1) : 0.0f, n[0], n[1], timer.ms(k, k + 1), image ? " and mark" : "",
+            timer.ms(k + 1, k + 2), timer.ms(k + 2, k + 3), p_bytes + temp_bytes + extra);
+  }
+  return rc;
+}
+
+int edtb200_connected_components(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                                 int64_t count, int connectivity, int flags, void* out, int out_bytes, int device,
+                                 void* stream_v) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (connectivity < 1 || connectivity > ndim)
+    return fail(EDTB200_EINVAL, "connectivity must be 1 to ndim (%d) (got %d)", ndim, connectivity);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_connected_components takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if ((rc = components_checks("edtb200_connected_components", vol, count, out_bytes))) return rc;
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, res_bytes = (size_t)total * (size_t)out_bytes;
+  if (same_side(flags) && overlaps(labels, lab_bytes, out, res_bytes)) return fail(EDTB200_EINVAL, "out overlaps labels");
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  const void* d_labels = nullptr;
+  void* d_out = nullptr;
+  Scratch out_stage;
+  if ((rc = io.in_labels(labels, lab_bytes, &d_labels)) ||
+      (rc = io.out_staged(out, res_bytes, out_stage, "the components", &d_out)))
+    return rc;
+  ComponentsJob j;
+  j.labels = d_labels;
+  j.label_bytes = label_bytes;
+  j.ndim = ndim; j.sx = sx; j.sy = sy; j.sz = sz; j.count = count;
+  j.connectivity = connectivity;
+  j.out_bytes = out_bytes;
+  rc = components_run("connected_components", j, nullptr, 0.0, d_out, io);
+  return rc ? rc : io.finish();
+}
+
+int edtb200_extended_maxima(const void* labels, int label_bytes, const float* image, int ndim, int64_t sx, int64_t sy,
+                            int64_t sz, int64_t count, double h, int connectivity, int flags, void* out, int out_bytes,
+                            int device, void* stream_v) {
+  if (!(label_bytes == 0 || label_bytes == 1 || label_bytes == 2 || label_bytes == 4 || label_bytes == 8))
+    return fail(EDTB200_EINVAL, "label_bytes must be 0 (no labels), 1, 2, 4 or 8 (got %d)", label_bytes);
+  int rc = check_dims(label_bytes ? label_bytes : 1, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (!(std::isfinite(h) && h >= 0.0)) return fail(EDTB200_EINVAL, "h must be finite and >= 0 (got %g)", h);
+  if (connectivity < 1 || connectivity > ndim)
+    return fail(EDTB200_EINVAL, "connectivity must be 1 to ndim (%d) (got %d)", ndim, connectivity);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_extended_maxima takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if ((rc = components_checks("edtb200_extended_maxima", vol, count, out_bytes))) return rc;
+  // the reconstruction's worklists hold 4-byte tile numbers
+  if (h > 0.0 && geodesic_tiles(ndim, sx, sy, sz, count) >= ((int64_t)1 << 32))
+    return fail(EDTB200_ELIMIT, "edtb200_extended_maxima with h > 0 takes stacks of fewer than 2^32 tiles");
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if ((label_bytes && !labels) || !image || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t lab_bytes = (size_t)total * (size_t)label_bytes, image_bytes = sizeof(float) * (size_t)total;
+  const size_t res_bytes = (size_t)total * (size_t)out_bytes;
+  if (same_side(flags) && label_bytes && overlaps(labels, lab_bytes, out, res_bytes))
+    return fail(EDTB200_EINVAL, "out overlaps labels");
+  if (same_side(flags) && overlaps(image, image_bytes, out, res_bytes)) return fail(EDTB200_EINVAL, "out overlaps image");
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  // host buffers are staged whole: the labels through this device's cached buffer, the image and the result
+  // through scratch
+  const void* d_labels = nullptr;
+  const float* d_image = nullptr;
+  void* d_out = nullptr;
+  Scratch image_stage, out_stage;
+  if (label_bytes && (rc = io.in_labels(labels, lab_bytes, &d_labels))) return rc;
+  if (!io.in_dev && (rc = image_stage.take(*io.dc, image_bytes, io.stream, "the staged image"))) return rc;
+  if ((rc = io.in(image, image_bytes, image_stage.get(), &d_image)) ||
+      (rc = io.out_staged(out, res_bytes, out_stage, "the maxima", &d_out)))
+    return rc;
+  ComponentsJob j;
+  j.labels = d_labels;
+  j.label_bytes = label_bytes;
+  j.ndim = ndim; j.sx = sx; j.sy = sy; j.sz = sz; j.count = count;
+  j.connectivity = connectivity;
+  j.out_bytes = out_bytes;
+  rc = components_run("extended_maxima", j, d_image, h, d_out, io);
+  return rc ? rc : io.finish();
+}
+
 // The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
 static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
                           const float w[3], int k, double max_distance) {

@@ -1,6 +1,6 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as sixteen translation units so that the kernel templates build in
+// The library is compiled as seventeen translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
@@ -9,7 +9,8 @@
 // dilation passes), edt_nearest.cu (the nearest-labels passes), edt_medial.cu (the medial
 // axis's mark kernel), edt_skeleton.cu (the skeleton's thinning kernel), edt_thickness.cu
 // (local thickness's levels, seeds and stores), edt_geodesic.cu (geodesic_distance's relaxation
-// passes) and edt_watershed.cu (watershed's relaxation passes).  The run-time label width
+// passes), edt_watershed.cu (watershed's relaxation passes) and edt_components.cu (the union-find passes of
+// connected_components and extended_maxima).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -60,6 +61,13 @@ int with_label_width(int label_bytes, F&& f) {
     case 8: return f(std::integral_constant<int, 8>{});
   }
   return fail(EDTB200_EINVAL, "label_bytes must be 1, 2, 4 or 8 (got %d)", label_bytes);
+}
+
+// with_label_width, and B = 0 for label_bytes 0 (no labels: every voxel inside the volume is a node).
+template <class F>
+int with_label_width_or_none(int label_bytes, F&& f) {
+  if (label_bytes == 0) return f(std::integral_constant<int, 0>{});
+  return with_label_width(label_bytes, f);
 }
 
 // cuTensorMapEncodeTiled, fetched through the runtime so that libcuda is not a link-time
@@ -499,6 +507,36 @@ int launch_watershed_store(int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t
 size_t watershed_control_bytes();
 // The rounds and tile visits of the level and label phases of the last call on `control` (synchronous).
 int watershed_stats(const void* control, unsigned long long out[4]);
+
+// The reconstruction of extended_maxima for h > 0 (edt_watershed.cu): -R, the least fixed point of
+// R[v] = max(R[v], min(f[v], R[u])) from m = fl32(f - h), into g.level, by the level phase of watershed on
+// negated values (altitude -f, written into neg_image, every node seeded at -m).  g as for watershed.
+int launch_hmax_phase(const void* labels, int label_bytes, const float* image, double h, float* neg_image, int ndim,
+                      int64_t sx, int64_t sy, int64_t sz, int64_t count, int connectivity, const WatershedScratch& g,
+                      DeviceCache& dc, cudaStream_t stream);
+
+// One call of connected_components or extended_maxima (edt_components.cu).  value null: the components of the
+// labels; else the plateaus of R (value = f as given, or -R with negated) and the mark pass.
+struct ComponentsJob {
+  const void* labels = nullptr;
+  int label_bytes = 0;              // 0: no labels
+  const float* value = nullptr;
+  bool negated = false;
+  uint32_t* parent = nullptr;       // one 4-byte parent per voxel
+  int ndim = 3;
+  int64_t sx = 1, sy = 1, sz = 1, count = 1;
+  int connectivity = 1;
+  int out_bytes = 4;
+};
+// The scratch of launch_components_number (the per-volume counts of a stack and cub's scan scratch).
+size_t components_temp_bytes(int64_t total, int64_t count, int out_bytes);
+// The tile pass and the border pass: P[v] = a node of v's component, its least index once both have run.
+int launch_components_union(const ComponentsJob& j, DeviceCache& dc, cudaStream_t stream);
+// The flatten pass (P = root, flags in out) and, for the plateaus, the mark pass.
+int launch_components_flatten(const ComponentsJob& j, void* out, DeviceCache& dc, cudaStream_t stream);
+// The per-volume prefix sum in place over out and the number pass.
+int launch_components_number(const ComponentsJob& j, void* out, void* temp, size_t temp_bytes, DeviceCache& dc,
+                             cudaStream_t stream);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

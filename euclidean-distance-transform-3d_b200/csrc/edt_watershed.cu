@@ -1,5 +1,5 @@
 // watershed's seed, relaxation and store kernels for every label width, no labels included (see
-// edt_watershed.cuh).
+// edt_watershed.cuh), and extended_maxima's reconstruction on the level phase's relaxation kernel.
 #include "edt_watershed.cuh"
 
 namespace edtb200 {
@@ -31,13 +31,9 @@ int64_t ws_blocks(int64_t total, const DeviceCache& dc) {
   return blocks > (int64_t)dc.sm_count * 16 ? (int64_t)dc.sm_count * 16 : blocks;
 }
 
-// One phase: clear the flags and the control block, seed, then the rounds in one cooperative launch.
+// The rounds of one phase in one cooperative launch, after its seed kernel.
 template <int LB, class WT, bool Label>
-int ws_phase(const void* labels, WsArgs a, DeviceCache& dc, cudaStream_t stream) {
-  CUDA_TRY(cudaMemsetAsync(a.flag, 0, sizeof(uint32_t) * (size_t)a.ntiles, stream));
-  CUDA_TRY(cudaMemsetAsync(a.ctl, 0, sizeof(WsControl), stream));
-  watershed_seed_kernel<LB, WT><<<(unsigned)ws_blocks(a.total, dc), 256, 0, stream>>>(labels, a, Label);
-  CUDA_TRY(cudaGetLastError());
+int ws_relax(const void* labels, WsArgs a, DeviceCache& dc, cudaStream_t stream) {
   // the grid barrier needs every block resident at once: as many blocks as fit, no more than the tiles
   int per_sm = 0;
   CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, watershed_relax_kernel<LB, WT, Label>, kWsThreads, 0));
@@ -50,11 +46,14 @@ int ws_phase(const void* labels, WsArgs a, DeviceCache& dc, cudaStream_t stream)
   return 0;
 }
 
-// f(std::integral_constant<int, B>{}) for the label width B, 0 (no labels) included.
-template <class F>
-int with_ws_label(int label_bytes, F&& f) {
-  if (label_bytes == 0) return f(std::integral_constant<int, 0>{});
-  return with_label_width(label_bytes, f);
+// One phase: clear the flags and the control block, seed, then the rounds in one cooperative launch.
+template <int LB, class WT, bool Label>
+int ws_phase(const void* labels, WsArgs a, DeviceCache& dc, cudaStream_t stream) {
+  CUDA_TRY(cudaMemsetAsync(a.flag, 0, sizeof(uint32_t) * (size_t)a.ntiles, stream));
+  CUDA_TRY(cudaMemsetAsync(a.ctl, 0, sizeof(WsControl), stream));
+  watershed_seed_kernel<LB, WT><<<(unsigned)ws_blocks(a.total, dc), 256, 0, stream>>>(labels, a, Label);
+  CUDA_TRY(cudaGetLastError());
+  return ws_relax<LB, WT, Label>(labels, a, dc, stream);
 }
 
 }  // namespace
@@ -69,11 +68,28 @@ int launch_watershed_phase(const void* labels, int label_bytes, const void* mark
   a.marker_bytes = marker_bytes;
   a.connectivity = connectivity;
   if (label_phase) a.ctl += 1;
-  return with_ws_label(label_bytes, [&](auto b) {
+  return with_label_width_or_none(label_bytes, [&](auto b) {
     constexpr int LB = decltype(b)::value;
     if (!label_phase) return ws_phase<LB, uint32_t, false>(labels, a, dc, stream);
     return marker_bytes == 8 ? ws_phase<LB, unsigned long long, true>(labels, a, dc, stream)
                              : ws_phase<LB, uint32_t, true>(labels, a, dc, stream);
+  });
+}
+
+int launch_hmax_phase(const void* labels, int label_bytes, const float* image, double h, float* neg_image, int ndim,
+                      int64_t sx, int64_t sy, int64_t sz, int64_t count, int connectivity, const WatershedScratch& g,
+                      DeviceCache& dc, cudaStream_t stream) {
+  WsArgs a = ws_args(g, ndim, sx, sy, sz, count);
+  a.image = image;
+  a.connectivity = connectivity;
+  return with_label_width_or_none(label_bytes, [&](auto b) {
+    constexpr int LB = decltype(b)::value;
+    CUDA_TRY(cudaMemsetAsync(a.flag, 0, sizeof(uint32_t) * (size_t)a.ntiles, stream));
+    CUDA_TRY(cudaMemsetAsync(a.ctl, 0, sizeof(WsControl), stream));
+    hmax_seed_kernel<LB><<<(unsigned)ws_blocks(a.total, dc), 256, 0, stream>>>(labels, a, neg_image, h);
+    CUDA_TRY(cudaGetLastError());
+    a.image = neg_image;
+    return ws_relax<LB, uint32_t, false>(labels, a, dc, stream);
   });
 }
 

@@ -100,6 +100,36 @@ watershed_seed_kernel(const void* __restrict__ labels, WsArgs a, bool label_phas
   }
 }
 
+// The seed kernel of extended_maxima's reconstruction (launch_hmax_phase): the level phase on negated values.
+// With f canonical (NaN read as -inf, -0.0 as +0.0) and m = fl32(fl64(f) - h) (-0.0 as +0.0), it writes the
+// altitude -f into neg_image, L = -m on every node (+inf elsewhere), and queues every tile holding a node for
+// round 1 (one queue per warp and tile).  The level phase then leaves L = -R, where R is the least fixed point
+// of R[v] = max(R[v], min(f[v], R[u])) from m: -R[v] = min(-R[v], max(-f[v], -R[u])).
+template <int LB>
+__global__ void __launch_bounds__(256)
+hmax_seed_kernel(const void* __restrict__ labels, WsArgs a, float* __restrict__ neg_image, double h) {
+  for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x; i0 < a.total; i0 += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = i0 + threadIdx.x;
+    int64_t t = -1;
+    if (i < a.total) {
+      float f = a.image[i];
+      f = f != f ? __int_as_float(0xff800000) : f == 0.0f ? 0.0f : f;
+      float m = (float)((double)f - h);
+      if (m == 0.0f) m = 0.0f;
+      neg_image[i] = f == 0.0f ? 0.0f : -f;
+      const bool node = ws_label<LB>(labels, i) != 0;
+      a.level[i] = node ? (m == 0.0f ? 0.0f : -m) : __int_as_float(0x7f800000);
+      if (node) {
+        const int64_t row = i / a.sx, x = i - row * a.sx, col = row / a.sy, y = row - col * a.sy;
+        const int64_t v = col / a.sz, z = col - v * a.sz;
+        t = ((v * a.nz + z / a.tz) * a.ny + y / a.ty) * a.nx + x / a.tx;
+      }
+    }
+    const unsigned same = __match_any_sync(0xffffffffu, t);
+    if (t >= 0 && (int)threadIdx.x % 32 == __ffs(same) - 1) ws_queue(a, t, 1u, 1, 1);
+  }
+}
+
 // The rounds of one phase, in ONE cooperative launch: Label false relaxes L, true relaxes W over the tight
 // edges of the fixed L.
 template <int LB, class WT, bool Label>

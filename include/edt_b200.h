@@ -39,7 +39,8 @@ extern "C" {
  * edtb200_expand_gather, edtb200_surface_count, edtb200_surface_distances, edtb200_morphology,
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
  * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness,
- * edtb200_geodesic, edtb200_noise_planes, edtb200_watershed)
+ * edtb200_geodesic, edtb200_noise_planes, edtb200_watershed, edtb200_connected_components,
+ * edtb200_extended_maxima)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -604,6 +605,63 @@ int edtb200_geodesic(const void *labels, int label_bytes, const void *seeds, int
 int edtb200_watershed(const void *labels, int label_bytes, const void *markers, int marker_bytes,
                       const float *image, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
                       int connectivity, int flags, void *out, float *level_out, int device, void *stream);
+
+/* Connected components and extended maxima (the markers of a watershed split: dist = edt(mask), markers =
+ * extended_maxima(dist, h), watershed(-dist, markers, mask)).  Volumes are x-fastest, as everywhere here.
+ *   graph      the watershed's: every voxel with a non-zero label is a node (label_bytes 0, extended_maxima
+ *              only: every voxel, all with one label); two nodes are joined when they are neighbours under
+ *              `connectivity` with the SAME label: an offset in {-1, 0, 1}^ndim counts when at most
+ *              `connectivity` of its components are non-zero.  Label 0 and the outside of the volume cannot be
+ *              crossed.
+ *   numbering  each component is numbered 1..n in increasing order of its least voxel index in memory order,
+ *              everything else 0; each volume of a stack is numbered on its own from 1.  For a C-ordered array
+ *              this is scipy.ndimage.label's numbering.
+ *
+ * edtb200_connected_components: the components of the graph, numbered.
+ * edtb200_extended_maxima: the regional maxima of the h-maxima transform (Soille's EMAX_h):
+ *   f = image, NaN read as -inf and -0.0 as +0.0; h finite and >= 0; m = fl32(fl64(f) - h), -0.0 as +0.0.
+ *   R is the least fixed point of R[v] = max(R[v], min(f[v], R[u])) over the joined neighbours u of v, from m:
+ *   the reconstruction by dilation of m under f, exact because min and max round nothing (h = 0: R = f).
+ *   A plateau is a component of the graph restricted to the edges with R[u] == R[v]; it is a maximum when no
+ *   node in it has a joined neighbour of larger R and its R is not -inf.  The result is the maximum plateaus,
+ *   numbered.  When f - h is exact in float32, a peak survives exactly when its dynamic (its height above the
+ *   highest pass to a higher voxel of its label) exceeds h.
+ *
+ *   labels, label_bytes  count * sx*sy*sz labels of 1, 2, 4 or 8 bytes (integers: compared by their bits),
+ *                        volumes back to back as for edtb200_transform_stack; label_bytes 0: no labels
+ *                        (extended_maxima only; labels is not read)
+ *   image                count * sx*sy*sz float32, laid out like the volume
+ *   connectivity         1 to ndim
+ *   flags                the residency flags only (EDTB200_LABELS_ON_DEVICE covers every input; both on the
+ *                        device: asynchronous on `stream`, no lock and no host wait; host buffers are staged
+ *                        whole, EDTB200_ENOMEM when they do not fit -- there is no chunked path)
+ *   out, out_bytes       count * sx*sy*sz numbers of 4 bytes (int32; volumes of fewer than 2^31 voxels) or 8
+ * Kernels, on one stream (edt_components.cuh).  Parents are 4-byte indices within a volume.  A tile pass
+ * (one CTA per 16x8x8 tile, 2-D 32x32, 1-D 1024) runs union-find on the tile's keys in shared memory; a border
+ * pass joins the joined edges that leave a tile by lock-free union in global memory, always hanging the larger
+ * root under the smaller (atomicMin), so that the final root of every component is its least index whatever
+ * order the races take; a flatten pass points every voxel at its root and flags the roots in out; for the
+ * plateaus a mark pass drops the root of every plateau with a larger joined neighbour or R = -inf; a prefix
+ * sum in place over out (cub::DeviceScan, per volume) and a number pass copy each kept root's number to its
+ * component.  For h > 0, R comes first from the level phase of edtb200_watershed on negated values
+ * (altitude -f, every node seeded at -m), on its tiles and worklists.
+ * Device memory beyond the inputs and outputs: 4 bytes per voxel of parents and the scan's scratch (8 bytes
+ * per volume of a stack and cub's); with h > 0 another 4 + 4 bytes per voxel (-R and -f) and 12 bytes per
+ * tile; and the staged image and result of a host call.
+ * Checks, in order: label width (extended_maxima also takes 0), ndim and sizes (as edtb200_transform),
+ * count >= 0, h (extended_maxima: finite and >= 0), connectivity, flags, out_bytes (4 or 8), the stack's size
+ * (within 2^62 voxels), the volume's size (fewer than 2^32 voxels, else EDTB200_ELIMIT), out_bytes 4 with a
+ * volume of 2^31 voxels or more (EDTB200_EINVAL), for extended_maxima with h > 0 the tiles (fewer than 2^32,
+ * else EDTB200_ELIMIT), emptiness (returns 0 touching nothing), pointers (labels unless label_bytes is 0,
+ * image, out), overlaps (out may not overlap an input on the same side), device.
+ * EDT_B200_VERBOSE=1 prints the device time of the reconstruction (with its rounds and tile visits), the
+ * union, the flatten and mark, and the numbering, on stderr. */
+int edtb200_connected_components(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy,
+                                 int64_t sz, int64_t count, int connectivity, int flags, void *out,
+                                 int out_bytes, int device, void *stream);
+int edtb200_extended_maxima(const void *labels, int label_bytes, const float *image, int ndim, int64_t sx,
+                            int64_t sy, int64_t sz, int64_t count, double h, int connectivity, int flags,
+                            void *out, int out_bytes, int device, void *stream);
 
 /* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
  * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between

@@ -40,7 +40,7 @@ __all__ = [
   "spherical_erode", "spherical_dilate", "spherical_open", "spherical_close",
   "parabolic_erode", "parabolic_dilate", "nearest_labels", "medial_axis",
   "skeletonize", "local_thickness", "geodesic_distance", "watershed",
-  "connected_components", "extended_maxima",
+  "connected_components", "extended_maxima", "fill_holes", "dust",
 ]
 
 FLAG_SQRT = 1
@@ -142,6 +142,10 @@ def _lib():
   lib.edtb200_connected_components.restype = ci
   lib.edtb200_extended_maxima.argtypes = [vp, ci, vp, ci, i64, i64, i64, i64, ctypes.c_double, ci, ci, vp, ci, ci, vp]
   lib.edtb200_extended_maxima.restype = ci
+  lib.edtb200_fill_holes.argtypes = [vp, ci, ci, i64, i64, i64, i64, ci, i64, ci, vp, vp, ci, vp]
+  lib.edtb200_fill_holes.restype = ci
+  lib.edtb200_dust.argtypes = [vp, ci, ci, i64, i64, i64, i64, ci, i64, ci, ci, vp, ci, vp]
+  lib.edtb200_dust.restype = ci
   lib.edtb200_expand_gather.argtypes = [vp, ci, ci, i64, i64, i64, i64, vp, vp, ctypes.c_double, ci, vp, ci, vp]
   lib.edtb200_expand_gather.restype = ci
   lib.edtb200_surface_count.argtypes = [vp, vp, ci, ci, i64, i64, i64, i64, vp, i64, ci, vp, ci, vp]
@@ -1967,6 +1971,137 @@ def extended_maxima(image, h=0.0, labels=None, *, connectivity=1, stacked=False,
 
 
 extended_maxima.__doc__ = _EXTENDED_MAXIMA_DOC
+
+
+# ---------------------------------------------------------------------------------------
+# hole filling and dust removal (edtb200_fill_holes, edtb200_dust)
+# ---------------------------------------------------------------------------------------
+
+_HOLES_IO = """
+  Input and output.  Volumes are x-fastest, as for edt(): x is the last axis of a C-ordered array and the first
+  of an F-ordered one.  1-D to 3-D arrays, or with stacked=True 2-D to 4-D whose slowest axis in memory indexes
+  same-shaped volumes, each with its own faces, so the result equals np.stack of the per-volume calls.  Labels
+  are bool or integer dtypes of 1, 2, 4 or 8 bytes and compare by their bits (float labels are a TypeError);
+  volumes of 2^32 voxels or more raise EDTError with code ELIMIT.  The result has the input's dtype, shape and
+  memory order.  numpy in gives numpy out; a torch CUDA tensor (or any __cuda_array_interface__ array) gives a
+  torch CUDA tensor computed on the current stream without a host synchronisation.  A host array that does not
+  fit on the GPU raises EDTError with code ENOMEM (there is no chunked path)."""
+
+
+def _size_bound(name, what, value):
+  if isinstance(value, (bool, np.bool_)) or not isinstance(value, (int, np.integer)):
+    raise TypeError("%s: %s must be an int, got %r" % (name, what, value))
+  if value < 0:
+    raise ValueError("%s: %s must be >= 0, got %d" % (name, what, value))
+  return min(int(value), (1 << 63) - 1)
+
+
+_FILL_HOLES_DOC = ("""Fill the holes of every label, on the GPU: scipy.ndimage.binary_fill_holes for every label at once,
+  fill_voids / kimimaro's fill_holes, porespy's blind pores.
+
+  Definition.  The graph and `connectivity` are connected_components': an offset counts when at most
+  `connectivity` of its components are non-zero (3-D 1/2/3: 6/18/26 neighbours, 2-D 1/2: 4/8).
+    background component  a component of the label-0 voxels under `connectivity`.
+    open                  it has a voxel on a face of its volume.
+    bordering labels      the non-zero labels of the voxels that neighbour it under `connectivity`.
+    hole of L             a background component that is not open, whose only bordering label is L, and, when
+                          max_size is given, that has at most max_size voxels.
+    result                the labels with every hole of L set to L; everything else unchanged.
+  For a bool mask this is exactly scipy.ndimage.binary_fill_holes(mask, generate_binary_structure(ndim,
+  connectivity)).  Per-label enclosure is fill_holes(labels == L): it fills L's mask whatever else L encloses.
+  In one multi-label call a background gap bordered by two labels stays 0: the gap between a cell (label 1) and
+  a nucleus (label 2) inside it borders both and is not filled, while a hole inside the nucleus becomes 2.
+
+  Examples (C order):
+      fill_holes(np.array([1, 0, 0, 1, 0]))                              ->  [1, 1, 1, 1, 0]
+      fill_holes(np.array([2, 0, 1, 0, 1]))                              ->  [2, 0, 1, 1, 1]
+      fill_holes(np.array([[0, 1, 0], [1, 0, 1], [0, 1, 0]]))            ->  [[0, 1, 0], [1, 1, 1], [0, 1, 0]]
+      fill_holes(np.array([[0, 1, 0], [1, 0, 1], [0, 1, 0]]), connectivity=2)   ->  unchanged: the middle 0
+        is joined to the corners, which are on the faces
+      fill_holes(np.array([1, 0, 0, 1]), max_size=1)                     ->  [1, 0, 0, 1]
+
+  `max_size`: None, or an int >= 0.  `return_fill_count=True` returns (result, filled): the number of voxels
+  filled, an int for one volume (for device input that int waits for the GPU) and an int64 array with one entry
+  per volume for a stack (a torch CUDA tensor for device input, without a host synchronisation).""" + _HOLES_IO + """
+
+  Cost.  The union-find passes of connected_components on the background, a tally pass that points every
+  background voxel at its root, sets OPEN and MIXED bits and claims the bordering labels at the root, and an
+  apply pass.  Device memory beyond the input and the output: 4 bytes per voxel of parents, 4 bytes per voxel
+  of claims (8 for 8-byte labels) and 1 byte per voxel of state, and with max_size another 4 bytes per voxel of
+  sizes.""")
+
+
+def fill_holes(labels, *, connectivity=1, max_size=None, return_fill_count=False, stacked=False, device=0):
+  name = "fill_holes"
+  if not isinstance(return_fill_count, (bool, np.bool_)):
+    raise TypeError("%s: return_fill_count must be True or False, got %r" % (name, return_fill_count))
+  bound = -1 if max_size is None else _size_bound(name, "max_size", max_size)
+  v = _Volume(name, labels, stacked, (1, 3), device)
+  conn = _connectivity(name, connectivity, v)
+  nbytes = _integer_bytes(v.dtype, "label", name)
+  v.set_weights(None, positive=False)
+  out = v.empty()
+  count = v.geometry[4]
+  counts = None
+  if return_fill_count:
+    if v.on_device:
+      import torch
+      counts = torch.zeros(count, dtype=torch.int64, device=v.arr.device)
+    else:
+      counts = np.zeros(count, np.int64)
+  if v.size:
+    vnd, sx, sy, sz = v.geometry[:4]
+    _check(_lib().edtb200_fill_holes(v.ptr, nbytes, vnd, sx, sy, sz, count, conn, bound, v.flags, v.ptr_of(out),
+                                     v.ptr_of(counts), *v.where))
+  if not return_fill_count:
+    return out
+  return out, (counts if stacked else int(counts[0]) if count else 0)
+
+
+fill_holes.__doc__ = _FILL_HOLES_DOC
+
+
+_DUST_DOC = ("""Remove the small components of every label, on the GPU: cc3d.dust, kimimaro's dust_threshold,
+  skimage.morphology.remove_small_objects for every label at once.
+
+  Definition.  The components are connected_components': voxels of the same non-zero label joined under
+  `connectivity` (an offset counts when at most `connectivity` of its components are non-zero).  Every voxel of
+  a component of FEWER than `threshold` voxels is set to 0, as in cc3d; a component of exactly `threshold`
+  voxels is kept.  With invert=True only the components of fewer than `threshold` voxels are kept.  skimage
+  versions disagree on whether their size bound is strict; this is the definition here.  cc3d's default of 26
+  neighbours is connectivity=3.
+
+  Examples (C order):
+      dust(np.array([1, 1, 0, 2, 0, 1]), 2)                   ->  [1, 1, 0, 0, 0, 0]
+      dust(np.array([1, 1, 0, 2, 0, 1]), 2, invert=True)      ->  [0, 0, 0, 2, 0, 1]
+      dust(np.array([[1, 0], [0, 1]]), 2)                     ->  [[0, 0], [0, 0]]
+      dust(np.array([[1, 0], [0, 1]]), 2, connectivity=2)     ->  [[1, 0], [0, 1]]
+
+  `threshold`: an int >= 0 (0 keeps everything).""" + _HOLES_IO + """
+
+  Cost.  The union-find passes of connected_components, a tally pass that adds every voxel to its root's size,
+  and an apply pass.  Device memory beyond the input and the output: 4 bytes per voxel of parents and 4 bytes
+  per voxel of sizes.""")
+
+
+def dust(labels, threshold, *, connectivity=1, invert=False, stacked=False, device=0):
+  name = "dust"
+  threshold = _size_bound(name, "threshold", threshold)
+  if not isinstance(invert, (bool, np.bool_)):
+    raise TypeError("%s: invert must be True or False, got %r" % (name, invert))
+  v = _Volume(name, labels, stacked, (1, 3), device)
+  conn = _connectivity(name, connectivity, v)
+  nbytes = _integer_bytes(v.dtype, "label", name)
+  v.set_weights(None, positive=False)
+  out = v.empty()
+  if v.size:
+    vnd, sx, sy, sz, count = v.geometry[:5]
+    _check(_lib().edtb200_dust(v.ptr, nbytes, vnd, sx, sy, sz, count, conn, threshold, int(bool(invert)), v.flags,
+                               v.ptr_of(out), *v.where))
+  return out
+
+
+dust.__doc__ = _DUST_DOC
 
 
 # ---------------------------------------------------------------------------------------

@@ -2549,6 +2549,145 @@ int edtb200_extended_maxima(const void* labels, int label_bytes, const float* im
   return rc ? rc : io.finish();
 }
 
+// The checks edtb200_fill_holes and edtb200_dust share, in their documented order: label width, ndim and
+// sizes, count >= 0, connectivity; after their own bound and flags they call holes_size_checks.
+static int holes_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
+                        int connectivity) {
+  int rc = check_dims(label_bytes, ndim, sx, sy, sz);
+  if (rc) return rc;
+  if (count < 0) return fail(EDTB200_EINVAL, "negative count");
+  if (connectivity < 1 || connectivity > ndim)
+    return fail(EDTB200_EINVAL, "connectivity must be 1 to ndim (%d) (got %d)", ndim, connectivity);
+  return 0;
+}
+
+// The stack's size and the volume's size (parents are 4-byte indices within a volume).
+static int holes_size_checks(const char* name, int64_t vol, int64_t count) {
+  if (const int rc = check_stack(vol, count, 1)) return rc;
+  if (vol >= ((int64_t)1 << 32)) return fail(EDTB200_ELIMIT, "%s takes volumes of fewer than 2^32 voxels", name);
+  return 0;
+}
+
+// The union, tally and apply passes of one call, device buffers in place.  Prints the phases with
+// EDT_B200_VERBOSE.
+static int holes_run(const char* name, HolesJob j, void* out, HostIO& io) {
+  const cudaStream_t s = io.stream;
+  const int64_t total = j.cc.sx * j.cc.sy * j.cc.sz * j.cc.count;
+  const bool sized = !j.fill || j.bound != ~(uint64_t)0;
+  const size_t p_bytes = sizeof(uint32_t) * (size_t)total, size_bytes = sized ? sizeof(uint32_t) * (size_t)total : 0;
+  const size_t claim_bytes = j.fill ? (j.cc.label_bytes == 8 ? 8 : 4) * (size_t)total : 0;
+  const size_t state_bytes = j.fill ? ((size_t)total + 3) & ~(size_t)3 : 0;
+  Scratch parents, sizes, claims;
+  int rc;
+  if ((rc = parents.take(*io.dc, p_bytes, s, "the component parents")) ||
+      (sized && (rc = sizes.take(*io.dc, size_bytes, s, "the component sizes"))) ||
+      (j.fill && (rc = claims.take(*io.dc, claim_bytes + state_bytes, s, "the hole claims"))))
+    return rc;
+  j.cc.parent = parents.get<uint32_t>();
+  j.size = sized ? sizes.get<uint32_t>() : nullptr;
+  if (j.fill) {
+    j.claim = claims.get();
+    j.state = claims.get<uint8_t>() + claim_bytes;
+  }
+  // what the tally and apply accumulate into starts at zero
+  if (sized) CUDA_TRY(cudaMemsetAsync(j.size, 0, size_bytes, s));
+  if (j.fill) CUDA_TRY(cudaMemsetAsync(j.claim, 0, claim_bytes + state_bytes, s));
+  if (j.counts) CUDA_TRY(cudaMemsetAsync(j.counts, 0, sizeof(unsigned long long) * (size_t)j.cc.count, s));
+  // steps: the union, the tally, the apply
+  StepTimer timer(s);
+  timer.stamp();
+  rc = launch_holes_union(j, *io.dc, s);
+  timer.stamp();
+  if (!rc) rc = launch_holes_tally(j, *io.dc, s);
+  timer.stamp();
+  if (!rc) rc = launch_holes_apply(j, out, *io.dc, s);
+  timer.stamp();
+  if (!rc && timer.synchronize())
+    fprintf(stderr, "[edt_b200] %s %lldx%lldx%lld x%lld L=%d c=%d  union %.3f ms  tally %.3f ms  apply %.3f ms  "
+                    "scratch %zu bytes\n",
+            name, (long long)j.cc.sx, (long long)j.cc.sy, (long long)j.cc.sz, (long long)j.cc.count,
+            j.cc.label_bytes, j.cc.connectivity, timer.ms(0, 1), timer.ms(1, 2), timer.ms(2, 3),
+            p_bytes + size_bytes + claim_bytes + state_bytes);
+  return rc;
+}
+
+int edtb200_fill_holes(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                       int64_t count, int connectivity, int64_t max_size, int flags, void* out, int64_t* fill_counts,
+                       int device, void* stream_v) {
+  int rc = holes_checks(label_bytes, ndim, sx, sy, sz, count, connectivity);
+  if (rc) return rc;
+  if (max_size < -1) return fail(EDTB200_EINVAL, "max_size must be -1 (none) or >= 0 (got %lld)", (long long)max_size);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_fill_holes takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if ((rc = holes_size_checks("edtb200_fill_holes", vol, count))) return rc;
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t res_bytes = (size_t)total * (size_t)label_bytes, counts_bytes = sizeof(int64_t) * (size_t)count;
+  if (same_side(flags) && overlaps(labels, res_bytes, out, res_bytes)) return fail(EDTB200_EINVAL, "out overlaps labels");
+  if (fill_counts && overlaps(fill_counts, counts_bytes, out, res_bytes))
+    return fail(EDTB200_EINVAL, "fill_counts overlaps out");
+  if (fill_counts && same_side(flags) && overlaps(fill_counts, counts_bytes, labels, res_bytes))
+    return fail(EDTB200_EINVAL, "fill_counts overlaps labels");
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  const void* d_labels = nullptr;
+  void* d_out = nullptr;
+  int64_t* d_counts = nullptr;
+  Scratch out_stage, counts_stage;
+  if ((rc = io.in_labels(labels, res_bytes, &d_labels)) ||
+      (rc = io.out_staged(out, res_bytes, out_stage, "the filled labels", &d_out)) ||
+      (fill_counts && (rc = io.out_staged(fill_counts, counts_bytes, counts_stage, "the fill counts", &d_counts))))
+    return rc;
+  HolesJob j;
+  j.cc.labels = d_labels;
+  j.cc.label_bytes = label_bytes;
+  j.cc.ndim = ndim; j.cc.sx = sx; j.cc.sy = sy; j.cc.sz = sz; j.cc.count = count;
+  j.cc.connectivity = connectivity;
+  j.fill = true;
+  j.bound = max_size < 0 ? ~(uint64_t)0 : (uint64_t)max_size;
+  j.counts = reinterpret_cast<unsigned long long*>(d_counts);
+  rc = holes_run("fill_holes", j, d_out, io);
+  return rc ? rc : io.finish();
+}
+
+int edtb200_dust(const void* labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz, int64_t count,
+                 int connectivity, int64_t threshold, int invert, int flags, void* out, int device, void* stream_v) {
+  int rc = holes_checks(label_bytes, ndim, sx, sy, sz, count, connectivity);
+  if (rc) return rc;
+  if (threshold < 0) return fail(EDTB200_EINVAL, "threshold must be >= 0 (got %lld)", (long long)threshold);
+  if (invert != 0 && invert != 1) return fail(EDTB200_EINVAL, "invert must be 0 or 1 (got %d)", invert);
+  if (flags & ~(EDTB200_LABELS_ON_DEVICE | EDTB200_OUT_ON_DEVICE))
+    return fail(EDTB200_EINVAL, "edtb200_dust takes only the residency flags (got %d)", flags);
+  const int64_t vol = sx * sy * sz;
+  if ((rc = holes_size_checks("edtb200_dust", vol, count))) return rc;
+  const int64_t total = vol * count;
+  if (total == 0) return 0;
+  if (!labels || !out) return fail(EDTB200_EINVAL, "null pointer");
+  const size_t res_bytes = (size_t)total * (size_t)label_bytes;
+  if (same_side(flags) && overlaps(labels, res_bytes, out, res_bytes)) return fail(EDTB200_EINVAL, "out overlaps labels");
+
+  HostIO io;
+  if ((rc = io.open(device, flags, stream_v))) return rc;
+  const void* d_labels = nullptr;
+  void* d_out = nullptr;
+  Scratch out_stage;
+  if ((rc = io.in_labels(labels, res_bytes, &d_labels)) ||
+      (rc = io.out_staged(out, res_bytes, out_stage, "the dusted labels", &d_out)))
+    return rc;
+  HolesJob j;
+  j.cc.labels = d_labels;
+  j.cc.label_bytes = label_bytes;
+  j.cc.ndim = ndim; j.cc.sx = sx; j.cc.sy = sy; j.cc.sz = sz; j.cc.count = count;
+  j.cc.connectivity = connectivity;
+  j.bound = (uint64_t)threshold;
+  j.invert = invert != 0;
+  rc = holes_run("dust", j, d_out, io);
+  return rc ? rc : io.finish();
+}
+
 // The checks edtb200_nearest_labels and its plan share, in their documented order, up to max_distance.
 static int nearest_checks(int label_bytes, int ndim, int64_t& sx, int64_t& sy, int64_t& sz, int64_t count,
                           const float w[3], int k, double max_distance) {

@@ -11,6 +11,8 @@ namespace {
 
 constexpr int kCcTileDims[4][3] = {{0, 0, 0}, {1024, 1, 1}, {32, 32, 1}, {16, 8, 8}};
 
+}  // namespace
+
 CcArgs cc_args(const ComponentsJob& j) {
   CcArgs a{};
   a.parent = j.parent;
@@ -30,6 +32,8 @@ unsigned cc_blocks(int64_t n, const DeviceCache& dc) {
   const int64_t blocks = (n + kCcThreads - 1) / kCcThreads, cap = (int64_t)dc.sm_count * 16;
   return (unsigned)(blocks > cap ? cap : blocks < 1 ? 1 : blocks);
 }
+
+namespace {
 
 template <class F>
 int with_out_width(int out_bytes, F&& f) {

@@ -296,4 +296,10 @@ __global__ void __launch_bounds__(kCcThreads, 4) components_number_kernel(CcArgs
   }
 }
 
+namespace host {
+// The kernel arguments of a job (edt_components.cu), and the grid of a pass with one thread per item.
+CcArgs cc_args(const ComponentsJob& j);
+unsigned cc_blocks(int64_t n, const DeviceCache& dc);
+}  // namespace host
+
 }  // namespace edtb200

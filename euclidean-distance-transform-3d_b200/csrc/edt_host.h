@@ -1,6 +1,6 @@
 // edt_host.h -- declarations shared by the host-side translation units of libedt_b200.so.
 //
-// The library is compiled as seventeen translation units so that the kernel templates build in
+// The library is compiled as eighteen translation units so that the kernel templates build in
 // parallel: edt_capi.cu (C ABI, staging, caches), edt_passes_b{1,2,4,8}.cu (the axis-pass
 // launchers of edt_passes.cuh instantiated for one label width each), edt_plan.cu (the
 // later-axis plan for host code that launches nothing), edt_bounded.cu (the bounded
@@ -9,8 +9,9 @@
 // dilation passes), edt_nearest.cu (the nearest-labels passes), edt_medial.cu (the medial
 // axis's mark kernel), edt_skeleton.cu (the skeleton's thinning kernel), edt_thickness.cu
 // (local thickness's levels, seeds and stores), edt_geodesic.cu (geodesic_distance's relaxation
-// passes), edt_watershed.cu (watershed's relaxation passes) and edt_components.cu (the union-find passes of
-// connected_components and extended_maxima).  The run-time label width
+// passes), edt_watershed.cu (watershed's relaxation passes), edt_components.cu (the union-find passes of
+// connected_components and extended_maxima) and edt_holes.cu (fill_holes' and dust's tally and apply
+// passes).  The run-time label width
 // becomes a template argument in one place, with_label_width below.
 #pragma once
 #include "../../include/edt_b200.h"
@@ -537,6 +538,25 @@ int launch_components_flatten(const ComponentsJob& j, void* out, DeviceCache& dc
 // The per-volume prefix sum in place over out and the number pass.
 int launch_components_number(const ComponentsJob& j, void* out, void* temp, size_t temp_bytes, DeviceCache& dc,
                              cudaStream_t stream);
+
+// One call of fill_holes or dust (edt_holes.cu): cc holds the labels, the geometry, the connectivity and the
+// parents; the buffers below are indexed by root and zeroed before the tally.
+struct HolesJob {
+  ComponentsJob cc;
+  bool fill = false;                // fill_holes, else dust
+  uint32_t* size = nullptr;         // one 4-byte size per voxel (null: fill_holes without max_size)
+  void* claim = nullptr;            // fill_holes: 4 bytes per voxel (8 with 8-byte labels)
+  uint8_t* state = nullptr;         // fill_holes: 1 byte per voxel, 4-byte aligned, padded to 4 bytes
+  uint64_t bound = 0;               // fill_holes: max_size (all ones: none); dust: threshold
+  bool invert = false;              // dust
+  unsigned long long* counts = nullptr;   // fill_holes: voxels filled per volume, or null
+};
+// The union: the tile and border passes on the background key (fill_holes) or the label key (dust).
+int launch_holes_union(const HolesJob& j, DeviceCache& dc, cudaStream_t stream);
+// The tally pass: P = root, sizes, and for fill_holes the OPEN / MIXED bits and the claims at the roots.
+int launch_holes_tally(const HolesJob& j, DeviceCache& dc, cudaStream_t stream);
+// The apply pass: out in the labels' width, and the fill counts.
+int launch_holes_apply(const HolesJob& j, void* out, DeviceCache& dc, cudaStream_t stream);
 
 // The surface kernels, one instantiation per label width in edt_surface.cu.  keys: nkeys labels on the
 // device.  mask non-null: surface_mask_kernel into the masks of slots [s0, s1); else values non-null:

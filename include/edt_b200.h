@@ -40,7 +40,7 @@ extern "C" {
  * edtb200_parabolic, edtb200_parabolic_sites, edtb200_nearest_labels, edtb200_nearest_labels_plan,
  * edtb200_medial_axis, edtb200_skeletonize, edtb200_pass_window, edtb200_local_thickness,
  * edtb200_geodesic, edtb200_noise_planes, edtb200_watershed, edtb200_connected_components,
- * edtb200_extended_maxima)
+ * edtb200_extended_maxima, edtb200_fill_holes, edtb200_dust)
  * keep the number: every 202-level entry point
  * keeps its signature and meaning, and a caller that needs a newer one looks its symbol up.  One
  * exception: edtb200_last_later_launch fills info[0..9) since the settled-tile skip (it filled
@@ -662,6 +662,60 @@ int edtb200_connected_components(const void *labels, int label_bytes, int ndim, 
 int edtb200_extended_maxima(const void *labels, int label_bytes, const float *image, int ndim, int64_t sx,
                             int64_t sy, int64_t sz, int64_t count, double h, int connectivity, int flags,
                             void *out, int out_bytes, int device, void *stream);
+
+/* Hole filling and dust removal: decide per component, then write every voxel.  Volumes are x-fastest, as
+ * everywhere here.  The graph and `connectivity` are connected_components': an offset in {-1, 0, 1}^ndim
+ * counts when at most `connectivity` of its components are non-zero.  Labels compare by their bits.
+ *
+ * edtb200_fill_holes: every hole of a label L takes L.
+ *   background component  a component of the label-0 voxels under `connectivity`; all background
+ *                         neighbours are joined.
+ *   open                  it contains a voxel on a face of its volume (in a stack each volume has its own
+ *                         faces).
+ *   bordering labels      the non-zero labels of the voxels that neighbour it under `connectivity`.
+ *   hole of L             a background component that is not open, whose only bordering label is L, and, when
+ *                         max_size >= 0, that has at most max_size voxels.
+ *   result                the labels with every hole of L set to L; everything else unchanged.  For one label
+ *                         this is scipy.ndimage.binary_fill_holes with generate_binary_structure(ndim,
+ *                         connectivity).  A background gap bordered by two labels (the gap between a cell and
+ *                         a nucleus inside it) stays 0.
+ *   fill_counts           NULL, or count int64: the voxels filled in each volume, on the side of out.
+ * edtb200_dust: every component (same label, joined under `connectivity`) of fewer than `threshold` voxels is
+ *   set to 0; with invert = 1 only those components are kept and every other labelled voxel is set to 0.
+ *
+ *   labels, label_bytes  count * sx*sy*sz labels of 1, 2, 4 or 8 bytes, volumes back to back as for
+ *                        edtb200_transform_stack
+ *   connectivity         1 to ndim
+ *   max_size             fill_holes: -1 (no bound) or >= 0
+ *   threshold, invert    dust: threshold >= 0 (0 keeps everything), invert 0 or 1
+ *   flags                the residency flags only (EDTB200_LABELS_ON_DEVICE covers the labels; both on the
+ *                        device: asynchronous on `stream`, no lock and no host wait; host buffers are staged
+ *                        whole, EDTB200_ENOMEM when they do not fit -- there is no chunked path)
+ *   out                  count * sx*sy*sz labels of label_bytes; it may not overlap the labels (no in-place call)
+ * Kernels, on one stream (edt_holes.cuh).  The union is the tile and border passes of
+ * edtb200_connected_components (edt_components.cuh): with the label key for dust, and for fill_holes with a
+ * key whose nodes are the label-0 voxels inside the volume, all joined.  A tally pass (one thread per voxel)
+ * points every node at its root and adds it to its root's 4-byte size, one atomic per run of equal roots in a
+ * warp; for fill_holes a node on a face sets an OPEN bit at its root, and a node with a neighbour of label
+ * L != 0 claims L at its root by atomicCAS(claim, 0, L) (4 bytes, 8 for 8-byte labels), setting a MIXED bit
+ * when the CAS returns another label.  Sums, ORs and "the claimed labels are one" do not depend on the order
+ * of the races.  An apply pass (one thread per voxel) writes out, and counts the filled voxels per volume by
+ * a block reduction and one atomic per block.
+ * Device memory beyond the inputs and outputs: 4 bytes per voxel of parents; 4 bytes per voxel of sizes for
+ * dust and for fill_holes with max_size >= 0; for fill_holes 4 bytes per voxel of claims (8 with 8-byte
+ * labels) and 1 byte per voxel of state; and the staged labels, result and fill counts of a host call.
+ * Checks, in order: label width, ndim and sizes (as edtb200_transform), count >= 0, connectivity, max_size
+ * (fill_holes) or threshold and invert (dust), flags, the stack's size (within 2^62 voxels), the volume's
+ * size (fewer than 2^32 voxels, else EDTB200_ELIMIT), emptiness (returns 0 touching nothing, fill_counts
+ * included), pointers (labels, out), overlaps (out may not overlap the labels on the same side; fill_counts
+ * may overlap neither), device.
+ * EDT_B200_VERBOSE=1 prints the device time of the union, the tally and the apply on stderr. */
+int edtb200_fill_holes(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                       int64_t count, int connectivity, int64_t max_size, int flags, void *out,
+                       int64_t *fill_counts, int device, void *stream);
+int edtb200_dust(const void *labels, int label_bytes, int ndim, int64_t sx, int64_t sy, int64_t sz,
+                 int64_t count, int connectivity, int64_t threshold, int invert, int flags, void *out,
+                 int device, void *stream);
 
 /* The k nearest distinct labels of every voxel within a distance: which objects are near p, and how far
  * away each is (the d1, d2 of the U-Net weight map w0 exp(-(d1 + d2)^2 / 2 sigma^2), contacts between
